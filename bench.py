@@ -35,7 +35,7 @@ ROOT = Path(__file__).resolve().parent
 sys.path.insert(0, str(ROOT))
 
 DEFAULT_BATCH = {"vgg16": 64, "resnet50": 128, "mobilenet_v1": 256, "single_conv": 64}
-L2_BYTES = 126 * 1024 * 1024
+L2_BYTES = 50 * 1024 * 1024  # H100 SXM
 
 
 def env_int(name: str, default: int) -> int:
@@ -52,8 +52,8 @@ def measured_peaks() -> tuple[dict, str]:
             return json.loads(p.read_text()), "measured"
         except Exception:
             pass
-    # fallback stated by /opt/skills/guides/B200_PROFILING.md
-    return {"hbm_gbs": 6650.0, "bf16_tflops": 1590.0, "bf16_tflops_sustained": 1400.0}, "fallback"
+    # fallback: NVIDIA's H100 SXM data sheet (dense BF16, HBM3), not a measured rate
+    return {"hbm_gbs": 3350.0, "bf16_tflops": 989.0, "bf16_tflops_sustained": 989.0}, "fallback"
 
 
 def model_files(model: str, rank: int, barrier) -> tuple[str, str, float, tuple]:
@@ -73,7 +73,7 @@ def model_files(model: str, rank: int, barrier) -> tuple[str, str, float, tuple]
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons DURING the timed regions (B200_PROFILING.md recipe).
+    """nvidia-smi clocks / throttle reasons DURING the timed regions.
 
     nvidia-smi needs ~0.1-0.5 s to deliver its first row, longer than a short timed region, so the poller is started
     before the warm-up and only the rows received inside the marked windows (device-resident leg and end-to-end leg,
@@ -202,8 +202,8 @@ def run_reference(args, rank: int, world: int) -> None:
     print(json.dumps(line), flush=True)
 
 
-KERNEL_CLASS_NAMES = ["tensor_gemm_ts_kernel (tcgen05 kind::tf32, Winograd/im2col/FC GEMM)",
-                      "conv_igemm_kernel (tcgen05 kind::f16 BF16x3 / kind::tf32 implicit-GEMM conv)", "wino_input_kernel",
+KERNEL_CLASS_NAMES = ["tensor_gemm_kernel (wgmma tf32, Winograd/im2col/FC GEMM)",
+                      "conv_igemm_kernel (wgmma bf16 BF16x3 / tf32 implicit-GEMM conv)", "wino_input_kernel",
                       "wino_output_kernel", "pooling_kernel", "depthwise kernels", "element-wise kernels"]
 
 
@@ -223,7 +223,7 @@ def roofline_leg(net, booster, dev_batches, n_rot, ms_step: float, model: str) -
             net.Forward()
         net.Synchronize()
         peaks, how = measured_peaks()
-        # kernels timed inside a long step -> the sustained figures; fallbacks = /opt/skills/guides/B200_PROFILING.md
+        # kernels timed inside a long step -> the sustained figures
         tf_peak = float(peaks.get("bf16_tflops_sustained", peaks.get("bf16_tflops", 1400.0)))
         hbm_peak = float(peaks.get("hbm_gbs", 6500.0))
         classes = []
@@ -257,16 +257,6 @@ def roofline_leg(net, booster, dev_batches, n_rot, ms_step: float, model: str) -
         roof = dict(classes[0])
         roof["peak_source"] = (f"{how}: " + ("bf16_tflops_sustained" if roof["bound"] == "tensor" else "hbm_gbs") +
                                " (kernel timed inside a long step)")
-        roof["traffic"] = None
-        for tr in sorted((ROOT / "profiles").glob("r0*_kernel_traffic.json"), reverse=True):
-            try:
-                v = json.loads(tr.read_text()).get(model, {}).get(roof["kernel"].split()[0])
-            except Exception:
-                v = None
-            if v is not None:
-                roof["traffic"] = v
-                roof["traffic_source"] = f"profiles/{tr.name} (dram__bytes_read+write per launch, ncu --set full)"
-                break
         roof["other_kernels"] = classes[1:]
         return roof
     except Exception as e:  # the roofline leg explains the number, it must never cost the bench line
@@ -376,6 +366,11 @@ def run_workload(args, model: str, B: int, rank: int, world: int, local_rank: in
         if sampler:
             sampler.end()
         ms_dev = max_over_ranks(e0.elapsed_time(e1))
+        if args.dump_outputs and rank == 0:
+            # what the timed path handed back in its last step: the output blob of batch (steps - 1) % n_rot
+            out_dir = Path(args.dump_outputs)
+            out_dir.mkdir(parents=True, exist_ok=True)
+            np.save(out_dir / f"{model}_{out_name}.npy", net.Extract(out_name).astype(np.float32))
 
         if args.lean:
             if sampler:
@@ -494,6 +489,9 @@ def main() -> None:
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--l2-chunk-mb", type=float, default=None)
     ap.add_argument("--lean", action="store_true", help="profiling aid: device-resident leg only (no e2e / roofline / cpu legs)")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="after the timed steps, write each workload's output blob of the last timed step as "
+                         "DIR/<model>_<blob>.npy (float32); inputs and weights are seeded, so runs are comparable")
     args = ap.parse_args()
     headline = args.model or "vgg16"
     extra = [] if (args.model or args.lean) else ["resnet50", "mobilenet_v1"]
@@ -557,7 +555,7 @@ def main() -> None:
         "config": cfg,
         "details": {"parallelism": f"batch-shard x{world} (weights broadcast once over NCCL, no collective in Forward)",
                     "tensor_core_mode": {"fp32split": "fp32-equivalent split operands, fp32 accumulation: BF16x3 (p1*q1 + p1*q2 + "
-                                                      "p2*q1, kind::f16) in the implicit GEMM, 3xTF32 in the Winograd / FC TensorGEMM; "
+                                                      "p2*q1, bf16 wgmma) in the implicit GEMM, 3xTF32 in the Winograd / FC TensorGEMM; "
                                                       "accuracy = parity_max_rel",
                                          "tf32x3": "3xTF32 split (fp32-equivalent) in every contraction",
                                          "tf32": "TF32"}[args.precision],
@@ -565,7 +563,7 @@ def main() -> None:
                                   "im2col -> implicit GEMM): Winograd F(6,3)+TensorGEMM / SGECONV implicit GEMM / depthwise",
                     "fusion": not args.no_fusion, "cuda_graph": not args.no_graph,
                     "l2_policy": f"{head['n_rot']} rotating input batches ({head['n_rot'] * head['batch_bytes'] / 2**20:.0f} MiB > L2); "
-                                 f"activations per step far exceed the 126 MB L2",
+                                 f"activations per step far exceed the 50 MB L2",
                     "gflop_per_image": head["gflop_per_image"], "load_s": head["load_s"]},
         "clocks": head["clocks"],
         "e2e": head["e2e"],

@@ -1,4 +1,4 @@
-"""feathercnn_b200 — B200-native (sm_100a) CNN inference backend behind FeatherCNN's API.
+"""feathercnn_b200 — H100-native (sm_90a) CNN inference backend behind FeatherCNN's API.
 
 The product is the native code: ``csrc/`` (hand-written CUDA kernels + the C ABI of ``include/fcuda.h``) and
 ``host/`` (C++ ``feather::Net``).  This Python package is a thin ctypes binding used by tests and bench.py;

@@ -279,7 +279,7 @@ def tensor_gemm(a: torch.Tensor, b: torch.Tensor, x3: bool = True) -> torch.Tens
     n = b.shape[1]
     a = a.contiguous(); b = b.contiguous()
     d = torch.empty((g, m, n), device=a.device)
-    if x3:  # A is split inside the kernel (tensor memory); B carries its hi / lo planes
+    if x3:  # A is split inside the kernel (registers); B carries its hi / lo planes
         bh, bl = torch.empty_like(b), torch.empty_like(b)
         _check("fcuda_split_tf32", lib.fcuda_split_tf32(_ptr(bh), _ptr(bl), _ptr(b), b.numel(), _stream()))
         _check("fcuda_tensor_gemm", lib.fcuda_tensor_gemm(_ptr(d), _ptr(a), _ptr(bh), _ptr(bl), m, n, k, g, _stream()))

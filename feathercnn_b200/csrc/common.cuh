@@ -1,4 +1,4 @@
-// Shared helpers for the fcuda kernels (sm_100a only).
+// Shared helpers for the fcuda kernels (sm_90a only).
 #pragma once
 
 #include <cuda_runtime.h>
@@ -32,7 +32,7 @@ void count_launch(int n = 1);
 unsigned long long launch_count();
 void reset_launch_count();
 
-// Number of SMs of the current device (148 on B200); cached per device.
+// Number of SMs of the current device (132 on H100 SXM); cached per device.
 int sm_count();
 
 // cudaFuncAttributeMaxDynamicSharedMemorySize is per (function, device): a process that drives several GPUs must opt
@@ -66,8 +66,7 @@ __device__ __forceinline__ void split_tf32(float v, float& hi, float& lo) {
 
 // Kernel-variant switches (defaults = the measured-best configuration; FCUDA_<NAME> in the environment or
 // fcuda_set_tuning() override them — the variants stay testable and benchmarkable side by side).
-enum TuneKey { TUNE_IGEMM_ISSUERS = 0, TUNE_IGEMM_SLAB, TUNE_IGEMM_CG, TUNE_DW_VEC, TUNE_GEMM_CLUSTER, TUNE_GEMM_TMA_STORE,
-               TUNE_IGEMM_TMA_OUT, TUNE_IGEMM_PW, TUNE_WINO_MLP, TUNE_MBAR_SUSPEND_NS, TUNE_IGEMM_TMA_LANES, TUNE_COUNT };
+enum TuneKey { TUNE_DW_VEC = 0, TUNE_WINO_MLP, TUNE_COUNT };
 int tune_get(int key);
 const char* tune_name(int key);             // registry name of a key (fcuda_set_tuning / fcuda_get_tuning)
 int tune_set(const char* name, int value);  // 0, or -200 for an unknown name / value

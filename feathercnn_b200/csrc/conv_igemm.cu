@@ -1,101 +1,49 @@
-// SGECONV — implicit-GEMM convolution straight from the NCHW blob on tcgen05 (sm_100a).
+// SGECONV — implicit-GEMM convolution straight from the NCHW blob on Hopper warpgroup MMA (sm_90a).
 //
-// Replaces the idea of the reference's SGECONV algorithm (/root/reference/src/booster/arm/sgeconv.cpp:1311-1856,
-// "packs B directly from the padded input, no materialised im2col"; a stub in the AVX dispatcher,
-// avx/booster.cpp:105-118) and of im2col + packed SGEMM (avx/booster.cpp:83-102) with a Blackwell formulation that
-// has NO intermediate in HBM and not even an A tile in shared memory:
+// Replaces the idea of the reference's SGECONV algorithm ("packs B directly from the padded input, no materialised
+// im2col"; a stub in its AVX dispatcher) and of im2col + packed SGEMM with a formulation that has NO intermediate in HBM
+// and no A tile in shared memory:
 //
 //   D[pixel][oc] = sum_k  A[pixel][k] * Wp[oc][k],    k = (u*KW + v)*IC + ic   (IC % 32 != 0)
 //                                                      k = ((ic/32)*KH*KW + u*KW + v)*32 + ic%32   (IC % 32 == 0: a k-block
-//                                                      is one tap x 32 channels, taps innermost so that the 3x3 slab
-//                                                      producer below serves all nine taps of a channel block from one slab)
-//   A[pixel][k]  = X[n][ic][oy*s+u-pad][ox*s+v-pad]   (0 outside the image: the im2col rule, generic_kernels.cpp:66-67)
+//                                                      is one tap x 32 channels -> one bounds check per pixel and k-block)
+//   A[pixel][k]  = X[n][ic][oy*s+u*d-pad][ox*s+v*d-pad]   (0 outside the image: the im2col rule)
 //
-//   M tile     = 128 output pixels = four 32-pixel row segments ("boxes", consecutive in (n, oy, ox/32) order; along the
-//                FLATTENED pixel index when the image is narrower than a box, and a 4 x 32 patch in the 3x3 slab kernel);
-//                pixel <-> TMEM lane.
-//   A operand  = lives in TENSOR MEMORY.  Twelve producer warps (3 groups x 4; group g serves every third k-block) each
-//                own 32 pixels (= their TMEM lane quadrant) and write the split operand with tcgen05.st into the ring.
-//                Where the 32 k-values of a pixel come from (template parameter SK):
-//                  1  3x3 / stride 1, IC % 32 == 0: the fp32 halo of the patch for 32 channels arrives ONCE by TMA (a
-//                     {48 columns, 6 rows, 32 channels} box, OOB zero fill = the padding); a k-block = one tap = 32 LDS.32
-//                     with immediate offsets.
-//                  2  1x1 / stride 1: four TMA boxes {32 pixels, 32 channels} per k-block, laid [channel][pixel].
-//                  0  everything else: gathered from global memory (coalesced across lanes along x, the NEXT k-block's
-//                     loads in flight while the current one is split); IC % 32 == 0: a k-block is one tap x 32 channels
-//                     -> one predicate, one IMAD.WIDE per address, otherwise offsets / taps from a small k-table.
-//                (TMA cannot gather a shifted tap: its innermost box coordinate must be 16-byte aligned; an A tile in
-//                shared memory costs 3x the instructions and +33 cycles per MMA.)
-//   arithmetic = template parameter PLANES: 3 (default) BF16x3 — x = p1 + p2 + r with p1 = RN_bf16(x), p2 = RN_bf16(x - p1),
-//                three kind::f16 MMAs p2*q1 + p1*q2 + p1*q1 per k-step of 16 (two values per TMEM column, 32 columns per
-//                ring stage, 8 stages); 2 = 3xTF32 (hi = x & 0xFFFFE000, lo = x - hi, three kind::tf32 MMAs per k-step of
-//                8, 64 columns per stage, 4 stages); 1 = plain TF32.
+//   M tile     = 128 output pixels, consecutive along the flattened (n, oy, ox) index; with a fused 2x2 max pooling a
+//                2-row x 64-column patch instead, laid out so that the four pixels of a pooling window sit in one thread
+//                (rows g, g + 8 of its fragment) and its neighbour lane (lane ^ 4).
+//   A operand  = gathered by the consumer threads straight from global memory into the registers of their wgmma
+//                fragment (the next k-block's loads are in flight while the current one is multiplied), split on chip:
+//                PLANES 3 (default) BF16x3 — x = p1 + p2 + r with p1 = RN_bf16(x), p2 = RN_bf16(x - p1), three bf16 MMAs
+//                p2*q1 + p1*q2 + p1*q1 per k-step of 16; 2 = 3xTF32 (hi = x & 0xFFFFE000, lo = x - hi, three tf32 MMAs per
+//                k-step of 8); 1 = plain TF32.
 //   B operand  = filters re-packed once at Init, K-major.  BF16x3: two bf16 planes PRE-TILED in global memory in the
-//                un-swizzled core-matrix order of tcgen05, [k-block][N tile][plane][row/8][16-byte k chunk][row%8][8]:
-//                a ring stage is one contiguous run, fetched by ONE cp.async.bulk.  3xTF32 / TF32: Wp[oc][k] fp32 rows
-//                (hi / lo planes), TMA tensor loads with the 128-byte swizzle.  One barrier per ring slot counts the 4
-//                producer arrivals and the copy's bytes.
-//   MMA        = tcgen05.mma with A from TMEM ("TS" form), issued by TWO elected threads that alternate k-blocks at
-//                N <= 64 (one accumulator each, folded in a fixed order by the epilogue: deterministic), one at N = 128;
-//                fp32 accumulators in a ring next to the A ring.
-//   epilogue   = tcgen05.ld -> +bias (staged in smem) [-> + residual, prefetched: fused Eltwise SUM] -> ReLU -> NCHW through
-//                a [channel][pixel] staging tile and one TMA store per 32-channel chunk; the fused 2x2 max-pool goes through
-//                swizzled shared memory (lane = channel).
-//   roles      = 20 warps: 0-3 epilogue, 4-15 producers (TMEM quadrant = warp % 4), 16 filter TMA, 17-18 MMA issuers, 19 slab TMA.
-//   hand-offs  = every role's loop is a chain of long-latency instructions (a barrier probe answers after ~200 cycles, a
-//                thread starts a TMA operation every ~280): TMA is issued by several lanes in lockstep, each owning its
-//                ring slots; issuers and slab producers probe the barrier of their NEXT k-block before working on the
-//                current one; every shared-memory access is an explicit ld/st.shared (a pointer into the dynamic array is
-//                generic to nvcc).  DESIGN.md section 3 has the measurements.
+//                un-swizzled core-matrix order of wgmma, [k-block][N tile][plane][row/8][16-byte k chunk][row%8][8]: a ring
+//                stage is one contiguous run fetched by ONE cp.async.bulk.  3xTF32 / TF32: Wp[oc][k] fp32 rows (hi / lo
+//                planes), TMA tensor loads with the 128-byte swizzle.  A producer warp keeps a 4-deep ring ahead.
+//   MMA        = wgmma.mma_async, A from registers, B from shared memory, fp32 register accumulators (two warpgroups of
+//                64 pixels).
+//   epilogue   = +bias [+ residual: fused Eltwise SUM] -> ReLU [-> 2x2 max pooling by one shuffle] -> NCHW stores.
 //
 // Used where non-fused Winograd is bandwidth-bound (large images, <= 128 channels) and for every layer the reference
-// sends to im2col + SGEMM (1x1, strided, 7x7, IC = 3, small images).  Measurements behind these choices: DESIGN.md section 3,
-// tests/cuda/mma_rate.cu, tests/cuda/igemm_trace.cu, tests/cuda/store_rate.cu.
+// sends to im2col + SGEMM (1x1, strided, 7x7, IC = 3, small images).
 #include "conv_igemm.cuh"
 
 #include "common.cuh"
 
 #include <stdlib.h>
-#include "tcgen05.cuh"
+#include <string.h>
+#include "wgmma.cuh"
 #include <cuda_bf16.h>
 
 namespace fcuda {
 
-// Optional timeline of CTA 0 (tests/cuda/igemm_trace.cu builds this file with -DFCUDA_IGEMM_TRACE): clock64() of the
-// hand-offs of the first 64 k-blocks, one row per event kind.
-#ifdef FCUDA_IGEMM_TRACE
-__device__ long long g_igemm_trace[16 * 64];
-#define IG_TRACE(slot, idx)                                                                              \
-    do {                                                                                                 \
-        if (blockIdx.x == 0 && (threadIdx.x & 31) == 0 && (idx) < 64u) g_igemm_trace[(slot) * 64 + (idx)] = clock64(); \
-    } while (0)
-#define IG_TRACE_T(slot, idx)  /* already single-threaded */                                           \
-    do {                                                                                                 \
-        if (blockIdx.x == 0 && (idx) < 64u) g_igemm_trace[(slot) * 64 + (idx)] = clock64();               \
-    } while (0)
-int igemm_trace_read(long long* host) {
-    return cudaMemcpyFromSymbol(host, g_igemm_trace, sizeof(long long) * 16 * 64) == cudaSuccess ? 0 : -1;
-}
-#else
-#define IG_TRACE(slot, idx) do {} while (0)
-#define IG_TRACE_T(slot, idx) do {} while (0)
-#endif
-
 namespace {
 
-constexpr int kGroups = 3;                                // producer groups, 4 warps (128 pixels) each
-constexpr int kWarpTma = 4 + 4 * kGroups;                  // warps 0-3 epilogue, 4.. producers (quadrant = warp % 4),
-constexpr int kWarpMma = kWarpTma + 1;                    // then one TMA(B) warp and TWO MMA-issuer warps (see the kernel)
-constexpr int kIssuers = 2;
-constexpr int kWarpSlab = kWarpMma + kIssuers;             // SLAB kernels: TMA producer of the input slabs (idle otherwise)
-constexpr int kThreadsIg = (kWarpSlab + 1) * 32;
-// Ring depth shared by the smem B tiles and the TMEM A tiles.  3xTF32: 4 (4 x 64 A columns + 256 accumulator columns fill
-// tensor memory).  BF16x3: 8 — its A stage is 32 columns and its filter stage half the bytes, and the ring was the limiter:
-// with 4 slots VGG conv1_2 ran a k-block every ~610 cycles in BOTH modes (ncu launch list r02o: 1.10 ms -> 1.04 ms although
-// the MMA time per k-block fell from 384 to 192 cycles) — a slot's cycle free -> produce -> full -> MMA -> retire -> free is a
-// ~2,400-cycle latency chain, so throughput = slots / chain.
-__host__ __device__ constexpr int igemm_stages(int planes) { return planes == 3 ? 8 : 4; }
-constexpr int kMaxTableK = 6144;                          // k-table entries that fit beside the B ring and the staging tiles
+constexpr int kConsumerWarps = 8;                      // two warpgroups x 64 pixels
+constexpr int kThreadsIg = (kConsumerWarps + 1) * 32;  // + the filter producer warp
+constexpr int kStagesIg = 4;
+constexpr int kMaxTableK = 6144;                       // k-table entries that fit beside the filter ring
 
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
                                   const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
@@ -125,1063 +73,244 @@ struct IgemmArgs {
     int K;                   // KH*KW*IC
     int kblocks;             // ceil(K / 32)
     int use_table;           // 0 => IC % 32 == 0: every k-block is 32 channels of ONE tap, offsets are arithmetic
-    int bpr;                 // 32-pixel boxes per output row
-    int per_img;             // OH * bpr boxes per image
-    unsigned long long m_per_img, m_bpr, m_num_n;  // ceil(2^64 / d): n / d == umul64hi(n, m) for any 32-bit n (d > 1)
-    int oc_pad;              // num_n * BN: floats of the bias copy in shared memory
-    long long total_boxes;   // N * OH * bpr  (< 2^31, checked on the host)
+    int taps;                // KH*KW
     int num_n;               // ceil(OC / BN)
-    long long pixel_tiles;   // ceil(total_boxes / 4)
+    long long total_pix;     // N * OH * OW
     int relu;
-    int issuers;             // MMA issuer threads: 2 when BN <= 64 and the tile has >= 2 k-blocks, else 1
-    int acc_stride;          // TMEM columns per accumulator slot: BN, or 2*BN with two issuers (one accumulator each)
-    int acc_slots;           // accumulator ring depth = accumulator columns / acc_stride (power of two, <= 4)
-    int tma_out;             // epilogue stores through shared memory + TMA (tmOut is valid); pooled tiles keep direct stores
-    int pool;                // SLAB only: fuse a following 2x2 / stride-2 max pooling; `out` is the pooled blob
-    int2 ktab1[32];          // use_table == 2 (K <= 32, e.g. IC = 3 first layers): the k-table in the kernel parameters
+    int pool;                // fuse a following 2x2 / stride-2 max pooling; `out` is the pooled blob
+    int tiles_x, tiles_y;    // pool: 64-column x 2-row patches per image
     const unsigned char* wbf;  // BF16x3: pre-tiled filter planes (see igemm_pack_weights_bf16_kernel)
     unsigned wbf_kb_bytes;     // bytes of one k-block (both planes, every N tile): 2 * ocpad * 64
-    int flat_ow;             // > 0: output pixels are boxed along the FLATTENED index oy * OW + ox (OH = 1, OW = OH*OW in this
-                             // struct) and flat_ow is the real output width the producers divide by (small images)
-    unsigned long long m_flat_ow;
-    int tma_lanes;           // lanes of the filter-TMA warp that issue in lockstep (1, 2 or 4)
-    unsigned suspend_ns;     // suspend hint of the ring / slab / accumulator waits (0 = poll), see ptx::mbar_try_wait_ns
-    int taps;                // KH*KW
-    unsigned tap_inv;        // ceil(65536 / KW): tap / KW == (tap * tap_inv) >> 16 for tap < 64
 };
 
-struct BoxCoord { int n, oy, ox0; bool valid; };
-
-// n / d for 32-bit n with the host-made multiplier m = ceil(2^64 / d); exact because n * d < 2^64.
-__device__ __forceinline__ uint32_t fast_div(uint32_t n, unsigned long long m, int d) {
-    return d == 1 ? n : static_cast<uint32_t>(__umul64hi(static_cast<unsigned long long>(n), m));
+// The k index (inside a 32-wide k-block) of fragment element j of lane column c: tf32 k-steps of 8 hold (c, c + 4),
+// bf16 k-steps of 16 hold the pairs (2c, 2c + 1) and (2c + 8, 2c + 9).
+template <bool BF>
+__device__ __forceinline__ int frag_k(int j, int c) {
+    return BF ? (j >> 2) * 16 + 2 * c + (j & 1) + 8 * ((j >> 1) & 1) : (j >> 1) * 8 + c + 4 * (j & 1);
 }
 
-__device__ __forceinline__ BoxCoord decode_box(uint32_t b, const IgemmArgs& a) {
-    BoxCoord c;
-    c.valid = b < static_cast<uint32_t>(a.total_boxes);
-    const uint32_t n = fast_div(b, a.m_per_img, a.per_img);
-    const uint32_t rem = b - n * static_cast<uint32_t>(a.per_img);
-    const uint32_t oy = fast_div(rem, a.m_bpr, a.bpr);
-    c.n = static_cast<int>(n);
-    c.oy = static_cast<int>(oy);
-    c.ox0 = static_cast<int>(rem - oy * static_cast<uint32_t>(a.bpr)) * 32;
-    return c;
-}
-
-// SLAB mode: a tile is a 4-row x 32-column patch of one image, tiles enumerated as (n, oy/4, ox/32); args.per_img =
-// ceil(OH/4) * bpr tiles per image, args.total_boxes = 4 * number of tiles.  Warp (TMEM quadrant) q covers the 2 x 16
-// sub-patch rows 2*(q>>1) .. +1, columns 16*(q&1) .. +15: lane l = row (l >> 4), column (l & 15).  Both pixels of a 2x2
-// pooling window then sit in ONE warp (lane ^ 16, lane ^ 1) and the epilogue can pool with two shuffles.
-__device__ __forceinline__ BoxCoord decode_patch(uint32_t ptile, const IgemmArgs& a) {  // oy / ox0 = patch origin
-    BoxCoord c;
-    const uint32_t n = fast_div(ptile, a.m_per_img, a.per_img);
-    const uint32_t rem = ptile - n * static_cast<uint32_t>(a.per_img);
-    const uint32_t ty = fast_div(rem, a.m_bpr, a.bpr);
-    c.n = static_cast<int>(n);
-    c.oy = static_cast<int>(ty) * 4;
-    c.ox0 = static_cast<int>(rem - ty * static_cast<uint32_t>(a.bpr)) * 32;
-    c.valid = ptile * 4u < static_cast<uint32_t>(a.total_boxes);
-    return c;
-}
-__device__ __forceinline__ int patch_row(int q, int lane) { return 2 * (q >> 1) + (lane >> 4); }
-__device__ __forceinline__ int patch_col(int q, int lane) { return 16 * (q & 1) + (lane & 15); }
-
-// 3x3 / stride-1 slab: the raw fp32 halo of a 4 x 32 output patch for one 32-channel block, landed by TMA: a
-// {48 columns, 6 rows, 32 channels} box of the NCHW input whose first column is the patch's first column minus 4 (the TMA's
-// innermost start coordinate must be a multiple of 16 bytes — measured, tests/cuda/tma_shift.cu; negative / past-the-end
-// coordinates are zero-filled, which IS the convolution's padding).  48 columns make the row stride 16 banks, so the two
-// half-warps of the 2 x 16 lane mapping read disjoint banks.
-constexpr int kSlabRows = 6, kSlabCols = 48, kSlabShift = 4;
-constexpr int kSlabChBytes = kSlabRows * kSlabCols * 4;       // 1,152 B per channel
-constexpr int kSlabStageBytes = 32 * kSlabChBytes;            // 36,864 B per (tile, channel block)
-__host__ __device__ constexpr int slab_stages(int bn) { return bn <= 64 ? 3 : 2; }
-
-// Pointwise slab (slab kind 2; 1x1 / stride 1 / no padding, each image addressed as one H*W-long row): the A tile of a
-// k-block — 128 pixels x 32 channels — is four {32 pixels, 32 channels} boxes of the NCHW input, one per TMEM lane quadrant
-// (a box never leaves its image; the part past the image end is zero-filled), landed by TMA as [channel][pixel] rows of
-// 128 bytes.  The producers then need no addresses, predicates or load latency: 32 conflict-free LDS.32 (lane = pixel)
-// with immediate offsets, the split, the tensor-memory stores.  Replaces the 32 LDG + IMAD.WIDE per thread and k-block of
-// the generic gather, which paced every short-K pointwise layer of ResNet-50 / MobileNet (0.08 of the tensor peak, 0.26
-// of HBM in round 1).
-constexpr int kPwBoxBytes = 32 * 32 * 4;              // one quadrant's box
-constexpr int kPwStageBytes = 4 * kPwBoxBytes;        // 16 KB per k-block
-__host__ __device__ constexpr int pw_stages(int bn, int planes) { return bn > 64 && planes >= 2 ? 3 : 6; }
-constexpr int kMaxSlabStages = 6;
-
-__device__ __forceinline__ void tma_load_4d(void* smem_dst, const CUtensorMap* map, uint64_t* bar, int c0, int c1, int c2,
-                                            int c3) {
-    asm volatile(
-        "cp.async.bulk.tensor.4d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], [%2];"
-        ::"r"(ptx::smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(map)), "r"(ptx::smem_u32(bar)), "r"(c0), "r"(c1),
-        "r"(c2), "r"(c3)
-        : "memory");
-}
-
-__device__ __forceinline__ void tma_store_4d(const CUtensorMap* map, const void* smem_src, int c0, int c1, int c2, int c3) {
-    asm volatile("cp.async.bulk.tensor.4d.global.shared::cta.bulk_group [%0, {%2, %3, %4, %5}], [%1];"
-                 ::"l"(reinterpret_cast<uint64_t>(map)), "r"(ptx::smem_u32(smem_src)), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
-                 : "memory");
-}
-
-// Ring-slot release.  A producer group visits only every third k-block and the two MMA issuers retire their k-blocks
-// independently of each other, so with ONE mbarrier per slot "the MMAs of k-block g-4 have retired" cannot be read off the
-// parity: a group whose last visit to the slot was three rounds ago sees the same parity when the lagging issuer is
-// still two rounds behind (observed with the fast slab producers: an unconsumed A tile was overwritten).  Each slot
-// therefore has TWO release barriers used by alternating rounds (round = g / STAGES): the barrier of round r completes a
-// phase every second round, so its parity distinguishes rounds r, r+2 and r-2, and being four rounds ahead is impossible —
-// the group's previous k-blocks g-3, g-6 needed slots released by BOTH issuers (odd and even k-blocks), each of which
-// retires in order.  Waiting too long cannot happen either: the barrier only advances again after g itself is consumed.
-template <int STAGES>
-__device__ __forceinline__ uint64_t* ring_release_bar(uint64_t (*empty_bar)[STAGES], uint32_t g) {
-    return &empty_bar[(g / STAGES) & 1u][g & (STAGES - 1)];
-}
-template <int STAGES>
-__device__ __forceinline__ void wait_ring_slot_free(uint64_t (*empty_bar)[STAGES], uint32_t g, uint32_t ns) {
-    if (g >= STAGES) {
-        const uint32_t gg = g - STAGES;  // the k-block that used this slot one round earlier
-        ptx::mbar_wait(ring_release_bar<STAGES>(empty_bar, gg), ((gg / STAGES) >> 1) & 1u, ns);
-    }
-}
-
-// Non-blocking look at the same condition: lets a role ask about its NEXT k-block before it starts the work of the current
-// one, so the ~200-cycle latency of the barrier probe (SYNCS.PHASECHK) hides under that work instead of heading the next
-// iteration's dependency chain.
-template <int STAGES>
-__device__ __forceinline__ bool probe_ring_slot_free(uint64_t (*empty_bar)[STAGES], uint32_t g) {
-    if (g < STAGES) return true;
-    const uint32_t gg = g - STAGES;
-    return ptx::mbar_test(ring_release_bar<STAGES>(empty_bar, gg), ((gg / STAGES) >> 1) & 1u);
-}
-
-// D[tmem] (+)= A[tmem] * B[smem]
-__device__ __forceinline__ void umma_tf32_ts(uint32_t tmem_d, uint32_t tmem_a, uint64_t desc_b, uint32_t idesc,
-                                             uint32_t accumulate) {
-    asm volatile(
-        "{\n\t"
-        ".reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::tf32 [%0], [%1], %2, %3, p;\n\t"
-        "}"
-        ::"r"(tmem_d), "r"(tmem_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-
-// D[tmem] (+)= A[tmem] * B[smem], bf16 operands (two per TMEM column / 64-byte swizzled smem rows), K = 16
-__device__ __forceinline__ void umma_bf16_ts(uint32_t tmem_d, uint32_t tmem_a, uint64_t desc_b, uint32_t idesc,
-                                             uint32_t accumulate) {
-    asm volatile(
-        "{\n\t"
-        ".reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n\t"
-        "}"
-        ::"r"(tmem_d), "r"(tmem_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-
-// cta_group::2: one thread of the pair's leader CTA issues for both SMs (M = 256: lanes 0-127 of each CTA's tensor memory)
-__device__ __forceinline__ void umma_tf32_ts_cg2(uint32_t tmem_d, uint32_t tmem_a, uint64_t desc_b, uint32_t idesc,
-                                                 uint32_t accumulate) {
-    asm volatile(
-        "{\n\t"
-        ".reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::2.kind::tf32 [%0], [%1], %2, %3, p;\n\t"
-        "}"
-        ::"r"(tmem_d), "r"(tmem_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-
-__device__ __forceinline__ void tmem_st_32x8(uint32_t taddr, const uint32_t (&r)[8]) {
-    asm volatile(
-        "tcgen05.st.sync.aligned.32x32b.x8.b32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8};"
-        ::"r"(taddr), "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7])
-        : "memory");
-}
-// Explicit shared-memory load: through a generic pointer derived from the dynamic shared array nvcc emitted LD.E (generic
-// address path, long-scoreboard latency) for every slab read of the producers (profiles/r02r source page).
-__device__ __forceinline__ float lds_f32(uint32_t smem_addr) {
-    float v;
-    asm volatile("ld.shared.f32 %0, [%1];" : "=f"(v) : "r"(smem_addr));
-    return v;
-}
-__device__ __forceinline__ float4 lds_f32x4(uint32_t smem_addr) {
-    float4 v;
-    asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "r"(smem_addr));
-    return v;
-}
-__device__ __forceinline__ void sts_f32(uint32_t smem_addr, float v) {
-    asm volatile("st.shared.f32 [%0], %1;" ::"r"(smem_addr), "f"(v) : "memory");
-}
-// 1-D bulk copy global -> shared (16-byte aligned, size a multiple of 16), completion on an mbarrier
-__device__ __forceinline__ void bulk_load_1d(void* smem_dst, const void* gmem_src, uint32_t bytes, uint64_t* bar) {
-    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
-                 ::"r"(ptx::smem_u32(smem_dst)), "l"(gmem_src), "r"(bytes), "r"(ptx::smem_u32(bar))
-                 : "memory");
-}
-__device__ __forceinline__ void tmem_st_wait() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
-
-// CG = 2: a CTA PAIR (thread-block cluster of 2, cta_group::2) works on 256 output pixels x BN channels: each CTA gathers /
-// stages the A rows of ITS 128 pixels into its own tensor memory and holds HALF of the filter tile (BN/2 rows) in its own
-// shared memory; one thread of the leader CTA issues M = 256 MMAs that read A from both tensor memories and B from both
-// shared memories.  Why: every tcgen05 kernel of this engine sat at ~105 B/clk of shared-memory traffic per SM (ncu
-// r02h: MMA filter reads 64 B/clk + filter TMA writes 43 + slab LDS 43 at N = 64; tensor pipe 65 % on VGG conv1_2, 82 % on
-// conv2_x) — the pair halves the first two terms per SM.  Cross-CTA hand-offs: the peer's producers and a relay warp (which
-// watches the peer's filter TMA) arrive REMOTELY on the leader's full barrier; the leader's tcgen05.commit multicasts the
-// slot-release and accumulator-ready arrivals to both CTAs; the peer's epilogue warps release the accumulator remotely.
-template <int BN, int PLANES, int SK, int CG>
+template <int BN, int PLANES>
 __global__ void __launch_bounds__(kThreadsIg, 1)
 conv_igemm_kernel(const __grid_constant__ CUtensorMap tmW, const __grid_constant__ CUtensorMap tmWlo,
-                  const __grid_constant__ CUtensorMap tmIn, const __grid_constant__ CUtensorMap tmOut,
                   const IgemmArgs args) {
-    constexpr int STAGES = igemm_stages(PLANES);
-    constexpr bool SLAB = SK == 1;                          // 3x3 / stride-1 halo slabs (patch-shaped tiles)
-    constexpr bool PW = SK == 2;                            // pointwise slabs (box-shaped tiles, like the generic gather)
-    static_assert(!(PW && CG == 2), "pairs are not combined with the pointwise slab");
-    // PLANES: 1 = TF32, 2 = 3xTF32, 3 = BF16x3 (operands split into two bf16 planes p1 = RN(x), p2 = RN(x - p1); three
-    // kind::f16 MMAs p2*q1 + p1*q2 + p1*q1 per k-step of SIXTEEN — twice the tensor throughput of 3xTF32 and half the
-    // shared-memory / tensor-memory operand bytes, dropped terms <= 3 * 2^-16 of a product)
     constexpr bool BF = PLANES == 3;
-    constexpr int NPL = BF ? 2 : PLANES;                    // operand planes in memory
-    static_assert(!(BF && CG == 2), "pairs are a TF32 variant");
-    constexpr int kBRows = BN / CG;                         // filter rows this CTA holds (CG = 2: half of the N tile)
-    constexpr int kBTile = kBRows * 32 * (BF ? 2 : 4);      // 32 k-values per row: 128 B of fp32 / 64 B of bf16
-    constexpr int kStage = NPL * kBTile;                    // smem per stage: [B_hi][B_lo]
-    static_assert(CG == 1 || kBRows % 8 == 0, "whole swizzle atoms per CTA");
-    // accumulator ring: as deep as tensor memory allows next to the A ring (4 x 64 columns in 3xTF32 mode).  Tiles with few
-    // k-blocks (IC = 3, pointwise layers) are a latency chain gather -> MMA -> epilogue; with 2 slots conv1_1 of VGG
-    // spent 3.8k cycles per tile for ~1k cycles of work in any one role.
-    constexpr int ACC = 4;                                  // barrier array size; args.acc_slots (<= 4) slots are in use
-    constexpr uint32_t kAccCols = BN <= 64 ? 256 : 2 * BN;  // carved at run time into args.acc_slots slots of args.acc_stride
-    constexpr uint32_t kAPlaneCols = BF ? 16 : 32;          // 32 k-values: fp32 columns, or bf16 pairs
-    constexpr uint32_t kAStageCols = kAPlaneCols * NPL;     // [A_hi][A_lo]
-    constexpr uint32_t kNeedCols = kAccCols + STAGES * kAStageCols;
-    constexpr uint32_t kTmemCols = kNeedCols <= 32 ? 32 : kNeedCols <= 64 ? 64 : kNeedCols <= 128 ? 128 : kNeedCols <= 256 ? 256 : 512;
-    static_assert(kNeedCols <= 512, "TMEM budget");
-
+    constexpr int NPL = BF ? 2 : PLANES;                  // operand planes in memory
+    constexpr int kBTile = BN * 32 * (BF ? 2 : 4);        // 32 k-values per row: 128 B of fp32 / 64 B of bf16
+    constexpr int kStage = NPL * kBTile;                  // [B_hi][B_lo]
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-    int2* ktab = reinterpret_cast<int2*>(smem + STAGES * kStage + 4 * ((SLAB && BN == 128 && CG == 1) ? 1 : 2) * 4096);  // {element offset, tap index} per k (non-SLAB)
-
-    // one barrier per ring slot covers both operands: 4 arrivals of the owning producer group (A in tensor memory)
-    // + 1 arrive.expect_tx of the TMA warp (B bytes landed) -> the MMA thread makes ONE wait per k-block
-    __shared__ uint64_t full_bar[STAGES];
-    __shared__ uint64_t bfull_bar[STAGES];     // CG = 2, peer CTA: its half of the filter tile has landed (relayed to the leader)
-    __shared__ uint64_t empty_bar[2][STAGES];  // MMAs that read the stage have retired; [round parity][slot], see wait_ring_slot_free
-    __shared__ uint64_t slab_full[kMaxSlabStages];    // SLAB: TMA landed the slab of an item (tile, channel block); PW: of a k-block
-    __shared__ uint64_t slab_empty[kMaxSlabStages];   // SLAB: all twelve producer warps have served the item's nine taps; PW: the
-                                                      // four warps of the k-block's group have read their boxes
-    __shared__ uint64_t tmem_full_bar[ACC];
-    __shared__ uint64_t tmem_empty_bar[ACC];
-    __shared__ uint32_t tmem_base_smem;
+    int2* ktab = reinterpret_cast<int2*>(smem + kStagesIg * kStage);  // use_table: {element offset, dy << 16 | dx} per k
+    __shared__ uint64_t full_bar[kStagesIg];
+    __shared__ uint64_t empty_bar[kStagesIg];
 
     const int warp = threadIdx.x >> 5;
     const int lane = threadIdx.x & 31;
-    // work items: (pixel tile or pair of pixel tiles, n-block); this CTA's pixel tile = item * CG + rank
-    const long long total_tiles = args.pixel_tiles * args.num_n;   // host: pixel_tiles already counts pairs when CG = 2
+    const int n_blk = static_cast<int>(blockIdx.x % static_cast<unsigned>(args.num_n));
+    const long long ptile = blockIdx.x / static_cast<unsigned>(args.num_n);
     const int kblocks = args.kblocks;
     const int plane = args.H * args.W;
-    const uint32_t cta_rank = CG == 1 ? 0u : ptx::cluster_ctarank();
-    const long long tile_first = CG == 1 ? static_cast<long long>(blockIdx.x) : static_cast<long long>(ptx::cluster_id_x());
-    const long long tile_step = CG == 1 ? static_cast<long long>(gridDim.x) : static_cast<long long>(ptx::cluster_count_x());
 
     if (threadIdx.x == 0) {
-        for (int s = 0; s < STAGES; ++s) {
-            // leader: own filter TMA (1) + own 4 producer warps, + with CG = 2 the peer's 4 producer warps and its relay
-            ptx::mbar_init(&full_bar[s], CG == 1 ? 5 : 10);
-            ptx::mbar_init(&bfull_bar[s], 1);
-            ptx::mbar_init(&empty_bar[0][s], 1);
-            ptx::mbar_init(&empty_bar[1][s], 1);
-        }
-        for (int s = 0; s < ACC; ++s) {
-            ptx::mbar_init(&tmem_full_bar[s], static_cast<uint32_t>(args.issuers));  // every issuer commits its own MMAs
-            ptx::mbar_init(&tmem_empty_bar[s], 4 * CG);  // CG = 2: the peer's epilogue warps arrive remotely on the leader's
-        }
-        for (int s = 0; s < kMaxSlabStages; ++s) {
-            ptx::mbar_init(&slab_full[s], 1);
-            ptx::mbar_init(&slab_empty[s], PW ? 4 : 4 * kGroups);
+        for (int s = 0; s < kStagesIg; ++s) {
+            ptx::mbar_init(&full_bar[s], 1);
+            ptx::mbar_init(&empty_bar[s], kConsumerWarps);
         }
         ptx::fence_barrier_init();
     }
-    if (warp == kWarpTma && lane == 0) {
-        ptx::prefetch_tensormap(&tmW);
-        if (NPL == 2) ptx::prefetch_tensormap(&tmWlo);
-        if (SLAB || PW) ptx::prefetch_tensormap(&tmIn);
-    }
-    if (args.use_table == 1) {
+    if (args.use_table) {
         for (int k = threadIdx.x; k < kblocks * 32; k += kThreadsIg) {
-            int2 e = make_int2(0, 63);  // padding rows: tap 63 is never valid
+            int2 e = make_int2(0, 0);
             if (k < args.K) {
                 const int tap = k / args.IC, ic = k - tap * args.IC;
-                const int u = tap / args.KW, v = tap - u * args.KW;
-                e = make_int2(ic * plane + u * args.dil_h * args.W + v * args.dil_w, tap);
+                const int dy = (tap / args.KW) * args.dil_h, dx = (tap % args.KW) * args.dil_w;
+                e = make_int2(ic * plane + dy * args.W + dx, (dy << 16) | dx);
             }
             ktab[k] = e;
         }
     }
-    // bias copy (zeros when the layer has none): the epilogue reads it with broadcast LDS.128
-    // SLAB: the input-slab ring sits right behind the filter ring (both multiples of 1 KB), then the bias copy
-    constexpr int SST = PW ? pw_stages(BN, PLANES) : slab_stages(BN);
-    constexpr int kRingBytes = SLAB ? SST * kSlabStageBytes : PW ? SST * kPwStageBytes : 0;
-    uint8_t* slab0 = smem + STAGES * kStage;
-    // epilogue staging tiles of the TMA-store path: kOutBufs x 4 KB per epilogue warp, right behind the slab ring
-    constexpr int kOutBufs = (SLAB && BN == 128 && CG == 1) ? 1 : 2;
-    uint8_t* stage_out = smem + STAGES * kStage + kRingBytes;
-    float* bias_s = reinterpret_cast<float*>(stage_out + 4 * kOutBufs * 4096 + (args.use_table == 1 ? kblocks * 32 * 8 : 0));
-
-    for (int i = threadIdx.x; i < args.oc_pad; i += kThreadsIg)
-        bias_s[i] = (args.bias != nullptr && i < args.OC) ? __ldg(args.bias + i) : 0.f;
-    if (warp == kWarpMma) {
-        if (CG == 1) {
-            ptx::tmem_alloc(&tmem_base_smem, kTmemCols);
-            ptx::tmem_relinquish();
-        } else {
-            ptx::tmem_alloc_cg2(&tmem_base_smem, kTmemCols);
-            ptx::tmem_relinquish_cg2();
-        }
-    }
-    ptx::tc_fence_before();
     __syncthreads();
-    if (CG == 2) ptx::cluster_sync_all();  // the peer's barriers exist before anyone arrives on them remotely
-    ptx::tc_fence_after();
-    const uint32_t tmem_base = tmem_base_smem;
-    const uint32_t tmem_a0 = tmem_base + kAccCols;
 
-    if (warp == kWarpTma) {
-        // ===================== TMA producer for the filter tiles =====================
-        // One thread can start a TMA operation only every ~280 cycles (tests/cuda/store_rate.cu: 276 cycles per bulk copy and
-        // issuing thread whatever its size, throughput scaling with the number of issuing threads), and the slot wait, the
-        // expect_tx arrive and the copy are a chain of long-latency SYNCS / UTMA instructions: ~560 cycles per k-block when
-        // ONE thread walked the k-blocks (igemm trace r02v) — that chain, not the tensor pipe or any bandwidth, paced every
-        // implicit-GEMM layer (VGG conv1_2 took 1.04-1.10 ms whatever the MMA mode, ring depth or filter layout was).
-        // So kTmaLanes lanes of this warp each take every kTmaLanes-th k-block and run the chain in lockstep: one
-        // instruction issue starts kTmaLanes copies.  (Lane j of a round needs the slot k-block g+j-STAGES used, whose filters
-        // were requested one or two rounds earlier: no cycle as long as kTmaLanes <= STAGES.)
-        // kTmaLanes (1, 2 or 4: divides the ring depth, so a lane owns its slots and meets every phase of their barriers) trades
-        // issue rate against prefetch distance: a round starts when the slot of its LAST k-block is free, so STAGES -
-        // kTmaLanes + 1 k-blocks of filters can be in flight ahead of the MMAs.
-        const int kTmaLanes = args.tma_lanes;
-        static_assert(STAGES % 4 == 0, "1, 2 or 4 lanes own whole ring slots");
-        if (lane < kTmaLanes) {
-            long long tile = tile_first;
-            int kb = lane;
-            uint32_t gb = static_cast<uint32_t>(lane);
-            for (;;) {
-                while (kb >= kblocks && tile < total_tiles) { kb -= kblocks; tile += tile_step; }
-                if (tile >= total_tiles) break;
-                const uint32_t pt = fast_div(static_cast<uint32_t>(tile), args.m_num_n, args.num_n);
-                const int n_blk = static_cast<int>(static_cast<uint32_t>(tile) - pt * static_cast<uint32_t>(args.num_n));
-                const int stage = static_cast<int>(gb & (STAGES - 1));
-                if (lane == 0) IG_TRACE_T(11, gb);
-                wait_ring_slot_free<STAGES>(empty_bar, gb, args.suspend_ns);
-                if (lane == 0) IG_TRACE_T(8, gb);
+    if (warp == kConsumerWarps) {
+        // ===================== filter producer =====================
+        if (lane == 0) {
+            if (!BF) {
+                ptx::prefetch_tensormap(&tmW);
+                if (NPL == 2) ptx::prefetch_tensormap(&tmWlo);
+            }
+            for (int kb = 0; kb < kblocks; ++kb) {
+                const int stage = kb % kStagesIg;
+                if (kb >= kStagesIg) ptx::mbar_wait(&empty_bar[stage], ((kb / kStagesIg) - 1) & 1);
                 uint8_t* st = smem + stage * kStage;
-                // CG = 2: rows [rank * BN/2, (rank+1) * BN/2) of the N tile; the peer CTA's copy completes on ITS bfull
-                // barrier, which its relay warp forwards to the leader CTA's full barrier
-                uint64_t* bar = (CG == 2 && cta_rank != 0) ? &bfull_bar[stage] : &full_bar[stage];
-                const int row0 = n_blk * BN + static_cast<int>(cta_rank) * kBRows;
-                ptx::mbar_arrive_expect_tx(bar, NPL * kBTile);
+                ptx::mbar_arrive_expect_tx(&full_bar[stage], kStage);
                 if (BF) {
-                    // BF16x3: [k-block][N tile][plane][BN rows x 64 B] in global memory, already in the shared-memory
-                    // (core-matrix) order: both planes of the tile are ONE run of whole 128-byte lines -> one 1-D bulk copy
-                    // (as a tensor box it was BN rows of 64 bytes per plane: half-used L2 lines, two operations)
-                    const unsigned char* src = args.wbf + static_cast<size_t>(kb) * args.wbf_kb_bytes + static_cast<size_t>(n_blk) * (2 * kBTile);
-                    bulk_load_1d(st, src, 2 * kBTile, bar);
+                    ptx::bulk_load_1d(st, args.wbf + static_cast<size_t>(kb) * args.wbf_kb_bytes + static_cast<size_t>(n_blk) * kStage,
+                                      kStage, &full_bar[stage]);
                 } else {
-                    ptx::tma_load_3d(st, &tmW, bar, kb * 32, row0, 0);
-                    if (NPL == 2) ptx::tma_load_3d(st + kBTile, &tmWlo, bar, kb * 32, row0, 0);
-                }
-                if (lane == 0) IG_TRACE_T(12, gb);
-                gb += kTmaLanes;
-                kb += kTmaLanes;
-            }
-        }
-    } else if (warp >= kWarpMma && warp < kWarpSlab) {
-        // ===================== MMA issuers: two elected threads alternate k-blocks =====================
-        // Measured on B200 (tests/cuda/mma_rate.cu, tests/cuda/igemm_trace.cu): a TS-form kind::tf32 MMA of N columns
-        // executes in N/2 cycles; the pipe holds ~6 MMAs and ISSUE BLOCKS beyond that; a pipe that has run dry needs
-        // ~390 cycles before the next MMA completes; and the scalar work of one k-block (barrier wait, fence,
-        // descriptor arithmetic, commit, loop) is ~300-400 cycles of dependent single-thread issue.  One issuer therefore
-        // leaves the pipe idle about half of the time at N = 64, so two threads alternate k-blocks there.
-        // Round 2: each issuer accumulates into ITS OWN accumulator (even k-blocks -> columns [0, BN), odd -> [BN, 2BN) of
-        // the slot) and the epilogue adds the two.  Round 1 let both threads accumulate into one accumulator, handing
-        // the issue order over through a shared counter; the determinism probe (scripts/determinism_probe.py) showed the
-        // tensor pipe does not keep MMAs of two issuing warps in issue order — results differed run to run in the last
-        // bit (fp32 summation order), and an overtaken accumulate=0 MMA would have been a silent wrong result.  With
-        // disjoint accumulators there is no cross-thread ordering left: each thread's commit covers exactly its own MMAs.
-        if (CG == 2 && cta_rank != 0) {
-            // peer CTA of a pair: no MMAs are issued here.  Its first "issuer" warp relays "my half of the filter tile has
-            // landed" (a local TMA completion) to the leader's full barrier, k-block by k-block, in order.
-            if (warp == kWarpMma && ptx::elect_one()) {
-                uint32_t g = 0;
-                for (long long tile = tile_first; tile < total_tiles; tile += tile_step)
-                    for (int kb = 0; kb < kblocks; ++kb, ++g) {
-                        ptx::mbar_wait(&bfull_bar[g & (STAGES - 1)], (g / STAGES) & 1u);
-                        ptx::mbar_arrive_remote(&full_bar[g & (STAGES - 1)], 0u);
-                    }
-            }
-        } else if (ptx::elect_one()) {
-            constexpr uint32_t idesc = BF ? make_idesc_bf16(BN, 128) : make_idesc_tf32(BN, 128 * CG);
-            // BF16x3: un-swizzled core-matrix layout [row / 8][16-byte k chunk (4)][row % 8][8 bf16]: 128 bytes between the
-            // core matrices of consecutive k chunks (LBO), 512 bytes between 8-row groups (SBO)
-            const uint64_t dB0 = BF ? make_smem_desc_none(ptx::smem_u32(smem), 128, 512) : make_smem_desc_sw128(ptx::smem_u32(smem));
-            const uint32_t me = static_cast<uint32_t>(warp - kWarpMma);
-            const uint32_t nissue = static_cast<uint32_t>(args.issuers);
-            uint32_t g = me;
-            long long tile = tile_first;
-            int kb = static_cast<int>(me);
-            uint32_t it = 0;
-            bool next_full = false;  // full_bar of this thread's next k-block already seen complete (probed during the MMAs)
-            if (me >= nissue) tile = total_tiles;  // single-issuer launch: the second issuer idles
-            for (;;) {
-                while (kb >= kblocks && tile < total_tiles) { kb -= kblocks; tile += tile_step; ++it; }
-                if (tile >= total_tiles) break;
-                const int stage = static_cast<int>(g & (STAGES - 1));
-                const uint32_t phase = (g / STAGES) & 1u;
-                const uint32_t as = it & static_cast<uint32_t>(args.acc_slots - 1);
-                const uint32_t tmem_d = tmem_base + as * static_cast<uint32_t>(args.acc_stride) + me * BN;
-                const uint64_t dB = dB0 + static_cast<uint64_t>(stage * (kStage >> 4));
-                const uint64_t dBlo = dB + static_cast<uint64_t>(kBTile >> 4);
-                const uint32_t ta = tmem_a0 + stage * kAStageCols;
-                const bool first_visit = kb < static_cast<int>(nissue);  // this thread's first k-block of the tile
-                IG_TRACE_T(6, g);
-                if (CG == 1) {
-                    if (first_visit) ptx::mbar_wait(&tmem_empty_bar[as], ((it / static_cast<uint32_t>(args.acc_slots)) & 1u) ^ 1u, args.suspend_ns);
-                    if (!next_full) ptx::mbar_wait(&full_bar[stage], phase, args.suspend_ns);
-                } else {  // arrivals from the peer CTA: acquire at cluster scope
-                    if (first_visit) ptx::mbar_wait_cluster(&tmem_empty_bar[as], ((it / static_cast<uint32_t>(args.acc_slots)) & 1u) ^ 1u);
-                    ptx::mbar_wait_cluster(&full_bar[stage], phase);
-                }
-                IG_TRACE_T(5, g);
-                ptx::tc_fence_after();
-                if (CG == 1) {  // my next k-block's operands: asked now, looked at after the MMAs below are issued
-                    const uint32_t gn = g + nissue;
-                    next_full = ptx::mbar_test(&full_bar[gn & (STAGES - 1)], (gn / STAGES) & 1u);
-                }
-                if (BF) {
-#pragma unroll
-                    for (int k = 0; k < 2; ++k) {  // 16 k-values (8 TMEM columns of bf16 pairs / 32 smem bytes) per MMA
-                        const uint32_t first = (first_visit && k == 0) ? 0u : 1u;
-                        // a k-step of 16 = two 16-byte chunks = two core matrices = 256 bytes further
-                        umma_bf16_ts(tmem_d, ta + 16 + k * 8, dB + 16 * k, idesc, first);   // A_p2 * B_p1
-                        umma_bf16_ts(tmem_d, ta + k * 8, dBlo + 16 * k, idesc, 1u);         // A_p1 * B_p2
-                        umma_bf16_ts(tmem_d, ta + k * 8, dB + 16 * k, idesc, 1u);           // A_p1 * B_p1
-                    }
-                }
-#pragma unroll
-                for (int k = 0; k < (BF ? 0 : 4); ++k) {  // 8 k-values (TMEM columns / 32 smem bytes) per MMA
-                    const uint32_t first = (first_visit && k == 0) ? 0u : 1u;
-                    if (CG == 1) {
-                        if (PLANES == 2) {
-                            umma_tf32_ts(tmem_d, ta + 32 + k * 8, dB + 2 * k, idesc, first);   // A_lo * B_hi
-                            umma_tf32_ts(tmem_d, ta + k * 8, dBlo + 2 * k, idesc, 1u);         // A_hi * B_lo
-                            umma_tf32_ts(tmem_d, ta + k * 8, dB + 2 * k, idesc, 1u);           // A_hi * B_hi
-                        } else {
-                            umma_tf32_ts(tmem_d, ta + k * 8, dB + 2 * k, idesc, first);
-                        }
-                    } else {
-                        if (PLANES == 2) {
-                            umma_tf32_ts_cg2(tmem_d, ta + 32 + k * 8, dB + 2 * k, idesc, first);
-                            umma_tf32_ts_cg2(tmem_d, ta + k * 8, dBlo + 2 * k, idesc, 1u);
-                            umma_tf32_ts_cg2(tmem_d, ta + k * 8, dB + 2 * k, idesc, 1u);
-                        } else {
-                            umma_tf32_ts_cg2(tmem_d, ta + k * 8, dB + 2 * k, idesc, first);
-                        }
-                    }
-                }
-                IG_TRACE_T(14, g);
-                if (CG == 1) {
-                    ptx::umma_commit(ring_release_bar<STAGES>(empty_bar, g));
-                    if (kb + static_cast<int>(nissue) >= kblocks) ptx::umma_commit(&tmem_full_bar[as]);  // my last k-block here
-                } else {  // both CTAs of the pair: slot release for their producers / TMA, accumulator-ready for their epilogues
-                    ptx::umma_commit_cg2(ring_release_bar<STAGES>(empty_bar, g), 3);
-                    if (kb + static_cast<int>(nissue) >= kblocks) ptx::umma_commit_cg2(&tmem_full_bar[as], 3);
-                }
-                IG_TRACE_T(7, g);
-                g += nissue;
-                kb += static_cast<int>(nissue);
-            }
-        }
-    } else if (warp == kWarpSlab) {
-        // ===================== SLAB: TMA producer of the input slabs =====================
-        // one {48 x 6 x 32} box per item (tile, channel block), SST items ahead of the producers
-        if (PW) {
-            // one 16 KB stage per k-block: four {32 pixels, 32 channels} boxes, SST k-blocks ahead of the producers.  Like the
-            // filter ring (see there) the boxes are issued in lockstep: lane = k-block slot * 4 + box, kPwK k-blocks per round —
-            // one thread needed ~280 cycles per TMA operation, four boxes a k-block, against 384 cycles of MMAs at N = 128.
-            // kPwK must DIVIDE the stage count: then a stage is always visited by the same lane group, in consecutive phases of
-            // its barriers.  (With 2 groups over 3 stages a group met a stage only every other phase, where a parity wait cannot
-            // tell "one phase behind" from "one ahead": a group that ran ahead of its twin after a divergent branch re-armed a
-            // barrier whose phase was still open — a dead-lock at bench batch sizes, profiles/r02aa.)
-            constexpr int kPwK = SST % 2 == 0 ? 2 : 3;
-            static_assert(SST % kPwK == 0 && kPwK <= SST, "one lane group per stage, and a round must not wait for its own stages");
-            if (lane < 4 * kPwK) {
-                const int ks = lane >> 2, q = lane & 3;
-                long long tile = tile_first;
-                int kb = ks;
-                uint32_t g = static_cast<uint32_t>(ks);
-                long long dec_tile = -1;
-                BoxCoord bx{};
-                uint32_t nvalid = 0;
-                for (;;) {
-                    while (kb >= kblocks && tile < total_tiles) { kb -= kblocks; tile += tile_step; }
-                    if (tile >= total_tiles) break;
-                    if (tile != dec_tile) {
-                        const uint32_t ptile = fast_div(static_cast<uint32_t>(tile), args.m_num_n, args.num_n);
-                        bx = decode_box(ptile * 4 + q, args);
-                        nvalid = 0;
-#pragma unroll
-                        for (int qq = 0; qq < 4; ++qq) nvalid += (ptile * 4 + qq) < static_cast<uint32_t>(args.total_boxes) ? 1u : 0u;
-                        dec_tile = tile;
-                    }
-                    const uint32_t st = g % SST;
-                    ptx::mbar_wait(&slab_empty[st], ((g / SST) & 1u) ^ 1u, args.suspend_ns);
-                    if (q == 0) ptx::mbar_arrive_expect_tx(&slab_full[st], nvalid * kPwBoxBytes);
-                    if (bx.valid)
-                        ptx::tma_load_3d(slab0 + st * kPwStageBytes + q * kPwBoxBytes, &tmIn, &slab_full[st], bx.ox0, kb * 32, bx.n);
-                    g += kPwK;
-                    kb += kPwK;
+                    ptx::tma_load_3d(st, &tmW, &full_bar[stage], kb * 32, n_blk * BN, 0);
+                    if (NPL == 2) ptx::tma_load_3d(st + kBTile, &tmWlo, &full_bar[stage], kb * 32, n_blk * BN, 0);
                 }
             }
         }
-        if (SLAB) {
-            const bool leader = ptx::elect_one();
-            const int cblocks = args.IC >> 5;
-            uint32_t j = 0;
-            for (long long tile = tile_first; tile < total_tiles; tile += tile_step) {
-                const uint32_t pitem = fast_div(static_cast<uint32_t>(tile), args.m_num_n, args.num_n);
-            const uint32_t ptile = pitem * CG + cta_rank;
-                const BoxCoord bx = decode_patch(ptile, args);
-                for (int cb = 0; cb < cblocks; ++cb, ++j) {
-                    const uint32_t st = j % SST;
-                    ptx::mbar_wait(&slab_empty[st], ((j / SST) & 1u) ^ 1u, args.suspend_ns);
-                    if (leader) {
-                        ptx::mbar_arrive_expect_tx(&slab_full[st], kSlabStageBytes);
-                        tma_load_4d(slab0 + st * kSlabStageBytes, &tmIn, &slab_full[st], bx.ox0 - kSlabShift,
-                                    bx.oy - args.pad_top, cb * 32, bx.n);
-                    }
-                    __syncwarp();
-                }
-            }
-        }
-    } else if (SLAB && warp >= 4) {
-        // ===================== A producers, 3x3 stride-1 slab variant =====================
-        // The generic producers below gather every k-block from global memory: each input element is loaded NINE times
-        // (once per tap) with an IMAD.WIDE + LDG + LOP + FADD each, issue-bound at N = 64 (VGG conv1_2).  Here the halo of
-        // the tile's 4 x 32 output patch for one 32-channel block arrives ONCE by TMA (see above: no load instructions,
-        // no register staging, padding by the OOB fill, SST items of prefetch), and a k-block = one tap is 32 LDS.32
-        // with immediate offsets + the 2-instruction TF32 split + 8 tcgen05.st per thread.  The item's 9 k-blocks go
-        // round-robin to the 3 groups, so group g always serves kernel COLUMN g (v = g, u = 0..2).
-        (void)plane;
-        const int pw = warp - 4;                               // 0..11
-        const int group = pw >> 2;
-        const int q = warp & 3;
-        const uint32_t lane_base = static_cast<uint32_t>(q * 32) << 16;
-        const int cblocks = args.IC >> 5;
-        // this lane's pixel inside the patch (2 x 16 sub-patch per warp) and its first slab element for tap row 0
-        const int lane_off = (patch_row(q, lane) * kSlabCols + patch_col(q, lane) + group - args.pad_left + kSlabShift) * 4;
-        uint32_t j = 0;  // running item index of this CTA; its k-blocks are 9j .. 9j+8
-        bool slot_free = false;  // ring slot of this warp's next k-block already seen released (probed one k-block ahead)
-        for (long long tile = tile_first; tile < total_tiles; tile += tile_step) {
-            for (int cb = 0; cb < cblocks; ++cb, ++j) {
-                const uint32_t st = j % SST;
-                ptx::mbar_wait(&slab_full[st], (j / SST) & 1u, args.suspend_ns);
-                const uint32_t tb = ptx::smem_u32(slab0 + st * kSlabStageBytes) + static_cast<uint32_t>(lane_off);
-#pragma unroll 1
-                for (int u = 0; u < 3; ++u) {
-                    const uint32_t g = j * 9u + static_cast<uint32_t>(3 * u + group);
-                    const int my_stage = static_cast<int>(g & (STAGES - 1));
-                    const uint32_t ta = tmem_a0 + lane_base + my_stage * kAStageCols;
-                    const uint32_t src = tb + static_cast<uint32_t>(u * (kSlabCols * 4));
-                    if (q == 0) IG_TRACE(0, g);
-                    if (!slot_free) wait_ring_slot_free<STAGES>(empty_bar, g, args.suspend_ns);
-                    if (q == 0) IG_TRACE(1, g);
-                    // this warp's next k-block: 3 further on inside the item, else the first one of the next item
-                    slot_free = probe_ring_slot_free<STAGES>(empty_bar, u < 2 ? g + 3u : (j + 1u) * 9u + static_cast<uint32_t>(group));
-                    ptx::tc_fence_after();
-                    if (BF) {
-#pragma unroll
-                        for (int part = 0; part < 2; ++part) {  // 16 channels -> 8 columns of bf16 pairs per plane
-                            uint32_t hi[8], lo[8];
-#pragma unroll
-                            for (int r = 0; r < 8; ++r) {
-                                const float x0 = lds_f32(src + (part * 16 + 2 * r) * kSlabChBytes);
-                                const float x1 = lds_f32(src + (part * 16 + 2 * r + 1) * kSlabChBytes);
-                                split_bf16x2(x0, x1, hi[r], lo[r]);
-                            }
-                            tmem_st_32x8(ta + part * 8, hi);
-                            tmem_st_32x8(ta + 16 + part * 8, lo);
-                        }
-                    }
-#pragma unroll
-                    for (int part = 0; part < (BF ? 0 : 4); ++part) {
-                        uint32_t hi[8], lo[8];
-#pragma unroll
-                        for (int r = 0; r < 8; ++r) {
-                            const float x = lds_f32(src + (part * 8 + r) * kSlabChBytes);
-                            hi[r] = PLANES == 2 ? (__float_as_uint(x) & 0xFFFFE000u) : __float_as_uint(x);
-                            lo[r] = __float_as_uint(x - __uint_as_float(hi[r]));
-                        }
-                        tmem_st_32x8(ta + part * 8, hi);
-                        if (PLANES == 2) tmem_st_32x8(ta + 32 + part * 8, lo);
-                    }
-                    if (q == 0) IG_TRACE(2, g);
-                    tmem_st_wait();
-                    if (q == 0) IG_TRACE(4, g);
-                    if (q == 3) IG_TRACE(3, g);
-                    ptx::tc_fence_before();
-                    __syncwarp();
-                    if (lane == 0) {
-                        if (CG == 2 && cta_rank != 0) ptx::mbar_arrive_remote(&full_bar[my_stage], 0u);
-                        else ptx::mbar_arrive(&full_bar[my_stage]);
-                    }
-                }
-                // (the __syncwarp above orders every lane's slab reads before the release)
-                if (lane == 0) ptx::mbar_arrive(&slab_empty[st]);
-            }
-        }
-    } else if (PW && warp >= 4) {
-        // ===================== A producers, pointwise slab variant =====================
-        // k-block g (running over all tiles of this CTA) belongs to group g % kGroups, ring slot g % STAGES and slab stage
-        // g % SST; this warp reads ITS quadrant's box: element (channel r, pixel lane) at r * 128 + lane * 4.
-        (void)plane;
-        const int group = (warp - 4) >> 2;
-        const int q = warp & 3;
-        const uint32_t lane_base = static_cast<uint32_t>(q * 32) << 16;
-        long long my_tiles = 0;
-        if (tile_first < total_tiles) my_tiles = (total_tiles - tile_first + tile_step - 1) / tile_step;
-        const uint32_t total_g = static_cast<uint32_t>(my_tiles) * static_cast<uint32_t>(kblocks);
-        bool slot_free = false;
-        for (uint32_t g = static_cast<uint32_t>(group); g < total_g; g += kGroups) {
-            const uint32_t st = g % SST;
-            const int my_stage = static_cast<int>(g & (STAGES - 1));
-            const uint32_t ta = tmem_a0 + lane_base + my_stage * kAStageCols;
-            const uint32_t src = ptx::smem_u32(slab0 + st * kPwStageBytes + q * kPwBoxBytes) + static_cast<uint32_t>(lane * 4);
-            ptx::mbar_wait(&slab_full[st], (g / SST) & 1u, args.suspend_ns);
-            if (!slot_free) wait_ring_slot_free<STAGES>(empty_bar, g, args.suspend_ns);
-            slot_free = probe_ring_slot_free<STAGES>(empty_bar, g + kGroups);
-            ptx::tc_fence_after();
-            if (BF) {
-#pragma unroll
-                for (int part = 0; part < 2; ++part) {
-                    uint32_t hi[8], lo[8];
-#pragma unroll
-                    for (int r = 0; r < 8; ++r) {
-                        const float x0 = lds_f32(src + (part * 16 + 2 * r) * 128);
-                        const float x1 = lds_f32(src + (part * 16 + 2 * r + 1) * 128);
-                        split_bf16x2(x0, x1, hi[r], lo[r]);
-                    }
-                    tmem_st_32x8(ta + part * 8, hi);
-                    tmem_st_32x8(ta + 16 + part * 8, lo);
-                }
-            }
-#pragma unroll
-            for (int part = 0; part < (BF ? 0 : 4); ++part) {
-                uint32_t hi[8], lo[8];
-#pragma unroll
-                for (int r = 0; r < 8; ++r) {
-                    const float x = lds_f32(src + (part * 8 + r) * 128);
-                    hi[r] = PLANES == 2 ? (__float_as_uint(x) & 0xFFFFE000u) : __float_as_uint(x);
-                    lo[r] = __float_as_uint(x - __uint_as_float(hi[r]));
-                }
-                tmem_st_32x8(ta + part * 8, hi);
-                if (PLANES == 2) tmem_st_32x8(ta + 32 + part * 8, lo);
-            }
-            tmem_st_wait();
-            ptx::tc_fence_before();
-            __syncwarp();  // every lane's slab reads are done (their values went through the stores above)
-            if (lane == 0) {
-                ptx::mbar_arrive(&full_bar[my_stage]);
-                ptx::mbar_arrive(&slab_empty[st]);
-            }
-        }
-    } else if (!SLAB && warp >= 4) {
-        // ===================== A producers: gather + 3xTF32 split -> tensor memory =====================
-        // k-block number g (running over all tiles of this CTA) belongs to group g % kGroups and ring slot
-        // g % STAGES; a group visits only its own k-blocks.  The group is latency-bound, not issue-bound (a gather
-        // is ~800 cycles from L2), so the loop is software-pipelined: the 32 loads of the group's NEXT k-block — which
-        // may belong to the next tile — are issued before it waits for the tensor-memory stores of the current one.
-        static_assert((STAGES & (STAGES - 1)) == 0, "ring slot = g & (STAGES-1)");
-        const int group = (warp - 4) >> 2;
-        const int q = warp & 3;  // TMEM lane quadrant this warp may write == box index inside the tile
-        const uint32_t lane_base = static_cast<uint32_t>(q * 32) << 16;
-        const uint32_t plane_bytes = static_cast<uint32_t>(plane) * 4u;  // host guarantees H*W < 2^30
-        const int kb_mod = kblocks % kGroups;
-
-        // cursor over this group's k-blocks
-        long long tile = tile_first;
-        uint32_t g0 = 0;   // running index of the current tile's k-block 0
-        int g0_mod = 0;    // g0 % kGroups
-        int kb = 0;
-        int tap = 0, tu = 0, tv = 0, cb = 0;  // fast path: k-block kb = cb * taps + tap, tap = tu*KW + tv
-        const float* base = args.in;
-        unsigned long long tapmask = 0;  // bit (u*KW+v) set <=> that tap of this lane's pixel lies inside the image
-        bool have = false;
-
-        // position the cursor on the first owned k-block of tile `tile` or a later tile
-        auto enter_tile = [&]() {
-            have = false;
-            while (tile < total_tiles) {
-                kb = group - g0_mod;
-                if (kb < 0) kb += kGroups;
-                if (kb < kblocks) { have = true; break; }
-                tile += tile_step;
-                g0 += static_cast<uint32_t>(kblocks);
-                g0_mod += kb_mod;
-                if (g0_mod >= kGroups) g0_mod -= kGroups;
-            }
-            if (!have) return;
-            const uint32_t pitem = fast_div(static_cast<uint32_t>(tile), args.m_num_n, args.num_n);
-            const uint32_t ptile = pitem * CG + cta_rank;
-            const BoxCoord bx = decode_box(ptile * 4 + q, args);
-            const int ox = bx.ox0 + lane;
-            const bool pix_ok = bx.valid && ox < args.OW;
-            int py = bx.oy, px = ox;
-            if (args.flat_ow > 0) {  // flattened boxes: this lane's pixel index -> (row, column) of the real output image
-                py = static_cast<int>(fast_div(static_cast<uint32_t>(ox), args.m_flat_ow, args.flat_ow));
-                px = ox - py * args.flat_ow;
-            }
-            const int iy0 = py * args.stride_h - args.pad_top;
-            const int ix0 = px * args.stride_w - args.pad_left;
-            tapmask = 0;
-            if (pix_ok) {  // row mask x column mask instead of KH*KW tests
-                unsigned long long cols = 0;
-                for (int v = 0; v < args.KW; ++v)
-                    if (static_cast<unsigned>(ix0 + v * args.dil_w) < static_cast<unsigned>(args.W)) cols |= 1ull << v;
-                for (int u = 0; u < args.KH; ++u)
-                    if (static_cast<unsigned>(iy0 + u * args.dil_h) < static_cast<unsigned>(args.H)) tapmask |= cols << (u * args.KW);
-            }
-            base = args.in + (static_cast<long long>(bx.valid ? bx.n : 0) * args.in_img_c) * plane +
-                   static_cast<long long>(iy0) * args.W + ix0;
-            asm volatile("" : "+l"(base));  // opaque: see gather()
-            cb = 0; tap = kb;  // kb < kGroups here; gather() normalises
-        };
-        auto advance = [&]() {
-            kb += kGroups;
-            tap += kGroups;
-            if (kb >= kblocks) {
-                tile += tile_step;
-                g0 += static_cast<uint32_t>(kblocks);
-                g0_mod += kb_mod;
-                if (g0_mod >= kGroups) g0_mod -= kGroups;
-                enter_tile();
-            }
-        };
-        // issue the 32 loads of the cursor's k-block
-        const uint32_t ktab_s = ptx::smem_u32(ktab);
-        auto gather = [&](float (&x)[32]) {
-            if (!args.use_table) {
-                // IC % 32 == 0: the whole k-block is one tap -> one predicate; the 32 channel addresses are
-                // kp + r*plane_bytes, one IMAD.WIDE each off an opaque pointer (otherwise nvcc re-derives every
-                // address from args.in with ~8 integer instructions per load)
-                while (tap >= args.taps) { tap -= args.taps; ++cb; }
-                tu = static_cast<int>((static_cast<unsigned>(tap) * args.tap_inv) >> 16);
-                tv = tap - tu * args.KW;
-                const char* kp = reinterpret_cast<const char*>(base) +
-                                 (static_cast<long long>(cb * 32) * plane + tu * args.dil_h * args.W + tv * args.dil_w) * 4;
-                asm volatile("" : "+l"(kp));
-                const bool kb_ok = ((tapmask >> tap) & 1ull) != 0;
-                if (__all_sync(0xffffffffu, kb_ok)) {  // interior: no predication, no zero fill
-#pragma unroll
-                    for (int r = 0; r < 32; ++r)
-                        x[r] = __ldg(reinterpret_cast<const float*>(
-                            kp + static_cast<unsigned long long>(plane_bytes) * static_cast<uint32_t>(r)));
-                } else {
-#pragma unroll
-                    for (int r = 0; r < 32; ++r)
-                        x[r] = kb_ok ? __ldg(reinterpret_cast<const float*>(
-                                           kp + static_cast<unsigned long long>(plane_bytes) * static_cast<uint32_t>(r)))
-                                     : 0.f;
-                }
-            } else if (args.use_table == 2) {
-                // single k-block (K <= 32): offsets and taps come from the kernel parameters (constant bank, compile-time
-                // index) — the shared-memory table put an LDS + dependent LDG chain on every element (55 % of the
-                // producers' stall cycles on VGG conv1_1, ncu r02f)
-#pragma unroll
-                for (int r = 0; r < 32; ++r) {
-                    const int2 e = args.ktab1[r];
-                    x[r] = ((tapmask >> e.y) & 1ull) ? __ldg(base + e.x) : 0.f;
-                }
-            } else {
-#pragma unroll
-                for (int r = 0; r < 32; ++r) {
-                    int2 e;  // explicit ld.shared (the table pointer is generic to nvcc)
-                    asm volatile("ld.shared.v2.s32 {%0, %1}, [%2];" : "=r"(e.x), "=r"(e.y) : "r"(ktab_s + static_cast<uint32_t>((kb * 32 + r) * 8)));
-                    x[r] = ((tapmask >> e.y) & 1ull) ? __ldg(base + e.x) : 0.f;
-                }
-            }
-        };
-
-        float x[32];
-        enter_tile();
-        if (have) gather(x);
-        while (have) {
-            const uint32_t g = g0 + static_cast<uint32_t>(kb);
-            const int my_stage = static_cast<int>(g & (STAGES - 1));
-            const uint32_t ta = tmem_a0 + lane_base + my_stage * kAStageCols;
-            if (q == 0) IG_TRACE(0, g);
-            wait_ring_slot_free<STAGES>(empty_bar, g, args.suspend_ns);
-            if (q == 0) IG_TRACE(1, g);
-            ptx::tc_fence_after();
-            if (BF) {
-#pragma unroll
-                for (int part = 0; part < 2; ++part) {
-                    uint32_t hi[8], lo[8];
-#pragma unroll
-                    for (int r = 0; r < 8; ++r) split_bf16x2(x[part * 16 + 2 * r], x[part * 16 + 2 * r + 1], hi[r], lo[r]);
-                    tmem_st_32x8(ta + part * 8, hi);
-                    tmem_st_32x8(ta + 16 + part * 8, lo);
-                }
-            }
-#pragma unroll
-            for (int part = 0; part < (BF ? 0 : 4); ++part) {  // 8 k-values at a time keeps the live set inside 96 registers
-                uint32_t hi[8];
-                if (PLANES == 2) {
-                    uint32_t lo[8];
-#pragma unroll
-                    for (int r = 0; r < 8; ++r) {
-                        // hi = x with the 13 sub-TF32 mantissa bits cleared (what the tensor core would read
-                        // anyway), lo = x - hi exactly: 2 instructions per element instead of 5 for round-to-nearest;
-                        // the residual after the hardware truncates lo is <= 2^-21 |x| either way
-                        hi[r] = __float_as_uint(x[part * 8 + r]) & 0xFFFFE000u;
-                        lo[r] = __float_as_uint(x[part * 8 + r] - __uint_as_float(hi[r]));
-                    }
-                    tmem_st_32x8(ta + part * 8, hi);
-                    tmem_st_32x8(ta + 32 + part * 8, lo);
-                } else {
-#pragma unroll
-                    for (int r = 0; r < 8; ++r) hi[r] = __float_as_uint(x[part * 8 + r]);
-                    tmem_st_32x8(ta + part * 8, hi);
-                }
-            }
-            if (q == 0) IG_TRACE(2, g);
-            advance();
-            if (have) gather(x);  // in flight across the store drain, the arrive and the next slot wait
-            if (q == 0) IG_TRACE(3, g);
-            tmem_st_wait();
-            if (q == 0) IG_TRACE(4, g);
-            ptx::tc_fence_before();
-            __syncwarp();
-            if (lane == 0) {
-                if (CG == 2 && cta_rank != 0) ptx::mbar_arrive_remote(&full_bar[my_stage], 0u);
-                else ptx::mbar_arrive(&full_bar[my_stage]);
-            }
-        }
-    } else {
-        // ===================== epilogue (warps 0..3) =====================
-        const int q = warp & 3;
-        const float floor_v = args.relu ? 0.f : -INFINITY;
-        // geometry of the blob that is stored: the convolution output, or (SLAB, args.pool) its 2x2 / stride-2 max pooling
-        const bool pool = SLAB && args.pool != 0;
-        const int SH = pool ? (args.OH + 1) >> 1 : args.OH, SW = pool ? (args.OW + 1) >> 1 : args.OW;
-        const uint32_t oplane_bytes = static_cast<uint32_t>(SH * SW) * 4u;  // host: OH*OW < 2^30
-        uint32_t it = 0;
-        uint32_t ebuf = 0;  // staging tile toggle of the TMA-store path
-        const bool tma_out = args.tma_out != 0 && !pool;
-        for (long long tile = tile_first; tile < total_tiles; tile += tile_step, ++it) {
-            const uint32_t pitem = fast_div(static_cast<uint32_t>(tile), args.m_num_n, args.num_n);
-            const uint32_t ptile = pitem * CG + cta_rank;
-            const int n_blk = static_cast<int>(static_cast<uint32_t>(tile) - pitem * static_cast<uint32_t>(args.num_n));
-            const uint32_t as = it & static_cast<uint32_t>(args.acc_slots - 1);
-            const uint32_t aphase = (it / static_cast<uint32_t>(args.acc_slots)) & 1u;
-            // this warp's 32 TMEM lanes: box q (32 pixels of one row), or in SLAB mode a 2 x 16 sub-patch of the tile
-            const BoxCoord bx = SLAB ? decode_patch(ptile, args) : decode_box(ptile * 4 + q, args);
-            const int oy = SLAB ? bx.oy + patch_row(q, lane) : bx.oy;
-            const int ox = SLAB ? bx.ox0 + patch_col(q, lane) : bx.ox0 + lane;
-            const bool ok = bx.valid && ox < args.OW && oy < args.OH;
-            const int sy = pool ? oy >> 1 : oy, sx = pool ? ox >> 1 : ox;  // where this lane stores
-            const uint32_t taddr0 = tmem_base + (static_cast<uint32_t>(q * 32) << 16) + as * static_cast<uint32_t>(args.acc_stride);
-            const bool dual = args.issuers == 2;  // second issuer's accumulator sits BN columns further
-            const size_t oplane = static_cast<size_t>(SH) * SW;
-            if (args.residual != nullptr && bx.valid) {
-                // The fused Eltwise addend comes from HBM; a load issued after the accumulator is ready would put its
-                // ~1k-cycle latency on every 32-column chunk (measured: ResNet-50 8.3 -> 12.0 ms per step).  Each lane
-                // prefetches whole 128-byte channel rows of this warp's box while the MMAs of the tile are still running.
-                const int prow = SLAB ? min(bx.oy + 2 * (q >> 1), args.OH - 1) : bx.oy, pcol = SLAB ? bx.ox0 + 16 * (q & 1) : bx.ox0;
-                const char* rbase = reinterpret_cast<const char*>(args.residual + (static_cast<size_t>(bx.n) * args.out_img_c) * oplane +
-                                                                 static_cast<size_t>(prow) * args.OW + pcol);
-                for (int c = lane; c < BN; c += 32) {
-                    const int oc = n_blk * BN + c;
-                    if (oc < args.OC) {
-                        asm volatile("prefetch.global.L1 [%0];" ::"l"(rbase + static_cast<unsigned long long>(oplane_bytes) * static_cast<uint32_t>(oc)));
-                        if (SLAB && prow + 1 < args.OH)  // the sub-patch's second row
-                            asm volatile("prefetch.global.L1 [%0];" ::"l"(rbase + static_cast<unsigned long long>(oplane_bytes) * static_cast<uint32_t>(oc) + static_cast<unsigned long long>(args.OW) * 4ull));
-                    }
-                }
-            }
-            ptx::mbar_wait_relaxed<200>(&tmem_full_bar[as], aphase);
-            if (q == 0) IG_TRACE(9, it);
-            ptx::tc_fence_after();
-#pragma unroll 1
-            for (int c0 = 0; c0 < BN; c0 += 32) {
-                const int oc0 = n_blk * BN + c0;
-                if (oc0 >= args.OC) break;
-                uint32_t r[32];
-                ptx::tmem_ld_32x32(taddr0 + c0, r);
-                char* dst = reinterpret_cast<char*>(args.out + (static_cast<size_t>(ok ? bx.n : 0) * args.out_img_c + oc0) * oplane +
-                                                    static_cast<size_t>(sy) * SW + sx);
-                asm volatile("" : "+l"(dst));  // one IMAD.WIDE per store off an opaque base
-                // fused Eltwise SUM: the other addend sits at the same NCHW position
-                const long long res_off = args.residual ? reinterpret_cast<const char*>(args.residual) - reinterpret_cast<const char*>(args.out) : 0;
-                const uint32_t b4 = ptx::smem_u32(bias_s + oc0);  // bias_s is padded with zeros up to oc_pad
-                // all addend loads first (32 in flight), then the accumulator wait: a load placed next to its store
-                // is serialised behind the previous store by the aliasing rules (measured 2.4x slower epilogue)
-                // plain = one accumulator, no fused addend: the common case of the short-K layers, whose epilogue is the
-                // critical role — it skips the 32 zero-fills and 32 additions of `res` (warp-uniform branch)
-                const bool plain = !dual && args.residual == nullptr;
-                float res[32];
-#pragma unroll
-                for (int j = 0; j < 32; ++j) res[j] = 0.f;
-                if (args.residual != nullptr && ok) {
-                    const char* rsrc = reinterpret_cast<const char*>(dst) + res_off;
-                    if (oc0 + 32 <= args.OC) {
-#pragma unroll
-                        for (int j = 0; j < 32; ++j)
-                            res[j] = __ldg(reinterpret_cast<const float*>(rsrc + static_cast<unsigned long long>(oplane_bytes) * static_cast<uint32_t>(j)));
-                    } else {
-#pragma unroll
-                        for (int j = 0; j < 32; ++j)
-                            if (oc0 + j < args.OC)
-                                res[j] = __ldg(reinterpret_cast<const float*>(rsrc + static_cast<unsigned long long>(oplane_bytes) * static_cast<uint32_t>(j)));
-                    }
-                }
-                ptx::tmem_ld_wait();
-                if (dual) {
-                    // even-k-block accumulator, then the odd-k-block one, folded in this fixed order (one register set:
-                    // both accumulators live at once would spill next to the residual)
-#pragma unroll
-                    for (int j = 0; j < 32; ++j) res[j] += __uint_as_float(r[j]);
-                    ptx::tmem_ld_32x32(taddr0 + BN + c0, r);
-                    ptx::tmem_ld_wait();
-                }
-                if (pool) {
-                    // 2x2 / stride-2 max pooling of the sub-patch (pooling_layer.h:38-91, pad 0): the window of the pixel at
-                    // an even (row, column) is lanes {l, l^1, l^16, l^17}; pixels outside the image hold -inf.  max commutes
-                    // with the per-channel bias and with ReLU, so both are applied to the pooled value.
-                    // The bias comes in ahead of the stores, 16 channels at a time: read through a generic pointer next to its
-                    // store (round 2 until r02r) every channel paid a full generic-load latency behind the previous store —
-                    // ~10k cycles per tile, the whole pooled layer was paced by this loop (ncu source page r02r).
-                    // Through shared memory instead of shuffles: the chunk is laid out [channel][pixel] (lane = pixel, 16-byte
-                    // pieces XOR-swizzled by the channel: conflict-free both ways), then lane c owns CHANNEL c: eight LDS.128
-                    // bring its 2 x 16 pixels, the four window members of a pooled pixel sit in its own registers, and the 8
-                    // pooled values leave as two 16-byte stores.  ~90 instructions per lane and chunk instead of ~230 (two
-                    // shuffles + a 4-byte store of 8 active lanes per channel): the pooled layers were epilogue-bound
-                    // (igemm trace r02x: 7.5k cycles per 128 x 64 tile against 3.5k cycles of MMAs).
-                    uint8_t* stg = stage_out + (q * kOutBufs) * 4096;
-                    const uint32_t sbase = ptx::smem_u32(stg);
-                    __syncwarp();  // the previous chunk's reads of this tile are done
-#pragma unroll
-                    for (int j = 0; j < 32; ++j) {
-                        const float v = ok ? __uint_as_float(r[j]) + res[j] : -INFINITY;
-                        sts_f32(sbase + static_cast<uint32_t>(j * 128 + ((((lane >> 2) ^ (j & 7)) << 4) | ((lane & 3) << 2))), v);
-                    }
-                    __syncwarp();
-                    float v[32];  // channel `lane`: v[0..15] = row 0, v[16..31] = row 1 of the 2 x 16 sub-patch
-#pragma unroll
-                    for (int k = 0; k < 8; ++k) {
-                        const float4 t = lds_f32x4(sbase + static_cast<uint32_t>(lane * 128 + ((k ^ (lane & 7)) << 4)));
-                        v[4 * k] = t.x; v[4 * k + 1] = t.y; v[4 * k + 2] = t.z; v[4 * k + 3] = t.w;
-                    }
-                    const int oc = oc0 + lane;
-                    const float bj = lds_f32(b4 + 4 * lane);
-                    float pv[8];
-#pragma unroll
-                    for (int pp = 0; pp < 8; ++pp)
-                        pv[pp] = fmaxf(fmaxf(fmaxf(v[2 * pp], v[2 * pp + 1]), fmaxf(v[16 + 2 * pp], v[17 + 2 * pp])) + bj, floor_v);
-                    // where the sub-patch's pooled row starts in the stored blob (the same for every lane of the warp)
-                    const int py = (bx.oy + 2 * (q >> 1)) >> 1, px0 = (bx.ox0 + 16 * (q & 1)) >> 1;
-                    if (bx.valid && oc < args.OC && py < SH && px0 < SW) {
-                        float* pd = args.out + (static_cast<size_t>(bx.n) * args.out_img_c + oc) * oplane + static_cast<size_t>(py) * SW + px0;
-                        if (px0 + 8 <= SW && (reinterpret_cast<uintptr_t>(pd) & 15) == 0) {
-                            *reinterpret_cast<float4*>(pd) = make_float4(pv[0], pv[1], pv[2], pv[3]);
-                            *reinterpret_cast<float4*>(pd + 4) = make_float4(pv[4], pv[5], pv[6], pv[7]);
-                        } else {
-#pragma unroll
-                            for (int pp = 0; pp < 8; ++pp)
-                                if (px0 + pp < SW) pd[pp] = pv[pp];
-                        }
-                    }
-                } else if (tma_out) {
-                    // Per-thread STG moved ~15 B/clk per SM here (igemm trace of VGG conv1_1: 2,250 cycles of epilogue per
-                    // 128 x 64 tile, the whole kernel paced by it).  Instead the 32-channel x 32-pixel chunk is laid out
-                    // [channel][pixel] in shared memory (lane = pixel: conflict-free STS) and leaves as ONE TMA store —
-                    // whole 128-byte rows per channel plane, image borders and the channel tail clipped by the tensor map.
-                    uint8_t* stg = stage_out + (q * kOutBufs + (kOutBufs == 2 ? (ebuf & 1u) : 0u)) * 4096;
-                    if (lane == 0) ptx::tma_store_wait_read<kOutBufs - 1>();  // the store that last read this tile is done with it
-                    __syncwarp();
-                    const uint32_t sp = ptx::smem_u32(stg) + static_cast<uint32_t>(lane * 4);
-                    if (plain) {
-#pragma unroll
-                        for (int j4 = 0; j4 < 8; ++j4) {
-                            const float4 bv = lds_f32x4(b4 + 16 * j4);
-                            const float bb[4] = {bv.x, bv.y, bv.z, bv.w};
-#pragma unroll
-                            for (int e = 0; e < 4; ++e) {
-                                const int j = j4 * 4 + e;
-                                sts_f32(sp + j * 128, fmaxf(__uint_as_float(r[j]) + bb[e], floor_v));
-                            }
-                        }
-                    } else {
-#pragma unroll
-                        for (int j4 = 0; j4 < 8; ++j4) {
-                            const float4 bv = lds_f32x4(b4 + 16 * j4);
-                            const float bb[4] = {bv.x, bv.y, bv.z, bv.w};
-#pragma unroll
-                            for (int e = 0; e < 4; ++e) {
-                                const int j = j4 * 4 + e;
-                                sts_f32(sp + j * 128, fmaxf(__uint_as_float(r[j]) + res[j] + bb[e], floor_v));
-                            }
-                        }
-                    }
-                    ptx::fence_proxy_async_smem();
-                    __syncwarp();
-                    if (lane == 0 && bx.valid) {
-                        if (SLAB) tma_store_4d(&tmOut, stg, bx.ox0 + 16 * (q & 1), bx.oy + 2 * (q >> 1), oc0, bx.n);
-                        else tma_store_4d(&tmOut, stg, bx.ox0, bx.oy, oc0, bx.n);
-                        ptx::tma_store_commit();
-                    }
-                    ++ebuf;
-                } else if (ok) {
-                    if (oc0 + 32 <= args.OC) {
-#pragma unroll
-                        for (int j4 = 0; j4 < 8; ++j4) {
-                            const float4 bv = lds_f32x4(b4 + 16 * j4);
-                            const float bb[4] = {bv.x, bv.y, bv.z, bv.w};
-#pragma unroll
-                            for (int e = 0; e < 4; ++e) {
-                                const int j = j4 * 4 + e;
-                                *reinterpret_cast<float*>(dst + static_cast<unsigned long long>(oplane_bytes) * static_cast<uint32_t>(j)) =
-                                    fmaxf(__uint_as_float(r[j]) + res[j] + bb[e], floor_v);
-                            }
-                        }
-                    } else {
-#pragma unroll
-                        for (int j = 0; j < 32; ++j)
-                            if (oc0 + j < args.OC)
-                                *reinterpret_cast<float*>(dst + static_cast<unsigned long long>(oplane_bytes) * static_cast<uint32_t>(j)) =
-                                    fmaxf(__uint_as_float(r[j]) + res[j] + lds_f32(b4 + 4 * j), floor_v);
-                    }
-                }
-            }
-            ptx::tc_fence_before();
-            __syncwarp();
-            if (q == 0) IG_TRACE(10, it);
-            if (lane == 0) {
-                if (CG == 2 && cta_rank != 0) ptx::mbar_arrive_remote(&tmem_empty_bar[as], 0u);
-                else ptx::mbar_arrive(&tmem_empty_bar[as]);
-            }
-        }
-        if (tma_out && lane == 0) ptx::tma_store_wait_all<0>();  // global writes complete before the CTA retires
+        return;
     }
 
-    ptx::tc_fence_before();
-    __syncthreads();
-    if (CG == 2) ptx::cluster_sync_all();  // the pair's MMAs, remote arrivals and tensor-memory reads are all done
-    if (warp == kWarpMma) {
-        ptx::tc_fence_after();
-        if (CG == 1) ptx::tmem_dealloc(tmem_base, kTmemCols);
-        else ptx::tmem_dealloc_cg2(tmem_base, kTmemCols);
+    // ===================== consumers =====================
+    const int gq = lane >> 2, c = lane & 3;
+    // the two pixels (fragment rows gq, gq + 8 of this warp's 16) this thread gathers and stores
+    int img[2], oy[2], ox[2];
+    bool valid[2];
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+        if (args.pool) {
+            const int per_img = args.tiles_x * args.tiles_y;
+            const int n = static_cast<int>(ptile / per_img);
+            const int rem = static_cast<int>(ptile - static_cast<long long>(n) * per_img);
+            const int ty = rem / args.tiles_x, tx = rem - ty * args.tiles_x;
+            img[h] = n;
+            oy[h] = 2 * ty + h;
+            ox[h] = 64 * tx + 8 * warp + gq;
+            valid[h] = oy[h] < args.OH && ox[h] < args.OW;
+        } else {
+            const long long m = ptile * 128 + warp * 16 + 8 * h + gq;
+            valid[h] = m < args.total_pix;
+            const long long mm = valid[h] ? m : 0;
+            const int pix_per_img = args.OH * args.OW;
+            img[h] = static_cast<int>(mm / pix_per_img);
+            const int pix = static_cast<int>(mm - static_cast<long long>(img[h]) * pix_per_img);
+            oy[h] = pix / args.OW;
+            ox[h] = pix - oy[h] * args.OW;
+        }
+    }
+    int iy0[2], ix0[2];
+    long long ibase[2];  // element offset of tap (0, 0), channel 0 of the pixel's receptive field
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+        iy0[h] = oy[h] * args.stride_h - args.pad_top;
+        ix0[h] = ox[h] * args.stride_w - args.pad_left;
+        ibase[h] = static_cast<long long>(img[h]) * args.in_img_c * plane + static_cast<long long>(iy0[h]) * args.W + ix0[h];
+    }
+    const float* __restrict__ in = args.in;
+
+    // raw A values of one k-block: [row h][fragment element j]
+    auto gather = [&](int kb, float (&raw)[2][8]) {
+        if (!args.use_table) {
+            const int cb = kb / args.taps, tap = kb - cb * args.taps;
+            const int dy = (tap / args.KW) * args.dil_h, dx = (tap % args.KW) * args.dil_w;
+            const long long koff = static_cast<long long>(cb) * 32 * plane + dy * args.W + dx;
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+                const bool ok = valid[h] && static_cast<unsigned>(iy0[h] + dy) < static_cast<unsigned>(args.H) &&
+                                static_cast<unsigned>(ix0[h] + dx) < static_cast<unsigned>(args.W);
+                const float* p = in + (ok ? ibase[h] + koff : 0);
+#pragma unroll
+                for (int j = 0; j < 8; ++j) raw[h][j] = ok ? __ldg(p + static_cast<size_t>(frag_k<BF>(j, c)) * plane) : 0.f;
+            }
+        } else {
+#pragma unroll
+            for (int j = 0; j < 8; ++j) {
+                const int k = kb * 32 + frag_k<BF>(j, c);
+                int2 e;
+                asm volatile("ld.shared.v2.s32 {%0, %1}, [%2];" : "=r"(e.x), "=r"(e.y) : "r"(ptx::smem_u32(ktab + k)));
+                const int dy = e.y >> 16, dx = e.y & 0xFFFF;
+#pragma unroll
+                for (int h = 0; h < 2; ++h) {
+                    const bool ok = valid[h] && k < args.K && static_cast<unsigned>(iy0[h] + dy) < static_cast<unsigned>(args.H) &&
+                                    static_cast<unsigned>(ix0[h] + dx) < static_cast<unsigned>(args.W);
+                    raw[h][j] = ok ? __ldg(in + ibase[h] + e.x) : 0.f;
+                }
+            }
+        }
+    };
+
+    float acc[BN / 2];
+#pragma unroll
+    for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+    float raw[2][8];
+    gather(0, raw);
+    for (int kb = 0; kb < kblocks; ++kb) {
+        const int stage = kb % kStagesIg;
+        // split this k-block's operand into the fragments, then start the next k-block's loads
+        uint32_t f1[4][4], f2[4][4];  // [k-step][a0..a3]: hi / p1 and lo / p2
+        if (BF) {
+#pragma unroll
+            for (int kk = 0; kk < 2; ++kk)
+#pragma unroll
+                for (int q = 0; q < 4; ++q) {  // a0 (row gq, pair 0), a1 (row gq + 8, pair 0), a2 (gq, pair 1), a3 (gq + 8, pair 1)
+                    const int h = q & 1, j = 4 * kk + 2 * (q >> 1);
+                    split_bf16x2(raw[h][j], raw[h][j + 1], f1[kk][q], f2[kk][q]);
+                }
+        } else {
+#pragma unroll
+            for (int kk = 0; kk < 4; ++kk)
+#pragma unroll
+                for (int q = 0; q < 4; ++q) {
+                    const float x = raw[q & 1][2 * kk + (q >> 1)];
+                    if (PLANES == 2) split_tf32_trunc(x, f1[kk][q], f2[kk][q]);
+                    else f1[kk][q] = __float_as_uint(x);
+                }
+        }
+        if (kb + 1 < kblocks) gather(kb + 1, raw);
+        ptx::mbar_wait(&full_bar[stage], (kb / kStagesIg) & 1);
+        const uint32_t b_base = ptx::smem_u32(smem + stage * kStage);
+        ptx::wgmma_fence();
+        if (BF) {
+            // un-swizzled core matrices: LBO = 128 B between k chunks, SBO = 512 B between 8-row groups; a k-step = 2 chunks
+            const uint64_t dQ1 = make_smem_desc_none(b_base, 128, 512);
+            const uint64_t dQ2 = make_smem_desc_none(b_base + kBTile, 128, 512);
+#pragma unroll
+            for (int kk = 0; kk < 2; ++kk) {
+                Wgmma<BN, 0>::mma(acc, f2[kk], dQ1 + 16 * kk, 1u);  // p2 * q1
+                Wgmma<BN, 0>::mma(acc, f1[kk], dQ2 + 16 * kk, 1u);  // p1 * q2
+                Wgmma<BN, 0>::mma(acc, f1[kk], dQ1 + 16 * kk, 1u);  // p1 * q1
+            }
+        } else {
+            const uint64_t dB = make_smem_desc_sw128(b_base);
+            const uint64_t dBlo = make_smem_desc_sw128(b_base + kBTile);
+#pragma unroll
+            for (int kk = 0; kk < 4; ++kk) {
+                if (PLANES == 2) {
+                    Wgmma<BN, 1>::mma(acc, f2[kk], dB + 2 * kk, 1u);    // A_lo * B_hi
+                    Wgmma<BN, 1>::mma(acc, f1[kk], dBlo + 2 * kk, 1u);  // A_hi * B_lo
+                    Wgmma<BN, 1>::mma(acc, f1[kk], dB + 2 * kk, 1u);    // A_hi * B_hi
+                } else {
+                    Wgmma<BN, 1>::mma(acc, f1[kk], dB + 2 * kk, 1u);
+                }
+            }
+        }
+        ptx::wgmma_commit();
+        ptx::wgmma_wait<0>();
+        __syncwarp();
+        if (lane == 0) ptx::mbar_arrive(&empty_bar[stage]);
+    }
+
+    // ===================== epilogue =====================
+    const int oplane = args.OH * args.OW;
+    const int SH = (args.OH + 1) >> 1, SW = (args.OW + 1) >> 1;  // pooled geometry
+#pragma unroll
+    for (int j = 0; j < BN / 8; ++j) {
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+            const int oc = n_blk * BN + 8 * j + 2 * c + e;
+            const bool oc_ok = oc < args.OC;
+            const float bv = (args.bias != nullptr && oc_ok) ? __ldg(args.bias + oc) : 0.f;
+            float v[2];
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+                v[h] = acc[4 * j + 2 * h + e] + bv;
+                const size_t o = (static_cast<size_t>(img[h]) * args.out_img_c + oc) * oplane + static_cast<size_t>(oy[h]) * args.OW + ox[h];
+                if (args.residual != nullptr && valid[h] && oc_ok) v[h] += __ldg(args.residual + o);
+                if (args.relu) v[h] = fmaxf(v[h], 0.f);
+                if (!args.pool && valid[h] && oc_ok) args.out[o] = v[h];
+            }
+            if (args.pool) {
+                float m = fmaxf(valid[0] ? v[0] : -INFINITY, valid[1] ? v[1] : -INFINITY);
+                m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, 4));  // the window's other column: pixel gq ^ 1
+                if ((gq & 1) == 0 && valid[0] && oc_ok)
+                    args.out[(static_cast<size_t>(img[0]) * args.out_img_c + oc) * (static_cast<size_t>(SH) * SW) +
+                             static_cast<size_t>(oy[0] >> 1) * SW + (ox[0] >> 1)] = m;
+            }
+        }
     }
 }
 
@@ -1221,7 +350,7 @@ igemm_pack_weights_kernel(const float* __restrict__ w, float* __restrict__ hi, f
 // BF16x3: two bf16 planes q1 = RN(w), q2 = RN(w - q1), PRE-TILED for the kernel's filter ring, ordered
 //     [k-block kb (32 k-values, same k order as above)][N tile nb (BN rows)][plane][row / 8][16-byte k chunk (4)][row % 8][8 bf16]
 // i.e. per (k-block, N tile) both planes are ONE contiguous run of 8-row x 16-byte core matrices — the un-swizzled K-major
-// shared-memory layout of tcgen05 — so the kernel fetches a ring stage with one 1-D bulk copy.  Rows >= OC and k >= K are
+// shared-memory layout of wgmma — so the kernel fetches a ring stage with one 1-D bulk copy.  Rows >= OC and k >= K are
 // zeros; BN = the N tile the dispatcher picks for this OC, OCpad = OC rounded up to it.
 __global__ void __launch_bounds__(256)
 igemm_pack_weights_bf16_kernel(const float* __restrict__ w, __nv_bfloat16* __restrict__ q, int OC, int IC, int taps, int KB,
@@ -1254,55 +383,45 @@ igemm_pack_weights_bf16_kernel(const float* __restrict__ w, __nv_bfloat16* __res
     q[dst + static_cast<size_t>(BN) * 32] = __float2bfloat16_rn(v - __bfloat162float(a));
 }
 
-// N tile the dispatcher uses for a layer with OC output channels (dispatch_igemm) and the padded row count of the tiled planes
+
+// N tile conv_igemm_forward uses for a layer with OC output channels and the padded row count of the tiled planes
 static int igemm_bn_for(int OC) { return OC <= 32 ? 32 : OC <= 64 ? 64 : 128; }
 static int igemm_ocpad(int OC) { const int bn = igemm_bn_for(OC); return (OC + bn - 1) / bn * bn; }
 
-template <int BN, int PLANES, int SK, int CG>
+template <int BN, int PLANES>
 int launch_igemm(const IgemmProblem& p, cudaStream_t stream) {
-    constexpr bool SLAB = SK == 1;
-    constexpr bool PW = SK == 2;
-    EncodeTiledFn enc = encode_fn();
-    if (!enc) return FCUDA_ERR_CUDA;
-    CUtensorMap tmW, tmWlo;
-    const int taps = p.KH * p.KW;
-    const int K = taps * p.IC;
     constexpr bool BF = PLANES == 3;
     constexpr int NPL = BF ? 2 : PLANES;
-    constexpr int kElt = BF ? 2 : 4;
-    const int Kf = BF ? (K + 7) & ~7 : (K + 3) & ~3;
-    for (int pl = 0; pl < (BF ? 0 : NPL); ++pl) {
-        cuuint64_t dims[3] = {(cuuint64_t)Kf, (cuuint64_t)p.OC, 1};
-        cuuint64_t strides[2] = {(cuuint64_t)Kf * kElt, (cuuint64_t)Kf * p.OC * kElt};
-        cuuint32_t box[3] = {32, (cuuint32_t)(BN / CG), 1};  // CG = 2: each CTA of the pair fetches half of the N tile
-        cuuint32_t estr[3] = {1, 1, 1};
-        const float* base = pl == 0 ? p.w_hi : p.w_lo;
-        CUresult r = enc(pl == 0 ? &tmW : &tmWlo, BF ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3,
-                         const_cast<float*>(base), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                         BF ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_128B,
-                         CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-        if (r != CUDA_SUCCESS) {
-            fprintf(stderr, "fcuda: igemm weight tensor map failed (%d)\n", (int)r);
-            return FCUDA_ERR_CUDA;
+    const int taps = p.KH * p.KW;
+    const int K = taps * p.IC;
+    CUtensorMap tmW, tmWlo;
+    memset(&tmW, 0, sizeof(tmW));
+    tmWlo = tmW;
+    if (!BF) {  // the BF16x3 planes are pre-tiled and fetched by 1-D bulk copies: no tensor map
+        EncodeTiledFn enc = encode_fn();
+        if (!enc) return FCUDA_ERR_CUDA;
+        const int Kf = (K + 3) & ~3;
+        for (int pl = 0; pl < NPL; ++pl) {
+            cuuint64_t dims[3] = {(cuuint64_t)Kf, (cuuint64_t)p.OC, 1};
+            cuuint64_t strides[2] = {(cuuint64_t)Kf * 4, (cuuint64_t)Kf * p.OC * 4};
+            cuuint32_t box[3] = {32, (cuuint32_t)BN, 1};
+            cuuint32_t estr[3] = {1, 1, 1};
+            const float* base = pl == 0 ? p.w_hi : p.w_lo;
+            CUresult r = enc(pl == 0 ? &tmW : &tmWlo, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, const_cast<float*>(base), dims, strides,
+                             box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
+                             CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+            if (r != CUDA_SUCCESS) {
+                fprintf(stderr, "fcuda: igemm weight tensor map failed (%d)\n", (int)r);
+                return FCUDA_ERR_CUDA;
+            }
         }
     }
-    if (BF) {  // no tensor map: the planes are pre-tiled, fetched by 1-D bulk copies
-        memset(&tmW, 0, sizeof(tmW));
-        tmWlo = tmW;
-    }
-    if (NPL == 1) tmWlo = tmW;
     IgemmArgs a;
     a.wbf = reinterpret_cast<const unsigned char*>(p.w_hi);
     a.wbf_kb_bytes = 2u * static_cast<unsigned>(igemm_ocpad(p.OC)) * 64u;
     if (BF && (igemm_bn_for(p.OC) != BN || static_cast<unsigned long long>(ceil_div(K, 32)) * igemm_ocpad(p.OC) * 128ull >= (1ull << 31))) return -1;
     a.in = p.input; a.out = p.output; a.bias = p.bias; a.residual = p.residual;
-    // Small images on the generic path: a 32-pixel box along ONE output row is mostly padding when OW < 32 (7x7: 7 of 32
-    // lanes, 4.6x the tiles — ResNet-50's stage-5 3x3 / strided 1x1 layers ran 385 us each).  Box the flattened pixel index
-    // oy * OW + ox instead (the epilogue then sees a 1 x OH*OW image, like the pointwise remap of fcuda_api.cu).
-    const bool flat = !SLAB && !PW && p.OH > 1 && p.OW < 28 && p.pool == 0;
-    const int OHe = flat ? 1 : p.OH, OWe = flat ? p.OH * p.OW : p.OW;   // what the boxes / the epilogue see
-    a.flat_ow = flat ? p.OW : 0;
-    a.N = p.N; a.IC = p.IC; a.H = p.H; a.W = p.W; a.OC = p.OC; a.OH = OHe; a.OW = OWe;
+    a.N = p.N; a.IC = p.IC; a.H = p.H; a.W = p.W; a.OC = p.OC; a.OH = p.OH; a.OW = p.OW;
     a.KH = p.KH; a.KW = p.KW; a.pad_top = p.pad_top; a.pad_left = p.pad_left;
     a.stride_h = p.stride_h; a.stride_w = p.stride_w;
     a.dil_h = p.dil_h > 1 ? p.dil_h : 1; a.dil_w = p.dil_w > 1 ? p.dil_w : 1;
@@ -1311,132 +430,33 @@ int launch_igemm(const IgemmProblem& p, cudaStream_t stream) {
     a.K = K;
     a.kblocks = ceil_div(K, 32);
     a.use_table = (p.IC % 32 == 0) ? 0 : 1;
-    a.bpr = ceil_div(OWe, 32);
-    a.per_img = (SLAB ? ceil_div(p.OH, 4) : OHe) * a.bpr;  // SLAB: tiles (4 x 32 patches) per image, else boxes per image
-    a.total_boxes = static_cast<long long>(p.N) * a.per_img * (SLAB ? 4 : 1);
-    a.pool = SLAB ? p.pool : 0;
     a.taps = taps;
-    a.tap_inv = (65536u + static_cast<unsigned>(p.KW) - 1u) / static_cast<unsigned>(p.KW);
-    auto magic = [](int d) { return d > 1 ? ~0ull / static_cast<unsigned long long>(d) + 1ull : 0ull; };
-    a.m_flat_ow = magic(p.OW);
-    a.m_per_img = magic(a.per_img);
-    a.m_bpr = magic(a.bpr);
     a.num_n = ceil_div(p.OC, BN);
-    a.m_num_n = magic(a.num_n);
-    a.oc_pad = a.num_n * BN;
-    a.pixel_tiles = ((a.total_boxes + 3) / 4 + CG - 1) / CG;  // work items: pixel tiles, or pairs of them (CG = 2)
-    // 32-bit box / tile arithmetic and 32-bit plane strides inside the kernel
-    if (a.total_boxes + 4 >= (1ll << 31) || a.pixel_tiles * a.num_n >= (1ll << 31) ||
-        static_cast<long long>(p.H) * p.W >= (1ll << 30) || static_cast<long long>(p.OH) * p.OW >= (1ll << 30))
-        return -1;
+    a.total_pix = static_cast<long long>(p.N) * p.OH * p.OW;
     a.relu = p.relu;
-    a.suspend_ns = static_cast<unsigned>(tune_get(TUNE_MBAR_SUSPEND_NS));
-    a.tma_lanes = tune_get(TUNE_IGEMM_TMA_LANES);
-    if (a.tma_lanes != 1 && a.tma_lanes != 2) a.tma_lanes = 4;
-    // two issuers (one accumulator each) where one thread cannot keep the pipe fed: N <= 64 and at least four k-blocks
-    // per tile (short-K tiles are epilogue-bound and would only pay the second accumulator read); BN = 128 has 768 cycles of MMA work per k-block against ~350 of issue work, and only 256 accumulator
-    // columns.  FCUDA_IGEMM_ISSUERS=1 forces one issuer (diagnostic).
-    const int issuers_env = tune_get(TUNE_IGEMM_ISSUERS);
-    a.issuers = (BN <= 64 && a.kblocks >= 4) ? issuers_env : 1;
-    a.acc_stride = a.issuers == 2 ? 2 * BN : BN;
-    a.acc_slots = (BN <= 64 ? 256 : 2 * BN) / a.acc_stride;
-    if (a.acc_slots > 4) a.acc_slots = 4;
-    const long long total = a.pixel_tiles * a.num_n;
-    int grid = static_cast<int>(total < sm_count() ? total : sm_count());
-    constexpr int kStage = NPL * (BN / CG) * 32 * kElt;
-    if (a.use_table && a.kblocks == 1) {
-        a.use_table = 2;
-        for (int k = 0; k < 32; ++k) {
-            a.ktab1[k] = make_int2(0, 63);  // padding rows: tap 63 is never valid
-            if (k < K) {
-                const int tap = k / p.IC, ic = k - tap * p.IC;
-                const int u = tap / p.KW, v = tap - u * p.KW;
-                a.ktab1[k] = make_int2(ic * p.H * p.W + u * a.dil_h * p.W + v * a.dil_w, tap);
-            }
-        }
-    }
-    const int table_bytes = a.use_table == 1 ? a.kblocks * 32 * 8 : 0;
-    constexpr int kOutStage = 4 * ((SLAB && BN == 128 && CG == 1) ? 1 : 2) * 4096;
-    const int smem = igemm_stages(PLANES) * kStage + (SLAB ? slab_stages(BN) * kSlabStageBytes : PW ? pw_stages(BN, PLANES) * kPwStageBytes : 0) +
-                     kOutStage + table_bytes + a.oc_pad * 4 + 1024;
-    if (smem > 227 * 1024 - 2048) return -1;
-    auto kern = conv_igemm_kernel<BN, PLANES, SK, CG>;
+    a.pool = p.pool ? 1 : 0;
+    a.tiles_x = ceil_div(p.OW, 64);
+    a.tiles_y = ceil_div(p.OH, 2);
+    const long long pixel_tiles = a.pool ? static_cast<long long>(p.N) * a.tiles_x * a.tiles_y : (a.total_pix + 127) / 128;
+    const long long total = pixel_tiles * a.num_n;
+    // 32-bit plane strides and packed tap offsets (dy << 16 | dx) inside the kernel
+    if (total >= (1ll << 31) || static_cast<long long>(p.H) * p.W >= (1ll << 30) || static_cast<long long>(p.OH) * p.OW >= (1ll << 30) ||
+        (p.KH - 1) * a.dil_h >= (1 << 15) || (p.KW - 1) * a.dil_w >= (1 << 16))
+        return -1;
+    constexpr int kStage = NPL * BN * 32 * (BF ? 2 : 4);
+    const int table_bytes = a.use_table ? a.kblocks * 32 * 8 : 0;
+    const int smem = kStagesIg * kStage + table_bytes + 1024;
+    if (smem > 227 * 1024) return -1;
+    auto kern = conv_igemm_kernel<BN, PLANES>;
     static SmemAttrCache attr_cache;
     if (int rc = ensure_dynamic_smem(kern, smem, attr_cache)) return rc;
     // algorithmic work of the layer: direct-convolution FLOPs; input + filters read once, output written once
     const double macs = static_cast<double>(p.N) * p.OC * p.OH * p.OW * p.IC * taps;
-    const double mma = 2.0 * static_cast<double>(a.pixel_tiles) * 128 * CG * (a.num_n * BN) * (a.kblocks * 32) * (PLANES >= 2 ? 3 : 1);
+    const double mma = 2.0 * static_cast<double>(pixel_tiles) * 128 * (a.num_n * BN) * (a.kblocks * 32) * (PLANES >= 2 ? 3 : 1);
     const int prof = prof_begin(stream, PROF_IGEMM, 2.0 * macs, mma,
                                 4.0 * (static_cast<double>(p.N) * p.IC * p.H * p.W + static_cast<double>(p.OC) * K +
                                        static_cast<double>(p.N) * p.OC * p.OH * p.OW * (p.residual ? 2 : 1)));
-    CUtensorMap tmIn = tmW;
-    if (SLAB) {  // 4-D map over the NCHW input (or a channel slice of it): {W, H, IC, N}, box {48, 6, 32, 1}, zero OOB fill
-        cuuint64_t dims[4] = {(cuuint64_t)p.W, (cuuint64_t)p.H, (cuuint64_t)p.IC, (cuuint64_t)p.N};
-        cuuint64_t strides[3] = {(cuuint64_t)p.W * 4, (cuuint64_t)p.W * p.H * 4, (cuuint64_t)a.in_img_c * p.W * p.H * 4};
-        cuuint32_t box[4] = {(cuuint32_t)kSlabCols, (cuuint32_t)kSlabRows, 32, 1};
-        cuuint32_t estr[4] = {1, 1, 1, 1};
-        CUresult r = enc(&tmIn, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, const_cast<float*>(p.input), dims, strides, box, estr,
-                         CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                         CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-        if (r != CUDA_SUCCESS) {
-            fprintf(stderr, "fcuda: igemm input tensor map failed (%d)\n", (int)r);
-            return FCUDA_ERR_CUDA;
-        }
-    }
-    if (PW) {  // 3-D map over the input with every image as one row: {H*W, IC, N}, box {32 pixels, 32 channels, 1}
-        cuuint64_t dims[3] = {(cuuint64_t)p.W, (cuuint64_t)p.IC, (cuuint64_t)p.N};
-        cuuint64_t strides[2] = {(cuuint64_t)p.W * 4, (cuuint64_t)a.in_img_c * p.W * 4};
-        cuuint32_t box[3] = {32, 32, 1};
-        cuuint32_t estr[3] = {1, 1, 1};
-        CUresult r = enc(&tmIn, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, const_cast<float*>(p.input), dims, strides, box, estr,
-                         CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                         CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-        if (r != CUDA_SUCCESS) {
-            fprintf(stderr, "fcuda: igemm pointwise input tensor map failed (%d)\n", (int)r);
-            return FCUDA_ERR_CUDA;
-        }
-    }
-    // 4-D map over the NCHW output (or a channel slice of it): {OW, OH, OC, N}; box = one epilogue chunk: 32 channels x
-    // (32 pixels of a row | a 2 x 16 sub-patch in SLAB mode).  Needs 16-byte rows; pooled launches keep direct stores.
-    CUtensorMap tmOut = tmW;
-    a.tma_out = 0;
-    if (tune_get(TUNE_IGEMM_TMA_OUT) && !a.pool && OWe % 4 == 0 && (reinterpret_cast<uintptr_t>(p.output) & 15) == 0) {
-        cuuint64_t dims[4] = {(cuuint64_t)OWe, (cuuint64_t)OHe, (cuuint64_t)p.OC, (cuuint64_t)p.N};
-        cuuint64_t strides[3] = {(cuuint64_t)OWe * 4, (cuuint64_t)OWe * OHe * 4, (cuuint64_t)a.out_img_c * OWe * OHe * 4};
-        cuuint32_t box[4] = {SLAB ? 16u : 32u, SLAB ? 2u : 1u, 32, 1};
-        cuuint32_t estr[4] = {1, 1, 1, 1};
-        CUresult r = enc(&tmOut, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, p.output, dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                         CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-        if (r != CUDA_SUCCESS) {
-            fprintf(stderr, "fcuda: igemm output tensor map failed (%d)\n", (int)r);
-            return FCUDA_ERR_CUDA;
-        }
-        a.tma_out = 1;
-    }
-    if (CG == 1) {
-        kern<<<grid, kThreadsIg, smem, stream>>>(tmW, tmWlo, tmIn, tmOut, a);
-    } else {  // CTA pairs: as many clusters as can be co-resident, never more than there are work items
-        cudaLaunchConfig_t cfg = {};
-        cudaLaunchAttribute attr[1];
-        attr[0].id = cudaLaunchAttributeClusterDimension;
-        attr[0].val.clusterDim.x = CG; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
-        cfg.blockDim = dim3(kThreadsIg); cfg.dynamicSmemBytes = smem; cfg.stream = stream; cfg.attrs = attr; cfg.numAttrs = 1;
-        static int max_clusters[kMaxDevices] = {};
-        const int dev = current_device();
-        if (max_clusters[dev] == 0) {
-            cfg.gridDim = dim3(static_cast<unsigned>(sm_count() / CG * CG));
-            int n = 0;
-            if (cudaOccupancyMaxActiveClusters(&n, kern, &cfg) != cudaSuccess || n <= 0) {
-                cudaGetLastError();
-                n = sm_count() / CG;
-            }
-            max_clusters[dev] = n;
-        }
-        const long long nclusters = total < max_clusters[dev] ? total : max_clusters[dev];
-        grid = static_cast<int>(nclusters * CG);
-        cfg.gridDim = dim3(static_cast<unsigned>(grid));
-        FCUDA_CHECK(cudaLaunchKernelEx(&cfg, kern, tmW, tmWlo, tmIn, tmOut, a));
-    }
+    kern<<<static_cast<unsigned>(total), kThreadsIg, smem, stream>>>(tmW, tmWlo, a);
     prof_end(prof, stream);
     FCUDA_CHECK_LAUNCH();
     count_launch();
@@ -1477,57 +497,21 @@ int conv_igemm_pack_weights(const float* w, float* w_hi, float* w_lo, int OC, in
     return 0;
 }
 
-// 3x3, stride 1, dense taps, whole 32-channel blocks: the slab producer (FCUDA_IGEMM_SLAB=0 keeps the generic gather)
-static bool slab_eligible(const IgemmProblem& p) {
-    const bool off = tune_get(TUNE_IGEMM_SLAB) == 0;
-    // + what the TMA needs: 16-byte rows and base (W % 4 == 0 keeps every channel / image / group slice aligned)
-    return !off && p.KH == 3 && p.KW == 3 && p.stride_h == 1 && p.stride_w == 1 && p.dil_h <= 1 && p.dil_w <= 1 &&
-           p.IC % 32 == 0 && p.pad_top <= 2 && p.pad_left <= 2 && p.W % 4 == 0 &&
+// The fused 2x2 max pooling serves the 3x3 / stride-1 layers with whole 32-channel blocks that precede a pooling layer
+// (VGG-style stacks); the other layers keep a separate pooling launch.
+bool conv_igemm_can_pool(const IgemmProblem& p) {
+    return p.KH == 3 && p.KW == 3 && p.stride_h == 1 && p.stride_w == 1 && p.dil_h <= 1 && p.dil_w <= 1 && p.IC % 32 == 0 &&
+           p.pad_top <= 2 && p.pad_left <= 2 && p.W % 4 == 0 && p.residual == nullptr &&
            (p.input == nullptr || (reinterpret_cast<uintptr_t>(p.input) & 15) == 0);
-}
-
-bool conv_igemm_can_pool(const IgemmProblem& p) { return slab_eligible(p) && p.residual == nullptr; }
-
-// CTA pairs (cta_group::2) when the layer has enough pixel tiles to keep every pair busy (FCUDA_IGEMM_CG=1|2 overrides)
-static int pick_cg(const IgemmProblem& p) {
-    // Measured on B200 (profiles/r02j_lean_cta_group2.log): pairs are bit-identical to single CTAs but slower (VGG-16 7.35 vs
-    // 5.82 ms, ResNet-50 10.2 vs 8.0) — with a 4-deep operand ring the two extra cross-CTA hops per k-block (multicast slot
-    // release, remote full arrival) are not hidden.  Default stays 1; FCUDA_IGEMM_CG=2 / fcuda_set_tuning select pairs.
-    if (p.planes != 2 || p.OC <= 32) return 1;
-    return tune_get(TUNE_IGEMM_CG);
-}
-
-// 1x1, stride 1, no padding, the image addressed as one row (fcuda_api.cu does that), whole 32-channel blocks and what the
-// TMA needs (16-byte image rows / base): the pointwise slab producer (FCUDA_IGEMM_PW=0 keeps the generic gather)
-static bool pw_eligible(const IgemmProblem& p) {
-    return tune_get(TUNE_IGEMM_PW) != 0 && p.KH == 1 && p.KW == 1 && p.stride_h == 1 && p.stride_w == 1 && p.pad_top == 0 &&
-           p.pad_left == 0 && p.H == 1 && p.OH == 1 && p.IC % 32 == 0 && p.W % 4 == 0 && p.pool == 0 &&
-           (reinterpret_cast<uintptr_t>(p.input) & 15) == 0;
-}
-
-template <int SLAB>
-static int dispatch_igemm(const IgemmProblem& p, cudaStream_t stream) {
-    if (p.planes == 3) {  // BF16x3
-        if (p.OC <= 32) return launch_igemm<32, 3, SLAB, 1>(p, stream);
-        if (p.OC <= 64) return launch_igemm<64, 3, SLAB, 1>(p, stream);
-        return launch_igemm<128, 3, SLAB, 1>(p, stream);
-    }
-    const bool x3 = p.planes == 2;
-    if (x3 && SLAB != 2 && pick_cg(p) == 2) {
-        if (p.OC <= 64) return launch_igemm<64, 2, SLAB == 2 ? 0 : SLAB, 2>(p, stream);
-        return launch_igemm<128, 2, SLAB == 2 ? 0 : SLAB, 2>(p, stream);
-    }
-    if (p.OC <= 32) return x3 ? launch_igemm<32, 2, SLAB, 1>(p, stream) : launch_igemm<32, 1, SLAB, 1>(p, stream);
-    if (p.OC <= 64) return x3 ? launch_igemm<64, 2, SLAB, 1>(p, stream) : launch_igemm<64, 1, SLAB, 1>(p, stream);
-    return x3 ? launch_igemm<128, 2, SLAB, 1>(p, stream) : launch_igemm<128, 1, SLAB, 1>(p, stream);
 }
 
 int conv_igemm_forward(const IgemmProblem& p, cudaStream_t stream) {
     if (!conv_igemm_supported(p.IC, p.KH, p.KW)) return -1;
     if (p.pool && !conv_igemm_can_pool(p)) return -200;
-    if (slab_eligible(p)) return dispatch_igemm<1>(p, stream);
-    if (pw_eligible(p)) return dispatch_igemm<2>(p, stream);
-    return dispatch_igemm<0>(p, stream);
+    const int bn = igemm_bn_for(p.OC);
+    if (p.planes == 3) return bn == 32 ? launch_igemm<32, 3>(p, stream) : bn == 64 ? launch_igemm<64, 3>(p, stream) : launch_igemm<128, 3>(p, stream);
+    if (p.planes == 2) return bn == 32 ? launch_igemm<32, 2>(p, stream) : bn == 64 ? launch_igemm<64, 2>(p, stream) : launch_igemm<128, 2>(p, stream);
+    return bn == 32 ? launch_igemm<32, 1>(p, stream) : bn == 64 ? launch_igemm<64, 1>(p, stream) : launch_igemm<128, 1>(p, stream);
 }
 
 }  // namespace fcuda

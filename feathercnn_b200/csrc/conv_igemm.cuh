@@ -1,4 +1,4 @@
-// Implicit-GEMM convolution on tcgen05 (see conv_igemm.cu).
+// Implicit-GEMM convolution on Hopper warpgroup MMA (see conv_igemm.cu).
 #pragma once
 #include <cuda_runtime.h>
 

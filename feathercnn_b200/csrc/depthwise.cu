@@ -321,7 +321,7 @@ dw3x3_plane_kernel(const float* __restrict__ in, const float* __restrict__ w, co
 // one plane — LP = 16 or 8 lanes per plane, 2 or 4 planes per warp — loads that column's H values up front (H independent
 // loads in flight per lane), gets the left / right neighbours of every row with sub-warp shuffles and writes its output
 // column.  ~13 instructions per output row and lane; the shared-memory plane kernel above needs ~300 warp instructions per
-// 14x14 plane, which is issue-bound at 0.32 of HBM bandwidth (profiles/r02k_mobilenet_v1_launches_summary.txt).
+// 14x14 plane and is issue-bound there.
 template <int LP>
 __global__ void __launch_bounds__(128)
 dw3x3_cols_kernel(const float* __restrict__ in, const float* __restrict__ w, const float* __restrict__ bias,

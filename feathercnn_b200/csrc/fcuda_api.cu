@@ -30,10 +30,9 @@ int env_precision() {
 size_t env_chunk() {
     const char* e = getenv("FCUDA_L2_CHUNK_MB");
     if (e) return static_cast<size_t>(atof(e) * 1024.0 * 1024.0);
-    // Default: effectively one chunk per layer.  Measured on B200 (profiles/r01_sweep_chunk.log): VGG-16 b64 runs
-    // 25.9 / 14.7 / 12.5 / 11.4 ms per step at 12 / 48 / 192 MiB / unbounded — the intermediates do not stay
-    // L2-resident across the three kernels, so smaller chunks only add launches and tail effects.  The bound keeps
-    // the scratch pool finite for very large batches.
+    // Default: effectively one chunk per layer (the Winograd / im2col intermediates of a layer exceed the L2 either way,
+    // so smaller chunks only add launches and tail effects).  The bound keeps the scratch pool finite for very large
+    // batches.
     return static_cast<size_t>(8) << 30;
 }
 

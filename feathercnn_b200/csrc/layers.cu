@@ -50,7 +50,7 @@ pooling_kernel(const float* __restrict__ in, float* __restrict__ out, PoolGeom g
 // 3x3 / stride 2 / no padding (ResNet-50's pool1, ceil mode: the last window may be clipped): a warp marches down 16 output
 // rows of a 32-column strip; per input row a lane loads one float2 (columns 2*ox, 2*ox+1) and takes column 2*ox+2 from the
 // next lane by shuffle; every input row is loaded once per strip (the generic kernel above issues 9 scalar loads and ~100
-// instructions of 64-bit index math per output: 0.31 of HBM bandwidth on ResNet-50, profiles/r02k_resnet50_launches_summary.txt).
+// instructions of 64-bit index math per output).
 __global__ void __launch_bounds__(128)
 pool3x3s2_kernel(const float* __restrict__ in, float* __restrict__ out, int H, int W, int OH, int OW, int type, long long items,
                  int xstrips, int ystrips) {

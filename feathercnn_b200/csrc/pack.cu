@@ -1,4 +1,4 @@
-// Operand packing kernels for the tcgen05 TensorGEMM.
+// Operand packing kernels for the wgmma TensorGEMM.
 //
 //   im2col_pack   replaces booster::im2col (/root/reference/src/booster/avx/generic_kernels.cpp:50-85) and
 //                 pack_B_avx (avx/sgemm.cpp:350-375): gathers the (ic,u,v) patch of every output pixel into a

@@ -1,27 +1,17 @@
-// TensorGEMM on tcgen05 (sm_100a).  See tensor_gemm.cuh for the contract.
+// TensorGEMM on Hopper warpgroup MMA (sm_90a).  See tensor_gemm.cuh for the contract.
 //
-// Two persistent kernels, one CTA per SM:
-//
-// tensor_gemm_ts_kernel<BN>  (3xTF32, the product path: Winograd's 64-way batched GEMM, im2col GEMM, InnerProduct)
-//   warp 0        TMA producer : per 32-wide k-block one raw fp32 A tile (128 rows) + the B_hi and B_lo tiles
-//                                (cp.async.bulk.tensor 3-D boxes, 128-byte swizzle) into a 4-deep smem ring
-//   warps 6..13   splitters    : two groups of 4 alternate k-blocks; a thread reads its (swizzled) A row from smem, splits
-//                                it into TF32 hi + fp32 lo (2 instructions per element) and parks both in tensor memory
-//                                (tcgen05.st), so A is ONE plane in HBM and the MMA takes it from TMEM (TS form: no 4 KB
-//                                smem read per instruction, measured 33 cycles each)
-//   warp 1        MMA issuer   : A_lo*B_hi + A_hi*B_lo + A_hi*B_hi per k-step into one fp32 TMEM accumulator; the next
-//                                slot's barrier is probed between MMAs because the pipe only queues ~6 of them
-//   warps 2..5    epilogue     : tcgen05.ld 32x32b -> fused store (row-major / NCHW+bias+ReLU / transposed split-K atomics)
-//   (a second issuer warp exists behind FCUDA_TS_ISSUERS=2; measured 2 % slower here, unlike in conv_igemm.cu)
-//
-// tensor_gemm_kernel<BN,PLANES,STAGES>  (plain TF32 mode and A/B tests: both operands from smem, "SS" form, 192 threads)
-//   warp 0 TMA, warp 1 MMA, warps 2..5 epilogue.
-//
-// Both: STAGES-deep operand ring (full/empty mbarriers) and a 2-deep TMEM accumulator ring (tmem_full/tmem_empty) so
-// the epilogue of tile i overlaps the MMAs of tile i+1; bounded mbarrier waits trap instead of hanging the GPU.
+// tensor_gemm_kernel<BN, PLANES>: one CTA per 128 x BN output tile (and k-split), 288 threads:
+//   warp 8        TMA producer : per 32-wide k-block the raw fp32 A tile (128 rows) and the B_hi (+ B_lo) tiles
+//                                (cp.async.bulk.tensor 3-D boxes, 128-byte swizzle) into a kStages-deep smem ring
+//   warps 0..7    two consumer warpgroups, 64 rows each: a thread reads its A fragment from the swizzled tile, splits it
+//                 into TF32 hi + fp32 lo (PLANES == 2) in registers and issues wgmma.mma_async with A from registers and B
+//                 from shared memory: A_lo*B_hi + A_hi*B_lo + A_hi*B_hi per k-step of 8 into fp32 register
+//                 accumulators; then the fused store (row-major / NCHW+bias+ReLU / k-split partial planes).
+// A is ONE fp32 plane in HBM (the split happens on chip); full / empty mbarriers hand the ring slots over, and a bounded
+// wait traps instead of hanging the GPU.
 #include "tensor_gemm.cuh"
 #include "common.cuh"
-#include "tcgen05.cuh"
+#include "wgmma.cuh"
 
 #include <atomic>
 #include <string.h>
@@ -36,7 +26,9 @@ namespace fcuda {
 // --------------------------------------------------------------------------------------------
 constexpr int kBM = 128;
 constexpr int kBK = 32;  // fp32 elements per k-block = 128 bytes = one swizzle atom
-constexpr int kThreads = 192;
+constexpr int kConsumerWarps = 8;
+constexpr int kThreads = (kConsumerWarps + 1) * 32;
+constexpr int kStages = 4;
 
 struct GemmKernelArgs {
     float* D;
@@ -46,640 +38,162 @@ struct GemmKernelArgs {
     int num_m, num_n, k_blocks_total;
     long long m_offset;
     long long split_stride;
-    int tma_store;   // EPI_ROWMAJOR through shared memory + cp.async.bulk.tensor stores (tmD is valid)
-    int st256;       // EPI_ROWMAJOR direct stores as 32-byte st.global.v8 (whole sectors per lane; gemm_tma_store = 2)
-    unsigned suspend_ns;  // suspend hint of the operand-ring waits (0 = poll), see ptx::mbar_try_wait_ns
+    int vec2;  // EPI_ROWMAJOR: pairs of columns leave as one 8-byte store (ldd even, D 8-byte aligned)
 };
 
-template <int BN, int PLANES>
-struct SmemLayout {
-    static constexpr int kATile = kBM * kBK * 4;  // 16 KB
-    static constexpr int kBTile = BN * kBK * 4;
-    static constexpr int kStage = PLANES * (kATile + kBTile);
-};
-
-// Drains one 128 x BN accumulator (TMEM lanes q*32 .. q*32+31 for this warp) through the fused store selected by
-// args.epilogue.  Shared by the smem-operand kernel and the TMEM-A (3xTF32) kernel.
+// Stores the two rows (m0, m0 + 8) x BN/4 column pairs this thread holds through the fused store of args.epilogue.
 template <int BN>
-__device__ __forceinline__ void epilogue_store(const GemmKernelArgs& args, uint32_t tmem_base, int as, int q, int lane,
-                                               int g, int m_blk, int n_blk, int ks) {
-    const int m = m_blk * kBM + q * 32 + lane;
-    const bool m_ok = m < args.M;
-    const uint32_t taddr0 = tmem_base + (static_cast<uint32_t>(q * 32) << 16) + as * BN;
-
-    // per-row output bases
-    size_t row_base = 0;
-    int img = 0, pix = 0;
-    if (args.epilogue == EPI_ROWMAJOR) {
-        row_base = (static_cast<size_t>(g) * args.M + (m_ok ? m : 0)) * args.ldd;
-    } else if (args.epilogue == EPI_NCHW) {
-        const long long mg = args.m_offset + (m_ok ? m : 0);
-        img = static_cast<int>(mg / args.P);
-        pix = static_cast<int>(mg - static_cast<long long>(img) * args.P);
-    }
-#pragma unroll 1
-    for (int c0 = 0; c0 < BN; c0 += 32) {
-        const int n0 = n_blk * BN + c0;
-        if (n0 >= args.N) break;  // warp-uniform
-        uint32_t r[32];
-        ptx::tmem_ld_32x32(taddr0 + c0, r);
-        ptx::tmem_ld_wait();
-        if (m_ok) {
-            if (args.epilogue == EPI_ROWMAJOR) {
-                float* dst = args.D + row_base + n0;
-                if (args.st256 && n0 + 32 <= args.N && (args.ldd & 7) == 0) {
-                    // a lane owns a 128-byte row piece: four 32-byte stores = four whole sectors, no shared-memory staging
+__device__ __forceinline__ void epilogue_store(const GemmKernelArgs& args, const float (&acc)[BN / 2], int g, int m0,
+                                               int n_base, int c, int ks) {
 #pragma unroll
-                    for (int j = 0; j < 32; j += 8)
-                        asm volatile("st.global.v8.b32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8};" ::"l"(dst + j), "r"(r[j]), "r"(r[j + 1]),
-                                     "r"(r[j + 2]), "r"(r[j + 3]), "r"(r[j + 4]), "r"(r[j + 5]), "r"(r[j + 6]), "r"(r[j + 7])
-                                     : "memory");
-                } else if (n0 + 32 <= args.N && (args.ldd & 3) == 0) {
+    for (int h = 0; h < 2; ++h) {
+        const int m = m0 + 8 * h;
+        if (m >= args.M) continue;
+        if (args.epilogue == EPI_ROWMAJOR) {
+            float* row = args.D + (static_cast<size_t>(g) * args.M + m) * args.ldd;
 #pragma unroll
-                    for (int j = 0; j < 32; j += 4) {
-                        float4 v = make_float4(__uint_as_float(r[j]), __uint_as_float(r[j + 1]),
-                                               __uint_as_float(r[j + 2]), __uint_as_float(r[j + 3]));
-                        *reinterpret_cast<float4*>(dst + j) = v;
-                    }
+            for (int j = 0; j < BN / 8; ++j) {
+                const int n = n_base + 8 * j + 2 * c;
+                const float v0 = acc[4 * j + 2 * h], v1 = acc[4 * j + 2 * h + 1];
+                if (args.vec2 && n + 1 < args.N) {
+                    *reinterpret_cast<float2*>(row + n) = make_float2(v0, v1);
                 } else {
-#pragma unroll
-                    for (int j = 0; j < 32; ++j)
-                        if (n0 + j < args.N) dst[j] = __uint_as_float(r[j]);
+                    if (n < args.N) row[n] = v0;
+                    if (n + 1 < args.N) row[n + 1] = v1;
                 }
-            } else if (args.epilogue == EPI_NCHW) {
-                // lanes hold consecutive pixels -> each column store is a coalesced 128-byte line
-                float* dst = args.D + (static_cast<size_t>(img) * args.N + n0) * args.P + pix;
+            }
+        } else if (args.epilogue == EPI_NCHW) {
+            const long long mg = args.m_offset + m;
+            const int img = static_cast<int>(mg / args.P);
+            const int pix = static_cast<int>(mg - static_cast<long long>(img) * args.P);
+            float* dst = args.D + static_cast<size_t>(img) * args.N * args.P + pix;
 #pragma unroll
-                for (int j = 0; j < 32; ++j) {
-                    if (n0 + j < args.N) {
-                        float v = __uint_as_float(r[j]);
-                        if (args.bias) v += __ldg(args.bias + n0 + j);
+            for (int j = 0; j < BN / 8; ++j) {
+#pragma unroll
+                for (int e = 0; e < 2; ++e) {
+                    const int n = n_base + 8 * j + 2 * c + e;
+                    if (n < args.N) {
+                        float v = acc[4 * j + 2 * h + e];
+                        if (args.bias) v += __ldg(args.bias + n);
                         if (args.relu) v = fmaxf(v, 0.f);
-                        dst[static_cast<size_t>(j) * args.P] = v;
+                        dst[static_cast<size_t>(n) * args.P] = v;
                     }
                 }
-            } else {  // EPI_COLMAJOR_PARTIAL: this k-split's plane, plain stores (lanes = consecutive m -> coalesced)
-                float* dst = args.D + static_cast<size_t>(ks) * args.split_stride + static_cast<size_t>(n0) * args.ldd + m;
+            }
+        } else {  // EPI_COLMAJOR_PARTIAL: this k-split's plane, plain stores
+            float* dst = args.D + static_cast<size_t>(ks) * args.split_stride + m;
 #pragma unroll
-                for (int j = 0; j < 32; ++j)
-                    if (n0 + j < args.N) dst[static_cast<size_t>(j) * args.ldd] = __uint_as_float(r[j]);
+            for (int j = 0; j < BN / 8; ++j) {
+#pragma unroll
+                for (int e = 0; e < 2; ++e) {
+                    const int n = n_base + 8 * j + 2 * c + e;
+                    if (n < args.N) dst[static_cast<size_t>(n) * args.ldd] = acc[4 * j + 2 * h + e];
+                }
             }
         }
     }
 }
 
-template <int BN, int PLANES, int STAGES>
+template <int BN, int PLANES>
 __global__ void __launch_bounds__(kThreads, 1)
-tensor_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmAlo,
-                   const __grid_constant__ CUtensorMap tmB, const __grid_constant__ CUtensorMap tmBlo,
-                   const GemmKernelArgs args) {
-    using L = SmemLayout<BN, PLANES>;
+tensor_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
+                   const __grid_constant__ CUtensorMap tmBlo, const GemmKernelArgs args) {
+    constexpr int kATile = kBM * kBK * 4;  // 16 KB raw A
+    constexpr int kBTile = BN * kBK * 4;
+    constexpr int kStage = kATile + PLANES * kBTile;  // [A raw][B_hi][B_lo]
     extern __shared__ uint8_t smem_raw[];
     // SWIZZLE_128B tiles need 1024-byte alignment.
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-
-    __shared__ uint64_t full_bar[STAGES];
-    __shared__ uint64_t empty_bar[STAGES];
-    __shared__ uint64_t tmem_full_bar[2];
-    __shared__ uint64_t tmem_empty_bar[2];
-    __shared__ uint32_t tmem_base_smem;
+    __shared__ uint64_t full_bar[kStages];
+    __shared__ uint64_t empty_bar[kStages];
 
     const int warp = threadIdx.x >> 5;
     const int lane = threadIdx.x & 31;
 
-    const int tiles_per_g = args.num_m * args.num_n;
-    const int total_tiles = tiles_per_g * args.G * args.split_k;
+    // tile = ((ks * G + g) * num_m + m_blk) * num_n + n_blk: neighbouring CTAs share the A tile
+    const int tile = blockIdx.x;
+    const int n_blk = tile % args.num_n;
+    const int t1 = tile / args.num_n;
+    const int m_blk = t1 % args.num_m;
+    const int t2 = t1 / args.num_m;
+    const int g = t2 % args.G;
+    const int ks = t2 / args.G;
     const int kb_per_split = (args.k_blocks_total + args.split_k - 1) / args.split_k;
+    const int kb0 = ks * kb_per_split;
+    const int nk = min(kb0 + kb_per_split, args.k_blocks_total) - kb0;
 
     if (threadIdx.x == 0) {
-        for (int s = 0; s < STAGES; ++s) {
+        for (int s = 0; s < kStages; ++s) {
             ptx::mbar_init(&full_bar[s], 1);
-            ptx::mbar_init(&empty_bar[s], 1);
-        }
-        for (int s = 0; s < 2; ++s) {
-            ptx::mbar_init(&tmem_full_bar[s], 1);
-            ptx::mbar_init(&tmem_empty_bar[s], 4);  // one arrive per epilogue warp
+            ptx::mbar_init(&empty_bar[s], kConsumerWarps);
         }
         ptx::fence_barrier_init();
     }
-    if (warp == 0 && lane == 0) {
-        ptx::prefetch_tensormap(&tmA);
-        ptx::prefetch_tensormap(&tmB);
-        if (PLANES == 2) {
-            ptx::prefetch_tensormap(&tmAlo);
-            ptx::prefetch_tensormap(&tmBlo);
-        }
-    }
-    constexpr uint32_t kTmemCols = (2 * BN <= 32) ? 32 : (2 * BN <= 64) ? 64 : (2 * BN <= 128) ? 128 : (2 * BN <= 256) ? 256 : 512;
-    if (warp == 1) {
-        ptx::tmem_alloc(&tmem_base_smem, kTmemCols);
-        ptx::tmem_relinquish();
-    }
-    ptx::tc_fence_before();
     __syncthreads();
-    ptx::tc_fence_after();
-    const uint32_t tmem_base = tmem_base_smem;
 
-    if (warp == 0) {
+    if (warp == kConsumerWarps) {
         // ===================== TMA producer =====================
-        // whole warp walks the loop (warp-uniform control flow), one elected lane issues
-        const bool leader = ptx::elect_one();
-        int stage = 0;
-        uint32_t phase = 0;
-        for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
-            const int ks = tile / (tiles_per_g * args.G);
-            const int rem = tile - ks * (tiles_per_g * args.G);
-            const int g = rem / tiles_per_g;
-            const int mn = rem - g * tiles_per_g;
-            const int m_blk = mn / args.num_n;
-            const int n_blk = mn - m_blk * args.num_n;
-            const int kb0 = ks * kb_per_split;
-            const int kb1 = min(kb0 + kb_per_split, args.k_blocks_total);
-            for (int kb = kb0; kb < kb1; ++kb) {
-                ptx::mbar_wait(&empty_bar[stage], phase ^ 1);
-                if (leader) {
-                    uint8_t* st = smem + stage * L::kStage;
-                    ptx::mbar_arrive_expect_tx(&full_bar[stage], L::kStage);
-                    ptx::tma_load_3d(st, &tmA, &full_bar[stage], kb * kBK, m_blk * kBM, g);
-                    ptx::tma_load_3d(st + L::kATile, &tmB, &full_bar[stage], kb * kBK, n_blk * BN, g);
-                    if (PLANES == 2) {
-                        ptx::tma_load_3d(st + L::kATile + L::kBTile, &tmAlo, &full_bar[stage], kb * kBK, m_blk * kBM, g);
-                        ptx::tma_load_3d(st + 2 * L::kATile + L::kBTile, &tmBlo, &full_bar[stage], kb * kBK, n_blk * BN, g);
-                    }
-                }
-                __syncwarp();
-                if (++stage == STAGES) { stage = 0; phase ^= 1; }
+        if (lane == 0) {
+            ptx::prefetch_tensormap(&tmA);
+            ptx::prefetch_tensormap(&tmB);
+            if (PLANES == 2) ptx::prefetch_tensormap(&tmBlo);
+            for (int i = 0; i < nk; ++i) {
+                const int stage = i % kStages;
+                if (i >= kStages) ptx::mbar_wait(&empty_bar[stage], ((i / kStages) - 1) & 1);
+                uint8_t* st = smem + stage * kStage;
+                const int kc = (kb0 + i) * kBK;
+                ptx::mbar_arrive_expect_tx(&full_bar[stage], kStage);
+                ptx::tma_load_3d(st, &tmA, &full_bar[stage], kc, m_blk * kBM, g);
+                ptx::tma_load_3d(st + kATile, &tmB, &full_bar[stage], kc, n_blk * BN, g);
+                if (PLANES == 2) ptx::tma_load_3d(st + kATile + kBTile, &tmBlo, &full_bar[stage], kc, n_blk * BN, g);
             }
         }
-    } else if (warp == 1) {
-        // ===================== MMA issuer =====================
-        constexpr uint32_t idesc = make_idesc_tf32(BN);
-        const bool leader = ptx::elect_one();
-        const uint64_t d0 = make_smem_desc_sw128(ptx::smem_u32(smem));  // descriptors differ only in the start address
-        int stage = 0;
-        uint32_t phase = 0;
-        int it = 0;
-        for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x, ++it) {
-            const int ks = tile / (tiles_per_g * args.G);
-            const int kb0 = ks * kb_per_split;
-            const int kb1 = min(kb0 + kb_per_split, args.k_blocks_total);
-            const int as = it & 1;
-            const uint32_t aphase = (it >> 1) & 1;
-            ptx::mbar_wait(&tmem_empty_bar[as], aphase ^ 1);
-            ptx::tc_fence_after();
-            const uint32_t tmem_d = tmem_base + as * BN;
-            for (int kb = kb0; kb < kb1; ++kb) {
-                ptx::mbar_wait(&full_bar[stage], phase);
-                ptx::tc_fence_after();
-                if (leader) {
-                    // start-address field is in 16-byte units; 32 bytes (8 tf32) per k-step inside the swizzle atom
-                    const uint64_t dA = d0 + static_cast<uint64_t>(stage * (L::kStage >> 4));
-                    const uint64_t dB = dA + static_cast<uint64_t>(L::kATile >> 4);
-                    const uint64_t dAlo = dB + static_cast<uint64_t>(L::kBTile >> 4);
-                    const uint64_t dBlo = dAlo + static_cast<uint64_t>(L::kATile >> 4);
-#pragma unroll
-                    for (int k = 0; k < kBK / 8; ++k) {
-                        const uint32_t first = (kb == kb0 && k == 0) ? 0u : 1u;
-                        if (PLANES == 2) {
-                            ptx::umma_tf32(tmem_d, dAlo + 2 * k, dB + 2 * k, idesc, first);
-                            ptx::umma_tf32(tmem_d, dA + 2 * k, dBlo + 2 * k, idesc, 1u);
-                            ptx::umma_tf32(tmem_d, dA + 2 * k, dB + 2 * k, idesc, 1u);
-                        } else {
-                            ptx::umma_tf32(tmem_d, dA + 2 * k, dB + 2 * k, idesc, first);
-                        }
-                    }
-                    ptx::umma_commit(&empty_bar[stage]);  // frees the smem slot when these MMAs retire
-                }
-                __syncwarp();
-                if (++stage == STAGES) { stage = 0; phase ^= 1; }
-            }
-            if (leader) ptx::umma_commit(&tmem_full_bar[as]);  // accumulator ready for the epilogue
-            __syncwarp();
-        }
-    } else {
-        // ===================== epilogue (warps 2..5) =====================
-        const int q = warp & 3;  // TMEM lane quadrant this warp may access
-        int it = 0;
-        for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x, ++it) {
-            const int ks = tile / (tiles_per_g * args.G);
-            const int rem = tile - ks * (tiles_per_g * args.G);
-            const int g = rem / tiles_per_g;
-            const int mn = rem - g * tiles_per_g;
-            const int m_blk = mn / args.num_n;
-            const int n_blk = mn - m_blk * args.num_n;
-            const int as = it & 1;
-            const uint32_t aphase = (it >> 1) & 1;
-            ptx::mbar_wait(&tmem_full_bar[as], aphase);
-            ptx::tc_fence_after();
-
-            epilogue_store<BN>(args, tmem_base, as, q, lane, g, m_blk, n_blk, ks);
-            // hand the accumulator stage back to the MMA warp
-            ptx::tc_fence_before();
-            __syncwarp();
-            if (lane == 0) ptx::mbar_arrive(&tmem_empty_bar[as]);
-        }
+        return;
     }
 
-    ptx::tc_fence_before();
-    __syncthreads();
-    if (warp == 1) {
-        ptx::tc_fence_after();
-        ptx::tmem_dealloc(tmem_base, kTmemCols);
-    }
-}
+    // ===================== consumers: two warpgroups of 64 rows =====================
+    const int gq = lane >> 2, c = lane & 3;
+    const int row0 = warp * 16 + gq;  // tile rows row0 and row0 + 8; row & 7 == gq for both (128B swizzle phase)
+    float acc[BN / 2];
+#pragma unroll
+    for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
 
-// --------------------------------------------------------------------------------------------
-// 3xTF32 kernel: A raw in global memory, split in-kernel into tensor memory, TS-form MMAs
-// --------------------------------------------------------------------------------------------
-// warp 0 TMA | warp 1 MMA | warps 2-5 epilogue | warps 6-9 and 10-13 splitter groups (alternate k-blocks)
-constexpr int kWarpIssuer2 = 14;     // second MMA issuer of the ISSUERS == 2 variant (the first is warp 1)
-constexpr int kDefaultTsIssuers = 1;
-constexpr int kThreadsTs = 14 * 32;
-constexpr int kStagesTs = 4;
-
-__device__ __forceinline__ void umma_tf32_ts(uint32_t tmem_d, uint32_t tmem_a, uint64_t desc_b, uint32_t idesc,
-                                             uint32_t accumulate) {
-    asm volatile(
-        "{\n\t"
-        ".reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::tf32 [%0], [%1], %2, %3, p;\n\t"
-        "}"
-        ::"r"(tmem_d), "r"(tmem_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-__device__ __forceinline__ void tmem_st_32x16(uint32_t taddr, const uint32_t (&r)[16]) {
-    asm volatile(
-        "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], "
-        "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16};"
-        ::"r"(taddr), "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(r[8]),
-        "r"(r[9]), "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15])
-        : "memory");
-}
-
-// CL > 1: CL CTAs of a thread-block cluster work on CL consecutive M tiles of the same (g, n-block) and share the B tiles:
-// each CTA fetches 1/CL of the B_hi / B_lo rows and TMA-multicasts them into every CTA's ring slot, so the L2 -> SM traffic of
-// B (the transformed filters, re-read by every M tile: 2.5 GB through L2 per VGG conv3 launch in round 1, the kernel's
-// measured limiter) drops by CL.  A slot may only be overwritten once EVERY CTA of the cluster has retired the MMAs that
-// read it: the producers exchange that through peer_free_bar (remote mbarrier arrives).
-template <int BN, int ISSUERS, int CL>
-__global__ void __launch_bounds__(kThreadsTs + 32 * (ISSUERS - 1), 1)
-tensor_gemm_ts_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
-                      const __grid_constant__ CUtensorMap tmBlo, const __grid_constant__ CUtensorMap tmD,
-                      const GemmKernelArgs args) {
-    constexpr int STAGES = kStagesTs;
-    constexpr int kATile = kBM * kBK * 4;  // 16 KB raw A
-    constexpr int kBTile = BN * kBK * 4;
-    constexpr int kStage = kATile + 2 * kBTile;  // [A raw][B_hi][B_lo]
-    constexpr uint32_t kAccCols = 2 * BN;
-    constexpr uint32_t kAStageCols = 64;         // [A_hi 32 cols][A_lo 32 cols]
-    constexpr uint32_t kNeedCols = kAccCols + STAGES * kAStageCols;
-    constexpr uint32_t kTmemCols = kNeedCols <= 64 ? 64 : kNeedCols <= 128 ? 128 : kNeedCols <= 256 ? 256 : 512;
-    static_assert(kNeedCols <= 512, "TMEM budget");
-
-    extern __shared__ uint8_t smem_raw[];
-    uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-
-    __shared__ uint64_t full_bar[STAGES];     // TMA landed A raw + B_hi + B_lo
-    __shared__ uint64_t a_ready_bar[STAGES];  // a splitter group parked A_hi/A_lo in TMEM
-    __shared__ uint64_t empty_bar[STAGES];    // MMAs reading the stage (smem B, TMEM A) retired
-    __shared__ uint64_t peer_free_bar[STAGES];  // CL > 1: the other CTAs of the cluster have released their copy of the slot
-    __shared__ uint64_t tmem_full_bar[2];
-    __shared__ uint64_t tmem_empty_bar[2];
-    __shared__ uint32_t tmem_base_smem;
-    __shared__ volatile uint32_t issued_g;  // ISSUERS == 2: k-blocks whose MMAs have been issued
-
-    const int warp = threadIdx.x >> 5;
-    const int lane = threadIdx.x & 31;
-    static_assert(CL == 1 || ISSUERS == 1, "the cluster variant uses one issuer");
-    static_assert(CL == 1 || (BN / CL) % 8 == 0, "each CTA multicasts whole 8-row swizzle atoms of B");
-    // work items: CL == 1: one M tile per item, strided by the grid; CL > 1: CL consecutive M tiles per item (args.num_m
-    // counts those groups), strided by the number of clusters, this CTA takes M tile  group * CL + rank
-    const int tiles_per_g = args.num_m * args.num_n;
-    const int total_tiles = tiles_per_g * args.G * args.split_k;
-    const int kb_per_split = (args.k_blocks_total + args.split_k - 1) / args.split_k;
-    const int t_first = CL == 1 ? static_cast<int>(blockIdx.x) : static_cast<int>(ptx::cluster_id_x());
-    const int t_step = CL == 1 ? static_cast<int>(gridDim.x) : static_cast<int>(ptx::cluster_count_x());
-    const int cta_rank = CL == 1 ? 0 : static_cast<int>(ptx::cluster_ctarank());
-
-    if (threadIdx.x == 0) {
-        issued_g = 0;
-        for (int s = 0; s < STAGES; ++s) {
-            ptx::mbar_init(&full_bar[s], 1);
-            ptx::mbar_init(&a_ready_bar[s], 4);
-            ptx::mbar_init(&empty_bar[s], 1);
-            ptx::mbar_init(&peer_free_bar[s], CL > 1 ? CL - 1 : 1);
-        }
-        for (int s = 0; s < 2; ++s) {
-            ptx::mbar_init(&tmem_full_bar[s], 1);
-            ptx::mbar_init(&tmem_empty_bar[s], 4);
-        }
-        ptx::fence_barrier_init();
-    }
-    if (warp == 0 && lane == 0) {
-        ptx::prefetch_tensormap(&tmA);
-        ptx::prefetch_tensormap(&tmB);
-        ptx::prefetch_tensormap(&tmBlo);
-    }
-    if (warp == 1) {
-        ptx::tmem_alloc(&tmem_base_smem, kTmemCols);
-        ptx::tmem_relinquish();
-    }
-    ptx::tc_fence_before();
-    __syncthreads();
-    if (CL > 1) ptx::cluster_sync_all();  // every CTA's barriers are initialised before a peer arrives on / multicasts to them
-    ptx::tc_fence_after();
-    const uint32_t tmem_base = tmem_base_smem;
-    const uint32_t tmem_a0 = tmem_base + kAccCols;
-
-    if (warp == 0 && CL == 1) {
-        // ===================== TMA producer =====================
-        // A thread can start a TMA operation only every ~280 cycles and the slot wait -> expect_tx -> three loads of a k-block are
-        // a chain of long-latency instructions: ~700 cycles per k-block when one thread walked them, against 768 cycles of
-        // MMAs at N = 128 — the reason this kernel sat at 60-72 % tensor pipe (tests/cuda/store_rate.cu, igemm trace r02v).
-        // Now kKG k-blocks x 3 operands are issued in lockstep by 3 * kKG lanes: lane = group * 3 + operand, group j takes
-        // every kKG-th k-block of this CTA's k-block sequence; one instruction issue starts 3 * kKG loads.
-        constexpr int kKG = 2;
-        static_assert(kKG <= STAGES && STAGES % kKG == 0, "a round must not wait for its own loads; one lane group per ring slot (consecutive barrier phases)");
-        if (lane < 3 * kKG) {
-            const int grp = lane / 3, op = lane - grp * 3;
-            const CUtensorMap* map = op == 0 ? &tmA : op == 1 ? &tmB : &tmBlo;
-            const uint32_t dst_off = op == 0 ? 0u : op == 1 ? static_cast<uint32_t>(kATile) : static_cast<uint32_t>(kATile + kBTile);
-            int tile = t_first;
-            int kb_off = grp;                          // offset inside the current tile's k range
-            uint32_t gi = static_cast<uint32_t>(grp);  // running k-block index of this CTA
-            int dec_tile = -1, g = 0, row = 0, kb0 = 0, nk = 0;
-            while (tile < total_tiles) {
-                if (tile != dec_tile) {
-                    const int ks = tile / (tiles_per_g * args.G);
-                    const int rem = tile - ks * (tiles_per_g * args.G);
-                    g = rem / tiles_per_g;
-                    const int mn = rem - g * tiles_per_g;
-                    const int m_grp = mn / args.num_n;
-                    const int n_blk = mn - m_grp * args.num_n;
-                    row = op == 0 ? m_grp * kBM : n_blk * BN;   // CL == 1: m_blk == m_grp
-                    kb0 = ks * kb_per_split;
-                    nk = min(kb0 + kb_per_split, args.k_blocks_total) - kb0;
-                    dec_tile = tile;
-                }
-                if (kb_off >= nk) { kb_off -= nk; tile += t_step; continue; }
-                const int stage = static_cast<int>(gi % STAGES);
-                const uint32_t phase = (gi / STAGES) & 1u;
-                ptx::mbar_wait(&empty_bar[stage], phase ^ 1, args.suspend_ns);
-                if (op == 0) ptx::mbar_arrive_expect_tx(&full_bar[stage], kStage);  // A + B_hi + B_lo
-                ptx::tma_load_3d(smem + stage * kStage + dst_off, map, &full_bar[stage], (kb0 + kb_off) * kBK, row, g);
-                gi += kKG;
-                kb_off += kKG;
+    for (int i = 0; i < nk; ++i) {
+        const int stage = i % kStages;
+        ptx::mbar_wait(&full_bar[stage], (i / kStages) & 1);
+        const uint32_t a_base = ptx::smem_u32(smem + stage * kStage);
+        uint32_t ahi[4][4], alo[4][4];
+#pragma unroll
+        for (int kk = 0; kk < 4; ++kk) {
+#pragma unroll
+            for (int q = 0; q < 4; ++q) {  // q: a0 (row0, k), a1 (row0 + 8, k), a2 (row0, k + 4), a3 (row0 + 8, k + 4)
+                const int row = row0 + 8 * (q & 1);
+                const uint32_t chunk = static_cast<uint32_t>(2 * kk + (q >> 1)) ^ static_cast<uint32_t>(gq);
+                float x;
+                asm volatile("ld.shared.f32 %0, [%1];" : "=f"(x) : "r"(a_base + row * 128 + (chunk << 4) + c * 4));
+                if (PLANES == 2) split_tf32_trunc(x, ahi[kk][q], alo[kk][q]);
+                else ahi[kk][q] = __float_as_uint(x);
             }
         }
-    } else if (warp == 0) {
-        // ===================== TMA producer, cluster-multicast variant =====================
-        const bool leader = ptx::elect_one();
-        int stage = 0;
-        uint32_t phase = 0;
-        for (int tile = t_first; tile < total_tiles; tile += t_step) {
-            const int ks = tile / (tiles_per_g * args.G);
-            const int rem = tile - ks * (tiles_per_g * args.G);
-            const int g = rem / tiles_per_g;
-            const int mn = rem - g * tiles_per_g;
-            const int m_grp = mn / args.num_n;
-            const int n_blk = mn - m_grp * args.num_n;
-            const int m_blk = m_grp * CL + cta_rank;
-            const int kb0 = ks * kb_per_split;
-            const int kb1 = min(kb0 + kb_per_split, args.k_blocks_total);
-            for (int kb = kb0; kb < kb1; ++kb) {
-                ptx::mbar_wait(&empty_bar[stage], phase ^ 1, args.suspend_ns);
-                if (CL > 1) {
-                    // my copy of the slot is free: tell the peers, then wait until theirs are (their multicast lands in
-                    // my slot, mine in theirs)
-                    if (leader) {
+        const uint64_t dB = make_smem_desc_sw128(a_base + kATile);
+        const uint64_t dBlo = make_smem_desc_sw128(a_base + kATile + kBTile);
+        ptx::wgmma_fence();
 #pragma unroll
-                        for (int c = 0; c < CL; ++c)
-                            if (c != cta_rank) ptx::mbar_arrive_remote(&peer_free_bar[stage], static_cast<uint32_t>(c));
-                    }
-                    __syncwarp();
-                    ptx::mbar_wait_cluster(&peer_free_bar[stage], phase);
-                }
-                if (leader) {
-                    uint8_t* st = smem + stage * kStage;
-                    ptx::mbar_arrive_expect_tx(&full_bar[stage], kStage);  // own A + all CL pieces of B_hi and B_lo
-                    ptx::tma_load_3d(st, &tmA, &full_bar[stage], kb * kBK, m_blk * kBM, g);
-                    if (CL == 1) {
-                        ptx::tma_load_3d(st + kATile, &tmB, &full_bar[stage], kb * kBK, n_blk * BN, g);
-                        ptx::tma_load_3d(st + kATile + kBTile, &tmBlo, &full_bar[stage], kb * kBK, n_blk * BN, g);
-                    } else {
-                        constexpr int kRows = BN / CL;          // B rows this CTA fetches for the whole cluster
-                        constexpr int kPiece = kRows * kBK * 4;
-                        constexpr uint16_t kMask = static_cast<uint16_t>((1u << CL) - 1u);
-                        ptx::tma_load_3d_multicast(st + kATile + cta_rank * kPiece, &tmB, &full_bar[stage], kb * kBK,
-                                                   n_blk * BN + cta_rank * kRows, g, kMask);
-                        ptx::tma_load_3d_multicast(st + kATile + kBTile + cta_rank * kPiece, &tmBlo, &full_bar[stage],
-                                                   kb * kBK, n_blk * BN + cta_rank * kRows, g, kMask);
-                    }
-                }
-                __syncwarp();
-                if (++stage == STAGES) { stage = 0; phase ^= 1; }
-            }
-        }
-    } else if (ISSUERS == 2 && (warp == 1 || warp == kWarpIssuer2)) {
-        // ===================== two MMA issuers alternating k-blocks (see conv_igemm.cu) =====================
-        if (ptx::elect_one()) {
-            constexpr uint32_t idesc = make_idesc_tf32(BN);
-            const uint32_t me = warp == 1 ? 0u : 1u;
-            const uint64_t dB0 = make_smem_desc_sw128(ptx::smem_u32(smem) + kATile);
-            uint32_t g = 0;  // running k-block index over this CTA's tiles
-            int it = 0;
-            for (int tile = t_first; tile < total_tiles; tile += t_step, ++it) {
-                const int ks = tile / (tiles_per_g * args.G);
-                const int kb0 = ks * kb_per_split;
-                const int kb1 = min(kb0 + kb_per_split, args.k_blocks_total);
-                const int as = it & 1;
-                const uint32_t aphase = (it >> 1) & 1;
-                const uint32_t tmem_d = tmem_base + as * BN;
-                const uint32_t g_end = g + static_cast<uint32_t>(kb1 - kb0);
-                for (uint32_t gg = g + ((g ^ me) & 1u); gg < g_end; gg += 2) {
-                    const int stage = static_cast<int>(gg & (STAGES - 1));
-                    const uint32_t phase = (gg / STAGES) & 1u;
-                    const uint64_t dB = dB0 + static_cast<uint64_t>(stage * (kStage >> 4));
-                    const uint64_t dBlo = dB + static_cast<uint64_t>(kBTile >> 4);
-                    const uint32_t ta = tmem_a0 + stage * kAStageCols;
-                    if (gg == g) ptx::mbar_wait(&tmem_empty_bar[as], aphase ^ 1);
-                    ptx::mbar_wait(&a_ready_bar[stage], phase);  // implies full_bar: the splitters waited on it
-                    while (issued_g < gg) {}                      // the other issuer has put k-block gg-1 into the pipe
-                    ptx::tc_fence_after();
-#pragma unroll
-                    for (int k = 0; k < kBK / 8; ++k) {
-                        const uint32_t first = (gg == g && k == 0) ? 0u : 1u;
-                        umma_tf32_ts(tmem_d, ta + 32 + k * 8, dB + 2 * k, idesc, first);   // A_lo * B_hi
-                        umma_tf32_ts(tmem_d, ta + k * 8, dBlo + 2 * k, idesc, 1u);         // A_hi * B_lo
-                        umma_tf32_ts(tmem_d, ta + k * 8, dB + 2 * k, idesc, 1u);           // A_hi * B_hi
-                    }
-                    issued_g = gg + 1;
-                    ptx::umma_commit(&empty_bar[stage]);
-                    if (gg + 1 == g_end) ptx::umma_commit(&tmem_full_bar[as]);
-                }
-                g = g_end;
-            }
-        }
-    } else if (ISSUERS == 1 && warp == 1) {
-        // ===================== MMA issuer =====================
-        constexpr uint32_t idesc = make_idesc_tf32(BN);
-        const bool leader = ptx::elect_one();
-        const uint64_t dB0 = make_smem_desc_sw128(ptx::smem_u32(smem) + kATile);
-        int stage = 0;
-        uint32_t phase = 0;
-        int it = 0;
-        bool ready = false;  // a_ready_bar[stage] already observed complete for `phase`
-        for (int tile = t_first; tile < total_tiles; tile += t_step, ++it) {
-            const int ks = tile / (tiles_per_g * args.G);
-            const int kb0 = ks * kb_per_split;
-            const int kb1 = min(kb0 + kb_per_split, args.k_blocks_total);
-            const int as = it & 1;
-            const uint32_t aphase = (it >> 1) & 1;
-            ptx::mbar_wait(&tmem_empty_bar[as], aphase ^ 1, args.suspend_ns);
-            ptx::tc_fence_after();
-            const uint32_t tmem_d = tmem_base + as * BN;
-            for (int kb = kb0; kb < kb1; ++kb) {
-                // a_ready implies full_bar (the splitters waited on it).  The tensor pipe's queue is shallow, so the
-                // NEXT slot's barrier is probed between this slot's MMAs; the blocking wait is the fallback.
-                if (!ready) ptx::mbar_wait(&a_ready_bar[stage], phase, args.suspend_ns);
-                ptx::tc_fence_after();
-                const int nstage = stage + 1 == STAGES ? 0 : stage + 1;
-                const uint32_t nphase = nstage == 0 ? phase ^ 1u : phase;
-                const uint64_t dB = dB0 + static_cast<uint64_t>(stage * (kStage >> 4));
-                const uint64_t dBlo = dB + static_cast<uint64_t>(kBTile >> 4);
-                const uint32_t ta = tmem_a0 + stage * kAStageCols;
-#pragma unroll
-                for (int k = 0; k < kBK / 8; ++k) {
-                    const uint32_t first = (kb == kb0 && k == 0) ? 0u : 1u;
-                    if (leader) {
-                        umma_tf32_ts(tmem_d, ta + 32 + k * 8, dB + 2 * k, idesc, first);   // A_lo * B_hi
-                        umma_tf32_ts(tmem_d, ta + k * 8, dBlo + 2 * k, idesc, 1u);         // A_hi * B_lo
-                        umma_tf32_ts(tmem_d, ta + k * 8, dB + 2 * k, idesc, 1u);           // A_hi * B_hi
-                    }
-                    if (k == 1) ready = ptx::mbar_test(&a_ready_bar[nstage], nphase);
-                }
-                if (leader) ptx::umma_commit(&empty_bar[stage]);
-                __syncwarp();
-                stage = nstage;
-                phase = nphase;
-            }
-            if (leader) ptx::umma_commit(&tmem_full_bar[as]);
-            __syncwarp();
-        }
-    } else if (warp >= 6 && warp < kWarpIssuer2) {
-        // ===================== splitters: smem raw A row -> TF32 hi / fp32 lo -> tensor memory =====================
-        const int group = (warp - 6) >> 2;
-        const int q = warp & 3;  // TMEM lane quadrant == 32-row slice of the tile
-        const int row = q * 32 + lane;
-        const uint32_t lane_base = static_cast<uint32_t>(q * 32) << 16;
-        const uint32_t row_off = static_cast<uint32_t>(row) * 128;
-        const uint32_t sw = static_cast<uint32_t>(row & 7);  // 128B swizzle: 16-byte chunk c lives at c ^ (row & 7)
-        int stage = 0, g_par = 0;
-        uint32_t phase = 0;
-        for (int tile = t_first; tile < total_tiles; tile += t_step) {
-            const int ks = tile / (tiles_per_g * args.G);
-            const int kb0 = ks * kb_per_split;
-            const int kb1 = min(kb0 + kb_per_split, args.k_blocks_total);
-            for (int kb = kb0; kb < kb1; ++kb) {
-                const bool mine = g_par == group;
-                const int my_stage = stage;
-                const uint32_t my_phase = phase;
-                g_par ^= 1;
-                if (++stage == STAGES) { stage = 0; phase ^= 1; }
-                if (!mine) continue;
-                ptx::mbar_wait(&full_bar[my_stage], my_phase, args.suspend_ns);
-                const uint32_t a = ptx::smem_u32(smem + my_stage * kStage) + row_off;
-                const uint32_t ta = tmem_a0 + lane_base + my_stage * kAStageCols;
-#pragma unroll
-                for (int half = 0; half < 2; ++half) {
-                    uint32_t hi[16], lo[16];
-#pragma unroll
-                    for (int c = 0; c < 4; ++c) {
-                        const uint32_t chunk = static_cast<uint32_t>(half * 4 + c) ^ sw;
-                        float x[4];  // explicit ld.shared: through the generic pointer nvcc emitted LD.E.128 (generic address path)
-                        asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(x[0]), "=f"(x[1]), "=f"(x[2]), "=f"(x[3]) : "r"(a + (chunk << 4)));
-#pragma unroll
-                        for (int j = 0; j < 4; ++j) {
-                            hi[c * 4 + j] = __float_as_uint(x[j]) & 0xFFFFE000u;   // what the tensor core would read
-                            lo[c * 4 + j] = __float_as_uint(x[j] - __uint_as_float(hi[c * 4 + j]));  // exact remainder
-                        }
-                    }
-                    tmem_st_32x16(ta + half * 16, hi);
-                    tmem_st_32x16(ta + 32 + half * 16, lo);
-                }
-                asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory");
-                ptx::tc_fence_before();
-                __syncwarp();
-                if (lane == 0) ptx::mbar_arrive(&a_ready_bar[my_stage]);
-            }
-        }
-    } else if (warp >= 2 && warp < 6) {
-        // ===================== epilogue (warps 2..5) =====================
-        const int q = warp & 3;
-        int it = 0;
-        uint32_t ebuf = 0;                                     // staging tile toggle of the TMA-store epilogue
-        uint8_t* stage_out = smem + STAGES * kStage;           // 4 warps x 2 tiles x 4 KB, 1024-byte aligned
-        for (int tile = t_first; tile < total_tiles; tile += t_step, ++it) {
-            const int ks = tile / (tiles_per_g * args.G);
-            const int rem = tile - ks * (tiles_per_g * args.G);
-            const int g = rem / tiles_per_g;
-            const int mn = rem - g * tiles_per_g;
-            const int m_grp = mn / args.num_n;
-            const int n_blk = mn - m_grp * args.num_n;
-            const int m_blk = m_grp * CL + cta_rank;
-            const int as = it & 1;
-            const uint32_t aphase = (it >> 1) & 1;
-            ptx::mbar_wait_relaxed(&tmem_full_bar[as], aphase);
-            ptx::tc_fence_after();
-            if (args.tma_store) {
-                // Row-major D[g][m][n] (the Winograd product buffer): a thread holds ONE row of the accumulator, so direct
-                // float4 stores put every lane in a different 128-byte line — 32 sectors per instruction, ~7.4k cycles per
-                // 128 x 128 tile, more than the tile's MMAs at K <= 256 (ncu round 1: tensor pipe 41 % at K = 128, 60 % at
-                // K = 256 = MMA time / this epilogue).  Instead: 32 x 32 chunks go through a 128B-swizzled shared-memory
-                // tile (STS.128, conflict-free per quarter warp) and leave by TMA, which writes whole rows and clips the
-                // M / N tails.  Two staging tiles per warp: the store of chunk i reads while chunk i+1 is being staged.
-                const uint32_t taddr0 = tmem_base + (static_cast<uint32_t>(q * 32) << 16) + as * BN;
-#pragma unroll 1
-                for (int c0 = 0; c0 < BN; c0 += 32) {
-                    const int n0 = n_blk * BN + c0;
-                    if (n0 >= args.N) break;  // warp-uniform
-                    uint32_t r[32];
-                    ptx::tmem_ld_32x32(taddr0 + c0, r);
-                    uint8_t* stg = stage_out + (q * 2 + (ebuf & 1)) * 4096;
-                    if (lane == 0) ptx::tma_store_wait_read<1>();  // the store issued two chunks ago has read this tile
-                    __syncwarp();
-                    ptx::tmem_ld_wait();
-                    const uint32_t rowp = ptx::smem_u32(stg) + static_cast<uint32_t>(lane * 128);
-#pragma unroll
-                    for (int j = 0; j < 8; ++j)
-                        asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(rowp + ((j ^ (lane & 7)) << 4)), "r"(r[4 * j]), "r"(r[4 * j + 1]),
-                                     "r"(r[4 * j + 2]), "r"(r[4 * j + 3]) : "memory");
-                    ptx::fence_proxy_async_smem();
-                    __syncwarp();
-                    if (lane == 0) {
-                        ptx::tma_store_3d(&tmD, stg, n0, m_blk * kBM + q * 32, g);
-                        ptx::tma_store_commit();
-                    }
-                    ++ebuf;
-                }
+        for (int kk = 0; kk < 4; ++kk) {
+            if (PLANES == 2) {
+                Wgmma<BN, 1>::mma(acc, alo[kk], dB + 2 * kk, 1u);    // A_lo * B_hi
+                Wgmma<BN, 1>::mma(acc, ahi[kk], dBlo + 2 * kk, 1u);  // A_hi * B_lo
+                Wgmma<BN, 1>::mma(acc, ahi[kk], dB + 2 * kk, 1u);    // A_hi * B_hi
             } else {
-                epilogue_store<BN>(args, tmem_base, as, q, lane, g, m_blk, n_blk, ks);
+                Wgmma<BN, 1>::mma(acc, ahi[kk], dB + 2 * kk, 1u);
             }
-            ptx::tc_fence_before();
-            __syncwarp();
-            if (lane == 0) ptx::mbar_arrive(&tmem_empty_bar[as]);
         }
-        if (args.tma_store && lane == 0) ptx::tma_store_wait_all<0>();  // global writes done before the CTA retires
+        ptx::wgmma_commit();
+        ptx::wgmma_wait<0>();
+        __syncwarp();
+        if (lane == 0) ptx::mbar_arrive(&empty_bar[stage]);
     }
-
-    ptx::tc_fence_before();
-    __syncthreads();
-    if (CL > 1) ptx::cluster_sync_all();  // no CTA may exit while a peer can still arrive on / multicast into its smem
-    if (warp == 1) {
-        ptx::tc_fence_after();
-        ptx::tmem_dealloc(tmem_base, kTmemCols);
-    }
+    epilogue_store<BN>(args, acc, g, m_blk * kBM + row0, n_blk * BN, c, ks);
 }
 
 // --------------------------------------------------------------------------------------------
@@ -712,17 +226,8 @@ void reset_launch_count() { g_launches.store(0, std::memory_order_relaxed); }
 namespace {
 struct TuneEntry { const char* name; const char* env; int def, lo, hi; int value; bool init; };
 TuneEntry g_tune[TUNE_COUNT] = {
-    {"igemm_issuers", "FCUDA_IGEMM_ISSUERS", 2, 1, 2, 0, false},     // MMA issuer threads of the implicit GEMM (BN <= 64)
-    {"igemm_slab", "FCUDA_IGEMM_SLAB", 1, 0, 1, 0, false},           // TMA-fed slab producer for 3x3 / stride-1 layers
-    {"igemm_cta_group", "FCUDA_IGEMM_CG", 1, 1, 2, 0, false},        // 2 = CTA pairs (cta_group::2, M = 256): correct, measured slower
     {"dw_vec", "FCUDA_DW_VEC", 1, 0, 1, 0, false},                   // vectorised depthwise kernel on wide planes
-    {"gemm_cluster", "FCUDA_GEMM_CLUSTER", 1, 1, 4, 0, false},       // TMA-multicast of B across a cluster: measured slower
-    {"gemm_tma_store", "FCUDA_GEMM_TMA_STORE", 1, 0, 2, 0, false},   // row-major epilogue through smem + TMA stores
-    {"igemm_tma_out", "FCUDA_IGEMM_TMA_OUT", 1, 0, 1, 0, false},     // implicit-GEMM epilogue through smem + TMA stores
-    {"igemm_pw", "FCUDA_IGEMM_PW", 1, 0, 1, 0, false},               // TMA-fed slab producer for 1x1 / stride-1 layers
-    {"wino_mlp", "FCUDA_WINO_MLP", 2, 0, 2, 0, false},
-    {"mbar_suspend_ns", "FCUDA_MBAR_SUSPEND_NS", 100000, 0, 1000000, 0, false},  // suspend hint of the implicit GEMM's hand-off waits (0 = poll)
-    {"igemm_tma_lanes", "FCUDA_IGEMM_TMA_LANES", 4, 1, 4, 0, false},  // lanes of the implicit GEMM's filter-TMA warp issuing in lockstep (1, 2, 4)               // Winograd transforms: asynchronous slab copies / all plane loads in flight
+    {"wino_mlp", "FCUDA_WINO_MLP", 2, 0, 2, 0, false},               // Winograd transforms: slab copies / all plane loads in flight
 };
 }  // namespace
 const char* tune_name(int key) { return key >= 0 && key < TUNE_COUNT ? g_tune[key].name : nullptr; }
@@ -743,7 +248,7 @@ int tune_set(const char* name, int value) {
     if (!name) return -200;
     for (int k = 0; k < TUNE_COUNT; ++k)
         if (!strcmp(name, g_tune[k].name)) {
-            if (value < g_tune[k].lo || value > g_tune[k].hi || (k == TUNE_GEMM_CLUSTER && value == 3)) return -200;
+            if (value < g_tune[k].lo || value > g_tune[k].hi || false) return -200;
             g_tune[k].value = value;
             g_tune[k].init = true;
             return 0;
@@ -813,7 +318,7 @@ int sm_count() {
     const int dev = current_device();
     if (n[dev] == 0) {
         int v = 0;
-        if (cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || v <= 0) return 148;
+        if (cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || v <= 0) return 132;
         n[dev] = v;
     }
     return n[dev];
@@ -843,25 +348,6 @@ static int make_map(CUtensorMap* map, const float* base, int K, int rows, int G,
     return 0;
 }
 
-// 3D map over [G][rows][cols] fp32 with explicit row / batch strides (floats) and a (box_cols x box_rows x 1) box, 128B swizzle.
-static int make_map_2(CUtensorMap* map, const float* base, int cols, int rows, int G, long long row_stride,
-                      long long batch_stride, int box_cols, int box_rows) {
-    EncodeTiledFn enc = get_encode_fn();
-    if (!enc) return FCUDA_ERR_CUDA;
-    cuuint64_t dims[3] = {static_cast<cuuint64_t>(cols), static_cast<cuuint64_t>(rows), static_cast<cuuint64_t>(G)};
-    cuuint64_t strides[2] = {static_cast<cuuint64_t>(row_stride) * 4, static_cast<cuuint64_t>(batch_stride) * 4};
-    cuuint32_t box[3] = {static_cast<cuuint32_t>(box_cols), static_cast<cuuint32_t>(box_rows), 1};
-    cuuint32_t estr[3] = {1, 1, 1};
-    CUresult r = enc(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, const_cast<float*>(base), dims, strides, box, estr,
-                     CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                     CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (r != CUDA_SUCCESS) {
-        fprintf(stderr, "fcuda: cuTensorMapEncodeTiled (D) failed (%d) cols=%d rows=%d G=%d\n", static_cast<int>(r), cols, rows, G);
-        return FCUDA_ERR_CUDA;
-    }
-    return 0;
-}
-
 bool tensor_gemm_supported(const GemmProblem& p) {
     if (p.M <= 0 || p.N <= 0 || p.K <= 0 || p.G <= 0) return false;
     if (p.K % 4 != 0) return false;
@@ -870,50 +356,6 @@ bool tensor_gemm_supported(const GemmProblem& p) {
     if (p.planes == 2 && (!p.B_lo || !aligned(p.B_lo))) return false;
     if (p.a_batch_stride % 4 != 0 || p.b_batch_stride % 4 != 0) return false;
     return true;
-}
-
-template <int BN, int PLANES, int STAGES>
-static int launch(const GemmProblem& p, cudaStream_t stream) {
-    using L = SmemLayout<BN, PLANES>;
-    static_assert(STAGES * L::kStage + 1024 <= 227 * 1024, "smem budget");
-    CUtensorMap tmA, tmAlo, tmB, tmBlo;
-    const long long as = p.a_batch_stride ? p.a_batch_stride : static_cast<long long>(p.M) * p.K;
-    const long long bs = p.b_batch_stride ? p.b_batch_stride : static_cast<long long>(p.N) * p.K;
-    int rc;
-    if ((rc = make_map(&tmA, p.A, p.K, p.M, p.G, as, kBM))) return rc;
-    if ((rc = make_map(&tmB, p.B_hi, p.K, p.N, p.G, bs, BN))) return rc;
-    if (PLANES == 2) {
-        tmAlo = tmA;
-        if ((rc = make_map(&tmBlo, p.B_lo, p.K, p.N, p.G, bs, BN))) return rc;
-    } else {
-        tmAlo = tmA;
-        tmBlo = tmB;
-    }
-    GemmKernelArgs a;
-    a.D = p.D; a.bias = p.bias;
-    a.M = p.M; a.N = p.N; a.K = p.K; a.G = p.G;
-    a.epilogue = p.epilogue; a.ldd = p.ldd; a.P = p.P > 0 ? p.P : 1; a.relu = p.relu;
-    a.m_offset = p.m_offset;
-    a.split_stride = p.split_stride;
-    a.num_m = ceil_div(p.M, kBM);
-    a.num_n = ceil_div(p.N, BN);
-    a.k_blocks_total = ceil_div(p.K, kBK);
-    a.split_k = tensor_gemm_effective_split(p.K, p.split_k);
-    const long long total = static_cast<long long>(a.num_m) * a.num_n * a.G * a.split_k;
-    if (total > 0x7fffffffLL) return -1;
-    const int grid = static_cast<int>(total < sm_count() ? total : sm_count());
-    const int smem = STAGES * L::kStage + 1024;
-    auto kern = tensor_gemm_kernel<BN, PLANES, STAGES>;
-    static SmemAttrCache attr_cache;
-    if (int rc = ensure_dynamic_smem(kern, smem, attr_cache)) return rc;
-    const double dense = 2.0 * p.M * static_cast<double>(p.N) * p.K * p.G;
-    const int prof = prof_begin(stream, PROF_TENSOR_GEMM, p.algo_flops > 0 ? p.algo_flops : dense,
-                                dense * (PLANES == 2 ? 3.0 : 1.0), gemm_algo_bytes(p));
-    kern<<<grid, kThreads, smem, stream>>>(tmA, tmAlo, tmB, tmBlo, a);
-    FCUDA_CHECK_LAUNCH();
-    count_launch();
-    prof_end(prof, stream);
-    return 0;
 }
 
 static void fill_kernel_args(const GemmProblem& p, int bn, GemmKernelArgs* a) {
@@ -926,6 +368,7 @@ static void fill_kernel_args(const GemmProblem& p, int bn, GemmKernelArgs* a) {
     a->num_n = ceil_div(p.N, bn);
     a->k_blocks_total = ceil_div(p.K, kBK);
     a->split_k = tensor_gemm_effective_split(p.K, p.split_k);
+    a->vec2 = (p.ldd % 2 == 0 && (reinterpret_cast<uintptr_t>(p.D) & 7) == 0) ? 1 : 0;
 }
 
 int tensor_gemm_effective_split(int K, int split_k) {
@@ -937,122 +380,48 @@ int tensor_gemm_effective_split(int K, int split_k) {
     return s;
 }
 
-static int ts_issuers() {  // FCUDA_TS_ISSUERS=1|2 (experiment switch)
-    static int v = 0;
-    if (v == 0) {
-        const char* e = getenv("FCUDA_TS_ISSUERS");
-        v = (e && e[0] == '2') ? 2 : (e && e[0] == '1') ? 1 : kDefaultTsIssuers;
-    }
-    return v;
-}
-
-static int gemm_cluster_env() { return tune_get(TUNE_GEMM_CLUSTER); }  // 1 | 2 | 4
-
-template <int BN, int ISSUERS, int CL>
-static int launch_ts(const GemmProblem& p, cudaStream_t stream) {
+template <int BN, int PLANES>
+static int launch(const GemmProblem& p, cudaStream_t stream) {
+    constexpr int kStage = kBM * kBK * 4 + PLANES * BN * kBK * 4;
+    static_assert(kStages * kStage + 1024 <= 227 * 1024, "smem budget");
     CUtensorMap tmA, tmB, tmBlo;
     const long long as = p.a_batch_stride ? p.a_batch_stride : static_cast<long long>(p.M) * p.K;
     const long long bs = p.b_batch_stride ? p.b_batch_stride : static_cast<long long>(p.N) * p.K;
     int rc;
     if ((rc = make_map(&tmA, p.A, p.K, p.M, p.G, as, kBM))) return rc;
-    if ((rc = make_map(&tmB, p.B_hi, p.K, p.N, p.G, bs, BN / CL))) return rc;   // CL > 1: each CTA fetches BN / CL rows
-    if ((rc = make_map(&tmBlo, p.B_lo, p.K, p.N, p.G, bs, BN / CL))) return rc;
+    if ((rc = make_map(&tmB, p.B_hi, p.K, p.N, p.G, bs, BN))) return rc;
+    tmBlo = tmB;
+    if (PLANES == 2 && (rc = make_map(&tmBlo, p.B_lo, p.K, p.N, p.G, bs, BN))) return rc;
     GemmKernelArgs a;
     fill_kernel_args(p, BN, &a);
-    if (CL > 1) a.num_m = ceil_div(a.num_m, CL);  // work items = groups of CL consecutive M tiles
-    // row-major D leaves through shared memory + TMA (see the epilogue); needs 16-byte rows
-    const bool tma_store_off = tune_get(TUNE_GEMM_TMA_STORE) != 1;
-    a.st256 = tune_get(TUNE_GEMM_TMA_STORE) == 2 && (reinterpret_cast<uintptr_t>(p.D) & 31) == 0 ? 1 : 0;
-    CUtensorMap tmD = tmA;
-    a.tma_store = 0;
-    a.suspend_ns = static_cast<unsigned>(tune_get(TUNE_MBAR_SUSPEND_NS));
-    if (p.epilogue == EPI_ROWMAJOR && !tma_store_off && p.ldd % 4 == 0 && (reinterpret_cast<uintptr_t>(p.D) & 15) == 0) {
-        if ((rc = make_map_2(&tmD, p.D, p.N, p.M, p.G, p.ldd, static_cast<long long>(p.M) * p.ldd, 32, 32))) return rc;
-        a.tma_store = 1;
-    }
     const long long total = static_cast<long long>(a.num_m) * a.num_n * a.G * a.split_k;
     if (total > 0x7fffffffLL) return -1;
-    constexpr int kStage = kBM * kBK * 4 + 2 * BN * kBK * 4;
-    static_assert(kStagesTs * kStage + 1024 <= 227 * 1024, "smem budget");
-    constexpr int kStageOut = 4 * 2 * 4096;  // epilogue staging tiles
-    static_assert(kStagesTs * kStage + kStageOut + 1024 <= 227 * 1024, "smem budget");
-    const int smem = kStagesTs * kStage + kStageOut + 1024;
-    auto kern = tensor_gemm_ts_kernel<BN, ISSUERS, CL>;
+    const int smem = kStages * kStage + 1024;
+    auto kern = tensor_gemm_kernel<BN, PLANES>;
     static SmemAttrCache attr_cache;
     if (int rc2 = ensure_dynamic_smem(kern, smem, attr_cache)) return rc2;
     const double dense = 2.0 * p.M * static_cast<double>(p.N) * p.K * p.G;
-    const int threads = kThreadsTs + 32 * (ISSUERS - 1);
-    if (CL == 1) {
-        const int grid = static_cast<int>(total < sm_count() ? total : sm_count());
-        const int prof = prof_begin(stream, PROF_TENSOR_GEMM, p.algo_flops > 0 ? p.algo_flops : dense, dense * 3.0,
-                                    gemm_algo_bytes(p));
-        kern<<<grid, threads, smem, stream>>>(tmA, tmB, tmBlo, tmD, a);
-        FCUDA_CHECK_LAUNCH();
-        count_launch();
-        prof_end(prof, stream);
-        return 0;
-    }
-    // cluster launch: as many clusters as can be co-resident (1 CTA per SM), never more than there are work items
-    cudaLaunchConfig_t cfg = {};
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeClusterDimension;
-    attr[0].val.clusterDim.x = CL; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
-    cfg.blockDim = dim3(threads); cfg.dynamicSmemBytes = smem; cfg.stream = stream; cfg.attrs = attr; cfg.numAttrs = 1;
-    static int max_clusters[kMaxDevices] = {};
-    const int dev = current_device();
-    if (max_clusters[dev] == 0) {
-        cfg.gridDim = dim3(static_cast<unsigned>(sm_count() / CL * CL));
-        int n = 0;
-        if (cudaOccupancyMaxActiveClusters(&n, kern, &cfg) != cudaSuccess || n <= 0) {
-            cudaGetLastError();
-            n = sm_count() / CL;
-        }
-        max_clusters[dev] = n;
-    }
-    const long long nclusters = total < max_clusters[dev] ? total : max_clusters[dev];
-    cfg.gridDim = dim3(static_cast<unsigned>(nclusters * CL));
-    const int prof = prof_begin(stream, PROF_TENSOR_GEMM, p.algo_flops > 0 ? p.algo_flops : dense, dense * 3.0,
-                                gemm_algo_bytes(p));
-    FCUDA_CHECK(cudaLaunchKernelEx(&cfg, kern, tmA, tmB, tmBlo, tmD, a));
+    const int prof = prof_begin(stream, PROF_TENSOR_GEMM, p.algo_flops > 0 ? p.algo_flops : dense,
+                                dense * (PLANES == 2 ? 3.0 : 1.0), gemm_algo_bytes(p));
+    kern<<<static_cast<unsigned>(total), kThreads, smem, stream>>>(tmA, tmB, tmBlo, a);
+    FCUDA_CHECK_LAUNCH();
     count_launch();
     prof_end(prof, stream);
     return 0;
 }
 
-// CTAs per cluster for a 3xTF32 problem: B sharing pays when several M tiles exist per (g, n-block); an odd M-tile count
-// costs one idle-rows tile per group, so small M keeps the plain kernel.
-static int pick_cluster(const GemmProblem& p) {
-    if (p.split_k > 1 || p.epilogue == EPI_COLMAJOR_PARTIAL) return 1;
-    const int e = gemm_cluster_env();
-    const int num_m = ceil_div(p.M, kBM);
-    if (e) return num_m >= e ? e : 1;
-    // Measured on B200 (profiles/r02e_lean.log, VGG-16 b64): 6.77 ms per step without clusters, 7.61 with pairs, 9.38 with
-    // quads — the per-k-block cross-CTA handshake costs more than the halved B traffic saves, because L2 was not the
-    // limiter (the epilogue was).  The multicast variant stays behind FCUDA_GEMM_CLUSTER for experiments.
-    return 1;
-}
-
 int tensor_gemm(const GemmProblem& p, cudaStream_t stream) {
     if (!tensor_gemm_supported(p)) return -1;
     if (p.split_k > 1 && p.epilogue != EPI_COLMAJOR_PARTIAL) return -1;
+    // N tile: the smallest supported tile that covers N (fewer wasted MMA columns), capped at 128
     if (p.planes == 2) {
-        if (ts_issuers() == 2) {
-            if (p.N <= 32) return launch_ts<32, 2, 1>(p, stream);
-            if (p.N <= 64) return launch_ts<64, 2, 1>(p, stream);
-            return launch_ts<128, 2, 1>(p, stream);
-        }
-        const int cl = pick_cluster(p);
-        if (p.N <= 32) return launch_ts<32, 1, 1>(p, stream);
-        if (p.N <= 64) return cl == 4 ? launch_ts<64, 1, 4>(p, stream) : cl == 2 ? launch_ts<64, 1, 2>(p, stream)
-                                                                                  : launch_ts<64, 1, 1>(p, stream);
-        return cl == 4 ? launch_ts<128, 1, 4>(p, stream) : cl == 2 ? launch_ts<128, 1, 2>(p, stream)
-                                                                    : launch_ts<128, 1, 1>(p, stream);
+        if (p.N <= 32) return launch<32, 2>(p, stream);
+        if (p.N <= 64) return launch<64, 2>(p, stream);
+        return launch<128, 2>(p, stream);
     }
-    // N tile: smallest supported tile that covers N (fewer wasted MMA columns), capped at 256.
-    if (p.N <= 32) return launch<32, 1, 8>(p, stream);
-    if (p.N <= 64) return launch<64, 1, 8>(p, stream);
-    if (p.N <= 128) return launch<128, 1, 6>(p, stream);
-    return launch<256, 1, 4>(p, stream);
+    if (p.N <= 32) return launch<32, 1>(p, stream);
+    if (p.N <= 64) return launch<64, 1>(p, stream);
+    return launch<128, 1>(p, stream);
 }
 
 // --------------------------------------------------------------------------------------------

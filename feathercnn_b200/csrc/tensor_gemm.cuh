@@ -1,19 +1,17 @@
-// TensorGEMM on tcgen05 — the B200 replacement for the reference's 64-way batched
-// "TensorGEMM" (/root/reference/src/booster/avx/winograd_kernels_F63.cpp:518-757) and for its
-// packed SGEMM (/root/reference/src/booster/avx/sgemm.cpp:377-433).
+// TensorGEMM on Hopper warpgroup MMA — the replacement for the reference's 64-way batched "TensorGEMM"
+// (avx/winograd_kernels_F63.cpp) and for its packed SGEMM (avx/sgemm.cpp).
 //
 //   for g in [0,G):   D_g[M x N] = A_g[M x K] * B_g[N x K]^T        (fp32 in, fp32 out)
 //
-// Both operands are K-major ("TN").  The contraction runs on the 5th-gen tensor cores as kind::tf32 UMMA with
-// fp32 accumulation in TMEM.  fp32 semantics are recovered with the 3xTF32 split (x = hi + lo exactly, hi
-// TF32-representable): each k-step issues  A_lo*B_hi + A_hi*B_lo + A_hi*B_hi.
+// Both operands are K-major ("TN").  The contraction runs on the tensor cores as tf32 wgmma with fp32 accumulation in
+// registers.  fp32 semantics are recovered with the 3xTF32 split (x = hi + lo exactly, hi TF32-representable): each
+// k-step issues  A_lo*B_hi + A_hi*B_lo + A_hi*B_hi.
 //   B (the small, reused operand: transformed filters / packed weights / FC activations) carries its hi and lo
 //     planes in global memory (made once by the producer kernel);
 //   A (the big streamed operand: Winograd V, im2col rows, FC weights) is stored ONCE as plain fp32: the kernel
-//     lands the raw tile in shared memory by TMA, four splitter warps turn each row into hi/lo and park it in
-//     TENSOR MEMORY (tcgen05.st), and the MMAs read A from TMEM ("TS" form).  That halves A's HBM traffic and takes
-//     the A reads off the shared-memory port.
-// planes == 1 runs plain TF32 (one MMA per k-step, operands straight from shared memory).
+//     lands the raw tile in shared memory by TMA and every consumer thread splits its own register fragment into
+//     hi / lo, so A is one plane in HBM.
+// planes == 1 runs plain TF32 (one MMA per k-step).
 #pragma once
 
 #include <cuda.h>
@@ -54,7 +52,7 @@ struct GemmProblem {
     double algo_flops;         // algorithmic FLOPs this launch stands for (profiling only; 0 => 2*M*N*K*G)
 };
 
-// Launches the persistent tcgen05 kernel on `stream`.  Returns 0 or a negative fcuda error.
+// Launches the wgmma kernel on `stream`.  Returns 0 or a negative fcuda error.
 // Requirements: K % 4 == 0, 16-byte aligned operand pointers.  M/N/K tails are zero-filled by TMA.
 int tensor_gemm(const GemmProblem& p, cudaStream_t stream);
 

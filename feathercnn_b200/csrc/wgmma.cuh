@@ -1,0 +1,256 @@
+// Inline-PTX wrappers for the Hopper (sm_90a) tensor-core path: mbarrier, TMA (cp.async.bulk[.tensor]), warpgroup MMA
+// (wgmma.mma_async with the A operand in registers, B in shared memory) and its shared-memory descriptors.
+// Shared by tensor_gemm.cu (K-major TensorGEMM) and conv_igemm.cu (implicit-GEMM convolution).
+#pragma once
+
+#include <cuda.h>
+#include <cuda_runtime.h>
+#include <stdint.h>
+#include <stdio.h>
+
+namespace fcuda {
+
+// --------------------------------------------------------------------------------------------
+// PTX wrappers
+// --------------------------------------------------------------------------------------------
+namespace ptx {
+
+__device__ __forceinline__ uint32_t smem_u32(const void* p) {
+    return static_cast<uint32_t>(__cvta_generic_to_shared(p));
+}
+
+__device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
+    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count) : "memory");
+}
+__device__ __forceinline__ void fence_barrier_init() {
+    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+}
+__device__ __forceinline__ void mbar_arrive_expect_tx(uint64_t* bar, uint32_t bytes) {
+    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes)
+                 : "memory");
+}
+__device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
+    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
+}
+__device__ __forceinline__ bool mbar_try_wait(uint64_t* bar, uint32_t parity) {
+    uint32_t ok;
+    asm volatile(
+        "{\n\t"
+        ".reg .pred p;\n\t"
+        "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
+        "selp.u32 %0, 1, 0, p;\n\t"
+        "}"
+        : "=r"(ok)
+        : "r"(smem_u32(bar)), "r"(parity)
+        : "memory");
+    return ok != 0;
+}
+// Bounded wait: a protocol bug must fail the launch (trap) instead of hanging the GPU.  The clock is read every 64th
+// failed poll only.
+static __device__ __noinline__ void mbar_timeout_trap() {
+    printf("fcuda: mbarrier wait timed out (block %d thread %d)\n", blockIdx.x, threadIdx.x);
+    __trap();
+}
+__device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
+    if (mbar_try_wait(bar, parity)) return;
+    long long t0 = 0;
+    for (uint32_t spins = 1; !mbar_try_wait(bar, parity); ++spins) {
+        if ((spins & 63u) == 0) {
+            const long long now = clock64();
+            if (t0 == 0) t0 = now;
+            else if (now - t0 > 4000000000LL) mbar_timeout_trap();  // ~2 s at 2 GHz
+        }
+    }
+}
+
+__device__ __forceinline__ void tma_load_3d(void* smem_dst, const CUtensorMap* map, uint64_t* bar, int c0, int c1,
+                                            int c2) {
+    asm volatile(
+        "cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];"
+        ::"r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(map)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2)
+        : "memory");
+}
+// 1-D bulk copy global -> shared (16-byte aligned, size a multiple of 16), completion on an mbarrier
+__device__ __forceinline__ void bulk_load_1d(void* smem_dst, const void* gmem_src, uint32_t bytes, uint64_t* bar) {
+    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
+                 ::"r"(smem_u32(smem_dst)), "l"(gmem_src), "r"(bytes), "r"(smem_u32(bar))
+                 : "memory");
+}
+
+__device__ __forceinline__ void prefetch_tensormap(const CUtensorMap* map) {
+    asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(map)) : "memory");
+}
+
+// ---- warpgroup MMA ordering ----------------------------------------------------------------------------------------
+// fence: register operands / accumulators written by ordinary instructions become visible to the following wgmma;
+// commit + wait<N>: at most N committed groups of this warpgroup still run (their registers may not be touched).
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() {
+    asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory");
+}
+
+}  // namespace ptx
+
+// --------------------------------------------------------------------------------------------
+// Shared-memory matrix descriptors (sm_90 layout: start >> 4 in bits 0-13, LBO >> 4 in 16-29, SBO >> 4 in 32-45,
+// swizzle mode in 62-63)
+// --------------------------------------------------------------------------------------------
+// K-major tile whose rows are 128 bytes (32 fp32) wide, laid out by TMA with CU_TENSOR_MAP_SWIZZLE_128B: 8-row groups of
+// 1024 B (SBO); LBO is unused for swizzled K-major tiles.  The tile must start on a 1024-byte boundary; a k-step of 8 tf32
+// inside the swizzle atom advances the start address by 32 bytes (+2 in the descriptor).
+__device__ __forceinline__ uint64_t make_smem_desc_sw128(uint32_t smem_addr) {
+    uint64_t d = 0;
+    d |= static_cast<uint64_t>((smem_addr >> 4) & 0x3FFF);
+    d |= static_cast<uint64_t>(1) << 16;
+    d |= static_cast<uint64_t>(1024 >> 4) << 32;
+    d |= static_cast<uint64_t>(1) << 62;  // SWIZZLE_128B
+    return d;
+}
+
+// Un-swizzled K-major tile: 8-row x 16-byte core matrices of 128 contiguous bytes; lbo = bytes between the core matrices of
+// consecutive 16-byte k chunks, sbo = bytes between consecutive 8-row groups.
+__device__ __forceinline__ uint64_t make_smem_desc_none(uint32_t smem_addr, uint32_t lbo, uint32_t sbo) {
+    uint64_t d = 0;
+    d |= static_cast<uint64_t>((smem_addr >> 4) & 0x3FFF);
+    d |= static_cast<uint64_t>((lbo >> 4) & 0x3FFF) << 16;
+    d |= static_cast<uint64_t>((sbo >> 4) & 0x3FFF) << 32;
+    return d;
+}
+
+// D[64 x N] (+)= A[64 x K] * B[N x K]^T for one warpgroup, fp32 accumulators in registers, A in registers (fragment of
+// the m16 x k rows of each warp: a0 = (g, c), a1 = (g + 8, c), a2 = (g, c + K/2), a3 = (g + 8, c + K/2), g = lane / 4,
+// c = lane % 4 (tf32: one value; bf16: the pair 2c, 2c + 1)), B K-major in shared memory.  TF32 = 1: kind tf32, K = 8;
+// TF32 = 0: bf16, K = 16.  Accumulator d[4j + i]: row g + 8 * (i >> 1), column 8j + 2c + (i & 1).  acc == 0 overwrites D.
+template <int N, int TF32> struct Wgmma;
+template <> struct Wgmma<32, 1> {
+    static __device__ __forceinline__ void mma(float (&d)[16], const uint32_t (&a)[4], uint64_t desc_b, uint32_t acc) {
+        asm volatile(
+            "{\n\t.reg .pred p;\n\t"
+            "setp.ne.b32 p, %21, 0;\n\t"
+            "wgmma.mma_async.sync.aligned.m64n32k8.f32.tf32.tf32 "
+            "{"
+            "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15"
+            "}, {%16, %17, %18, %19}, %20, p, 1, 1;\n\t}"
+            : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+              "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+            : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(desc_b), "r"(acc));
+    }
+};
+template <> struct Wgmma<32, 0> {
+    static __device__ __forceinline__ void mma(float (&d)[16], const uint32_t (&a)[4], uint64_t desc_b, uint32_t acc) {
+        asm volatile(
+            "{\n\t.reg .pred p;\n\t"
+            "setp.ne.b32 p, %21, 0;\n\t"
+            "wgmma.mma_async.sync.aligned.m64n32k16.f32.bf16.bf16 "
+            "{"
+            "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15"
+            "}, {%16, %17, %18, %19}, %20, p, 1, 1, 0;\n\t}"
+            : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+              "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+            : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(desc_b), "r"(acc));
+    }
+};
+template <> struct Wgmma<64, 1> {
+    static __device__ __forceinline__ void mma(float (&d)[32], const uint32_t (&a)[4], uint64_t desc_b, uint32_t acc) {
+        asm volatile(
+            "{\n\t.reg .pred p;\n\t"
+            "setp.ne.b32 p, %37, 0;\n\t"
+            "wgmma.mma_async.sync.aligned.m64n64k8.f32.tf32.tf32 "
+            "{"
+            "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+            "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31"
+            "}, {%32, %33, %34, %35}, %36, p, 1, 1;\n\t}"
+            : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+              "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+              "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+              "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+            : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(desc_b), "r"(acc));
+    }
+};
+template <> struct Wgmma<64, 0> {
+    static __device__ __forceinline__ void mma(float (&d)[32], const uint32_t (&a)[4], uint64_t desc_b, uint32_t acc) {
+        asm volatile(
+            "{\n\t.reg .pred p;\n\t"
+            "setp.ne.b32 p, %37, 0;\n\t"
+            "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 "
+            "{"
+            "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+            "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31"
+            "}, {%32, %33, %34, %35}, %36, p, 1, 1, 0;\n\t}"
+            : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+              "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+              "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+              "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+            : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(desc_b), "r"(acc));
+    }
+};
+template <> struct Wgmma<128, 1> {
+    static __device__ __forceinline__ void mma(float (&d)[64], const uint32_t (&a)[4], uint64_t desc_b, uint32_t acc) {
+        asm volatile(
+            "{\n\t.reg .pred p;\n\t"
+            "setp.ne.b32 p, %69, 0;\n\t"
+            "wgmma.mma_async.sync.aligned.m64n128k8.f32.tf32.tf32 "
+            "{"
+            "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+            "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+            "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+            "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63"
+            "}, {%64, %65, %66, %67}, %68, p, 1, 1;\n\t}"
+            : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+              "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+              "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+              "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+              "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+              "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+              "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
+              "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+            : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(desc_b), "r"(acc));
+    }
+};
+template <> struct Wgmma<128, 0> {
+    static __device__ __forceinline__ void mma(float (&d)[64], const uint32_t (&a)[4], uint64_t desc_b, uint32_t acc) {
+        asm volatile(
+            "{\n\t.reg .pred p;\n\t"
+            "setp.ne.b32 p, %69, 0;\n\t"
+            "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 "
+            "{"
+            "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+            "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+            "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+            "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63"
+            "}, {%64, %65, %66, %67}, %68, p, 1, 1, 0;\n\t}"
+            : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+              "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+              "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+              "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+              "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+              "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+              "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
+              "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+            : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(desc_b), "r"(acc));
+    }
+};
+
+// Two fp32 values -> one register of two bf16 (round to nearest even): `lo` in bits 0-15, `hi` in bits 16-31.
+__device__ __forceinline__ uint32_t pack_bf16x2_rn(float lo, float hi) {
+    uint32_t r;
+    asm("cvt.rn.bf16x2.f32 %0, %1, %2;" : "=r"(r) : "f"(hi), "f"(lo));
+    return r;
+}
+// bf16x3 operand split of a PAIR of fp32 values (k even in the low half): p1 = RN_bf16(x), p2 = RN_bf16(x - p1).
+// x - p1 is exact in fp32; |x - p1 - p2| <= 2^-16 |x|.
+__device__ __forceinline__ void split_bf16x2(float x0, float x1, uint32_t& p1, uint32_t& p2) {
+    p1 = pack_bf16x2_rn(x0, x1);
+    const float r0 = x0 - __uint_as_float(p1 << 16);
+    const float r1 = x1 - __uint_as_float(p1 & 0xFFFF0000u);
+    p2 = pack_bf16x2_rn(r0, r1);
+}
+// 3xTF32 operand split: hi = what the tensor core reads of x (low 13 mantissa bits dropped), lo = x - hi exactly.
+__device__ __forceinline__ void split_tf32_trunc(float x, uint32_t& hi, uint32_t& lo) {
+    hi = __float_as_uint(x) & 0xFFFFE000u;
+    lo = __float_as_uint(x - __uint_as_float(hi));
+}
+
+}  // namespace fcuda

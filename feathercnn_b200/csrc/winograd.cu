@@ -1,11 +1,11 @@
-// Winograd F(6,3) and F(2,3) transform kernels (sm_100a).
+// Winograd F(6,3) and F(2,3) transform kernels (sm_90a).
 //
 // Replaces, on the GPU:
 //   transformKernel_F6x6_3x3           /root/reference/src/booster/avx/winograd_kernels_F63.cpp:222-271   (filter, at Init)
 //   pad_input + winogradInputFrameTransformSeq   generic_kernels.cpp:31-48, winograd_kernels_F63.cpp:272-513
 //   winogradOutputTransform<RELU,BIAS>           winograd_kernels_F63.cpp:1029-1269
 //   F(2,3) variant                     /root/reference/src/booster/arm/winograd_kernels.cpp:115-279 (NEON only upstream)
-// The 64 (16) per-tile-element GEMMs in between run on tcgen05 (tensor_gemm.cu).
+// The 64 (16) per-tile-element GEMMs in between run on wgmma (tensor_gemm.cu).
 //
 // Layouts (private to this backend — parity is defined on NCHW blobs only, SURVEY.md §8):
 //   U[e][oc][ic]   transformed filters, K-major rows for the TensorGEMM B operand

@@ -117,7 +117,7 @@ public:
             tops[0]->ReshapeWithRealloc(batch, conv_param.output_channels, (conv_param.output_h + 1) / 2, (conv_param.output_w + 1) / 2);
         else
             tops[0]->ReshapeWithRealloc(batch, conv_param.output_channels, conv_param.output_h, conv_param.output_w);
-        // FEATHER_ALGO_POLICY=reference keeps avx/booster.cpp:283-310 verbatim; default is the B200 cost model
+        // FEATHER_ALGO_POLICY=reference keeps avx/booster.cpp:283-310 verbatim; default is the tuned cost model
         static const bool reference_policy = [] {
             const char* e = getenv("FEATHER_ALGO_POLICY");
             return e && e[0] == 'r';

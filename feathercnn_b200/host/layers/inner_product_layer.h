@@ -1,5 +1,5 @@
 // InnerProductLayer (mirrors /root/reference/src/layers/inner_product_layer.h:26-171).  The per-image SGEMV
-// of the reference becomes one weight-streaming tcgen05 GEMM over the batch (fcuda_inner_product_forward).
+// of the reference becomes one weight-streaming wgmma GEMM over the batch (fcuda_inner_product_forward).
 #pragma once
 
 #include <fcuda.h>

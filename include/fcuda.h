@@ -1,4 +1,4 @@
-/* fcuda.h — C ABI of the B200 (sm_100a) compute backend that replaces FeatherCNN's `booster`.
+/* fcuda.h — C ABI of the H100 (sm_90a) compute backend that replaces FeatherCNN's `booster`.
  *
  * Every entry point cites the reference interface it replaces (paths relative to /root/reference).
  * Conventions, all inherited from the reference boundary (SURVEY.md §8b):
@@ -24,11 +24,11 @@ extern "C" {
 /* booster::ConvAlgo, src/booster/include/booster/booster.h:42-51 (same numbering). */
 enum FcudaConvAlgo {
     FCUDA_NAIVE = 0,            /* CUDA-core fp32 implicit GEMM (device-side second opinion) */
-    FCUDA_IM2COL = 1,           /* pack kernel + tcgen05 TensorGEMM, bias/ReLU fused in the epilogue */
-    FCUDA_SGECONV = 2,          /* implicit GEMM straight from NCHW: patches gathered inside the tcgen05 kernel, no packed
+    FCUDA_IM2COL = 1,           /* pack kernel + wgmma TensorGEMM, bias/ReLU fused in the epilogue */
+    FCUDA_SGECONV = 2,          /* implicit GEMM straight from NCHW: patches gathered inside the wgmma kernel, no packed
                                    intermediate; a stub in the reference's AVX dispatcher (avx/booster.cpp:105-118) */
     FCUDA_DEPTHWISE = 3,        /* warp-shuffle stencil */
-    FCUDA_WINOGRADF63 = 4,      /* F(6,3): input transform -> 64-way tcgen05 TensorGEMM -> output transform(+bias+ReLU) */
+    FCUDA_WINOGRADF63 = 4,      /* F(6,3): input transform -> 64-way wgmma TensorGEMM -> output transform(+bias+ReLU) */
     FCUDA_WINOGRADF63FUSED = 5, /* not selected by the reference (avx/booster.cpp:291-292); unsupported (-1) */
     FCUDA_WINOGRADF23 = 6       /* F(2,3): 16-way TensorGEMM; stub in both reference dispatchers, real here */
 };
@@ -72,7 +72,7 @@ int fcuda_get_precision(void);
 
 /* Upper bound (bytes) on the Winograd / im2col intermediates of one chunk: a layer whose packed operands exceed it is
  * processed in several pack -> TensorGEMM -> unpack rounds over the batch (default 8 GiB, i.e. one round for the
- * benchmark configs — small L2-sized chunks measured slower on B200; 0 = never chunk). */
+ * benchmark configs; 0 = never chunk). */
 int fcuda_set_l2_chunk_bytes(size_t bytes);
 size_t fcuda_get_l2_chunk_bytes(void);
 
@@ -82,7 +82,7 @@ int fcuda_conv_assign_output_dim(FcudaConvParam* param);
 /* ConvBooster::SelectAlgo, avx/booster.cpp:283-310 (same rule, same -1 for partial groups). */
 int fcuda_conv_select_algo(const FcudaConvParam* param, int* algo);
 
-/* B200 cost-model variant of SelectAlgo: starts from the reference rule and moves bandwidth-bound Winograd layers
+/* Tuned cost-model variant of SelectAlgo: starts from the reference rule and moves bandwidth-bound Winograd layers
  * (<= 128 channels on images >= 28 wide) and the im2col layers to FCUDA_SGECONV.  Unlike the reference rule it treats
  * group == 1 with one input channel as an ordinary convolution, requires group > 1 and OC == IC for FCUDA_DEPTHWISE, and
  * sends partial groups / channel-multiplier depthwise to the grouped FCUDA_SGECONV instead of returning -1. */
@@ -104,7 +104,7 @@ int fcuda_conv_forward(const FcudaConvParam* param, int algo, float* output, con
 
 /* The 64-way batched "TensorGEMM" itself (avx/winograd_kernels_F63.cpp:518-757), exposed for tests and
  * profiling:  for g < G:  D[g][m][n] = sum_k A[g][m][k] * B[g][n][k]   (row-major, K-major operands).
- * `a` is plain fp32 (split into TF32 hi + fp32 lo inside the kernel, in tensor memory); b_hi/b_lo are the planes of
+ * `a` is plain fp32 (split into TF32 hi + fp32 lo inside the kernel, in registers); b_hi/b_lo are the planes of
  * fcuda_split_tf32(b) (b_lo NULL => plain TF32 on a and b_hi). */
 int fcuda_tensor_gemm(float* d, const float* a, const float* b_hi, const float* b_lo, int m, int n, int k, int g,
                       void* stream);
@@ -196,21 +196,10 @@ int fcuda_conv_forward_ext(const FcudaConvParam* param, int algo, float* output,
 
 /* Kernel-variant switches for A/B measurements and tests.  Defaults are the measured-best configuration; the environment
  * variable FCUDA_<NAME> sets the initial value.  Names (value range, default):
- *   igemm_issuers (1-2, 2)    MMA issuer threads of the implicit GEMM at BN <= 64 (each with its own accumulator)
- *   igemm_slab (0-1, 1)       TMA-fed input-slab producer for 3x3 / stride-1 layers (0: generic gather)
- *   igemm_cta_group (1-2, 1)  2: CTA pairs with tcgen05 cta_group::2 (M = 256, half of the filter tile per SM)
  *   dw_vec (0-1, 1)           vectorised depthwise kernel on wide planes
- *   gemm_cluster (1|2|4, 1)   TMA multicast of the B operand across a thread-block cluster in the TensorGEMM
- *   gemm_tma_store (0-2, 1)   row-major TensorGEMM epilogue: 1 = through shared memory + TMA stores, 0 = direct 16-byte
- *                             stores, 2 = direct 32-byte stores (st.global.v8: whole sectors, no shared-memory staging)
- *   igemm_tma_out (0-1, 1)    implicit-GEMM epilogue through shared memory + TMA stores (0: per-thread stores)
- *   igemm_pw (0-1, 1)         TMA-fed [32 channels][32 pixels] A boxes for 1x1 / stride-1 layers (0: generic gather)
  *   wino_mlp (0-2, 2)         Winograd transforms: 1 = every global load of a block in flight at once (cp.async slab /
  *                             back-to-back plane loads) instead of register-staged rounds; 2 = also launch the channel
  *                             blocks of a tile group next to each other (whole 1 KB rows of V / M in flight together)
- *   igemm_tma_lanes (1|2|4, 4) lanes of the implicit GEMM's filter-TMA warp that issue in lockstep (a thread starts a TMA
- *                             operation only every ~280 cycles; VGG-16 5.45 / 5.05 / 5.05 ms with 1 / 2 / 4 lanes)
- *   mbar_suspend_ns (0-1000000, 100000) suspend hint of the operand-ring barrier waits, 0 = poll (no measurable difference)
  * Every variant computes the same result (tests/test_gpu_variants.py).  Returns 0 / the value, -200 for an unknown name or value. */
 int fcuda_set_tuning(const char* name, int value);
 int fcuda_get_tuning(const char* name);

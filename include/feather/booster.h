@@ -41,7 +41,7 @@ class ConvBooster {
 public:
     ConvBooster() : algo(-1) {}
     int SelectAlgo(ConvParam* param) { return fcuda_conv_select_algo(param, &algo); }            // reference rule
-    int SelectAlgoTuned(ConvParam* param) { return fcuda_conv_select_algo_tuned(param, &algo); }  // B200 cost model
+    int SelectAlgoTuned(ConvParam* param) { return fcuda_conv_select_algo_tuned(param, &algo); }  // tuned cost model
     int ForceSelectAlgo(ConvAlgo a) { algo = static_cast<int>(a); return 0; }
     int SetFuncs() { return algo < 0 ? -1 : 0; }
     int GetBufferSize(ConvParam* param, size_t* buffer_size, size_t* processed_kernel_size, int batch = 1) const {

@@ -11,7 +11,7 @@ if str(ROOT) not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run with -m gpu on the B200 box)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (run with -m gpu on the H100 box)")
 
 
 def rel_err(got: np.ndarray, ref: np.ndarray) -> float:

@@ -1,4 +1,4 @@
-// Stand-alone self test for the tcgen05 TensorGEMM kernel (needs a B200).
+// Stand-alone self test for the wgmma TensorGEMM kernel (needs an H100).
 //   build: make -C feathercnn_b200/csrc selftest      run: build/gemm_selftest [--bench]
 // Compares tensor_gemm (TF32 and 3xTF32) against a double-precision host GEMM on small shapes and
 // against the CUDA-core fp32 kernel on large ones, for every epilogue.  Exit code != 0 on mismatch.

@@ -4,6 +4,9 @@
 The reference ships no golden vectors of its own (SURVEY.md §4), so these are outputs of the reference itself:
   conv_cases.npz   ConvBooster::Forward outputs for small layers covering every SelectAlgo branch
   mini_net.npz     every blob of feather::Net::Forward on the "mini" model (all layer types), seed-fixed input
+  reference_build_conv.npz   ConvBooster::Forward of the layers of tests/test_gpu_conv.py::REF_CASES (inputs from that
+                   test's seeded generator): a fixed sample of 4096 output values per layer plus max|y| of the whole output
+                   (python tests/golden/make_golden.py reference_build_conv)
 Inputs and weights are stored too, so the fixtures do not depend on NumPy's RNG staying stable.
 """
 import sys
@@ -60,5 +63,22 @@ def main():
     print("wrote", out / "conv_cases.npz", out / "mini_net.npz", out / "mini.param", out / "mini.bin")
 
 
+def reference_build_conv():
+    sys.path.insert(0, str(ROOT / "tests"))
+    import test_gpu_conv as T
+    out = Path(__file__).resolve().parent
+    O.build(ref=True)
+    ref = O.Reference()
+    gold = {}
+    for case in T.REF_CASES:
+        p, x, wt, b = T._data(O, case, 1, seed=7)
+        y = ref.conv(p, x[0], wt, b).ravel()
+        idx = np.sort(np.random.default_rng(1234).choice(y.size, min(4096, y.size), replace=False)).astype(np.int32)
+        gold[case[0] + "/idx"], gold[case[0] + "/y"] = idx, y[idx].astype(np.float32)
+        gold[case[0] + "/absmax"] = np.float64(np.abs(y).max())
+    np.savez_compressed(out / "reference_build_conv.npz", **gold)
+    print("wrote", out / "reference_build_conv.npz")
+
+
 if __name__ == "__main__":
-    main()
+    reference_build_conv() if sys.argv[1:] == ["reference_build_conv"] else main()

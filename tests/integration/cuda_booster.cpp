@@ -4,7 +4,7 @@
 //     FORWARD_FUNC table     (/root/reference/src/booster/include/booster/booster.h:151-170)
 // — on top of the C ABI of libfcuda.so (include/fcuda.h), in place of src/booster/avx/booster.cpp.  oracle/Makefile links
 // it with the UNMODIFIED reference objects (feather::Net, ConvLayer, ncnn loader, the AVX element-wise kernels) into
-// oracle/_ref/libfeather_ref_cuda.so, and tests/test_gpu_integration.py runs the reference's feather::Net on the B200
+// oracle/_ref/libfeather_ref_cuda.so, and tests/test_gpu_integration.py runs the reference's feather::Net on the GPU
 // kernels against the reference's AVX build.  Nothing in the product path includes or links this file.
 //
 // The reference host keeps HOST blobs and is batch-1 (src/blob.cpp:73), so this binding stages through device memory

@@ -1,6 +1,6 @@
-"""Every kernel variant behind fcuda_set_tuning computes the same convolution: the CTA-pair implicit GEMM (tcgen05
-cta_group::2), the TMA-fed slab producer vs the generic gather, one vs two MMA issuers, the cluster-multicast TensorGEMM,
-its TMA-store epilogue, the vectorised depthwise kernel.  Variants that only change data movement must be BIT-identical."""
+"""Every kernel variant behind fcuda_set_tuning computes the same convolution (the vectorised depthwise kernel must be
+BIT-identical to the plain one), and the implicit-GEMM / TensorGEMM arithmetic modes agree with the CUDA-core direct
+convolution and with each other."""
 import numpy as np
 import pytest
 
@@ -11,7 +11,7 @@ pytestmark = pytest.mark.gpu
 def tuning():
     from feathercnn_b200._lib import fcuda
     lib = fcuda()
-    names = ["igemm_issuers", "igemm_slab", "igemm_cta_group", "dw_vec", "gemm_cluster", "gemm_tma_store", "igemm_tma_out", "igemm_pw", "igemm_tma_lanes", "mbar_suspend_ns"]
+    names = ["dw_vec", "wino_mlp"]
     saved = {n: lib.fcuda_get_tuning(n.encode()) for n in names}
 
     def setter(**kw):
@@ -42,65 +42,41 @@ IGEMM_GEOMS = [(64, 64, 96, 96, 3, 1, 1, 3), (128, 64, 56, 56, 3, 1, 1, 4), (256
 
 
 @pytest.mark.parametrize("geom", IGEMM_GEOMS)
-def test_implicit_gemm_variants_are_bit_identical(cuda, tuning, geom):
+def test_implicit_gemm_variants_are_bit_identical(cuda, geom):
+    """3xTF32 implicit GEMM: within 2e-4 of the CUDA-core direct convolution and bit-identical from run to run."""
     from feathercnn_b200 import booster
     booster.set_precision(booster.PRECISION_TF32X3)
-    tuning(igemm_cta_group=1, igemm_slab=1, igemm_issuers=2)
     base = _conv(cuda, booster, geom, booster.SGECONV)
     naive = _conv(cuda, booster, geom, booster.NAIVE)
     assert np.abs(base - naive).max() / np.abs(naive).max() < 2e-4
-    tuning(igemm_cta_group=2)                      # CTA pairs: M = 256 MMAs, half of the filter tile per SM
-    np.testing.assert_array_equal(_conv(cuda, booster, geom, booster.SGECONV), base)
-    tuning(igemm_cta_group=1, igemm_slab=0)        # generic gather instead of the TMA slab
-    np.testing.assert_array_equal(_conv(cuda, booster, geom, booster.SGECONV), base)
-    tuning(igemm_slab=1, igemm_issuers=1)          # one issuer: one accumulator, same k order within it
-    one = _conv(cuda, booster, geom, booster.SGECONV)
-    assert np.abs(one - base).max() / np.abs(base).max() < 1e-5   # summation order differs (even/odd k-blocks vs all)
-    tuning(igemm_issuers=2, igemm_cta_group=2, igemm_slab=0)
-    np.testing.assert_array_equal(_conv(cuda, booster, geom, booster.SGECONV), base)
-    tuning(igemm_cta_group=1, igemm_slab=1, igemm_tma_out=0)   # per-thread stores instead of the TMA-store epilogue
-    np.testing.assert_array_equal(_conv(cuda, booster, geom, booster.SGECONV), base)
-    tuning(igemm_tma_out=1, igemm_pw=0)            # generic gather instead of the pointwise TMA boxes
     np.testing.assert_array_equal(_conv(cuda, booster, geom, booster.SGECONV), base)
 
 
 @pytest.mark.parametrize("geom", IGEMM_GEOMS)
-def test_bf16x3_implicit_gemm_variants(cuda, tuning, geom):
-    """The default split mode (BF16x3 operands in the implicit GEMM): data-movement variants stay bit-identical, and the
-    result sits within 5e-5 of the 3xTF32 one (dropped terms <= 3 * 2^-16 per product, random sign)."""
+def test_bf16x3_implicit_gemm_variants(cuda, geom):
+    """The default split mode (BF16x3 operands in the implicit GEMM): within 5e-5 of the 3xTF32 result (dropped terms
+    <= 3 * 2^-16 per product, random sign) and bit-identical from run to run."""
     from feathercnn_b200 import booster
     booster.set_precision(booster.PRECISION_TF32X3)
-    tuning(igemm_cta_group=1, igemm_slab=1, igemm_issuers=2)
     ref = _conv(cuda, booster, geom, booster.SGECONV)
     booster.set_precision(booster.PRECISION_FP32_SPLIT)
     base = _conv(cuda, booster, geom, booster.SGECONV)
     assert np.abs(base - ref).max() / np.abs(ref).max() < 5e-5
     np.testing.assert_array_equal(_conv(cuda, booster, geom, booster.SGECONV), base)   # run to run
-    tuning(igemm_slab=0)
-    np.testing.assert_array_equal(_conv(cuda, booster, geom, booster.SGECONV), base)
-    tuning(igemm_slab=1, igemm_tma_out=0)
-    np.testing.assert_array_equal(_conv(cuda, booster, geom, booster.SGECONV), base)
-    tuning(igemm_tma_out=1, igemm_pw=0)
-    np.testing.assert_array_equal(_conv(cuda, booster, geom, booster.SGECONV), base)
-    tuning(igemm_pw=1, igemm_tma_lanes=1, mbar_suspend_ns=0)   # one filter-TMA lane, polling barrier waits
-    np.testing.assert_array_equal(_conv(cuda, booster, geom, booster.SGECONV), base)
-    tuning(igemm_tma_lanes=2, mbar_suspend_ns=100000)
-    np.testing.assert_array_equal(_conv(cuda, booster, geom, booster.SGECONV), base)
-    tuning(igemm_tma_lanes=4, igemm_issuers=1)
-    one = _conv(cuda, booster, geom, booster.SGECONV)
-    assert np.abs(one - base).max() / np.abs(base).max() < 1e-5
 
 
 @pytest.mark.parametrize("geom", [(64, 64, 56, 56, 3, 1, 1, 4), (256, 128, 28, 28, 3, 1, 1, 8), (512, 256, 14, 14, 3, 1, 1, 16)])
 def test_tensor_gemm_variants_are_bit_identical(cuda, tuning, geom):
+    """Winograd F(6,3) through the 3xTF32 TensorGEMM: within 2e-4 of the direct convolution; the Winograd transform
+    variants (wino_mlp) only change data movement and stay bit-identical."""
     from feathercnn_b200 import booster
     booster.set_precision(booster.PRECISION_TF32X3)
-    tuning(gemm_cluster=1, gemm_tma_store=1)
+    tuning(wino_mlp=2)
     base = _conv(cuda, booster, geom, booster.WINOGRADF63)
     naive = _conv(cuda, booster, geom, booster.NAIVE)
     assert np.abs(base - naive).max() / np.abs(naive).max() < 2e-4
-    for cluster, store in ((1, 0), (1, 2), (2, 1), (4, 1), (2, 0)):   # store 2: direct 32-byte st.global.v8 epilogue
-        tuning(gemm_cluster=cluster, gemm_tma_store=store)
+    for mlp in (0, 1, 2):
+        tuning(wino_mlp=mlp)
         np.testing.assert_array_equal(_conv(cuda, booster, geom, booster.WINOGRADF63), base)
 
 
