@@ -439,9 +439,12 @@ int launch_igemm(const IgemmProblem& p, cudaStream_t stream) {
     a.tiles_y = ceil_div(p.OH, 2);
     const long long pixel_tiles = a.pool ? static_cast<long long>(p.N) * a.tiles_x * a.tiles_y : (a.total_pix + 127) / 128;
     const long long total = pixel_tiles * a.num_n;
-    // 32-bit plane strides and packed tap offsets (dy << 16 | dx) inside the kernel
+    // 32-bit plane strides and packed tap offsets (dy << 16 | dx) inside the kernel; the k-table's element offsets
+    // ic * H * W + dy * W + dx are 32-bit as well
+    const long long table_max = static_cast<long long>(p.IC - 1) * p.H * p.W + static_cast<long long>(p.KH - 1) * a.dil_h * p.W +
+                                static_cast<long long>(p.KW - 1) * a.dil_w;
     if (total >= (1ll << 31) || static_cast<long long>(p.H) * p.W >= (1ll << 30) || static_cast<long long>(p.OH) * p.OW >= (1ll << 30) ||
-        (p.KH - 1) * a.dil_h >= (1 << 15) || (p.KW - 1) * a.dil_w >= (1 << 16))
+        (p.KH - 1) * a.dil_h >= (1 << 15) || (p.KW - 1) * a.dil_w >= (1 << 16) || (a.use_table && table_max >= (1ll << 31)))
         return -1;
     constexpr int kStage = NPL * BN * 32 * (BF ? 2 : 4);
     const int table_bytes = a.use_table ? a.kblocks * 32 * 8 : 0;
