@@ -466,7 +466,418 @@ int launch_igemm(const IgemmProblem& p, cudaStream_t stream) {
     return 0;
 }
 
+// ===================================================================================================================
+// Halo kernel: stride-1, dense layers with IC % 32 == 0 (k = ((ic/32)*taps + tap)*32 + ic%32, as above).
+//
+//   M tile     = an R x C patch of output pixels inside one image (R * C = 128, C in {8, 16, 32, 64}); warp w covers rows
+//                2*(w / (C/8)) + {0, 1} (fragment rows gq, gq + 8) and columns 8*(w % (C/8)) + gq, so a fused 2x2 pooling
+//                window still sits in one thread and its lane ^ 4 neighbour.
+//   A operand  = per 32-channel block ONE 4-D TMA box {Cb, Rb, 32, 1} of the input blob at (x0 - xpad, y0 - pad_top),
+//                xpad = pad_left rounded up to 4 so that every box row starts on a 16-byte boundary: the patch plus its
+//                halo, zero-filled outside the image (= the im2col padding).  Every tap (dy, dx) of the
+//                block reads it as a shifted view with ld.shared, so each input value crosses L2 -> SM once per channel
+//                block instead of once per tap.  Boxes have their own 2-deep ring; Rb / Cb are padded until the warp's 32
+//                words of one gather (8 columns x 4 channel planes) hit 32 different banks (halo_banks_conflict_free).
+//   B operand  = the same pre-tiled filter planes / swizzled TMA rows and the same 4-deep ring as conv_igemm_kernel.
+//   pipeline   = two fragment sets: k-block kb + 1 is gathered and split while kb's wgmma group runs (wgmma_wait<1>); a
+//                filter stage is released once its group retired.  Persistent CTAs loop over tiles, so the producer warp
+//                fetches the next tile's halo and filters during the epilogue.
+//
+// Per k-block the wgmma sequence (p2*q1, p1*q2, p1*q1 per k-step), the operand values, the k order and BN are those of
+// conv_igemm_kernel: the result is bit-identical to it.
+constexpr int kHaloStages = 2;
+
+struct HaloArgs {
+    const float* residual;
+    float* out;
+    const float* bias;
+    int OC, OH, OW, KW, taps;
+    int out_img_c;
+    int kblocks, num_n;
+    int relu, pool;
+    int R, C;              // output patch rows x columns (128 pixels)
+    int tiles_x, tiles_y;  // patches per image
+    int Rb, Cb;            // halo box rows / columns in shared memory (padded)
+    int pad_top, xpad;     // box origin relative to the patch: rows -pad_top, columns -xpad (xpad % 4 == 0)
+    int xshift;            // xpad - pad_left: box column of tap dx = 0 for patch column 0
+    long long tiles;       // N * tiles_y * tiles_x * num_n
+    const unsigned char* wbf;
+    unsigned wbf_kb_bytes;
+};
+
+template <int BN, int PLANES>
+__global__ void __launch_bounds__(kThreadsIg, 1)
+conv_igemm_halo_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__ CUtensorMap tmW,
+                       const __grid_constant__ CUtensorMap tmWlo, const HaloArgs args) {
+    constexpr bool BF = PLANES == 3;
+    constexpr int NPL = BF ? 2 : PLANES;
+    constexpr int kBTile = BN * 32 * (BF ? 2 : 4);
+    constexpr int kStage = NPL * kBTile;
+    extern __shared__ uint8_t smem_raw[];
+    // indexing smem_raw itself (not a re-cast integer) keeps the halo reads ld.shared
+    uint8_t* smem = smem_raw + ((1024u - (ptx::smem_u32(smem_raw) & 1023u)) & 1023u);
+    const float* halo = reinterpret_cast<const float*>(smem + kStagesIg * kStage);
+    const int cstride = args.Rb * args.Cb;  // floats between the channel planes of a box
+    const int hstage = 32 * cstride;        // floats per box
+    __shared__ uint64_t full_bar[kStagesIg];
+    __shared__ uint64_t empty_bar[kStagesIg];
+    __shared__ uint64_t hfull_bar[kHaloStages];
+    __shared__ uint64_t hempty_bar[kHaloStages];
+
+    const int warp = threadIdx.x >> 5;
+    const int lane = threadIdx.x & 31;
+    const int per_img = args.tiles_x * args.tiles_y;
+    const int kblocks = args.kblocks, taps = args.taps;
+    const int ncb = kblocks / taps;
+
+    if (threadIdx.x == 0) {
+        for (int s = 0; s < kStagesIg; ++s) {
+            ptx::mbar_init(&full_bar[s], 1);
+            ptx::mbar_init(&empty_bar[s], kConsumerWarps);
+        }
+        for (int s = 0; s < kHaloStages; ++s) {
+            ptx::mbar_init(&hfull_bar[s], 1);
+            ptx::mbar_init(&hempty_bar[s], kConsumerWarps);
+        }
+        ptx::fence_barrier_init();
+    }
+    __syncthreads();
+
+    if (warp == kConsumerWarps) {
+        // ===================== producer: halo boxes + filters, in consumption order =====================
+        if (lane == 0) {
+            ptx::prefetch_tensormap(&tmX);
+            if (!BF) {
+                ptx::prefetch_tensormap(&tmW);
+                if (NPL == 2) ptx::prefetch_tensormap(&tmWlo);
+            }
+            int hb = 0;   // boxes issued
+            int kbg = 0;  // filter stages issued
+            auto load_halo = [&](long long t, int cb) {
+                const long long pt = t / args.num_n;
+                const int n = static_cast<int>(pt / per_img);
+                const int rem = static_cast<int>(pt - static_cast<long long>(n) * per_img);
+                const int ty = rem / args.tiles_x, tx = rem - ty * args.tiles_x;
+                const int hs = hb % kHaloStages;
+                if (hb >= kHaloStages) ptx::mbar_wait_nocall(&hempty_bar[hs], ((hb / kHaloStages) - 1) & 1);
+                ptx::mbar_arrive_expect_tx(&hfull_bar[hs], static_cast<uint32_t>(hstage) * 4u);
+                ptx::tma_load_4d(const_cast<float*>(halo) + hs * hstage, &tmX, &hfull_bar[hs], tx * args.C - args.xpad,
+                                 ty * args.R - args.pad_top, cb * 32, n);
+                ++hb;
+            };
+            if (blockIdx.x < args.tiles) load_halo(blockIdx.x, 0);
+            for (long long t = blockIdx.x; t < args.tiles; t += gridDim.x) {
+                const int n_blk = static_cast<int>(t % args.num_n);
+                for (int cb = 0, kb = 0; cb < ncb; ++cb) {
+                    for (int tap = 0; tap < taps; ++tap, ++kb, ++kbg) {
+                        const int stage = kbg % kStagesIg;
+                        if (kbg >= kStagesIg) ptx::mbar_wait_nocall(&empty_bar[stage], ((kbg / kStagesIg) - 1) & 1);
+                        uint8_t* st = smem + stage * kStage;
+                        ptx::mbar_arrive_expect_tx(&full_bar[stage], kStage);
+                        if (BF) {
+                            ptx::bulk_load_1d(st, args.wbf + static_cast<size_t>(kb) * args.wbf_kb_bytes + static_cast<size_t>(n_blk) * kStage,
+                                              kStage, &full_bar[stage]);
+                        } else {
+                            ptx::tma_load_3d(st, &tmW, &full_bar[stage], kb * 32, n_blk * BN, 0);
+                            if (NPL == 2) ptx::tma_load_3d(st + kBTile, &tmWlo, &full_bar[stage], kb * 32, n_blk * BN, 0);
+                        }
+                        if (tap == 0) {  // the next box (this tile's next channel block or the next tile's first) lands meanwhile
+                            if (cb + 1 < ncb) load_halo(t, cb + 1);
+                            else if (t + gridDim.x < args.tiles) load_halo(t + gridDim.x, 0);
+                        }
+                    }
+                }
+            }
+        }
+        return;
+    }
+
+    // ===================== consumers =====================
+    const int gq = lane >> 2, c = lane & 3;
+    const int wcols = args.C >> 3;
+    const int wy = warp / wcols, wx = warp - wy * wcols;
+    const int prow = 2 * wy, pcol = 8 * wx + gq;  // this thread's pixels in the patch: rows prow + h, column pcol
+    // word offset of (channel frag_k(0, c), row prow, column pcol) inside a box; tap (dy, dx) adds dy * Cb + dx
+    const int abase = (BF ? 2 * c : c) * cstride + prow * args.Cb + pcol + args.xshift;
+
+    auto gather = [&](const float* box, int toff, float (&raw)[2][8]) {
+#pragma unroll
+        for (int h = 0; h < 2; ++h)
+#pragma unroll
+            for (int j = 0; j < 8; ++j) raw[h][j] = box[abase + toff + h * args.Cb + frag_k<BF>(j, 0) * cstride];
+    };
+    auto split = [&](const float (&raw)[2][8], uint32_t (&f1)[4][4], uint32_t (&f2)[4][4]) {
+        if (BF) {
+#pragma unroll
+            for (int kk = 0; kk < 2; ++kk)
+#pragma unroll
+                for (int q = 0; q < 4; ++q) {
+                    const int h = q & 1, j = 4 * kk + 2 * (q >> 1);
+                    split_bf16x2(raw[h][j], raw[h][j + 1], f1[kk][q], f2[kk][q]);
+                }
+        } else {
+#pragma unroll
+            for (int kk = 0; kk < 4; ++kk)
+#pragma unroll
+                for (int q = 0; q < 4; ++q) {
+                    const float x = raw[q & 1][2 * kk + (q >> 1)];
+                    if (PLANES == 2) split_tf32_trunc(x, f1[kk][q], f2[kk][q]);
+                    else f1[kk][q] = __float_as_uint(x);
+                }
+        }
+    };
+
+    const int oplane = args.OH * args.OW;
+    const int SH = (args.OH + 1) >> 1, SW = (args.OW + 1) >> 1;  // pooled geometry
+    int kbg = 0;  // filter stages consumed
+    int hb = 0;   // boxes consumed
+    for (long long t = blockIdx.x; t < args.tiles; t += gridDim.x) {
+        const int n_blk = static_cast<int>(t % args.num_n);
+        const long long pt = t / args.num_n;
+        const int img = static_cast<int>(pt / per_img);
+        const int rem = static_cast<int>(pt - static_cast<long long>(img) * per_img);
+        const int ty = rem / args.tiles_x, tx = rem - ty * args.tiles_x;
+        int oy[2];
+        bool valid[2];
+        const int ox = tx * args.C + pcol;
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+            oy[h] = ty * args.R + prow + h;
+            valid[h] = oy[h] < args.OH && ox < args.OW;
+        }
+
+        float acc[BN / 2];
+#pragma unroll
+        for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+        float raw[2][8];
+        uint32_t fa1[4][4], fa2[4][4], fb1[4][4], fb2[4][4];  // two fragment sets: [k-step][a0..a3], hi / p1 and lo / p2
+        int tap = 0, dy = 0, dx = 0;                          // tap of the k-block in `raw`
+        ptx::mbar_wait_nocall(&hfull_bar[hb % kHaloStages], (hb / kHaloStages) & 1);
+        gather(halo + (hb % kHaloStages) * hstage, 0, raw);
+
+        auto step = [&](uint32_t (&f1)[4][4], uint32_t (&f2)[4][4], int kb) {
+            split(raw, f1, f2);
+            if (++tap == taps) {  // the box's last tap is in registers: hand the box back
+                tap = dy = dx = 0;
+                __syncwarp();
+                ptx::mbar_arrive_if(&hempty_bar[hb % kHaloStages], lane == 0);
+                ++hb;
+            } else if (++dx == args.KW) {
+                dx = 0;
+                ++dy;
+            }
+            if (kb + 1 < kblocks) {
+                if (tap == 0) ptx::mbar_wait_nocall(&hfull_bar[hb % kHaloStages], (hb / kHaloStages) & 1);
+                gather(halo + (hb % kHaloStages) * hstage, dy * args.Cb + dx, raw);
+            }
+            const int stage = kbg % kStagesIg;
+            ptx::mbar_wait_nocall(&full_bar[stage], (kbg / kStagesIg) & 1);
+            const uint32_t b_base = ptx::smem_u32(smem + stage * kStage);
+            ptx::wgmma_fence();
+            if (BF) {
+                const uint64_t dQ1 = make_smem_desc_none(b_base, 128, 512);
+                const uint64_t dQ2 = make_smem_desc_none(b_base + kBTile, 128, 512);
+#pragma unroll
+                for (int kk = 0; kk < 2; ++kk) {
+                    Wgmma<BN, 0>::mma(acc, f2[kk], dQ1 + 16 * kk, 1u);  // p2 * q1
+                    Wgmma<BN, 0>::mma(acc, f1[kk], dQ2 + 16 * kk, 1u);  // p1 * q2
+                    Wgmma<BN, 0>::mma(acc, f1[kk], dQ1 + 16 * kk, 1u);  // p1 * q1
+                }
+            } else {
+                const uint64_t dB = make_smem_desc_sw128(b_base);
+                const uint64_t dBlo = make_smem_desc_sw128(b_base + kBTile);
+#pragma unroll
+                for (int kk = 0; kk < 4; ++kk) {
+                    if (PLANES == 2) {
+                        Wgmma<BN, 1>::mma(acc, f2[kk], dB + 2 * kk, 1u);    // A_lo * B_hi
+                        Wgmma<BN, 1>::mma(acc, f1[kk], dBlo + 2 * kk, 1u);  // A_hi * B_lo
+                        Wgmma<BN, 1>::mma(acc, f1[kk], dB + 2 * kk, 1u);    // A_hi * B_hi
+                    } else {
+                        Wgmma<BN, 1>::mma(acc, f1[kk], dB + 2 * kk, 1u);
+                    }
+                }
+            }
+            ptx::wgmma_commit();
+            ptx::wgmma_wait<1>();  // k-block kb - 1 retired: its filter stage and fragment set are free
+            __syncwarp();
+            ptx::mbar_arrive_if(&empty_bar[(kbg + kStagesIg - 1) % kStagesIg], kb > 0 && lane == 0);
+            ++kbg;
+        };
+        for (int kb = 0; kb < kblocks; kb += 2) {
+            step(fa1, fa2, kb);
+            if (kb + 1 < kblocks) step(fb1, fb2, kb + 1);
+        }
+        ptx::wgmma_wait<0>();
+        __syncwarp();
+        ptx::mbar_arrive_if(&empty_bar[(kbg - 1) % kStagesIg], lane == 0);
+
+        // ===================== epilogue (as conv_igemm_kernel) =====================
+#pragma unroll
+        for (int j = 0; j < BN / 8; ++j) {
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {
+                const int oc = n_blk * BN + 8 * j + 2 * c + e;
+                const bool oc_ok = oc < args.OC;
+                const float bv = (args.bias != nullptr && oc_ok) ? __ldg(args.bias + oc) : 0.f;
+                float v[2];
+#pragma unroll
+                for (int h = 0; h < 2; ++h) {
+                    v[h] = acc[4 * j + 2 * h + e] + bv;
+                    const size_t o = (static_cast<size_t>(img) * args.out_img_c + oc) * oplane + static_cast<size_t>(oy[h]) * args.OW + ox;
+                    if (args.residual != nullptr && valid[h] && oc_ok) v[h] += __ldg(args.residual + o);
+                    if (args.relu) v[h] = fmaxf(v[h], 0.f);
+                    if (!args.pool && valid[h] && oc_ok) args.out[o] = v[h];
+                }
+                if (args.pool) {
+                    float m = fmaxf(valid[0] ? v[0] : -INFINITY, valid[1] ? v[1] : -INFINITY);
+                    m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, 4));  // the window's other column: pixel gq ^ 1
+                    if ((gq & 1) == 0 && valid[0] && oc_ok)
+                        args.out[(static_cast<size_t>(img) * args.out_img_c + oc) * (static_cast<size_t>(SH) * SW) +
+                                 static_cast<size_t>(oy[0] >> 1) * SW + (ox >> 1)] = m;
+                }
+            }
+        }
+    }
+}
+
+// Bank model of one ld.shared of the halo gather: lane l reads column l / 4 of channel plane (l % 4) * (2 for the bf16
+// pairs, 1 for tf32); the warp is conflict-free when its 32 words fall in 32 different banks (the starting column and
+// row only rotate the pattern).
+static bool halo_banks_conflict_free(int cstride, bool bf) {
+    unsigned used = 0;
+    for (int l = 0; l < 32; ++l) used |= 1u << (((l >> 2) + (bf ? 2 : 1) * (l & 3) * cstride) & 31);
+    return used == 0xFFFFFFFFu;
+}
+
+static int halo_smem_bytes(int OC, int planes, int Rb, int Cb) {
+    const int npl = planes == 3 ? 2 : planes;
+    const int b_stage = npl * igemm_bn_for(OC) * 32 * (planes == 3 ? 2 : 4);
+    return kStagesIg * b_stage + kHaloStages * 32 * Rb * Cb * 4 + 1024;
+}
+
+// Patch and box of the halo kernel for a layer, or false when the layer keeps conv_igemm_kernel.  Among the patches
+// 16x8, 32x4, 8x16 and 64x2 (columns x rows) the one that computes the fewest padded pixels wins (earlier on a tie:
+// smaller halo).
+static bool halo_geometry(const IgemmProblem& p, HaloGeom& g) {
+    if (p.stride_h != 1 || p.stride_w != 1 || p.dil_h > 1 || p.dil_w > 1 || p.IC % 32 != 0) return false;
+    const int taps = p.KH * p.KW;
+    if (taps < 2 || taps > 63 || p.W % 4 != 0 || p.OH < 1 || p.OW < 1) return false;  // 1x1: no tap reuse
+    if (p.input != nullptr && (reinterpret_cast<uintptr_t>(p.input) & 15) != 0) return false;  // TMA: 16-byte base
+    static const int kCols[4] = {16, 32, 8, 64};
+    long long best = -1;
+    for (int C : kCols) {
+        const int R = 128 / C;
+        const long long cost = static_cast<long long>(ceil_div(p.OW, C)) * C * ceil_div(p.OH, R) * R;
+        const int xshift = ((p.pad_left + 3) & ~3) - p.pad_left;
+        const int rb0 = R + p.KH - 1, cb0 = (C + p.KW - 1 + xshift + 3) & ~3;  // 16-byte box rows
+        int rb = 0, cbx = 0;
+        for (int dc = 0; dc <= 12; dc += 4)
+            for (int dr = 0; dr < 8; ++dr) {
+                const int r = rb0 + dr, cc = cb0 + dc;
+                if (r > 256 || cc > 256 || !halo_banks_conflict_free(r * cc, p.planes == 3)) continue;
+                if (rb == 0 || r * cc < rb * cbx) { rb = r; cbx = cc; }
+            }
+        if (rb == 0 || halo_smem_bytes(p.OC, p.planes, rb, cbx) > 227 * 1024) continue;
+        if (best < 0 || cost < best) {
+            best = cost;
+            g.R = R; g.C = C; g.Rb = rb; g.Cb = cbx;
+        }
+    }
+    return best >= 0;
+}
+
+template <int BN, int PLANES>
+int launch_igemm_halo(const IgemmProblem& p, const HaloGeom& hg, cudaStream_t stream) {
+    constexpr bool BF = PLANES == 3;
+    constexpr int NPL = BF ? 2 : PLANES;
+    const int taps = p.KH * p.KW;
+    const int K = taps * p.IC;
+    EncodeTiledFn enc = encode_fn();
+    if (!enc) return FCUDA_ERR_CUDA;
+    CUtensorMap tmX, tmW, tmWlo;
+    memset(&tmW, 0, sizeof(tmW));
+    tmWlo = tmW;
+    if (!BF) {
+        const int Kf = (K + 3) & ~3;
+        for (int pl = 0; pl < NPL; ++pl) {
+            cuuint64_t dims[3] = {(cuuint64_t)Kf, (cuuint64_t)p.OC, 1};
+            cuuint64_t strides[2] = {(cuuint64_t)Kf * 4, (cuuint64_t)Kf * p.OC * 4};
+            cuuint32_t box[3] = {32, (cuuint32_t)BN, 1};
+            cuuint32_t estr[3] = {1, 1, 1};
+            const float* base = pl == 0 ? p.w_hi : p.w_lo;
+            CUresult r = enc(pl == 0 ? &tmW : &tmWlo, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, const_cast<float*>(base), dims, strides,
+                             box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
+                             CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+            if (r != CUDA_SUCCESS) {
+                fprintf(stderr, "fcuda: igemm weight tensor map failed (%d)\n", (int)r);
+                return FCUDA_ERR_CUDA;
+            }
+        }
+    }
+    {   // the input blob [N][in_img_c][H][W] (the IC channels of this slice); boxes past its edges read as zeros
+        const cuuint64_t in_c = static_cast<cuuint64_t>(p.in_c_total > 0 ? p.in_c_total : p.IC);
+        cuuint64_t dims[4] = {(cuuint64_t)p.W, (cuuint64_t)p.H, (cuuint64_t)p.IC, (cuuint64_t)p.N};
+        cuuint64_t strides[3] = {(cuuint64_t)p.W * 4, (cuuint64_t)p.W * p.H * 4, in_c * p.H * p.W * 4};
+        cuuint32_t box[4] = {(cuuint32_t)hg.Cb, (cuuint32_t)hg.Rb, 32, 1};
+        cuuint32_t estr[4] = {1, 1, 1, 1};
+        CUresult r = enc(&tmX, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, const_cast<float*>(p.input), dims, strides, box, estr,
+                         CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                         CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+        if (r != CUDA_SUCCESS) {
+            fprintf(stderr, "fcuda: igemm input tensor map failed (%d)\n", (int)r);
+            return FCUDA_ERR_CUDA;
+        }
+    }
+    if (BF && (igemm_bn_for(p.OC) != BN || static_cast<unsigned long long>(ceil_div(K, 32)) * igemm_ocpad(p.OC) * 128ull >= (1ull << 31))) return -1;
+    HaloArgs a;
+    a.residual = p.residual; a.out = p.output; a.bias = p.bias;
+    a.OC = p.OC; a.OH = p.OH; a.OW = p.OW; a.KW = p.KW; a.taps = taps;
+    a.out_img_c = p.out_c_total > 0 ? p.out_c_total : p.OC;
+    a.kblocks = ceil_div(K, 32);
+    a.num_n = ceil_div(p.OC, BN);
+    a.relu = p.relu;
+    a.pool = p.pool ? 1 : 0;
+    a.R = hg.R; a.C = hg.C;
+    a.tiles_x = ceil_div(p.OW, hg.C);
+    a.tiles_y = ceil_div(p.OH, hg.R);
+    a.Rb = hg.Rb; a.Cb = hg.Cb;
+    a.pad_top = p.pad_top;
+    a.xpad = (p.pad_left + 3) & ~3;
+    a.xshift = a.xpad - p.pad_left;
+    const long long pixel_tiles = static_cast<long long>(p.N) * a.tiles_x * a.tiles_y;
+    a.tiles = pixel_tiles * a.num_n;
+    a.wbf = reinterpret_cast<const unsigned char*>(p.w_hi);
+    a.wbf_kb_bytes = 2u * static_cast<unsigned>(igemm_ocpad(p.OC)) * 64u;
+    if (static_cast<long long>(p.OH) * p.OW >= (1ll << 30) || a.tiles * a.kblocks >= (1ll << 31)) return -1;
+    const int smem = halo_smem_bytes(p.OC, PLANES, hg.Rb, hg.Cb);
+    auto kern = conv_igemm_halo_kernel<BN, PLANES>;
+    static SmemAttrCache attr_cache;
+    if (int rc = ensure_dynamic_smem(kern, smem, attr_cache)) return rc;
+    int per_sm = 0;
+    FCUDA_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, kThreadsIg, smem));
+    const long long slots = static_cast<long long>(sm_count()) * (per_sm > 0 ? per_sm : 1);
+    const unsigned grid = static_cast<unsigned>(a.tiles < slots ? a.tiles : slots);
+    // the same algorithmic work as conv_igemm_kernel; the issued MMA work includes the padded patch pixels
+    const double macs = static_cast<double>(p.N) * p.OC * p.OH * p.OW * p.IC * taps;
+    const double mma = 2.0 * static_cast<double>(pixel_tiles) * 128 * (a.num_n * BN) * (a.kblocks * 32) * (PLANES >= 2 ? 3 : 1);
+    const int prof = prof_begin(stream, PROF_IGEMM, 2.0 * macs, mma,
+                                4.0 * (static_cast<double>(p.N) * p.IC * p.H * p.W + static_cast<double>(p.OC) * K +
+                                       static_cast<double>(p.N) * p.OC * p.OH * p.OW * (p.residual ? 2 : 1)));
+    kern<<<grid, kThreadsIg, smem, stream>>>(tmX, tmW, tmWlo, a);
+    prof_end(prof, stream);
+    FCUDA_CHECK_LAUNCH();
+    count_launch();
+    return 0;
+}
+
 }  // namespace
+
+bool conv_igemm_halo_geometry(const IgemmProblem& p, HaloGeom* g) {
+    HaloGeom tmp;
+    const bool ok = halo_geometry(p, tmp);
+    if (ok && g) *g = tmp;
+    return ok;
+}
 
 bool conv_igemm_supported(int IC, int KH, int KW) {
     if (KH * KW > 63) return false;                               // per-pixel tap validity mask is 64-bit
@@ -512,6 +923,12 @@ int conv_igemm_forward(const IgemmProblem& p, cudaStream_t stream) {
     if (!conv_igemm_supported(p.IC, p.KH, p.KW)) return -1;
     if (p.pool && !conv_igemm_can_pool(p)) return -200;
     const int bn = igemm_bn_for(p.OC);
+    HaloGeom hg;
+    if (tune_get(TUNE_IGEMM_HALO) != 0 && halo_geometry(p, hg)) {
+        if (p.planes == 3) return bn == 32 ? launch_igemm_halo<32, 3>(p, hg, stream) : bn == 64 ? launch_igemm_halo<64, 3>(p, hg, stream) : launch_igemm_halo<128, 3>(p, hg, stream);
+        if (p.planes == 2) return bn == 32 ? launch_igemm_halo<32, 2>(p, hg, stream) : bn == 64 ? launch_igemm_halo<64, 2>(p, hg, stream) : launch_igemm_halo<128, 2>(p, hg, stream);
+        return bn == 32 ? launch_igemm_halo<32, 1>(p, hg, stream) : bn == 64 ? launch_igemm_halo<64, 1>(p, hg, stream) : launch_igemm_halo<128, 1>(p, hg, stream);
+    }
     if (p.planes == 3) return bn == 32 ? launch_igemm<32, 3>(p, stream) : bn == 64 ? launch_igemm<64, 3>(p, stream) : launch_igemm<128, 3>(p, stream);
     if (p.planes == 2) return bn == 32 ? launch_igemm<32, 2>(p, stream) : bn == 64 ? launch_igemm<64, 2>(p, stream) : launch_igemm<128, 2>(p, stream);
     return bn == 32 ? launch_igemm<32, 1>(p, stream) : bn == 64 ? launch_igemm<64, 1>(p, stream) : launch_igemm<128, 1>(p, stream);

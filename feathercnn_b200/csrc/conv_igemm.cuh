@@ -33,6 +33,11 @@ int conv_igemm_pack_weights(const float* w, float* w_hi, float* w_lo, int OC, in
                             int bf16x3 = 0);
 // True when the launch can apply a fused 2x2 / stride-2 max pooling (the 3x3 stride-1 slab kernel without a residual).
 bool conv_igemm_can_pool(const IgemmProblem& p);
+// Output patch (R x C pixels) and shared-memory halo box (Rb x Cb) of the halo kernel conv_igemm_forward uses for
+// stride-1, dense layers with IC % 32 == 0 and W % 4 == 0 (switch igemm_halo); false when the layer keeps the
+// gathering kernel.  Reads IC, OC, H, W, OH, OW, KH, KW, strides, dilation, planes and the input address.
+struct HaloGeom { int R, C, Rb, Cb; };
+bool conv_igemm_halo_geometry(const IgemmProblem& p, HaloGeom* g);
 int conv_igemm_forward(const IgemmProblem& p, cudaStream_t stream);
 
 }  // namespace fcuda

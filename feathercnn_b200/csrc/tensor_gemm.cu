@@ -228,6 +228,7 @@ struct TuneEntry { const char* name; const char* env; int def, lo, hi; int value
 TuneEntry g_tune[TUNE_COUNT] = {
     {"dw_vec", "FCUDA_DW_VEC", 1, 0, 1, 0, false},                   // vectorised depthwise kernel on wide planes
     {"wino_mlp", "FCUDA_WINO_MLP", 2, 0, 2, 0, false},               // Winograd transforms: slab copies / all plane loads in flight
+    {"igemm_halo", "FCUDA_IGEMM_HALO", 1, 0, 1, 0, false},           // implicit GEMM: TMA halo tiles + pipelined wgmma (stride 1)
 };
 }  // namespace
 const char* tune_name(int key) { return key >= 0 && key < TUNE_COUNT ? g_tune[key].name : nullptr; }

@@ -63,11 +63,42 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
     }
 }
 
+// The same bounded wait without a function call, for waits inside a running wgmma pipeline: ptxas serialises every
+// wgmma of a function whose pipeline crosses a call (the diagnostic's printf is one).  Traps silently.
+__device__ __forceinline__ void mbar_wait_nocall(uint64_t* bar, uint32_t parity) {
+    if (mbar_try_wait(bar, parity)) return;
+    long long t0 = 0;
+    for (uint32_t spins = 1; !mbar_try_wait(bar, parity); ++spins) {
+        if ((spins & 63u) == 0) {
+            const long long now = clock64();
+            if (t0 == 0) t0 = now;
+            else if (now - t0 > 4000000000LL) __trap();  // ~2 s at 2 GHz
+        }
+    }
+}
+// mbarrier arrive by the lanes with pred != 0, issued by the whole warp as one predicated instruction (no branch)
+__device__ __forceinline__ void mbar_arrive_if(uint64_t* bar, bool pred) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\t"
+        "setp.ne.b32 p, %1, 0;\n\t"
+        "@p mbarrier.arrive.shared::cta.b64 _, [%0];\n\t}"
+        ::"r"(smem_u32(bar)), "r"(static_cast<int>(pred))
+        : "memory");
+}
+
 __device__ __forceinline__ void tma_load_3d(void* smem_dst, const CUtensorMap* map, uint64_t* bar, int c0, int c1,
                                             int c2) {
     asm volatile(
         "cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];"
         ::"r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(map)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2)
+        : "memory");
+}
+__device__ __forceinline__ void tma_load_4d(void* smem_dst, const CUtensorMap* map, uint64_t* bar, int c0, int c1,
+                                            int c2, int c3) {
+    asm volatile(
+        "cp.async.bulk.tensor.4d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], [%2];"
+        ::"r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(map)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2),
+          "r"(c3)
         : "memory");
 }
 // 1-D bulk copy global -> shared (16-byte aligned, size a multiple of 16), completion on an mbarrier

@@ -167,6 +167,12 @@ int fcuda_conv_forward_residual(const FcudaConvParam* param, int algo, float* ou
  * says whether the algorithm can do it (Winograd F(6,3)/F(2,3): the output tile is pooled in registers; FCUDA_SGECONV:
  * 3x3 / stride-1 layers with IC % 32 == 0, pooled by two shuffles per value); otherwise the call returns -200. */
 int fcuda_conv_can_pool(const FcudaConvParam* param, int algo);
+
+/* FCUDA_SGECONV in the current arithmetic mode: 1 when the layer (output_h / output_w assigned) runs on the halo kernel
+ * (switch igemm_halo below: stride 1, no dilation, more than one tap, input_channels / group % 32 == 0, input_w % 4 == 0,
+ * 16-byte aligned input), with geom[0..3] = output patch rows, patch columns, shared-memory box rows, box columns;
+ * 0 when it keeps the gathering kernel.  The switch itself is not consulted. */
+int fcuda_igemm_halo_tile(const FcudaConvParam* param, int* geom);
 int fcuda_conv_forward_pool(const FcudaConvParam* param, int algo, float* output, const float* input,
                             const float* packed_kernel, float* scratch, const float* bias, int batch, void* stream);
 
@@ -200,6 +206,9 @@ int fcuda_conv_forward_ext(const FcudaConvParam* param, int algo, float* output,
  *   wino_mlp (0-2, 2)         Winograd transforms: 1 = every global load of a block in flight at once (cp.async slab /
  *                             back-to-back plane loads) instead of register-staged rounds; 2 = also launch the channel
  *                             blocks of a tile group next to each other (whole 1 KB rows of V / M in flight together)
+ *   igemm_halo (0-1, 1)       implicit GEMM on stride-1, dense layers with IC % 32 == 0 (per group) and W % 4 == 0: the
+ *                             input patch of 32 channels plus its halo arrives by one TMA load and serves every tap;
+ *                             persistent CTAs, split and MMA of neighbouring k-blocks overlap.  0 = the gathering kernel
  * Every variant computes the same result (tests/test_gpu_variants.py).  Returns 0 / the value, -200 for an unknown name or value. */
 int fcuda_set_tuning(const char* name, int value);
 int fcuda_get_tuning(const char* name);
