@@ -140,7 +140,7 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tmW, const __grid_constant
             }
             for (int kb = 0; kb < kblocks; ++kb) {
                 const int stage = kb % kStagesIg;
-                if (kb >= kStagesIg) ptx::mbar_wait(&empty_bar[stage], ((kb / kStagesIg) - 1) & 1);
+                if (kb >= kStagesIg) ptx::mbar_wait_nocall(&empty_bar[stage], ((kb / kStagesIg) - 1) & 1);
                 uint8_t* st = smem + stage * kStage;
                 ptx::mbar_arrive_expect_tx(&full_bar[stage], kStage);
                 if (BF) {
@@ -251,7 +251,7 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tmW, const __grid_constant
                 }
         }
         if (kb + 1 < kblocks) gather(kb + 1, raw);
-        ptx::mbar_wait(&full_bar[stage], (kb / kStagesIg) & 1);
+        ptx::mbar_wait_nocall(&full_bar[stage], (kb / kStagesIg) & 1);
         const uint32_t b_base = ptx::smem_u32(smem + stage * kStage);
         ptx::wgmma_fence();
         if (BF) {

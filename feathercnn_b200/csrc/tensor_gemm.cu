@@ -9,6 +9,9 @@
 //                 accumulators; then the fused store (row-major / NCHW+bias+ReLU / k-split partial planes).
 // A is ONE fp32 plane in HBM (the split happens on chip); full / empty mbarriers hand the ring slots over, and a bounded
 // wait traps instead of hanging the GPU.
+//
+// tensor_gemm_pipe_kernel<BN, PLANES> (switch gemm_pipe, the default) runs the same tiles and MMA sequence with
+// persistent CTAs and overlapped k-blocks; see its comment below.
 #include "tensor_gemm.cuh"
 #include "common.cuh"
 #include "wgmma.cuh"
@@ -196,6 +199,145 @@ tensor_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constan
     epilogue_store<BN>(args, acc, g, m_blk * kBM + row0, n_blk * BN, c, ks);
 }
 
+// tensor_gemm_pipe_kernel<BN, PLANES>: the same tiles, k-blocks, wgmma sequence and epilogue as tensor_gemm_kernel, so the
+// result is bit-identical to it, with
+//   - two A-fragment sets: k-block kb + 1 is read from the swizzled tile and split while kb's commit group runs
+//     (wgmma_wait<1>); a ring stage is released once the group that read its B planes retired;
+//   - call-free bounded waits: a call inside the pipeline would make ptxas serialise every wgmma;
+//   - persistent CTAs that walk the tile order with a static stride; the producer keeps a running k-block count across
+//     tiles, so it fills the next tile's stages while the consumers run the epilogue.
+struct TileCoord { int g, m_blk, n_blk, ks, kb0, nk; };
+
+__device__ __forceinline__ TileCoord tile_coord(const GemmKernelArgs& args, int tile) {
+    TileCoord t;
+    t.n_blk = tile % args.num_n;
+    const int t1 = tile / args.num_n;
+    t.m_blk = t1 % args.num_m;
+    const int t2 = t1 / args.num_m;
+    t.g = t2 % args.G;
+    t.ks = t2 / args.G;
+    const int kb_per_split = (args.k_blocks_total + args.split_k - 1) / args.split_k;
+    t.kb0 = t.ks * kb_per_split;
+    t.nk = min(t.kb0 + kb_per_split, args.k_blocks_total) - t.kb0;
+    return t;
+}
+
+template <int BN, int PLANES>
+__global__ void __launch_bounds__(kThreads, 1)
+tensor_gemm_pipe_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
+                        const __grid_constant__ CUtensorMap tmBlo, const GemmKernelArgs args, int tiles) {
+    constexpr int kATile = kBM * kBK * 4;
+    constexpr int kBTile = BN * kBK * 4;
+    constexpr int kStage = kATile + PLANES * kBTile;  // [A raw][B_hi][B_lo]
+    extern __shared__ uint8_t smem_raw[];
+    uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+    __shared__ uint64_t full_bar[kStages];
+    __shared__ uint64_t empty_bar[kStages];
+
+    const int warp = threadIdx.x >> 5;
+    const int lane = threadIdx.x & 31;
+
+    if (threadIdx.x == 0) {
+        for (int s = 0; s < kStages; ++s) {
+            ptx::mbar_init(&full_bar[s], 1);
+            ptx::mbar_init(&empty_bar[s], kConsumerWarps);
+        }
+        ptx::fence_barrier_init();
+    }
+    __syncthreads();
+
+    if (warp == kConsumerWarps) {
+        // ===================== TMA producer =====================
+        if (lane == 0) {
+            ptx::prefetch_tensormap(&tmA);
+            ptx::prefetch_tensormap(&tmB);
+            if (PLANES == 2) ptx::prefetch_tensormap(&tmBlo);
+            int kbg = 0;  // k-blocks issued by this CTA over all its tiles
+            for (int tile = blockIdx.x; tile < tiles; tile += gridDim.x) {
+                const TileCoord tc = tile_coord(args, tile);
+                for (int i = 0; i < tc.nk; ++i, ++kbg) {
+                    const int stage = kbg % kStages;
+                    if (kbg >= kStages) ptx::mbar_wait_nocall(&empty_bar[stage], ((kbg / kStages) - 1) & 1);
+                    uint8_t* st = smem + stage * kStage;
+                    const int kc = (tc.kb0 + i) * kBK;
+                    ptx::mbar_arrive_expect_tx(&full_bar[stage], kStage);
+                    ptx::tma_load_3d(st, &tmA, &full_bar[stage], kc, tc.m_blk * kBM, tc.g);
+                    ptx::tma_load_3d(st + kATile, &tmB, &full_bar[stage], kc, tc.n_blk * BN, tc.g);
+                    if (PLANES == 2) ptx::tma_load_3d(st + kATile + kBTile, &tmBlo, &full_bar[stage], kc, tc.n_blk * BN, tc.g);
+                }
+            }
+        }
+        return;
+    }
+
+    // ===================== consumers: two warpgroups of 64 rows =====================
+    const int gq = lane >> 2, c = lane & 3;
+    const int row0 = warp * 16 + gq;
+    int kbg = 0;  // k-blocks consumed by this CTA over all its tiles
+    for (int tile = blockIdx.x; tile < tiles; tile += gridDim.x) {
+        const TileCoord tc = tile_coord(args, tile);
+        float acc[BN / 2];
+#pragma unroll
+        for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+        uint32_t fa1[4][4], fa2[4][4], fb1[4][4], fb2[4][4];  // two fragment sets: [k-step][a0..a3], hi and lo
+
+        auto step = [&](uint32_t (&f1)[4][4], uint32_t (&f2)[4][4], int i) {
+            const int stage = kbg % kStages;
+            ptx::mbar_wait_nocall(&full_bar[stage], (kbg / kStages) & 1);
+            const uint32_t a_base = ptx::smem_u32(smem + stage * kStage);
+#pragma unroll
+            for (int kk = 0; kk < 4; ++kk) {
+#pragma unroll
+                for (int q = 0; q < 4; ++q) {  // as tensor_gemm_kernel
+                    const int row = row0 + 8 * (q & 1);
+                    const uint32_t chunk = static_cast<uint32_t>(2 * kk + (q >> 1)) ^ static_cast<uint32_t>(gq);
+                    float x;
+                    asm volatile("ld.shared.f32 %0, [%1];" : "=f"(x) : "r"(a_base + row * 128 + (chunk << 4) + c * 4));
+                    if (PLANES == 2) split_tf32_trunc(x, f1[kk][q], f2[kk][q]);
+                    else f1[kk][q] = __float_as_uint(x);
+                }
+            }
+            const uint64_t dB = make_smem_desc_sw128(a_base + kATile);
+            const uint64_t dBlo = make_smem_desc_sw128(a_base + kATile + kBTile);
+            ptx::wgmma_fence();
+#pragma unroll
+            for (int kk = 0; kk < 4; ++kk) {
+                if (PLANES == 2) {
+                    Wgmma<BN, 1>::mma(acc, f2[kk], dB + 2 * kk, 1u);    // A_lo * B_hi
+                    Wgmma<BN, 1>::mma(acc, f1[kk], dBlo + 2 * kk, 1u);  // A_hi * B_lo
+                    Wgmma<BN, 1>::mma(acc, f1[kk], dB + 2 * kk, 1u);    // A_hi * B_hi
+                } else {
+                    Wgmma<BN, 1>::mma(acc, f1[kk], dB + 2 * kk, 1u);
+                }
+            }
+            ptx::wgmma_commit();
+            ptx::wgmma_wait<1>();  // k-block i - 1 retired: its stage's B planes and its fragment set are free
+            __syncwarp();
+            ptx::mbar_arrive_if(&empty_bar[(kbg + kStages - 1) % kStages], i > 0 && lane == 0);
+            ++kbg;
+        };
+        // k-blocks in pairs, one per fragment set.  Both loop shapes issue the same sequence; ptxas keeps the wgmma
+        // pipelined only with the odd tail inside the loop for PLANES 2 (else C7512) and after it for PLANES 1 (else C7513).
+        if (PLANES == 2) {
+            for (int i = 0; i < tc.nk; i += 2) {
+                step(fa1, fa2, i);
+                if (i + 1 < tc.nk) step(fb1, fb2, i + 1);
+            }
+        } else {
+            int i = 0;
+            for (; i + 1 < tc.nk; i += 2) {
+                step(fa1, fa2, i);
+                step(fb1, fb2, i + 1);
+            }
+            if (i < tc.nk) step(fa1, fa2, i);
+        }
+        ptx::wgmma_wait<0>();
+        __syncwarp();
+        ptx::mbar_arrive_if(&empty_bar[(kbg - 1) % kStages], lane == 0);  // the producer refills it during the epilogue
+        epilogue_store<BN>(args, acc, tc.g, tc.m_blk * kBM + row0, tc.n_blk * BN, c, tc.ks);
+    }
+}
+
 // --------------------------------------------------------------------------------------------
 // Host side
 // --------------------------------------------------------------------------------------------
@@ -229,6 +371,7 @@ TuneEntry g_tune[TUNE_COUNT] = {
     {"dw_vec", "FCUDA_DW_VEC", 1, 0, 1, 0, false},                   // vectorised depthwise kernel on wide planes
     {"wino_mlp", "FCUDA_WINO_MLP", 2, 0, 2, 0, false},               // Winograd transforms: slab copies / all plane loads in flight
     {"igemm_halo", "FCUDA_IGEMM_HALO", 1, 0, 1, 0, false},           // implicit GEMM: TMA halo tiles + pipelined wgmma (stride 1)
+    {"gemm_pipe", "FCUDA_GEMM_PIPE", 1, 0, 1, 0, false},             // TensorGEMM: persistent CTAs + pipelined wgmma
 };
 }  // namespace
 const char* tune_name(int key) { return key >= 0 && key < TUNE_COUNT ? g_tune[key].name : nullptr; }
@@ -398,13 +541,24 @@ static int launch(const GemmProblem& p, cudaStream_t stream) {
     const long long total = static_cast<long long>(a.num_m) * a.num_n * a.G * a.split_k;
     if (total > 0x7fffffffLL) return -1;
     const int smem = kStages * kStage + 1024;
+    const bool pipe = tune_get(TUNE_GEMM_PIPE) != 0;
     auto kern = tensor_gemm_kernel<BN, PLANES>;
-    static SmemAttrCache attr_cache;
-    if (int rc2 = ensure_dynamic_smem(kern, smem, attr_cache)) return rc2;
+    auto pkern = tensor_gemm_pipe_kernel<BN, PLANES>;
+    static SmemAttrCache attr_cache, pattr_cache;
+    if (int rc2 = pipe ? ensure_dynamic_smem(pkern, smem, pattr_cache) : ensure_dynamic_smem(kern, smem, attr_cache))
+        return rc2;
+    unsigned grid = static_cast<unsigned>(total);
+    if (pipe) {  // persistent: at most one wave of CTAs
+        int per_sm = 0;
+        FCUDA_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, pkern, kThreads, smem));
+        const long long slots = static_cast<long long>(sm_count()) * (per_sm > 0 ? per_sm : 1);
+        grid = static_cast<unsigned>(total < slots ? total : slots);
+    }
     const double dense = 2.0 * p.M * static_cast<double>(p.N) * p.K * p.G;
     const int prof = prof_begin(stream, PROF_TENSOR_GEMM, p.algo_flops > 0 ? p.algo_flops : dense,
                                 dense * (PLANES == 2 ? 3.0 : 1.0), gemm_algo_bytes(p));
-    kern<<<static_cast<unsigned>(total), kThreads, smem, stream>>>(tmA, tmB, tmBlo, a);
+    if (pipe) pkern<<<grid, kThreads, smem, stream>>>(tmA, tmB, tmBlo, a, static_cast<int>(total));
+    else kern<<<grid, kThreads, smem, stream>>>(tmA, tmB, tmBlo, a);
     FCUDA_CHECK_LAUNCH();
     count_launch();
     prof_end(prof, stream);

@@ -209,6 +209,9 @@ int fcuda_conv_forward_ext(const FcudaConvParam* param, int algo, float* output,
  *   igemm_halo (0-1, 1)       implicit GEMM on stride-1, dense layers with IC % 32 == 0 (per group) and W % 4 == 0: the
  *                             input patch of 32 channels plus its halo arrives by one TMA load and serves every tap;
  *                             persistent CTAs, split and MMA of neighbouring k-blocks overlap.  0 = the gathering kernel
+ *   gemm_pipe (0-1, 1)        TensorGEMM (Winograd, im2col, InnerProduct): persistent CTAs that fill the next tile's ring
+ *                             stages during the epilogue; the split and MMAs of neighbouring k-blocks overlap and no wgmma
+ *                             waits for the one before it.  Bit-identical to 0 = one CTA per tile, drained per k-block
  * Every variant computes the same result (tests/test_gpu_variants.py).  Returns 0 / the value, -200 for an unknown name or value. */
 int fcuda_set_tuning(const char* name, int value);
 int fcuda_get_tuning(const char* name);
