@@ -139,6 +139,7 @@ def feather() -> ctypes.CDLL:
             "fnet_modelbin_load_mem": (ctypes.c_long, [ctypes.c_char_p, i, i, ctypes.POINTER(ctypes.c_float)]),
             "fnet_fuse_now": (i, [vp]),
             "fnet_layer_fused_away": (i, [vp, cp]),
+            "fnet_layer_conv_algo": (i, [vp, cp]),
             "fnet_input_name": (cp, [vp]),
             "fgroup_create": (vp, []),
             "fgroup_destroy": (None, [vp]),

@@ -42,6 +42,7 @@ long fnet_modelbin_load_mem(const unsigned char* buf, int w, int type, float* ou
 }
 int fnet_fuse_now(void* h) { return static_cast<Net*>(h)->FuseNow(); }
 int fnet_layer_fused_away(void* h, const char* name) { return static_cast<Net*>(h)->LayerFusedAway(name ? name : ""); }
+int fnet_layer_conv_algo(void* h, const char* name) { return static_cast<Net*>(h)->LayerConvAlgo(name ? name : ""); }
 void fnet_set_stream(void* h, void* stream) { static_cast<Net*>(h)->SetStream(stream); }
 int fnet_load_param(void* h, const char* path) { FNET_GUARD(static_cast<Net*>(h)->LoadParam(path)) }
 int fnet_load_param_text(void* h, const char* text) { FNET_GUARD(static_cast<Net*>(h)->LoadParamFromText(text)) }

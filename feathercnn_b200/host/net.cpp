@@ -591,6 +591,15 @@ int Net::LayerFusedAway(const std::string& layer_name) const {
     return -1;
 }
 
+int Net::LayerConvAlgo(const std::string& layer_name) const {
+    for (size_t i = 0; i < layers.size(); ++i) {
+        if (layers[i]->name != layer_name) continue;
+        const ConvLayer* conv = dynamic_cast<const ConvLayer*>(layers[i]);
+        return (conv && !conv->_fused_away) ? conv->algo() : -1;
+    }
+    return -1;
+}
+
 void Net::ResetGraph() {
     for (auto& kv : graph_cache_) cudaGraphExecDestroy(static_cast<cudaGraphExec_t>(kv.second));
     graph_cache_.clear();

@@ -162,6 +162,11 @@ class Net:
     def LayerFusedAway(self, layer_name: str) -> int:
         return int(self._lib.fnet_layer_fused_away(self._h, layer_name.encode()))
 
+    def LayerConvAlgo(self, layer_name: str) -> int:
+        """The FcudaConvAlgo a convolution layer runs (valid after a Forward); -1 for an unknown layer, a layer that is
+        not a convolution, or one fused away."""
+        return int(self._lib.fnet_layer_conv_algo(self._h, layer_name.encode()))
+
     def BlobNames(self) -> list[str]:
         need = self._lib.fnet_blob_names(self._h, None, 0)
         buf = ctypes.create_string_buffer(need)

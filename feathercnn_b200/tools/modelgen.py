@@ -10,6 +10,7 @@ that exercises every layer type.  Weight statistics follow SURVEY.md §8(d).
 """
 from __future__ import annotations
 
+import math
 import struct
 from pathlib import Path
 
@@ -17,8 +18,10 @@ import numpy as np
 
 
 class ModelWriter:
-    def __init__(self, seed: int = 0):
+    def __init__(self, seed: int = 0, wide_stats: bool = False):
         self.rng = np.random.default_rng(seed)
+        self.wide_stats = wide_stats       # BatchNorm / Scale statistics of _batchnorm_wide (default: mild, near identity)
+        self._bn_mul: dict[str, np.ndarray] = {}
         self.lines: list[str] = []
         self.blobs: set[str] = set()
         self.bin = bytearray()
@@ -93,9 +96,12 @@ class ModelWriter:
         self.flops += 2.0 * out * n_in
         return top
 
-    def batchnorm(self, name, bottom, top=None, eps=1e-5):
+    def batchnorm(self, name, bottom, top=None, eps=None):
         top = top or name
         c = self.shape[bottom][0]
+        if self.wide_stats:
+            return self._batchnorm_wide(name, bottom, top, c, 1e-3 if eps is None else eps)
+        eps = 1e-5 if eps is None else eps
         self._layer("BatchNorm", name, [bottom], [top], {0: c, 1: f"{eps:e}"})
         r = self.rng
         self._weights(r.uniform(0.9, 1.1, c).astype(np.float32), False)   # slope
@@ -105,13 +111,47 @@ class ModelWriter:
         self.shape[top] = self.shape[bottom]
         return top
 
+    def _batchnorm_wide(self, name, bottom, top, c, eps):
+        """Statistics under which a wrong BN / Scale fold is visible per element (wide_stats=True):
+        - the per-channel multiplier slope / sqrt(var + eps) is log-uniform over five decades, rescaled to RMS 1;
+        - about 10% of the multipliers are negative and one channel is dead (slope 0);
+        - eps defaults to 1e-3 and ceil(30%) of the channels have var <= eps, so dropping eps changes their multiplier by
+          >= sqrt(2);
+        - |mean| up to 2, so the offset bias - slope * mean / sqrt(var + eps) is O(1), not a small correction."""
+        r = self.rng
+        self._layer("BatchNorm", name, [bottom], [top], {0: c, 1: f"{eps:e}"})
+        var = eps * 10.0 ** r.uniform(1, 4, c)                     # 10 to 1e4 times eps ...
+        small = r.permutation(c)[:math.ceil(0.3 * c)]
+        var[small] = r.uniform(0.1, 1.0, small.size) * eps       # ... except on these channels
+        mul = 10.0 ** r.uniform(-2.5, 2.5, c) * np.where(r.random(c) < 0.1, -1.0, 1.0)
+        mul[r.integers(c)] = 0.0
+        mul /= np.sqrt(np.mean(mul ** 2))
+        var32 = var.astype(np.float32)
+        self._weights((mul * np.sqrt(var32.astype(np.float64) + eps)).astype(np.float32), False)  # slope
+        self._weights(r.uniform(-2, 2, c).astype(np.float32), False)   # mean
+        self._weights(var32, False)                                      # var
+        self._weights(r.uniform(-1, 1, c).astype(np.float32), False)   # bias
+        self._bn_mul[top] = mul
+        self.shape[top] = self.shape[bottom]
+        return top
+
     def scale(self, name, bottom, bias=True, top=None, center=1.0):
         top = top or name
         c = self.shape[bottom][0]
         self._layer("Scale", name, [bottom], [top], {0: c, 1: int(bias)})
-        self._weights((center * self.rng.uniform(0.9, 1.1, c)).astype(np.float32), False)
-        if bias:
-            self._weights(self.rng.uniform(-0.1, 0.1, c).astype(np.float32), False)
+        if self.wide_stats:
+            # a positive multiplier in [0.5, 2]; its product with the BatchNorm's is rescaled to RMS `center`
+            s = self.rng.uniform(0.5, 2.0, c)
+            prev = self._bn_mul.get(bottom)
+            if prev is not None and np.any(prev * s):
+                s *= center / np.sqrt(np.mean((prev * s) ** 2))
+            self._weights(s.astype(np.float32), False)
+            if bias:
+                self._weights(self.rng.uniform(-1, 1, c).astype(np.float32), False)
+        else:
+            self._weights((center * self.rng.uniform(0.9, 1.1, c)).astype(np.float32), False)
+            if bias:
+                self._weights(self.rng.uniform(-0.1, 0.1, c).astype(np.float32), False)
         self.shape[top] = self.shape[bottom]
         return top
 
@@ -191,9 +231,9 @@ def _bn_scale_relu(m: ModelWriter, tag: str, x: str, relu=True, center=1.0):
     return x
 
 
-def resnet50(seed=0, num_classes=1000, size=224) -> ModelWriter:
+def resnet50(seed=0, num_classes=1000, size=224, wide_stats=False) -> ModelWriter:
     """Caffe ResNet-50 layout: stride on the first 1x1 of each stage, BN/Scale/ReLU layers, Split/Eltwise."""
-    m = ModelWriter(seed)
+    m = ModelWriter(seed, wide_stats)
     x = m.input("data", 3, size, size)
     x = m.conv("conv1", x, 64, 7, 2, 3, True)
     x = _bn_scale_relu(m, "_conv1", x)
@@ -223,8 +263,8 @@ def resnet50(seed=0, num_classes=1000, size=224) -> ModelWriter:
     return m
 
 
-def mobilenet_v1(seed=0, num_classes=1000, size=224) -> ModelWriter:
-    m = ModelWriter(seed)
+def mobilenet_v1(seed=0, num_classes=1000, size=224, wide_stats=False) -> ModelWriter:
+    m = ModelWriter(seed, wide_stats)
     x = m.input("data", 3, size, size)
     x = m.conv("conv1", x, 32, 3, 2, 1, False)
     x = _bn_scale_relu(m, "_conv1", x)
@@ -242,9 +282,9 @@ def mobilenet_v1(seed=0, num_classes=1000, size=224) -> ModelWriter:
     return m
 
 
-def mini(seed=0, size=32, ch=16) -> ModelWriter:
+def mini(seed=0, size=32, ch=16, wide_stats=False) -> ModelWriter:
     """Small net touching every layer type (SURVEY.md §8c's 12-layer probe net, plus concat/dropout/depthwise)."""
-    m = ModelWriter(seed)
+    m = ModelWriter(seed, wide_stats)
     x = m.input("data", 4, size, size)
     x = m.conv("conv1", x, ch, 3, 1, 1, True)               # Winograd F63 eligible (size > 8, ch % 4 == 0)
     x = m.batchnorm("bn1", x); x = m.scale("scale1", x, True); x = m.relu("relu1", x)

@@ -93,6 +93,9 @@ public:
     // returns how many layers were absorbed into their producers.  LayerFusedAway: 1 / 0, -1 for an unknown layer.
     int FuseNow();
     int LayerFusedAway(const std::string& layer_name) const;
+    // The FcudaConvAlgo the convolution layer's booster holds (set by Reshape, so valid after a Forward); -1 for an
+    // unknown layer, a layer that is not a convolution, or a layer fused away.
+    int LayerConvAlgo(const std::string& layer_name) const;
 
 private:
     int ParseParamText(const char* text);

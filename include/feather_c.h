@@ -20,6 +20,8 @@ void fnet_set_cuda_graph(void* net, int enable);
 long fnet_modelbin_load_mem(const unsigned char* buf, int w, int type, float* out);
 int fnet_fuse_now(void* net);                                    /* run the fusion rewrite now; returns #layers absorbed */
 int fnet_layer_fused_away(void* net, const char* layer_name);    /* 1 / 0, -1 unknown layer */
+/* FcudaConvAlgo a convolution layer runs (after a Forward); -1: unknown layer, not a convolution, or fused away */
+int fnet_layer_conv_algo(void* net, const char* layer_name);
 void fnet_set_stream(void* net, void* cuda_stream);
 int fnet_load_param(void* net, const char* param_path);          /* Net::LoadParam, net.cpp:54-170 */
 int fnet_load_param_text(void* net, const char* param_text);     /* same grammar from memory */

@@ -516,6 +516,13 @@ def _fc_split(in_size, out_size, batch, mode) -> int:
     return rest // (batch * out_size)
 
 
+def ip_rule(in_size: int, mode: int) -> tuple[str, float]:
+    """(path, coef) of an InnerProduct with `in_size` inputs: the TensorGEMM when in_size % 4 == 0 (operands split per
+    mode), else the fp32 SIMT kernel; coef multiplies S = |b| + sum |x w|."""
+    path = "ip" if in_size % 4 == 0 else "simt"
+    return path, eps_for(path, mode) + in_size * U
+
+
 def run_inner_product(in_size, out_size, batch, relu, mode, seed=0):
     from feathercnn_b200 import booster
     booster.set_precision(mode)
@@ -530,8 +537,8 @@ def run_inner_product(in_size, out_size, batch, relu, mode, seed=0):
     if relu:
         ref = ref.clamp_min(0)
     s = x.double().abs() @ w.double().abs().T + b.double().abs()
-    path = "ip" if in_size % 4 == 0 else "simt"
-    used, rel = excess(got, ref, s, eps_for(path, mode) + in_size * U)
+    path, coef = ip_rule(in_size, mode)
+    used, rel = excess(got, ref, s, coef)
     _record(path, mode, rel, used)
     return used
 

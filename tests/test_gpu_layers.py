@@ -58,6 +58,16 @@ POOL_CASES = [
     (1, 3, 2, (0, 0, 0, 0), False, (8, 57, 64)),      # 3x3 s2 strip kernel, average, several strips
     (0, 3, 2, (0, 0, 0, 0), False, (4, 50, 50)),      # 3x3 s2 strip kernel, last window clipped in x and y (ceil mode)
     (1, 3, 2, (0, 0, 0, 0), False, (4, 50, 50)),      # same, average divides by the in-bounds count (pooling_layer.h:84)
+    (0, 3, 2, (0, 0, 0, 0), False, (3, 20, 46)),      # OW = 23: one below the strip kernel's dispatch boundary
+    (1, 3, 2, (0, 0, 0, 0), False, (3, 20, 46)),
+    (0, 3, 2, (0, 0, 0, 0), False, (3, 20, 48)),      # OW = 24: the smallest strip-kernel output
+    (1, 3, 2, (0, 0, 0, 0), False, (3, 20, 48)),
+    (1, 3, 2, (0, 0, 0, 0), False, (3, 21, 47)),      # odd H and W: generic kernel, windows end on the last row / column
+    (0, 3, 2, (0, 0, 0, 0), False, (3, 34, 64)),      # strip kernel, last row and column clipped in both axes
+    (1, 3, 2, (0, 0, 0, 0), False, (3, 34, 64)),
+    (1, 2, 2, (0, 0, 0, 0), False, (3, 10, 4)),       # 2x2 fast path, average, one output pair per row
+    (0, 2, 2, (0, 0, 0, 0), False, (2, 6, 256)),      # 2x2 fast path, 64 output pairs per row
+    (1, 2, 2, (0, 0, 0, 0), False, (2, 6, 256)),
 ]
 
 
