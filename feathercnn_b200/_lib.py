@@ -45,6 +45,15 @@ class FcudaConvParam(ctypes.Structure):
                                                                    ("activation", ctypes.c_int)]
 
 
+class FcudaDeconvParam(ctypes.Structure):
+    """include/fcuda.h FcudaDeconvParam (total channel counts; output_h / output_w filled by fcuda_deconv_output_dim)."""
+
+    _fields_ = [(n, ctypes.c_int) for n in (
+        "output_channels input_channels input_h input_w kernel_h kernel_w stride_h stride_w dilation_h dilation_w "
+        "pad_left pad_right pad_top pad_bottom output_pad_right output_pad_bottom group bias_term activation "
+        "output_h output_w").split()]
+
+
 def fcuda() -> ctypes.CDLL:
     global _fcuda
     if _fcuda is None:
@@ -52,7 +61,13 @@ def fcuda() -> ctypes.CDLL:
         vp, sz, i = ctypes.c_void_p, ctypes.c_size_t, ctypes.c_int
         P = ctypes.POINTER(FcudaConvParam)
         szp = ctypes.POINTER(ctypes.c_size_t)
+        D = ctypes.POINTER(FcudaDeconvParam)
         sigs = {
+            "fcuda_deconv_output_dim": (i, [D]),
+            "fcuda_deconv_plan": (i, [D, P, ctypes.POINTER(i)]),
+            "fcuda_deconv_get_buffer_size": (i, [D, i, szp, szp]),
+            "fcuda_deconv_init": (i, [D, vp, vp, vp]),
+            "fcuda_deconv_forward": (i, [D, vp, vp, vp, vp, vp, i, vp]),
             "fcuda_set_precision": (i, [i]),
             "fcuda_get_precision": (i, []),
             "fcuda_set_l2_chunk_bytes": (i, [sz]),

@@ -12,6 +12,7 @@ import ctypes
 import torch
 
 from ._lib import FcudaConvParam, fcuda
+from ._lib import FcudaDeconvParam as DeconvParam
 
 NAIVE, IM2COL, SGECONV, DEPTHWISE, WINOGRADF63, WINOGRADF63FUSED, WINOGRADF23 = range(7)
 ALGO_NAMES = ["NAIVE", "IM2COL", "SGECONV", "DEPTHWISE", "WINOGRADF63", "WINOGRADF63FUSED", "WINOGRADF23"]
@@ -160,6 +161,56 @@ def conv_forward(param: ConvParam, x: torch.Tensor, w: torch.Tensor, b: torch.Te
     else:
         cb.ForwardResidual(param, out, x.contiguous(), packed, scratch, b, residual.contiguous(), relu_after_add, n)
     return out, cb.algo
+
+
+# ---- deconvolution ---------------------------------------------------------------------------------
+def _hw(v) -> tuple[int, int]:
+    return (int(v), int(v)) if isinstance(v, int) else (int(v[0]), int(v[1]))
+
+
+def deconv_param(oc: int, ic: int, h: int, w: int, kh: int, kw: int | None = None, stride=1, pad=0, output_pad=0,
+                 dilation=1, group: int = 1, bias: bool = True, relu: bool = False) -> DeconvParam:
+    """FcudaDeconvParam with output_h / output_w filled.  stride, dilation and output_pad are an int or (h, w);
+    pad is an int or (top, bottom, left, right)."""
+    kw = kh if kw is None else kw
+    sh, sw = _hw(stride)
+    dh, dw = _hw(dilation)
+    oph, opw = _hw(output_pad)
+    pt, pb, pl, pr = (pad,) * 4 if isinstance(pad, int) else tuple(pad)
+    p = DeconvParam(output_channels=oc, input_channels=ic, input_h=h, input_w=w, kernel_h=kh, kernel_w=kw, stride_h=sh,
+                    stride_w=sw, dilation_h=dh, dilation_w=dw, pad_left=pl, pad_right=pr, pad_top=pt, pad_bottom=pb,
+                    output_pad_right=opw, output_pad_bottom=oph, group=group, bias_term=int(bool(bias)),
+                    activation=int(bool(relu)))
+    _check("fcuda_deconv_output_dim", fcuda().fcuda_deconv_output_dim(ctypes.byref(p)))
+    return p
+
+
+def deconv_plan(param: DeconvParam) -> tuple[FcudaConvParam, int]:
+    """The equivalent stride-1 convolution and the algorithm it runs with (DEPTHWISE: the direct gather kernel)."""
+    eq, algo = FcudaConvParam(), ctypes.c_int(-1)
+    _check("fcuda_deconv_plan", fcuda().fcuda_deconv_plan(ctypes.byref(param), ctypes.byref(eq), ctypes.byref(algo)))
+    return eq, algo.value
+
+
+def deconv_forward(x: torch.Tensor, w: torch.Tensor, b: torch.Tensor | None = None, stride=1, pad=0, output_pad=0,
+                   dilation=1, group: int = 1, relu: bool = False) -> tuple[torch.Tensor, int]:
+    """ncnn Deconvolution of x (N, IC, H, W) with w (OC, IC/group, KH, KW), not flipped.  Returns (output, conv_algo)."""
+    n, ic, h, wd = x.shape
+    oc, _, kh, kw = w.shape
+    p = deconv_param(oc, ic, h, wd, kh, kw, stride, pad, output_pad, dilation, group, b is not None, relu)
+    _, algo = deconv_plan(p)
+    lib = fcuda()
+    s, k = ctypes.c_size_t(0), ctypes.c_size_t(0)
+    _check("fcuda_deconv_get_buffer_size", lib.fcuda_deconv_get_buffer_size(ctypes.byref(p), n, ctypes.byref(s), ctypes.byref(k)))
+    packed = torch.empty(max(k.value, 1), device=x.device, dtype=torch.float32)
+    scratch = torch.empty(max(s.value, 1), device=x.device, dtype=torch.float32)
+    w = w.contiguous()
+    _check("fcuda_deconv_init", lib.fcuda_deconv_init(ctypes.byref(p), _ptr(packed), ctypes.c_void_p(w.data_ptr()), _stream()))
+    out = torch.empty((n, oc, p.output_h, p.output_w), device=x.device, dtype=torch.float32)
+    _check("fcuda_deconv_forward",
+           lib.fcuda_deconv_forward(ctypes.byref(p), _ptr(out), _ptr(x.contiguous()), _ptr(packed), _ptr(scratch), _ptr(b), n,
+                                    _stream()))
+    return out, algo
 
 
 # ---- other layer entry points (thin wrappers used by the parity tests) ------------------------------

@@ -1,5 +1,5 @@
 // Built-in layer registrations: the 13 ncnn type names the reference serves (/root/reference/src/layer_factory.cpp:53-68)
-// mapped onto this host's layer classes.  A table of {type name, factory} pairs instead of one macro line per layer; the
+// plus Deconvolution / DeconvolutionDepthWise, 15 in all, mapped onto this host's layer classes.  A table of {type name, factory} pairs instead of one macro line per layer; the
 // DEFINE_LAYER_CREATOR / REGISTER_LAYER_CREATOR macros of <feather/layer_factory.h> remain the plugin API for user layers.
 #include <feather/layer_factory.h>
 
@@ -7,6 +7,7 @@
 
 #include "layers/batchnorm_layer.h"
 #include "layers/conv_layer.h"
+#include "layers/deconv_layer.h"
 #include "layers/eltwise_layer.h"
 #include "layers/inner_product_layer.h"
 #include "layers/misc_layers.h"
@@ -29,7 +30,8 @@ struct BuiltIn {
     LayerRegistry::Creator create;
 };
 
-// "Convolution" and "ConvolutionDepthWise" share one class: group == channels selects the depthwise algorithm.
+// "Convolution" and "ConvolutionDepthWise" share one class: group == channels selects the depthwise algorithm; so do
+// "Deconvolution" and "DeconvolutionDepthWise".
 const BuiltIn kBuiltIns[] = {
     {"Input", make_layer<InputLayer>},
     {"Convolution", make_layer<ConvLayer>},
@@ -44,6 +46,8 @@ const BuiltIn kBuiltIns[] = {
     {"Dropout", make_layer<DropoutLayer>},
     {"Split", make_layer<SplitLayer>},
     {"Concat", make_layer<ConcatLayer>},
+    {"Deconvolution", make_layer<DeconvLayer>},
+    {"DeconvolutionDepthWise", make_layer<DeconvLayer>},
 };
 
 }  // namespace

@@ -7,7 +7,7 @@ models saved by Caffe carry the full layer definitions next to the weights) with
 no caffe / protobuf-generated code is needed — and writes the ncnn text ``.param`` + ``.bin`` the loader expects:
 
 * layer grammar and parameter ids as ``ConvLayer::LoadParam`` & co. read them (``src/layers/*.h``; ids follow ncnn's
-  caffe2ncnn): Convolution / ConvolutionDepthWise, InnerProduct, Pooling, ReLU, BatchNorm, Scale, Eltwise, Concat, Dropout,
+  caffe2ncnn): Convolution / ConvolutionDepthWise, Deconvolution / DeconvolutionDepthWise, InnerProduct, Pooling, ReLU, BatchNorm, Scale, Eltwise, Concat, Dropout,
   Softmax, Split, Input;
 * in-place Caffe layers (top == bottom) get a fresh blob name, and a blob read by several layers gets an explicit
   ``Split`` layer — the reference's Net looks blobs up by name and its layers own their tops (``net.cpp:112-160``);
@@ -214,6 +214,26 @@ def convert(caffemodel: bytes) -> tuple[str, bytes]:
             w = blobs[0]
             ltype = "ConvolutionDepthWise" if group > 1 else "Convolution"
             ps = f"0={num_output} 1={kw} 11={kh} 2={dil[0]} 3={sw} 13={sh} 4={pw} 14={ph} 5={bias} 6={w.size}"
+            if group > 1:
+                ps += f" 7={group}"
+            out.layer(ltype, name, bottoms, tops, ps)
+            out.weights(w, True)
+            if bias:
+                out.weights(blobs[1], False)
+        elif type_ == "Deconvolution":
+            # same convolution_param; Caffe's blob is (IC, OC/group, kh, kw), ncnn's [group][OC/group][IC/group][kh][kw]
+            p = parse_message(_first(L, 106, b""))
+            num_output = int(_first(p, 1, 0))
+            bias = int(_first(p, 2, 1))
+            kh, kw = _hw(p, 4, 11, 12, 1)
+            sh, sw = _hw(p, 6, 13, 14, 1)
+            ph, pw = _hw(p, 3, 9, 10, 0)
+            dil = _ints(p.get(18, [])) or [1]
+            group = int(_first(p, 5, 1))
+            ocg = num_output // group
+            w = blobs[0].reshape(group, -1, ocg, kh, kw).transpose(0, 2, 1, 3, 4)
+            ltype = "DeconvolutionDepthWise" if group > 1 else "Deconvolution"
+            ps = f"0={num_output} 1={kw} 11={kh} 2={dil[-1]} 12={dil[0]} 3={sw} 13={sh} 4={pw} 14={ph} 5={bias} 6={w.size}"
             if group > 1:
                 ps += f" 7={group}"
             out.layer(ltype, name, bottoms, tops, ps)

@@ -65,6 +65,29 @@ class ModelWriter:
         self.flops += 2.0 * oc * icg * oh * ow * k * k
         return top
 
+    def deconv(self, name, bottom, oc, k, stride=1, pad=0, bias=True, group=1, top=None, weights=None):
+        """ncnn Deconvolution (DeconvolutionDepthWise when group > 1): weights [group][oc/group][ic/group][k][k], He init
+        over the k*k/stride^2 taps that reach one output, or `weights` as given."""
+        top = top or name
+        ic, h, w = self.shape[bottom]
+        icg = ic // group
+        if weights is None:
+            std = np.sqrt(2.0 * stride * stride / (icg * k * k))
+            weights = self.rng.standard_normal((oc, icg, k, k)) * std
+        wts = np.ascontiguousarray(weights, np.float32)
+        assert wts.shape == (oc, icg, k, k), wts.shape
+        ltype = "DeconvolutionDepthWise" if group > 1 else "Deconvolution"
+        params = {0: oc, 1: k, 3: stride, 4: pad, 5: int(bias), 6: wts.size}
+        if group > 1:
+            params[7] = group
+        self._layer(ltype, name, [bottom], [top], params)
+        self._weights(wts, True)
+        if bias:
+            self._weights(self.rng.uniform(-0.1, 0.1, oc).astype(np.float32), False)
+        self.shape[top] = (oc, (h - 1) * stride + k - 2 * pad, (w - 1) * stride + k - 2 * pad)
+        self.flops += 2.0 * ic * (oc // group) * h * w * k * k
+        return top
+
     def relu(self, name, bottom, top=None):
         top = top or name
         self._layer("ReLU", name, [bottom], [top])
@@ -309,7 +332,36 @@ def mini(seed=0, size=32, ch=16, wide_stats=False) -> ModelWriter:
     return m
 
 
-ZOO = {"single_conv": single_conv, "vgg16": vgg16, "resnet50": resnet50, "mobilenet_v1": mobilenet_v1, "mini": mini}
+def bilinear_kernel(channels: int, k: int) -> np.ndarray:
+    """(channels, 1, k, k) bilinear upsampling filter, as Caffe's "bilinear" filler makes it (FCN's upsampling layers)."""
+    f = math.ceil(k / 2)
+    c = (2 * f - 1 - f % 2) / (2.0 * f)
+    t = 1 - np.abs(np.arange(k) / f - c)
+    return np.broadcast_to(np.outer(t, t), (channels, 1, k, k)).astype(np.float32)
+
+
+def decoder_tiny(seed=0, size=16, classes=4) -> ModelWriter:
+    """Encoder-decoder with a Split/Concat skip connection: learned upsampling by Deconvolution (k4 s2 p1 + BN + Scale +
+    ReLU, k2 s2 + ReLU), a 1x1 classifier and FCN's fixed bilinear DeconvolutionDepthWise (k4 s2 p1, no bias)."""
+    m = ModelWriter(seed)
+    x = m.input("data", 3, size, size)
+    x = m.conv("enc1", x, 16, 3, 1, 1, True)
+    x = m.relu("enc1_relu", x)
+    skip, x = m.split("enc1_split", x, ["skip", "down_in"])
+    x = m.conv("enc2", x, 32, 3, 2, 1, True)
+    x = m.relu("enc2_relu", x)
+    x = m.deconv("up1", x, 16, 4, 2, 1, True)
+    x = _bn_scale_relu(m, "_up1", x)
+    x = m.concat("cat1", [skip, x])
+    x = m.deconv("up2", x, 16, 2, 2, 0, True)
+    x = m.relu("up2_relu", x)
+    x = m.conv("score", x, classes, 1, 1, 0, True)
+    m.deconv("upscore", x, classes, 4, 2, 1, False, group=classes, weights=bilinear_kernel(classes, 4))
+    return m
+
+
+ZOO = {"single_conv": single_conv, "vgg16": vgg16, "resnet50": resnet50, "mobilenet_v1": mobilenet_v1, "mini": mini,
+       "decoder_tiny": decoder_tiny}
 
 
 def synthetic_input(shape, index: int = 0) -> np.ndarray:

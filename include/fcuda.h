@@ -200,6 +200,44 @@ int fcuda_conv_forward_ext(const FcudaConvParam* param, int algo, float* output,
                            const float* packed_kernel, float* scratch, const float* bias, const float* residual,
                            int relu_after_add, int dilation_h, int dilation_w, int batch, void* stream);
 
+/* ncnn's Deconvolution / DeconvolutionDepthWise (transposed convolution; the reference has no such layer).  Weights are
+ * (OC, IC/group, KH, KW) as ncnn stores them (group-major, not flipped); channel counts are TOTAL counts.  With
+ *   Hf = (H-1)*stride_h + dilation_h*(KH-1) + 1 + output_pad_bottom     (Wf likewise with output_pad_right)
+ *   full[n][oc][Y][X] = bias[oc] + sum of x[n][ic][i][j] * w[oc][ic - g0][ky][kx] over ic in oc's group and
+ *                       i*stride_h + ky*dilation_h = Y, j*stride_w + kx*dilation_w = X
+ * the output is act(full) cropped by the four pads: output_h = Hf - pad_top - pad_bottom (output_w likewise).
+ * Rejected with -200: a negative pad or output pad, activation other than none / ReLU, stride > 1 together with
+ * dilation > 1 in one direction, OC or IC not divisible by group.  -100 for empty sizes or an empty output.
+ * How it runs (fcuda_deconv_plan):
+ *   group == IC == OC > 1  a CUDA-core gather kernel, one output per thread, taps in ascending (ky, kx) order;
+ *   stride 1               the flipped filter as a stride-1 convolution (dilation kept) that writes the output directly
+ *                          with bias and ReLU, when every pad is <= dilation*(K-1) and output_pad <= the pad on its side;
+ *   otherwise              one stride-1 convolution with OC' = stride_h*stride_w*OC channels ordered
+ *                          (group, Y % stride_h, X % stride_w, oc in group) and kernel ceil(K/stride) (the sub-pixel
+ *                          phases of the filter), pads (kernel-1)*dilation, into scratch; then a scatter kernel adds the
+ *                          bias once, applies the ReLU and writes the cropped output. */
+typedef struct FcudaDeconvParam {
+    int output_channels, input_channels, input_h, input_w, kernel_h, kernel_w, stride_h, stride_w, dilation_h, dilation_w,
+        pad_left, pad_right, pad_top, pad_bottom, output_pad_right, output_pad_bottom, group, bias_term, activation,
+        output_h, output_w;
+} FcudaDeconvParam;
+/* Validates the parameters and fills output_h / output_w. */
+int fcuda_deconv_output_dim(FcudaDeconvParam* param);
+/* The equivalent convolution (output_h / output_w assigned) and the algorithm it runs with: fcuda_conv_select_algo_tuned,
+ * except FCUDA_SGECONV with dilation or with group > 1.  FCUDA_DEPTHWISE means the gather kernel; `equivalent` is then
+ * zeroed.  Either output pointer may be NULL. */
+int fcuda_deconv_plan(const FcudaDeconvParam* param, FcudaConvParam* equivalent, int* conv_algo);
+/* Scratch for `batch` images: the equivalent convolution's scratch (rounded up to 64 floats) plus
+ * batch * OC' * Hc * Wc floats for its output on the sub-pixel path; packed = the equivalent convolution's packed filter
+ * (IC*KH*KW floats for the gather kernel). */
+int fcuda_deconv_get_buffer_size(const FcudaDeconvParam* param, int batch, size_t* scratch_floats, size_t* packed_floats);
+/* Builds the equivalent filter from the raw weights (host or device pointer) and packs it like fcuda_conv_init.  Synchronous. */
+int fcuda_deconv_init(const FcudaDeconvParam* param, float* packed, const float* raw, void* stream);
+/* output (batch, OC, output_h, output_w) <- input (batch, IC, H, W).  `bias` is OC floats, or NULL when !bias_term.
+ * Allocates nothing and does not synchronise. */
+int fcuda_deconv_forward(const FcudaDeconvParam* param, float* output, const float* input, const float* packed,
+                         float* scratch, const float* bias, int batch, void* stream);
+
 /* Kernel-variant switches for A/B measurements and tests.  Defaults are the measured-best configuration; the environment
  * variable FCUDA_<NAME> sets the initial value.  Names (value range, default):
  *   dw_vec (0-1, 1)           vectorised depthwise kernel on wide planes
@@ -224,7 +262,7 @@ void fcuda_profile_tensor_gemm(int enable);
 int fcuda_profile_collect(double* total_ms, double* algo_flops, double* mma_flops, long long* launches);
 /* Same, per kernel class, for every instrumented launch (the enable switch above covers all of them):
  * kind 0 TensorGEMM, 1 implicit-GEMM conv, 2 Winograd input transform, 3 Winograd output transform, 4 pooling,
- * 5 depthwise, 6 element-wise (BN/Scale/Eltwise), < 0 all.  algo_bytes = the bytes the operation must move (inputs
+ * 5 depthwise, 6 element-wise (BN/Scale/Eltwise), 7 deconvolution scatter / depthwise gather, < 0 all.  algo_bytes = the bytes the operation must move (inputs
  * read once + outputs written once). */
 int fcuda_profile_collect_kind(int kind, double* total_ms, double* algo_flops, double* mma_flops, double* algo_bytes,
                                long long* launches);

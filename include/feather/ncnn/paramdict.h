@@ -9,7 +9,8 @@
 namespace ncnn {
 inline namespace b200 {  // ABI tag: keeps these symbols apart from the reference build when both are loaded
 
-#define NCNN_MAX_PARAM_COUNT 20
+// ncnn's own limit; Deconvolution's output_w / output_h are ids 20 / 21
+#define NCNN_MAX_PARAM_COUNT 32
 
 class ParamDict {
 public:
