@@ -81,6 +81,7 @@ def fcuda() -> ctypes.CDLL:
             "fcuda_conv_forward_residual": (i, [P, i, vp, vp, vp, vp, vp, vp, i, i, vp]),
             "fcuda_conv_can_pool": (i, [P, i]),
             "fcuda_igemm_halo_tile": (i, [P, ctypes.POINTER(i)]),
+            "fcuda_igemm_presplit_tile": (i, [P, ctypes.POINTER(i)]),
             "fcuda_conv_forward_pool": (i, [P, i, vp, vp, vp, vp, vp, i, vp]),
             "fcuda_conv_forward_ext": (i, [P, i, vp, vp, vp, vp, vp, vp, i, i, i, i, vp]),
             "fcuda_eltwise_forward": (i, [vp, vp, vp, sz, i, ctypes.c_float, ctypes.c_float, i, vp]),

@@ -503,7 +503,99 @@ struct HaloArgs {
     long long tiles;       // N * tiles_y * tiles_x * num_n
     const unsigned char* wbf;
     unsigned wbf_kb_bytes;
+    int pr, pc;            // conv_igemm_presplit_kernel: rows x columns of the bf16 planes (R + KH - 1, C + KW - 1)
 };
+
+// Epilogue of the halo kernels for one m64 accumulator (as conv_igemm_kernel): this thread's pixels are rows oy[0..1]
+// of column ox in image img.
+template <int BN>
+__device__ __forceinline__ void halo_epilogue(const float (&acc)[BN / 2], const HaloArgs& args, int n_blk, int img,
+                                              const int (&oy)[2], const bool (&valid)[2], int ox, int oplane, int SH,
+                                              int SW, int c, int gq) {
+#pragma unroll
+    for (int j = 0; j < BN / 8; ++j) {
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+            const int oc = n_blk * BN + 8 * j + 2 * c + e;
+            const bool oc_ok = oc < args.OC;
+            const float bv = (args.bias != nullptr && oc_ok) ? __ldg(args.bias + oc) : 0.f;
+            float v[2];
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+                v[h] = acc[4 * j + 2 * h + e] + bv;
+                const size_t o = (static_cast<size_t>(img) * args.out_img_c + oc) * oplane + static_cast<size_t>(oy[h]) * args.OW + ox;
+                if (args.residual != nullptr && valid[h] && oc_ok) v[h] += __ldg(args.residual + o);
+                if (args.relu) v[h] = fmaxf(v[h], 0.f);
+                if (!args.pool && valid[h] && oc_ok) args.out[o] = v[h];
+            }
+            if (args.pool) {
+                float m = fmaxf(valid[0] ? v[0] : -INFINITY, valid[1] ? v[1] : -INFINITY);
+                m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, 4));  // the window's other column: pixel gq ^ 1
+                if ((gq & 1) == 0 && valid[0] && oc_ok)
+                    args.out[(static_cast<size_t>(img) * args.out_img_c + oc) * (static_cast<size_t>(SH) * SW) +
+                             static_cast<size_t>(oy[0] >> 1) * SW + (ox >> 1)] = m;
+            }
+        }
+    }
+}
+
+// Producer warp of the halo kernels (lane 0 only): the HS-deep ring of input boxes and the filter ring, in consumption
+// order.  A tile is args.R x args.C output pixels; its box for channel block cb starts at (x0 - xpad, y0 - pad_top).
+template <int BN, int PLANES, int HS>
+__device__ __forceinline__ void halo_producer(const CUtensorMap* tmX, const CUtensorMap* tmW, const CUtensorMap* tmWlo,
+                                              const HaloArgs& args, uint8_t* smem, float* halo, int hstage,
+                                              uint64_t* full_bar, uint64_t* empty_bar, uint64_t* hfull_bar,
+                                              uint64_t* hempty_bar) {
+    constexpr bool BF = PLANES == 3;
+    constexpr int NPL = BF ? 2 : PLANES;
+    constexpr int kBTile = BN * 32 * (BF ? 2 : 4);
+    constexpr int kStage = NPL * kBTile;
+    const int per_img = args.tiles_x * args.tiles_y;
+    const int taps = args.taps;
+    const int ncb = args.kblocks / taps;
+    ptx::prefetch_tensormap(tmX);
+    if (!BF) {
+        ptx::prefetch_tensormap(tmW);
+        if (NPL == 2) ptx::prefetch_tensormap(tmWlo);
+    }
+    int hb = 0;   // boxes issued
+    int kbg = 0;  // filter stages issued
+    auto load_halo = [&](long long t, int cb) {
+        const long long pt = t / args.num_n;
+        const int n = static_cast<int>(pt / per_img);
+        const int rem = static_cast<int>(pt - static_cast<long long>(n) * per_img);
+        const int ty = rem / args.tiles_x, tx = rem - ty * args.tiles_x;
+        const int hs = hb % HS;
+        if (hb >= HS) ptx::mbar_wait_nocall(&hempty_bar[hs], ((hb / HS) - 1) & 1);
+        ptx::mbar_arrive_expect_tx(&hfull_bar[hs], static_cast<uint32_t>(hstage) * 4u);
+        ptx::tma_load_4d(halo + hs * hstage, tmX, &hfull_bar[hs], tx * args.C - args.xpad, ty * args.R - args.pad_top,
+                         cb * 32, n);
+        ++hb;
+    };
+    if (blockIdx.x < args.tiles) load_halo(blockIdx.x, 0);
+    for (long long t = blockIdx.x; t < args.tiles; t += gridDim.x) {
+        const int n_blk = static_cast<int>(t % args.num_n);
+        for (int cb = 0, kb = 0; cb < ncb; ++cb) {
+            for (int tap = 0; tap < taps; ++tap, ++kb, ++kbg) {
+                const int stage = kbg % kStagesIg;
+                if (kbg >= kStagesIg) ptx::mbar_wait_nocall(&empty_bar[stage], ((kbg / kStagesIg) - 1) & 1);
+                uint8_t* st = smem + stage * kStage;
+                ptx::mbar_arrive_expect_tx(&full_bar[stage], kStage);
+                if (BF) {
+                    ptx::bulk_load_1d(st, args.wbf + static_cast<size_t>(kb) * args.wbf_kb_bytes + static_cast<size_t>(n_blk) * kStage,
+                                      kStage, &full_bar[stage]);
+                } else {
+                    ptx::tma_load_3d(st, tmW, &full_bar[stage], kb * 32, n_blk * BN, 0);
+                    if (NPL == 2) ptx::tma_load_3d(st + kBTile, tmWlo, &full_bar[stage], kb * 32, n_blk * BN, 0);
+                }
+                if (tap == 0) {  // the next box (this tile's next channel block or the next tile's first) lands meanwhile
+                    if (cb + 1 < ncb) load_halo(t, cb + 1);
+                    else if (t + gridDim.x < args.tiles) load_halo(t + gridDim.x, 0);
+                }
+            }
+        }
+    }
+}
 
 template <int BN, int PLANES>
 __global__ void __launch_bounds__(kThreadsIg, 1)
@@ -528,7 +620,6 @@ conv_igemm_halo_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_con
     const int lane = threadIdx.x & 31;
     const int per_img = args.tiles_x * args.tiles_y;
     const int kblocks = args.kblocks, taps = args.taps;
-    const int ncb = kblocks / taps;
 
     if (threadIdx.x == 0) {
         for (int s = 0; s < kStagesIg; ++s) {
@@ -545,50 +636,9 @@ conv_igemm_halo_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_con
 
     if (warp == kConsumerWarps) {
         // ===================== producer: halo boxes + filters, in consumption order =====================
-        if (lane == 0) {
-            ptx::prefetch_tensormap(&tmX);
-            if (!BF) {
-                ptx::prefetch_tensormap(&tmW);
-                if (NPL == 2) ptx::prefetch_tensormap(&tmWlo);
-            }
-            int hb = 0;   // boxes issued
-            int kbg = 0;  // filter stages issued
-            auto load_halo = [&](long long t, int cb) {
-                const long long pt = t / args.num_n;
-                const int n = static_cast<int>(pt / per_img);
-                const int rem = static_cast<int>(pt - static_cast<long long>(n) * per_img);
-                const int ty = rem / args.tiles_x, tx = rem - ty * args.tiles_x;
-                const int hs = hb % kHaloStages;
-                if (hb >= kHaloStages) ptx::mbar_wait_nocall(&hempty_bar[hs], ((hb / kHaloStages) - 1) & 1);
-                ptx::mbar_arrive_expect_tx(&hfull_bar[hs], static_cast<uint32_t>(hstage) * 4u);
-                ptx::tma_load_4d(const_cast<float*>(halo) + hs * hstage, &tmX, &hfull_bar[hs], tx * args.C - args.xpad,
-                                 ty * args.R - args.pad_top, cb * 32, n);
-                ++hb;
-            };
-            if (blockIdx.x < args.tiles) load_halo(blockIdx.x, 0);
-            for (long long t = blockIdx.x; t < args.tiles; t += gridDim.x) {
-                const int n_blk = static_cast<int>(t % args.num_n);
-                for (int cb = 0, kb = 0; cb < ncb; ++cb) {
-                    for (int tap = 0; tap < taps; ++tap, ++kb, ++kbg) {
-                        const int stage = kbg % kStagesIg;
-                        if (kbg >= kStagesIg) ptx::mbar_wait_nocall(&empty_bar[stage], ((kbg / kStagesIg) - 1) & 1);
-                        uint8_t* st = smem + stage * kStage;
-                        ptx::mbar_arrive_expect_tx(&full_bar[stage], kStage);
-                        if (BF) {
-                            ptx::bulk_load_1d(st, args.wbf + static_cast<size_t>(kb) * args.wbf_kb_bytes + static_cast<size_t>(n_blk) * kStage,
-                                              kStage, &full_bar[stage]);
-                        } else {
-                            ptx::tma_load_3d(st, &tmW, &full_bar[stage], kb * 32, n_blk * BN, 0);
-                            if (NPL == 2) ptx::tma_load_3d(st + kBTile, &tmWlo, &full_bar[stage], kb * 32, n_blk * BN, 0);
-                        }
-                        if (tap == 0) {  // the next box (this tile's next channel block or the next tile's first) lands meanwhile
-                            if (cb + 1 < ncb) load_halo(t, cb + 1);
-                            else if (t + gridDim.x < args.tiles) load_halo(t + gridDim.x, 0);
-                        }
-                    }
-                }
-            }
-        }
+        if (lane == 0)
+            halo_producer<BN, PLANES, kHaloStages>(&tmX, &tmW, &tmWlo, args, smem, const_cast<float*>(halo), hstage, full_bar,
+                                                   empty_bar, hfull_bar, hempty_bar);
         return;
     }
 
@@ -710,33 +760,196 @@ conv_igemm_halo_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_con
         ptx::wgmma_wait<0>();
         __syncwarp();
         ptx::mbar_arrive_if(&empty_bar[(kbg - 1) % kStagesIg], lane == 0);
+        halo_epilogue<BN>(acc, args, n_blk, img, oy, valid, ox, oplane, SH, SW, c, gq);
+    }
+}
 
-        // ===================== epilogue (as conv_igemm_kernel) =====================
+// Pre-split halo kernel (BF16x3, switch igemm_presplit): the producer and the filter ring of conv_igemm_halo_kernel, but
+// each 32-channel fp32 box is split ONCE, not once per tap.
+//   split      = when a box lands, the 256 consumer threads convert it (split_bf16x2, the same bits as the per-tap split)
+//                into two bf16 planes p1 / p2, [ch / 8][R + KH - 1 rows][C + KW - 1 columns][8 ch]: a pixel's 8 channels
+//                are one 16-byte row.  The fp32 box goes back to the producer as soon as the conversion has read it; the
+//                planes are double-buffered, so box b + 1 is converted (during the last k-block of box b, behind its
+//                MMAs) while warps still read box b, and one named barrier of the consumers per box suffices.
+//   A operand  = per k-block and warp 4 ldmatrix.x4 (2 k-steps x 2 planes): the 8 rows of each 8 x 8 matrix are
+//                8 consecutive pixels of one patch row, so every tap (dy, dx) is the row address + (dy * pc + dx) * 16
+//                bytes, 16-byte aligned and free of bank conflicts.  ldmatrix yields the m16n8k16 A layout of wgmma.
+//   tile       = the halo kernel's 128-pixel patch.  A 256-pixel tile (two m64 accumulators per warpgroup) would halve
+//                the filter bytes per output where BN = 64, but a 288-thread CTA gets at most 168 registers per thread
+//                and the second accumulator and fragment sets do not fit: ptxas then serialises the wgmma.
+// Per k-block the wgmma sequence (p2*q1, p1*q2, p1*q1 per k-step), the operand values, the k order and BN are those of conv_igemm_halo_kernel<BN, 3>: the result is bit-identical to it.
+template <int BN>
+__global__ void __launch_bounds__(kThreadsIg, 1)
+conv_igemm_presplit_kernel(const __grid_constant__ CUtensorMap tmX, const HaloArgs args) {
+    constexpr int kBTile = BN * 32 * 2;
+    constexpr int kStage = 2 * kBTile;
+    constexpr int HS = kHaloStages;  // fp32 boxes in flight
+    constexpr int kConsumers = kConsumerWarps * 32;
+    extern __shared__ uint8_t smem_raw[];
+    uint8_t* smem = smem_raw + ((1024u - (ptx::smem_u32(smem_raw) & 1023u)) & 1023u);
+    float* halo = reinterpret_cast<float*>(smem + kStagesIg * kStage);
+    const int cstride = args.Rb * args.Cb;
+    const int hstage = 32 * cstride;
+    const int units = 4 * args.pr * args.pc;  // 16-byte rows per bf16 plane
+    const uint32_t pbytes = 16u * static_cast<uint32_t>(units);
+    // [buffer 2][p1, p2][units][16 B], then the box word offset of every unit
+    const uint32_t planes = ptx::smem_u32(halo + HS * hstage);
+    const int* utab = reinterpret_cast<const int*>(smem + kStagesIg * kStage + HS * hstage * 4 + 4 * pbytes);
+    __shared__ uint64_t full_bar[kStagesIg];
+    __shared__ uint64_t empty_bar[kStagesIg];
+    __shared__ uint64_t hfull_bar[HS];
+    __shared__ uint64_t hempty_bar[HS];
+
+    const int warp = threadIdx.x >> 5;
+    const int lane = threadIdx.x & 31;
+    const int per_img = args.tiles_x * args.tiles_y;
+    const int taps = args.taps, KW = args.KW;
+    const int ncb = args.kblocks / taps;
+
+    if (threadIdx.x == 0) {
+        for (int s = 0; s < kStagesIg; ++s) {
+            ptx::mbar_init(&full_bar[s], 1);
+            ptx::mbar_init(&empty_bar[s], kConsumerWarps);
+        }
+        for (int s = 0; s < HS; ++s) {
+            ptx::mbar_init(&hfull_bar[s], 1);
+            ptx::mbar_init(&hempty_bar[s], kConsumerWarps);
+        }
+        ptx::fence_barrier_init();
+    }
+    for (int u = threadIdx.x; u < units; u += kThreadsIg) {
+        const int ch8 = u / (args.pr * args.pc), rem = u - ch8 * args.pr * args.pc;
+        const int row = rem / args.pc, col = rem - row * args.pc;
+        const_cast<int*>(utab)[u] = 8 * ch8 * cstride + row * args.Cb + col + args.xshift;
+    }
+    __syncthreads();
+
+    if (warp == kConsumerWarps) {
+        if (lane == 0)
+            halo_producer<BN, 3, HS>(&tmX, nullptr, nullptr, args, smem, halo, hstage, full_bar, empty_bar, hfull_bar,
+                                     hempty_bar);
+        return;
+    }
+
+    // ===================== consumers =====================
+    const int gq = lane >> 2, c = lane & 3;
+    const int wcols = args.C >> 3;
+    const int wy = warp / wcols, wx = warp - wy * wcols;
+    const int prow = 2 * wy, pcol = 8 * wx + gq;     // this thread's pixels in each patch: rows prow + h, column pcol
+    // ldmatrix row of this lane: matrix lane / 8 = (channels 8-15 of the k-step) * 2 + (pixel row prow + 1), its row
+    // lane % 8 = patch column 8 * wx + lane % 8
+    const int lm = lane >> 3;
+    const uint32_t lrow = planes + 16u * static_cast<uint32_t>(((lm >> 1) * args.pr + prow + (lm & 1)) * args.pc + 8 * wx + (lane & 7));
+    const uint32_t kstep_bytes = pbytes / 2;                                   // channels 16-31 of the block
+
+    int hb = 0;   // boxes converted
+    int kbg = 0;  // filter stages consumed
+    // split box hb into plane buffer hb & 1 and hand the fp32 box back
+    auto convert_next = [&]() {
+        const int hs = hb % HS;
+        ptx::mbar_wait_nocall(&hfull_bar[hs], (hb / HS) & 1);
+        const float* box = halo + hs * hstage;
+        const uint32_t dst = planes + static_cast<uint32_t>(hb & 1) * 2u * pbytes;
+        for (int u = threadIdx.x; u < units; u += kConsumers) {
+            const float* s = box + utab[u];
+            float x[8];
 #pragma unroll
-        for (int j = 0; j < BN / 8; ++j) {
+            for (int i = 0; i < 8; ++i) x[i] = s[i * cstride];
+            uint32_t p1[4], p2[4];
 #pragma unroll
-            for (int e = 0; e < 2; ++e) {
-                const int oc = n_blk * BN + 8 * j + 2 * c + e;
-                const bool oc_ok = oc < args.OC;
-                const float bv = (args.bias != nullptr && oc_ok) ? __ldg(args.bias + oc) : 0.f;
-                float v[2];
+            for (int w = 0; w < 4; ++w) split_bf16x2(x[2 * w], x[2 * w + 1], p1[w], p2[w]);
+            ptx::st_shared_v4(dst + 16u * u, p1);
+            ptx::st_shared_v4(dst + pbytes + 16u * u, p2);
+        }
+        __syncwarp();
+        ptx::mbar_arrive_if(&hempty_bar[hs], lane == 0);
+        ++hb;
+    };
+
+    const int oplane = args.OH * args.OW;
+    const int SH = (args.OH + 1) >> 1, SW = (args.OW + 1) >> 1;
+    convert_next();  // grid <= tiles: every CTA has a first box
+    for (long long t = blockIdx.x; t < args.tiles; t += gridDim.x) {
+        const int n_blk = static_cast<int>(t % args.num_n);
+        const long long pt = t / args.num_n;
+        const int img = static_cast<int>(pt / per_img);
+        const int rem = static_cast<int>(pt - static_cast<long long>(img) * per_img);
+        const int ty = rem / args.tiles_x, tx = rem - ty * args.tiles_x;
+        const bool more_tiles = t + gridDim.x < args.tiles;
+        const int kbg0 = kbg;
+
+        float acc[BN / 2];
 #pragma unroll
-                for (int h = 0; h < 2; ++h) {
-                    v[h] = acc[4 * j + 2 * h + e] + bv;
-                    const size_t o = (static_cast<size_t>(img) * args.out_img_c + oc) * oplane + static_cast<size_t>(oy[h]) * args.OW + ox;
-                    if (args.residual != nullptr && valid[h] && oc_ok) v[h] += __ldg(args.residual + o);
-                    if (args.relu) v[h] = fmaxf(v[h], 0.f);
-                    if (!args.pool && valid[h] && oc_ok) args.out[o] = v[h];
-                }
-                if (args.pool) {
-                    float m = fmaxf(valid[0] ? v[0] : -INFINITY, valid[1] ? v[1] : -INFINITY);
-                    m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, 4));  // the window's other column: pixel gq ^ 1
-                    if ((gq & 1) == 0 && valid[0] && oc_ok)
-                        args.out[(static_cast<size_t>(img) * args.out_img_c + oc) * (static_cast<size_t>(SH) * SW) +
-                                 static_cast<size_t>(oy[0] >> 1) * SW + (ox >> 1)] = m;
-                }
+        for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+        uint32_t fa1[2][4], fa2[2][4], fb1[2][4], fb2[2][4], fc1[2][4], fc2[2][4];  // fragment sets: [k-step][a0..a3], p1 / p2
+        uint32_t abuf = 0, toff = 0;  // ldmatrix row of the current box's buffer, byte offset of the current tap
+        int dx = 0;
+
+        // one k-block: fragments by ldmatrix, then the MMAs; `last` = the box's last k-block, behind whose MMAs the next
+        // box is split (when there is one)
+        auto step = [&](uint32_t (&f1)[2][4], uint32_t (&f2)[2][4], bool last, bool next) {
+#pragma unroll
+            for (int kk = 0; kk < 2; ++kk) {
+                const uint32_t a = abuf + toff + kk * kstep_bytes;
+                ptx::ldsm_x4(a, f1[kk]);
+                ptx::ldsm_x4(a + pbytes, f2[kk]);
+            }
+            toff += 16;
+            if (++dx == KW) {
+                dx = 0;
+                toff += 16u * static_cast<uint32_t>(args.pc - KW);
+            }
+            const int stage = kbg & (kStagesIg - 1);
+            ptx::mbar_wait_nocall(&full_bar[stage], (kbg / kStagesIg) & 1);
+            const uint32_t b_base = ptx::smem_u32(smem) + stage * kStage;
+            ptx::wgmma_fence();
+            const uint64_t dQ1 = make_smem_desc_none(b_base, 128, 512);
+            const uint64_t dQ2 = make_smem_desc_none(b_base + kBTile, 128, 512);
+#pragma unroll
+            for (int kk = 0; kk < 2; ++kk) {
+                Wgmma<BN, 0>::mma(acc, f2[kk], dQ1 + 16 * kk, 1u);  // p2 * q1
+                Wgmma<BN, 0>::mma(acc, f1[kk], dQ2 + 16 * kk, 1u);  // p1 * q2
+                Wgmma<BN, 0>::mma(acc, f1[kk], dQ1 + 16 * kk, 1u);  // p1 * q1
+            }
+            ptx::wgmma_commit();
+            ptx::wgmma_wait<1>();  // k-block kbg - 1 retired: its filter stage and fragment set are free
+            if (last && next) convert_next();
+            __syncwarp();
+            ptx::mbar_arrive_if(&empty_bar[(kbg + kStagesIg - 1) & (kStagesIg - 1)], kbg != kbg0 && lane == 0);
+            ++kbg;
+        };
+        for (int cb = 0; cb < ncb; ++cb) {
+            ptx::named_bar_sync(1, kConsumers);  // every consumer has split this box and left the buffer it overwrote
+            abuf = lrow + static_cast<uint32_t>((hb - 1) & 1) * 2u * pbytes;
+            toff = 0;
+            dx = 0;
+            const bool next = cb + 1 < ncb || more_tiles;
+            // fragment sets a, b alternate; an odd box ends on set c, so the next box starts on a free set a either way
+            int i = 0;
+            for (; i + 2 < taps; i += 2) {
+                step(fa1, fa2, false, false);
+                step(fb1, fb2, false, false);
+            }
+            if (i + 1 < taps) {
+                step(fa1, fa2, false, false);
+                step(fb1, fb2, true, next);
+            } else {
+                step(fc1, fc2, true, next);
             }
         }
+        ptx::wgmma_wait<0>();
+        __syncwarp();
+        ptx::mbar_arrive_if(&empty_bar[(kbg - 1) & (kStagesIg - 1)], lane == 0);
+
+        const int ox = tx * args.C + pcol;
+        int oy[2];
+        bool valid[2];
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+            oy[h] = ty * args.R + prow + h;
+            valid[h] = oy[h] < args.OH && ox < args.OW;
+        }
+        halo_epilogue<BN>(acc, args, n_blk, img, oy, valid, ox, oplane, SH, SW, c, gq);
     }
 }
 
@@ -786,6 +999,99 @@ static bool halo_geometry(const IgemmProblem& p, HaloGeom& g) {
     return best >= 0;
 }
 
+// Box of conv_igemm_presplit_kernel for a layer the halo kernel takes in BF16x3 mode, or false (the layer keeps the
+// halo kernel).  The patch is the halo kernel's; the box is the patch plus its halo, unpadded: the split reads it along
+// rows, free of bank conflicts at any plane stride.
+static int presplit_smem_bytes(int OC, int Rb, int Cb, int pr, int pc) {
+    const int units = 4 * pr * pc;
+    return kStagesIg * 2 * igemm_bn_for(OC) * 64 + kHaloStages * 32 * Rb * Cb * 4 + 2 * 32 * units + 4 * units + 1024;
+}
+
+static bool presplit_geometry(const IgemmProblem& p, HaloGeom& g) {
+    HaloGeom h;
+    if (p.planes != 3 || !halo_geometry(p, h)) return false;
+    const int xshift = ((p.pad_left + 3) & ~3) - p.pad_left;
+    g.R = h.R; g.C = h.C;
+    g.Rb = h.R + p.KH - 1;
+    g.Cb = (h.C + p.KW - 1 + xshift + 3) & ~3;
+    return presplit_smem_bytes(p.OC, g.Rb, g.Cb, g.Rb, h.C + p.KW - 1) <= 227 * 1024;
+}
+
+// The input blob [N][in_img_c][H][W] (the IC channels of this slice) in boxes of hg.Cb x hg.Rb x 32 channels; boxes past
+// its edges read as zeros
+static int halo_input_map(const IgemmProblem& p, const HaloGeom& hg, EncodeTiledFn enc, CUtensorMap* tmX) {
+    const cuuint64_t in_c = static_cast<cuuint64_t>(p.in_c_total > 0 ? p.in_c_total : p.IC);
+    cuuint64_t dims[4] = {(cuuint64_t)p.W, (cuuint64_t)p.H, (cuuint64_t)p.IC, (cuuint64_t)p.N};
+    cuuint64_t strides[3] = {(cuuint64_t)p.W * 4, (cuuint64_t)p.W * p.H * 4, in_c * p.H * p.W * 4};
+    cuuint32_t box[4] = {(cuuint32_t)hg.Cb, (cuuint32_t)hg.Rb, 32, 1};
+    cuuint32_t estr[4] = {1, 1, 1, 1};
+    CUresult r = enc(tmX, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, const_cast<float*>(p.input), dims, strides, box, estr,
+                     CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                     CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+    if (r != CUDA_SUCCESS) {
+        fprintf(stderr, "fcuda: igemm input tensor map failed (%d)\n", (int)r);
+        return FCUDA_ERR_CUDA;
+    }
+    return 0;
+}
+
+static HaloArgs halo_args(const IgemmProblem& p, const HaloGeom& hg, int BN) {
+    const int taps = p.KH * p.KW;
+    HaloArgs a;
+    a.residual = p.residual; a.out = p.output; a.bias = p.bias;
+    a.OC = p.OC; a.OH = p.OH; a.OW = p.OW; a.KW = p.KW; a.taps = taps;
+    a.out_img_c = p.out_c_total > 0 ? p.out_c_total : p.OC;
+    a.kblocks = ceil_div(taps * p.IC, 32);
+    a.num_n = ceil_div(p.OC, BN);
+    a.relu = p.relu;
+    a.pool = p.pool ? 1 : 0;
+    a.R = hg.R; a.C = hg.C;
+    a.tiles_x = ceil_div(p.OW, hg.C);
+    a.tiles_y = ceil_div(p.OH, hg.R);
+    a.Rb = hg.Rb; a.Cb = hg.Cb;
+    a.pad_top = p.pad_top;
+    a.xpad = (p.pad_left + 3) & ~3;
+    a.xshift = a.xpad - p.pad_left;
+    a.tiles = static_cast<long long>(p.N) * a.tiles_x * a.tiles_y * a.num_n;
+    a.wbf = reinterpret_cast<const unsigned char*>(p.w_hi);
+    a.wbf_kb_bytes = 2u * static_cast<unsigned>(igemm_ocpad(p.OC)) * 64u;
+    a.pr = hg.R + p.KH - 1;
+    a.pc = hg.C + p.KW - 1;
+    return a;
+}
+
+template <int BN>
+int launch_igemm_presplit(const IgemmProblem& p, const HaloGeom& hg, cudaStream_t stream) {
+    EncodeTiledFn enc = encode_fn();
+    if (!enc) return FCUDA_ERR_CUDA;
+    CUtensorMap tmX;
+    if (int rc = halo_input_map(p, hg, enc, &tmX)) return rc;
+    const int taps = p.KH * p.KW;
+    if (igemm_bn_for(p.OC) != BN || static_cast<unsigned long long>(ceil_div(taps * p.IC, 32)) * igemm_ocpad(p.OC) * 128ull >= (1ull << 31))
+        return -1;
+    HaloArgs a = halo_args(p, hg, BN);
+    const long long pixel_tiles = a.tiles / a.num_n;
+    if (static_cast<long long>(p.OH) * p.OW >= (1ll << 30) || a.tiles * a.kblocks >= (1ll << 31)) return -1;
+    const int smem = presplit_smem_bytes(p.OC, hg.Rb, hg.Cb, a.pr, a.pc);
+    auto kern = conv_igemm_presplit_kernel<BN>;
+    static SmemAttrCache attr_cache;
+    if (int rc = ensure_dynamic_smem(kern, smem, attr_cache)) return rc;
+    int per_sm = 0;
+    FCUDA_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, kThreadsIg, smem));
+    const long long slots = static_cast<long long>(sm_count()) * (per_sm > 0 ? per_sm : 1);
+    const unsigned grid = static_cast<unsigned>(a.tiles < slots ? a.tiles : slots);
+    const double macs = static_cast<double>(p.N) * p.OC * p.OH * p.OW * p.IC * taps;
+    const double mma = 2.0 * static_cast<double>(pixel_tiles) * hg.R * hg.C * (a.num_n * BN) * (a.kblocks * 32) * 3;
+    const int prof = prof_begin(stream, PROF_IGEMM, 2.0 * macs, mma,
+                                4.0 * (static_cast<double>(p.N) * p.IC * p.H * p.W + static_cast<double>(p.OC) * taps * p.IC +
+                                       static_cast<double>(p.N) * p.OC * p.OH * p.OW * (p.residual ? 2 : 1)));
+    kern<<<grid, kThreadsIg, smem, stream>>>(tmX, a);
+    prof_end(prof, stream);
+    FCUDA_CHECK_LAUNCH();
+    count_launch();
+    return 0;
+}
+
 template <int BN, int PLANES>
 int launch_igemm_halo(const IgemmProblem& p, const HaloGeom& hg, cudaStream_t stream) {
     constexpr bool BF = PLANES == 3;
@@ -814,40 +1120,10 @@ int launch_igemm_halo(const IgemmProblem& p, const HaloGeom& hg, cudaStream_t st
             }
         }
     }
-    {   // the input blob [N][in_img_c][H][W] (the IC channels of this slice); boxes past its edges read as zeros
-        const cuuint64_t in_c = static_cast<cuuint64_t>(p.in_c_total > 0 ? p.in_c_total : p.IC);
-        cuuint64_t dims[4] = {(cuuint64_t)p.W, (cuuint64_t)p.H, (cuuint64_t)p.IC, (cuuint64_t)p.N};
-        cuuint64_t strides[3] = {(cuuint64_t)p.W * 4, (cuuint64_t)p.W * p.H * 4, in_c * p.H * p.W * 4};
-        cuuint32_t box[4] = {(cuuint32_t)hg.Cb, (cuuint32_t)hg.Rb, 32, 1};
-        cuuint32_t estr[4] = {1, 1, 1, 1};
-        CUresult r = enc(&tmX, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, const_cast<float*>(p.input), dims, strides, box, estr,
-                         CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                         CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-        if (r != CUDA_SUCCESS) {
-            fprintf(stderr, "fcuda: igemm input tensor map failed (%d)\n", (int)r);
-            return FCUDA_ERR_CUDA;
-        }
-    }
+    if (int rc = halo_input_map(p, hg, enc, &tmX)) return rc;
     if (BF && (igemm_bn_for(p.OC) != BN || static_cast<unsigned long long>(ceil_div(K, 32)) * igemm_ocpad(p.OC) * 128ull >= (1ull << 31))) return -1;
-    HaloArgs a;
-    a.residual = p.residual; a.out = p.output; a.bias = p.bias;
-    a.OC = p.OC; a.OH = p.OH; a.OW = p.OW; a.KW = p.KW; a.taps = taps;
-    a.out_img_c = p.out_c_total > 0 ? p.out_c_total : p.OC;
-    a.kblocks = ceil_div(K, 32);
-    a.num_n = ceil_div(p.OC, BN);
-    a.relu = p.relu;
-    a.pool = p.pool ? 1 : 0;
-    a.R = hg.R; a.C = hg.C;
-    a.tiles_x = ceil_div(p.OW, hg.C);
-    a.tiles_y = ceil_div(p.OH, hg.R);
-    a.Rb = hg.Rb; a.Cb = hg.Cb;
-    a.pad_top = p.pad_top;
-    a.xpad = (p.pad_left + 3) & ~3;
-    a.xshift = a.xpad - p.pad_left;
-    const long long pixel_tiles = static_cast<long long>(p.N) * a.tiles_x * a.tiles_y;
-    a.tiles = pixel_tiles * a.num_n;
-    a.wbf = reinterpret_cast<const unsigned char*>(p.w_hi);
-    a.wbf_kb_bytes = 2u * static_cast<unsigned>(igemm_ocpad(p.OC)) * 64u;
+    HaloArgs a = halo_args(p, hg, BN);
+    const long long pixel_tiles = a.tiles / a.num_n;
     if (static_cast<long long>(p.OH) * p.OW >= (1ll << 30) || a.tiles * a.kblocks >= (1ll << 31)) return -1;
     const int smem = halo_smem_bytes(p.OC, PLANES, hg.Rb, hg.Cb);
     auto kern = conv_igemm_halo_kernel<BN, PLANES>;
@@ -875,6 +1151,13 @@ int launch_igemm_halo(const IgemmProblem& p, const HaloGeom& hg, cudaStream_t st
 bool conv_igemm_halo_geometry(const IgemmProblem& p, HaloGeom* g) {
     HaloGeom tmp;
     const bool ok = halo_geometry(p, tmp);
+    if (ok && g) *g = tmp;
+    return ok;
+}
+
+bool conv_igemm_presplit_geometry(const IgemmProblem& p, HaloGeom* g) {
+    HaloGeom tmp;
+    const bool ok = presplit_geometry(p, tmp);
     if (ok && g) *g = tmp;
     return ok;
 }
@@ -925,6 +1208,9 @@ int conv_igemm_forward(const IgemmProblem& p, cudaStream_t stream) {
     const int bn = igemm_bn_for(p.OC);
     HaloGeom hg;
     if (tune_get(TUNE_IGEMM_HALO) != 0 && halo_geometry(p, hg)) {
+        HaloGeom pg;
+        if (p.planes == 3 && tune_get(TUNE_IGEMM_PRESPLIT) != 0 && presplit_geometry(p, pg))
+            return bn == 32 ? launch_igemm_presplit<32>(p, pg, stream) : bn == 64 ? launch_igemm_presplit<64>(p, pg, stream) : launch_igemm_presplit<128>(p, pg, stream);
         if (p.planes == 3) return bn == 32 ? launch_igemm_halo<32, 3>(p, hg, stream) : bn == 64 ? launch_igemm_halo<64, 3>(p, hg, stream) : launch_igemm_halo<128, 3>(p, hg, stream);
         if (p.planes == 2) return bn == 32 ? launch_igemm_halo<32, 2>(p, hg, stream) : bn == 64 ? launch_igemm_halo<64, 2>(p, hg, stream) : launch_igemm_halo<128, 2>(p, hg, stream);
         return bn == 32 ? launch_igemm_halo<32, 1>(p, hg, stream) : bn == 64 ? launch_igemm_halo<64, 1>(p, hg, stream) : launch_igemm_halo<128, 1>(p, hg, stream);

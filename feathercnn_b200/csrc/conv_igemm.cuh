@@ -38,6 +38,9 @@ bool conv_igemm_can_pool(const IgemmProblem& p);
 // gathering kernel.  Reads IC, OC, H, W, OH, OW, KH, KW, strides, dilation, planes and the input address.
 struct HaloGeom { int R, C, Rb, Cb; };
 bool conv_igemm_halo_geometry(const IgemmProblem& p, HaloGeom* g);
+// Tile (R x C pixels, R * C = 128 or 256) and box of the pre-split halo kernel conv_igemm_forward uses in BF16x3 mode
+// (switch igemm_presplit) on a layer that takes the halo kernel; false when the layer keeps the halo kernel.
+bool conv_igemm_presplit_geometry(const IgemmProblem& p, HaloGeom* g);
 int conv_igemm_forward(const IgemmProblem& p, cudaStream_t stream);
 
 }  // namespace fcuda

@@ -494,6 +494,21 @@ int fcuda_igemm_halo_tile(const FcudaConvParam* p, int* geom) {
     return 1;
 }
 
+int fcuda_igemm_presplit_tile(const FcudaConvParam* p, int* geom) {
+    if (!p) return 0;
+    IgemmProblem g{};
+    const int G = p->group > 0 ? p->group : 1;
+    g.N = 1; g.IC = p->input_channels / G; g.OC = p->output_channels / G;
+    g.H = p->input_h; g.W = p->input_w; g.OH = p->output_h; g.OW = p->output_w;
+    g.KH = p->kernel_h; g.KW = p->kernel_w; g.stride_h = p->stride_h; g.stride_w = p->stride_w;
+    g.pad_top = p->pad_top; g.pad_left = p->pad_left;
+    g.planes = igemm_planes();
+    HaloGeom hg;
+    if (!conv_igemm_presplit_geometry(g, &hg)) return 0;
+    if (geom) { geom[0] = hg.R; geom[1] = hg.C; geom[2] = hg.Rb; geom[3] = hg.Cb; }
+    return 1;
+}
+
 int fcuda_conv_forward_pool(const FcudaConvParam* p, int algo, float* output, const float* input, const float* packed,
                             float* scratch, const float* bias, int batch, void* stream) {
     if (!p) return -100;

@@ -372,6 +372,7 @@ TuneEntry g_tune[TUNE_COUNT] = {
     {"wino_mlp", "FCUDA_WINO_MLP", 2, 0, 2, 0, false},               // Winograd transforms: slab copies / all plane loads in flight
     {"igemm_halo", "FCUDA_IGEMM_HALO", 1, 0, 1, 0, false},           // implicit GEMM: TMA halo tiles + pipelined wgmma (stride 1)
     {"gemm_pipe", "FCUDA_GEMM_PIPE", 1, 0, 1, 0, false},             // TensorGEMM: persistent CTAs + pipelined wgmma
+    {"igemm_presplit", "FCUDA_IGEMM_PRESPLIT", 1, 0, 1, 0, false},   // BF16x3 halo kernel: one split per box, ldmatrix fragments
 };
 }  // namespace
 const char* tune_name(int key) { return key >= 0 && key < TUNE_COUNT ? g_tune[key].name : nullptr; }

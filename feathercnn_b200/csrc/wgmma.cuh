@@ -112,6 +112,23 @@ __device__ __forceinline__ void prefetch_tensormap(const CUtensorMap* map) {
     asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(map)) : "memory");
 }
 
+// Barrier `id` (1-15; 0 is __syncthreads) over the first `count` threads of the CTA.
+__device__ __forceinline__ void named_bar_sync(uint32_t id, uint32_t count) {
+    asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(count) : "memory");
+}
+// Four 8x8 b16 matrices: lane l supplies the 16-byte row address of row l % 8 of matrix l / 8 and receives in r[i] the
+// elements (l / 4, 2 * (l % 4)) and (l / 4, 2 * (l % 4) + 1) of matrix i.
+__device__ __forceinline__ void ldsm_x4(uint32_t addr, uint32_t (&r)[4]) {
+    asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0, %1, %2, %3}, [%4];"
+                 : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3])
+                 : "r"(addr)
+                 : "memory");
+}
+__device__ __forceinline__ void st_shared_v4(uint32_t addr, const uint32_t (&v)[4]) {
+    asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(v[0]), "r"(v[1]), "r"(v[2]), "r"(v[3])
+                 : "memory");
+}
+
 // ---- warpgroup MMA ordering ----------------------------------------------------------------------------------------
 // fence: register operands / accumulators written by ordinary instructions become visible to the following wgmma;
 // commit + wait<N>: at most N committed groups of this warpgroup still run (their registers may not be touched).

@@ -173,6 +173,10 @@ int fcuda_conv_can_pool(const FcudaConvParam* param, int algo);
  * 16-byte aligned input), with geom[0..3] = output patch rows, patch columns, shared-memory box rows, box columns;
  * 0 when it keeps the gathering kernel.  The switch itself is not consulted. */
 int fcuda_igemm_halo_tile(const FcudaConvParam* param, int* geom);
+/* The same for the pre-split halo kernel (switch igemm_presplit below; fp32split mode only): 1 when the layer runs on it,
+ * with geom[0..3] = tile rows, tile columns (rows * columns = 256 where the layer's N tile is 64 output channels, else 128),
+ * fp32 box rows, box columns; 0 otherwise.  The switch itself is not consulted. */
+int fcuda_igemm_presplit_tile(const FcudaConvParam* param, int* geom);
 int fcuda_conv_forward_pool(const FcudaConvParam* param, int algo, float* output, const float* input,
                             const float* packed_kernel, float* scratch, const float* bias, int batch, void* stream);
 
@@ -250,6 +254,9 @@ int fcuda_deconv_forward(const FcudaDeconvParam* param, float* output, const flo
  *   gemm_pipe (0-1, 1)        TensorGEMM (Winograd, im2col, InnerProduct): persistent CTAs that fill the next tile's ring
  *                             stages during the epilogue; the split and MMAs of neighbouring k-blocks overlap and no wgmma
  *                             waits for the one before it.  Bit-identical to 0 = one CTA per tile, drained per k-block
+ *   igemm_presplit (0-1, 1)   halo kernel in fp32split mode: each 32-channel input box is split into its two bf16 planes
+ *                             once instead of once per tap, the A fragments are loaded by ldmatrix, and layers with a
+ *                             64-channel N tile use 256-pixel tiles.  Bit-identical to 0 = the per-tap split
  * Every variant computes the same result (tests/test_gpu_variants.py).  Returns 0 / the value, -200 for an unknown name or value. */
 int fcuda_set_tuning(const char* name, int value);
 int fcuda_get_tuning(const char* name);

@@ -1,12 +1,13 @@
-"""Per-layer timing of the implicit-GEMM convolution (SGECONV): the halo kernel (igemm_halo = 1) against the gathering
-kernel (igemm_halo = 0), for every layer of the benchmark nets that fcuda_conv_select_algo_tuned sends to SGECONV, at the
-nets' benchmark batch sizes.
+"""Per-layer timing of the implicit-GEMM convolution (SGECONV), switch --switch at 0 against 1: igemm_presplit (default:
+the pre-split halo kernel against the per-tap split) or igemm_halo (the halo kernel against the gathering kernel), for
+every layer of the benchmark nets that fcuda_conv_select_algo_tuned sends to SGECONV, at the nets' benchmark batch sizes.
 
-    python scripts/igemm_layer_bench.py --out DIR [--reps 5] [--iters 20]
+    python scripts/igemm_layer_bench.py --out DIR [--reps 5] [--iters 20] [--switch igemm_presplit]
 
 For each layer: CUDA-event time per launch of both kernels (alternated over --reps repetitions; median and every value),
 the algorithmic rate (direct-convolution FLOPs), the issued tensor-pipe rate (padded patch pixels, N tiles and the three
-MMAs per product of the split modes) and that rate's fraction of the H100 SXM data-sheet dense BF16 rate.  The Winograd
+MMAs per product of the split modes) and that rate's fraction of the H100 SXM data-sheet dense BF16 rate, and for the
+halo kernels the bytes one launch moves from L2 to the SMs (filter ring stages + input boxes, from the geometry).  The Winograd
 F(6,3) time of the same shape is listed for reference only.  Writes DIR/igemm_layer_bench.json with the card's name and
 power limit.  Needs a CUDA device."""
 from __future__ import annotations
@@ -76,6 +77,7 @@ def main() -> None:
     ap.add_argument("--reps", type=int, default=5)
     ap.add_argument("--iters", type=int, default=20, help="launches per timed repetition")
     ap.add_argument("--models", default="vgg16,resnet50,mobilenet_v1")
+    ap.add_argument("--switch", default="igemm_presplit", choices=["igemm_presplit", "igemm_halo"])
     args = ap.parse_args()
 
     import torch
@@ -85,7 +87,8 @@ def main() -> None:
         raise SystemExit("igemm_layer_bench needs a CUDA device")
     torch.cuda.set_device(0)
     lib = fcuda()
-    saved = lib.fcuda_get_tuning(b"igemm_halo")
+    switch = args.switch.encode()
+    saved = lib.fcuda_get_tuning(switch)
     stream = booster._stream
 
     def prepare(pfields, algo, n, pool):
@@ -126,7 +129,7 @@ def main() -> None:
         torch.cuda.synchronize()
         return e0.elapsed_time(e1) / iters
 
-    result = {"card": card(), "reps": args.reps, "iters": args.iters,
+    result = {"card": card(), "switch": args.switch, "reps": args.reps, "iters": args.iters,
               "datasheet_bf16_dense_tflops": DATASHEET_BF16_DENSE / 1e12,
               "precision": {0: "tf32x3", 1: "tf32", 2: "fp32split"}[lib.fcuda_get_precision()], "layers": []}
     try:
@@ -140,11 +143,13 @@ def main() -> None:
                 p, launch, out = prepare(pf, booster.SGECONV, n, pool)
                 geom = (ctypes.c_int * 4)()
                 halo = lib.fcuda_igemm_halo_tile(ctypes.byref(p), geom) == 1
+                pgeom = (ctypes.c_int * 4)()
+                presplit = lib.fcuda_igemm_presplit_tile(ctypes.byref(p), pgeom) == 1
                 t = {0: [], 1: []}
                 outs = {}
                 for _ in range(args.reps):
                     for sw in (0, 1):
-                        lib.fcuda_set_tuning(b"igemm_halo", sw)
+                        lib.fcuda_set_tuning(switch, sw)
                         t[sw].append(time_ms(launch, args.iters))
                         outs[sw] = out.clone()
                 identical = bool(torch.equal(outs[0], outs[1]))
@@ -162,6 +167,14 @@ def main() -> None:
                 else:
                     pix = -(-(n * p.output_h * p.output_w) // 128) * 128
                 mult = 3 if result["precision"] != "tf32" else 1
+
+                def l2_to_sm_bytes(g):
+                    """Filter ring stages + input boxes one launch fetches: per tile, every k-block's filter stage and
+                    one box of 32 channels x box rows x box columns (fp32) per channel block."""
+                    r, c, rb, cb = g[0], g[1], g[2], g[3]
+                    tiles = n * -(-p.output_h // r) * -(-p.output_w // c) * (ocp // bn)
+                    stage = bn * 32 * (2 if result["precision"] == "fp32split" else 4) * (1 if result["precision"] == "tf32" else 2)
+                    return tiles * ((kpad // 32) * stage + (ic // group // 32) * 32 * rb * cb * 4)
                 issued_new = 2.0 * pix * ocp * kpad * mult
                 old_ms, new_ms = statistics.median(t[0]), statistics.median(t[1])
                 wino_ms = None  # Winograd F(6,3) on the same shape (3x3, stride 1), for reference only
@@ -181,14 +194,18 @@ def main() -> None:
                        "algo_tflops_old": algo_flops / old_ms / 1e9, "algo_tflops_new": algo_flops / new_ms / 1e9,
                        "issued_tflops_new": issued_new / new_ms / 1e9,
                        "issued_fraction_of_datasheet_bf16_new": issued_new / new_ms / 1e-3 / DATASHEET_BF16_DENSE,
-                       "winograd_f63_ms_reference_only": wino_ms}
+                       "winograd_f63_ms_reference_only": wino_ms,
+                       "presplit_tile_rows_cols_box": list(pgeom) if presplit else None,
+                       "l2_to_sm_bytes_halo": l2_to_sm_bytes(geom) if halo else None,
+                       "l2_to_sm_bytes_presplit": l2_to_sm_bytes(pgeom) if presplit else None}
                 result["layers"].append(rec)
                 print(json.dumps({k2: rec[k2] for k2 in ("model", "layer", "old_ms_median", "new_ms_median", "speedup",
-                                                          "bit_identical", "algo_tflops_new", "winograd_f63_ms_reference_only")}),
+                                                          "bit_identical", "algo_tflops_new", "issued_tflops_new",
+                                                          "l2_to_sm_bytes_presplit")}),
                       flush=True)
                 torch.cuda.empty_cache()
     finally:
-        lib.fcuda_set_tuning(b"igemm_halo", saved)
+        lib.fcuda_set_tuning(switch, saved)
     for model in BATCH:
         rows = [r for r in result["layers"] if r["model"] == model]
         if rows:
