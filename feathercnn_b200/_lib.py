@@ -54,6 +54,14 @@ class FcudaDeconvParam(ctypes.Structure):
         "output_h output_w").split()]
 
 
+class FcudaInterpParam(ctypes.Structure):
+    """include/fcuda.h FcudaInterpParam (output_h / output_w filled by fcuda_interp_output_dim)."""
+
+    _fields_ = ([("resize_type", ctypes.c_int), ("align_corner", ctypes.c_int), ("height_scale", ctypes.c_float),
+                 ("width_scale", ctypes.c_float)] +
+                [(n, ctypes.c_int) for n in "output_height output_width input_h input_w output_h output_w".split()])
+
+
 def fcuda() -> ctypes.CDLL:
     global _fcuda
     if _fcuda is None:
@@ -62,7 +70,11 @@ def fcuda() -> ctypes.CDLL:
         P = ctypes.POINTER(FcudaConvParam)
         szp = ctypes.POINTER(ctypes.c_size_t)
         D = ctypes.POINTER(FcudaDeconvParam)
+        R = ctypes.POINTER(FcudaInterpParam)
         sigs = {
+            "fcuda_interp_output_dim": (i, [R]),
+            "fcuda_interp_forward": (i, [R, vp, vp, i, i, vp]),
+            "fcuda_crop_forward": (i, [vp, vp] + [i] * 10 + [vp]),
             "fcuda_deconv_output_dim": (i, [D]),
             "fcuda_deconv_plan": (i, [D, P, ctypes.POINTER(i)]),
             "fcuda_deconv_get_buffer_size": (i, [D, i, szp, szp]),

@@ -13,6 +13,7 @@ import torch
 
 from ._lib import FcudaConvParam, fcuda
 from ._lib import FcudaDeconvParam as DeconvParam
+from ._lib import FcudaInterpParam as InterpParam
 
 NAIVE, IM2COL, SGECONV, DEPTHWISE, WINOGRADF63, WINOGRADF63FUSED, WINOGRADF23 = range(7)
 ALGO_NAMES = ["NAIVE", "IM2COL", "SGECONV", "DEPTHWISE", "WINOGRADF63", "WINOGRADF63FUSED", "WINOGRADF23"]
@@ -211,6 +212,42 @@ def deconv_forward(x: torch.Tensor, w: torch.Tensor, b: torch.Tensor | None = No
            lib.fcuda_deconv_forward(ctypes.byref(p), _ptr(out), _ptr(x.contiguous()), _ptr(packed), _ptr(scratch), _ptr(b), n,
                                     _stream()))
     return out, algo
+
+
+# ---- resize / crop ---------------------------------------------------------------------------------
+INTERP_NEAREST, INTERP_BILINEAR = 1, 2
+
+
+def interp_param(h: int, w: int, out_h: int, out_w: int, mode: str = "bilinear", align_corners: bool = False,
+                 scale=None) -> InterpParam:
+    """FcudaInterpParam with output_h / output_w filled.  out_h / out_w are ncnn's output_height / output_width; `scale`
+    (a float or (h, w)) sets height_scale / width_scale, which size the output when out_h or out_w is 0."""
+    sh, sw = (1.0, 1.0) if scale is None else ((scale, scale) if isinstance(scale, (int, float)) else scale)
+    rt = {"nearest": INTERP_NEAREST, "bilinear": INTERP_BILINEAR}.get(mode, mode)
+    p = InterpParam(resize_type=rt, align_corner=int(bool(align_corners)), height_scale=sh, width_scale=sw,
+                    output_height=out_h, output_width=out_w, input_h=h, input_w=w)
+    _check("fcuda_interp_output_dim", fcuda().fcuda_interp_output_dim(ctypes.byref(p)))
+    return p
+
+
+def interp(x: torch.Tensor, out_h: int, out_w: int, mode: str = "bilinear", align_corners: bool = False,
+           scale=None) -> torch.Tensor:
+    """ncnn Interp of x (N, C, H, W): mode "nearest" (resize_type 1) or "bilinear" (2)."""
+    n, c, h, w = x.shape
+    p = interp_param(h, w, out_h, out_w, mode, align_corners, scale)
+    out = torch.empty((n, c, p.output_h, p.output_w), device=x.device, dtype=torch.float32)
+    _check("fcuda_interp_forward",
+           fcuda().fcuda_interp_forward(ctypes.byref(p), _ptr(out), _ptr(x.contiguous()), c, n, _stream()))
+    return out
+
+
+def crop(x: torch.Tensor, coff: int, hoff: int, woff: int, oc: int, oh: int, ow: int) -> torch.Tensor:
+    """out[n][c][y][x] = x[n][c + coff][y + hoff][x + woff], shape (N, oc, oh, ow)."""
+    n, c, h, w = x.shape
+    out = torch.empty((n, oc, oh, ow), device=x.device, dtype=torch.float32)
+    _check("fcuda_crop_forward",
+           fcuda().fcuda_crop_forward(_ptr(out), _ptr(x.contiguous()), c, h, w, coff, hoff, woff, oc, oh, ow, n, _stream()))
+    return out
 
 
 # ---- other layer entry points (thin wrappers used by the parity tests) ------------------------------

@@ -10,6 +10,7 @@
 #include "layers.cuh"
 #include "pack.cuh"
 #include "preprocess.cuh"
+#include "resize.cuh"
 #include "tensor_gemm.cuh"
 #include "winograd.cuh"
 
@@ -43,6 +44,37 @@ inline int planes() { return g_precision == FCUDA_PRECISION_TF32 ? 1 : 2; }
 // operand format of the implicit GEMM (IgemmProblem::planes): 3 = BF16x3 in the default fp32-split mode
 inline int igemm_planes() { return g_precision == FCUDA_PRECISION_FP32_SPLIT ? 3 : planes(); }
 inline cudaStream_t as_stream(void* s) { return static_cast<cudaStream_t>(s); }
+
+int interp_check_and_size(FcudaInterpParam* p) {
+    if (!p) return -100;
+    if (p->resize_type != 1 && p->resize_type != 2) return -200;
+    if (p->input_h <= 0 || p->input_w <= 0 || p->output_height < 0 || p->output_width < 0) return -100;
+    const bool sized = p->output_height > 0 && p->output_width > 0;
+    // the scales are read where they size the output, and by nearest where its explicit size is absent
+    const bool scale_h_used = !sized || (p->resize_type == 1 && !p->output_height);
+    const bool scale_w_used = !sized || (p->resize_type == 1 && !p->output_width);
+    if ((scale_h_used && !(p->height_scale > 0.f)) || (scale_w_used && !(p->width_scale > 0.f))) return -100;
+    long long oh = p->output_height, ow = p->output_width;
+    if (!sized) {  // ncnn: static_cast<int>(h * height_scale), an fp32 product
+        const float fh = static_cast<float>(p->input_h) * p->height_scale;
+        const float fw = static_cast<float>(p->input_w) * p->width_scale;
+        if (!(fh < 2147483648.f) || !(fw < 2147483648.f)) return -100;
+        oh = static_cast<long long>(fh);
+        ow = static_cast<long long>(fw);
+    }
+    if (oh <= 0 || ow <= 0 || oh * ow > 0x7fffffffLL || static_cast<long long>(p->input_h) * p->input_w > 0x7fffffffLL)
+        return -100;
+    p->output_h = static_cast<int>(oh);
+    p->output_w = static_cast<int>(ow);
+    return 0;
+}
+
+// The fp32 source-coordinate scale of one axis (include/fcuda.h, fcuda_interp_forward)
+float interp_scale(const FcudaInterpParam& p, int in, int out, int explicit_out, float scale) {
+    if (p.resize_type == 1) return explicit_out ? static_cast<float>(in) / static_cast<float>(out) : 1.f / scale;
+    if (p.align_corner) return out > 1 ? static_cast<float>(in - 1) / static_cast<float>(out - 1) : 0.f;
+    return static_cast<float>(in) / static_cast<float>(out);
+}
 
 struct ConvPlan {
     int algo = -1;
@@ -680,6 +712,39 @@ int fcuda_copy_channels(float* dst, int dst_channels, int dst_channel_offset, co
         return -100;
     return copy_channels(src, dst, static_cast<size_t>(channels) * stride, static_cast<size_t>(dst_channels) * stride,
                          static_cast<size_t>(dst_channel_offset) * stride, batch, as_stream(stream));
+}
+
+int fcuda_interp_output_dim(FcudaInterpParam* param) { return interp_check_and_size(param); }
+
+int fcuda_interp_forward(const FcudaInterpParam* param, float* output, const float* input, int channels, int batch,
+                         void* stream) {
+    if (!param) return -100;
+    FcudaInterpParam p = *param;
+    const int rc = interp_check_and_size(&p);
+    if (rc) return rc;
+    if (!output || !input || channels <= 0 || batch < 1) return -100;
+    InterpGeom g;
+    g.H = p.input_h; g.W = p.input_w; g.OH = p.output_h; g.OW = p.output_w;
+    g.mode = p.resize_type;
+    g.align_corner = p.align_corner != 0;
+    g.scale_h = interp_scale(p, p.input_h, p.output_h, p.output_height, p.height_scale);
+    g.scale_w = interp_scale(p, p.input_w, p.output_w, p.output_width, p.width_scale);
+    return interp_forward(input, output, g, static_cast<long long>(batch) * channels, as_stream(stream));
+}
+
+int fcuda_crop_forward(float* output, const float* input, int channels, int in_h, int in_w, int coff, int hoff, int woff,
+                       int out_c, int out_h, int out_w, int batch, void* stream) {
+    if (channels <= 0 || in_h <= 0 || in_w <= 0 || out_c <= 0 || out_h <= 0 || out_w <= 0 || batch < 1 || coff < 0 ||
+        hoff < 0 || woff < 0)
+        return -100;
+    if (static_cast<long long>(coff) + out_c > channels || static_cast<long long>(hoff) + out_h > in_h ||
+        static_cast<long long>(woff) + out_w > in_w)
+        return -100;
+    if (!output || !input) return -100;
+    CropGeom g;
+    g.C = channels; g.H = in_h; g.W = in_w; g.coff = coff; g.hoff = hoff; g.woff = woff;
+    g.OC = out_c; g.OH = out_h; g.OW = out_w;
+    return crop_forward(input, output, g, batch, as_stream(stream));
 }
 
 int fcuda_pixel_channels(int type, int* src_channels, int* out_channels) { return pixel_channels(type, src_channels, out_channels); }

@@ -1,5 +1,5 @@
 // Built-in layer registrations: the 13 ncnn type names the reference serves (/root/reference/src/layer_factory.cpp:53-68)
-// plus Deconvolution / DeconvolutionDepthWise, 15 in all, mapped onto this host's layer classes.  A table of {type name, factory} pairs instead of one macro line per layer; the
+// plus Deconvolution / DeconvolutionDepthWise, Interp and Crop, 17 in all, mapped onto this host's layer classes.  A table of {type name, factory} pairs instead of one macro line per layer; the
 // DEFINE_LAYER_CREATOR / REGISTER_LAYER_CREATOR macros of <feather/layer_factory.h> remain the plugin API for user layers.
 #include <feather/layer_factory.h>
 
@@ -13,6 +13,7 @@
 #include "layers/misc_layers.h"
 #include "layers/pooling_layer.h"
 #include "layers/relu_layer.h"
+#include "layers/resize_layers.h"
 #include "layers/scale_layer.h"
 
 namespace feather {
@@ -48,6 +49,8 @@ const BuiltIn kBuiltIns[] = {
     {"Concat", make_layer<ConcatLayer>},
     {"Deconvolution", make_layer<DeconvLayer>},
     {"DeconvolutionDepthWise", make_layer<DeconvLayer>},
+    {"Interp", make_layer<InterpLayer>},
+    {"Crop", make_layer<CropLayer>},
 };
 
 }  // namespace

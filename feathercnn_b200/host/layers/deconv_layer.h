@@ -1,12 +1,15 @@
 // DeconvLayer — serves ncnn "Deconvolution" and "DeconvolutionDepthWise" (transposed convolution; the reference has no
 // such layer).  Same protocol as ConvLayer: LoadParam creates the weight / bias blobs, Reshape sizes the top and requests
 // scratch, Init packs, Forward runs fcuda_deconv_forward.  Deliberately not a ConvLayer: Net::ApplyFusion's residual pass
-// and LayerConvAlgo look for ConvLayer, and a deconvolution can fuse neither an Eltwise shortcut nor a pooling.  Only a
-// following ReLU fuses (into the scatter / gather kernel); BatchNorm / Scale after it run as their own layers.
+// and LayerConvAlgo look for ConvLayer, and a deconvolution can fuse neither an Eltwise shortcut nor a pooling.  A
+// following ReLU fuses (into the scatter / gather kernel) and a following Crop folds into the pads (FoldCrop);
+// BatchNorm / Scale after it run as their own layers.
 #pragma once
 
 #include <fcuda.h>
 #include <feather/layer.h>
+
+#include "resize_layers.h"
 
 namespace feather {
 inline namespace b200 {  // ABI tag: keeps these symbols apart from the reference build when both are loaded
@@ -89,8 +92,25 @@ public:
         }
         param.input_h = bottom->height();
         param.input_w = bottom->width();
+        if (crop_folded) {
+            param.pad_top = own_pads[0]; param.pad_bottom = own_pads[1];
+            param.pad_left = own_pads[2]; param.pad_right = own_pads[3];
+        }
         int rc = fcuda_deconv_output_dim(&param);
         if (rc) return rc;
+        if (crop_folded) {  // the folded Crop's window, from this input's (and the reference blob's) shape
+            int oc = 0, oh = 0, ow = 0;
+            if (!crop.Resolve(param.output_channels, param.output_h, param.output_w, crop_reference, &oc, &oh, &ow)) {
+                LOGE("Layer %s: the folded crop window does not fit the %dx%d deconvolution output", this->name.c_str(),
+                     param.output_h, param.output_w);
+                return FEATHER_ERR_TOPOLOGY;
+            }
+            param.pad_top += crop.hoff;
+            param.pad_left += crop.woff;
+            param.pad_bottom += param.output_h - crop.hoff - oh;
+            param.pad_right += param.output_w - crop.woff - ow;
+            if ((rc = fcuda_deconv_output_dim(&param))) return rc;
+        }
         const int batch = bottom->num();
         tops[0]->ReshapeWithRealloc(batch, param.output_channels, param.output_h, param.output_w);
         size_t scratch = 0, packed = 0;
@@ -128,8 +148,30 @@ public:
         return 1;
     }
 
+    // Net::ApplyFusion: a Crop of this layer's otherwise unread top, in h and w only, becomes part of the pads: pad_top
+    // grows by hoff, pad_left by woff, pad_bottom / pad_right by what remains below and to the right of the window
+    // (resolved in Reshape).  fcuda_deconv_forward crops by the pads on every path, so the result is bit-identical.  A
+    // stride-1 layer that is not depthwise keeps its Crop: its plan depends on the pads (the direct convolution only while
+    // every pad <= dilation * (K - 1)), and the grown pads are known only once the shapes are.  Returns 1 when folded.
+    int FoldCrop(const CropWindow& window, Blob<float>* reference) {
+        const bool depthwise = param.group > 1 && param.group == param.input_channels &&
+                               param.output_channels == param.input_channels;
+        if (crop_folded || window.coff != 0 || window.outc != 0) return 0;
+        if (param.stride_h == 1 && param.stride_w == 1 && !depthwise) return 0;
+        crop = window;
+        crop_reference = reference;
+        own_pads[0] = param.pad_top; own_pads[1] = param.pad_bottom;
+        own_pads[2] = param.pad_left; own_pads[3] = param.pad_right;
+        crop_folded = true;
+        return 1;
+    }
+
 private:
     FcudaDeconvParam param;
+    bool crop_folded = false;
+    CropWindow crop;
+    const Blob<float>* crop_reference = NULL;  // shape only; NULL for a one-bottom Crop
+    int own_pads[4] = {0, 0, 0, 0};            // top, bottom, left, right as loaded
     int weight_data_size = 0;
     int init_algo = -1;
     Blob<float>* processed_weights = NULL;

@@ -12,8 +12,10 @@
 #include <feather/layer_factory.h>
 
 #include "layers/conv_layer.h"
+#include "layers/deconv_layer.h"
 #include "layers/eltwise_layer.h"
 #include "layers/misc_layers.h"
+#include "layers/resize_layers.h"
 
 namespace feather {
 inline namespace b200 {  // ABI tag: keeps these symbols apart from the reference build when both are loaded
@@ -570,6 +572,30 @@ int Net::ApplyFusion() {
             e->_fused_away = true;
             break;
         }
+    }
+    // Third pass: a Crop of a deconvolution's otherwise unread top becomes part of the deconvolution's pads (FCN's final
+    // crop of the upsampled scores to the input size: one full read and write of the largest blob fewer).  Like the
+    // residual addend, the Crop's reference blob must already exist when the deconvolution runs.
+    for (size_t j = 0; j < layers.size(); ++j) {
+        CropLayer* c = dynamic_cast<CropLayer*>(layers[j]);
+        if (!c || c->_fused_away || c->bottoms.empty() || c->tops.size() != 1) continue;
+        Blob<float>* mine = c->bottoms[0];
+        Blob<float>* ref = c->reference();
+        if (mine == ref || readers[mine] != 1 || !producer.count(mine)) continue;
+        const size_t i = producer[mine];
+        DeconvLayer* d = dynamic_cast<DeconvLayer*>(layers[i]);
+        if (!d || i >= j || d->_fused_away || d->tops.size() != 1) continue;
+        if (ref && producer.count(ref) && producer[ref] >= i) continue;  // not computed yet when the deconvolution runs
+        if (d->FoldCrop(c->window(), ref) != 1) continue;
+        Blob<float>* dead = d->tops[0];
+        blob_map.erase(dead->name);
+        producer.erase(dead);
+        delete dead;
+        d->tops[0] = c->tops[0];
+        producer[d->tops[0]] = i;
+        c->tops.clear();
+        c->bottoms.clear();
+        c->_fused_away = true;
     }
     return 0;
 }

@@ -8,7 +8,10 @@ no caffe / protobuf-generated code is needed — and writes the ncnn text ``.par
 
 * layer grammar and parameter ids as ``ConvLayer::LoadParam`` & co. read them (``src/layers/*.h``; ids follow ncnn's
   caffe2ncnn): Convolution / ConvolutionDepthWise, Deconvolution / DeconvolutionDepthWise, InnerProduct, Pooling, ReLU, BatchNorm, Scale, Eltwise, Concat, Dropout,
-  Softmax, Split, Input;
+  Softmax, Split, Input, Crop;
+* Crop (``axis`` 2 or 3, FCN's score crops) becomes ncnn's two-bottom Crop: the output height and width are the reference
+  bottom's, the offsets are ``offset``'s; with axis 3 the height offset is 0, and the reference must then have the height
+  of the cropped blob, as ncnn's two-bottom Crop takes both sizes from it;
 * in-place Caffe layers (top == bottom) get a fresh blob name, and a blob read by several layers gets an explicit
   ``Split`` layer — the reference's Net looks blobs up by name and its layers own their tops (``net.cpp:112-160``);
 * weight blobs are written with the 4-byte raw-fp32 tag, bias / BatchNorm / Scale blobs raw (``modelbin.cpp:47-197``);
@@ -295,6 +298,23 @@ def convert(caffemodel: bytes) -> tuple[str, bytes]:
             out.layer("Softmax", name, bottoms, tops)
         elif type_ == "Split":
             out.layer("Split", name, bottoms, tops)
+        elif type_ == "Crop":
+            # crop_param = 144: axis = 1 (default 2), offset = 2 (repeated; one value applies to every cropped axis)
+            p = parse_message(_first(L, 144, b""))
+            axis = int(_first(p, 1, 2))
+            if axis >= 1 << 63:  # a negative int32 on the wire
+                axis -= 1 << 64
+            axis = axis + 4 if axis < 0 else axis
+            if axis not in (2, 3) or len(bottoms) != 2:
+                raise ValueError(f"layer {name}: Crop with axis {axis} (channels or batch) or without a reference bottom "
+                                 f"has no FeatherCNN counterpart")
+            offs = _ints(p.get(2, [])) or [0]
+            n_axes = 4 - axis
+            if len(offs) not in (1, n_axes):
+                raise ValueError(f"layer {name}: Crop has {len(offs)} offsets for {n_axes} cropped axes")
+            offs = offs * n_axes if len(offs) == 1 else offs
+            hoff, woff = (offs[0], offs[1]) if axis == 2 else (0, offs[0])
+            out.layer("Crop", name, bottoms, tops, f"0={woff} 1={hoff}")
         else:
             raise ValueError(f"layer {name}: Caffe type {type_!r} has no FeatherCNN counterpart (layer_factory.cpp:55-67)")
         for t in tops:

@@ -44,7 +44,7 @@ class ModelWriter:
         self.shape = {name: (c, h, w)}
         return name
 
-    def conv(self, name, bottom, oc, k, stride=1, pad=0, bias=True, group=1, top=None, gain=None):
+    def conv(self, name, bottom, oc, k, stride=1, pad=0, bias=True, group=1, top=None, gain=None, dilation=1):
         top = top or name
         ic, h, w = self.shape[bottom]
         icg = ic // group
@@ -55,12 +55,14 @@ class ModelWriter:
         params = {0: oc, 1: k, 3: stride, 4: pad, 5: int(bias), 6: wts.size}
         if group > 1:
             params[7] = group
+        if dilation > 1:
+            params[2] = dilation
         self._layer(ltype, name, [bottom], [top], params)
         self._weights(wts, True)
         if bias:
             self._weights(self.rng.uniform(-0.1, 0.1, oc).astype(np.float32), False)
-        oh = (h + 2 * pad - k) // stride + 1
-        ow = (w + 2 * pad - k) // stride + 1
+        oh = (h + 2 * pad - dilation * (k - 1) - 1) // stride + 1
+        ow = (w + 2 * pad - dilation * (k - 1) - 1) // stride + 1
         self.shape[top] = (oc, oh, ow)
         self.flops += 2.0 * oc * icg * oh * ow * k * k
         return top
@@ -207,6 +209,40 @@ class ModelWriter:
         top = top or name
         self._layer("Dropout", name, [bottom], [top], {} if scale is None else {0: f"{scale:e}"})
         self.shape[top] = self.shape[bottom]
+        return top
+
+    def interp(self, name, bottom, resize_type=2, out_h=0, out_w=0, scale=None, align_corner=0, top=None):
+        """ncnn Interp: resize_type 1 nearest, 2 bilinear; an explicit (out_h, out_w), or `scale` when either is 0."""
+        top = top or name
+        c, h, w = self.shape[bottom]
+        params = {0: resize_type}
+        if scale is not None:
+            params[1] = params[2] = f"{scale:e}"
+        if out_h or out_w:
+            params[3], params[4] = out_h, out_w
+        if align_corner:
+            params[6] = 1
+        self._layer("Interp", name, [bottom], [top], params)
+        if out_h and out_w:
+            self.shape[top] = (c, out_h, out_w)
+        else:  # fp32 products, truncated (fcuda_interp_output_dim)
+            s = np.float32(1.0 if scale is None else scale)
+            self.shape[top] = (c, int(np.float32(h) * s), int(np.float32(w) * s))
+        return top
+
+    def crop(self, name, bottom, woff=0, hoff=0, reference=None, coff=0, outc=0, outh=0, outw=0, top=None):
+        """ncnn Crop: with `reference` the output height and width are that blob's; a size of 0 runs to the end."""
+        top = top or name
+        c, h, w = self.shape[bottom]
+        params = {k: v for k, v in ((0, woff), (1, hoff), (2, coff), (3, outw), (4, outh), (5, outc)) if v or k < 2}
+        self._layer("Crop", name, [bottom] + ([reference] if reference else []), [top], params)
+        oc = outc or c - coff
+        if reference:
+            oh, ow = self.shape[reference][1:]
+        else:
+            oh, ow = outh or h - hoff, outw or w - woff
+        assert coff + oc <= c and hoff + oh <= h and woff + ow <= w, (name, self.shape[bottom], (oc, oh, ow))
+        self.shape[top] = (oc, oh, ow)
         return top
 
     # ---- output ------------------------------------------------------------------------------
@@ -360,8 +396,59 @@ def decoder_tiny(seed=0, size=16, classes=4) -> ModelWriter:
     return m
 
 
+def fcn8s_tiny(seed=0, size=64, classes=5) -> ModelWriter:
+    """FCN-8s topology at small width: five 2x2 poolings behind a first convolution padded by 50 (FCN pads by 100) and
+    an unpadded 5x5 "fc6", score convolutions on pool3 / pool4, k4 s2 deconvolutions with two-bottom crops of the skip
+    scores before each Eltwise SUM, and a k16 s8 deconvolution cropped to the input.  The crop offsets (5, 7, 27) are
+    odd, like FCN's (5, 9, 31); the windows fit sizes 32 to 700 except those = 30 (mod 32)."""
+    m = ModelWriter(seed)
+    data = m.input("data", 3, size, size)
+    x = m.relu("relu1", m.conv("conv1", data, 16, 3, 1, 50, True))
+    x = m.pool("pool1", x)
+    x = m.relu("relu2", m.conv("conv2", x, 16, 3, 1, 1, True))
+    x = m.pool("pool2", x)
+    x = m.relu("relu3", m.conv("conv3", x, 32, 3, 1, 1, True))
+    pool3 = m.pool("pool3", x)
+    p3a, p3b = m.split("pool3_split", pool3, ["pool3_a", "pool3_b"])
+    x = m.relu("relu4", m.conv("conv4", p3a, 32, 3, 1, 1, True))
+    pool4 = m.pool("pool4", x)
+    p4a, p4b = m.split("pool4_split", pool4, ["pool4_a", "pool4_b"])
+    x = m.relu("relu5", m.conv("conv5", p4a, 64, 3, 1, 1, True))
+    x = m.pool("pool5", x)
+    x = m.relu("relu_fc6", m.conv("fc6", x, 64, 5, 1, 0, True))
+    x = m.relu("relu_fc7", m.conv("fc7", x, 64, 1, 1, 0, True))
+    x = m.conv("score_fr", x, classes, 1, 1, 0, True)
+    up2 = m.deconv("upscore2", x, classes, 4, 2, 0, False)
+    up2a, up2b = m.split("upscore2_split", up2, ["upscore2_a", "upscore2_b"])
+    sp4 = m.conv("score_pool4", p4b, classes, 1, 1, 0, True, gain=0.01)
+    sp4c = m.crop("score_pool4c", sp4, 5, 5, reference=up2a)
+    x = m.eltwise("fuse_pool4", [up2b, sp4c])
+    upp4 = m.deconv("upscore_pool4", x, classes, 4, 2, 0, False)
+    upp4a, upp4b = m.split("upscore_pool4_split", upp4, ["upscore_pool4_a", "upscore_pool4_b"])
+    sp3 = m.conv("score_pool3", p3b, classes, 1, 1, 0, True, gain=0.001)
+    sp3c = m.crop("score_pool3c", sp3, 7, 7, reference=upp4a)
+    x = m.eltwise("fuse_pool3", [upp4b, sp3c])
+    x = m.deconv("upscore8", x, classes, 16, 8, 0, False)
+    m.crop("score", x, 27, 27, reference=data)
+    return m
+
+
+def deeplab_head_tiny(seed=0, size=32, classes=5) -> ModelWriter:
+    """DeepLab-style head: a stride-8 encoder, a dilated 3x3 convolution (dilation 2), a 1x1 classifier and a fixed x8
+    bilinear Interp (scales, half-pixel) back to the input size."""
+    m = ModelWriter(seed)
+    x = m.input("data", 3, size, size)
+    x = m.relu("relu1", m.conv("conv1", x, 16, 3, 2, 1, True))
+    x = m.relu("relu2", m.conv("conv2", x, 32, 3, 2, 1, True))
+    x = m.relu("relu3", m.conv("conv3", x, 32, 3, 2, 1, True))
+    x = m.relu("relu_aspp", m.conv("aspp", x, 32, 3, 1, 2, True, dilation=2))
+    x = m.conv("classifier", x, classes, 1, 1, 0, True)
+    m.interp("upsample", x, 2, scale=8.0)
+    return m
+
+
 ZOO = {"single_conv": single_conv, "vgg16": vgg16, "resnet50": resnet50, "mobilenet_v1": mobilenet_v1, "mini": mini,
-       "decoder_tiny": decoder_tiny}
+       "decoder_tiny": decoder_tiny, "fcn8s_tiny": fcn8s_tiny, "deeplab_head_tiny": deeplab_head_tiny}
 
 
 def synthetic_input(shape, index: int = 0) -> np.ndarray:

@@ -242,6 +242,37 @@ int fcuda_deconv_init(const FcudaDeconvParam* param, float* packed, const float*
 int fcuda_deconv_forward(const FcudaDeconvParam* param, float* output, const float* input, const float* packed,
                          float* scratch, const float* bias, int batch, void* stream);
 
+/* ncnn's Interp (the reference has no such layer; its unused caffe_cpu_interp2 maps src = dst * in / out, which is neither
+ * ncnn mode): input (batch, C, input_h, input_w) -> output (batch, C, output_h, output_w).
+ *   resize_type 1 nearest:  hs = output_height ? input_h / (float)output_h : 1.f / height_scale (fp32, ws likewise),
+ *                           source row min((int)(y * hs), input_h - 1); a pure gather, bit-exact.
+ *   resize_type 2 bilinear: scales from the sizes.  align_corner 0 (half pixel): fy = (y + 0.5) * input_h / output_h - 0.5,
+ *                           negative fy clamped to 0; align_corner 1: fy = y * (input_h - 1) / (output_h - 1), 0 when
+ *                           output_h == 1.  Neighbours y0 = (int)fy, y1 = min(y0 + 1, input_h - 1), weight fy - y0; x
+ *                           likewise; interpolated horizontally on both rows, then vertically (PyTorch's
+ *                           F.interpolate(mode="bilinear", align_corners=...) definition).
+ * Equal input and output sizes (and, for nearest, hs == ws == 1) are a straight copy.
+ * Rejected with -200: resize_type other than 1 / 2 (bicubic is not built).  -100: empty input or output, or a
+ * non-positive scale where a scale is used. */
+typedef struct FcudaInterpParam {
+    int resize_type, align_corner;
+    float height_scale, width_scale;
+    int output_height, output_width; /* explicit size; when either is 0 both come from the scales */
+    int input_h, input_w;
+    int output_h, output_w;          /* filled by fcuda_interp_output_dim */
+} FcudaInterpParam;
+/* Validates the parameters and fills output_h / output_w: output_height / output_width when both are set, otherwise
+ * (int)(input_h * height_scale) and (int)(input_w * width_scale) with fp32 products, as ncnn computes them. */
+int fcuda_interp_output_dim(FcudaInterpParam* param);
+/* output <- input for `channels` planes of each of `batch` images.  Allocates nothing and does not synchronise. */
+int fcuda_interp_forward(const FcudaInterpParam* param, float* output, const float* input, int channels, int batch,
+                         void* stream);
+/* ncnn / Caffe Crop: output (batch, out_c, out_h, out_w)[n][c][y][x] = input (batch, channels, in_h, in_w)
+ * [n][c + coff][y + hoff][x + woff].  -100 for empty sizes, a negative offset or a window outside the input.  Allocates
+ * nothing and does not synchronise. */
+int fcuda_crop_forward(float* output, const float* input, int channels, int in_h, int in_w, int coff, int hoff, int woff,
+                       int out_c, int out_h, int out_w, int batch, void* stream);
+
 /* Kernel-variant switches for A/B measurements and tests.  Defaults are the measured-best configuration; the environment
  * variable FCUDA_<NAME> sets the initial value.  Names (value range, default):
  *   dw_vec (0-1, 1)           vectorised depthwise kernel on wide planes
@@ -269,7 +300,8 @@ void fcuda_profile_tensor_gemm(int enable);
 int fcuda_profile_collect(double* total_ms, double* algo_flops, double* mma_flops, long long* launches);
 /* Same, per kernel class, for every instrumented launch (the enable switch above covers all of them):
  * kind 0 TensorGEMM, 1 implicit-GEMM conv, 2 Winograd input transform, 3 Winograd output transform, 4 pooling,
- * 5 depthwise, 6 element-wise (BN/Scale/Eltwise), 7 deconvolution scatter / depthwise gather, < 0 all.  algo_bytes = the bytes the operation must move (inputs
+ * 5 depthwise, 6 element-wise (BN/Scale/Eltwise), 7 deconvolution scatter / depthwise gather, 8 resize / crop (Interp,
+ * Crop), < 0 all.  algo_bytes = the bytes the operation must move (inputs
  * read once + outputs written once). */
 int fcuda_profile_collect_kind(int kind, double* total_ms, double* algo_flops, double* mma_flops, double* algo_bytes,
                                long long* launches);
