@@ -774,9 +774,9 @@ conv_igemm_halo_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_con
 //   A operand  = per k-block and warp 4 ldmatrix.x4 (2 k-steps x 2 planes): the 8 rows of each 8 x 8 matrix are
 //                8 consecutive pixels of one patch row, so every tap (dy, dx) is the row address + (dy * pc + dx) * 16
 //                bytes, 16-byte aligned and free of bank conflicts.  ldmatrix yields the m16n8k16 A layout of wgmma.
-//   tile       = the halo kernel's 128-pixel patch.  A 256-pixel tile (two m64 accumulators per warpgroup) would halve
-//                the filter bytes per output where BN = 64, but a 288-thread CTA gets at most 168 registers per thread
-//                and the second accumulator and fragment sets do not fit: ptxas then serialises the wgmma.
+//   tile       = the halo kernel's 128-pixel patch.  A 256-pixel tile (two m64 accumulators per warpgroup) does not fit
+//                the 168 registers a 288-thread CTA gets beside the fragment sets (ptxas then serialises the wgmma);
+//                conv_igemm_wide_kernel reaches larger tiles by moving the pixels to the wgmma N side instead.
 // Per k-block the wgmma sequence (p2*q1, p1*q2, p1*q1 per k-step), the operand values, the k order and BN are those of conv_igemm_halo_kernel<BN, 3>: the result is bit-identical to it.
 template <int BN>
 __global__ void __launch_bounds__(kThreadsIg, 1)
@@ -953,6 +953,276 @@ conv_igemm_presplit_kernel(const __grid_constant__ CUtensorMap tmX, const HaloAr
     }
 }
 
+// Wide pre-split kernel (BF16x3, switch igemm_wide): the GEMM of conv_igemm_presplit_kernel turned around,
+// D[oc][pixel] = W[oc][k] * X[pixel][k]^T, so that the pixels sit on the N side of wgmma, read by descriptor, and need no
+// fragment registers.  That leaves room for 224 pixels per warpgroup: the filter stage a tile fetches serves 1.75x (BN
+// 128) or 3.5x (BN 64) as many pixels as on the 128-pixel tile.
+//   tile       = 28 rows x 8 columns of one image with a 128-channel N tile (the warpgroups share the pixels, warpgroup w
+//                takes output channels 64w..64w+63), 28 x 16 with a 64-channel N tile (warpgroup w takes columns
+//                8w..8w+7, both read the whole filter stage).  One SS wgmma m64n224k16 per product.
+//   A operand  = the filter ring stage as loaded: [plane][row / 8][k chunk][row % 8][8 bf16] is the un-swizzled K-major
+//                layout (LBO 128 B, SBO 512 B).
+//   B operand  = the presplit bf16 planes [ch / 8][pr][pc][8 ch]: the 8 pixels of one strip row are one 128-byte core
+//                matrix, strip rows are pc * 16 bytes apart (SBO), 8-channel chunks pr * pc * 16 (LBO); tap (dy, dx) adds
+//                (dy * pc + dx) * 16 bytes to the start address.
+//   boxes      = 16-channel halves of the fp32 box in a one-deep ring (the whole box and two plane buffers do not fit
+//                beside a 448-pixel tile); the next channel block's halves are split into the free plane buffer behind
+//                k-blocks wide_half0_tap() and taps - 1 of the current one.  The split writes are fenced to the async proxy
+//                before the consumers' named barrier.
+// Per k-block the products p2*q1, p1*q2, p1*q1 per k-step, the operand bits, the k order and BN are those of
+// conv_igemm_presplit_kernel.
+constexpr int kWideRows = 28;
+
+// k-block of a channel block behind which the first half of the next box is split.  At least 3: the consumer waiting for
+// filter stage kb there has seen every warp release stage kb - 4, so every warp has retired the previous channel block's
+// MMAs, the last readers of the plane buffer being overwritten.  Needs taps >= 5 (wide_geometry).
+__device__ __forceinline__ int wide_half0_tap(int taps) { return taps / 2 > 3 ? taps / 2 : 3; }
+
+// Producer of the wide kernel (lane 0): the filter ring of halo_producer; the half boxes of channel block cb + 1 go out
+// with the filter stages of taps 2 and wide_half0_tap + 3 of block cb, when the consumers have already freed the slot.
+template <int BN>
+__device__ __forceinline__ void wide_producer(const CUtensorMap* tmX, const HaloArgs& args, uint8_t* smem, float* halo,
+                                              int hstage, uint64_t* full_bar, uint64_t* empty_bar, uint64_t* hfull_bar,
+                                              uint64_t* hempty_bar) {
+    constexpr int kStage = 2 * BN * 64;
+    const int per_img = args.tiles_x * args.tiles_y;
+    const int taps = args.taps;
+    const int ncb = args.kblocks / taps;
+    const int p1 = wide_half0_tap(taps) + 3 < taps ? wide_half0_tap(taps) + 3 : taps - 1;
+    ptx::prefetch_tensormap(tmX);
+    int nh = 0;   // half boxes issued
+    int kbg = 0;  // filter stages issued
+    auto load_half = [&](long long t, int cb, int h) {
+        const long long pt = t / args.num_n;
+        const int n = static_cast<int>(pt / per_img);
+        const int rem = static_cast<int>(pt - static_cast<long long>(n) * per_img);
+        const int ty = rem / args.tiles_x, tx = rem - ty * args.tiles_x;
+        if (nh > 0) ptx::mbar_wait_nocall(hempty_bar, (nh - 1) & 1);
+        ptx::mbar_arrive_expect_tx(hfull_bar, static_cast<uint32_t>(hstage) * 4u);
+        ptx::tma_load_4d(halo, tmX, hfull_bar, tx * args.C - args.xpad, ty * args.R - args.pad_top, cb * 32 + 16 * h, n);
+        ++nh;
+    };
+    if (blockIdx.x < args.tiles) {
+        load_half(blockIdx.x, 0, 0);
+        load_half(blockIdx.x, 0, 1);
+    }
+    for (long long t = blockIdx.x; t < args.tiles; t += gridDim.x) {
+        const int n_blk = static_cast<int>(t % args.num_n);
+        for (int cb = 0, kb = 0; cb < ncb; ++cb) {
+            for (int tap = 0; tap < taps; ++tap, ++kb, ++kbg) {
+                const int stage = kbg % kStagesIg;
+                if (kbg >= kStagesIg) ptx::mbar_wait_nocall(&empty_bar[stage], ((kbg / kStagesIg) - 1) & 1);
+                ptx::mbar_arrive_expect_tx(&full_bar[stage], kStage);
+                ptx::bulk_load_1d(smem + stage * kStage,
+                                  args.wbf + static_cast<size_t>(kb) * args.wbf_kb_bytes + static_cast<size_t>(n_blk) * kStage,
+                                  kStage, &full_bar[stage]);
+                if (tap == 2 || tap == p1) {
+                    const int h = tap == 2 ? 0 : 1;
+                    if (cb + 1 < ncb) load_half(t, cb + 1, h);
+                    else if (t + gridDim.x < args.tiles) load_half(t + gridDim.x, 0, h);
+                }
+            }
+        }
+    }
+}
+
+// Epilogue of the wide kernel: accumulator d[4j + i] is output channel oc0 + 8 * (i >> 1), pixel (oy0 + j, ox0 + (i & 1)).
+// Each thread holds both columns of its pooling windows and both rows (j even, j + 1), so pooling needs no shuffle; the
+// order of the bias, residual, ReLU and max operations is halo_epilogue's.
+__device__ __forceinline__ void wide_epilogue(const float (&acc)[112], const HaloArgs& args, int img, int oc0, int oy0,
+                                              int ox0) {
+    const int oplane = args.OH * args.OW;
+    const int SH = (args.OH + 1) >> 1, SW = (args.OW + 1) >> 1;
+    const bool xok[2] = {ox0 < args.OW, ox0 + 1 < args.OW};
+#pragma unroll
+    for (int e = 0; e < 2; ++e) {
+        const int oc = oc0 + 8 * e;
+        if (oc >= args.OC) continue;
+        const float bv = args.bias != nullptr ? __ldg(args.bias + oc) : 0.f;
+        const size_t cbase = (static_cast<size_t>(img) * args.out_img_c + oc) * oplane;
+#pragma unroll
+        for (int j = 0; j < kWideRows; j += 2) {
+            float v[2][2];
+            bool ok[2][2];
+#pragma unroll
+            for (int r = 0; r < 2; ++r) {
+                const int oy = oy0 + j + r;
+                const size_t o = cbase + static_cast<size_t>(oy) * args.OW + ox0;
+#pragma unroll
+                for (int x = 0; x < 2; ++x) {
+                    ok[r][x] = oy < args.OH && xok[x];
+                    v[r][x] = acc[4 * (j + r) + 2 * e + x] + bv;
+                    if (args.residual != nullptr && ok[r][x]) v[r][x] += __ldg(args.residual + o + x);
+                    if (args.relu) v[r][x] = fmaxf(v[r][x], 0.f);
+                }
+                if (!args.pool && ok[r][0]) {
+                    float* dst = args.out + o;
+                    if (ok[r][1] && (reinterpret_cast<uintptr_t>(dst) & 7) == 0) {
+                        *reinterpret_cast<float2*>(dst) = make_float2(v[r][0], v[r][1]);
+                    } else {
+                        dst[0] = v[r][0];
+                        if (ok[r][1]) dst[1] = v[r][1];
+                    }
+                }
+            }
+            if (args.pool && ok[0][0]) {
+                const float m0 = fmaxf(ok[0][0] ? v[0][0] : -INFINITY, ok[1][0] ? v[1][0] : -INFINITY);
+                const float m1 = fmaxf(ok[0][1] ? v[0][1] : -INFINITY, ok[1][1] ? v[1][1] : -INFINITY);
+                args.out[(static_cast<size_t>(img) * args.out_img_c + oc) * (static_cast<size_t>(SH) * SW) +
+                         static_cast<size_t>((oy0 + j) >> 1) * SW + (ox0 >> 1)] = fmaxf(m0, m1);
+            }
+        }
+    }
+}
+
+template <int BN>
+__global__ void __launch_bounds__(kThreadsIg, 1)
+conv_igemm_wide_kernel(const __grid_constant__ CUtensorMap tmX, const HaloArgs args) {
+    constexpr int kBTile = BN * 32 * 2;
+    constexpr int kStage = 2 * kBTile;
+    constexpr int kConsumers = kConsumerWarps * 32;
+    extern __shared__ uint8_t smem_raw[];
+    uint8_t* smem = smem_raw + ((1024u - (ptx::smem_u32(smem_raw) & 1023u)) & 1023u);
+    float* halo = reinterpret_cast<float*>(smem + kStagesIg * kStage);
+    const int cstride = args.Rb * args.Cb;
+    const int hstage = 16 * cstride;           // floats per half box
+    const int hunits = 2 * args.pr * args.pc;  // 16-byte rows per plane and half box
+    const uint32_t pbytes = 32u * static_cast<uint32_t>(hunits);
+    // [buffer 2][p1, p2][ch / 8][pr][pc][16 B], then the half-box word offset of every unit of a half
+    const uint32_t planes = ptx::smem_u32(halo + hstage);
+    const int* utab = reinterpret_cast<const int*>(smem + kStagesIg * kStage + hstage * 4 + 4 * pbytes);
+    __shared__ uint64_t full_bar[kStagesIg];
+    __shared__ uint64_t empty_bar[kStagesIg];
+    __shared__ uint64_t hfull_bar, hempty_bar;
+
+    const int warp = threadIdx.x >> 5;
+    const int lane = threadIdx.x & 31;
+    const int per_img = args.tiles_x * args.tiles_y;
+    const int taps = args.taps, KW = args.KW;
+    const int ncb = args.kblocks / taps;
+
+    if (threadIdx.x == 0) {
+        for (int s = 0; s < kStagesIg; ++s) {
+            ptx::mbar_init(&full_bar[s], 1);
+            ptx::mbar_init(&empty_bar[s], kConsumerWarps);
+        }
+        ptx::mbar_init(&hfull_bar, 1);
+        ptx::mbar_init(&hempty_bar, kConsumerWarps);
+        ptx::fence_barrier_init();
+    }
+    for (int u = threadIdx.x; u < hunits; u += kThreadsIg) {
+        const int ch8 = u / (args.pr * args.pc), rem = u - ch8 * args.pr * args.pc;
+        const int row = rem / args.pc, col = rem - row * args.pc;
+        const_cast<int*>(utab)[u] = 8 * ch8 * cstride + row * args.Cb + col + args.xshift;
+    }
+    __syncthreads();
+
+    if (warp == kConsumerWarps) {
+        if (lane == 0) wide_producer<BN>(&tmX, args, smem, halo, hstage, full_bar, empty_bar, &hfull_bar, &hempty_bar);
+        return;
+    }
+
+    // ===================== consumers =====================
+    const int gq = lane >> 2, c = lane & 3;
+    const int wg = warp >> 2;
+    const uint32_t a_off = BN == 128 ? 4096u * wg : 0u;  // this warpgroup's 64 filter rows
+    const uint32_t b_off = BN == 64 ? 128u * wg : 0u;    // this warpgroup's 8 strip columns
+    const uint32_t lbo = 16u * static_cast<uint32_t>(args.pr * args.pc), sbo = 16u * static_cast<uint32_t>(args.pc);
+    const int h0 = wide_half0_tap(taps);
+
+    int nc = 0;   // half boxes split
+    int kbg = 0;  // filter stages consumed
+    // split half h of box nc / 2 into plane buffer (nc / 2) & 1 and hand the fp32 half box back
+    auto convert_half = [&](int h) {
+        ptx::mbar_wait_nocall(&hfull_bar, nc & 1);
+        const uint32_t dst = planes + static_cast<uint32_t>((nc >> 1) & 1) * 2u * pbytes + 16u * static_cast<uint32_t>(h * hunits);
+#pragma unroll 1
+        for (int u = threadIdx.x; u < hunits; u += kConsumers) {
+            const float* s = halo + utab[u];
+            float x[8];
+#pragma unroll
+            for (int i = 0; i < 8; ++i) x[i] = s[i * cstride];
+            uint32_t p1[4], p2[4];
+#pragma unroll
+            for (int w = 0; w < 4; ++w) split_bf16x2(x[2 * w], x[2 * w + 1], p1[w], p2[w]);
+            ptx::st_shared_v4(dst + 16u * u, p1);
+            ptx::st_shared_v4(dst + pbytes + 16u * u, p2);
+        }
+        ptx::fence_proxy_async_smem();
+        __syncwarp();
+        ptx::mbar_arrive_if(&hempty_bar, lane == 0);
+        ++nc;
+    };
+
+    convert_half(0);  // grid <= tiles: every CTA has a first box
+    convert_half(1);
+    for (long long t = blockIdx.x; t < args.tiles; t += gridDim.x) {
+        const bool more_tiles = t + gridDim.x < args.tiles;
+        const int kbg0 = kbg;
+
+        float acc[112];
+#pragma unroll
+        for (int i = 0; i < 112; ++i) acc[i] = 0.f;
+        uint32_t bbuf = 0, toff = 0;  // plane buffer of the current box (+ this warpgroup's columns), byte offset of the tap
+        int dx = 0;
+
+        // one k-block: the six MMAs, then (half >= 0) the split of that half of the next box behind them
+        auto step = [&](int half) {
+            const int stage = kbg & (kStagesIg - 1);
+            ptx::mbar_wait_nocall(&full_bar[stage], (kbg / kStagesIg) & 1);
+            const uint32_t a_base = ptx::smem_u32(smem) + stage * kStage + a_off;
+            const uint64_t dQ1 = make_smem_desc_none(a_base, 128, 512);
+            const uint64_t dQ2 = make_smem_desc_none(a_base + kBTile, 128, 512);
+            const uint64_t dP1 = make_smem_desc_none(bbuf + toff, lbo, sbo);
+            const uint64_t dP2 = dP1 + (pbytes >> 4);
+            const uint64_t kstep = pbytes >> 5;  // channels 16-31 of the block: two 8-channel chunks on
+            ptx::wgmma_fence();
+#pragma unroll
+            for (int kk = 0; kk < 2; ++kk) {
+                WgmmaSS<224>::mma(acc, dQ1 + 16 * kk, dP2 + kstep * kk, 1u);  // q1 * p2
+                WgmmaSS<224>::mma(acc, dQ2 + 16 * kk, dP1 + kstep * kk, 1u);  // q2 * p1
+                WgmmaSS<224>::mma(acc, dQ1 + 16 * kk, dP1 + kstep * kk, 1u);  // q1 * p1
+            }
+            ptx::wgmma_commit();
+            ptx::wgmma_wait<1>();  // k-block kbg - 1 retired: its filter stage is free
+            if (half >= 0) convert_half(half);
+            __syncwarp();
+            ptx::mbar_arrive_if(&empty_bar[(kbg + kStagesIg - 1) & (kStagesIg - 1)], kbg != kbg0 && lane == 0);
+            ++kbg;
+            toff += 16;
+            if (++dx == KW) {
+                dx = 0;
+                toff += 16u * static_cast<uint32_t>(args.pc - KW);
+            }
+        };
+        for (int cb = 0; cb < ncb; ++cb) {
+            ptx::named_bar_sync(1, kConsumers);  // every consumer has split this box (both halves)
+            bbuf = planes + static_cast<uint32_t>(((nc >> 1) - 1) & 1) * 2u * pbytes + b_off;
+            toff = 0;
+            dx = 0;
+            const bool next = cb + 1 < ncb || more_tiles;
+            int i = 0;
+            for (; i < h0; ++i) step(-1);
+            step(next ? 0 : -1);
+            for (++i; i < taps - 1; ++i) step(-1);
+            step(next ? 1 : -1);
+        }
+        ptx::wgmma_wait<0>();
+        __syncwarp();
+        ptx::mbar_arrive_if(&empty_bar[(kbg - 1) & (kStagesIg - 1)], lane == 0);
+
+        // the tile's coordinates, computed here rather than kept in registers through the main loop
+        const int n_blk = static_cast<int>(t % args.num_n);
+        const long long pt = t / args.num_n;
+        const int img = static_cast<int>(pt / per_img);
+        const int rem = static_cast<int>(pt - static_cast<long long>(img) * per_img);
+        const int ty = rem / args.tiles_x, tx = rem - ty * args.tiles_x;
+        const int oc0 = n_blk * BN + (BN == 128 ? 64 * wg : 0) + 16 * (warp & 3) + gq;
+        const int ox0 = tx * args.C + (BN == 64 ? 8 * wg : 0) + 2 * c;
+        wide_epilogue(acc, args, img, oc0, ty * kWideRows, ox0);
+    }
+}
+
 // Bank model of one ld.shared of the halo gather: lane l reads column l / 4 of channel plane (l % 4) * (2 for the bf16
 // pairs, 1 for tf32); the warp is conflict-free when its 32 words fall in 32 different banks (the starting column and
 // row only rotate the pattern).
@@ -1017,13 +1287,35 @@ static bool presplit_geometry(const IgemmProblem& p, HaloGeom& g) {
     return presplit_smem_bytes(p.OC, g.Rb, g.Cb, g.Rb, h.C + p.KW - 1) <= 227 * 1024;
 }
 
-// The input blob [N][in_img_c][H][W] (the IC channels of this slice) in boxes of hg.Cb x hg.Rb x 32 channels; boxes past
-// its edges read as zeros
-static int halo_input_map(const IgemmProblem& p, const HaloGeom& hg, EncodeTiledFn enc, CUtensorMap* tmX) {
+// Filter ring, one fp32 half box, two plane buffers and the unit table of conv_igemm_wide_kernel
+static int wide_smem_bytes(int OC, int Rb, int Cb, int pr, int pc) {
+    const int hunits = 2 * pr * pc;
+    return kStagesIg * 2 * igemm_bn_for(OC) * 64 + 16 * Rb * Cb * 4 + 2 * 64 * hunits + 4 * hunits + 1024;
+}
+
+// Tile and box of conv_igemm_wide_kernel for a layer that takes the pre-split kernel, or false (the layer keeps it): N
+// tiles of 64 or 128 channels, at least 5 taps (wide_half0_tap), and no more padded tile pixels than the pre-split patch.
+static bool wide_geometry(const IgemmProblem& p, HaloGeom& g) {
+    HaloGeom h;
+    const int bn = igemm_bn_for(p.OC);
+    if (bn == 32 || p.KH * p.KW < 5 || !presplit_geometry(p, h)) return false;
+    const int R = kWideRows, C = bn == 64 ? 16 : 8;
+    const long long cost = static_cast<long long>(ceil_div(p.OW, C)) * C * ceil_div(p.OH, R) * R;
+    if (cost > static_cast<long long>(ceil_div(p.OW, h.C)) * h.C * ceil_div(p.OH, h.R) * h.R) return false;
+    const int xshift = ((p.pad_left + 3) & ~3) - p.pad_left;
+    g.R = R; g.C = C;
+    g.Rb = R + p.KH - 1;
+    g.Cb = (C + p.KW - 1 + xshift + 3) & ~3;
+    return wide_smem_bytes(p.OC, g.Rb, g.Cb, g.Rb, C + p.KW - 1) <= 227 * 1024;
+}
+
+// The input blob [N][in_img_c][H][W] (the IC channels of this slice) in boxes of hg.Cb x hg.Rb x `chans` channels; boxes
+// past its edges read as zeros
+static int halo_input_map(const IgemmProblem& p, const HaloGeom& hg, EncodeTiledFn enc, CUtensorMap* tmX, int chans = 32) {
     const cuuint64_t in_c = static_cast<cuuint64_t>(p.in_c_total > 0 ? p.in_c_total : p.IC);
     cuuint64_t dims[4] = {(cuuint64_t)p.W, (cuuint64_t)p.H, (cuuint64_t)p.IC, (cuuint64_t)p.N};
     cuuint64_t strides[3] = {(cuuint64_t)p.W * 4, (cuuint64_t)p.W * p.H * 4, in_c * p.H * p.W * 4};
-    cuuint32_t box[4] = {(cuuint32_t)hg.Cb, (cuuint32_t)hg.Rb, 32, 1};
+    cuuint32_t box[4] = {(cuuint32_t)hg.Cb, (cuuint32_t)hg.Rb, (cuuint32_t)chans, 1};
     cuuint32_t estr[4] = {1, 1, 1, 1};
     CUresult r = enc(tmX, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, const_cast<float*>(p.input), dims, strides, box, estr,
                      CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
@@ -1074,6 +1366,38 @@ int launch_igemm_presplit(const IgemmProblem& p, const HaloGeom& hg, cudaStream_
     if (static_cast<long long>(p.OH) * p.OW >= (1ll << 30) || a.tiles * a.kblocks >= (1ll << 31)) return -1;
     const int smem = presplit_smem_bytes(p.OC, hg.Rb, hg.Cb, a.pr, a.pc);
     auto kern = conv_igemm_presplit_kernel<BN>;
+    static SmemAttrCache attr_cache;
+    if (int rc = ensure_dynamic_smem(kern, smem, attr_cache)) return rc;
+    int per_sm = 0;
+    FCUDA_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, kThreadsIg, smem));
+    const long long slots = static_cast<long long>(sm_count()) * (per_sm > 0 ? per_sm : 1);
+    const unsigned grid = static_cast<unsigned>(a.tiles < slots ? a.tiles : slots);
+    const double macs = static_cast<double>(p.N) * p.OC * p.OH * p.OW * p.IC * taps;
+    const double mma = 2.0 * static_cast<double>(pixel_tiles) * hg.R * hg.C * (a.num_n * BN) * (a.kblocks * 32) * 3;
+    const int prof = prof_begin(stream, PROF_IGEMM, 2.0 * macs, mma,
+                                4.0 * (static_cast<double>(p.N) * p.IC * p.H * p.W + static_cast<double>(p.OC) * taps * p.IC +
+                                       static_cast<double>(p.N) * p.OC * p.OH * p.OW * (p.residual ? 2 : 1)));
+    kern<<<grid, kThreadsIg, smem, stream>>>(tmX, a);
+    prof_end(prof, stream);
+    FCUDA_CHECK_LAUNCH();
+    count_launch();
+    return 0;
+}
+
+template <int BN>
+int launch_igemm_wide(const IgemmProblem& p, const HaloGeom& hg, cudaStream_t stream) {
+    EncodeTiledFn enc = encode_fn();
+    if (!enc) return FCUDA_ERR_CUDA;
+    CUtensorMap tmX;
+    if (int rc = halo_input_map(p, hg, enc, &tmX, 16)) return rc;
+    const int taps = p.KH * p.KW;
+    if (igemm_bn_for(p.OC) != BN || static_cast<unsigned long long>(ceil_div(taps * p.IC, 32)) * igemm_ocpad(p.OC) * 128ull >= (1ull << 31))
+        return -1;
+    HaloArgs a = halo_args(p, hg, BN);
+    const long long pixel_tiles = a.tiles / a.num_n;
+    if (static_cast<long long>(p.OH) * p.OW >= (1ll << 30) || a.tiles * a.kblocks >= (1ll << 31)) return -1;
+    const int smem = wide_smem_bytes(p.OC, hg.Rb, hg.Cb, a.pr, a.pc);
+    auto kern = conv_igemm_wide_kernel<BN>;
     static SmemAttrCache attr_cache;
     if (int rc = ensure_dynamic_smem(kern, smem, attr_cache)) return rc;
     int per_sm = 0;
@@ -1162,6 +1486,13 @@ bool conv_igemm_presplit_geometry(const IgemmProblem& p, HaloGeom* g) {
     return ok;
 }
 
+bool conv_igemm_wide_geometry(const IgemmProblem& p, HaloGeom* g) {
+    HaloGeom tmp;
+    const bool ok = wide_geometry(p, tmp);
+    if (ok && g) *g = tmp;
+    return ok;
+}
+
 bool conv_igemm_supported(int IC, int KH, int KW) {
     if (KH * KW > 63) return false;                               // per-pixel tap validity mask is 64-bit
     if (IC % 32 != 0 && KH * KW * IC > kMaxTableK) return false;  // k-table must fit in shared memory
@@ -1208,9 +1539,12 @@ int conv_igemm_forward(const IgemmProblem& p, cudaStream_t stream) {
     const int bn = igemm_bn_for(p.OC);
     HaloGeom hg;
     if (tune_get(TUNE_IGEMM_HALO) != 0 && halo_geometry(p, hg)) {
-        HaloGeom pg;
-        if (p.planes == 3 && tune_get(TUNE_IGEMM_PRESPLIT) != 0 && presplit_geometry(p, pg))
+        HaloGeom pg, wg;
+        if (p.planes == 3 && tune_get(TUNE_IGEMM_PRESPLIT) != 0 && presplit_geometry(p, pg)) {
+            if (tune_get(TUNE_IGEMM_WIDE) != 0 && wide_geometry(p, wg))
+                return bn == 64 ? launch_igemm_wide<64>(p, wg, stream) : launch_igemm_wide<128>(p, wg, stream);
             return bn == 32 ? launch_igemm_presplit<32>(p, pg, stream) : bn == 64 ? launch_igemm_presplit<64>(p, pg, stream) : launch_igemm_presplit<128>(p, pg, stream);
+        }
         if (p.planes == 3) return bn == 32 ? launch_igemm_halo<32, 3>(p, hg, stream) : bn == 64 ? launch_igemm_halo<64, 3>(p, hg, stream) : launch_igemm_halo<128, 3>(p, hg, stream);
         if (p.planes == 2) return bn == 32 ? launch_igemm_halo<32, 2>(p, hg, stream) : bn == 64 ? launch_igemm_halo<64, 2>(p, hg, stream) : launch_igemm_halo<128, 2>(p, hg, stream);
         return bn == 32 ? launch_igemm_halo<32, 1>(p, hg, stream) : bn == 64 ? launch_igemm_halo<64, 1>(p, hg, stream) : launch_igemm_halo<128, 1>(p, hg, stream);

@@ -38,9 +38,12 @@ bool conv_igemm_can_pool(const IgemmProblem& p);
 // gathering kernel.  Reads IC, OC, H, W, OH, OW, KH, KW, strides, dilation, planes and the input address.
 struct HaloGeom { int R, C, Rb, Cb; };
 bool conv_igemm_halo_geometry(const IgemmProblem& p, HaloGeom* g);
-// Tile (R x C pixels, R * C = 128 or 256) and box of the pre-split halo kernel conv_igemm_forward uses in BF16x3 mode
+// Tile (R x C pixels, R * C = 128) and box of the pre-split halo kernel conv_igemm_forward uses in BF16x3 mode
 // (switch igemm_presplit) on a layer that takes the halo kernel; false when the layer keeps the halo kernel.
 bool conv_igemm_presplit_geometry(const IgemmProblem& p, HaloGeom* g);
+// Tile (28 x 16 pixels with a 64-channel N tile, 28 x 8 with a 128-channel one) and box of the wide pre-split kernel
+// (switch igemm_wide) on a layer that takes the pre-split kernel; false when the layer keeps the pre-split kernel.
+bool conv_igemm_wide_geometry(const IgemmProblem& p, HaloGeom* g);
 int conv_igemm_forward(const IgemmProblem& p, cudaStream_t stream);
 
 }  // namespace fcuda

@@ -373,6 +373,7 @@ TuneEntry g_tune[TUNE_COUNT] = {
     {"igemm_halo", "FCUDA_IGEMM_HALO", 1, 0, 1, 0, false},           // implicit GEMM: TMA halo tiles + pipelined wgmma (stride 1)
     {"gemm_pipe", "FCUDA_GEMM_PIPE", 1, 0, 1, 0, false},             // TensorGEMM: persistent CTAs + pipelined wgmma
     {"igemm_presplit", "FCUDA_IGEMM_PRESPLIT", 1, 0, 1, 0, false},   // BF16x3 halo kernel: one split per box, ldmatrix fragments
+    {"igemm_wide", "FCUDA_IGEMM_WIDE", 1, 0, 1, 0, false},           // pre-split kernel: 224-pixel N side, filters on M
 };
 }  // namespace
 const char* tune_name(int key) { return key >= 0 && key < TUNE_COUNT ? g_tune[key].name : nullptr; }

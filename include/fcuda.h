@@ -174,9 +174,14 @@ int fcuda_conv_can_pool(const FcudaConvParam* param, int algo);
  * 0 when it keeps the gathering kernel.  The switch itself is not consulted. */
 int fcuda_igemm_halo_tile(const FcudaConvParam* param, int* geom);
 /* The same for the pre-split halo kernel (switch igemm_presplit below; fp32split mode only): 1 when the layer runs on it,
- * with geom[0..3] = tile rows, tile columns (rows * columns = 256 where the layer's N tile is 64 output channels, else 128),
- * fp32 box rows, box columns; 0 otherwise.  The switch itself is not consulted. */
+ * with geom[0..3] = tile rows, tile columns (rows * columns = 128), fp32 box rows, box columns; 0 otherwise.  The switch
+ * itself is not consulted. */
 int fcuda_igemm_presplit_tile(const FcudaConvParam* param, int* geom);
+/* The same for the wide pre-split kernel (switch igemm_wide below), which takes a layer of the pre-split kernel whose N
+ * tile is 64 or 128 output channels, with at least 5 taps, where its tile pads no more pixels than the pre-split patch:
+ * 1 with geom[0..3] = tile rows (28), tile columns (16 for a 64-channel N tile, 8 for 128), fp32 box rows, box columns;
+ * 0 otherwise.  The switches themselves are not consulted. */
+int fcuda_igemm_wide_tile(const FcudaConvParam* param, int* geom);
 int fcuda_conv_forward_pool(const FcudaConvParam* param, int algo, float* output, const float* input,
                             const float* packed_kernel, float* scratch, const float* bias, int batch, void* stream);
 
@@ -286,8 +291,12 @@ int fcuda_crop_forward(float* output, const float* input, int channels, int in_h
  *                             stages during the epilogue; the split and MMAs of neighbouring k-blocks overlap and no wgmma
  *                             waits for the one before it.  Bit-identical to 0 = one CTA per tile, drained per k-block
  *   igemm_presplit (0-1, 1)   halo kernel in fp32split mode: each 32-channel input box is split into its two bf16 planes
- *                             once instead of once per tap, the A fragments are loaded by ldmatrix, and layers with a
- *                             64-channel N tile use 256-pixel tiles.  Bit-identical to 0 = the per-tap split
+ *                             once instead of once per tap and the A fragments are loaded by ldmatrix (128-pixel
+ *                             tiles).  Bit-identical to 0 = the per-tap split
+ *   igemm_wide (0-1, 1)       read only when igemm_presplit is 1: the layers fcuda_igemm_wide_tile names run with the
+ *                             GEMM turned around (output channels on the wgmma M side, 224 pixels per warpgroup on N,
+ *                             read from the split planes by descriptor), so each filter byte serves 1.75x (N tile 128)
+ *                             or 3.5x (N tile 64) as many pixels.  Bit-identical to 0 = the pre-split kernel
  * Every variant computes the same result (tests/test_gpu_variants.py).  Returns 0 / the value, -200 for an unknown name or value. */
 int fcuda_set_tuning(const char* name, int value);
 int fcuda_get_tuning(const char* name);

@@ -1,8 +1,9 @@
 """Per-layer timing of the implicit-GEMM convolution (SGECONV), switch --switch at 0 against 1: igemm_presplit (default:
-the pre-split halo kernel against the per-tap split) or igemm_halo (the halo kernel against the gathering kernel), for
+the pre-split halo kernel against the per-tap split), igemm_wide (the wide pre-split kernel against the pre-split kernel)
+or igemm_halo (the halo kernel against the gathering kernel), for
 every layer of the benchmark nets that fcuda_conv_select_algo_tuned sends to SGECONV, at the nets' benchmark batch sizes.
 
-    python scripts/igemm_layer_bench.py --out DIR [--reps 5] [--iters 20] [--switch igemm_presplit]
+    python scripts/igemm_layer_bench.py --out DIR [--reps 5] [--iters 20] [--switch igemm_presplit|igemm_wide|igemm_halo]
 
 For each layer: CUDA-event time per launch of both kernels (alternated over --reps repetitions; median and every value),
 the algorithmic rate (direct-convolution FLOPs), the issued tensor-pipe rate (padded patch pixels, N tiles and the three
@@ -77,7 +78,7 @@ def main() -> None:
     ap.add_argument("--reps", type=int, default=5)
     ap.add_argument("--iters", type=int, default=20, help="launches per timed repetition")
     ap.add_argument("--models", default="vgg16,resnet50,mobilenet_v1")
-    ap.add_argument("--switch", default="igemm_presplit", choices=["igemm_presplit", "igemm_halo"])
+    ap.add_argument("--switch", default="igemm_presplit", choices=["igemm_presplit", "igemm_wide", "igemm_halo"])
     args = ap.parse_args()
 
     import torch
@@ -145,6 +146,8 @@ def main() -> None:
                 halo = lib.fcuda_igemm_halo_tile(ctypes.byref(p), geom) == 1
                 pgeom = (ctypes.c_int * 4)()
                 presplit = lib.fcuda_igemm_presplit_tile(ctypes.byref(p), pgeom) == 1
+                wgeom = (ctypes.c_int * 4)()
+                wide = lib.fcuda_igemm_wide_tile(ctypes.byref(p), wgeom) == 1
                 t = {0: [], 1: []}
                 outs = {}
                 for _ in range(args.reps):
@@ -159,7 +162,10 @@ def main() -> None:
                 bn = 32 if oc // group <= 32 else 64 if oc // group <= 64 else 128
                 ocp = -(-(oc // group) // bn) * bn * group
                 kpad = -(-((ic // group) * k * k) // 32) * 32
-                if halo:
+                if wide and args.switch == "igemm_wide":
+                    r, c = wgeom[0], wgeom[1]
+                    pix = n * (-(-p.output_h // r) * r) * (-(-p.output_w // c) * c)
+                elif halo:
                     r, c = geom[0], geom[1]
                     pix = n * (-(-p.output_h // r) * r) * (-(-p.output_w // c) * c)
                 elif pool:
@@ -170,7 +176,8 @@ def main() -> None:
 
                 def l2_to_sm_bytes(g):
                     """Filter ring stages + input boxes one launch fetches: per tile, every k-block's filter stage and
-                    one box of 32 channels x box rows x box columns (fp32) per channel block."""
+                    one box of 32 channels x box rows x box columns (fp32) per channel block (the wide kernel fetches
+                    it as two 16-channel halves: the same bytes)."""
                     r, c, rb, cb = g[0], g[1], g[2], g[3]
                     tiles = n * -(-p.output_h // r) * -(-p.output_w // c) * (ocp // bn)
                     stage = bn * 32 * (2 if result["precision"] == "fp32split" else 4) * (1 if result["precision"] == "tf32" else 2)
@@ -197,11 +204,13 @@ def main() -> None:
                        "winograd_f63_ms_reference_only": wino_ms,
                        "presplit_tile_rows_cols_box": list(pgeom) if presplit else None,
                        "l2_to_sm_bytes_halo": l2_to_sm_bytes(geom) if halo else None,
-                       "l2_to_sm_bytes_presplit": l2_to_sm_bytes(pgeom) if presplit else None}
+                       "l2_to_sm_bytes_presplit": l2_to_sm_bytes(pgeom) if presplit else None,
+                       "wide_tile_rows_cols_box": list(wgeom) if wide else None,
+                       "l2_to_sm_bytes_wide": l2_to_sm_bytes(wgeom) if wide else None}
                 result["layers"].append(rec)
                 print(json.dumps({k2: rec[k2] for k2 in ("model", "layer", "old_ms_median", "new_ms_median", "speedup",
                                                           "bit_identical", "algo_tflops_new", "issued_tflops_new",
-                                                          "l2_to_sm_bytes_presplit")}),
+                                                          "l2_to_sm_bytes_presplit", "l2_to_sm_bytes_wide")}),
                       flush=True)
                 torch.cuda.empty_cache()
     finally:
