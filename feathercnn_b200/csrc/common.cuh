@@ -54,6 +54,16 @@ static inline int ensure_dynamic_smem(Kernel kern, int bytes, SmemAttrCache& cac
     return 0;
 }
 
+// Grid of a persistent kernel: as many CTAs as fit on the device at once (occupancy x SMs), at most one per tile.
+template <class Kernel>
+static inline int persistent_grid(Kernel kern, int threads, int smem, long long tiles, unsigned* grid) {
+    int per_sm = 0;
+    FCUDA_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, threads, smem));
+    const long long slots = static_cast<long long>(sm_count()) * (per_sm > 0 ? per_sm : 1);
+    *grid = static_cast<unsigned>(tiles < slots ? tiles : slots);
+    return 0;
+}
+
 // Split an fp32 value into a TF32-representable "hi" (round-to-nearest on the 13 dropped
 // mantissa bits) and the exact fp32 remainder "lo".  hi + lo == v exactly; the tensor
 // core then truncates lo to TF32, leaving a relative error of ~2^-22 per operand.

@@ -33,6 +33,7 @@
 
 #include <stdlib.h>
 #include <string.h>
+#include "tensor_gemm.cuh"
 #include "wgmma.cuh"
 #include <cuda_bf16.h>
 
@@ -44,22 +45,6 @@ constexpr int kConsumerWarps = 8;                      // two warpgroups x 64 pi
 constexpr int kThreadsIg = (kConsumerWarps + 1) * 32;  // + the filter producer warp
 constexpr int kStagesIg = 4;
 constexpr int kMaxTableK = 6144;                       // k-table entries that fit beside the filter ring
-
-typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
-                                  const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
-                                  CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-
-EncodeTiledFn encode_fn() {
-    static EncodeTiledFn fn = nullptr;
-    if (!fn) {
-        void* p = nullptr;
-        cudaDriverEntryPointQueryResult q;
-        if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &q) == cudaSuccess &&
-            q == cudaDriverEntryPointSuccess)
-            fn = reinterpret_cast<EncodeTiledFn>(p);
-    }
-    return fn;
-}
 
 struct IgemmArgs {
     const float* residual;   // added to the output before the activation, or null
@@ -90,6 +75,27 @@ __device__ __forceinline__ int frag_k(int j, int c) {
     return BF ? (j >> 2) * 16 + 2 * c + (j & 1) + 8 * ((j >> 1) & 1) : (j >> 1) * 8 + c + 4 * (j & 1);
 }
 
+// Producer (lane 0): filter ring stage kbg % kStagesIg, once every consumer warp has released it, receives k-block kb of
+// N tile n_blk: the pre-tiled BF16x3 planes by one 1-D bulk copy, or the hi (+ lo) rows by 128-byte-swizzled TMA tiles.
+template <int BN, int PLANES>
+__device__ __forceinline__ void load_filter_stage(uint8_t* smem, uint64_t* full_bar, uint64_t* empty_bar, int kbg, int kb,
+                                                  int n_blk, const CUtensorMap* tmW, const CUtensorMap* tmWlo,
+                                                  const unsigned char* wbf, unsigned wbf_kb_bytes) {
+    constexpr int kBTile = BN * 32 * (PLANES == 3 ? 2 : 4);
+    constexpr int kStage = (PLANES == 3 ? 2 : PLANES) * kBTile;
+    const int stage = kbg % kStagesIg;
+    if (kbg >= kStagesIg) ptx::mbar_wait_nocall(&empty_bar[stage], ((kbg / kStagesIg) - 1) & 1);
+    uint8_t* st = smem + stage * kStage;
+    ptx::mbar_arrive_expect_tx(&full_bar[stage], kStage);
+    if (PLANES == 3) {
+        ptx::bulk_load_1d(st, wbf + static_cast<size_t>(kb) * wbf_kb_bytes + static_cast<size_t>(n_blk) * kStage, kStage,
+                          &full_bar[stage]);
+    } else {
+        ptx::tma_load_3d(st, tmW, &full_bar[stage], kb * 32, n_blk * BN, 0);
+        if (PLANES == 2) ptx::tma_load_3d(st + kBTile, tmWlo, &full_bar[stage], kb * 32, n_blk * BN, 0);
+    }
+}
+
 template <int BN, int PLANES>
 __global__ void __launch_bounds__(kThreadsIg, 1)
 conv_igemm_kernel(const __grid_constant__ CUtensorMap tmW, const __grid_constant__ CUtensorMap tmWlo,
@@ -112,10 +118,7 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tmW, const __grid_constant
     const int plane = args.H * args.W;
 
     if (threadIdx.x == 0) {
-        for (int s = 0; s < kStagesIg; ++s) {
-            ptx::mbar_init(&full_bar[s], 1);
-            ptx::mbar_init(&empty_bar[s], kConsumerWarps);
-        }
+        ptx::mbar_init_ring(full_bar, empty_bar, kStagesIg, kConsumerWarps);
         ptx::fence_barrier_init();
     }
     if (args.use_table) {
@@ -138,19 +141,9 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tmW, const __grid_constant
                 ptx::prefetch_tensormap(&tmW);
                 if (NPL == 2) ptx::prefetch_tensormap(&tmWlo);
             }
-            for (int kb = 0; kb < kblocks; ++kb) {
-                const int stage = kb % kStagesIg;
-                if (kb >= kStagesIg) ptx::mbar_wait_nocall(&empty_bar[stage], ((kb / kStagesIg) - 1) & 1);
-                uint8_t* st = smem + stage * kStage;
-                ptx::mbar_arrive_expect_tx(&full_bar[stage], kStage);
-                if (BF) {
-                    ptx::bulk_load_1d(st, args.wbf + static_cast<size_t>(kb) * args.wbf_kb_bytes + static_cast<size_t>(n_blk) * kStage,
-                                      kStage, &full_bar[stage]);
-                } else {
-                    ptx::tma_load_3d(st, &tmW, &full_bar[stage], kb * 32, n_blk * BN, 0);
-                    if (NPL == 2) ptx::tma_load_3d(st + kBTile, &tmWlo, &full_bar[stage], kb * 32, n_blk * BN, 0);
-                }
-            }
+            for (int kb = 0; kb < kblocks; ++kb)
+                load_filter_stage<BN, PLANES>(smem, full_bar, empty_bar, kb, kb, n_blk, &tmW, &tmWlo, args.wbf,
+                                              args.wbf_kb_bytes);
         }
         return;
     }
@@ -232,52 +225,12 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tmW, const __grid_constant
         const int stage = kb % kStagesIg;
         // split this k-block's operand into the fragments, then start the next k-block's loads
         uint32_t f1[4][4], f2[4][4];  // [k-step][a0..a3]: hi / p1 and lo / p2
-        if (BF) {
-#pragma unroll
-            for (int kk = 0; kk < 2; ++kk)
-#pragma unroll
-                for (int q = 0; q < 4; ++q) {  // a0 (row gq, pair 0), a1 (row gq + 8, pair 0), a2 (gq, pair 1), a3 (gq + 8, pair 1)
-                    const int h = q & 1, j = 4 * kk + 2 * (q >> 1);
-                    split_bf16x2(raw[h][j], raw[h][j + 1], f1[kk][q], f2[kk][q]);
-                }
-        } else {
-#pragma unroll
-            for (int kk = 0; kk < 4; ++kk)
-#pragma unroll
-                for (int q = 0; q < 4; ++q) {
-                    const float x = raw[q & 1][2 * kk + (q >> 1)];
-                    if (PLANES == 2) split_tf32_trunc(x, f1[kk][q], f2[kk][q]);
-                    else f1[kk][q] = __float_as_uint(x);
-                }
-        }
+        split_fragments<PLANES>(raw, f1, f2);
         if (kb + 1 < kblocks) gather(kb + 1, raw);
         ptx::mbar_wait_nocall(&full_bar[stage], (kb / kStagesIg) & 1);
         const uint32_t b_base = ptx::smem_u32(smem + stage * kStage);
         ptx::wgmma_fence();
-        if (BF) {
-            // un-swizzled core matrices: LBO = 128 B between k chunks, SBO = 512 B between 8-row groups; a k-step = 2 chunks
-            const uint64_t dQ1 = make_smem_desc_none(b_base, 128, 512);
-            const uint64_t dQ2 = make_smem_desc_none(b_base + kBTile, 128, 512);
-#pragma unroll
-            for (int kk = 0; kk < 2; ++kk) {
-                Wgmma<BN, 0>::mma(acc, f2[kk], dQ1 + 16 * kk, 1u);  // p2 * q1
-                Wgmma<BN, 0>::mma(acc, f1[kk], dQ2 + 16 * kk, 1u);  // p1 * q2
-                Wgmma<BN, 0>::mma(acc, f1[kk], dQ1 + 16 * kk, 1u);  // p1 * q1
-            }
-        } else {
-            const uint64_t dB = make_smem_desc_sw128(b_base);
-            const uint64_t dBlo = make_smem_desc_sw128(b_base + kBTile);
-#pragma unroll
-            for (int kk = 0; kk < 4; ++kk) {
-                if (PLANES == 2) {
-                    Wgmma<BN, 1>::mma(acc, f2[kk], dB + 2 * kk, 1u);    // A_lo * B_hi
-                    Wgmma<BN, 1>::mma(acc, f1[kk], dBlo + 2 * kk, 1u);  // A_hi * B_lo
-                    Wgmma<BN, 1>::mma(acc, f1[kk], dB + 2 * kk, 1u);    // A_hi * B_hi
-                } else {
-                    Wgmma<BN, 1>::mma(acc, f1[kk], dB + 2 * kk, 1u);
-                }
-            }
-        }
+        mma_kblock<BN, PLANES>(acc, f1, f2, b_base, b_base + kBTile);
         ptx::wgmma_commit();
         ptx::wgmma_wait<0>();
         __syncwarp();
@@ -388,6 +341,34 @@ igemm_pack_weights_bf16_kernel(const float* __restrict__ w, __nv_bfloat16* __res
 static int igemm_bn_for(int OC) { return OC <= 32 ? 32 : OC <= 64 ? 64 : 128; }
 static int igemm_ocpad(int OC) { const int bn = igemm_bn_for(OC); return (OC + bn - 1) / bn * bn; }
 
+// Tensor maps of the 3xTF32 / TF32 filter planes: K-major rows of Kf = K rounded up to 4, boxes of 32 k-values x BN rows.
+// The pre-tiled BF16x3 planes are fetched by 1-D bulk copies and need none.
+static int filter_maps(const IgemmProblem& p, int BN, int planes, CUtensorMap* tmW, CUtensorMap* tmWlo) {
+    memset(tmW, 0, sizeof(*tmW));
+    *tmWlo = *tmW;
+    if (planes == 3) return 0;
+    const int Kf = (p.KH * p.KW * p.IC + 3) & ~3;
+    if (int rc = make_map(tmW, p.w_hi, Kf, p.OC, 1, 0, BN)) return rc;
+    return planes == 2 ? make_map(tmWlo, p.w_lo, Kf, p.OC, 1, 0, BN) : 0;
+}
+
+// The pre-tiled BF16x3 planes were packed for this N tile, and their byte offsets stay 32-bit
+static bool bf16_filters_fit(const IgemmProblem& p, int BN) {
+    return igemm_bn_for(p.OC) == BN &&
+           static_cast<unsigned long long>(ceil_div(p.KH * p.KW * p.IC, 32)) * igemm_ocpad(p.OC) * 128ull < (1ull << 31);
+}
+
+// Profile record of an implicit-GEMM launch: the layer's algorithmic work (direct-convolution FLOPs; input + filters read
+// once, output written once) and the MMA work issued over `tile_pixels` (padded) pixels x `n_cols` channels x `kblocks`.
+static int prof_igemm(const IgemmProblem& p, cudaStream_t stream, long long tile_pixels, int n_cols, int kblocks) {
+    const int taps = p.KH * p.KW;
+    const double macs = static_cast<double>(p.N) * p.OC * p.OH * p.OW * p.IC * taps;
+    const double mma = 2.0 * static_cast<double>(tile_pixels) * n_cols * (kblocks * 32) * (p.planes >= 2 ? 3 : 1);
+    return prof_begin(stream, PROF_IGEMM, 2.0 * macs, mma,
+                      4.0 * (static_cast<double>(p.N) * p.IC * p.H * p.W + static_cast<double>(p.OC) * taps * p.IC +
+                             static_cast<double>(p.N) * p.OC * p.OH * p.OW * (p.residual ? 2 : 1)));
+}
+
 template <int BN, int PLANES>
 int launch_igemm(const IgemmProblem& p, cudaStream_t stream) {
     constexpr bool BF = PLANES == 3;
@@ -395,31 +376,11 @@ int launch_igemm(const IgemmProblem& p, cudaStream_t stream) {
     const int taps = p.KH * p.KW;
     const int K = taps * p.IC;
     CUtensorMap tmW, tmWlo;
-    memset(&tmW, 0, sizeof(tmW));
-    tmWlo = tmW;
-    if (!BF) {  // the BF16x3 planes are pre-tiled and fetched by 1-D bulk copies: no tensor map
-        EncodeTiledFn enc = encode_fn();
-        if (!enc) return FCUDA_ERR_CUDA;
-        const int Kf = (K + 3) & ~3;
-        for (int pl = 0; pl < NPL; ++pl) {
-            cuuint64_t dims[3] = {(cuuint64_t)Kf, (cuuint64_t)p.OC, 1};
-            cuuint64_t strides[2] = {(cuuint64_t)Kf * 4, (cuuint64_t)Kf * p.OC * 4};
-            cuuint32_t box[3] = {32, (cuuint32_t)BN, 1};
-            cuuint32_t estr[3] = {1, 1, 1};
-            const float* base = pl == 0 ? p.w_hi : p.w_lo;
-            CUresult r = enc(pl == 0 ? &tmW : &tmWlo, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, const_cast<float*>(base), dims, strides,
-                             box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
-                             CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-            if (r != CUDA_SUCCESS) {
-                fprintf(stderr, "fcuda: igemm weight tensor map failed (%d)\n", (int)r);
-                return FCUDA_ERR_CUDA;
-            }
-        }
-    }
+    if (int rc = filter_maps(p, BN, PLANES, &tmW, &tmWlo)) return rc;
+    if (BF && !bf16_filters_fit(p, BN)) return -1;
     IgemmArgs a;
     a.wbf = reinterpret_cast<const unsigned char*>(p.w_hi);
     a.wbf_kb_bytes = 2u * static_cast<unsigned>(igemm_ocpad(p.OC)) * 64u;
-    if (BF && (igemm_bn_for(p.OC) != BN || static_cast<unsigned long long>(ceil_div(K, 32)) * igemm_ocpad(p.OC) * 128ull >= (1ull << 31))) return -1;
     a.in = p.input; a.out = p.output; a.bias = p.bias; a.residual = p.residual;
     a.N = p.N; a.IC = p.IC; a.H = p.H; a.W = p.W; a.OC = p.OC; a.OH = p.OH; a.OW = p.OW;
     a.KH = p.KH; a.KW = p.KW; a.pad_top = p.pad_top; a.pad_left = p.pad_left;
@@ -453,12 +414,7 @@ int launch_igemm(const IgemmProblem& p, cudaStream_t stream) {
     auto kern = conv_igemm_kernel<BN, PLANES>;
     static SmemAttrCache attr_cache;
     if (int rc = ensure_dynamic_smem(kern, smem, attr_cache)) return rc;
-    // algorithmic work of the layer: direct-convolution FLOPs; input + filters read once, output written once
-    const double macs = static_cast<double>(p.N) * p.OC * p.OH * p.OW * p.IC * taps;
-    const double mma = 2.0 * static_cast<double>(pixel_tiles) * 128 * (a.num_n * BN) * (a.kblocks * 32) * (PLANES >= 2 ? 3 : 1);
-    const int prof = prof_begin(stream, PROF_IGEMM, 2.0 * macs, mma,
-                                4.0 * (static_cast<double>(p.N) * p.IC * p.H * p.W + static_cast<double>(p.OC) * K +
-                                       static_cast<double>(p.N) * p.OC * p.OH * p.OW * (p.residual ? 2 : 1)));
+    const int prof = prof_igemm(p, stream, pixel_tiles * 128, a.num_n * BN, a.kblocks);
     kern<<<static_cast<unsigned>(total), kThreadsIg, smem, stream>>>(tmW, tmWlo, a);
     prof_end(prof, stream);
     FCUDA_CHECK_LAUNCH();
@@ -506,6 +462,20 @@ struct HaloArgs {
     int pr, pc;            // conv_igemm_presplit_kernel: rows x columns of the bf16 planes (R + KH - 1, C + KW - 1)
 };
 
+// Tile t of the halo kernels: N tile n_blk of the R x C patch (ty, tx) of image img
+struct HaloTile { int n_blk, img, ty, tx; };
+
+__device__ __forceinline__ HaloTile halo_tile(const HaloArgs& args, int per_img, long long t) {
+    HaloTile h;
+    h.n_blk = static_cast<int>(t % args.num_n);
+    const long long pt = t / args.num_n;
+    h.img = static_cast<int>(pt / per_img);
+    const int rem = static_cast<int>(pt - static_cast<long long>(h.img) * per_img);
+    h.ty = rem / args.tiles_x;
+    h.tx = rem - h.ty * args.tiles_x;
+    return h;
+}
+
 // Epilogue of the halo kernels for one m64 accumulator (as conv_igemm_kernel): this thread's pixels are rows oy[0..1]
 // of column ox in image img.
 template <int BN>
@@ -539,6 +509,36 @@ __device__ __forceinline__ void halo_epilogue(const float (&acc)[BN / 2], const 
     }
 }
 
+// Box word offset of every 16-byte row of the pre-split planes [ch / 8][pr][pc][8 ch]: the `units` rows of 8 channels
+// a box (or half box) covers.  Filled by the whole CTA.
+__device__ __forceinline__ void fill_unit_table(int* utab, int units, const HaloArgs& args) {
+    const int cstride = args.Rb * args.Cb;
+    for (int u = threadIdx.x; u < units; u += kThreadsIg) {
+        const int ch8 = u / (args.pr * args.pc), rem = u - ch8 * args.pr * args.pc;
+        const int row = rem / args.pc, col = rem - row * args.pc;
+        utab[u] = 8 * ch8 * cstride + row * args.Cb + col + args.xshift;
+    }
+}
+
+// The consumers' share of splitting `units` 16-byte rows of an fp32 box (channel planes cstride floats apart, rows at
+// box + utab[u]) into the bf16 planes p1 at shared address dst and p2 at dst + pbytes, with split_bf16x2: the bits of
+// the per-tap split.
+__device__ __forceinline__ void split_box(const float* box, const int* utab, int cstride, int units, uint32_t dst,
+                                          uint32_t pbytes) {
+#pragma unroll 1
+    for (int u = threadIdx.x; u < units; u += kConsumerWarps * 32) {
+        const float* s = box + utab[u];
+        float x[8];
+#pragma unroll
+        for (int i = 0; i < 8; ++i) x[i] = s[i * cstride];
+        uint32_t p1[4], p2[4];
+#pragma unroll
+        for (int w = 0; w < 4; ++w) split_bf16x2(x[2 * w], x[2 * w + 1], p1[w], p2[w]);
+        ptx::st_shared_v4(dst + 16u * u, p1);
+        ptx::st_shared_v4(dst + pbytes + 16u * u, p2);
+    }
+}
+
 // Producer warp of the halo kernels (lane 0 only): the HS-deep ring of input boxes and the filter ring, in consumption
 // order.  A tile is args.R x args.C output pixels; its box for channel block cb starts at (x0 - xpad, y0 - pad_top).
 template <int BN, int PLANES, int HS>
@@ -546,30 +546,23 @@ __device__ __forceinline__ void halo_producer(const CUtensorMap* tmX, const CUte
                                               const HaloArgs& args, uint8_t* smem, float* halo, int hstage,
                                               uint64_t* full_bar, uint64_t* empty_bar, uint64_t* hfull_bar,
                                               uint64_t* hempty_bar) {
-    constexpr bool BF = PLANES == 3;
-    constexpr int NPL = BF ? 2 : PLANES;
-    constexpr int kBTile = BN * 32 * (BF ? 2 : 4);
-    constexpr int kStage = NPL * kBTile;
     const int per_img = args.tiles_x * args.tiles_y;
     const int taps = args.taps;
     const int ncb = args.kblocks / taps;
     ptx::prefetch_tensormap(tmX);
-    if (!BF) {
+    if (PLANES != 3) {
         ptx::prefetch_tensormap(tmW);
-        if (NPL == 2) ptx::prefetch_tensormap(tmWlo);
+        if (PLANES == 2) ptx::prefetch_tensormap(tmWlo);
     }
     int hb = 0;   // boxes issued
     int kbg = 0;  // filter stages issued
     auto load_halo = [&](long long t, int cb) {
-        const long long pt = t / args.num_n;
-        const int n = static_cast<int>(pt / per_img);
-        const int rem = static_cast<int>(pt - static_cast<long long>(n) * per_img);
-        const int ty = rem / args.tiles_x, tx = rem - ty * args.tiles_x;
+        const HaloTile h = halo_tile(args, per_img, t);
         const int hs = hb % HS;
         if (hb >= HS) ptx::mbar_wait_nocall(&hempty_bar[hs], ((hb / HS) - 1) & 1);
         ptx::mbar_arrive_expect_tx(&hfull_bar[hs], static_cast<uint32_t>(hstage) * 4u);
-        ptx::tma_load_4d(halo + hs * hstage, tmX, &hfull_bar[hs], tx * args.C - args.xpad, ty * args.R - args.pad_top,
-                         cb * 32, n);
+        ptx::tma_load_4d(halo + hs * hstage, tmX, &hfull_bar[hs], h.tx * args.C - args.xpad, h.ty * args.R - args.pad_top,
+                         cb * 32, h.img);
         ++hb;
     };
     if (blockIdx.x < args.tiles) load_halo(blockIdx.x, 0);
@@ -577,17 +570,8 @@ __device__ __forceinline__ void halo_producer(const CUtensorMap* tmX, const CUte
         const int n_blk = static_cast<int>(t % args.num_n);
         for (int cb = 0, kb = 0; cb < ncb; ++cb) {
             for (int tap = 0; tap < taps; ++tap, ++kb, ++kbg) {
-                const int stage = kbg % kStagesIg;
-                if (kbg >= kStagesIg) ptx::mbar_wait_nocall(&empty_bar[stage], ((kbg / kStagesIg) - 1) & 1);
-                uint8_t* st = smem + stage * kStage;
-                ptx::mbar_arrive_expect_tx(&full_bar[stage], kStage);
-                if (BF) {
-                    ptx::bulk_load_1d(st, args.wbf + static_cast<size_t>(kb) * args.wbf_kb_bytes + static_cast<size_t>(n_blk) * kStage,
-                                      kStage, &full_bar[stage]);
-                } else {
-                    ptx::tma_load_3d(st, tmW, &full_bar[stage], kb * 32, n_blk * BN, 0);
-                    if (NPL == 2) ptx::tma_load_3d(st + kBTile, tmWlo, &full_bar[stage], kb * 32, n_blk * BN, 0);
-                }
+                load_filter_stage<BN, PLANES>(smem, full_bar, empty_bar, kbg, kb, n_blk, tmW, tmWlo, args.wbf,
+                                              args.wbf_kb_bytes);
                 if (tap == 0) {  // the next box (this tile's next channel block or the next tile's first) lands meanwhile
                     if (cb + 1 < ncb) load_halo(t, cb + 1);
                     else if (t + gridDim.x < args.tiles) load_halo(t + gridDim.x, 0);
@@ -622,14 +606,8 @@ conv_igemm_halo_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_con
     const int kblocks = args.kblocks, taps = args.taps;
 
     if (threadIdx.x == 0) {
-        for (int s = 0; s < kStagesIg; ++s) {
-            ptx::mbar_init(&full_bar[s], 1);
-            ptx::mbar_init(&empty_bar[s], kConsumerWarps);
-        }
-        for (int s = 0; s < kHaloStages; ++s) {
-            ptx::mbar_init(&hfull_bar[s], 1);
-            ptx::mbar_init(&hempty_bar[s], kConsumerWarps);
-        }
+        ptx::mbar_init_ring(full_bar, empty_bar, kStagesIg, kConsumerWarps);
+        ptx::mbar_init_ring(hfull_bar, hempty_bar, kHaloStages, kConsumerWarps);
         ptx::fence_barrier_init();
     }
     __syncthreads();
@@ -656,37 +634,13 @@ conv_igemm_halo_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_con
 #pragma unroll
             for (int j = 0; j < 8; ++j) raw[h][j] = box[abase + toff + h * args.Cb + frag_k<BF>(j, 0) * cstride];
     };
-    auto split = [&](const float (&raw)[2][8], uint32_t (&f1)[4][4], uint32_t (&f2)[4][4]) {
-        if (BF) {
-#pragma unroll
-            for (int kk = 0; kk < 2; ++kk)
-#pragma unroll
-                for (int q = 0; q < 4; ++q) {
-                    const int h = q & 1, j = 4 * kk + 2 * (q >> 1);
-                    split_bf16x2(raw[h][j], raw[h][j + 1], f1[kk][q], f2[kk][q]);
-                }
-        } else {
-#pragma unroll
-            for (int kk = 0; kk < 4; ++kk)
-#pragma unroll
-                for (int q = 0; q < 4; ++q) {
-                    const float x = raw[q & 1][2 * kk + (q >> 1)];
-                    if (PLANES == 2) split_tf32_trunc(x, f1[kk][q], f2[kk][q]);
-                    else f1[kk][q] = __float_as_uint(x);
-                }
-        }
-    };
-
     const int oplane = args.OH * args.OW;
     const int SH = (args.OH + 1) >> 1, SW = (args.OW + 1) >> 1;  // pooled geometry
     int kbg = 0;  // filter stages consumed
     int hb = 0;   // boxes consumed
     for (long long t = blockIdx.x; t < args.tiles; t += gridDim.x) {
-        const int n_blk = static_cast<int>(t % args.num_n);
-        const long long pt = t / args.num_n;
-        const int img = static_cast<int>(pt / per_img);
-        const int rem = static_cast<int>(pt - static_cast<long long>(img) * per_img);
-        const int ty = rem / args.tiles_x, tx = rem - ty * args.tiles_x;
+        const HaloTile tile = halo_tile(args, per_img, t);
+        const int n_blk = tile.n_blk, img = tile.img, ty = tile.ty, tx = tile.tx;
         int oy[2];
         bool valid[2];
         const int ox = tx * args.C + pcol;
@@ -706,7 +660,7 @@ conv_igemm_halo_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_con
         gather(halo + (hb % kHaloStages) * hstage, 0, raw);
 
         auto step = [&](uint32_t (&f1)[4][4], uint32_t (&f2)[4][4], int kb) {
-            split(raw, f1, f2);
+            split_fragments<PLANES>(raw, f1, f2);
             if (++tap == taps) {  // the box's last tap is in registers: hand the box back
                 tap = dy = dx = 0;
                 __syncwarp();
@@ -724,29 +678,7 @@ conv_igemm_halo_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_con
             ptx::mbar_wait_nocall(&full_bar[stage], (kbg / kStagesIg) & 1);
             const uint32_t b_base = ptx::smem_u32(smem + stage * kStage);
             ptx::wgmma_fence();
-            if (BF) {
-                const uint64_t dQ1 = make_smem_desc_none(b_base, 128, 512);
-                const uint64_t dQ2 = make_smem_desc_none(b_base + kBTile, 128, 512);
-#pragma unroll
-                for (int kk = 0; kk < 2; ++kk) {
-                    Wgmma<BN, 0>::mma(acc, f2[kk], dQ1 + 16 * kk, 1u);  // p2 * q1
-                    Wgmma<BN, 0>::mma(acc, f1[kk], dQ2 + 16 * kk, 1u);  // p1 * q2
-                    Wgmma<BN, 0>::mma(acc, f1[kk], dQ1 + 16 * kk, 1u);  // p1 * q1
-                }
-            } else {
-                const uint64_t dB = make_smem_desc_sw128(b_base);
-                const uint64_t dBlo = make_smem_desc_sw128(b_base + kBTile);
-#pragma unroll
-                for (int kk = 0; kk < 4; ++kk) {
-                    if (PLANES == 2) {
-                        Wgmma<BN, 1>::mma(acc, f2[kk], dB + 2 * kk, 1u);    // A_lo * B_hi
-                        Wgmma<BN, 1>::mma(acc, f1[kk], dBlo + 2 * kk, 1u);  // A_hi * B_lo
-                        Wgmma<BN, 1>::mma(acc, f1[kk], dB + 2 * kk, 1u);    // A_hi * B_hi
-                    } else {
-                        Wgmma<BN, 1>::mma(acc, f1[kk], dB + 2 * kk, 1u);
-                    }
-                }
-            }
+            mma_kblock<BN, PLANES>(acc, f1, f2, b_base, b_base + kBTile);
             ptx::wgmma_commit();
             ptx::wgmma_wait<1>();  // k-block kb - 1 retired: its filter stage and fragment set are free
             __syncwarp();
@@ -807,21 +739,11 @@ conv_igemm_presplit_kernel(const __grid_constant__ CUtensorMap tmX, const HaloAr
     const int ncb = args.kblocks / taps;
 
     if (threadIdx.x == 0) {
-        for (int s = 0; s < kStagesIg; ++s) {
-            ptx::mbar_init(&full_bar[s], 1);
-            ptx::mbar_init(&empty_bar[s], kConsumerWarps);
-        }
-        for (int s = 0; s < HS; ++s) {
-            ptx::mbar_init(&hfull_bar[s], 1);
-            ptx::mbar_init(&hempty_bar[s], kConsumerWarps);
-        }
+        ptx::mbar_init_ring(full_bar, empty_bar, kStagesIg, kConsumerWarps);
+        ptx::mbar_init_ring(hfull_bar, hempty_bar, HS, kConsumerWarps);
         ptx::fence_barrier_init();
     }
-    for (int u = threadIdx.x; u < units; u += kThreadsIg) {
-        const int ch8 = u / (args.pr * args.pc), rem = u - ch8 * args.pr * args.pc;
-        const int row = rem / args.pc, col = rem - row * args.pc;
-        const_cast<int*>(utab)[u] = 8 * ch8 * cstride + row * args.Cb + col + args.xshift;
-    }
+    fill_unit_table(const_cast<int*>(utab), units, args);
     __syncthreads();
 
     if (warp == kConsumerWarps) {
@@ -848,19 +770,7 @@ conv_igemm_presplit_kernel(const __grid_constant__ CUtensorMap tmX, const HaloAr
     auto convert_next = [&]() {
         const int hs = hb % HS;
         ptx::mbar_wait_nocall(&hfull_bar[hs], (hb / HS) & 1);
-        const float* box = halo + hs * hstage;
-        const uint32_t dst = planes + static_cast<uint32_t>(hb & 1) * 2u * pbytes;
-        for (int u = threadIdx.x; u < units; u += kConsumers) {
-            const float* s = box + utab[u];
-            float x[8];
-#pragma unroll
-            for (int i = 0; i < 8; ++i) x[i] = s[i * cstride];
-            uint32_t p1[4], p2[4];
-#pragma unroll
-            for (int w = 0; w < 4; ++w) split_bf16x2(x[2 * w], x[2 * w + 1], p1[w], p2[w]);
-            ptx::st_shared_v4(dst + 16u * u, p1);
-            ptx::st_shared_v4(dst + pbytes + 16u * u, p2);
-        }
+        split_box(halo + hs * hstage, utab, cstride, units, planes + static_cast<uint32_t>(hb & 1) * 2u * pbytes, pbytes);
         __syncwarp();
         ptx::mbar_arrive_if(&hempty_bar[hs], lane == 0);
         ++hb;
@@ -870,11 +780,8 @@ conv_igemm_presplit_kernel(const __grid_constant__ CUtensorMap tmX, const HaloAr
     const int SH = (args.OH + 1) >> 1, SW = (args.OW + 1) >> 1;
     convert_next();  // grid <= tiles: every CTA has a first box
     for (long long t = blockIdx.x; t < args.tiles; t += gridDim.x) {
-        const int n_blk = static_cast<int>(t % args.num_n);
-        const long long pt = t / args.num_n;
-        const int img = static_cast<int>(pt / per_img);
-        const int rem = static_cast<int>(pt - static_cast<long long>(img) * per_img);
-        const int ty = rem / args.tiles_x, tx = rem - ty * args.tiles_x;
+        const HaloTile tile = halo_tile(args, per_img, t);
+        const int n_blk = tile.n_blk, img = tile.img, ty = tile.ty, tx = tile.tx;
         const bool more_tiles = t + gridDim.x < args.tiles;
         const int kbg0 = kbg;
 
@@ -903,14 +810,7 @@ conv_igemm_presplit_kernel(const __grid_constant__ CUtensorMap tmX, const HaloAr
             ptx::mbar_wait_nocall(&full_bar[stage], (kbg / kStagesIg) & 1);
             const uint32_t b_base = ptx::smem_u32(smem) + stage * kStage;
             ptx::wgmma_fence();
-            const uint64_t dQ1 = make_smem_desc_none(b_base, 128, 512);
-            const uint64_t dQ2 = make_smem_desc_none(b_base + kBTile, 128, 512);
-#pragma unroll
-            for (int kk = 0; kk < 2; ++kk) {
-                Wgmma<BN, 0>::mma(acc, f2[kk], dQ1 + 16 * kk, 1u);  // p2 * q1
-                Wgmma<BN, 0>::mma(acc, f1[kk], dQ2 + 16 * kk, 1u);  // p1 * q2
-                Wgmma<BN, 0>::mma(acc, f1[kk], dQ1 + 16 * kk, 1u);  // p1 * q1
-            }
+            mma_kblock<BN, 3>(acc, f1, f2, b_base, b_base + kBTile);
             ptx::wgmma_commit();
             ptx::wgmma_wait<1>();  // k-block kbg - 1 retired: its filter stage and fragment set are free
             if (last && next) convert_next();
@@ -984,7 +884,6 @@ template <int BN>
 __device__ __forceinline__ void wide_producer(const CUtensorMap* tmX, const HaloArgs& args, uint8_t* smem, float* halo,
                                               int hstage, uint64_t* full_bar, uint64_t* empty_bar, uint64_t* hfull_bar,
                                               uint64_t* hempty_bar) {
-    constexpr int kStage = 2 * BN * 64;
     const int per_img = args.tiles_x * args.tiles_y;
     const int taps = args.taps;
     const int ncb = args.kblocks / taps;
@@ -993,13 +892,11 @@ __device__ __forceinline__ void wide_producer(const CUtensorMap* tmX, const Halo
     int nh = 0;   // half boxes issued
     int kbg = 0;  // filter stages issued
     auto load_half = [&](long long t, int cb, int h) {
-        const long long pt = t / args.num_n;
-        const int n = static_cast<int>(pt / per_img);
-        const int rem = static_cast<int>(pt - static_cast<long long>(n) * per_img);
-        const int ty = rem / args.tiles_x, tx = rem - ty * args.tiles_x;
+        const HaloTile tile = halo_tile(args, per_img, t);
         if (nh > 0) ptx::mbar_wait_nocall(hempty_bar, (nh - 1) & 1);
         ptx::mbar_arrive_expect_tx(hfull_bar, static_cast<uint32_t>(hstage) * 4u);
-        ptx::tma_load_4d(halo, tmX, hfull_bar, tx * args.C - args.xpad, ty * args.R - args.pad_top, cb * 32 + 16 * h, n);
+        ptx::tma_load_4d(halo, tmX, hfull_bar, tile.tx * args.C - args.xpad, tile.ty * args.R - args.pad_top,
+                         cb * 32 + 16 * h, tile.img);
         ++nh;
     };
     if (blockIdx.x < args.tiles) {
@@ -1010,12 +907,8 @@ __device__ __forceinline__ void wide_producer(const CUtensorMap* tmX, const Halo
         const int n_blk = static_cast<int>(t % args.num_n);
         for (int cb = 0, kb = 0; cb < ncb; ++cb) {
             for (int tap = 0; tap < taps; ++tap, ++kb, ++kbg) {
-                const int stage = kbg % kStagesIg;
-                if (kbg >= kStagesIg) ptx::mbar_wait_nocall(&empty_bar[stage], ((kbg / kStagesIg) - 1) & 1);
-                ptx::mbar_arrive_expect_tx(&full_bar[stage], kStage);
-                ptx::bulk_load_1d(smem + stage * kStage,
-                                  args.wbf + static_cast<size_t>(kb) * args.wbf_kb_bytes + static_cast<size_t>(n_blk) * kStage,
-                                  kStage, &full_bar[stage]);
+                load_filter_stage<BN, 3>(smem, full_bar, empty_bar, kbg, kb, n_blk, nullptr, nullptr, args.wbf,
+                                         args.wbf_kb_bytes);
                 if (tap == 2 || tap == p1) {
                     const int h = tap == 2 ? 0 : 1;
                     if (cb + 1 < ncb) load_half(t, cb + 1, h);
@@ -1102,19 +995,11 @@ conv_igemm_wide_kernel(const __grid_constant__ CUtensorMap tmX, const HaloArgs a
     const int ncb = args.kblocks / taps;
 
     if (threadIdx.x == 0) {
-        for (int s = 0; s < kStagesIg; ++s) {
-            ptx::mbar_init(&full_bar[s], 1);
-            ptx::mbar_init(&empty_bar[s], kConsumerWarps);
-        }
-        ptx::mbar_init(&hfull_bar, 1);
-        ptx::mbar_init(&hempty_bar, kConsumerWarps);
+        ptx::mbar_init_ring(full_bar, empty_bar, kStagesIg, kConsumerWarps);
+        ptx::mbar_init_ring(&hfull_bar, &hempty_bar, 1, kConsumerWarps);
         ptx::fence_barrier_init();
     }
-    for (int u = threadIdx.x; u < hunits; u += kThreadsIg) {
-        const int ch8 = u / (args.pr * args.pc), rem = u - ch8 * args.pr * args.pc;
-        const int row = rem / args.pc, col = rem - row * args.pc;
-        const_cast<int*>(utab)[u] = 8 * ch8 * cstride + row * args.Cb + col + args.xshift;
-    }
+    fill_unit_table(const_cast<int*>(utab), hunits, args);
     __syncthreads();
 
     if (warp == kConsumerWarps) {
@@ -1135,19 +1020,8 @@ conv_igemm_wide_kernel(const __grid_constant__ CUtensorMap tmX, const HaloArgs a
     // split half h of box nc / 2 into plane buffer (nc / 2) & 1 and hand the fp32 half box back
     auto convert_half = [&](int h) {
         ptx::mbar_wait_nocall(&hfull_bar, nc & 1);
-        const uint32_t dst = planes + static_cast<uint32_t>((nc >> 1) & 1) * 2u * pbytes + 16u * static_cast<uint32_t>(h * hunits);
-#pragma unroll 1
-        for (int u = threadIdx.x; u < hunits; u += kConsumers) {
-            const float* s = halo + utab[u];
-            float x[8];
-#pragma unroll
-            for (int i = 0; i < 8; ++i) x[i] = s[i * cstride];
-            uint32_t p1[4], p2[4];
-#pragma unroll
-            for (int w = 0; w < 4; ++w) split_bf16x2(x[2 * w], x[2 * w + 1], p1[w], p2[w]);
-            ptx::st_shared_v4(dst + 16u * u, p1);
-            ptx::st_shared_v4(dst + pbytes + 16u * u, p2);
-        }
+        split_box(halo, utab, cstride, hunits,
+                  planes + static_cast<uint32_t>((nc >> 1) & 1) * 2u * pbytes + 16u * static_cast<uint32_t>(h * hunits), pbytes);
         ptx::fence_proxy_async_smem();
         __syncwarp();
         ptx::mbar_arrive_if(&hempty_bar, lane == 0);
@@ -1212,14 +1086,10 @@ conv_igemm_wide_kernel(const __grid_constant__ CUtensorMap tmX, const HaloArgs a
         ptx::mbar_arrive_if(&empty_bar[(kbg - 1) & (kStagesIg - 1)], lane == 0);
 
         // the tile's coordinates, computed here rather than kept in registers through the main loop
-        const int n_blk = static_cast<int>(t % args.num_n);
-        const long long pt = t / args.num_n;
-        const int img = static_cast<int>(pt / per_img);
-        const int rem = static_cast<int>(pt - static_cast<long long>(img) * per_img);
-        const int ty = rem / args.tiles_x, tx = rem - ty * args.tiles_x;
-        const int oc0 = n_blk * BN + (BN == 128 ? 64 * wg : 0) + 16 * (warp & 3) + gq;
-        const int ox0 = tx * args.C + (BN == 64 ? 8 * wg : 0) + 2 * c;
-        wide_epilogue(acc, args, img, oc0, ty * kWideRows, ox0);
+        const HaloTile tile = halo_tile(args, per_img, t);
+        const int oc0 = tile.n_blk * BN + (BN == 128 ? 64 * wg : 0) + 16 * (warp & 3) + gq;
+        const int ox0 = tile.tx * args.C + (BN == 64 ? 8 * wg : 0) + 2 * c;
+        wide_epilogue(acc, args, tile.img, oc0, tile.ty * kWideRows, ox0);
     }
 }
 
@@ -1272,9 +1142,9 @@ static bool halo_geometry(const IgemmProblem& p, HaloGeom& g) {
 // Box of conv_igemm_presplit_kernel for a layer the halo kernel takes in BF16x3 mode, or false (the layer keeps the
 // halo kernel).  The patch is the halo kernel's; the box is the patch plus its halo, unpadded: the split reads it along
 // rows, free of bank conflicts at any plane stride.
-static int presplit_smem_bytes(int OC, int Rb, int Cb, int pr, int pc) {
-    const int units = 4 * pr * pc;
-    return kStagesIg * 2 * igemm_bn_for(OC) * 64 + kHaloStages * 32 * Rb * Cb * 4 + 2 * 32 * units + 4 * units + 1024;
+static int presplit_smem_bytes(const IgemmProblem& p, const HaloGeom& g) {
+    const int units = 4 * (g.R + p.KH - 1) * (g.C + p.KW - 1);
+    return kStagesIg * 2 * igemm_bn_for(p.OC) * 64 + kHaloStages * 32 * g.Rb * g.Cb * 4 + 2 * 32 * units + 4 * units + 1024;
 }
 
 static bool presplit_geometry(const IgemmProblem& p, HaloGeom& g) {
@@ -1284,13 +1154,13 @@ static bool presplit_geometry(const IgemmProblem& p, HaloGeom& g) {
     g.R = h.R; g.C = h.C;
     g.Rb = h.R + p.KH - 1;
     g.Cb = (h.C + p.KW - 1 + xshift + 3) & ~3;
-    return presplit_smem_bytes(p.OC, g.Rb, g.Cb, g.Rb, h.C + p.KW - 1) <= 227 * 1024;
+    return presplit_smem_bytes(p, g) <= 227 * 1024;
 }
 
 // Filter ring, one fp32 half box, two plane buffers and the unit table of conv_igemm_wide_kernel
-static int wide_smem_bytes(int OC, int Rb, int Cb, int pr, int pc) {
-    const int hunits = 2 * pr * pc;
-    return kStagesIg * 2 * igemm_bn_for(OC) * 64 + 16 * Rb * Cb * 4 + 2 * 64 * hunits + 4 * hunits + 1024;
+static int wide_smem_bytes(const IgemmProblem& p, const HaloGeom& g) {
+    const int hunits = 2 * (g.R + p.KH - 1) * (g.C + p.KW - 1);
+    return kStagesIg * 2 * igemm_bn_for(p.OC) * 64 + 16 * g.Rb * g.Cb * 4 + 2 * 64 * hunits + 4 * hunits + 1024;
 }
 
 // Tile and box of conv_igemm_wide_kernel for a layer that takes the pre-split kernel, or false (the layer keeps it): N
@@ -1306,12 +1176,14 @@ static bool wide_geometry(const IgemmProblem& p, HaloGeom& g) {
     g.R = R; g.C = C;
     g.Rb = R + p.KH - 1;
     g.Cb = (C + p.KW - 1 + xshift + 3) & ~3;
-    return wide_smem_bytes(p.OC, g.Rb, g.Cb, g.Rb, C + p.KW - 1) <= 227 * 1024;
+    return wide_smem_bytes(p, g) <= 227 * 1024;
 }
 
 // The input blob [N][in_img_c][H][W] (the IC channels of this slice) in boxes of hg.Cb x hg.Rb x `chans` channels; boxes
 // past its edges read as zeros
-static int halo_input_map(const IgemmProblem& p, const HaloGeom& hg, EncodeTiledFn enc, CUtensorMap* tmX, int chans = 32) {
+static int halo_input_map(const IgemmProblem& p, const HaloGeom& hg, int chans, CUtensorMap* tmX) {
+    EncodeTiledFn enc = encode_tiled_fn();
+    if (!enc) return FCUDA_ERR_CUDA;
     const cuuint64_t in_c = static_cast<cuuint64_t>(p.in_c_total > 0 ? p.in_c_total : p.IC);
     cuuint64_t dims[4] = {(cuuint64_t)p.W, (cuuint64_t)p.H, (cuuint64_t)p.IC, (cuuint64_t)p.N};
     cuuint64_t strides[3] = {(cuuint64_t)p.W * 4, (cuuint64_t)p.W * p.H * 4, in_c * p.H * p.W * 4};
@@ -1352,146 +1224,65 @@ static HaloArgs halo_args(const IgemmProblem& p, const HaloGeom& hg, int BN) {
     return a;
 }
 
-template <int BN>
-int launch_igemm_presplit(const IgemmProblem& p, const HaloGeom& hg, cudaStream_t stream) {
-    EncodeTiledFn enc = encode_fn();
-    if (!enc) return FCUDA_ERR_CUDA;
+// Launch of a halo-family kernel on tile geometry hg: input boxes of `box_chans` channels, `smem` bytes of dynamic shared
+// memory, persistent CTAs.  `wmaps` are the filter tensor maps conv_igemm_halo_kernel takes.
+template <auto Kernel, class... Maps>
+int launch_halo_family(const IgemmProblem& p, const HaloGeom& hg, int BN, int smem, int box_chans, cudaStream_t stream,
+                       const Maps&... wmaps) {
     CUtensorMap tmX;
-    if (int rc = halo_input_map(p, hg, enc, &tmX)) return rc;
-    const int taps = p.KH * p.KW;
-    if (igemm_bn_for(p.OC) != BN || static_cast<unsigned long long>(ceil_div(taps * p.IC, 32)) * igemm_ocpad(p.OC) * 128ull >= (1ull << 31))
-        return -1;
-    HaloArgs a = halo_args(p, hg, BN);
-    const long long pixel_tiles = a.tiles / a.num_n;
+    if (int rc = halo_input_map(p, hg, box_chans, &tmX)) return rc;
+    if (p.planes == 3 && !bf16_filters_fit(p, BN)) return -1;
+    const HaloArgs a = halo_args(p, hg, BN);
     if (static_cast<long long>(p.OH) * p.OW >= (1ll << 30) || a.tiles * a.kblocks >= (1ll << 31)) return -1;
-    const int smem = presplit_smem_bytes(p.OC, hg.Rb, hg.Cb, a.pr, a.pc);
-    auto kern = conv_igemm_presplit_kernel<BN>;
     static SmemAttrCache attr_cache;
-    if (int rc = ensure_dynamic_smem(kern, smem, attr_cache)) return rc;
-    int per_sm = 0;
-    FCUDA_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, kThreadsIg, smem));
-    const long long slots = static_cast<long long>(sm_count()) * (per_sm > 0 ? per_sm : 1);
-    const unsigned grid = static_cast<unsigned>(a.tiles < slots ? a.tiles : slots);
-    const double macs = static_cast<double>(p.N) * p.OC * p.OH * p.OW * p.IC * taps;
-    const double mma = 2.0 * static_cast<double>(pixel_tiles) * hg.R * hg.C * (a.num_n * BN) * (a.kblocks * 32) * 3;
-    const int prof = prof_begin(stream, PROF_IGEMM, 2.0 * macs, mma,
-                                4.0 * (static_cast<double>(p.N) * p.IC * p.H * p.W + static_cast<double>(p.OC) * taps * p.IC +
-                                       static_cast<double>(p.N) * p.OC * p.OH * p.OW * (p.residual ? 2 : 1)));
-    kern<<<grid, kThreadsIg, smem, stream>>>(tmX, a);
+    if (int rc = ensure_dynamic_smem(Kernel, smem, attr_cache)) return rc;
+    unsigned grid = 0;
+    if (int rc = persistent_grid(Kernel, kThreadsIg, smem, a.tiles, &grid)) return rc;
+    // the issued MMA work includes the padded tile pixels
+    const int prof = prof_igemm(p, stream, a.tiles / a.num_n * hg.R * hg.C, a.num_n * BN, a.kblocks);
+    Kernel<<<grid, kThreadsIg, smem, stream>>>(tmX, wmaps..., a);
     prof_end(prof, stream);
     FCUDA_CHECK_LAUNCH();
     count_launch();
     return 0;
 }
 
-template <int BN>
-int launch_igemm_wide(const IgemmProblem& p, const HaloGeom& hg, cudaStream_t stream) {
-    EncodeTiledFn enc = encode_fn();
-    if (!enc) return FCUDA_ERR_CUDA;
-    CUtensorMap tmX;
-    if (int rc = halo_input_map(p, hg, enc, &tmX, 16)) return rc;
-    const int taps = p.KH * p.KW;
-    if (igemm_bn_for(p.OC) != BN || static_cast<unsigned long long>(ceil_div(taps * p.IC, 32)) * igemm_ocpad(p.OC) * 128ull >= (1ull << 31))
-        return -1;
-    HaloArgs a = halo_args(p, hg, BN);
-    const long long pixel_tiles = a.tiles / a.num_n;
-    if (static_cast<long long>(p.OH) * p.OW >= (1ll << 30) || a.tiles * a.kblocks >= (1ll << 31)) return -1;
-    const int smem = wide_smem_bytes(p.OC, hg.Rb, hg.Cb, a.pr, a.pc);
-    auto kern = conv_igemm_wide_kernel<BN>;
-    static SmemAttrCache attr_cache;
-    if (int rc = ensure_dynamic_smem(kern, smem, attr_cache)) return rc;
-    int per_sm = 0;
-    FCUDA_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, kThreadsIg, smem));
-    const long long slots = static_cast<long long>(sm_count()) * (per_sm > 0 ? per_sm : 1);
-    const unsigned grid = static_cast<unsigned>(a.tiles < slots ? a.tiles : slots);
-    const double macs = static_cast<double>(p.N) * p.OC * p.OH * p.OW * p.IC * taps;
-    const double mma = 2.0 * static_cast<double>(pixel_tiles) * hg.R * hg.C * (a.num_n * BN) * (a.kblocks * 32) * 3;
-    const int prof = prof_begin(stream, PROF_IGEMM, 2.0 * macs, mma,
-                                4.0 * (static_cast<double>(p.N) * p.IC * p.H * p.W + static_cast<double>(p.OC) * taps * p.IC +
-                                       static_cast<double>(p.N) * p.OC * p.OH * p.OW * (p.residual ? 2 : 1)));
-    kern<<<grid, kThreadsIg, smem, stream>>>(tmX, a);
-    prof_end(prof, stream);
-    FCUDA_CHECK_LAUNCH();
-    count_launch();
-    return 0;
-}
-
+// The kernel a layer takes for one N tile and operand format: the gathering kernel, or with switch igemm_halo on a
+// layer halo_geometry accepts the per-tap halo kernel, in BF16x3 mode the pre-split kernel (switch igemm_presplit) and
+// the wide one (switch igemm_wide).
 template <int BN, int PLANES>
-int launch_igemm_halo(const IgemmProblem& p, const HaloGeom& hg, cudaStream_t stream) {
-    constexpr bool BF = PLANES == 3;
-    constexpr int NPL = BF ? 2 : PLANES;
-    const int taps = p.KH * p.KW;
-    const int K = taps * p.IC;
-    EncodeTiledFn enc = encode_fn();
-    if (!enc) return FCUDA_ERR_CUDA;
-    CUtensorMap tmX, tmW, tmWlo;
-    memset(&tmW, 0, sizeof(tmW));
-    tmWlo = tmW;
-    if (!BF) {
-        const int Kf = (K + 3) & ~3;
-        for (int pl = 0; pl < NPL; ++pl) {
-            cuuint64_t dims[3] = {(cuuint64_t)Kf, (cuuint64_t)p.OC, 1};
-            cuuint64_t strides[2] = {(cuuint64_t)Kf * 4, (cuuint64_t)Kf * p.OC * 4};
-            cuuint32_t box[3] = {32, (cuuint32_t)BN, 1};
-            cuuint32_t estr[3] = {1, 1, 1};
-            const float* base = pl == 0 ? p.w_hi : p.w_lo;
-            CUresult r = enc(pl == 0 ? &tmW : &tmWlo, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, const_cast<float*>(base), dims, strides,
-                             box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
-                             CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-            if (r != CUDA_SUCCESS) {
-                fprintf(stderr, "fcuda: igemm weight tensor map failed (%d)\n", (int)r);
-                return FCUDA_ERR_CUDA;
-            }
+int launch_conv(const IgemmProblem& p, cudaStream_t stream) {
+    HaloGeom hg;
+    if (tune_get(TUNE_IGEMM_HALO) == 0 || !halo_geometry(p, hg)) return launch_igemm<BN, PLANES>(p, stream);
+    if constexpr (PLANES == 3) {
+        HaloGeom pg;
+        if (tune_get(TUNE_IGEMM_PRESPLIT) != 0 && presplit_geometry(p, pg)) {
+            HaloGeom wg;
+            if constexpr (BN != 32)  // wide_geometry takes N tiles of 64 and 128 channels only
+                if (tune_get(TUNE_IGEMM_WIDE) != 0 && wide_geometry(p, wg))
+                    return launch_halo_family<conv_igemm_wide_kernel<BN>>(p, wg, BN, wide_smem_bytes(p, wg), 16, stream);
+            return launch_halo_family<conv_igemm_presplit_kernel<BN>>(p, pg, BN, presplit_smem_bytes(p, pg), 32, stream);
         }
     }
-    if (int rc = halo_input_map(p, hg, enc, &tmX)) return rc;
-    if (BF && (igemm_bn_for(p.OC) != BN || static_cast<unsigned long long>(ceil_div(K, 32)) * igemm_ocpad(p.OC) * 128ull >= (1ull << 31))) return -1;
-    HaloArgs a = halo_args(p, hg, BN);
-    const long long pixel_tiles = a.tiles / a.num_n;
-    if (static_cast<long long>(p.OH) * p.OW >= (1ll << 30) || a.tiles * a.kblocks >= (1ll << 31)) return -1;
-    const int smem = halo_smem_bytes(p.OC, PLANES, hg.Rb, hg.Cb);
-    auto kern = conv_igemm_halo_kernel<BN, PLANES>;
-    static SmemAttrCache attr_cache;
-    if (int rc = ensure_dynamic_smem(kern, smem, attr_cache)) return rc;
-    int per_sm = 0;
-    FCUDA_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, kThreadsIg, smem));
-    const long long slots = static_cast<long long>(sm_count()) * (per_sm > 0 ? per_sm : 1);
-    const unsigned grid = static_cast<unsigned>(a.tiles < slots ? a.tiles : slots);
-    // the same algorithmic work as conv_igemm_kernel; the issued MMA work includes the padded patch pixels
-    const double macs = static_cast<double>(p.N) * p.OC * p.OH * p.OW * p.IC * taps;
-    const double mma = 2.0 * static_cast<double>(pixel_tiles) * 128 * (a.num_n * BN) * (a.kblocks * 32) * (PLANES >= 2 ? 3 : 1);
-    const int prof = prof_begin(stream, PROF_IGEMM, 2.0 * macs, mma,
-                                4.0 * (static_cast<double>(p.N) * p.IC * p.H * p.W + static_cast<double>(p.OC) * K +
-                                       static_cast<double>(p.N) * p.OC * p.OH * p.OW * (p.residual ? 2 : 1)));
-    kern<<<grid, kThreadsIg, smem, stream>>>(tmX, tmW, tmWlo, a);
-    prof_end(prof, stream);
-    FCUDA_CHECK_LAUNCH();
-    count_launch();
-    return 0;
+    CUtensorMap tmW, tmWlo;
+    if (int rc = filter_maps(p, BN, PLANES, &tmW, &tmWlo)) return rc;
+    return launch_halo_family<conv_igemm_halo_kernel<BN, PLANES>>(p, hg, BN, halo_smem_bytes(p.OC, PLANES, hg.Rb, hg.Cb),
+                                                                  32, stream, tmW, tmWlo);
+}
+
+// The geometry query behind the exported conv_igemm_*_geometry: g is written only when the layer takes the kernel
+static bool geometry_query(bool (*geometry)(const IgemmProblem&, HaloGeom&), const IgemmProblem& p, HaloGeom* g) {
+    HaloGeom tmp;
+    const bool ok = geometry(p, tmp);
+    if (ok && g) *g = tmp;
+    return ok;
 }
 
 }  // namespace
 
-bool conv_igemm_halo_geometry(const IgemmProblem& p, HaloGeom* g) {
-    HaloGeom tmp;
-    const bool ok = halo_geometry(p, tmp);
-    if (ok && g) *g = tmp;
-    return ok;
-}
-
-bool conv_igemm_presplit_geometry(const IgemmProblem& p, HaloGeom* g) {
-    HaloGeom tmp;
-    const bool ok = presplit_geometry(p, tmp);
-    if (ok && g) *g = tmp;
-    return ok;
-}
-
-bool conv_igemm_wide_geometry(const IgemmProblem& p, HaloGeom* g) {
-    HaloGeom tmp;
-    const bool ok = wide_geometry(p, tmp);
-    if (ok && g) *g = tmp;
-    return ok;
-}
+bool conv_igemm_halo_geometry(const IgemmProblem& p, HaloGeom* g) { return geometry_query(halo_geometry, p, g); }
+bool conv_igemm_presplit_geometry(const IgemmProblem& p, HaloGeom* g) { return geometry_query(presplit_geometry, p, g); }
+bool conv_igemm_wide_geometry(const IgemmProblem& p, HaloGeom* g) { return geometry_query(wide_geometry, p, g); }
 
 bool conv_igemm_supported(int IC, int KH, int KW) {
     if (KH * KW > 63) return false;                               // per-pixel tap validity mask is 64-bit
@@ -1536,22 +1327,12 @@ bool conv_igemm_can_pool(const IgemmProblem& p) {
 int conv_igemm_forward(const IgemmProblem& p, cudaStream_t stream) {
     if (!conv_igemm_supported(p.IC, p.KH, p.KW)) return -1;
     if (p.pool && !conv_igemm_can_pool(p)) return -200;
-    const int bn = igemm_bn_for(p.OC);
-    HaloGeom hg;
-    if (tune_get(TUNE_IGEMM_HALO) != 0 && halo_geometry(p, hg)) {
-        HaloGeom pg, wg;
-        if (p.planes == 3 && tune_get(TUNE_IGEMM_PRESPLIT) != 0 && presplit_geometry(p, pg)) {
-            if (tune_get(TUNE_IGEMM_WIDE) != 0 && wide_geometry(p, wg))
-                return bn == 64 ? launch_igemm_wide<64>(p, wg, stream) : launch_igemm_wide<128>(p, wg, stream);
-            return bn == 32 ? launch_igemm_presplit<32>(p, pg, stream) : bn == 64 ? launch_igemm_presplit<64>(p, pg, stream) : launch_igemm_presplit<128>(p, pg, stream);
-        }
-        if (p.planes == 3) return bn == 32 ? launch_igemm_halo<32, 3>(p, hg, stream) : bn == 64 ? launch_igemm_halo<64, 3>(p, hg, stream) : launch_igemm_halo<128, 3>(p, hg, stream);
-        if (p.planes == 2) return bn == 32 ? launch_igemm_halo<32, 2>(p, hg, stream) : bn == 64 ? launch_igemm_halo<64, 2>(p, hg, stream) : launch_igemm_halo<128, 2>(p, hg, stream);
-        return bn == 32 ? launch_igemm_halo<32, 1>(p, hg, stream) : bn == 64 ? launch_igemm_halo<64, 1>(p, hg, stream) : launch_igemm_halo<128, 1>(p, hg, stream);
-    }
-    if (p.planes == 3) return bn == 32 ? launch_igemm<32, 3>(p, stream) : bn == 64 ? launch_igemm<64, 3>(p, stream) : launch_igemm<128, 3>(p, stream);
-    if (p.planes == 2) return bn == 32 ? launch_igemm<32, 2>(p, stream) : bn == 64 ? launch_igemm<64, 2>(p, stream) : launch_igemm<128, 2>(p, stream);
-    return bn == 32 ? launch_igemm<32, 1>(p, stream) : bn == 64 ? launch_igemm<64, 1>(p, stream) : launch_igemm<128, 1>(p, stream);
+    using Launch = int (*)(const IgemmProblem&, cudaStream_t);
+    static const Launch kLaunch[3][3] = {  // [N tile 32, 64, 128][planes 1, 2, 3]
+        {launch_conv<32, 1>, launch_conv<32, 2>, launch_conv<32, 3>},
+        {launch_conv<64, 1>, launch_conv<64, 2>, launch_conv<64, 3>},
+        {launch_conv<128, 1>, launch_conv<128, 2>, launch_conv<128, 3>}};
+    return kLaunch[igemm_bn_for(p.OC) / 64][p.planes == 3 ? 2 : p.planes == 2 ? 1 : 0](p, stream);
 }
 
 }  // namespace fcuda

@@ -495,66 +495,38 @@ static int conv_forward_impl(const FcudaConvParam* p, int algo, float* output, c
     }
 }
 
+// The implicit-GEMM problem of one group of a layer, without tensors (N = 1): what the tile and pooling queries read
+static IgemmProblem igemm_problem(const FcudaConvParam* p) {
+    IgemmProblem g{};
+    const int G = p->group > 0 ? p->group : 1;
+    g.N = 1; g.IC = p->input_channels / G; g.OC = p->output_channels / G;
+    g.H = p->input_h; g.W = p->input_w; g.OH = p->output_h; g.OW = p->output_w;
+    g.KH = p->kernel_h; g.KW = p->kernel_w; g.stride_h = p->stride_h; g.stride_w = p->stride_w;
+    g.pad_top = p->pad_top; g.pad_left = p->pad_left;
+    g.planes = igemm_planes();
+    return g;
+}
+
 // Can fcuda_conv_forward_pool fuse the pooling for this layer?  Winograd: always (the output tile starts at an even
 // coordinate); implicit GEMM: the 3x3 / stride-1 slab kernel (group 1).
 int fcuda_conv_can_pool(const FcudaConvParam* p, int algo) {
     if (!p) return 0;
     if (algo == FCUDA_WINOGRADF63 || algo == FCUDA_WINOGRADF23) return 1;
-    if (algo == FCUDA_SGECONV) {
-        IgemmProblem g{};
-        g.IC = p->input_channels / (p->group > 0 ? p->group : 1);
-        g.KH = p->kernel_h; g.KW = p->kernel_w; g.stride_h = p->stride_h; g.stride_w = p->stride_w;
-        g.pad_top = p->pad_top; g.pad_left = p->pad_left;
-        g.H = p->input_h; g.W = p->input_w;
-        return conv_igemm_can_pool(g) ? 1 : 0;
-    }
+    if (algo == FCUDA_SGECONV) return conv_igemm_can_pool(igemm_problem(p)) ? 1 : 0;
     return 0;
 }
 
-int fcuda_igemm_halo_tile(const FcudaConvParam* p, int* geom) {
+static int igemm_tile(const FcudaConvParam* p, int* geom, bool (*geometry)(const IgemmProblem&, HaloGeom*)) {
     if (!p) return 0;
-    IgemmProblem g{};
-    const int G = p->group > 0 ? p->group : 1;
-    g.N = 1; g.IC = p->input_channels / G; g.OC = p->output_channels / G;
-    g.H = p->input_h; g.W = p->input_w; g.OH = p->output_h; g.OW = p->output_w;
-    g.KH = p->kernel_h; g.KW = p->kernel_w; g.stride_h = p->stride_h; g.stride_w = p->stride_w;
-    g.pad_top = p->pad_top; g.pad_left = p->pad_left;
-    g.planes = igemm_planes();
     HaloGeom hg;
-    if (!conv_igemm_halo_geometry(g, &hg)) return 0;
+    if (!geometry(igemm_problem(p), &hg)) return 0;
     if (geom) { geom[0] = hg.R; geom[1] = hg.C; geom[2] = hg.Rb; geom[3] = hg.Cb; }
     return 1;
 }
 
-int fcuda_igemm_presplit_tile(const FcudaConvParam* p, int* geom) {
-    if (!p) return 0;
-    IgemmProblem g{};
-    const int G = p->group > 0 ? p->group : 1;
-    g.N = 1; g.IC = p->input_channels / G; g.OC = p->output_channels / G;
-    g.H = p->input_h; g.W = p->input_w; g.OH = p->output_h; g.OW = p->output_w;
-    g.KH = p->kernel_h; g.KW = p->kernel_w; g.stride_h = p->stride_h; g.stride_w = p->stride_w;
-    g.pad_top = p->pad_top; g.pad_left = p->pad_left;
-    g.planes = igemm_planes();
-    HaloGeom hg;
-    if (!conv_igemm_presplit_geometry(g, &hg)) return 0;
-    if (geom) { geom[0] = hg.R; geom[1] = hg.C; geom[2] = hg.Rb; geom[3] = hg.Cb; }
-    return 1;
-}
-
-int fcuda_igemm_wide_tile(const FcudaConvParam* p, int* geom) {
-    if (!p) return 0;
-    IgemmProblem g{};
-    const int G = p->group > 0 ? p->group : 1;
-    g.N = 1; g.IC = p->input_channels / G; g.OC = p->output_channels / G;
-    g.H = p->input_h; g.W = p->input_w; g.OH = p->output_h; g.OW = p->output_w;
-    g.KH = p->kernel_h; g.KW = p->kernel_w; g.stride_h = p->stride_h; g.stride_w = p->stride_w;
-    g.pad_top = p->pad_top; g.pad_left = p->pad_left;
-    g.planes = igemm_planes();
-    HaloGeom hg;
-    if (!conv_igemm_wide_geometry(g, &hg)) return 0;
-    if (geom) { geom[0] = hg.R; geom[1] = hg.C; geom[2] = hg.Rb; geom[3] = hg.Cb; }
-    return 1;
-}
+int fcuda_igemm_halo_tile(const FcudaConvParam* p, int* geom) { return igemm_tile(p, geom, conv_igemm_halo_geometry); }
+int fcuda_igemm_presplit_tile(const FcudaConvParam* p, int* geom) { return igemm_tile(p, geom, conv_igemm_presplit_geometry); }
+int fcuda_igemm_wide_tile(const FcudaConvParam* p, int* geom) { return igemm_tile(p, geom, conv_igemm_wide_geometry); }
 
 int fcuda_conv_forward_pool(const FcudaConvParam* p, int algo, float* output, const float* input, const float* packed,
                             float* scratch, const float* bias, int batch, void* stream) {

@@ -97,115 +97,7 @@ __device__ __forceinline__ void epilogue_store(const GemmKernelArgs& args, const
     }
 }
 
-template <int BN, int PLANES>
-__global__ void __launch_bounds__(kThreads, 1)
-tensor_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
-                   const __grid_constant__ CUtensorMap tmBlo, const GemmKernelArgs args) {
-    constexpr int kATile = kBM * kBK * 4;  // 16 KB raw A
-    constexpr int kBTile = BN * kBK * 4;
-    constexpr int kStage = kATile + PLANES * kBTile;  // [A raw][B_hi][B_lo]
-    extern __shared__ uint8_t smem_raw[];
-    // SWIZZLE_128B tiles need 1024-byte alignment.
-    uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-    __shared__ uint64_t full_bar[kStages];
-    __shared__ uint64_t empty_bar[kStages];
-
-    const int warp = threadIdx.x >> 5;
-    const int lane = threadIdx.x & 31;
-
-    // tile = ((ks * G + g) * num_m + m_blk) * num_n + n_blk: neighbouring CTAs share the A tile
-    const int tile = blockIdx.x;
-    const int n_blk = tile % args.num_n;
-    const int t1 = tile / args.num_n;
-    const int m_blk = t1 % args.num_m;
-    const int t2 = t1 / args.num_m;
-    const int g = t2 % args.G;
-    const int ks = t2 / args.G;
-    const int kb_per_split = (args.k_blocks_total + args.split_k - 1) / args.split_k;
-    const int kb0 = ks * kb_per_split;
-    const int nk = min(kb0 + kb_per_split, args.k_blocks_total) - kb0;
-
-    if (threadIdx.x == 0) {
-        for (int s = 0; s < kStages; ++s) {
-            ptx::mbar_init(&full_bar[s], 1);
-            ptx::mbar_init(&empty_bar[s], kConsumerWarps);
-        }
-        ptx::fence_barrier_init();
-    }
-    __syncthreads();
-
-    if (warp == kConsumerWarps) {
-        // ===================== TMA producer =====================
-        if (lane == 0) {
-            ptx::prefetch_tensormap(&tmA);
-            ptx::prefetch_tensormap(&tmB);
-            if (PLANES == 2) ptx::prefetch_tensormap(&tmBlo);
-            for (int i = 0; i < nk; ++i) {
-                const int stage = i % kStages;
-                if (i >= kStages) ptx::mbar_wait(&empty_bar[stage], ((i / kStages) - 1) & 1);
-                uint8_t* st = smem + stage * kStage;
-                const int kc = (kb0 + i) * kBK;
-                ptx::mbar_arrive_expect_tx(&full_bar[stage], kStage);
-                ptx::tma_load_3d(st, &tmA, &full_bar[stage], kc, m_blk * kBM, g);
-                ptx::tma_load_3d(st + kATile, &tmB, &full_bar[stage], kc, n_blk * BN, g);
-                if (PLANES == 2) ptx::tma_load_3d(st + kATile + kBTile, &tmBlo, &full_bar[stage], kc, n_blk * BN, g);
-            }
-        }
-        return;
-    }
-
-    // ===================== consumers: two warpgroups of 64 rows =====================
-    const int gq = lane >> 2, c = lane & 3;
-    const int row0 = warp * 16 + gq;  // tile rows row0 and row0 + 8; row & 7 == gq for both (128B swizzle phase)
-    float acc[BN / 2];
-#pragma unroll
-    for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
-
-    for (int i = 0; i < nk; ++i) {
-        const int stage = i % kStages;
-        ptx::mbar_wait(&full_bar[stage], (i / kStages) & 1);
-        const uint32_t a_base = ptx::smem_u32(smem + stage * kStage);
-        uint32_t ahi[4][4], alo[4][4];
-#pragma unroll
-        for (int kk = 0; kk < 4; ++kk) {
-#pragma unroll
-            for (int q = 0; q < 4; ++q) {  // q: a0 (row0, k), a1 (row0 + 8, k), a2 (row0, k + 4), a3 (row0 + 8, k + 4)
-                const int row = row0 + 8 * (q & 1);
-                const uint32_t chunk = static_cast<uint32_t>(2 * kk + (q >> 1)) ^ static_cast<uint32_t>(gq);
-                float x;
-                asm volatile("ld.shared.f32 %0, [%1];" : "=f"(x) : "r"(a_base + row * 128 + (chunk << 4) + c * 4));
-                if (PLANES == 2) split_tf32_trunc(x, ahi[kk][q], alo[kk][q]);
-                else ahi[kk][q] = __float_as_uint(x);
-            }
-        }
-        const uint64_t dB = make_smem_desc_sw128(a_base + kATile);
-        const uint64_t dBlo = make_smem_desc_sw128(a_base + kATile + kBTile);
-        ptx::wgmma_fence();
-#pragma unroll
-        for (int kk = 0; kk < 4; ++kk) {
-            if (PLANES == 2) {
-                Wgmma<BN, 1>::mma(acc, alo[kk], dB + 2 * kk, 1u);    // A_lo * B_hi
-                Wgmma<BN, 1>::mma(acc, ahi[kk], dBlo + 2 * kk, 1u);  // A_hi * B_lo
-                Wgmma<BN, 1>::mma(acc, ahi[kk], dB + 2 * kk, 1u);    // A_hi * B_hi
-            } else {
-                Wgmma<BN, 1>::mma(acc, ahi[kk], dB + 2 * kk, 1u);
-            }
-        }
-        ptx::wgmma_commit();
-        ptx::wgmma_wait<0>();
-        __syncwarp();
-        if (lane == 0) ptx::mbar_arrive(&empty_bar[stage]);
-    }
-    epilogue_store<BN>(args, acc, g, m_blk * kBM + row0, n_blk * BN, c, ks);
-}
-
-// tensor_gemm_pipe_kernel<BN, PLANES>: the same tiles, k-blocks, wgmma sequence and epilogue as tensor_gemm_kernel, so the
-// result is bit-identical to it, with
-//   - two A-fragment sets: k-block kb + 1 is read from the swizzled tile and split while kb's commit group runs
-//     (wgmma_wait<1>); a ring stage is released once the group that read its B planes retired;
-//   - call-free bounded waits: a call inside the pipeline would make ptxas serialise every wgmma;
-//   - persistent CTAs that walk the tile order with a static stride; the producer keeps a running k-block count across
-//     tiles, so it fills the next tile's stages while the consumers run the epilogue.
+// tile = ((ks * G + g) * num_m + m_blk) * num_n + n_blk: neighbouring CTAs share the A tile
 struct TileCoord { int g, m_blk, n_blk, ks, kb0, nk; };
 
 __device__ __forceinline__ TileCoord tile_coord(const GemmKernelArgs& args, int tile) {
@@ -222,6 +114,99 @@ __device__ __forceinline__ TileCoord tile_coord(const GemmKernelArgs& args, int 
     return t;
 }
 
+// This thread's A fragments of one k-block, read from the raw fp32 tile at a_base (128-byte rows, 128-byte swizzle) and
+// split as split_fragments does: rows row0 and row0 + 8, whose swizzle phase row & 7 is gq for both.
+template <int PLANES>
+__device__ __forceinline__ void load_a_fragments(uint32_t a_base, int row0, int gq, int c, uint32_t (&f1)[4][4],
+                                                 uint32_t (&f2)[4][4]) {
+#pragma unroll
+    for (int kk = 0; kk < 4; ++kk) {
+#pragma unroll
+        for (int q = 0; q < 4; ++q) {  // q: a0 (row0, k), a1 (row0 + 8, k), a2 (row0, k + 4), a3 (row0 + 8, k + 4)
+            const int row = row0 + 8 * (q & 1);
+            const uint32_t chunk = static_cast<uint32_t>(2 * kk + (q >> 1)) ^ static_cast<uint32_t>(gq);
+            float x;
+            asm volatile("ld.shared.f32 %0, [%1];" : "=f"(x) : "r"(a_base + row * 128 + (chunk << 4) + c * 4));
+            if (PLANES == 2) split_tf32_trunc(x, f1[kk][q], f2[kk][q]);
+            else f1[kk][q] = __float_as_uint(x);
+        }
+    }
+}
+
+template <int BN, int PLANES>
+__global__ void __launch_bounds__(kThreads, 1)
+tensor_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
+                   const __grid_constant__ CUtensorMap tmBlo, const GemmKernelArgs args) {
+    constexpr int kATile = kBM * kBK * 4;  // 16 KB raw A
+    constexpr int kBTile = BN * kBK * 4;
+    constexpr int kStage = kATile + PLANES * kBTile;  // [A raw][B_hi][B_lo]
+    extern __shared__ uint8_t smem_raw[];
+    // SWIZZLE_128B tiles need 1024-byte alignment.
+    uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+    __shared__ uint64_t full_bar[kStages];
+    __shared__ uint64_t empty_bar[kStages];
+
+    const int warp = threadIdx.x >> 5;
+    const int lane = threadIdx.x & 31;
+
+    const TileCoord tc = tile_coord(args, blockIdx.x);
+
+    if (threadIdx.x == 0) {
+        ptx::mbar_init_ring(full_bar, empty_bar, kStages, kConsumerWarps);
+        ptx::fence_barrier_init();
+    }
+    __syncthreads();
+
+    if (warp == kConsumerWarps) {
+        // ===================== TMA producer =====================
+        if (lane == 0) {
+            ptx::prefetch_tensormap(&tmA);
+            ptx::prefetch_tensormap(&tmB);
+            if (PLANES == 2) ptx::prefetch_tensormap(&tmBlo);
+            for (int i = 0; i < tc.nk; ++i) {
+                const int stage = i % kStages;
+                if (i >= kStages) ptx::mbar_wait(&empty_bar[stage], ((i / kStages) - 1) & 1);
+                uint8_t* st = smem + stage * kStage;
+                const int kc = (tc.kb0 + i) * kBK;
+                ptx::mbar_arrive_expect_tx(&full_bar[stage], kStage);
+                ptx::tma_load_3d(st, &tmA, &full_bar[stage], kc, tc.m_blk * kBM, tc.g);
+                ptx::tma_load_3d(st + kATile, &tmB, &full_bar[stage], kc, tc.n_blk * BN, tc.g);
+                if (PLANES == 2) ptx::tma_load_3d(st + kATile + kBTile, &tmBlo, &full_bar[stage], kc, tc.n_blk * BN, tc.g);
+            }
+        }
+        return;
+    }
+
+    // ===================== consumers: two warpgroups of 64 rows =====================
+    const int gq = lane >> 2, c = lane & 3;
+    const int row0 = warp * 16 + gq;  // tile rows row0 and row0 + 8; row & 7 == gq for both (128B swizzle phase)
+    float acc[BN / 2];
+#pragma unroll
+    for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+
+    for (int i = 0; i < tc.nk; ++i) {
+        const int stage = i % kStages;
+        ptx::mbar_wait(&full_bar[stage], (i / kStages) & 1);
+        const uint32_t a_base = ptx::smem_u32(smem + stage * kStage);
+        uint32_t ahi[4][4], alo[4][4];
+        load_a_fragments<PLANES>(a_base, row0, gq, c, ahi, alo);
+        ptx::wgmma_fence();
+        mma_kblock<BN, PLANES>(acc, ahi, alo, a_base + kATile, a_base + kATile + kBTile);
+        ptx::wgmma_commit();
+        ptx::wgmma_wait<0>();
+        __syncwarp();
+        if (lane == 0) ptx::mbar_arrive(&empty_bar[stage]);
+    }
+    epilogue_store<BN>(args, acc, tc.g, tc.m_blk * kBM + row0, tc.n_blk * BN, c, tc.ks);
+}
+
+// tensor_gemm_pipe_kernel<BN, PLANES>: the same tiles, k-blocks, wgmma sequence and epilogue as tensor_gemm_kernel, so the
+// result is bit-identical to it, with
+//   - two A-fragment sets: k-block kb + 1 is read from the swizzled tile and split while kb's commit group runs
+//     (wgmma_wait<1>); a ring stage is released once the group that read its B planes retired;
+//   - call-free bounded waits: a call inside the pipeline would make ptxas serialise every wgmma;
+//   - persistent CTAs that walk the tile order with a static stride; the producer keeps a running k-block count across
+//     tiles, so it fills the next tile's stages while the consumers run the epilogue.
 template <int BN, int PLANES>
 __global__ void __launch_bounds__(kThreads, 1)
 tensor_gemm_pipe_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
@@ -238,10 +223,7 @@ tensor_gemm_pipe_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_co
     const int lane = threadIdx.x & 31;
 
     if (threadIdx.x == 0) {
-        for (int s = 0; s < kStages; ++s) {
-            ptx::mbar_init(&full_bar[s], 1);
-            ptx::mbar_init(&empty_bar[s], kConsumerWarps);
-        }
+        ptx::mbar_init_ring(full_bar, empty_bar, kStages, kConsumerWarps);
         ptx::fence_barrier_init();
     }
     __syncthreads();
@@ -285,31 +267,9 @@ tensor_gemm_pipe_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_co
             const int stage = kbg % kStages;
             ptx::mbar_wait_nocall(&full_bar[stage], (kbg / kStages) & 1);
             const uint32_t a_base = ptx::smem_u32(smem + stage * kStage);
-#pragma unroll
-            for (int kk = 0; kk < 4; ++kk) {
-#pragma unroll
-                for (int q = 0; q < 4; ++q) {  // as tensor_gemm_kernel
-                    const int row = row0 + 8 * (q & 1);
-                    const uint32_t chunk = static_cast<uint32_t>(2 * kk + (q >> 1)) ^ static_cast<uint32_t>(gq);
-                    float x;
-                    asm volatile("ld.shared.f32 %0, [%1];" : "=f"(x) : "r"(a_base + row * 128 + (chunk << 4) + c * 4));
-                    if (PLANES == 2) split_tf32_trunc(x, f1[kk][q], f2[kk][q]);
-                    else f1[kk][q] = __float_as_uint(x);
-                }
-            }
-            const uint64_t dB = make_smem_desc_sw128(a_base + kATile);
-            const uint64_t dBlo = make_smem_desc_sw128(a_base + kATile + kBTile);
+            load_a_fragments<PLANES>(a_base, row0, gq, c, f1, f2);
             ptx::wgmma_fence();
-#pragma unroll
-            for (int kk = 0; kk < 4; ++kk) {
-                if (PLANES == 2) {
-                    Wgmma<BN, 1>::mma(acc, f2[kk], dB + 2 * kk, 1u);    // A_lo * B_hi
-                    Wgmma<BN, 1>::mma(acc, f1[kk], dBlo + 2 * kk, 1u);  // A_hi * B_lo
-                    Wgmma<BN, 1>::mma(acc, f1[kk], dB + 2 * kk, 1u);    // A_hi * B_hi
-                } else {
-                    Wgmma<BN, 1>::mma(acc, f1[kk], dB + 2 * kk, 1u);
-                }
-            }
+            mma_kblock<BN, PLANES>(acc, f1, f2, a_base + kATile, a_base + kATile + kBTile);
             ptx::wgmma_commit();
             ptx::wgmma_wait<1>();  // k-block i - 1 retired: its stage's B planes and its fragment set are free
             __syncwarp();
@@ -341,11 +301,7 @@ tensor_gemm_pipe_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_co
 // --------------------------------------------------------------------------------------------
 // Host side
 // --------------------------------------------------------------------------------------------
-typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
-                                  const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
-                                  CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-
-static EncodeTiledFn get_encode_fn() {
+EncodeTiledFn encode_tiled_fn() {
     static EncodeTiledFn fn = nullptr;
     static std::once_flag once;
     std::call_once(once, [] {
@@ -470,10 +426,8 @@ int sm_count() {
     return n[dev];
 }
 
-// 3D map over [G][rows][K] fp32 with a (32 x box_rows x 1) box and 128B swizzle.
-static int make_map(CUtensorMap* map, const float* base, int K, int rows, int G, long long batch_stride,
-                    int box_rows) {
-    EncodeTiledFn enc = get_encode_fn();
+int make_map(CUtensorMap* map, const float* base, int K, int rows, int G, long long batch_stride, int box_rows) {
+    EncodeTiledFn enc = encode_tiled_fn();
     if (!enc) {
         fprintf(stderr, "fcuda: cuTensorMapEncodeTiled unavailable (no CUDA driver?)\n");
         return FCUDA_ERR_CUDA;
@@ -550,11 +504,8 @@ static int launch(const GemmProblem& p, cudaStream_t stream) {
     if (int rc2 = pipe ? ensure_dynamic_smem(pkern, smem, pattr_cache) : ensure_dynamic_smem(kern, smem, attr_cache))
         return rc2;
     unsigned grid = static_cast<unsigned>(total);
-    if (pipe) {  // persistent: at most one wave of CTAs
-        int per_sm = 0;
-        FCUDA_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, pkern, kThreads, smem));
-        const long long slots = static_cast<long long>(sm_count()) * (per_sm > 0 ? per_sm : 1);
-        grid = static_cast<unsigned>(total < slots ? total : slots);
+    if (pipe) {
+        if (int rc2 = persistent_grid(pkern, kThreads, smem, total, &grid)) return rc2;
     }
     const double dense = 2.0 * p.M * static_cast<double>(p.N) * p.K * p.G;
     const int prof = prof_begin(stream, PROF_TENSOR_GEMM, p.algo_flops > 0 ? p.algo_flops : dense,

@@ -67,6 +67,16 @@ int tensor_gemm_effective_split(int K, int split_k);
 // True when the problem satisfies the TMA alignment rules above.
 bool tensor_gemm_supported(const GemmProblem& p);
 
+// cuTensorMapEncodeTiled, resolved once through the runtime (the library does not link libcuda); null without a driver.
+typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
+                                  const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
+                                  CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
+EncodeTiledFn encode_tiled_fn();
+
+// K-major 3-D map over [G][rows][K] fp32 (batch_stride floats between consecutive g, 0 => rows * K) with a
+// 32 x box_rows x 1 box and the 128-byte swizzle.  Returns 0 or FCUDA_ERR_CUDA.
+int make_map(CUtensorMap* map, const float* base, int K, int rows, int G, long long batch_stride, int box_rows);
+
 // Reference CUDA-core fp32 GEMM with identical semantics (used by the self-test and as
 // the fallback for shapes TMA cannot describe).
 int simt_gemm(const GemmProblem& p, cudaStream_t stream);

@@ -144,6 +144,15 @@ __device__ __forceinline__ void wgmma_wait() {
     asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory");
 }
 
+// A ring of `stages` full / empty mbarrier pairs: one producer arrival (plus the transaction bytes) fills a slot, one
+// arrival of each of `consumers` warps empties it.  Thread 0 only; fence_barrier_init and a CTA barrier follow.
+__device__ __forceinline__ void mbar_init_ring(uint64_t* full, uint64_t* empty, int stages, uint32_t consumers) {
+    for (int s = 0; s < stages; ++s) {
+        mbar_init(&full[s], 1);
+        mbar_init(&empty[s], consumers);
+    }
+}
+
 }  // namespace ptx
 
 // --------------------------------------------------------------------------------------------
@@ -340,6 +349,67 @@ __device__ __forceinline__ void split_bf16x2(float x0, float x1, uint32_t& p1, u
 __device__ __forceinline__ void split_tf32_trunc(float x, uint32_t& hi, uint32_t& lo) {
     hi = __float_as_uint(x) & 0xFFFFE000u;
     lo = __float_as_uint(x - __uint_as_float(hi));
+}
+
+// Operand formats of the register-A kernels (PLANES): 3 = BF16x3 (x = p1 + p2 + r, three bf16 MMAs p2*q1, p1*q2, p1*q1
+// per k-step of 16), 2 = 3xTF32 (hi = x & 0xFFFFE000, lo = x - hi, three tf32 MMAs lo*hi, hi*lo, hi*hi per k-step of 8),
+// 1 = plain TF32.
+
+// The fragments of one 32-wide k-block from its raw fp32 values raw[h][j] (row gq + 8h, fragment element j: tf32 k-steps
+// of 8 hold k = (c, c + 4) at j = 2kk, 2kk + 1; bf16 k-steps of 16 hold the pairs (2c, 2c + 1), (2c + 8, 2c + 9) at
+// j = 4kk .. 4kk + 3).  f1 = hi / p1, f2 = lo / p2 (unused for TF32), [k-step][a0..a3].
+template <int PLANES>
+__device__ __forceinline__ void split_fragments(const float (&raw)[2][8], uint32_t (&f1)[4][4], uint32_t (&f2)[4][4]) {
+    if (PLANES == 3) {
+#pragma unroll
+        for (int kk = 0; kk < 2; ++kk)
+#pragma unroll
+            for (int q = 0; q < 4; ++q) {  // a0 (row gq, pair 0), a1 (row gq + 8, pair 0), a2 (gq, pair 1), a3 (gq + 8, pair 1)
+                const int h = q & 1, j = 4 * kk + 2 * (q >> 1);
+                split_bf16x2(raw[h][j], raw[h][j + 1], f1[kk][q], f2[kk][q]);
+            }
+    } else {
+#pragma unroll
+        for (int kk = 0; kk < 4; ++kk)
+#pragma unroll
+            for (int q = 0; q < 4; ++q) {
+                const float x = raw[q & 1][2 * kk + (q >> 1)];
+                if (PLANES == 2) split_tf32_trunc(x, f1[kk][q], f2[kk][q]);
+                else f1[kk][q] = __float_as_uint(x);
+            }
+    }
+}
+
+// The MMAs of one 32-wide k-block into an m64 x BN accumulator: A fragments f1 / f2 from split_fragments (KS >= 2 k-steps
+// for BF16x3, 4 otherwise), the B planes at shared addresses b_hi / b_lo (b_lo unused for TF32).  BF16x3 B is the
+// un-swizzled K-major core-matrix layout (LBO = 128 B between k chunks, SBO = 512 B between 8-row groups, a k-step = 2
+// chunks); tf32 B is 128-byte-swizzled rows.  The caller fences before and commits after.
+template <int BN, int PLANES, int KS>
+__device__ __forceinline__ void mma_kblock(float (&acc)[BN / 2], const uint32_t (&f1)[KS][4], const uint32_t (&f2)[KS][4],
+                                           uint32_t b_hi, uint32_t b_lo) {
+    if constexpr (PLANES == 3) {
+        const uint64_t dQ1 = make_smem_desc_none(b_hi, 128, 512);
+        const uint64_t dQ2 = make_smem_desc_none(b_lo, 128, 512);
+#pragma unroll
+        for (int kk = 0; kk < 2; ++kk) {
+            Wgmma<BN, 0>::mma(acc, f2[kk], dQ1 + 16 * kk, 1u);  // p2 * q1
+            Wgmma<BN, 0>::mma(acc, f1[kk], dQ2 + 16 * kk, 1u);  // p1 * q2
+            Wgmma<BN, 0>::mma(acc, f1[kk], dQ1 + 16 * kk, 1u);  // p1 * q1
+        }
+    } else {
+        const uint64_t dB = make_smem_desc_sw128(b_hi);
+        const uint64_t dBlo = make_smem_desc_sw128(b_lo);
+#pragma unroll
+        for (int kk = 0; kk < 4; ++kk) {
+            if (PLANES == 2) {
+                Wgmma<BN, 1>::mma(acc, f2[kk], dB + 2 * kk, 1u);    // A_lo * B_hi
+                Wgmma<BN, 1>::mma(acc, f1[kk], dBlo + 2 * kk, 1u);  // A_hi * B_lo
+                Wgmma<BN, 1>::mma(acc, f1[kk], dB + 2 * kk, 1u);    // A_hi * B_hi
+            } else {
+                Wgmma<BN, 1>::mma(acc, f1[kk], dB + 2 * kk, 1u);
+            }
+        }
+    }
 }
 
 }  // namespace fcuda
