@@ -90,6 +90,7 @@ def fcuda() -> ctypes.CDLL:
             "fcuda_conv_get_buffer_size": (i, [P, i, i, szp, szp]),
             "fcuda_conv_init": (i, [P, i, vp, vp, vp]),
             "fcuda_conv_forward": (i, [P, i, vp, vp, vp, vp, vp, i, vp]),
+            "fcuda_conv_forward_clip": (i, [P, i, vp, vp, vp, vp, vp, ctypes.c_float, ctypes.c_float, i, vp]),
             "fcuda_conv_forward_residual": (i, [P, i, vp, vp, vp, vp, vp, vp, i, i, vp]),
             "fcuda_conv_can_pool": (i, [P, i]),
             "fcuda_igemm_halo_tile": (i, [P, ctypes.POINTER(i)]),
@@ -113,6 +114,8 @@ def fcuda() -> ctypes.CDLL:
             "fcuda_scale_forward": (i, [vp, vp, i, sz, vp, vp, i, vp]),
             "fcuda_eltwise_add_forward": (i, [vp, vp, vp, sz, i, vp]),
             "fcuda_relu_forward": (i, [vp, vp, sz, vp]),
+            "fcuda_clip_forward": (i, [vp, vp, sz, ctypes.c_float, ctypes.c_float, vp]),
+            "fcuda_prelu_forward": (i, [vp, vp, i, sz, vp, i, i, vp]),
             "fcuda_softmax_forward": (i, [vp, vp, sz, i, vp]),
             "fcuda_dropout_forward": (i, [vp, vp, sz, ctypes.c_float, vp]),
             "fcuda_copy_channels": (i, [vp, i, i, vp, i, sz, i, vp]),

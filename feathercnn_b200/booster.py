@@ -18,6 +18,7 @@ from ._lib import FcudaInterpParam as InterpParam
 NAIVE, IM2COL, SGECONV, DEPTHWISE, WINOGRADF63, WINOGRADF63FUSED, WINOGRADF23 = range(7)
 ALGO_NAMES = ["NAIVE", "IM2COL", "SGECONV", "DEPTHWISE", "WINOGRADF63", "WINOGRADF63FUSED", "WINOGRADF23"]
 PRECISION_TF32X3, PRECISION_TF32, PRECISION_FP32_SPLIT = 0, 1, 2
+ACT_NONE, ACT_RELU, ACT_CLIP = 0, 1, 2  # FcudaActivation
 
 
 class FcudaError(RuntimeError):
@@ -124,13 +125,22 @@ class ConvBooster:
                fcuda().fcuda_conv_forward(ctypes.byref(param), self.algo, _ptr(output), _ptr(input), _ptr(kernel),
                                           _ptr(buffer), _ptr(bias_arr), batch, _stream()))
 
+    def ForwardClip(self, param: ConvParam, output, input, kernel, buffer, bias_arr, clip_min: float, clip_max: float,
+                    batch: int = 1) -> None:
+        """Forward with param.activation == ACT_CLIP: the output clamped to [clip_min, clip_max] in the epilogue."""
+        _check("fcuda_conv_forward_clip",
+               fcuda().fcuda_conv_forward_clip(ctypes.byref(param), self.algo, _ptr(output), _ptr(input), _ptr(kernel),
+                                               _ptr(buffer), _ptr(bias_arr), float(clip_min), float(clip_max), batch,
+                                               _stream()))
+
 
 def conv_forward(param: ConvParam, x: torch.Tensor, w: torch.Tensor, b: torch.Tensor | None = None,
                  algo: int | None = None, residual: torch.Tensor | None = None,
                  relu_after_add: bool = False, dilation: int = 1, tuned: bool = False,
-                 pool: bool = False) -> tuple[torch.Tensor, int]:
+                 pool: bool = False, clip: tuple[float, float] | None = None) -> tuple[torch.Tensor, int]:
     """Whole ConvBooster protocol for a batch x (N, IC, H, W) -> (N, OC, OH, OW).  Returns (output, algo).
     With `residual` (shaped like the output) the fused Eltwise-SUM entry point is used instead of Forward.
+    With `clip` = (min, max) ForwardClip runs instead (param.activation must be ACT_CLIP).
     `dilation` > 1 goes through fcuda_conv_forward_ext (the caller sets param.output_h/w for the dilated extent)."""
     cb = ConvBooster()
     if algo is None:
@@ -157,6 +167,8 @@ def conv_forward(param: ConvParam, x: torch.Tensor, w: torch.Tensor, b: torch.Te
                fcuda().fcuda_conv_forward_ext(ctypes.byref(param), cb.algo, _ptr(out), _ptr(x.contiguous()), _ptr(packed),
                                               _ptr(scratch), _ptr(b), _ptr(residual.contiguous()) if residual is not None else None,
                                               int(relu_after_add), dilation, dilation, n, _stream()))
+    elif clip is not None:
+        cb.ForwardClip(param, out, x.contiguous(), packed, scratch, b, clip[0], clip[1], n)
     elif residual is None:
         cb.Forward(param, out, x.contiguous(), packed, scratch, b, n)
     else:
@@ -344,6 +356,24 @@ def eltwise_add(a, b, relu=False):
 def relu(x):
     out = torch.empty_like(x)
     _check("fcuda_relu_forward", fcuda().fcuda_relu_forward(_ptr(out), _ptr(x.contiguous()), x.numel(), _stream()))
+    return out
+
+
+def clip(x, lo, hi, out=None):
+    """ncnn Clip: min(max(x, lo), hi), NaN -> lo.  `out` may be `x` (in place)."""
+    out = torch.empty_like(x) if out is None else out
+    _check("fcuda_clip_forward",
+           fcuda().fcuda_clip_forward(_ptr(out), _ptr(x.contiguous()), x.numel(), float(lo), float(hi), _stream()))
+    return out
+
+
+def prelu(x, slope, out=None):
+    """ncnn PReLU over (N, C, ...): x < 0 ? x * slope[c] : x; a one-element `slope` is shared.  `out` may be `x`."""
+    n, c = x.shape[:2]
+    out = torch.empty_like(x) if out is None else out
+    _check("fcuda_prelu_forward",
+           fcuda().fcuda_prelu_forward(_ptr(out), _ptr(x.contiguous()), c, x[0, 0].numel(), _ptr(slope), slope.numel(), n,
+                                       _stream()))
     return out
 
 

@@ -67,6 +67,13 @@ static inline int persistent_grid(Kernel kern, int threads, int smem, long long 
 // Split an fp32 value into a TF32-representable "hi" (round-to-nearest on the 13 dropped
 // mantissa bits) and the exact fp32 remainder "lo".  hi + lo == v exactly; the tensor
 // core then truncates lo to TF32, leaving a relative error of ~2^-22 per operand.
+// The activation of the convolution epilogues: a Clip clamps to [lo, hi] (NaN -> lo); without CLIP it is the ReLU,
+// fmaxf(v, 0).  The Clip kernels are instantiations of their own, so the ReLU kernels keep their code and registers.
+template <bool CLIP>
+__device__ __forceinline__ float act_clamp(float v, float lo, float hi) {
+    return CLIP ? fminf(fmaxf(v, lo), hi) : fmaxf(v, 0.f);
+}
+
 __device__ __forceinline__ void split_tf32(float v, float& hi, float& lo) {
     uint32_t r;
     asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(r) : "f"(v));  // round to nearest (ties away), low 13 mantissa bits zero

@@ -10,9 +10,10 @@
 
 namespace fcuda {
 
+template <bool CLIP>
 __global__ void __launch_bounds__(256)
 conv_direct_kernel(const float* __restrict__ in, const float* __restrict__ w, const float* __restrict__ bias,
-                   float* __restrict__ out, PackGeom g, int OC, int relu) {
+                   float* __restrict__ out, PackGeom g, int OC, int act, float lo, float hi) {
     __shared__ float sW[16][64 + 4];
     __shared__ float sX[16][64 + 4];
     const int n = blockIdx.z;
@@ -67,16 +68,17 @@ conv_direct_kernel(const float* __restrict__ in, const float* __restrict__ w, co
             const int pix = p0 + tx * 4 + j;
             if (pix >= P) continue;
             float v = acc[i][j] + bv;
-            if (relu) v = fmaxf(v, 0.f);
+            if (act) v = act_clamp<CLIP>(v, lo, hi);
             out[(static_cast<size_t>(n) * OC + oc) * P + pix] = v;
         }
     }
 }
 
-int conv_direct(const float* in, const float* w, const float* bias, float* out, const PackGeom& g, int OC, int relu,
-                int batch, cudaStream_t s) {
+int conv_direct(const float* in, const float* w, const float* bias, float* out, const PackGeom& g, int OC, int act,
+                float lo, float hi, int batch, cudaStream_t s) {
     dim3 grid(ceil_div(g.OH * g.OW, 64), ceil_div(OC, 64), batch);
-    conv_direct_kernel<<<grid, 256, 0, s>>>(in, w, bias, out, g, OC, relu);
+    if (act == 2) conv_direct_kernel<true><<<grid, 256, 0, s>>>(in, w, bias, out, g, OC, act, lo, hi);
+    else conv_direct_kernel<false><<<grid, 256, 0, s>>>(in, w, bias, out, g, OC, act, lo, hi);
     FCUDA_CHECK_LAUNCH();
     count_launch();
     return 0;

@@ -23,7 +23,7 @@
 //                planes), TMA tensor loads with the 128-byte swizzle.  A producer warp keeps a 4-deep ring ahead.
 //   MMA        = wgmma.mma_async, A from registers, B from shared memory, fp32 register accumulators (two warpgroups of
 //                64 pixels).
-//   epilogue   = +bias [+ residual: fused Eltwise SUM] -> ReLU [-> 2x2 max pooling by one shuffle] -> NCHW stores.
+//   epilogue   = +bias [+ residual: fused Eltwise SUM] -> ReLU / Clip clamp [-> 2x2 max pooling by one shuffle] -> NCHW stores.
 //
 // Used where non-fused Winograd is bandwidth-bound (large images, <= 128 channels) and for every layer the reference
 // sends to im2col + SGEMM (1x1, strided, 7x7, IC = 3, small images).
@@ -61,7 +61,8 @@ struct IgemmArgs {
     int taps;                // KH*KW
     int num_n;               // ceil(OC / BN)
     long long total_pix;     // N * OH * OW
-    int relu;
+    int act;                 // 0 none, 1 ReLU, 2 Clip: clamp to [lo, hi]
+    float lo, hi;
     int pool;                // fuse a following 2x2 / stride-2 max pooling; `out` is the pooled blob
     int tiles_x, tiles_y;    // pool: 64-column x 2-row patches per image
     const unsigned char* wbf;  // BF16x3: pre-tiled filter planes (see igemm_pack_weights_bf16_kernel)
@@ -96,7 +97,7 @@ __device__ __forceinline__ void load_filter_stage(uint8_t* smem, uint64_t* full_
     }
 }
 
-template <int BN, int PLANES>
+template <int BN, int PLANES, bool CLIP>
 __global__ void __launch_bounds__(kThreadsIg, 1)
 conv_igemm_kernel(const __grid_constant__ CUtensorMap tmW, const __grid_constant__ CUtensorMap tmWlo,
                   const IgemmArgs args) {
@@ -253,7 +254,7 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tmW, const __grid_constant
                 v[h] = acc[4 * j + 2 * h + e] + bv;
                 const size_t o = (static_cast<size_t>(img[h]) * args.out_img_c + oc) * oplane + static_cast<size_t>(oy[h]) * args.OW + ox[h];
                 if (args.residual != nullptr && valid[h] && oc_ok) v[h] += __ldg(args.residual + o);
-                if (args.relu) v[h] = fmaxf(v[h], 0.f);
+                if (args.act) v[h] = act_clamp<CLIP>(v[h], args.lo, args.hi);
                 if (!args.pool && valid[h] && oc_ok) args.out[o] = v[h];
             }
             if (args.pool) {
@@ -369,7 +370,7 @@ static int prof_igemm(const IgemmProblem& p, cudaStream_t stream, long long tile
                              static_cast<double>(p.N) * p.OC * p.OH * p.OW * (p.residual ? 2 : 1)));
 }
 
-template <int BN, int PLANES>
+template <int BN, int PLANES, bool CLIP>
 int launch_igemm(const IgemmProblem& p, cudaStream_t stream) {
     constexpr bool BF = PLANES == 3;
     constexpr int NPL = BF ? 2 : PLANES;
@@ -394,7 +395,7 @@ int launch_igemm(const IgemmProblem& p, cudaStream_t stream) {
     a.taps = taps;
     a.num_n = ceil_div(p.OC, BN);
     a.total_pix = static_cast<long long>(p.N) * p.OH * p.OW;
-    a.relu = p.relu;
+    a.act = p.act; a.lo = p.lo; a.hi = p.hi;
     a.pool = p.pool ? 1 : 0;
     a.tiles_x = ceil_div(p.OW, 64);
     a.tiles_y = ceil_div(p.OH, 2);
@@ -411,7 +412,7 @@ int launch_igemm(const IgemmProblem& p, cudaStream_t stream) {
     const int table_bytes = a.use_table ? a.kblocks * 32 * 8 : 0;
     const int smem = kStagesIg * kStage + table_bytes + 1024;
     if (smem > 227 * 1024) return -1;
-    auto kern = conv_igemm_kernel<BN, PLANES>;
+    auto kern = conv_igemm_kernel<BN, PLANES, CLIP>;
     static SmemAttrCache attr_cache;
     if (int rc = ensure_dynamic_smem(kern, smem, attr_cache)) return rc;
     const int prof = prof_igemm(p, stream, pixel_tiles * 128, a.num_n * BN, a.kblocks);
@@ -450,7 +451,8 @@ struct HaloArgs {
     int OC, OH, OW, KW, taps;
     int out_img_c;
     int kblocks, num_n;
-    int relu, pool;
+    int act, pool;         // act: 0 none, 1 ReLU, 2 Clip: clamp to [lo, hi]
+    float lo, hi;
     int R, C;              // output patch rows x columns (128 pixels)
     int tiles_x, tiles_y;  // patches per image
     int Rb, Cb;            // halo box rows / columns in shared memory (padded)
@@ -478,7 +480,7 @@ __device__ __forceinline__ HaloTile halo_tile(const HaloArgs& args, int per_img,
 
 // Epilogue of the halo kernels for one m64 accumulator (as conv_igemm_kernel): this thread's pixels are rows oy[0..1]
 // of column ox in image img.
-template <int BN>
+template <int BN, bool CLIP>
 __device__ __forceinline__ void halo_epilogue(const float (&acc)[BN / 2], const HaloArgs& args, int n_blk, int img,
                                               const int (&oy)[2], const bool (&valid)[2], int ox, int oplane, int SH,
                                               int SW, int c, int gq) {
@@ -495,7 +497,7 @@ __device__ __forceinline__ void halo_epilogue(const float (&acc)[BN / 2], const 
                 v[h] = acc[4 * j + 2 * h + e] + bv;
                 const size_t o = (static_cast<size_t>(img) * args.out_img_c + oc) * oplane + static_cast<size_t>(oy[h]) * args.OW + ox;
                 if (args.residual != nullptr && valid[h] && oc_ok) v[h] += __ldg(args.residual + o);
-                if (args.relu) v[h] = fmaxf(v[h], 0.f);
+                if (args.act) v[h] = act_clamp<CLIP>(v[h], args.lo, args.hi);
                 if (!args.pool && valid[h] && oc_ok) args.out[o] = v[h];
             }
             if (args.pool) {
@@ -581,10 +583,9 @@ __device__ __forceinline__ void halo_producer(const CUtensorMap* tmX, const CUte
     }
 }
 
-template <int BN, int PLANES>
-__global__ void __launch_bounds__(kThreadsIg, 1)
-conv_igemm_halo_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__ CUtensorMap tmW,
-                       const __grid_constant__ CUtensorMap tmWlo, const HaloArgs args) {
+template <int BN, int PLANES, bool CLIP>
+__device__ __forceinline__ void halo_body(const CUtensorMap& tmX, const CUtensorMap& tmW, const CUtensorMap& tmWlo,
+                                          const HaloArgs& args) {
     constexpr bool BF = PLANES == 3;
     constexpr int NPL = BF ? 2 : PLANES;
     constexpr int kBTile = BN * 32 * (BF ? 2 : 4);
@@ -692,8 +693,22 @@ conv_igemm_halo_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_con
         ptx::wgmma_wait<0>();
         __syncwarp();
         ptx::mbar_arrive_if(&empty_bar[(kbg - 1) % kStagesIg], lane == 0);
-        halo_epilogue<BN>(acc, args, n_blk, img, oy, valid, ox, oplane, SH, SW, c, gq);
+        halo_epilogue<BN, CLIP>(acc, args, n_blk, img, oy, valid, ox, oplane, SH, SW, c, gq);
     }
+}
+
+// The per-tap halo kernel without / with a Clip (see conv_igemm_wide_kernel below).
+template <int BN, int PLANES>
+__global__ void __launch_bounds__(kThreadsIg, 1)
+conv_igemm_halo_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__ CUtensorMap tmW,
+                       const __grid_constant__ CUtensorMap tmWlo, const HaloArgs args) {
+    halo_body<BN, PLANES, false>(tmX, tmW, tmWlo, args);
+}
+template <int BN, int PLANES>
+__global__ void __launch_bounds__(kThreadsIg, 1)
+conv_igemm_halo_clip_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__ CUtensorMap tmW,
+                            const __grid_constant__ CUtensorMap tmWlo, const HaloArgs args) {
+    halo_body<BN, PLANES, true>(tmX, tmW, tmWlo, args);
 }
 
 // Pre-split halo kernel (BF16x3, switch igemm_presplit): the producer and the filter ring of conv_igemm_halo_kernel, but
@@ -710,9 +725,8 @@ conv_igemm_halo_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_con
 //                the 168 registers a 288-thread CTA gets beside the fragment sets (ptxas then serialises the wgmma);
 //                conv_igemm_wide_kernel reaches larger tiles by moving the pixels to the wgmma N side instead.
 // Per k-block the wgmma sequence (p2*q1, p1*q2, p1*q1 per k-step), the operand values, the k order and BN are those of conv_igemm_halo_kernel<BN, 3>: the result is bit-identical to it.
-template <int BN>
-__global__ void __launch_bounds__(kThreadsIg, 1)
-conv_igemm_presplit_kernel(const __grid_constant__ CUtensorMap tmX, const HaloArgs args) {
+template <int BN, bool CLIP>
+__device__ __forceinline__ void presplit_body(const CUtensorMap& tmX, const HaloArgs& args) {
     constexpr int kBTile = BN * 32 * 2;
     constexpr int kStage = 2 * kBTile;
     constexpr int HS = kHaloStages;  // fp32 boxes in flight
@@ -849,8 +863,20 @@ conv_igemm_presplit_kernel(const __grid_constant__ CUtensorMap tmX, const HaloAr
             oy[h] = ty * args.R + prow + h;
             valid[h] = oy[h] < args.OH && ox < args.OW;
         }
-        halo_epilogue<BN>(acc, args, n_blk, img, oy, valid, ox, oplane, SH, SW, c, gq);
+        halo_epilogue<BN, CLIP>(acc, args, n_blk, img, oy, valid, ox, oplane, SH, SW, c, gq);
     }
+}
+
+// The pre-split kernel without / with a Clip (see conv_igemm_wide_kernel below).
+template <int BN>
+__global__ void __launch_bounds__(kThreadsIg, 1)
+conv_igemm_presplit_kernel(const __grid_constant__ CUtensorMap tmX, const HaloArgs args) {
+    presplit_body<BN, false>(tmX, args);
+}
+template <int BN>
+__global__ void __launch_bounds__(kThreadsIg, 1)
+conv_igemm_presplit_clip_kernel(const __grid_constant__ CUtensorMap tmX, const HaloArgs args) {
+    presplit_body<BN, true>(tmX, args);
 }
 
 // Wide pre-split kernel (BF16x3, switch igemm_wide): the GEMM of conv_igemm_presplit_kernel turned around,
@@ -921,7 +947,8 @@ __device__ __forceinline__ void wide_producer(const CUtensorMap* tmX, const Halo
 
 // Epilogue of the wide kernel: accumulator d[4j + i] is output channel oc0 + 8 * (i >> 1), pixel (oy0 + j, ox0 + (i & 1)).
 // Each thread holds both columns of its pooling windows and both rows (j even, j + 1), so pooling needs no shuffle; the
-// order of the bias, residual, ReLU and max operations is halo_epilogue's.
+// order of the bias, residual, clamp and max operations is halo_epilogue's.
+template <bool CLIP>
 __device__ __forceinline__ void wide_epilogue(const float (&acc)[112], const HaloArgs& args, int img, int oc0, int oy0,
                                               int ox0) {
     const int oplane = args.OH * args.OW;
@@ -946,7 +973,7 @@ __device__ __forceinline__ void wide_epilogue(const float (&acc)[112], const Hal
                     ok[r][x] = oy < args.OH && xok[x];
                     v[r][x] = acc[4 * (j + r) + 2 * e + x] + bv;
                     if (args.residual != nullptr && ok[r][x]) v[r][x] += __ldg(args.residual + o + x);
-                    if (args.relu) v[r][x] = fmaxf(v[r][x], 0.f);
+                    if (args.act) v[r][x] = act_clamp<CLIP>(v[r][x], args.lo, args.hi);
                 }
                 if (!args.pool && ok[r][0]) {
                     float* dst = args.out + o;
@@ -968,9 +995,8 @@ __device__ __forceinline__ void wide_epilogue(const float (&acc)[112], const Hal
     }
 }
 
-template <int BN>
-__global__ void __launch_bounds__(kThreadsIg, 1)
-conv_igemm_wide_kernel(const __grid_constant__ CUtensorMap tmX, const HaloArgs args) {
+template <int BN, bool CLIP>
+__device__ __forceinline__ void wide_body(const CUtensorMap& tmX, const HaloArgs& args) {
     constexpr int kBTile = BN * 32 * 2;
     constexpr int kStage = 2 * kBTile;
     constexpr int kConsumers = kConsumerWarps * 32;
@@ -1089,8 +1115,21 @@ conv_igemm_wide_kernel(const __grid_constant__ CUtensorMap tmX, const HaloArgs a
         const HaloTile tile = halo_tile(args, per_img, t);
         const int oc0 = tile.n_blk * BN + (BN == 128 ? 64 * wg : 0) + 16 * (warp & 3) + gq;
         const int ox0 = tile.tx * args.C + (BN == 64 ? 8 * wg : 0) + 2 * c;
-        wide_epilogue(acc, args, tile.img, oc0, tile.ty * kWideRows, ox0);
+        wide_epilogue<CLIP>(acc, args, tile.img, oc0, tile.ty * kWideRows, ox0);
     }
+}
+
+// The wide kernel without / with a Clip: conv_igemm_wide_kernel serves no activation and ReLU with the ReLU epilogue of
+// the other kernels (fmaxf(v, 0)); conv_igemm_wide_clip_kernel clamps to [args.lo, args.hi] (fcuda_conv_forward_clip).
+template <int BN>
+__global__ void __launch_bounds__(kThreadsIg, 1)
+conv_igemm_wide_kernel(const __grid_constant__ CUtensorMap tmX, const HaloArgs args) {
+    wide_body<BN, false>(tmX, args);
+}
+template <int BN>
+__global__ void __launch_bounds__(kThreadsIg, 1)
+conv_igemm_wide_clip_kernel(const __grid_constant__ CUtensorMap tmX, const HaloArgs args) {
+    wide_body<BN, true>(tmX, args);
 }
 
 // Bank model of one ld.shared of the halo gather: lane l reads column l / 4 of channel plane (l % 4) * (2 for the bf16
@@ -1207,7 +1246,7 @@ static HaloArgs halo_args(const IgemmProblem& p, const HaloGeom& hg, int BN) {
     a.out_img_c = p.out_c_total > 0 ? p.out_c_total : p.OC;
     a.kblocks = ceil_div(taps * p.IC, 32);
     a.num_n = ceil_div(p.OC, BN);
-    a.relu = p.relu;
+    a.act = p.act; a.lo = p.lo; a.hi = p.hi;
     a.pool = p.pool ? 1 : 0;
     a.R = hg.R; a.C = hg.C;
     a.tiles_x = ceil_div(p.OW, hg.C);
@@ -1250,24 +1289,31 @@ int launch_halo_family(const IgemmProblem& p, const HaloGeom& hg, int BN, int sm
 // The kernel a layer takes for one N tile and operand format: the gathering kernel, or with switch igemm_halo on a
 // layer halo_geometry accepts the per-tap halo kernel, in BF16x3 mode the pre-split kernel (switch igemm_presplit) and
 // the wide one (switch igemm_wide).
-template <int BN, int PLANES>
+// CLIP: the Clip instantiations (IgemmProblem::act == 2); the others apply a ReLU as fmaxf(v, 0).
+template <int BN, int PLANES, bool CLIP>
 int launch_conv(const IgemmProblem& p, cudaStream_t stream) {
     HaloGeom hg;
-    if (tune_get(TUNE_IGEMM_HALO) == 0 || !halo_geometry(p, hg)) return launch_igemm<BN, PLANES>(p, stream);
+    if (tune_get(TUNE_IGEMM_HALO) == 0 || !halo_geometry(p, hg)) return launch_igemm<BN, PLANES, CLIP>(p, stream);
     if constexpr (PLANES == 3) {
         HaloGeom pg;
         if (tune_get(TUNE_IGEMM_PRESPLIT) != 0 && presplit_geometry(p, pg)) {
             HaloGeom wg;
             if constexpr (BN != 32)  // wide_geometry takes N tiles of 64 and 128 channels only
-                if (tune_get(TUNE_IGEMM_WIDE) != 0 && wide_geometry(p, wg))
+                if (tune_get(TUNE_IGEMM_WIDE) != 0 && wide_geometry(p, wg)) {
+                    if constexpr (CLIP)
+                        return launch_halo_family<conv_igemm_wide_clip_kernel<BN>>(p, wg, BN, wide_smem_bytes(p, wg), 16, stream);
                     return launch_halo_family<conv_igemm_wide_kernel<BN>>(p, wg, BN, wide_smem_bytes(p, wg), 16, stream);
+                }
+            if constexpr (CLIP)
+                return launch_halo_family<conv_igemm_presplit_clip_kernel<BN>>(p, pg, BN, presplit_smem_bytes(p, pg), 32, stream);
             return launch_halo_family<conv_igemm_presplit_kernel<BN>>(p, pg, BN, presplit_smem_bytes(p, pg), 32, stream);
         }
     }
     CUtensorMap tmW, tmWlo;
     if (int rc = filter_maps(p, BN, PLANES, &tmW, &tmWlo)) return rc;
-    return launch_halo_family<conv_igemm_halo_kernel<BN, PLANES>>(p, hg, BN, halo_smem_bytes(p.OC, PLANES, hg.Rb, hg.Cb),
-                                                                  32, stream, tmW, tmWlo);
+    const int smem = halo_smem_bytes(p.OC, PLANES, hg.Rb, hg.Cb);
+    if constexpr (CLIP) return launch_halo_family<conv_igemm_halo_clip_kernel<BN, PLANES>>(p, hg, BN, smem, 32, stream, tmW, tmWlo);
+    return launch_halo_family<conv_igemm_halo_kernel<BN, PLANES>>(p, hg, BN, smem, 32, stream, tmW, tmWlo);
 }
 
 // The geometry query behind the exported conv_igemm_*_geometry: g is written only when the layer takes the kernel
@@ -1328,11 +1374,14 @@ int conv_igemm_forward(const IgemmProblem& p, cudaStream_t stream) {
     if (!conv_igemm_supported(p.IC, p.KH, p.KW)) return -1;
     if (p.pool && !conv_igemm_can_pool(p)) return -200;
     using Launch = int (*)(const IgemmProblem&, cudaStream_t);
-    static const Launch kLaunch[3][3] = {  // [N tile 32, 64, 128][planes 1, 2, 3]
-        {launch_conv<32, 1>, launch_conv<32, 2>, launch_conv<32, 3>},
-        {launch_conv<64, 1>, launch_conv<64, 2>, launch_conv<64, 3>},
-        {launch_conv<128, 1>, launch_conv<128, 2>, launch_conv<128, 3>}};
-    return kLaunch[igemm_bn_for(p.OC) / 64][p.planes == 3 ? 2 : p.planes == 2 ? 1 : 0](p, stream);
+    static const Launch kLaunch[2][3][3] = {  // [Clip][N tile 32, 64, 128][planes 1, 2, 3]
+        {{launch_conv<32, 1, false>, launch_conv<32, 2, false>, launch_conv<32, 3, false>},
+         {launch_conv<64, 1, false>, launch_conv<64, 2, false>, launch_conv<64, 3, false>},
+         {launch_conv<128, 1, false>, launch_conv<128, 2, false>, launch_conv<128, 3, false>}},
+        {{launch_conv<32, 1, true>, launch_conv<32, 2, true>, launch_conv<32, 3, true>},
+         {launch_conv<64, 1, true>, launch_conv<64, 2, true>, launch_conv<64, 3, true>},
+         {launch_conv<128, 1, true>, launch_conv<128, 2, true>, launch_conv<128, 3, true>}}};
+    return kLaunch[p.act == 2][igemm_bn_for(p.OC) / 64][p.planes == 3 ? 2 : p.planes == 2 ? 1 : 0](p, stream);
 }
 
 }  // namespace fcuda

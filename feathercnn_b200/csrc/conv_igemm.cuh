@@ -13,7 +13,8 @@ struct IgemmProblem {
     int N, IC, H, W, OC, OH, OW;
     int KH, KW, pad_top, pad_left, stride_h, stride_w;
     int planes;           // 1 = TF32, 2 = 3xTF32, 3 = BF16x3 (w_hi / w_lo then hold the two bf16 planes)
-    int relu;
+    int act;              // 0 none, 1 ReLU, 2 Clip: clamp to [lo, hi] (the Clip instantiations of every kernel)
+    float lo, hi;
     const float* residual;  // optional (N, OC, OH, OW) tensor added before the activation (fused Eltwise SUM), or null
     // Extensions beyond the reference (it rejects both: conv_layer.h:43-47, avx/booster.cpp:304-308); 0 = default.
     int dil_h, dil_w;       // dilation (0 or 1 = dense taps)

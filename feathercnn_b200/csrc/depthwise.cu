@@ -17,11 +17,11 @@ namespace fcuda {
 
 constexpr int kDwRows = 16;  // output rows marched by one warp
 
-template <int STRIDE>
+template <int STRIDE, bool CLIP>
 __global__ void __launch_bounds__(128)
 dw3x3_shuffle_kernel(const float* __restrict__ in, const float* __restrict__ w, const float* __restrict__ bias,
-                     float* __restrict__ out, int C, int H, int W, int OH, int OW, int relu, long long items,
-                     int xstrips, int ystrips) {
+                     float* __restrict__ out, int C, int H, int W, int OH, int OW, int act, float lo, float hi,
+                     long long items, int xstrips, int ystrips) {
     const long long item = static_cast<long long>(blockIdx.x) * 4 + (threadIdx.x >> 5);
     if (item >= items) return;
     const int lane = threadIdx.x & 31;
@@ -88,7 +88,7 @@ dw3x3_shuffle_kernel(const float* __restrict__ in, const float* __restrict__ w, 
                 float v = fma3(bv, 0, tl, tm, tr);
                 v = fma3(v, 1, ml, mm, mr);
                 v = fma3(v, 2, cl[i], cm[i], cr[i]);
-                if (relu) v = fmaxf(v, 0.f);
+                if (act) v = act_clamp<CLIP>(v, lo, hi);
                 if (ox < OW && oy + i < oy1) op[static_cast<long long>(oy + i) * OW + ox] = v;
             }
             al = cl[NB - 2]; am = cm[NB - 2]; ar = cr[NB - 2];
@@ -125,7 +125,7 @@ dw3x3_shuffle_kernel(const float* __restrict__ in, const float* __restrict__ w, 
                 float v = fma3(bv, 0, tl, tm, tr);
                 v = fma3(v, 1, cl[2 * i], cm[2 * i], cr[2 * i]);
                 v = fma3(v, 2, cl[2 * i + 1], cm[2 * i + 1], cr[2 * i + 1]);
-                if (relu) v = fmaxf(v, 0.f);
+                if (act) v = act_clamp<CLIP>(v, lo, hi);
                 if (ox < OW && oy + i < oy1) op[static_cast<long long>(oy + i) * OW + ox] = v;
             }
             al = cl[2 * NB - 1]; am = cm[2 * NB - 1]; ar = cr[2 * NB - 1];
@@ -146,11 +146,11 @@ template <> struct VecT<1> { typedef float type; };
 template <> struct VecT<2> { typedef float2 type; };
 template <> struct VecT<4> { typedef float4 type; };
 
-template <int STRIDE, int VEC>
+template <int STRIDE, int VEC, bool CLIP>
 __global__ void __launch_bounds__(128)
 dw3x3_vec_kernel(const float* __restrict__ in, const float* __restrict__ w, const float* __restrict__ bias,
-                 float* __restrict__ out, int C, int H, int W, int OH, int OW, int relu, long long items, int xstrips,
-                 int ystrips) {
+                 float* __restrict__ out, int C, int H, int W, int OH, int OW, int act, float lo, float hi, long long items,
+                 int xstrips, int ystrips) {
     constexpr int LW = STRIDE * VEC;  // floats loaded per lane and input row
     typedef typename VecT<LW>::type LoadT;
     typedef typename VecT<VEC>::type StoreT;
@@ -219,7 +219,7 @@ dw3x3_vec_kernel(const float* __restrict__ in, const float* __restrict__ w, cons
             float v = tap(bv, 0, r0, j);
             v = tap(v, 1, r1, j);
             v = tap(v, 2, r2, j);
-            o[j] = relu ? fmaxf(v, 0.f) : v;
+            o[j] = act ? act_clamp<CLIP>(v, lo, hi) : v;
         }
         if (ox0 < OW && oy < oy1) *reinterpret_cast<StoreT*>(op + static_cast<long long>(oy) * OW + ox0) = *reinterpret_cast<StoreT*>(o);
     };
@@ -265,11 +265,11 @@ dw3x3_vec_kernel(const float* __restrict__ in, const float* __restrict__ w, cons
 // 3x3 depthwise on small planes (MobileNet's 14x14 and 7x7 stages, where a 32-wide strip would idle most lanes): one warp
 // per (image, channel) plane.  The plane goes to shared memory with a zero halo of one pixel, then every lane computes
 // output pixels lane, lane+32, ...; row/column come from a 16-bit reciprocal multiply (exact for planes <= 34x34).
-template <int STRIDE>
+template <int STRIDE, bool CLIP>
 __global__ void __launch_bounds__(128)
 dw3x3_plane_kernel(const float* __restrict__ in, const float* __restrict__ w, const float* __restrict__ bias,
-                   float* __restrict__ out, int C, int H, int W, int OH, int OW, int pad_top, int pad_left, int relu,
-                   long long planes) {
+                   float* __restrict__ out, int C, int H, int W, int OH, int OW, int pad_top, int pad_left,
+                   int act, float lo, float hi, long long planes) {
     extern __shared__ float dw_smem[];
     const int PW = W + 2, PH = H + 2;
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -312,7 +312,7 @@ dw3x3_plane_kernel(const float* __restrict__ in, const float* __restrict__ w, co
         for (int u = 0; u < 3; ++u)
 #pragma unroll
             for (int x = 0; x < 3; ++x) v = fmaf(k[u * 3 + x], t[u * PW + x], v);
-        if (relu) v = fmaxf(v, 0.f);
+        if (act) v = act_clamp<CLIP>(v, lo, hi);
         op[o] = v;
     }
 }
@@ -322,10 +322,10 @@ dw3x3_plane_kernel(const float* __restrict__ in, const float* __restrict__ w, co
 // loads in flight per lane), gets the left / right neighbours of every row with sub-warp shuffles and writes its output
 // column.  ~13 instructions per output row and lane; the shared-memory plane kernel above needs ~300 warp instructions per
 // 14x14 plane and is issue-bound there.
-template <int LP>
+template <int LP, bool CLIP>
 __global__ void __launch_bounds__(128)
 dw3x3_cols_kernel(const float* __restrict__ in, const float* __restrict__ w, const float* __restrict__ bias,
-                  float* __restrict__ out, int C, int H, int W, int relu, long long planes) {
+                  float* __restrict__ out, int C, int H, int W, int act, float lo, float hi, long long planes) {
     constexpr int PPW = 32 / LP;  // planes per warp
     const int lane = threadIdx.x & 31, sub = lane / LP, col = lane % LP;
     const long long plane = (static_cast<long long>(blockIdx.x) * 4 + (threadIdx.x >> 5)) * PPW + sub;
@@ -356,16 +356,17 @@ dw3x3_cols_kernel(const float* __restrict__ in, const float* __restrict__ w, con
             if (oy > 0) { v = fmaf(k[0], l[oy - 1], v); v = fmaf(k[1], m[oy - 1], v); v = fmaf(k[2], rr[oy - 1], v); }
             v = fmaf(k[3], l[oy], v); v = fmaf(k[4], m[oy], v); v = fmaf(k[5], rr[oy], v);
             if (oy + 1 < 16) { v = fmaf(k[6], l[oy + 1], v); v = fmaf(k[7], m[oy + 1], v); v = fmaf(k[8], rr[oy + 1], v); }
-            if (relu) v = fmaxf(v, 0.f);
+            if (act) v = act_clamp<CLIP>(v, lo, hi);
             if (ok) op[oy * W] = v;
         }
     }
 }
 
 // Generic k x k / any stride / any padding depthwise: one thread per output element.
+template <bool CLIP>
 __global__ void __launch_bounds__(256)
 dw_generic_kernel(const float* __restrict__ in, const float* __restrict__ w, const float* __restrict__ bias,
-                  float* __restrict__ out, DwGeom g, int relu, long long total) {
+                  float* __restrict__ out, DwGeom g, int act, float lo, float hi, long long total) {
     const long long idx = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
     if (idx >= total) return;
     const int ox = static_cast<int>(idx % g.OW);
@@ -386,17 +387,16 @@ dw_generic_kernel(const float* __restrict__ in, const float* __restrict__ w, con
         }
     }
     if (bias) v += __ldg(bias + c);
-    if (relu) v = fmaxf(v, 0.f);
+    if (act) v = act_clamp<CLIP>(v, lo, hi);
     out[idx] = v;
 }
 
-int depthwise_forward(const float* in, const float* w, const float* bias, float* out, const DwGeom& g, int relu,
-                      int batch, cudaStream_t s) {
+// The kernel choice of depthwise_forward; CLIP selects the Clip instantiations (act == 2).
+template <bool CLIP>
+static void dw_launch(const float* in, const float* w, const float* bias, float* out, const DwGeom& g, int act, float lo,
+                      float hi, int batch, cudaStream_t s) {
     const bool k3 = g.KH == 3 && g.KW == 3 && g.pad_top == 1 && g.pad_left == 1 && g.stride_h == g.stride_w &&
                     (g.stride_h == 1 || g.stride_h == 2) && g.OW >= 24;
-    const double planes = static_cast<double>(batch) * g.C;
-    const int prof = prof_begin(s, PROF_DEPTHWISE, 2.0 * planes * g.OH * g.OW * g.KH * g.KW, 0,
-                                4.0 * planes * (static_cast<double>(g.H) * g.W + static_cast<double>(g.OH) * g.OW));
     // vector width: the widest VEC whose strips (32 * VEC outputs) still fill most lanes and keep accesses aligned
     const bool vec_off = tune_get(TUNE_DW_VEC) == 0;
     int vec = 1;
@@ -410,7 +410,7 @@ int depthwise_forward(const float* in, const float* w, const float* bias, float*
         const int xstrips = ceil_div(g.OW, 32 * vec), ystrips = ceil_div(g.OH, kDwRows);
         const long long items = static_cast<long long>(batch) * g.C * xstrips * ystrips;
         const unsigned blocks = static_cast<unsigned>((items + 3) / 4);
-#define DW_VEC_LAUNCH(S, V) dw3x3_vec_kernel<S, V><<<blocks, 128, 0, s>>>(in, w, bias, out, g.C, g.H, g.W, g.OH, g.OW, relu, items, xstrips, ystrips)
+#define DW_VEC_LAUNCH(S, V) dw3x3_vec_kernel<S, V, CLIP><<<blocks, 128, 0, s>>>(in, w, bias, out, g.C, g.H, g.W, g.OH, g.OW, act, lo, hi, items, xstrips, ystrips)
         if (g.stride_h == 1 && vec == 4) DW_VEC_LAUNCH(1, 4);
         else if (g.stride_h == 1) DW_VEC_LAUNCH(1, 2);
         else DW_VEC_LAUNCH(2, 2);
@@ -420,20 +420,20 @@ int depthwise_forward(const float* in, const float* w, const float* bias, float*
         const long long items = static_cast<long long>(batch) * g.C * xstrips * ystrips;
         const unsigned blocks = static_cast<unsigned>((items + 3) / 4);
         if (g.stride_h == 1)
-            dw3x3_shuffle_kernel<1><<<blocks, 128, 0, s>>>(in, w, bias, out, g.C, g.H, g.W, g.OH, g.OW, relu, items,
+            dw3x3_shuffle_kernel<1, CLIP><<<blocks, 128, 0, s>>>(in, w, bias, out, g.C, g.H, g.W, g.OH, g.OW, act, lo, hi, items,
                                                             xstrips, ystrips);
         else
-            dw3x3_shuffle_kernel<2><<<blocks, 128, 0, s>>>(in, w, bias, out, g.C, g.H, g.W, g.OH, g.OW, relu, items,
+            dw3x3_shuffle_kernel<2, CLIP><<<blocks, 128, 0, s>>>(in, w, bias, out, g.C, g.H, g.W, g.OH, g.OW, act, lo, hi, items,
                                                             xstrips, ystrips);
     } else if (!vec_off && g.KH == 3 && g.KW == 3 && g.pad_top == 1 && g.pad_left == 1 && g.stride_h == 1 && g.stride_w == 1 &&
                g.H <= 16 && g.W <= 16 && g.OH == g.H && g.OW == g.W) {
         const long long planes_ll = static_cast<long long>(batch) * g.C;
         if (g.W <= 8) {
             const unsigned blocks = static_cast<unsigned>((planes_ll + 15) / 16);
-            dw3x3_cols_kernel<8><<<blocks, 128, 0, s>>>(in, w, bias, out, g.C, g.H, g.W, relu, planes_ll);
+            dw3x3_cols_kernel<8, CLIP><<<blocks, 128, 0, s>>>(in, w, bias, out, g.C, g.H, g.W, act, lo, hi, planes_ll);
         } else {
             const unsigned blocks = static_cast<unsigned>((planes_ll + 7) / 8);
-            dw3x3_cols_kernel<16><<<blocks, 128, 0, s>>>(in, w, bias, out, g.C, g.H, g.W, relu, planes_ll);
+            dw3x3_cols_kernel<16, CLIP><<<blocks, 128, 0, s>>>(in, w, bias, out, g.C, g.H, g.W, act, lo, hi, planes_ll);
         }
     } else if (g.KH == 3 && g.KW == 3 && (g.pad_top == 0 || g.pad_top == 1) && (g.pad_left == 0 || g.pad_left == 1) &&
                g.stride_h == g.stride_w && (g.stride_h == 1 || g.stride_h == 2) && g.H <= 34 && g.W <= 34 &&
@@ -443,15 +443,24 @@ int depthwise_forward(const float* in, const float* w, const float* bias, float*
         const unsigned blocks = static_cast<unsigned>((planes_ll + 3) / 4);
         const int smem = 4 * (g.H + 2) * (g.W + 2) * static_cast<int>(sizeof(float));
         if (g.stride_h == 1)
-            dw3x3_plane_kernel<1><<<blocks, 128, smem, s>>>(in, w, bias, out, g.C, g.H, g.W, g.OH, g.OW, g.pad_top,
-                                                             g.pad_left, relu, planes_ll);
+            dw3x3_plane_kernel<1, CLIP><<<blocks, 128, smem, s>>>(in, w, bias, out, g.C, g.H, g.W, g.OH, g.OW, g.pad_top,
+                                                             g.pad_left, act, lo, hi, planes_ll);
         else
-            dw3x3_plane_kernel<2><<<blocks, 128, smem, s>>>(in, w, bias, out, g.C, g.H, g.W, g.OH, g.OW, g.pad_top,
-                                                             g.pad_left, relu, planes_ll);
+            dw3x3_plane_kernel<2, CLIP><<<blocks, 128, smem, s>>>(in, w, bias, out, g.C, g.H, g.W, g.OH, g.OW, g.pad_top,
+                                                             g.pad_left, act, lo, hi, planes_ll);
     } else {
         const long long total = static_cast<long long>(batch) * g.C * g.OH * g.OW;
-        dw_generic_kernel<<<static_cast<unsigned>((total + 255) / 256), 256, 0, s>>>(in, w, bias, out, g, relu, total);
+        dw_generic_kernel<CLIP><<<static_cast<unsigned>((total + 255) / 256), 256, 0, s>>>(in, w, bias, out, g, act, lo, hi, total);
     }
+}
+
+int depthwise_forward(const float* in, const float* w, const float* bias, float* out, const DwGeom& g, int act, float lo,
+                      float hi, int batch, cudaStream_t s) {
+    const double planes = static_cast<double>(batch) * g.C;
+    const int prof = prof_begin(s, PROF_DEPTHWISE, 2.0 * planes * g.OH * g.OW * g.KH * g.KW, 0,
+                                4.0 * planes * (static_cast<double>(g.H) * g.W + static_cast<double>(g.OH) * g.OW));
+    if (act == 2) dw_launch<true>(in, w, bias, out, g, act, lo, hi, batch, s);
+    else dw_launch<false>(in, w, bias, out, g, act, lo, hi, batch, s);
     prof_end(prof, s);
     FCUDA_CHECK_LAUNCH();
     count_launch();

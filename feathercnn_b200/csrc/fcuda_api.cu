@@ -356,7 +356,7 @@ int fcuda_conv_init(const FcudaConvParam* p, int algo, float* packed, const floa
 
 static int conv_forward_impl(const FcudaConvParam* p, int algo, float* output, const float* input, const float* packed,
                              float* scratch, const float* bias, const float* residual, int relu_after_add, int batch,
-                             void* stream, int dil_h = 1, int dil_w = 1, int pool = 0);
+                             void* stream, int dil_h = 1, int dil_w = 1, int pool = 0, const float* clip = nullptr);
 
 int fcuda_conv_forward_ext(const FcudaConvParam* p, int algo, float* output, const float* input, const float* packed,
                            float* scratch, const float* bias, const float* residual, int relu_after_add, int dilation_h,
@@ -376,6 +376,14 @@ int fcuda_conv_forward(const FcudaConvParam* p, int algo, float* output, const f
     return conv_forward_impl(p, algo, output, input, packed, scratch, bias, nullptr, 0, batch, stream);
 }
 
+int fcuda_conv_forward_clip(const FcudaConvParam* p, int algo, float* output, const float* input, const float* packed,
+                            float* scratch, const float* bias, float clip_min, float clip_max, int batch, void* stream) {
+    if (!p) return -100;
+    if (p->activation != FCUDA_ACT_CLIP || !(clip_min <= clip_max)) return -200;
+    const float clip[2] = {clip_min, clip_max};
+    return conv_forward_impl(p, algo, output, input, packed, scratch, bias, nullptr, 0, batch, stream, 1, 1, 0, clip);
+}
+
 int fcuda_conv_forward_residual(const FcudaConvParam* p, int algo, float* output, const float* input, const float* packed,
                                 float* scratch, const float* bias, const float* residual, int relu_after_add, int batch,
                                 void* stream) {
@@ -391,16 +399,22 @@ int fcuda_conv_forward_residual(const FcudaConvParam* p, int algo, float* output
 
 static int conv_forward_impl(const FcudaConvParam* p, int algo, float* output, const float* input, const float* packed,
                              float* scratch, const float* bias, const float* residual, int relu_after_add, int batch,
-                             void* stream, int dil_h, int dil_w, int pool) {
+                             void* stream, int dil_h, int dil_w, int pool, const float* clip) {
     ConvPlan pl;
     int rc = make_plan(p, algo, batch, &pl);
     if (rc) return rc;
+    if (p->activation == FCUDA_ACT_CLIP && !clip) return -200;  // only fcuda_conv_forward_clip carries the bounds
     if (!output || !input || !packed) return -100;
     if (pl.scratch_floats && !scratch) return -100;
     cudaStream_t s = as_stream(stream);
     const int IC = p->input_channels, OC = p->output_channels;
     const float* b = p->bias_term ? bias : nullptr;
-    const int relu = p->activation == FCUDA_ACT_RELU;
+    // epilogue activation: 0 none, 1 ReLU (fmaxf(v, 0)), 2 Clip: min(max(v, lo), hi) in the Clip instantiations of the
+    // kernels.  [0, +inf] stands for a ReLU where a kernel takes the bounds at run time (fminf(fmaxf(v, 0), +inf) is
+    // fmaxf(v, 0) bit for bit, NaN included).
+    const int act = p->activation == FCUDA_ACT_RELU ? 1 : p->activation == FCUDA_ACT_CLIP ? 2 : 0;
+    const float lo = act == 2 ? clip[0] : 0.f;
+    const float hi = act == 2 ? clip[1] : INFINITY;
     switch (algo) {
         case FCUDA_WINOGRADF63:
         case FCUDA_WINOGRADF23: {
@@ -422,7 +436,7 @@ static int conv_forward_impl(const FcudaConvParam* p, int algo, float* output, c
                 g.algo_flops = 2.0 * OC * IC * 9.0 * p->output_h * p->output_w * batch *
                                (static_cast<double>(R1 - R0) / pl.total_tile_rows);
                 if ((rc = tensor_gemm(g, s))) return rc;
-                if ((rc = wino_output_transform(pl.tile, Mbuf, output, b, pl.wg, R0, R1, relu, pool, s))) return rc;
+                if ((rc = wino_output_transform(pl.tile, Mbuf, output, b, pl.wg, R0, R1, act, lo, hi, pool, s))) return rc;
             }
             return 0;
         }
@@ -440,7 +454,8 @@ static int conv_forward_impl(const FcudaConvParam* p, int algo, float* output, c
                 g.D = output;
                 g.M = rows; g.N = OC; g.K = pl.pg.Kp; g.G = 1;
                 g.planes = pl.np; g.epilogue = EPI_NCHW; g.P = p->output_h * p->output_w; g.m_offset = m0;
-                g.bias = b; g.relu = relu; g.split_k = 1;
+                g.bias = b; g.relu = act != 0; g.split_k = 1;
+                g.clip = act == 2; g.clip_lo = lo; g.clip_hi = hi;
                 g.algo_flops = 2.0 * OC * pl.pg.K * static_cast<double>(rows);
                 if ((rc = tensor_gemm(g, s))) return rc;
             }
@@ -474,7 +489,12 @@ static int conv_forward_impl(const FcudaConvParam* p, int algo, float* output, c
                 } else {
                     g.H = p->input_h; g.W = p->input_w; g.OH = p->output_h; g.OW = p->output_w;
                 }
-                g.planes = igemm_planes(); g.relu = residual ? relu_after_add : relu;
+                g.planes = igemm_planes();
+                if (residual) {  // the convolution has no activation of its own (see fcuda_conv_forward_residual)
+                    g.act = relu_after_add; g.lo = 0.f; g.hi = INFINITY;
+                } else {
+                    g.act = act; g.lo = lo; g.hi = hi;
+                }
                 g.pool = pool;
                 if (pool) {  // pooled output planes
                     g.output = output + static_cast<size_t>(gi) * OCg * (static_cast<size_t>((p->output_h + 1) / 2) * ((p->output_w + 1) / 2));
@@ -486,10 +506,10 @@ static int conv_forward_impl(const FcudaConvParam* p, int algo, float* output, c
         }
         case FCUDA_NAIVE:
             if (pool) return -200;
-            return conv_direct(input, packed, b, output, pl.pg, OC, relu, batch, s);
+            return conv_direct(input, packed, b, output, pl.pg, OC, act, lo, hi, batch, s);
         case FCUDA_DEPTHWISE:
             if (pool) return -200;
-            return depthwise_forward(input, packed, b, output, pl.dg, relu, batch, s);
+            return depthwise_forward(input, packed, b, output, pl.dg, act, lo, hi, batch, s);
         default:
             return -1;
     }
@@ -681,6 +701,19 @@ int fcuda_eltwise_forward(float* output, const float* a, const float* b, size_t 
 int fcuda_relu_forward(float* output, const float* input, size_t n, void* stream) {
     if (!output || !input) return -100;
     return scale_relu(input, output, n, 1.f, 1, as_stream(stream));
+}
+
+int fcuda_clip_forward(float* output, const float* input, size_t n, float min, float max, void* stream) {
+    if (!output || !input) return -100;
+    if (!(min <= max)) return -200;
+    return clip(input, output, n, min, max, as_stream(stream));
+}
+
+int fcuda_prelu_forward(float* output, const float* input, int channels, size_t plane, const float* slope, int num_slope,
+                        int batch, void* stream) {
+    if (!output || !input || !slope || channels <= 0 || plane == 0 || batch < 1) return -100;
+    if (num_slope != 1 && num_slope != channels) return -200;
+    return prelu(input, output, slope, channels, plane, num_slope == 1, batch, as_stream(stream));
 }
 
 int fcuda_softmax_forward(float* output, const float* input, size_t n_per_image, int batch, void* stream) {

@@ -213,6 +213,45 @@ scale_relu_kernel(const float* __restrict__ in, float* __restrict__ out, size_t 
     }
 }
 
+// ncnn's Clip (and Caffe's ReLU6 = Clip 0..6): y = min(max(x, lo), hi).  NaN becomes lo: fmaxf returns its non-NaN
+// operand (ncnn's compare-and-assign passes NaN through).  In place (in == out) is allowed.
+__global__ void __launch_bounds__(256)
+clip_kernel(const float* in, float* out, size_t n, float lo, float hi) {
+    const size_t stride = static_cast<size_t>(gridDim.x) * blockDim.x;
+    const bool vec = ((reinterpret_cast<uintptr_t>(in) | reinterpret_cast<uintptr_t>(out)) & 15) == 0;
+    const size_t nv = vec ? n >> 2 : 0;
+    for (size_t i = static_cast<size_t>(blockIdx.x) * blockDim.x + threadIdx.x; i < nv; i += stride) {
+        const float4 x = reinterpret_cast<const float4*>(in)[i];
+        reinterpret_cast<float4*>(out)[i] = make_float4(fminf(fmaxf(x.x, lo), hi), fminf(fmaxf(x.y, lo), hi),
+                                                        fminf(fmaxf(x.z, lo), hi), fminf(fmaxf(x.w, lo), hi));
+    }
+    for (size_t i = (nv << 2) + static_cast<size_t>(blockIdx.x) * blockDim.x + threadIdx.x; i < n; i += stride)
+        out[i] = fminf(fmaxf(in[i], lo), hi);
+}
+
+// ncnn's PReLU: y = x < 0 ? x * slope[c] : x over (batch, channels, plane); one slope per channel, or slope[0] for all
+// (shared).  VEC: plane % 4 == 0 and 16-byte aligned tensors, so a float4 never straddles two channels.  In place allowed.
+template <bool VEC>
+__global__ void __launch_bounds__(256)
+prelu_kernel(const float* in, float* out, const float* __restrict__ slope, int channels, size_t plane, int shared,
+             size_t n) {
+    const size_t stride = static_cast<size_t>(gridDim.x) * blockDim.x;
+    const size_t items = VEC ? n >> 2 : n;
+    for (size_t i = static_cast<size_t>(blockIdx.x) * blockDim.x + threadIdx.x; i < items; i += stride) {
+        const size_t e = VEC ? i << 2 : i;
+        const float a = __ldg(slope + (shared ? 0 : static_cast<int>((e / plane) % channels)));
+        if (VEC) {
+            float4 x = reinterpret_cast<const float4*>(in)[i];
+            x = make_float4(x.x < 0.f ? x.x * a : x.x, x.y < 0.f ? x.y * a : x.y, x.z < 0.f ? x.z * a : x.z,
+                            x.w < 0.f ? x.w * a : x.w);
+            reinterpret_cast<float4*>(out)[i] = x;
+        } else {
+            const float x = in[i];
+            out[i] = x < 0.f ? x * a : x;
+        }
+    }
+}
+
 // SoftmaxLayer::Forward, softmax_layer.h:32-55: max-subtracted softmax over the whole blob of one image.
 // One block per image.
 __global__ void __launch_bounds__(256)
@@ -349,6 +388,28 @@ int eltwise(const float* a, const float* b, float* out, size_t n, int op, float 
 
 int scale_relu(const float* in, float* out, size_t n, float scale, int relu, cudaStream_t s) {
     scale_relu_kernel<<<grid_for(n / 4 + 1, 256), 256, 0, s>>>(in, out, n, scale, relu);
+    FCUDA_CHECK_LAUNCH();
+    count_launch();
+    return 0;
+}
+
+int clip(const float* in, float* out, size_t n, float lo, float hi, cudaStream_t s) {
+    const int prof = prof_begin(s, PROF_ELEMENTWISE, 0, 0, 8.0 * n);
+    clip_kernel<<<grid_for(n / 4 + 1, 256), 256, 0, s>>>(in, out, n, lo, hi);
+    prof_end(prof, s);
+    FCUDA_CHECK_LAUNCH();
+    count_launch();
+    return 0;
+}
+
+int prelu(const float* in, float* out, const float* slope, int channels, size_t plane, int shared, int batch,
+          cudaStream_t s) {
+    const size_t n = static_cast<size_t>(batch) * channels * plane;
+    const int prof = prof_begin(s, PROF_ELEMENTWISE, 0, 0, 8.0 * n + 4.0 * (shared ? 1 : channels));
+    const bool vec = plane % 4 == 0 && ((reinterpret_cast<uintptr_t>(in) | reinterpret_cast<uintptr_t>(out)) & 15) == 0;
+    if (vec) prelu_kernel<true><<<grid_for(n / 4 + 1, 256), 256, 0, s>>>(in, out, slope, channels, plane, shared, n);
+    else prelu_kernel<false><<<grid_for(n, 256), 256, 0, s>>>(in, out, slope, channels, plane, shared, n);
+    prof_end(prof, s);
     FCUDA_CHECK_LAUNCH();
     count_launch();
     return 0;

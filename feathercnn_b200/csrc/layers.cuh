@@ -13,6 +13,11 @@ int add_relu(const float* a, const float* b, float* out, size_t n, int relu, cud
 // op 0 = a*b, 1 = ca*a + cb*b, 2 = max(a, b); then optional ReLU (ncnn Eltwise semantics)
 int eltwise(const float* a, const float* b, float* out, size_t n, int op, float ca, float cb, int relu, cudaStream_t s);
 int scale_relu(const float* in, float* out, size_t n, float scale, int relu, cudaStream_t s);
+// y = min(max(x, lo), hi) (NaN -> lo); in place allowed.
+int clip(const float* in, float* out, size_t n, float lo, float hi, cudaStream_t s);
+// y = x < 0 ? x * slope[c] : x over (batch, channels, plane); shared != 0: slope[0] for every channel.  In place allowed.
+int prelu(const float* in, float* out, const float* slope, int channels, size_t plane, int shared, int batch,
+          cudaStream_t s);
 int softmax_forward(const float* in, float* out, size_t n_per_image, int batch, cudaStream_t s);
 int copy_channels(const float* src, float* dst, size_t per_image, size_t dst_image, size_t dst_offset, int batch,
                   cudaStream_t s);

@@ -37,7 +37,8 @@ struct GemmKernelArgs {
     float* D;
     const float* bias;
     int M, N, K, G;
-    int epilogue, ldd, P, relu, split_k;
+    int epilogue, ldd, P, act, split_k;
+    float lo, hi;  // EPI_NCHW, act != 0: the Clip bounds ([0, +inf] for a ReLU, which the simt kernel clamps to)
     int num_m, num_n, k_blocks_total;
     long long m_offset;
     long long split_stride;
@@ -45,7 +46,7 @@ struct GemmKernelArgs {
 };
 
 // Stores the two rows (m0, m0 + 8) x BN/4 column pairs this thread holds through the fused store of args.epilogue.
-template <int BN>
+template <int BN, bool CLIP>
 __device__ __forceinline__ void epilogue_store(const GemmKernelArgs& args, const float (&acc)[BN / 2], int g, int m0,
                                                int n_base, int c, int ks) {
 #pragma unroll
@@ -78,7 +79,7 @@ __device__ __forceinline__ void epilogue_store(const GemmKernelArgs& args, const
                     if (n < args.N) {
                         float v = acc[4 * j + 2 * h + e];
                         if (args.bias) v += __ldg(args.bias + n);
-                        if (args.relu) v = fmaxf(v, 0.f);
+                        if (args.act) v = act_clamp<CLIP>(v, args.lo, args.hi);
                         dst[static_cast<size_t>(n) * args.P] = v;
                     }
                 }
@@ -133,7 +134,7 @@ __device__ __forceinline__ void load_a_fragments(uint32_t a_base, int row0, int 
     }
 }
 
-template <int BN, int PLANES>
+template <int BN, int PLANES, bool CLIP>
 __global__ void __launch_bounds__(kThreads, 1)
 tensor_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                    const __grid_constant__ CUtensorMap tmBlo, const GemmKernelArgs args) {
@@ -197,7 +198,7 @@ tensor_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constan
         __syncwarp();
         if (lane == 0) ptx::mbar_arrive(&empty_bar[stage]);
     }
-    epilogue_store<BN>(args, acc, tc.g, tc.m_blk * kBM + row0, tc.n_blk * BN, c, tc.ks);
+    epilogue_store<BN, CLIP>(args, acc, tc.g, tc.m_blk * kBM + row0, tc.n_blk * BN, c, tc.ks);
 }
 
 // tensor_gemm_pipe_kernel<BN, PLANES>: the same tiles, k-blocks, wgmma sequence and epilogue as tensor_gemm_kernel, so the
@@ -207,7 +208,7 @@ tensor_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constan
 //   - call-free bounded waits: a call inside the pipeline would make ptxas serialise every wgmma;
 //   - persistent CTAs that walk the tile order with a static stride; the producer keeps a running k-block count across
 //     tiles, so it fills the next tile's stages while the consumers run the epilogue.
-template <int BN, int PLANES>
+template <int BN, int PLANES, bool CLIP>
 __global__ void __launch_bounds__(kThreads, 1)
 tensor_gemm_pipe_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                         const __grid_constant__ CUtensorMap tmBlo, const GemmKernelArgs args, int tiles) {
@@ -294,7 +295,7 @@ tensor_gemm_pipe_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_co
         ptx::wgmma_wait<0>();
         __syncwarp();
         ptx::mbar_arrive_if(&empty_bar[(kbg - 1) % kStages], lane == 0);  // the producer refills it during the epilogue
-        epilogue_store<BN>(args, acc, tc.g, tc.m_blk * kBM + row0, tc.n_blk * BN, c, tc.ks);
+        epilogue_store<BN, CLIP>(args, acc, tc.g, tc.m_blk * kBM + row0, tc.n_blk * BN, c, tc.ks);
     }
 }
 
@@ -458,10 +459,18 @@ bool tensor_gemm_supported(const GemmProblem& p) {
     return true;
 }
 
+// The epilogue clamp of a problem: its Clip bounds, or [0, +inf] for a ReLU (fmaxf(v, 0) bit for bit, NaN included)
+static void set_activation(const GemmProblem& p, int* act, float* lo, float* hi) {
+    *act = p.clip || p.relu;
+    *lo = p.clip ? p.clip_lo : 0.f;
+    *hi = p.clip ? p.clip_hi : INFINITY;
+}
+
 static void fill_kernel_args(const GemmProblem& p, int bn, GemmKernelArgs* a) {
     a->D = p.D; a->bias = p.bias;
     a->M = p.M; a->N = p.N; a->K = p.K; a->G = p.G;
-    a->epilogue = p.epilogue; a->ldd = p.ldd; a->P = p.P > 0 ? p.P : 1; a->relu = p.relu;
+    a->epilogue = p.epilogue; a->ldd = p.ldd; a->P = p.P > 0 ? p.P : 1;
+    set_activation(p, &a->act, &a->lo, &a->hi);
     a->m_offset = p.m_offset;
     a->split_stride = p.split_stride;
     a->num_m = ceil_div(p.M, kBM);
@@ -480,7 +489,7 @@ int tensor_gemm_effective_split(int K, int split_k) {
     return s;
 }
 
-template <int BN, int PLANES>
+template <int BN, int PLANES, bool CLIP>
 static int launch(const GemmProblem& p, cudaStream_t stream) {
     constexpr int kStage = kBM * kBK * 4 + PLANES * BN * kBK * 4;
     static_assert(kStages * kStage + 1024 <= 227 * 1024, "smem budget");
@@ -498,8 +507,8 @@ static int launch(const GemmProblem& p, cudaStream_t stream) {
     if (total > 0x7fffffffLL) return -1;
     const int smem = kStages * kStage + 1024;
     const bool pipe = tune_get(TUNE_GEMM_PIPE) != 0;
-    auto kern = tensor_gemm_kernel<BN, PLANES>;
-    auto pkern = tensor_gemm_pipe_kernel<BN, PLANES>;
+    auto kern = tensor_gemm_kernel<BN, PLANES, CLIP>;
+    auto pkern = tensor_gemm_pipe_kernel<BN, PLANES, CLIP>;
     static SmemAttrCache attr_cache, pattr_cache;
     if (int rc2 = pipe ? ensure_dynamic_smem(pkern, smem, pattr_cache) : ensure_dynamic_smem(kern, smem, attr_cache))
         return rc2;
@@ -518,18 +527,24 @@ static int launch(const GemmProblem& p, cudaStream_t stream) {
     return 0;
 }
 
+// N tile: the smallest supported tile that covers N (fewer wasted MMA columns), capped at 128.  CLIP: the instantiations
+// whose EPI_NCHW epilogue clamps to [clip_lo, clip_hi]; the others apply a ReLU as fmaxf(v, 0).
+template <bool CLIP>
+static int launch_tile(const GemmProblem& p, cudaStream_t stream) {
+    if (p.planes == 2) {
+        if (p.N <= 32) return launch<32, 2, CLIP>(p, stream);
+        if (p.N <= 64) return launch<64, 2, CLIP>(p, stream);
+        return launch<128, 2, CLIP>(p, stream);
+    }
+    if (p.N <= 32) return launch<32, 1, CLIP>(p, stream);
+    if (p.N <= 64) return launch<64, 1, CLIP>(p, stream);
+    return launch<128, 1, CLIP>(p, stream);
+}
+
 int tensor_gemm(const GemmProblem& p, cudaStream_t stream) {
     if (!tensor_gemm_supported(p)) return -1;
     if (p.split_k > 1 && p.epilogue != EPI_COLMAJOR_PARTIAL) return -1;
-    // N tile: the smallest supported tile that covers N (fewer wasted MMA columns), capped at 128
-    if (p.planes == 2) {
-        if (p.N <= 32) return launch<32, 2>(p, stream);
-        if (p.N <= 64) return launch<64, 2>(p, stream);
-        return launch<128, 2>(p, stream);
-    }
-    if (p.N <= 32) return launch<32, 1>(p, stream);
-    if (p.N <= 64) return launch<64, 1>(p, stream);
-    return launch<128, 1>(p, stream);
+    return p.clip ? launch_tile<true>(p, stream) : launch_tile<false>(p, stream);
 }
 
 // --------------------------------------------------------------------------------------------
@@ -590,7 +605,7 @@ simt_gemm_kernel(const float* __restrict__ A_hi, const float* __restrict__ A_lo,
                 const long long mg = args.m_offset + m;
                 const int img = static_cast<int>(mg / args.P), pix = static_cast<int>(mg - static_cast<long long>(img) * args.P);
                 if (args.bias) v += args.bias[n];
-                if (args.relu) v = fmaxf(v, 0.f);
+                if (args.act) v = fminf(fmaxf(v, args.lo), args.hi);
                 args.D[(static_cast<size_t>(img) * args.N + n) * args.P + pix] = v;
             } else {
                 args.D[static_cast<size_t>(n) * args.ldd + m] = v;
@@ -603,8 +618,9 @@ int simt_gemm(const GemmProblem& p, cudaStream_t stream) {
     GemmKernelArgs a;
     a.D = p.D; a.bias = p.bias;
     a.M = p.M; a.N = p.N; a.K = p.K; a.G = p.G;
-    a.epilogue = p.epilogue; a.ldd = p.ldd; a.P = p.P > 0 ? p.P : 1; a.relu = p.relu; a.split_k = 1; a.m_offset = p.m_offset; a.split_stride = 0;
+    a.epilogue = p.epilogue; a.ldd = p.ldd; a.P = p.P > 0 ? p.P : 1; a.split_k = 1; a.m_offset = p.m_offset; a.split_stride = 0;
     a.num_m = ceil_div(p.M, 64); a.num_n = ceil_div(p.N, 64); a.k_blocks_total = 0;
+    set_activation(p, &a.act, &a.lo, &a.hi);
     const long long as = p.a_batch_stride ? p.a_batch_stride : static_cast<long long>(p.M) * p.K;
     const long long bs = p.b_batch_stride ? p.b_batch_stride : static_cast<long long>(p.N) * p.K;
     dim3 grid(a.num_n, a.num_m, p.G);

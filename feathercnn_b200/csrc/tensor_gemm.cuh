@@ -45,6 +45,8 @@ struct GemmProblem {
     long long m_offset;  // EPI_NCHW: global pixel index of row 0 (chunked im2col); image = (m_offset + m) / P
     const float* bias; // EPI_NCHW: per-n bias or null
     int relu;          // EPI_NCHW: fuse max(0, .)
+    int clip;          // EPI_NCHW: fuse min(max(., clip_lo), clip_hi) instead of the ReLU
+    float clip_lo, clip_hi;
     int split_k;       // >=1; only with EPI_COLMAJOR_PARTIAL
     long long split_stride;  // EPI_COLMAJOR_PARTIAL: floats between the partial planes of consecutive k-splits
     long long a_batch_stride;  // floats between consecutive g in A; 0 => dense (M*K)

@@ -270,14 +270,14 @@ wino_input_kernel(const float* __restrict__ in, float* __restrict__ V, WinoGeom 
 }
 
 // ------------------------------------------------------------------------------------------------
-// Output transform  Y = A^T M A  (+bias, ReLU), clipped NCHW store; POOL: a following 2x2 / stride-2 max pooling
+// Output transform  Y = A^T M A  (+bias, ReLU / Clip clamp), clipped NCHW store; POOL: a following 2x2 / stride-2 max pooling
 // (pooling_layer.h:38-91, pad 0) is applied to the tile in registers — the 6x6 (2x2) output tile starts at an even
 // coordinate, so no window straddles two tiles — and only the pooled (OH+1)/2 x (OW+1)/2 blob is written.
 // ------------------------------------------------------------------------------------------------
-template <int T, bool POOL, bool MLP>
+template <int T, bool POOL, bool MLP, bool CLIP>
 __global__ void __launch_bounds__(kXformThreads)
 wino_output_kernel(const float* __restrict__ M, float* __restrict__ out, const float* __restrict__ bias, WinoGeom g,
-                   int R0, int Tc, int relu, int ncb) {
+                   int R0, int Tc, int act, float lo, float hi, int ncb) {
     using W = Wino<T>;
     constexpr int OT = W::kOut;
     constexpr int ST = POOL ? OT / 2 : OT;     // rows / columns of the tile as stored
@@ -335,7 +335,7 @@ wino_output_kernel(const float* __restrict__ M, float* __restrict__ out, const f
 #pragma unroll
                 for (int j = 0; j < OT; ++j) {
                     float v = s[j] + bv;
-                    if (relu) v = fmaxf(v, 0.f);
+                    if (act) v = act_clamp<CLIP>(v, lo, hi);
                     dst[i * COLS + j] = v;
                 }
             }
@@ -357,8 +357,8 @@ wino_output_kernel(const float* __restrict__ M, float* __restrict__ out, const f
                         v = fmaxf(v, s1[j]);
                         if (c1) v = fmaxf(v, s1[j + 1]);
                     }
-                    v += bv;  // max commutes with the per-channel bias and with ReLU
-                    if (relu) v = fmaxf(v, 0.f);
+                    v += bv;  // max commutes with the per-channel bias and with the clamp
+                    if (act) v = act_clamp<CLIP>(v, lo, hi);
                     dst[(i >> 1) * COLS + (j >> 1)] = v;
                 }
             }
@@ -427,8 +427,25 @@ int wino_input_transform(int tile, const float* in, float* V, const WinoGeom& g,
     return 0;
 }
 
+template <bool CLIP>
+static void wino_output_launch(int tile, int pool, bool mlp, dim3 grid, const float* M, float* out, const float* bias,
+                               const WinoGeom& g, int R0, int Tc, int act, float lo, float hi, int ncb, cudaStream_t s) {
+    if (tile == 8) {
+        if (mlp) {
+            if (pool) wino_output_kernel<8, true, true, CLIP><<<grid, kXformThreads, 0, s>>>(M, out, bias, g, R0, Tc, act, lo, hi, ncb);
+            else wino_output_kernel<8, false, true, CLIP><<<grid, kXformThreads, 0, s>>>(M, out, bias, g, R0, Tc, act, lo, hi, ncb);
+        } else {
+            if (pool) wino_output_kernel<8, true, false, CLIP><<<grid, kXformThreads, 0, s>>>(M, out, bias, g, R0, Tc, act, lo, hi, ncb);
+            else wino_output_kernel<8, false, false, CLIP><<<grid, kXformThreads, 0, s>>>(M, out, bias, g, R0, Tc, act, lo, hi, ncb);
+        }
+    } else {
+        if (pool) wino_output_kernel<4, true, false, CLIP><<<grid, kXformThreads, 0, s>>>(M, out, bias, g, R0, Tc, act, lo, hi, ncb);
+        else wino_output_kernel<4, false, false, CLIP><<<grid, kXformThreads, 0, s>>>(M, out, bias, g, R0, Tc, act, lo, hi, ncb);
+    }
+}
+
 int wino_output_transform(int tile, const float* M, float* out, const float* bias, const WinoGeom& g, int R0, int R1,
-                          int relu, int pool, cudaStream_t s) {
+                          int act, float lo, float hi, int pool, cudaStream_t s) {
     const int segs = ceil_div(g.tilesX, kSegTiles);
     const int Tc = (R1 - R0) * g.tilesX;
     dim3 grid(static_cast<unsigned>(segs) * (R1 - R0), ceil_div(g.C_out, kChBlock));
@@ -442,18 +459,8 @@ int wino_output_transform(int tile, const float* M, float* out, const float* bia
     const int prof = prof_begin(s, PROF_WINO_OUTPUT, 0, 0,
                                 4.0 * (imgs * g.C_out * out_px + static_cast<double>(tile) * tile * Tc * g.C_out));
     const bool mlp = tune_get(TUNE_WINO_MLP) != 0;
-    if (tile == 8) {
-        if (mlp) {
-            if (pool) wino_output_kernel<8, true, true><<<grid, kXformThreads, 0, s>>>(M, out, bias, g, R0, Tc, relu, ncb);
-            else wino_output_kernel<8, false, true><<<grid, kXformThreads, 0, s>>>(M, out, bias, g, R0, Tc, relu, ncb);
-        } else {
-            if (pool) wino_output_kernel<8, true, false><<<grid, kXformThreads, 0, s>>>(M, out, bias, g, R0, Tc, relu, ncb);
-            else wino_output_kernel<8, false, false><<<grid, kXformThreads, 0, s>>>(M, out, bias, g, R0, Tc, relu, ncb);
-        }
-    } else {
-        if (pool) wino_output_kernel<4, true, false><<<grid, kXformThreads, 0, s>>>(M, out, bias, g, R0, Tc, relu, ncb);
-        else wino_output_kernel<4, false, false><<<grid, kXformThreads, 0, s>>>(M, out, bias, g, R0, Tc, relu, ncb);
-    }
+    if (act == 2) wino_output_launch<true>(tile, pool, mlp, grid, M, out, bias, g, R0, Tc, act, lo, hi, ncb, s);
+    else wino_output_launch<false>(tile, pool, mlp, grid, M, out, bias, g, R0, Tc, act, lo, hi, ncb, s);
     prof_end(prof, s);
     FCUDA_CHECK_LAUNCH();
     count_launch();

@@ -16,8 +16,8 @@ struct WinoGeom {
 int wino_filter_transform(int tile, const float* w, float* U_hi, float* U_lo, int OC, int IC, cudaStream_t s);
 // Transforms tile-rows [R0, R1) (a tile-row = one row of tiles of one image; R = img * tilesY + ty).
 int wino_input_transform(int tile, const float* in, float* V, const WinoGeom& g, int R0, int R1, cudaStream_t s);
-// pool != 0: a following 2x2 / stride-2 max pooling is applied in registers; `out` is the pooled (C_out, (OH+1)/2, (OW+1)/2) blob.
+// act: 0 none, 1 ReLU, 2 Clip to [lo, hi].  pool != 0: a following 2x2 / stride-2 max pooling is applied in registers; `out` is the pooled (C_out, (OH+1)/2, (OW+1)/2) blob.
 int wino_output_transform(int tile, const float* M, float* out, const float* bias, const WinoGeom& g, int R0, int R1,
-                          int relu, int pool, cudaStream_t s);
+                          int act, float lo, float hi, int pool, cudaStream_t s);
 
 }  // namespace fcuda

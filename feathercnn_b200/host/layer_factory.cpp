@@ -1,11 +1,12 @@
 // Built-in layer registrations: the 13 ncnn type names the reference serves (/root/reference/src/layer_factory.cpp:53-68)
-// plus Deconvolution / DeconvolutionDepthWise, Interp and Crop, 17 in all, mapped onto this host's layer classes.  A table of {type name, factory} pairs instead of one macro line per layer; the
+// plus Deconvolution / DeconvolutionDepthWise, Interp, Crop, Clip and PReLU, 19 in all, mapped onto this host's layer classes.  A table of {type name, factory} pairs instead of one macro line per layer; the
 // DEFINE_LAYER_CREATOR / REGISTER_LAYER_CREATOR macros of <feather/layer_factory.h> remain the plugin API for user layers.
 #include <feather/layer_factory.h>
 
 #include <stdio.h>
 
 #include "layers/batchnorm_layer.h"
+#include "layers/clip_prelu_layers.h"
 #include "layers/conv_layer.h"
 #include "layers/deconv_layer.h"
 #include "layers/eltwise_layer.h"
@@ -51,6 +52,8 @@ const BuiltIn kBuiltIns[] = {
     {"DeconvolutionDepthWise", make_layer<DeconvLayer>},
     {"Interp", make_layer<InterpLayer>},
     {"Crop", make_layer<CropLayer>},
+    {"Clip", make_layer<ClipLayer>},
+    {"PReLU", make_layer<PReLULayer>},
 };
 
 }  // namespace

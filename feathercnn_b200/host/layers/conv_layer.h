@@ -9,6 +9,7 @@
 
 #include <vector>
 
+#include "clip_prelu_layers.h"
 #include "pooling_layer.h"
 
 namespace feather {
@@ -218,6 +219,9 @@ public:
             return fcuda_conv_forward_ext(&conv_param, conv_booster.GetAlgo(), tops[0]->data(), bottoms[0]->data(),
                                           processed_kernel, buffer, bias_data, residual ? residual->data() : NULL,
                                           relu_after_add, dilation_h, dilation_w, bottoms[0]->num(), stream());
+        if (conv_param.activation == booster::Clip)
+            return conv_booster.ForwardClip(&conv_param, tops[0]->data(), bottoms[0]->data(), processed_kernel, buffer,
+                                            bias_data, clip_min, clip_max, bottoms[0]->num(), stream());
         if (residual != NULL)
             return conv_booster.ForwardResidual(&conv_param, tops[0]->data(), bottoms[0]->data(), processed_kernel, buffer,
                                                 bias_data, residual->data(), relu_after_add, bottoms[0]->num(), stream());
@@ -233,17 +237,30 @@ public:
         return 1;
     }
 
-    int Fuse(Layer* next_layer) {  // conv_layer.h:174-185, extended to BatchNorm, Scale and a trailing 2x2 max pooling
+    // conv_layer.h:174-185, extended to BatchNorm, Scale, Clip and a trailing 2x2 max pooling
+    int Fuse(Layer* next_layer) {
         if (fused_pool) return 0;  // the pooling is always last
         if (next_layer->type.compare("Pooling") == 0) {
             PoolingLayer* pl = dynamic_cast<PoolingLayer*>(next_layer);
-            if (!pl || !pl->IsMax2x2Stride2() || residual != NULL) return 0;
+            // A clamped convolution keeps its pooling separate: the pooled epilogue entry point
+            // (fcuda_conv_forward_pool) has no clip bounds, and fcuda_conv_forward_clip does not pool.
+            if (!pl || !pl->IsMax2x2Stride2() || residual != NULL || conv_param.activation == booster::Clip) return 0;
             fused_pool = true;
             return 1;
         }
-        if (conv_param.activation == booster::ReLU) return 0;  // the activation precedes only the pooling
+        if (conv_param.activation != booster::None) return 0;  // the activation precedes only the pooling
         if (next_layer->type.compare("ReLU") == 0) {
             conv_param.activation = booster::ReLU;
+            return 1;
+        }
+        if (next_layer->type.compare("Clip") == 0) {
+            // after any BatchNorm / Scale folding, so conv -> BN -> Scale -> Clip is one kernel.  Dilated convolutions run
+            // through fcuda_conv_forward_ext, which has no clip bounds: their Clip stays a layer of its own.
+            const ClipLayer* cl = dynamic_cast<const ClipLayer*>(next_layer);
+            if (!cl || residual != NULL || dilation_h > 1 || dilation_w > 1) return 0;
+            conv_param.activation = booster::Clip;
+            clip_min = cl->min_value;
+            clip_max = cl->max_value;
             return 1;
         }
         const bool is_bn = next_layer->type.compare("BatchNorm") == 0;
@@ -291,6 +308,8 @@ protected:
     std::vector<float> fold_mul, fold_add;
     bool had_bias = false;
     Blob<float>* folded_bias = NULL;
+    // fused Clip (ConvLayer::Fuse): the epilogue's clamp bounds when conv_param.activation == booster::Clip
+    float clip_min = 0.f, clip_max = 0.f;
     // fused Eltwise SUM (Net::ApplyFusion)
     Blob<float>* residual = NULL;
     int relu_after_add = 0;

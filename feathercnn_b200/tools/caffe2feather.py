@@ -8,7 +8,9 @@ no caffe / protobuf-generated code is needed — and writes the ncnn text ``.par
 
 * layer grammar and parameter ids as ``ConvLayer::LoadParam`` & co. read them (``src/layers/*.h``; ids follow ncnn's
   caffe2ncnn): Convolution / ConvolutionDepthWise, Deconvolution / DeconvolutionDepthWise, InnerProduct, Pooling, ReLU, BatchNorm, Scale, Eltwise, Concat, Dropout,
-  Softmax, Split, Input, Crop;
+  Softmax, Split, Input, Crop, Clip, PReLU;
+* ReLU6 (the type MobileNet-v2 Caffe ports use) becomes ``Clip 0=0 1=6``, Caffe's Clip (``clip_param.min / max``) Clip with its
+  bounds, PReLU ``PReLU 0=num_slope`` with its slopes (one, ``channel_shared``, or one per channel) raw in the ``.bin``;
 * Crop (``axis`` 2 or 3, FCN's score crops) becomes ncnn's two-bottom Crop: the output height and width are the reference
   bottom's, the offsets are ``offset``'s; with axis 3 the height offset is 0, and the reference must then have the height
   of the cropped blob, as ncnn's two-bottom Crop takes both sizes from it;
@@ -261,6 +263,18 @@ def convert(caffemodel: bytes) -> tuple[str, bytes]:
         elif type_ == "ReLU":
             slope = _f32(_first(parse_message(_first(L, 123, b"")), 1), 0.0)
             out.layer("ReLU", name, bottoms, tops, f"0={slope:e}" if slope else "")
+        elif type_ == "ReLU6":
+            out.layer("Clip", name, bottoms, tops, f"0={0.0:e} 1={6.0:e}")
+        elif type_ == "Clip":
+            p = parse_message(_first(L, 148, b""))  # clip_param = 148: min = 1, max = 2 (both required)
+            if 1 not in p or 2 not in p:
+                raise ValueError(f"layer {name}: Clip without clip_param.min / max")
+            out.layer("Clip", name, bottoms, tops, f"0={_f32(_first(p, 1), 0.0):.8e} 1={_f32(_first(p, 2), 0.0):.8e}")
+        elif type_ == "PReLU":
+            # prelu_param = 131 (filler, channel_shared) only shapes the blob: (1,) when shared, (channels,) otherwise
+            slope = blobs[0].reshape(-1)
+            out.layer("PReLU", name, bottoms, tops, f"0={slope.size}")
+            out.weights(slope, False)
         elif type_ == "BatchNorm":
             p = parse_message(_first(L, 139, b""))
             eps = _f32(_first(p, 3), 1e-5)

@@ -5,7 +5,7 @@ weight blobs, raw fp32 for bias/BN/Scale blobs) — /root/reference/src/net.cpp:
 /root/reference/src/ncnn/modelbin.cpp:47-197.  Its own converter (``tools/``) is absent from the
 snapshot, and there is no network for pretrained checkpoints, so benchmarks and tests use random-init
 models of the architectures BASELINE.json names: a single 3x3 conv, VGG-16, ResNet-50 (Caffe topology:
-BN + Scale + ReLU as separate layers, Split/Eltwise residuals), MobileNet-v1, plus a small "mini" net
+BN + Scale + ReLU as separate layers, Split/Eltwise residuals), MobileNet-v1, MobileNet-v2 (ReLU6 as Clip), plus a small "mini" net
 that exercises every layer type.  Weight statistics follow SURVEY.md §8(d).
 """
 from __future__ import annotations
@@ -93,6 +93,27 @@ class ModelWriter:
     def relu(self, name, bottom, top=None):
         top = top or name
         self._layer("ReLU", name, [bottom], [top])
+        self.shape[top] = self.shape[bottom]
+        return top
+
+    def clip(self, name, bottom, lo=0.0, hi=6.0, top=None):
+        """ncnn Clip 0=min 1=max (Caffe's ReLU6 is Clip 0..6)."""
+        top = top or name
+        self._layer("Clip", name, [bottom], [top], {0: f"{lo:e}", 1: f"{hi:e}"})
+        self.shape[top] = self.shape[bottom]
+        return top
+
+    def prelu(self, name, bottom, shared=False, top=None, slopes=None):
+        """ncnn PReLU 0=num_slope: one slope per channel (or one for all when `shared`), raw fp32 in the bin."""
+        top = top or name
+        c = self.shape[bottom][0]
+        n = 1 if shared else c
+        if slopes is None:
+            slopes = self.rng.uniform(0.05, 0.3, n)
+        slopes = np.ascontiguousarray(slopes, np.float32)
+        assert slopes.shape == (n,), slopes.shape
+        self._layer("PReLU", name, [bottom], [top], {0: n})
+        self._weights(slopes, False)
         self.shape[top] = self.shape[bottom]
         return top
 
@@ -341,6 +362,65 @@ def mobilenet_v1(seed=0, num_classes=1000, size=224, wide_stats=False) -> ModelW
     return m
 
 
+def _bn_scale_clip(m: ModelWriter, tag: str, x: str, clip=True, center=1.0):
+    x = m.batchnorm("bn" + tag, x)
+    x = m.scale("scale" + tag, x, True, center=center)
+    if clip:
+        x = m.clip(tag.lstrip("_") + "_relu6", x, 0.0, 6.0)
+    return x
+
+
+def mobilenet_v2(seed=0, num_classes=1000, size=224, wide_stats=False) -> ModelWriter:
+    """MobileNet-v2 (Sandler et al. 2018): inverted residual blocks from the (t, c, n, s) table, every convolution followed
+    by BatchNorm + Scale, ReLU6 as ncnn's Clip 0..6 after the stem, expansion and depthwise convolutions, linear
+    projections, and an Eltwise SUM shortcut (through a Split) where the stride is 1 and the channel count is kept."""
+    m = ModelWriter(seed, wide_stats)
+    x = m.input("data", 3, size, size)
+    x = m.conv("conv1", x, 32, 3, 2, 1, False)
+    x = _bn_scale_clip(m, "_conv1", x)
+    table = [(1, 16, 1, 1), (6, 24, 2, 2), (6, 32, 3, 2), (6, 64, 4, 2), (6, 96, 3, 1), (6, 160, 3, 2), (6, 320, 1, 1)]
+    for bi, (t, c, n, s) in enumerate(table, 2):
+        for i in range(n):
+            tag = f"{bi}_{i + 1}"
+            stride = s if i == 0 else 1
+            ic = m.shape[x][0]
+            shortcut = stride == 1 and ic == c
+            if shortcut:
+                sc, x = m.split(f"block{tag}_split", x, [f"block{tag}_in_a", f"block{tag}_in_b"])
+            y = x
+            if t != 1:
+                y = m.conv(f"conv{tag}_expand", y, ic * t, 1, 1, 0, False)
+                y = _bn_scale_clip(m, f"_conv{tag}_expand", y)
+            y = m.conv(f"conv{tag}_dw", y, ic * t, 3, stride, 1, False, group=ic * t)
+            y = _bn_scale_clip(m, f"_conv{tag}_dw", y)
+            y = m.conv(f"conv{tag}_linear", y, c, 1, 1, 0, False)
+            y = _bn_scale_clip(m, f"_conv{tag}_linear", y, clip=False, center=0.3 if shortcut else 1.0)
+            x = m.eltwise(f"block{tag}", [sc, y]) if shortcut else y
+    x = m.conv("conv_last", x, 1280, 1, 1, 0, False)
+    x = _bn_scale_clip(m, "_conv_last", x)
+    x = m.pool("pool_last", x, 1, 7, 1, 0, global_pooling=True)
+    x = m.conv("fc", x, num_classes, 1, 1, 0, True)
+    m.softmax("prob", x)
+    return m
+
+
+def prelu_tiny(seed=0, size=15, classes=10, wide_stats=False) -> ModelWriter:
+    """Convolutions followed by BatchNorm + Scale + PReLU, as in face-detection nets (MTCNN, MobileFaceNet): per-channel
+    slopes on a 15 x 15 plane (not a multiple of 4: the scalar kernel), one shared slope on the 8 x 8 plane after it."""
+    m = ModelWriter(seed, wide_stats)
+    x = m.input("data", 3, size, size)
+    x = m.conv("conv1", x, 16, 3, 1, 1, True)
+    x = m.batchnorm("bn1", x); x = m.scale("scale1", x, True)
+    x = m.prelu("prelu1", x)
+    x = m.conv("conv2", x, 32, 3, 2, 1, True)
+    x = m.batchnorm("bn2", x); x = m.scale("scale2", x, True)
+    x = m.prelu("prelu2", x, shared=True)
+    x = m.pool("pool2", x, 1, 2, 2, 0, global_pooling=True)
+    x = m.conv("fc", x, classes, 1, 1, 0, True)
+    m.softmax("prob", x)
+    return m
+
+
 def mini(seed=0, size=32, ch=16, wide_stats=False) -> ModelWriter:
     """Small net touching every layer type (SURVEY.md §8c's 12-layer probe net, plus concat/dropout/depthwise)."""
     m = ModelWriter(seed, wide_stats)
@@ -448,7 +528,8 @@ def deeplab_head_tiny(seed=0, size=32, classes=5) -> ModelWriter:
 
 
 ZOO = {"single_conv": single_conv, "vgg16": vgg16, "resnet50": resnet50, "mobilenet_v1": mobilenet_v1, "mini": mini,
-       "decoder_tiny": decoder_tiny, "fcn8s_tiny": fcn8s_tiny, "deeplab_head_tiny": deeplab_head_tiny}
+       "decoder_tiny": decoder_tiny, "fcn8s_tiny": fcn8s_tiny, "deeplab_head_tiny": deeplab_head_tiny,
+       "mobilenet_v2": mobilenet_v2, "prelu_tiny": prelu_tiny}
 
 
 def synthetic_input(shape, index: int = 0) -> np.ndarray:

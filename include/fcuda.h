@@ -33,8 +33,10 @@ enum FcudaConvAlgo {
     FCUDA_WINOGRADF23 = 6       /* F(2,3): 16-way TensorGEMM; stub in both reference dispatchers, real here */
 };
 
-/* booster::ActivationType, booster.h:53-57 */
-enum FcudaActivation { FCUDA_ACT_NONE = 0, FCUDA_ACT_RELU = 1 };
+/* booster::ActivationType, booster.h:53-57, plus FCUDA_ACT_CLIP (ncnn's Clip / Caffe's ReLU6, an extension): a clamp to
+ * [clip_min, clip_max] whose bounds only fcuda_conv_forward_clip carries — every other convolution entry point returns -200
+ * for it. */
+enum FcudaActivation { FCUDA_ACT_NONE = 0, FCUDA_ACT_RELU = 1, FCUDA_ACT_CLIP = 2 };
 
 /* Field-compatible with booster::ConvParam (booster.h:59-77): 15 ints, bool, enum. */
 typedef struct FcudaConvParam {
@@ -102,6 +104,16 @@ int fcuda_conv_init(const FcudaConvParam* param, int algo, float* packed_kernel,
 int fcuda_conv_forward(const FcudaConvParam* param, int algo, float* output, const float* input,
                        const float* packed_kernel, float* scratch, const float* bias, int batch, void* stream);
 
+/* fcuda_conv_forward with param->activation == FCUDA_ACT_CLIP (-200 otherwise, and for clip_min > clip_max or a NaN
+ * bound): output = min(max(conv(input) [+bias], clip_min), clip_max), the clamp applied in the epilogue of the same
+ * kernels every algorithm runs (Caffe's ReLU6 is clip_min = 0, clip_max = 6).  The bits before the clamp are those of
+ * fcuda_conv_forward with FCUDA_ACT_NONE.  NaN maps to clip_min (fmaxf returns the non-NaN operand); ncnn's
+ * compare-and-assign Clip passes NaN through.  Runs the Clip instantiations of the kernels; the ReLU and plain launches
+ * of the other entry points are unchanged. */
+int fcuda_conv_forward_clip(const FcudaConvParam* param, int algo, float* output, const float* input,
+                            const float* packed_kernel, float* scratch, const float* bias, float clip_min, float clip_max,
+                            int batch, void* stream);
+
 /* The 64-way batched "TensorGEMM" itself (avx/winograd_kernels_F63.cpp:518-757), exposed for tests and
  * profiling:  for g < G:  D[g][m][n] = sum_k A[g][m][k] * B[g][n][k]   (row-major, K-major operands).
  * `a` is plain fp32 (split into TF32 hi + fp32 lo inside the kernel, in registers); b_hi/b_lo are the planes of
@@ -143,6 +155,15 @@ int fcuda_eltwise_forward(float* output, const float* a, const float* b, size_t 
                           int relu, void* stream);
 /* ReluLayer::Forward (src/layers/relu_layer.h:29-41). */
 int fcuda_relu_forward(float* output, const float* input, size_t n, void* stream);
+/* ncnn's Clip (the reference has no such layer; Caffe's ReLU6 is min 0, max 6): y = min(max(x, min), max) over n
+ * floats.  NaN maps to min (ncnn's compare-and-assign passes it through).  -200 for min > max or a NaN bound.  In-place
+ * (output == input) is allowed. */
+int fcuda_clip_forward(float* output, const float* input, size_t n, float min, float max, void* stream);
+/* ncnn's PReLU (the reference has none): y = x < 0 ? x * slope[c] : x over (batch, channels, plane) with num_slope ==
+ * channels slopes, or one slope shared by every channel (num_slope == 1); -200 for any other num_slope.  NaN passes
+ * through.  `slope` is a device pointer.  In-place (output == input) is allowed. */
+int fcuda_prelu_forward(float* output, const float* input, int channels, size_t plane, const float* slope, int num_slope,
+                        int batch, void* stream);
 /* SoftmaxLayer::Forward (src/layers/softmax_layer.h:32-55): over each image's whole blob. */
 int fcuda_softmax_forward(float* output, const float* input, size_t n_per_image, int batch, void* stream);
 /* DropoutLayer::Forward (src/layers/dropout_layer.h:36-57): y = x*scale (copy when scale == 1). */
@@ -309,7 +330,7 @@ void fcuda_profile_tensor_gemm(int enable);
 int fcuda_profile_collect(double* total_ms, double* algo_flops, double* mma_flops, long long* launches);
 /* Same, per kernel class, for every instrumented launch (the enable switch above covers all of them):
  * kind 0 TensorGEMM, 1 implicit-GEMM conv, 2 Winograd input transform, 3 Winograd output transform, 4 pooling,
- * 5 depthwise, 6 element-wise (BN/Scale/Eltwise), 7 deconvolution scatter / depthwise gather, 8 resize / crop (Interp,
+ * 5 depthwise, 6 element-wise (BN/Scale/Eltwise/Clip/PReLU), 7 deconvolution scatter / depthwise gather, 8 resize / crop (Interp,
  * Crop), < 0 all.  algo_bytes = the bytes the operation must move (inputs
  * read once + outputs written once). */
 int fcuda_profile_collect_kind(int kind, double* total_ms, double* algo_flops, double* mma_flops, double* algo_bytes,

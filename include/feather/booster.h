@@ -12,7 +12,7 @@ namespace booster {
 inline namespace b200 {  // ABI tag: keeps these symbols apart from the reference build when both are loaded
 
 enum ConvAlgo { NAIVE, IM2COL, SGECONV, DEPTHWISE, WINOGRADF63, WINOGRADF63FUSED, WINOGRADF23 };
-enum ActivationType { None, ReLU };
+enum ActivationType { None, ReLU, Clip };  // Clip == FCUDA_ACT_CLIP: bounds passed to ForwardClip
 
 struct ConvParam : FcudaConvParam {
     ConvParam() { *static_cast<FcudaConvParam*>(this) = FcudaConvParam(); }
@@ -60,6 +60,12 @@ public:
                         void* stream = nullptr) const {
         return fcuda_conv_forward_residual(param, algo, output, input, kernel, buffer, bias_arr, residual, relu_after_add,
                                            batch, stream);
+    }
+    // Forward with param->activation == Clip: the output clamped to [clip_min, clip_max] in the epilogue
+    int ForwardClip(ConvParam* param, float* output, const float* input, const float* kernel, float* buffer,
+                    const float* bias_arr, float clip_min, float clip_max, int batch = 1, void* stream = nullptr) const {
+        return fcuda_conv_forward_clip(param, algo, output, input, kernel, buffer, bias_arr, clip_min, clip_max, batch,
+                                       stream);
     }
     int GetAlgo() const { return algo; }
 
