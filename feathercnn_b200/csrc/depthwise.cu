@@ -399,12 +399,15 @@ static void dw_launch(const float* in, const float* w, const float* bias, float*
                     (g.stride_h == 1 || g.stride_h == 2) && g.OW >= 24;
     // vector width: the widest VEC whose strips (32 * VEC outputs) still fill most lanes and keep accesses aligned
     const bool vec_off = tune_get(TUNE_DW_VEC) == 0;
+    const uintptr_t ia = reinterpret_cast<uintptr_t>(in), oa = reinterpret_cast<uintptr_t>(out);
     int vec = 1;
     if (k3 && !vec_off && g.stride_h == 1 && g.OW == g.W) {
-        if (g.W % 4 == 0 && g.OW >= 96) vec = 4;
-        else if (g.W % 2 == 0 && g.OW >= 48) vec = 2;
+        // float4 / float2 loads and stores: in and out aligned to the access width (a C ABI caller may pass any float*)
+        if (g.W % 4 == 0 && g.OW >= 96 && ((ia | oa) & 15) == 0) vec = 4;
+        else if (g.W % 2 == 0 && g.OW >= 48 && ((ia | oa) & 7) == 0) vec = 2;
     } else if (k3 && !vec_off && g.stride_h == 2 && g.W == 2 * g.OW) {
-        if (g.W % 4 == 0 && g.OW >= 48) vec = 2;
+        // float4 loads, float2 stores: in 16-byte, out 8-byte aligned
+        if (g.W % 4 == 0 && g.OW >= 48 && (ia & 15) == 0 && (oa & 7) == 0) vec = 2;
     }
     if (k3 && vec > 1) {
         const int xstrips = ceil_div(g.OW, 32 * vec), ystrips = ceil_div(g.OH, kDwRows);

@@ -330,19 +330,22 @@ fc_reduce_kernel(float* __restrict__ out, const float* __restrict__ part, const 
 int pooling_forward(const float* in, float* out, const PoolGeom& g, int channels, int batch, cudaStream_t s) {
     const size_t planes = static_cast<size_t>(batch) * channels;
     const int prof = prof_begin(s, PROF_POOL, 0, 0, 4.0 * planes * (static_cast<double>(g.H) * g.W + static_cast<double>(g.OH) * g.OW));
+    const uintptr_t ia = reinterpret_cast<uintptr_t>(in), oa = reinterpret_cast<uintptr_t>(out);
     if (g.OH == 1 && g.OW == 1 && g.KH >= g.H && g.KW >= g.W && g.pad_top + g.pad_bottom == 0 &&
         g.pad_left + g.pad_right == 0) {
         global_pool_kernel<<<static_cast<unsigned>(ceil_div_sz(planes * 32, 256)), 256, 0, s>>>(in, out, g.H * g.W,
                                                                                               g.type, planes);
     } else if (g.KH == 2 && g.KW == 2 && g.stride_h == 2 && g.stride_w == 2 && g.pad_top + g.pad_bottom == 0 &&
                g.pad_left + g.pad_right == 0 && g.W % 4 == 0 && g.H % 2 == 0 && g.OW == g.W / 2 && g.OH == g.H / 2 &&
-               planes * g.OH * (g.OW / 2) < (1ull << 31)) {
+               planes * g.OH * (g.OW / 2) < (1ull << 31) &&
+               (ia & 15) == 0 && (oa & 7) == 0) {  // float4 loads, float2 stores: a C ABI caller may pass any float*
         const int pairs = g.OW / 2;
         const unsigned total = static_cast<unsigned>(planes * g.OH * pairs);
         const unsigned long long m = pairs > 1 ? ~0ull / static_cast<unsigned long long>(pairs) + 1ull : 0ull;
         pool2x2_kernel<<<(total + 255) / 256, 256, 0, s>>>(in, out, g.W, g.OW, pairs, m, g.type, total);
     } else if (g.KH == 3 && g.KW == 3 && g.stride_h == 2 && g.stride_w == 2 && g.pad_top + g.pad_bottom == 0 &&
-               g.pad_left + g.pad_right == 0 && g.W % 2 == 0 && g.OW >= 24 && 2 * (g.OW - 1) < g.W && 2 * (g.OH - 1) < g.H) {
+               g.pad_left + g.pad_right == 0 && g.W % 2 == 0 && g.OW >= 24 && 2 * (g.OW - 1) < g.W && 2 * (g.OH - 1) < g.H &&
+               (ia & 7) == 0) {  // float2 loads: the input 8-byte aligned
         const int xstrips = (g.OW + 31) / 32, ystrips = (g.OH + 15) / 16;
         const long long items = static_cast<long long>(planes) * xstrips * ystrips;
         pool3x3s2_kernel<<<static_cast<unsigned>((items + 3) / 4), 128, 0, s>>>(in, out, g.H, g.W, g.OH, g.OW, g.type, items,

@@ -148,6 +148,7 @@ class Conv:
     batch: int = 2
     algo: int | None = None      # None: the tuned policy (what feather::Net uses)
     chunk: int | None = None     # L2 chunk bytes for the Winograd / im2col intermediates
+    clip: tuple[float, float] | None = None   # (lo, hi): the Clip epilogue of fcuda_conv_forward_clip, after any ReLU
 
     def __post_init__(self):
         self.kw = self.kh if self.kw is None else self.kw
@@ -200,6 +201,8 @@ def conv_ref(c: Conv, x, w, b, r, absolute=False):
     y = F.conv2d(F.pad(x, (pl, pr, pt, pb)), w, b, stride=(c.sh, c.sw), dilation=c.dil, groups=c.group)
     if not absolute and c.relu:
         y = y.clamp_min(0)
+    if not absolute and c.clip is not None:
+        y = y.clamp(*c.clip)
     if r is not None:
         y = y + (r.to(torch.float64).abs() if absolute else r.to(torch.float64))
         if not absolute and c.relu_after_add:
@@ -263,6 +266,8 @@ def wino_model(c: Conv, x, w, b, tile: int, mode: int | None):
 def wino_finish(c: Conv, y, r):
     if c.relu:
         y = y.clamp_min(0)
+    if c.clip is not None:
+        y = y.clamp(*c.clip)
     if r is not None:
         y = y + r.to(torch.float64)
         if c.relu_after_add:
@@ -283,6 +288,8 @@ def run_conv(c: Conv, mode: int, expect_algo: int | None = None, tuned: bool = F
     pl, pb, pr, pt = c.pad
     p = booster.ConvParam.make(c.oc, c.ic, c.h, c.w, c.kh, c.kw, stride=c.sh, stride_w=c.sw, pad_lbrt=c.pad,
                                group=c.group, bias=c.bias, relu=c.relu)
+    if c.clip is not None:
+        p.activation = booster.ACT_CLIP
     oh, ow = c.out_hw
     p.output_h, p.output_w = oh, ow  # (what AssignOutputDim gives without dilation)
     default_chunk = booster.fcuda().fcuda_get_l2_chunk_bytes() if c.chunk else None
@@ -290,7 +297,7 @@ def run_conv(c: Conv, mode: int, expect_algo: int | None = None, tuned: bool = F
         booster.set_l2_chunk_bytes(c.chunk)
     try:
         got, algo = booster.conv_forward(p, x, w, b, algo=c.algo, residual=r, relu_after_add=c.relu_after_add,
-                                         dilation=c.dil, tuned=tuned, pool=c.pool)
+                                         dilation=c.dil, tuned=tuned, pool=c.pool, clip=c.clip)
         torch.cuda.synchronize()
     finally:
         if c.chunk:
@@ -313,13 +320,15 @@ def run_conv(c: Conv, mode: int, expect_algo: int | None = None, tuned: bool = F
         sl = slice(i0, i0 + step)
         ref = conv_ref(c, x[sl], w, b, r[sl] if r is not None else None)
         s = conv_ref(c, x[sl], w, b, r[sl] if r is not None else None, absolute=True)
-        bound = coef * s + U * ref.abs()
+        # a clamp is 1-Lipschitz: the bound of the unclamped result holds for the clamped one
+        free = ref if c.clip is None else conv_ref(dataclasses.replace(c, clip=None), x[sl], w, b, r[sl] if r is not None else None)
+        bound = coef * s + U * free.abs()
         if c.pool:
             ref, s, bound = pool2(ref), pool2(s), pool2(bound)
         used, _ = excess(got[sl], ref, bound, 1.0, 0.0)
         _, rel = excess(got[sl], ref, s, 1.0, 0.0)
         worst_used, worst_rel = max(worst_used, used), max(worst_rel, rel)
-        del ref, s, bound
+        del ref, s, bound, free
     _record(path, mode, worst_rel, worst_used)
     return worst_used, worst_rel, algo
 
