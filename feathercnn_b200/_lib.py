@@ -62,6 +62,16 @@ class FcudaInterpParam(ctypes.Structure):
                 [(n, ctypes.c_int) for n in "output_height output_width input_h input_w output_h output_w".split()])
 
 
+class FcudaPriorBoxParam(ctypes.Structure):
+    """include/fcuda.h FcudaPriorBoxParam (fixed arrays of FCUDA_PRIORBOX_MAX = 16)."""
+
+    _fields_ = ([("num_min_sizes", ctypes.c_int), ("num_max_sizes", ctypes.c_int), ("num_aspect_ratios", ctypes.c_int),
+                 ("min_sizes", ctypes.c_float * 16), ("max_sizes", ctypes.c_float * 16),
+                 ("aspect_ratios", ctypes.c_float * 16), ("variances", ctypes.c_float * 4), ("flip", ctypes.c_int),
+                 ("clip", ctypes.c_int), ("step_w", ctypes.c_float), ("step_h", ctypes.c_float),
+                 ("offset", ctypes.c_float)])
+
+
 def fcuda() -> ctypes.CDLL:
     global _fcuda
     if _fcuda is None:
@@ -71,7 +81,16 @@ def fcuda() -> ctypes.CDLL:
         szp = ctypes.POINTER(ctypes.c_size_t)
         D = ctypes.POINTER(FcudaDeconvParam)
         R = ctypes.POINTER(FcudaInterpParam)
+        PB = ctypes.POINTER(FcudaPriorBoxParam)
+        f = ctypes.c_float
         sigs = {
+            "fcuda_permute_forward": (i, [vp, vp, i, i, i, i, i, vp]),
+            "fcuda_softmax_axis_forward": (i, [vp, vp, i, i, i, i, vp]),
+            "fcuda_priorbox_per_location": (i, [PB, ctypes.POINTER(i)]),
+            "fcuda_priorbox_forward": (i, [vp, PB, i, i, i, i, vp]),
+            "fcuda_ssd_decode": (i, [vp, vp, vp, i, i, vp]),
+            "fcuda_detection_output_workspace_size": (i, [i, i, i, i, szp]),
+            "fcuda_detection_output_forward": (i, [vp, vp, vp, vp, i, i, f, f, i, i, vp, i, vp]),
             "fcuda_interp_output_dim": (i, [R]),
             "fcuda_interp_forward": (i, [R, vp, vp, i, i, vp]),
             "fcuda_crop_forward": (i, [vp, vp] + [i] * 10 + [vp]),
@@ -163,6 +182,7 @@ def feather() -> ctypes.CDLL:
             "fnet_wait_batch": (i, [vp, i]),
             "fnet_synchronize": (i, [vp]),
             "fnet_blob_shape": (i, [vp, cp, ip, ip, ip, ip]),
+            "fnet_blob_dims": (i, [vp, cp]),
             "fnet_extract_blob": (i, [vp, cp, vp]),
             "fnet_extract_device": (i, [vp, cp, ctypes.POINTER(vp), ip, ip, ip, ip]),
             "fnet_launches_per_forward": (ctypes.c_ulonglong, [vp]),

@@ -14,6 +14,7 @@ import torch
 from ._lib import FcudaConvParam, fcuda
 from ._lib import FcudaDeconvParam as DeconvParam
 from ._lib import FcudaInterpParam as InterpParam
+from ._lib import FcudaPriorBoxParam as PriorBoxParam
 
 NAIVE, IM2COL, SGECONV, DEPTHWISE, WINOGRADF63, WINOGRADF63FUSED, WINOGRADF23 = range(7)
 ALGO_NAMES = ["NAIVE", "IM2COL", "SGECONV", "DEPTHWISE", "WINOGRADF63", "WINOGRADF63FUSED", "WINOGRADF23"]
@@ -259,6 +260,85 @@ def crop(x: torch.Tensor, coff: int, hoff: int, woff: int, oc: int, oh: int, ow:
     out = torch.empty((n, oc, oh, ow), device=x.device, dtype=torch.float32)
     _check("fcuda_crop_forward",
            fcuda().fcuda_crop_forward(_ptr(out), _ptr(x.contiguous()), c, h, w, coff, hoff, woff, oc, oh, ow, n, _stream()))
+    return out
+
+
+# ---- SSD detection head ----------------------------------------------------------------------------
+def permute(x: torch.Tensor, order: int) -> torch.Tensor:
+    """ncnn Permute of x (N, C, H, W): order 0 (c,h,w) 1 (c,w,h) 2 (h,c,w) 3 (h,w,c) 4 (w,c,h) 5 (w,h,c)."""
+    n, c, h, w = x.shape
+    axes = [(0, 1, 2), (0, 2, 1), (1, 0, 2), (1, 2, 0), (2, 0, 1), (2, 1, 0)][order] if 0 <= order <= 5 else (0, 1, 2)
+    d = (c, h, w)
+    out = torch.empty((n,) + tuple(d[a] for a in axes), device=x.device, dtype=torch.float32)
+    _check("fcuda_permute_forward",
+           fcuda().fcuda_permute_forward(_ptr(out), _ptr(x.contiguous()), c, h, w, order, n, _stream()))
+    return out
+
+
+def softmax_axis(x: torch.Tensor, outer: int, length: int, inner: int) -> torch.Tensor:
+    """Softmax over the middle axis of each image of x viewed as (N, outer, length, inner)."""
+    out = torch.empty_like(x)
+    _check("fcuda_softmax_axis_forward",
+           fcuda().fcuda_softmax_axis_forward(_ptr(out), _ptr(x.contiguous()), outer, length, inner, x.shape[0], _stream()))
+    return out
+
+
+def priorbox_param(min_sizes, max_sizes=(), aspect_ratios=(), variances=(0.1, 0.1, 0.2, 0.2), flip=True, clip=False,
+                   step=(0.0, 0.0), offset=0.5) -> PriorBoxParam:
+    """FcudaPriorBoxParam; step (w, h) <= 0 derives the step from the image and feature sizes."""
+    p = PriorBoxParam()
+    p.num_min_sizes, p.num_max_sizes, p.num_aspect_ratios = len(min_sizes), len(max_sizes), len(aspect_ratios)
+    for dst, src in ((p.min_sizes, min_sizes), (p.max_sizes, max_sizes), (p.aspect_ratios, aspect_ratios),
+                     (p.variances, variances)):
+        for k, v in enumerate(list(src)[:len(dst)]):
+            dst[k] = float(v)
+    p.flip, p.clip = int(bool(flip)), int(bool(clip))
+    p.step_w, p.step_h = float(step[0]), float(step[1])
+    p.offset = float(offset)
+    return p
+
+
+def priorbox_per_location(p: PriorBoxParam) -> int:
+    n = ctypes.c_int(0)
+    _check("fcuda_priorbox_per_location", fcuda().fcuda_priorbox_per_location(ctypes.byref(p), ctypes.byref(n)))
+    return n.value
+
+
+def priorbox(p: PriorBoxParam, feat_w: int, feat_h: int, img_w: int, img_h: int, device="cuda") -> torch.Tensor:
+    """(2, 4 * P) priors: row 0 the boxes, row 1 the variances."""
+    num = feat_w * feat_h * priorbox_per_location(p)
+    out = torch.empty((2, 4 * num), device=device, dtype=torch.float32)
+    _check("fcuda_priorbox_forward",
+           fcuda().fcuda_priorbox_forward(_ptr(out), ctypes.byref(p), feat_w, feat_h, img_w, img_h, _stream()))
+    return out
+
+
+def ssd_decode(loc: torch.Tensor, priors: torch.Tensor) -> torch.Tensor:
+    """loc (N, 4P), priors (2, 4P) -> boxes (N, P, 4) as (xmin, ymin, xmax, ymax)."""
+    n = loc.shape[0]
+    num = priors.shape[-1] // 4
+    out = torch.empty((n, num, 4), device=loc.device, dtype=torch.float32)
+    _check("fcuda_ssd_decode", fcuda().fcuda_ssd_decode(_ptr(out), _ptr(loc.contiguous()), _ptr(priors.contiguous()), num, n,
+                                                        _stream()))
+    return out
+
+
+def detection_output(loc: torch.Tensor, conf: torch.Tensor, priors: torch.Tensor, num_classes: int,
+                     conf_threshold: float = 0.5, nms_threshold: float = 0.05, nms_top_k: int = 300,
+                     keep_top_k: int = 100) -> torch.Tensor:
+    """loc (N, 4P), conf (N, P * C), priors (2, 4P) -> (N, keep_top_k, 6) rows [label, score, xmin, ymin, xmax, ymax]."""
+    lib = fcuda()
+    n = loc.shape[0]
+    num = priors.shape[-1] // 4
+    ws = ctypes.c_size_t(0)
+    _check("fcuda_detection_output_workspace_size",
+           lib.fcuda_detection_output_workspace_size(num, num_classes, nms_top_k, n, ctypes.byref(ws)))
+    workspace = torch.empty(max(ws.value, 1), device=loc.device, dtype=torch.float32)
+    out = torch.empty((n, keep_top_k, 6), device=loc.device, dtype=torch.float32)
+    _check("fcuda_detection_output_forward",
+           lib.fcuda_detection_output_forward(_ptr(out), _ptr(loc.contiguous()), _ptr(conf.contiguous()),
+                                              _ptr(priors.contiguous()), num, num_classes, float(conf_threshold),
+                                              float(nms_threshold), nms_top_k, keep_top_k, _ptr(workspace), n, _stream()))
     return out
 
 

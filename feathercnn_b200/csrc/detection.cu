@@ -1,0 +1,508 @@
+// SSD detection head: ncnn's Permute, a softmax over one axis, Caffe / ncnn PriorBox, and DetectionOutput (centre-size
+// decode, per-class top-k and greedy NMS, merge over the classes) as stream-ordered kernels that allocate nothing, so a
+// detection net stays on the device and inside one CUDA graph from pixels to boxes.
+//
+// DetectionOutput runs three kernels:
+//   decode     one thread per (image, prior): the boxes into the workspace;
+//   nms_class  one CTA per (image, class): radix-select the nms_top_k best candidates (score, then prior index), sort
+//              them bitonically in shared memory, then sweep them in order; each box still standing suppresses the later
+//              ones in parallel.  The kept keys go to the workspace in sorted order;
+//   merge      one CTA per image: the same select and sort over the kept lists of all classes, then the output rows.
+// Keys are 64 bits: an order-preserving image of the fp32 score above 32 bits of (0xffffffff - index), so one descending
+// sort gives score descending and index ascending.
+#include "common.cuh"
+#include "detection.cuh"
+
+#include <math.h>
+#include <stdint.h>
+
+namespace fcuda {
+
+namespace {
+
+constexpr int kDetThreads = 512;
+constexpr int kDetWarps = kDetThreads / 32;
+constexpr int kMaxTopK = 1024;  // nms_top_k and keep_top_k limit: the candidates of one CTA live in shared memory
+
+// ---- Permute --------------------------------------------------------------------------------------------------------
+// Input axis (0 = c, 1 = h, 2 = w) of each output axis, per ncnn order_type.
+__constant__ int kPermAxes[6][3] = {{0, 1, 2}, {0, 2, 1}, {1, 0, 2}, {1, 2, 0}, {2, 0, 1}, {2, 1, 0}};
+
+__global__ void __launch_bounds__(256)
+permute_kernel(const float* __restrict__ in, float* __restrict__ out, int c, int h, int w, int order, long long total) {
+    const int dims[3] = {c, h, w};
+    const long long strides[3] = {static_cast<long long>(h) * w, w, 1};
+    const int a0 = kPermAxes[order][0], a1 = kPermAxes[order][1], a2 = kPermAxes[order][2];
+    const int d1 = dims[a1], d2 = dims[a2];
+    const long long s0 = strides[a0], s1 = strides[a1], s2 = strides[a2];
+    const long long image = static_cast<long long>(c) * h * w;
+    for (long long idx = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x; idx < total;
+         idx += static_cast<long long>(gridDim.x) * blockDim.x) {
+        const long long n = idx / image;
+        long long r = idx - n * image;
+        const long long o2 = r % d2;
+        r /= d2;
+        const long long o1 = r % d1, o0 = r / d1;
+        out[idx] = __ldg(in + n * image + o0 * s0 + o1 * s1 + o2 * s2);
+    }
+}
+
+// Order 3, (c, h, w) -> (h, w, c): a transpose of the (c, h*w) matrix of each image through a 32 x 33 shared tile, so
+// both the reads (along h*w) and the writes (along c) are coalesced.
+constexpr int kTile = 32;
+__global__ void __launch_bounds__(kTile * 8)
+transpose_kernel(const float* __restrict__ in, float* __restrict__ out, int rows, int cols) {
+    __shared__ float tile[kTile][kTile + 1];
+    const size_t image = static_cast<size_t>(rows) * cols;
+    const float* ip = in + image * blockIdx.z;
+    float* op = out + image * blockIdx.z;
+    const int c0 = blockIdx.x * kTile, r0 = blockIdx.y * kTile;
+    for (int y = threadIdx.y; y < kTile; y += 8) {
+        const int r = r0 + y, cc = c0 + threadIdx.x;
+        if (r < rows && cc < cols) tile[y][threadIdx.x] = __ldg(ip + static_cast<size_t>(r) * cols + cc);
+    }
+    __syncthreads();
+    for (int y = threadIdx.y; y < kTile; y += 8) {
+        const int cc = c0 + y, r = r0 + threadIdx.x;
+        if (r < rows && cc < cols) op[static_cast<size_t>(cc) * rows + r] = tile[threadIdx.x][y];
+    }
+}
+
+// ---- softmax over one axis ------------------------------------------------------------------------------------------
+// inner == 1: one warp per row of `len` contiguous values.
+__global__ void __launch_bounds__(256)
+softmax_rows_kernel(const float* __restrict__ in, float* __restrict__ out, long long rows, int len) {
+    const long long row = static_cast<long long>(blockIdx.x) * 8 + (threadIdx.x >> 5);
+    if (row >= rows) return;
+    const int lane = threadIdx.x & 31;
+    const float* ip = in + row * len;
+    float* op = out + row * len;
+    float m = -INFINITY;
+    for (int j = lane; j < len; j += 32) m = fmaxf(m, ip[j]);
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
+    float s = 0.f;
+    for (int j = lane; j < len; j += 32) {
+        const float e = expf(ip[j] - m);
+        op[j] = e;
+        s += e;
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+    for (int j = lane; j < len; j += 32) op[j] = op[j] / s;
+}
+
+// inner > 1: one thread per (image, outer, inner) column of `len` values `inner` apart; neighbouring threads read
+// neighbouring columns.
+__global__ void __launch_bounds__(256)
+softmax_cols_kernel(const float* __restrict__ in, float* __restrict__ out, long long cols, int len, int inner) {
+    const long long col = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
+    if (col >= cols) return;
+    const long long o = col / inner, i = col - o * inner;
+    const size_t base = static_cast<size_t>(o) * len * inner + i;
+    float m = -INFINITY;
+    for (int j = 0; j < len; ++j) m = fmaxf(m, in[base + static_cast<size_t>(j) * inner]);
+    float s = 0.f;
+    for (int j = 0; j < len; ++j) {
+        const float e = expf(in[base + static_cast<size_t>(j) * inner] - m);
+        out[base + static_cast<size_t>(j) * inner] = e;
+        s += e;
+    }
+    for (int j = 0; j < len; ++j) out[base + static_cast<size_t>(j) * inner] /= s;
+}
+
+// ---- PriorBox -------------------------------------------------------------------------------------------------------
+__device__ __forceinline__ void put_box(float* o, float cx, float cy, float bw, float bh, float iw, float ih, int clip) {
+    float v[4] = {__fdiv_rn(__fsub_rn(cx, __fmul_rn(bw, 0.5f)), iw), __fdiv_rn(__fsub_rn(cy, __fmul_rn(bh, 0.5f)), ih),
+                  __fdiv_rn(__fadd_rn(cx, __fmul_rn(bw, 0.5f)), iw), __fdiv_rn(__fadd_rn(cy, __fmul_rn(bh, 0.5f)), ih)};
+#pragma unroll
+    for (int k = 0; k < 4; ++k) o[k] = clip ? fminf(fmaxf(v[k], 0.f), 1.f) : v[k];
+}
+
+// one thread per feature-map location; out row 0 = boxes, row 1 (at 4 * total) = variances
+__global__ void __launch_bounds__(256)
+priorbox_kernel(float* __restrict__ out, const FcudaPriorBoxParam p, int per_loc, int fw, int fh, float iw, float ih,
+                float step_w, float step_h) {
+    const int loc = blockIdx.x * blockDim.x + threadIdx.x;
+    if (loc >= fw * fh) return;
+    const int y = loc / fw, x = loc - y * fw;
+    const float cx = __fmul_rn(__fadd_rn(static_cast<float>(x), p.offset), step_w);
+    const float cy = __fmul_rn(__fadd_rn(static_cast<float>(y), p.offset), step_h);
+    const size_t total4 = static_cast<size_t>(fw) * fh * per_loc * 4;
+    float* o = out + static_cast<size_t>(loc) * per_loc * 4;
+    for (int k = 0; k < p.num_min_sizes; ++k) {
+        const float mn = p.min_sizes[k];
+        put_box(o, cx, cy, mn, mn, iw, ih, p.clip);
+        o += 4;
+        if (p.num_max_sizes > 0) {
+            const float sz = sqrtf(__fmul_rn(mn, p.max_sizes[k]));
+            put_box(o, cx, cy, sz, sz, iw, ih, p.clip);
+            o += 4;
+        }
+        for (int a = 0; a < p.num_aspect_ratios; ++a) {
+            const float ar = p.aspect_ratios[a];
+            if (fabsf(ar - 1.f) < 1e-6f) continue;
+            const float r = sqrtf(ar);
+            put_box(o, cx, cy, __fmul_rn(mn, r), __fdiv_rn(mn, r), iw, ih, p.clip);
+            o += 4;
+            if (p.flip) {
+                put_box(o, cx, cy, __fdiv_rn(mn, r), __fmul_rn(mn, r), iw, ih, p.clip);
+                o += 4;
+            }
+        }
+    }
+    float* v = out + total4 + static_cast<size_t>(loc) * per_loc * 4;
+    for (int j = 0; j < per_loc * 4; ++j) v[j] = p.variances[j & 3];
+}
+
+// ---- DetectionOutput ------------------------------------------------------------------------------------------------
+// cx = var0 * l0 * pw + pcx, w = expf(var2 * l2) * pw, ...; every product and sum rounded on its own (no FMA)
+__global__ void __launch_bounds__(256)
+decode_kernel(float* __restrict__ boxes, const float* __restrict__ loc, const float* __restrict__ priors, int P,
+              long long total) {
+    const long long t = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
+    if (t >= total) return;
+    const int p = static_cast<int>(t % P);
+    const float* pb = priors + static_cast<size_t>(p) * 4;
+    const float* var = priors + static_cast<size_t>(P) * 4 + static_cast<size_t>(p) * 4;
+    const float* l = loc + static_cast<size_t>(t) * 4;
+    const float pw = __fsub_rn(pb[2], pb[0]), ph = __fsub_rn(pb[3], pb[1]);
+    const float pcx = __fmul_rn(__fadd_rn(pb[0], pb[2]), 0.5f), pcy = __fmul_rn(__fadd_rn(pb[1], pb[3]), 0.5f);
+    const float cx = __fadd_rn(__fmul_rn(__fmul_rn(var[0], l[0]), pw), pcx);
+    const float cy = __fadd_rn(__fmul_rn(__fmul_rn(var[1], l[1]), ph), pcy);
+    const float w = __fmul_rn(expf(__fmul_rn(var[2], l[2])), pw);
+    const float h = __fmul_rn(expf(__fmul_rn(var[3], l[3])), ph);
+    float* b = boxes + static_cast<size_t>(t) * 4;
+    b[0] = __fsub_rn(cx, __fmul_rn(w, 0.5f));
+    b[1] = __fsub_rn(cy, __fmul_rn(h, 0.5f));
+    b[2] = __fadd_rn(cx, __fmul_rn(w, 0.5f));
+    b[3] = __fadd_rn(cy, __fmul_rn(h, 0.5f));
+}
+
+__device__ __forceinline__ uint32_t orderable(float f) {
+    const uint32_t b = __float_as_uint(f);
+    return (b & 0x80000000u) ? ~b : (b | 0x80000000u);
+}
+__device__ __forceinline__ float from_orderable(uint32_t u) {
+    return __uint_as_float((u & 0x80000000u) ? (u & 0x7fffffffu) : ~u);
+}
+__device__ __forceinline__ unsigned long long make_key(uint32_t u, int i) {
+    return (static_cast<unsigned long long>(u) << 32) | (0xffffffffu - static_cast<uint32_t>(i));
+}
+__device__ __forceinline__ int key_index(unsigned long long k) {
+    return static_cast<int>(0xffffffffu - static_cast<uint32_t>(k));
+}
+
+struct SelectSmem {
+    unsigned long long keys[kMaxTopK];
+    int hist[256];
+    int warp_sums[kDetWarps];
+    int bcast[2];
+};
+
+// Exclusive prefix of a 0/1 flag over the CTA in thread order; *total gets the CTA's sum.  Every thread calls it.
+__device__ __forceinline__ int block_scan(int flag, int* total, SelectSmem& sm) {
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const unsigned m = __ballot_sync(0xffffffffu, flag);
+    if (lane == 0) sm.warp_sums[warp] = __popc(m);
+    __syncthreads();
+    int before = 0, sum = 0;
+#pragma unroll
+    for (int w = 0; w < kDetWarps; ++w) {
+        const int c = sm.warp_sums[w];
+        before += w < warp ? c : 0;
+        sum += c;
+    }
+    __syncthreads();
+    *total = sum;
+    return before + __popc(m & ((1u << lane) - 1u));
+}
+
+__device__ __forceinline__ int block_sum(int v, SelectSmem& sm) {
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+    if (threadIdx.x == 0) sm.bcast[0] = 0;
+    __syncthreads();
+    if ((threadIdx.x & 31) == 0) atomicAdd(&sm.bcast[0], v);
+    __syncthreads();
+    const int r = sm.bcast[0];
+    __syncthreads();
+    return r;
+}
+
+// The k largest keys (score image u descending, then index ascending) among the valid elements 0..n-1 of get(i, u):
+// their keys go to sm.keys[0..m) sorted descending, m = min(k, number valid) is returned.  An exact radix select of the
+// k-th largest u (four 8-bit passes) gives the threshold T; every element above T is taken, and of those equal to T the
+// ones with the smallest indices (an ordered scan).  Every thread calls it.
+template <class Get>
+__device__ int select_top_k(int n, int k, Get get, SelectSmem& sm) {
+    const int tid = threadIdx.x;
+    int local = 0;
+    for (int i = tid; i < n; i += kDetThreads) {
+        uint32_t u;
+        local += get(i, u) ? 1 : 0;
+    }
+    const int valid = block_sum(local, sm);
+    const bool all = valid <= k;
+    uint32_t prefix = 0, mask = 0;
+    int need = k;
+    if (!all) {
+        for (int shift = 24; shift >= 0; shift -= 8) {
+            for (int b = tid; b < 256; b += kDetThreads) sm.hist[b] = 0;
+            __syncthreads();
+            for (int i = tid; i < n; i += kDetThreads) {
+                uint32_t u;
+                if (get(i, u) && (u & mask) == prefix) atomicAdd(&sm.hist[(u >> shift) & 255u], 1);
+            }
+            __syncthreads();
+            if (tid == 0) {
+                int acc = 0, b = 255;
+                for (; b > 0; --b) {
+                    if (acc + sm.hist[b] >= need) break;
+                    acc += sm.hist[b];
+                }
+                sm.bcast[0] = b;
+                sm.bcast[1] = need - acc;
+            }
+            __syncthreads();
+            prefix |= static_cast<uint32_t>(sm.bcast[0]) << shift;
+            mask |= 255u << shift;
+            need = sm.bcast[1];
+            __syncthreads();
+        }
+    }
+    const int m = all ? valid : k;
+    // compaction: above T, or the first `need` equal to T in index order
+    if (tid == 0) sm.bcast[1] = 0;
+    __syncthreads();
+    int ties = 0;
+    for (int base = 0; base < n; base += kDetThreads) {
+        const int i = base + tid;
+        uint32_t u = 0;
+        const bool v = i < n && get(i, u);
+        const bool eq = v && !all && u == prefix;
+        int chunk_ties;
+        const int before = block_scan(eq, &chunk_ties, sm);
+        if (v && (all || u > prefix || (eq && ties + before < need))) sm.keys[atomicAdd(&sm.bcast[1], 1)] = make_key(u, i);
+        ties += chunk_ties;
+    }
+    // bitonic sort, descending, over the next power of two (padding keys 0 sort last: a real key is >= 1)
+    int len = 1;
+    while (len < m) len <<= 1;
+    __syncthreads();
+    for (int i = m + tid; i < len; i += kDetThreads) sm.keys[i] = 0;
+    __syncthreads();
+    for (int size = 2; size <= len; size <<= 1)
+        for (int stride = size >> 1; stride > 0; stride >>= 1) {
+            for (int t = tid; t < (len >> 1); t += kDetThreads) {
+                const int lo = (t / stride) * stride * 2 + (t % stride), hi = lo + stride;
+                const bool desc = (lo & size) == 0;
+                const unsigned long long a = sm.keys[lo], b = sm.keys[hi];
+                if (desc ? a < b : a > b) {
+                    sm.keys[lo] = b;
+                    sm.keys[hi] = a;
+                }
+            }
+            __syncthreads();
+        }
+    return m;
+}
+
+// IoU of two boxes, operation by operation as include/fcuda.h states it (no contraction into FMA)
+__device__ __forceinline__ float box_iou(const float* a, float area_a, const float* b, float area_b) {
+    const float iw = fmaxf(__fsub_rn(fminf(a[2], b[2]), fmaxf(a[0], b[0])), 0.f);
+    const float ih = fmaxf(__fsub_rn(fminf(a[3], b[3]), fmaxf(a[1], b[1])), 0.f);
+    const float inter = __fmul_rn(iw, ih);
+    return __fdiv_rn(inter, __fsub_rn(__fadd_rn(area_a, area_b), inter));
+}
+
+__global__ void __launch_bounds__(kDetThreads)
+nms_class_kernel(const float* __restrict__ conf, const float* __restrict__ boxes, int P, int C, float conf_thr,
+                 float nms_thr, int top_k, unsigned long long* __restrict__ kept, int* __restrict__ kept_count) {
+    __shared__ SelectSmem sm;
+    __shared__ float sb[kMaxTopK][4];
+    __shared__ float sarea[kMaxTopK];
+    __shared__ unsigned char sup[kMaxTopK];
+    const int c = blockIdx.x, n = blockIdx.y;
+    const int tid = threadIdx.x;
+    const size_t list = static_cast<size_t>(n) * C + c;
+    if (c == 0) {  // background
+        if (tid == 0) kept_count[list] = 0;
+        return;
+    }
+    const float* cf = conf + static_cast<size_t>(n) * P * C + c;
+    const int m = select_top_k(P, top_k, [&](int i, uint32_t& u) {
+        const float s = cf[static_cast<size_t>(i) * C];
+        u = orderable(s);
+        return s > conf_thr;
+    }, sm);
+    const float* ib = boxes + static_cast<size_t>(n) * P * 4;
+    for (int j = tid; j < m; j += kDetThreads) {
+        const float* b = ib + static_cast<size_t>(key_index(sm.keys[j])) * 4;
+#pragma unroll
+        for (int q = 0; q < 4; ++q) sb[j][q] = b[q];
+        sarea[j] = __fmul_rn(__fsub_rn(b[2], b[0]), __fsub_rn(b[3], b[1]));
+        sup[j] = 0;
+    }
+    __syncthreads();
+    for (int i = 0; i < m; ++i) {
+        if (!sup[i])  // uniform: sup[i] was settled before the last barrier
+            for (int j = i + 1 + tid; j < m; j += kDetThreads)
+                if (!sup[j] && box_iou(sb[i], sarea[i], sb[j], sarea[j]) > nms_thr) sup[j] = 1;
+        __syncthreads();
+    }
+    unsigned long long* out = kept + list * top_k;
+    int written = 0;
+    for (int base = 0; base < m; base += kDetThreads) {
+        const int j = base + tid;
+        const int keep = j < m && !sup[j];
+        int total;
+        const int pos = block_scan(keep, &total, sm);
+        if (keep) out[written + pos] = sm.keys[j];
+        written += total;
+    }
+    if (tid == 0) kept_count[list] = written;
+}
+
+__global__ void __launch_bounds__(kDetThreads)
+merge_kernel(float* __restrict__ out, const float* __restrict__ boxes, const unsigned long long* __restrict__ kept,
+             const int* __restrict__ kept_count, int P, int C, int top_k, int keep_top_k) {
+    __shared__ SelectSmem sm;
+    const int n = blockIdx.x;
+    const unsigned long long* lists = kept + static_cast<size_t>(n) * C * top_k;
+    const int* counts = kept_count + static_cast<size_t>(n) * C;
+    // v = class * top_k + rank in that class's kept list: for equal scores, ascending v is (class, prior) ascending
+    const int m = select_top_k(C * top_k, keep_top_k, [&](int v, uint32_t& u) {
+        const int c = v / top_k;
+        if (c == 0 || v - c * top_k >= counts[c]) return false;
+        u = static_cast<uint32_t>(lists[v] >> 32);
+        return true;
+    }, sm);
+    const float* ib = boxes + static_cast<size_t>(n) * P * 4;
+    float* o = out + static_cast<size_t>(n) * keep_top_k * 6;
+    for (int r = threadIdx.x; r < keep_top_k; r += kDetThreads) {
+        float* row = o + static_cast<size_t>(r) * 6;
+        if (r < m) {
+            const int v = key_index(sm.keys[r]);
+            const unsigned long long k = lists[v];
+            const float* b = ib + static_cast<size_t>(key_index(k)) * 4;
+            row[0] = static_cast<float>(v / top_k);
+            row[1] = from_orderable(static_cast<uint32_t>(k >> 32));
+            row[2] = b[0];
+            row[3] = b[1];
+            row[4] = b[2];
+            row[5] = b[3];
+        } else {
+            row[0] = -1.f;
+            row[1] = row[2] = row[3] = row[4] = row[5] = 0.f;
+        }
+    }
+}
+
+struct DetWorkspace {
+    float* boxes;
+    unsigned long long* kept;
+    int* counts;
+};
+
+DetWorkspace carve(float* ws, int P, int C, int top_k, int batch) {
+    DetWorkspace w;
+    const size_t box_floats = round_up_sz(static_cast<size_t>(batch) * P * 4, 4);
+    const size_t kept_floats = static_cast<size_t>(batch) * C * top_k * 2;
+    w.boxes = ws;
+    w.kept = reinterpret_cast<unsigned long long*>(ws + box_floats);
+    w.counts = reinterpret_cast<int*>(ws + box_floats + kept_floats);
+    return w;
+}
+
+}  // namespace
+
+int permute_forward(const float* in, float* out, int c, int h, int w, int order, int batch, cudaStream_t s) {
+    const long long total = static_cast<long long>(batch) * c * h * w;
+    const int prof = prof_begin(s, PROF_DETECTION, 0, 0, 8.0 * total);
+    if (order == 0) {
+        FCUDA_CHECK(cudaMemcpyAsync(out, in, static_cast<size_t>(total) * sizeof(float), cudaMemcpyDeviceToDevice, s));
+    } else if (order == 3 && batch <= 65535) {
+        const int rows = c, cols = h * w;
+        const dim3 grid(static_cast<unsigned>(ceil_div(cols, kTile)), static_cast<unsigned>(ceil_div(rows, kTile)),
+                        static_cast<unsigned>(batch));
+        transpose_kernel<<<grid, dim3(kTile, 8), 0, s>>>(in, out, rows, cols);
+        FCUDA_CHECK_LAUNCH();
+    } else {
+        const long long blocks = (total + 255) / 256;
+        permute_kernel<<<static_cast<unsigned>(blocks < 65536 * 4 ? blocks : 65536 * 4), 256, 0, s>>>(in, out, c, h, w, order,
+                                                                                                       total);
+        FCUDA_CHECK_LAUNCH();
+    }
+    prof_end(prof, s);
+    count_launch();
+    return 0;
+}
+
+int softmax_axis_forward(const float* in, float* out, int outer, int len, int inner, int batch, cudaStream_t s) {
+    const long long lines = static_cast<long long>(batch) * outer * inner;
+    const int prof = prof_begin(s, PROF_DETECTION, 0, 0, 8.0 * lines * len);
+    if (inner == 1) {
+        const long long blocks = (lines + 7) / 8;
+        if (blocks > 0x7fffffffLL) return -100;
+        softmax_rows_kernel<<<static_cast<unsigned>(blocks), 256, 0, s>>>(in, out, lines, len);
+    } else {
+        const long long blocks = (lines + 255) / 256;
+        if (blocks > 0x7fffffffLL) return -100;
+        softmax_cols_kernel<<<static_cast<unsigned>(blocks), 256, 0, s>>>(in, out, lines, len, inner);
+    }
+    FCUDA_CHECK_LAUNCH();
+    prof_end(prof, s);
+    count_launch();
+    return 0;
+}
+
+int priorbox_forward(float* out, const FcudaPriorBoxParam& p, int per_loc, int feat_w, int feat_h, float img_w, float img_h,
+                     float step_w, float step_h, cudaStream_t s) {
+    const int locs = feat_w * feat_h;
+    const int prof = prof_begin(s, PROF_DETECTION, 0, 0, 32.0 * locs * per_loc);
+    priorbox_kernel<<<static_cast<unsigned>(ceil_div(locs, 256)), 256, 0, s>>>(out, p, per_loc, feat_w, feat_h, img_w, img_h,
+                                                                              step_w, step_h);
+    FCUDA_CHECK_LAUNCH();
+    prof_end(prof, s);
+    count_launch();
+    return 0;
+}
+
+int ssd_decode(float* boxes, const float* loc, const float* priors, int num_priors, int batch, cudaStream_t s) {
+    const long long total = static_cast<long long>(batch) * num_priors;
+    const int prof = prof_begin(s, PROF_DETECTION, 0, 0, 32.0 * total + 32.0 * num_priors);
+    decode_kernel<<<static_cast<unsigned>((total + 255) / 256), 256, 0, s>>>(boxes, loc, priors, num_priors, total);
+    FCUDA_CHECK_LAUNCH();
+    prof_end(prof, s);
+    count_launch();
+    return 0;
+}
+
+size_t detection_output_workspace(int num_priors, int num_classes, int nms_top_k, int batch) {
+    return round_up_sz(static_cast<size_t>(batch) * num_priors * 4, 4) + static_cast<size_t>(batch) * num_classes * nms_top_k * 2 +
+           static_cast<size_t>(batch) * num_classes;
+}
+
+int detection_output(float* out, const float* loc, const float* conf, const float* priors, int P, int C, float conf_threshold,
+                     float nms_threshold, int nms_top_k, int keep_top_k, float* workspace, int batch, cudaStream_t s) {
+    const DetWorkspace w = carve(workspace, P, C, nms_top_k, batch);
+    int rc = ssd_decode(w.boxes, loc, priors, P, batch, s);
+    if (rc) return rc;
+    const double scores = static_cast<double>(batch) * P * C;
+    int prof = prof_begin(s, PROF_DETECTION, 0, 0, 4.0 * scores + 16.0 * batch * P);
+    nms_class_kernel<<<dim3(static_cast<unsigned>(C), static_cast<unsigned>(batch)), kDetThreads, 0, s>>>(
+        conf, w.boxes, P, C, conf_threshold, nms_threshold, nms_top_k, w.kept, w.counts);
+    FCUDA_CHECK_LAUNCH();
+    prof_end(prof, s);
+    count_launch();
+    prof = prof_begin(s, PROF_DETECTION, 0, 0, 24.0 * batch * keep_top_k);
+    merge_kernel<<<static_cast<unsigned>(batch), kDetThreads, 0, s>>>(out, w.boxes, w.kept, w.counts, P, C, nms_top_k,
+                                                                       keep_top_k);
+    FCUDA_CHECK_LAUNCH();
+    prof_end(prof, s);
+    count_launch();
+    return 0;
+}
+
+}  // namespace fcuda

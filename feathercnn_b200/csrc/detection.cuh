@@ -1,0 +1,22 @@
+#pragma once
+#include <cuda_runtime.h>
+#include <stddef.h>
+
+#include "fcuda.h"
+
+namespace fcuda {
+// ncnn Permute of `batch` (c, h, w) images; order_type 0-5 as in include/fcuda.h.  Order 3 is a tiled transpose.
+int permute_forward(const float* in, float* out, int c, int h, int w, int order, int batch, cudaStream_t s);
+// Max-subtracted softmax over the middle axis of `batch` (outer, len, inner) views.
+int softmax_axis_forward(const float* in, float* out, int outer, int len, int inner, int batch, cudaStream_t s);
+// Caffe / ncnn PriorBox of a feat_w x feat_h map: out is (2, 4 * priors) floats, boxes then variances.
+int priorbox_forward(float* out, const FcudaPriorBoxParam& p, int per_loc, int feat_w, int feat_h, float img_w, float img_h,
+                     float step_w, float step_h, cudaStream_t s);
+// Centre-size decode of `batch` images of `num_priors` loc rows against one priors blob.
+int ssd_decode(float* boxes, const float* loc, const float* priors, int num_priors, int batch, cudaStream_t s);
+// Workspace (floats) of detection_output.
+size_t detection_output_workspace(int num_priors, int num_classes, int nms_top_k, int batch);
+int detection_output(float* out, const float* loc, const float* conf, const float* priors, int num_priors, int num_classes,
+                     float conf_threshold, float nms_threshold, int nms_top_k, int keep_top_k, float* workspace, int batch,
+                     cudaStream_t s);
+}  // namespace fcuda

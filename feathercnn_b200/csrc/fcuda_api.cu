@@ -7,6 +7,7 @@
 #include "conv_direct.cuh"
 #include "conv_igemm.cuh"
 #include "depthwise.cuh"
+#include "detection.cuh"
 #include "layers.cuh"
 #include "pack.cuh"
 #include "preprocess.cuh"
@@ -74,6 +75,34 @@ float interp_scale(const FcudaInterpParam& p, int in, int out, int explicit_out,
     if (p.resize_type == 1) return explicit_out ? static_cast<float>(in) / static_cast<float>(out) : 1.f / scale;
     if (p.align_corner) return out > 1 ? static_cast<float>(in - 1) / static_cast<float>(out - 1) : 0.f;
     return static_cast<float>(in) / static_cast<float>(out);
+}
+
+// Prior count of one feature-map location (include/fcuda.h, fcuda_priorbox_forward); -200 outside the limits.
+int priorbox_count(const FcudaPriorBoxParam* p, int* per_loc) {
+    if (!p) return -100;
+    if (p->num_min_sizes < 1 || p->num_min_sizes > FCUDA_PRIORBOX_MAX || p->num_aspect_ratios < 0 ||
+        p->num_aspect_ratios > FCUDA_PRIORBOX_MAX || (p->num_max_sizes != 0 && p->num_max_sizes != p->num_min_sizes))
+        return -200;
+    int ars = 0;
+    for (int a = 0; a < p->num_aspect_ratios; ++a) {
+        if (!(p->aspect_ratios[a] > 0.f) || !isfinite(p->aspect_ratios[a])) return -200;
+        ars += fabsf(p->aspect_ratios[a] - 1.f) < 1e-6f ? 0 : (p->flip ? 2 : 1);
+    }
+    for (int k = 0; k < p->num_min_sizes; ++k) {
+        if (!(p->min_sizes[k] > 0.f) || !isfinite(p->min_sizes[k])) return -200;
+        if (p->num_max_sizes && !(p->max_sizes[k] > p->min_sizes[k] && isfinite(p->max_sizes[k]))) return -200;
+    }
+    if (!isfinite(p->offset) || !isfinite(p->step_w) || !isfinite(p->step_h)) return -200;
+    *per_loc = p->num_min_sizes * (1 + (p->num_max_sizes ? 1 : 0) + ars);
+    return 0;
+}
+
+constexpr long long kMaxPriors = 1LL << 24;
+
+int detection_limits(int P, int C, int nms_top_k, int batch) {
+    if (P < 1 || C < 1 || batch < 1) return -100;
+    if (P >= kMaxPriors || C > 1024 || nms_top_k < 1 || nms_top_k > 1024 || batch > 65535) return -200;
+    return 0;
 }
 
 struct ConvPlan {
@@ -765,6 +794,60 @@ int fcuda_crop_forward(float* output, const float* input, int channels, int in_h
     g.C = channels; g.H = in_h; g.W = in_w; g.coff = coff; g.hoff = hoff; g.woff = woff;
     g.OC = out_c; g.OH = out_h; g.OW = out_w;
     return crop_forward(input, output, g, batch, as_stream(stream));
+}
+
+int fcuda_permute_forward(float* output, const float* input, int c, int h, int w, int order_type, int batch, void* stream) {
+    if (!output || !input || c < 1 || h < 1 || w < 1 || batch < 1) return -100;
+    if (order_type < 0 || order_type > 5) return -200;
+    return permute_forward(input, output, c, h, w, order_type, batch, as_stream(stream));
+}
+
+int fcuda_softmax_axis_forward(float* output, const float* input, int outer, int len, int inner, int batch, void* stream) {
+    if (!output || !input || outer < 1 || len < 1 || inner < 1 || batch < 1) return -100;
+    return softmax_axis_forward(input, output, outer, len, inner, batch, as_stream(stream));
+}
+
+int fcuda_priorbox_per_location(const FcudaPriorBoxParam* param, int* per_location) {
+    if (!per_location) return -100;
+    return priorbox_count(param, per_location);
+}
+
+int fcuda_priorbox_forward(float* output, const FcudaPriorBoxParam* param, int feat_w, int feat_h, int img_w, int img_h,
+                           void* stream) {
+    int per_loc = 0;
+    const int rc = priorbox_count(param, &per_loc);
+    if (rc) return rc;
+    if (!output || feat_w < 1 || feat_h < 1 || img_w < 1 || img_h < 1) return -100;
+    if (static_cast<long long>(feat_w) * feat_h * per_loc >= kMaxPriors) return -200;
+    const float step_w = param->step_w > 0.f ? param->step_w : static_cast<float>(img_w) / static_cast<float>(feat_w);
+    const float step_h = param->step_h > 0.f ? param->step_h : static_cast<float>(img_h) / static_cast<float>(feat_h);
+    return priorbox_forward(output, *param, per_loc, feat_w, feat_h, static_cast<float>(img_w), static_cast<float>(img_h),
+                            step_w, step_h, as_stream(stream));
+}
+
+int fcuda_ssd_decode(float* boxes, const float* loc, const float* priors, int num_priors, int batch, void* stream) {
+    if (!boxes || !loc || !priors || num_priors < 1 || batch < 1) return -100;
+    if (num_priors >= kMaxPriors) return -200;
+    return ssd_decode(boxes, loc, priors, num_priors, batch, as_stream(stream));
+}
+
+int fcuda_detection_output_workspace_size(int num_priors, int num_classes, int nms_top_k, int batch, size_t* floats) {
+    if (!floats) return -100;
+    const int rc = detection_limits(num_priors, num_classes, nms_top_k, batch);
+    if (rc) return rc;
+    *floats = detection_output_workspace(num_priors, num_classes, nms_top_k, batch);
+    return 0;
+}
+
+int fcuda_detection_output_forward(float* output, const float* loc, const float* conf, const float* priors, int num_priors,
+                                   int num_classes, float conf_threshold, float nms_threshold, int nms_top_k, int keep_top_k,
+                                   float* workspace, int batch, void* stream) {
+    const int rc = detection_limits(num_priors, num_classes, nms_top_k, batch);
+    if (rc) return rc;
+    if (keep_top_k < 1 || keep_top_k > 1024 || isnan(nms_threshold)) return -200;
+    if (!output || !loc || !conf || !priors || !workspace || (reinterpret_cast<uintptr_t>(workspace) & 7)) return -100;
+    return detection_output(output, loc, conf, priors, num_priors, num_classes, conf_threshold, nms_threshold, nms_top_k,
+                            keep_top_k, workspace, batch, as_stream(stream));
 }
 
 int fcuda_pixel_channels(int type, int* src_channels, int* out_channels) { return pixel_channels(type, src_channels, out_channels); }

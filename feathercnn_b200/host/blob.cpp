@@ -19,6 +19,7 @@ void Blob<Dtype>::Free() {
 template <class Dtype>
 void Blob<Dtype>::ReshapeWithRealloc(const Blob<Dtype>* p_blob) {
     ReshapeWithRealloc(p_blob->num(), p_blob->channels(), p_blob->height(), p_blob->width());
+    _dims = p_blob->dims();
 }
 
 template <class Dtype>
@@ -29,6 +30,7 @@ void Blob<Dtype>::ReshapeWithRealloc(int num, int channels, int height, int widt
     _channels = channels;
     _height = height;
     _width = width;
+    _dims = 3;
 }
 
 template <class Dtype>
@@ -118,8 +120,9 @@ void Blob<Dtype>::BindExternal(Dtype* device_ptr) {
 }
 
 template <class Dtype>
-void Blob<Dtype>::ViewExternal(Dtype* device_ptr, int num, int channels, int height, int width) {
+void Blob<Dtype>::ViewExternal(Dtype* device_ptr, int num, int channels, int height, int width, int dims) {
     _num = num;
+    _dims = dims;
     _channels = channels;
     _height = height;
     _width = width;

@@ -81,6 +81,11 @@ int fnet_blob_shape(void* h, const char* name, int* n, int* c, int* hh, int* w) 
     *n = it->second->num(); *c = it->second->channels(); *hh = it->second->height(); *w = it->second->width();
     return 0;
 }
+int fnet_blob_dims(void* h, const char* name) {
+    Net* net = static_cast<Net*>(h);
+    std::map<std::string, feather::Blob<float>*>::iterator it = net->blob_map.find(name);
+    return it == net->blob_map.end() ? -1 : it->second->dims();
+}
 int fnet_extract_blob(void* h, const char* name, float* host_out) { return static_cast<Net*>(h)->ExtractBlob(host_out, name); }
 int fnet_extract_device(void* h, const char* name, const float** dev, int* n, int* c, int* hh, int* w) {
     return static_cast<Net*>(h)->ExtractDevice(name, dev, n, c, hh, w);

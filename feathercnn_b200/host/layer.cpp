@@ -41,7 +41,7 @@ int Layer::Fuse(Layer*) { return 0; }
 int Layer::Reshape() {
     // default: one top shaped like the single bottom (layer.cpp:103-114)
     if (tops.size() != 1 || bottoms.size() != 1) return FEATHER_ERR_BASE_LAYER;
-    tops[0]->ReshapeWithRealloc(bottoms[0]->num(), bottoms[0]->channels(), bottoms[0]->height(), bottoms[0]->width());
+    tops[0]->ReshapeWithRealloc(bottoms[0]);
     return 0;
 }
 

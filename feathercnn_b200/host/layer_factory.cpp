@@ -1,5 +1,6 @@
 // Built-in layer registrations: the 13 ncnn type names the reference serves (/root/reference/src/layer_factory.cpp:53-68)
-// plus Deconvolution / DeconvolutionDepthWise, Interp, Crop, Clip and PReLU, 19 in all, mapped onto this host's layer classes.  A table of {type name, factory} pairs instead of one macro line per layer; the
+// plus Deconvolution / DeconvolutionDepthWise, Interp, Crop, Clip, PReLU and SSD's Permute, Flatten, Reshape, PriorBox and
+// DetectionOutput, 24 in all, mapped onto this host's layer classes.  A table of {type name, factory} pairs instead of one macro line per layer; the
 // DEFINE_LAYER_CREATOR / REGISTER_LAYER_CREATOR macros of <feather/layer_factory.h> remain the plugin API for user layers.
 #include <feather/layer_factory.h>
 
@@ -9,6 +10,7 @@
 #include "layers/clip_prelu_layers.h"
 #include "layers/conv_layer.h"
 #include "layers/deconv_layer.h"
+#include "layers/detection_layers.h"
 #include "layers/eltwise_layer.h"
 #include "layers/inner_product_layer.h"
 #include "layers/misc_layers.h"
@@ -54,6 +56,11 @@ const BuiltIn kBuiltIns[] = {
     {"Crop", make_layer<CropLayer>},
     {"Clip", make_layer<ClipLayer>},
     {"PReLU", make_layer<PReLULayer>},
+    {"Permute", make_layer<PermuteLayer>},
+    {"Flatten", make_layer<FlattenLayer>},
+    {"Reshape", make_layer<ReshapeLayer>},
+    {"PriorBox", make_layer<PriorBoxLayer>},
+    {"DetectionOutput", make_layer<DetectionOutputLayer>},
 };
 
 }  // namespace

@@ -22,7 +22,7 @@ public:
                 LOGE("Shape mismatch among bottoms of layer %s.", this->name.c_str());
                 return FEATHER_ERR_WEIGHTS;
             }
-        for (size_t i = 0; i < tops.size(); ++i) tops[i]->ReshapeWithRealloc(n, c, h, w);
+        for (size_t i = 0; i < tops.size(); ++i) tops[i]->ReshapeWithRealloc(bottoms[0]);
         return 0;
     }
 

@@ -438,6 +438,13 @@ int Net::Extract(std::string blob_name, ncnn::Mat& out) {
     int n, c, h, w;
     int rc = Extract(blob_name, &data, &n, &c, &h, &w);
     if (rc) return rc;
+    const int rank = blob_map[blob_name]->dims();
+    if (rank == 1 || rank == 2) {  // ncnn Mat(w) / Mat(w, h): dense, no channel step
+        if (rank == 1) out.create(w, static_cast<size_t>(4));
+        else out.create(w, h, static_cast<size_t>(4));
+        memcpy(out.data, data, sizeof(float) * static_cast<size_t>(w) * h);
+        return 0;
+    }
     out.create(w, h, c, 4U);
     const size_t stride = static_cast<size_t>(w) * h;
     for (int ch = 0; ch < c; ++ch) memcpy(out.channel(ch).data, data + stride * ch, sizeof(float) * stride);

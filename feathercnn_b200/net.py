@@ -139,6 +139,14 @@ class Net:
                                                       ctypes.byref(h), ctypes.byref(w)))
         return n.value, c.value, h.value, w.value
 
+    def BlobDims(self, name: str) -> int:
+        """ncnn rank of one image of the blob: 1 = Mat(w), 2 = Mat(w, h), 3 = Mat(w, h, c).  BlobShape is (n, c, h, w)
+        whatever the rank (a rank-1 blob is (n, 1, 1, w), a rank-2 one (n, 1, h, w))."""
+        d = int(self._lib.fnet_blob_dims(self._h, name.encode()))
+        if d < 0:
+            raise FeatherError("BlobDims", d)
+        return d
+
     def Extract(self, name: str) -> np.ndarray:
         shape = self.BlobShape(name)
         out = np.empty(shape, np.float32)

@@ -6,7 +6,8 @@ weight blobs, raw fp32 for bias/BN/Scale blobs) — /root/reference/src/net.cpp:
 snapshot, and there is no network for pretrained checkpoints, so benchmarks and tests use random-init
 models of the architectures BASELINE.json names: a single 3x3 conv, VGG-16, ResNet-50 (Caffe topology:
 BN + Scale + ReLU as separate layers, Split/Eltwise residuals), MobileNet-v1, MobileNet-v2 (ReLU6 as Clip), plus a small "mini" net
-that exercises every layer type.  Weight statistics follow SURVEY.md §8(d).
+that exercises every layer type, and single-shot detectors (MobileNet-SSD, a two-head tiny SSD).  Weight statistics follow
+SURVEY.md §8(d).
 """
 from __future__ import annotations
 
@@ -26,6 +27,7 @@ class ModelWriter:
         self.blobs: set[str] = set()
         self.bin = bytearray()
         self.flops = 0.0  # direct-conv FLOPs per image, booster.h:145-148 convention
+        self.rank: dict[str, int] = {}  # ncnn rank of a blob (1, 2 or 3; absent = 3); shape stays (c, h, w) storage
 
     # ---- low level ---------------------------------------------------------------------------
     def _layer(self, type_: str, name: str, bottoms: list[str], tops: list[str], params: dict | None = None):
@@ -213,17 +215,91 @@ class ModelWriter:
         self.shape[top] = self.shape[bottoms[0]]
         return top
 
-    def concat(self, name, bottoms, top=None):
+    def concat(self, name, bottoms, top=None, axis=0):
+        """ncnn Concat over `axis` of the bottoms' rank (rank 1: 0 = w; rank 2: 0 = h, 1 = w; rank 3: 0 = c, 1 = h, 2 = w)."""
         top = top or name
-        self._layer("Concat", name, bottoms, [top], {0: 0})
-        c = sum(self.shape[b][0] for b in bottoms)
-        self.shape[top] = (c,) + self.shape[bottoms[0]][1:]
+        self._layer("Concat", name, bottoms, [top], {0: axis})
+        rank = self.rank.get(bottoms[0], 3)
+        a = (axis + rank if axis < 0 else axis) + 3 - rank
+        shape = list(self.shape[bottoms[0]])
+        shape[a] = sum(self.shape[b][a] for b in bottoms)
+        self.shape[top] = tuple(shape)
+        self.rank[top] = rank
         return top
 
-    def softmax(self, name, bottom, top=None):
+    def softmax(self, name, bottom, top=None, axis=None):
+        """Without `axis` (no 0= emitted): over each image's whole blob; with it, ncnn's softmax over that axis."""
         top = top or name
-        self._layer("Softmax", name, [bottom], [top])
+        self._layer("Softmax", name, [bottom], [top], None if axis is None else {0: axis, 1: 1})
         self.shape[top] = self.shape[bottom]
+        self.rank[top] = self.rank.get(bottom, 3)
+        return top
+
+    def permute(self, name, bottom, order, top=None):
+        """ncnn Permute 0=order_type: (c,h,w) -> 0 (c,h,w) 1 (c,w,h) 2 (h,c,w) 3 (h,w,c) 4 (w,c,h) 5 (w,h,c)."""
+        top = top or name
+        self._layer("Permute", name, [bottom], [top], {0: order})
+        axes = [(0, 1, 2), (0, 2, 1), (1, 0, 2), (1, 2, 0), (2, 0, 1), (2, 1, 0)][order]
+        self.shape[top] = tuple(self.shape[bottom][a] for a in axes)
+        return top
+
+    def flatten(self, name, bottom, top=None):
+        top = top or name
+        self._layer("Flatten", name, [bottom], [top])
+        self.shape[top] = (1, 1, int(np.prod(self.shape[bottom])))
+        self.rank[top] = 1
+        return top
+
+    def reshape(self, name, bottom, w, h=-233, c=-233, top=None):
+        """ncnn Reshape 0=w 1=h 2=c (-233 absent: the rank is the number present; 0 keeps the bottom's, -1 infers)."""
+        top = top or name
+        params = {k: v for k, v in ((0, w), (1, h), (2, c)) if v != -233}
+        self._layer("Reshape", name, [bottom], [top], params)
+        bc, bh, bw = self.shape[bottom]
+        total = bc * bh * bw
+        d = [v if v != 0 else keep for v, keep in zip((w, h, c)[:len(params)], (bw, bh, bc))]
+        if -1 in d:
+            d[d.index(-1)] = total // int(np.prod([v for v in d if v != -1]))
+        d += [1] * (3 - len(d))
+        assert d[0] * d[1] * d[2] == total, (name, d, total)
+        self.shape[top] = (d[2], d[1], d[0])
+        self.rank[top] = len(params)
+        return top
+
+    @staticmethod
+    def _floats(vals) -> str:
+        return f"{len(vals)}," + ",".join(f"{float(v):e}" for v in vals)
+
+    def priorbox(self, name, feat, image, min_sizes, max_sizes=(), aspect_ratios=(), flip=True, clip=False,
+                 variances=(0.1, 0.1, 0.2, 0.2), step=None, offset=0.5, top=None):
+        """ncnn PriorBox on a feature map and the image: a rank-2 (2, 4 * P) blob of one image (boxes, variances)."""
+        top = top or name
+        params = {-23300: self._floats(min_sizes)}
+        if max_sizes:
+            params[-23301] = self._floats(max_sizes)
+        if aspect_ratios:
+            params[-23302] = self._floats(aspect_ratios)
+        for k, v in zip((3, 4, 5, 6), variances):
+            params[k] = f"{v:e}"
+        params[7], params[8] = int(flip), int(clip)
+        if step is not None:
+            params[11], params[12] = f"{float(step[0]):e}", f"{float(step[1]):e}"
+        params[13] = f"{offset:e}"
+        self._layer("PriorBox", name, [feat, image], [top], params)
+        ars = sum(0 if abs(a - 1) < 1e-6 else (2 if flip else 1) for a in aspect_ratios)
+        per_loc = len(min_sizes) * (1 + (1 if max_sizes else 0) + ars)
+        _, fh, fw = self.shape[feat]
+        self.shape[top] = (1, 2, 4 * fh * fw * per_loc)
+        self.rank[top] = 2
+        return top
+
+    def detection_output(self, name, loc, conf, priors, num_classes, nms_threshold=0.45, nms_top_k=100, keep_top_k=100,
+                         conf_threshold=0.25, top=None):
+        top = top or name
+        self._layer("DetectionOutput", name, [loc, conf, priors], [top],
+                    {0: num_classes, 1: f"{nms_threshold:e}", 2: nms_top_k, 3: keep_top_k, 4: f"{conf_threshold:e}"})
+        self.shape[top] = (1, keep_top_k, 6)
+        self.rank[top] = 2
         return top
 
     def dropout(self, name, bottom, top=None, scale=None):
@@ -527,9 +603,74 @@ def deeplab_head_tiny(seed=0, size=32, classes=5) -> ModelWriter:
     return m
 
 
+def _ssd_heads(m: ModelWriter, data: str, sources, num_classes: int, conf_gain: float, conf_threshold: float,
+               nms_top_k: int = 100, keep_top_k: int = 100):
+    """3x3 loc / conf heads and PriorBoxes on each (blob, min_sizes, max_sizes, aspect_ratios) source; Permute 0=3 ->
+    Flatten -> Concat, the conf branch through Reshape (w = classes) -> Softmax over the class axis -> Flatten; and
+    DetectionOutput (nms 0.45)."""
+    locs, confs, priors = [], [], []
+    for src, mins, maxs, ars in sources:
+        per_loc = len(mins) * (1 + (1 if maxs else 0) + 2 * sum(abs(a - 1) >= 1e-6 for a in ars))
+        fan_in = m.shape[src][0] * 9
+        x = m.conv(f"{src}_mbox_loc", src, per_loc * 4, 3, 1, 1, True)
+        locs.append(m.flatten(f"{src}_mbox_loc_flat", m.permute(f"{src}_mbox_loc_perm", x, 3)))
+        x = m.conv(f"{src}_mbox_conf", src, per_loc * num_classes, 3, 1, 1, True, gain=conf_gain * np.sqrt(2.0 / fan_in))
+        confs.append(m.flatten(f"{src}_mbox_conf_flat", m.permute(f"{src}_mbox_conf_perm", x, 3)))
+        priors.append(m.priorbox(f"{src}_mbox_priorbox", src, data, mins, maxs, ars, flip=True, clip=False))
+    loc = m.concat("mbox_loc", locs, axis=0)
+    conf = m.concat("mbox_conf", confs, axis=0)
+    pri = m.concat("mbox_priorbox", priors, axis=1)
+    conf = m.reshape("mbox_conf_reshape", conf, num_classes, -1)
+    conf = m.softmax("mbox_conf_softmax", conf, axis=1)
+    conf = m.flatten("mbox_conf_flatten", conf)
+    return m.detection_output("detection_out", loc, conf, pri, num_classes, 0.45, nms_top_k, keep_top_k, conf_threshold)
+
+
+def mobilenet_ssd(seed=0, size=300, num_classes=21, conf_threshold=0.25, conf_gain=1.0) -> ModelWriter:
+    """MobileNet-SSD in chuanqi305's Caffe layout: the MobileNet-v1 body (conv0 .. conv13, BatchNorm + Scale + ReLU after
+    every convolution), extras conv14_1/2 .. conv17_1/2 (1x1 then 3x3 stride 2), 3x3 loc and conf heads on conv11 (3 priors
+    per location, min 60), conv13 (6, 105 / 150) and the four extras (150 / 195, 195 / 240, 240 / 285, 285 / 300), aspect
+    ratios 2 (and 3 from conv13 on), flipped, and DetectionOutput 0=21 1=0.45 2=100 3=100.  1917 priors at 300 x 300.
+    conf_gain scales the spread of the conf head's logits (more, sharper candidates above the threshold)."""
+    m = ModelWriter(seed)
+    data = m.input("data", 3, size, size)
+    x = _bn_scale_relu(m, "_conv0", m.conv("conv0", data, 32, 3, 2, 1, False))
+    cfg = [(64, 1), (128, 2), (128, 1), (256, 2), (256, 1), (512, 2), (512, 1), (512, 1), (512, 1), (512, 1), (512, 1),
+           (1024, 2), (1024, 1)]
+    for i, (oc, s) in enumerate(cfg, 1):
+        ic = m.shape[x][0]
+        x = _bn_scale_relu(m, f"_conv{i}_dw", m.conv(f"conv{i}_dw", x, ic, 3, s, 1, False, group=ic))
+        x = _bn_scale_relu(m, f"_conv{i}", m.conv(f"conv{i}_pw", x, oc, 1, 1, 0, False))
+        if i == 11:
+            conv11 = x
+    conv13 = x
+    extras = []
+    for i, (mid, oc) in enumerate([(256, 512), (128, 256), (128, 256), (64, 128)], 14):
+        x = _bn_scale_relu(m, f"_conv{i}_1", m.conv(f"conv{i}_1", x, mid, 1, 1, 0, False))
+        x = _bn_scale_relu(m, f"_conv{i}_2", m.conv(f"conv{i}_2", x, oc, 3, 2, 1, False))
+        extras.append(x)
+    sizes = [(150, 195), (195, 240), (240, 285), (285, 300)]
+    sources = [(conv11, [60.0], [], [2.0]), (conv13, [105.0], [150.0], [2.0, 3.0])]
+    sources += [(e, [float(a)], [float(b)], [2.0, 3.0]) for e, (a, b) in zip(extras, sizes)]
+    _ssd_heads(m, data, sources, num_classes, conf_gain, conf_threshold)
+    return m
+
+
+def ssd_tiny(seed=0, size=64, num_classes=5, conf_threshold=0.05, conf_gain=3.0) -> ModelWriter:
+    """Two-head SSD at small size: heads on a 16 x 16 map (min 12, aspect ratio 2: 3 priors per location) and an 8 x 8 map
+    (min 24, max 40, aspect ratios 2 and 3: 6 per location); 1152 priors at 64 x 64."""
+    m = ModelWriter(seed)
+    data = m.input("data", 3, size, size)
+    x = m.relu("relu1", m.conv("conv1", data, 16, 3, 2, 1, True))
+    a = m.relu("relu2", m.conv("conv2", x, 32, 3, 2, 1, True))
+    b = m.relu("relu3", m.conv("conv3", a, 32, 3, 2, 1, True))
+    _ssd_heads(m, data, [(a, [12.0], [], [2.0]), (b, [24.0], [40.0], [2.0, 3.0])], num_classes, conf_gain, conf_threshold)
+    return m
+
+
 ZOO = {"single_conv": single_conv, "vgg16": vgg16, "resnet50": resnet50, "mobilenet_v1": mobilenet_v1, "mini": mini,
        "decoder_tiny": decoder_tiny, "fcn8s_tiny": fcn8s_tiny, "deeplab_head_tiny": deeplab_head_tiny,
-       "mobilenet_v2": mobilenet_v2, "prelu_tiny": prelu_tiny}
+       "mobilenet_v2": mobilenet_v2, "prelu_tiny": prelu_tiny, "mobilenet_ssd": mobilenet_ssd, "ssd_tiny": ssd_tiny}
 
 
 def synthetic_input(shape, index: int = 0) -> np.ndarray:

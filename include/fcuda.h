@@ -299,6 +299,70 @@ int fcuda_interp_forward(const FcudaInterpParam* param, float* output, const flo
 int fcuda_crop_forward(float* output, const float* input, int channels, int in_h, int in_w, int coff, int hoff, int woff,
                        int out_c, int out_h, int out_w, int batch, void* stream);
 
+/* ---- SSD detection head (the reference has none of these layers) ---------------------------------------------------
+ * Every call below is stream-ordered: none allocates, synchronises or copies to the host, so all may be captured in a
+ * CUDA graph.  -100: a NULL pointer or an empty size; -200: a parameter outside the documented limits. */
+
+/* ncnn's Permute of `batch` (c, h, w) images.  Output (c', h', w') by order_type: 0 (c,h,w), 1 (c,w,h), 2 (h,c,w),
+ * 3 (h,w,c), 4 (w,c,h), 5 (w,h,c); -200 for any other order.  A pure gather, bit-exact.  Order 3 (NCHW -> NHWC, SSD's
+ * head layout) is a shared-memory tiled transpose with coalesced reads and writes. */
+int fcuda_permute_forward(float* output, const float* input, int c, int h, int w, int order_type, int batch, void* stream);
+
+/* Max-subtracted softmax over the middle axis of each of `batch` (outer, len, inner) views:
+ * y = expf(x - max) / sum(expf(x - max)).  inner == 1 (SSD's class axis) takes one warp per row of len values.
+ * fcuda_softmax_forward (the whole-blob softmax) is a separate kernel. */
+int fcuda_softmax_axis_forward(float* output, const float* input, int outer, int len, int inner, int batch, void* stream);
+
+/* Caffe / ncnn PriorBox.  Per location (x, y) of a feat_w x feat_h map, centre ((x + offset) * step_w,
+ * (y + offset) * step_h), a step <= 0 meaning img / feat; for each min size in order: the min x min box, then the
+ * sqrt(min * max) square if max sizes are given (one per min size), then for each aspect ratio ar (an ar within 1e-6 of 1
+ * is skipped) the (min * sqrt(ar), min / sqrt(ar)) box followed by its flip (min / sqrt(ar), min * sqrt(ar)) when `flip`.
+ * A box of width bw, height bh is ((cx - bw/2) / img_w, (cy - bh/2) / img_h, (cx + bw/2) / img_w, (cy + bh/2) / img_h),
+ * each operation rounded in fp32, clamped to [0, 1] when `clip`.
+ * Output: 2 rows of 4 * P floats (P = feat_w * feat_h * per-location count): row 0 the boxes, row 1 the variances.
+ * Limits (else -200): 1..16 min sizes, 0 or as many max sizes each > its min size, 0..16 aspect ratios > 0, min sizes > 0,
+ * P < 2^24. */
+#define FCUDA_PRIORBOX_MAX 16
+typedef struct FcudaPriorBoxParam {
+    int num_min_sizes, num_max_sizes, num_aspect_ratios;
+    float min_sizes[FCUDA_PRIORBOX_MAX], max_sizes[FCUDA_PRIORBOX_MAX], aspect_ratios[FCUDA_PRIORBOX_MAX];
+    float variances[4];
+    int flip, clip;
+    float step_w, step_h; /* <= 0: img / feat */
+    float offset;
+} FcudaPriorBoxParam;
+/* Validates the parameters and gives the number of priors per location. */
+int fcuda_priorbox_per_location(const FcudaPriorBoxParam* param, int* per_location);
+int fcuda_priorbox_forward(float* output, const FcudaPriorBoxParam* param, int feat_w, int feat_h, int img_w, int img_h,
+                           void* stream);
+
+/* SSD centre-size decode (ncnn / Caffe, no clipping) of `batch` images.  loc: (batch, num_priors * 4); priors: the
+ * PriorBox output (2, num_priors * 4), shared by every image; boxes: (batch, num_priors * 4) as (xmin, ymin, xmax, ymax).
+ *   pw = p2 - p0, ph = p3 - p1, pcx = (p0 + p2) * 0.5, pcy = (p1 + p3) * 0.5
+ *   cx = var0 * l0 * pw + pcx, cy = var1 * l1 * ph + pcy, w = expf(var2 * l2) * pw, h = expf(var3 * l3) * ph
+ *   box = (cx - w * 0.5, cy - h * 0.5, cx + w * 0.5, cy + h * 0.5)
+ * every operation rounded in fp32 left to right (no FMA).  The boxes DetectionOutput uses are these bits. */
+int fcuda_ssd_decode(float* boxes, const float* loc, const float* priors, int num_priors, int batch, void* stream);
+
+/* ncnn's DetectionOutput with a fixed-shape output.  conf: (batch, P * C), class fastest; class 0 is background.
+ * For each image and class c >= 1: the candidates are the priors with score > conf_threshold, ordered by (score
+ * descending, prior ascending), the first nms_top_k kept; then greedy NMS over them in that order: a candidate is kept
+ * iff no earlier kept box has IoU > nms_threshold, where for boxes a (the kept one) and b, in fp32, each operation rounded:
+ *   area   = (x1 - x0) * (y1 - y0)
+ *   iw     = min(a.x1, b.x1) - max(a.x0, b.x0), then 0 if negative     (ih likewise with y)
+ *   inter  = iw * ih
+ *   union  = (area_b + area_a) - inter
+ *   IoU    = inter / union                       a NaN IoU (0 / 0 of two empty boxes) suppresses nothing.
+ * The kept boxes of all classes are merged, ordered by (score descending, class ascending, prior ascending), and the first
+ * keep_top_k written.  output: (batch, keep_top_k, 6) rows [label, score, xmin, ymin, xmax, ymax] with the boxes of
+ * fcuda_ssd_decode; rows past an image's count are [-1, 0, 0, 0, 0, 0].
+ * Limits (else -200): 1 <= nms_top_k <= 1024, 1 <= keep_top_k <= 1024, 1 <= C <= 1024, 1 <= P < 2^24, batch <= 65535,
+ * nms_threshold not NaN.  `workspace` holds fcuda_detection_output_workspace_size floats, 8-byte aligned (else -100). */
+int fcuda_detection_output_workspace_size(int num_priors, int num_classes, int nms_top_k, int batch, size_t* floats);
+int fcuda_detection_output_forward(float* output, const float* loc, const float* conf, const float* priors, int num_priors,
+                                   int num_classes, float conf_threshold, float nms_threshold, int nms_top_k, int keep_top_k,
+                                   float* workspace, int batch, void* stream);
+
 /* Kernel-variant switches for A/B measurements and tests.  Defaults are the measured-best configuration; the environment
  * variable FCUDA_<NAME> sets the initial value.  Names (value range, default):
  *   dw_vec (0-1, 1)           vectorised depthwise kernel on wide planes
@@ -331,7 +395,7 @@ int fcuda_profile_collect(double* total_ms, double* algo_flops, double* mma_flop
 /* Same, per kernel class, for every instrumented launch (the enable switch above covers all of them):
  * kind 0 TensorGEMM, 1 implicit-GEMM conv, 2 Winograd input transform, 3 Winograd output transform, 4 pooling,
  * 5 depthwise, 6 element-wise (BN/Scale/Eltwise/Clip/PReLU), 7 deconvolution scatter / depthwise gather, 8 resize / crop (Interp,
- * Crop), < 0 all.  algo_bytes = the bytes the operation must move (inputs
+ * Crop), 9 detection (Permute, axis Softmax, PriorBox, decode, NMS, merge), < 0 all.  algo_bytes = the bytes the operation must move (inputs
  * read once + outputs written once). */
 int fcuda_profile_collect_kind(int kind, double* total_ms, double* algo_flops, double* mma_flops, double* algo_bytes,
                                long long* launches);

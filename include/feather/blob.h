@@ -20,15 +20,17 @@ inline namespace b200 {  // ABI tag: keeps these symbols apart from the referenc
 template <class Dtype>
 class Blob {
 public:
-    Blob() : name(), _data(nullptr), _capacity(0), _owned(true), _num(0), _channels(0), _height(0), _width(0) {}
+    Blob() : name(), _data(nullptr), _capacity(0), _owned(true), _num(0), _channels(0), _height(0), _width(0), _dims(3) {}
     explicit Blob(std::string name)
-        : name(name), _data(nullptr), _capacity(0), _owned(true), _num(0), _channels(0), _height(0), _width(0) {}
+        : name(name), _data(nullptr), _capacity(0), _owned(true), _num(0), _channels(0), _height(0), _width(0), _dims(3) {}
     ~Blob() { Free(); }
     Blob(const Blob&) = delete;
     Blob& operator=(const Blob&) = delete;
 
     void Free();
+    // Copies p_blob's shape and rank.
     void ReshapeWithRealloc(const Blob<Dtype>* p_blob);
+    // Rank 3 (every layer that computes its own (c, h, w) top).
     void ReshapeWithRealloc(int num, int channels, int height, int width);
     void Realloc(size_t elem_size);
 
@@ -47,7 +49,12 @@ public:
     const std::vector<Dtype>& host_stage() const { return _host; }
     void BindExternal(Dtype* device_ptr);  // non-owning; drops the host stage
     // Non-owning view of caller-provided device memory with the given shape (Net::FeedInputDevice).
-    void ViewExternal(Dtype* device_ptr, int num, int channels, int height, int width);
+    void ViewExternal(Dtype* device_ptr, int num, int channels, int height, int width, int dims = 3);
+    // ncnn rank of one image: 1 = Mat(w), stored as (c=1, h=1, w); 2 = Mat(w, h), stored as (c=1, h, w); 3 = Mat(w, h, c).
+    // Storage does not depend on it; it gives ncnn's per-rank axis numbers (Concat, Softmax) and Extract's Mat their
+    // meaning.
+    int dims() const { return _dims; }
+    void set_dims(int dims) { _dims = dims; }
 
     Dtype* data() const { return _data; }
     size_t data_size() const { return _num * _channels * _height * _width; }
@@ -66,6 +73,7 @@ private:
     bool _stage = false;
     std::vector<Dtype> _host;
     size_t _num, _channels, _height, _width;
+    int _dims;
 };
 
 }  // inline namespace b200

@@ -15,6 +15,7 @@ inline namespace b200 {  // ABI tag: keeps these symbols apart from the referenc
 class ParamDict {
 public:
     ParamDict() { clear(); }
+    bool has(int id) const { return params[id].loaded != 0; }  // the id appeared on the layer's line
     int get(int id, int def) const { return params[id].loaded ? params[id].i : def; }
     float get(int id, float def) const { return params[id].loaded ? params[id].f : def; }
     Mat get(int id, const Mat& def) const { return params[id].loaded ? params[id].v : def; }

@@ -41,7 +41,8 @@ public:
     // Returns a HOST pointer (a mirror refreshed by this call, valid until the next Extract of that blob).
     int Extract(std::string blob_name, float** output_ptr, int* n, int* c, int* h, int* w);
     int Extract(std::string blob_name, ncnn::Mat& out);  // image 0; copies every channel (the reference's
-                                                         // version repeats channel 0, net.cpp:291-294)
+                                                         // version repeats channel 0, net.cpp:291-294); a Mat of
+                                                         // the blob's ncnn rank (Blob::dims)
     int BuildBlobMap();
     std::map<std::string, Blob<float>*> blob_map;
 

@@ -45,6 +45,8 @@ int fnet_submit_batch(void* net, const float* host_nchw, int batch, const char* 
 int fnet_wait_batch(void* net, int ticket);
 int fnet_synchronize(void* net);
 int fnet_blob_shape(void* net, const char* blob, int* n, int* c, int* h, int* w);
+/* ncnn rank of one image of the blob (1, 2 or 3); -1 for an unknown blob. */
+int fnet_blob_dims(void* net, const char* blob);
 int fnet_extract_blob(void* net, const char* blob, float* host_out);  /* README.md:69 */
 int fnet_extract_device(void* net, const char* blob, const float** device_ptr, int* n, int* c, int* h, int* w);
 unsigned long long fnet_launches_per_forward(void* net);
