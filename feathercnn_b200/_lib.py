@@ -45,6 +45,14 @@ class FcudaConvParam(ctypes.Structure):
                                                                    ("activation", ctypes.c_int)]
 
 
+class FcudaConvOptions(ctypes.Structure):
+    """include/fcuda.h FcudaConvOptions: what fcuda_conv_forward_opts fuses beyond fcuda_conv_forward (all zero)."""
+
+    _fields_ = [("residual", ctypes.c_void_p), ("relu_after_add", ctypes.c_int), ("clip_min", ctypes.c_float),
+                ("clip_max", ctypes.c_float), ("dilation_h", ctypes.c_int), ("dilation_w", ctypes.c_int),
+                ("pool", ctypes.c_int)]
+
+
 class FcudaDeconvParam(ctypes.Structure):
     """include/fcuda.h FcudaDeconvParam (total channel counts; output_h / output_w filled by fcuda_deconv_output_dim)."""
 
@@ -109,6 +117,7 @@ def fcuda() -> ctypes.CDLL:
             "fcuda_conv_get_buffer_size": (i, [P, i, i, szp, szp]),
             "fcuda_conv_init": (i, [P, i, vp, vp, vp]),
             "fcuda_conv_forward": (i, [P, i, vp, vp, vp, vp, vp, i, vp]),
+            "fcuda_conv_forward_opts": (i, [P, i, vp, vp, vp, vp, vp, ctypes.POINTER(FcudaConvOptions), i, vp]),
             "fcuda_conv_forward_clip": (i, [P, i, vp, vp, vp, vp, vp, ctypes.c_float, ctypes.c_float, i, vp]),
             "fcuda_conv_forward_residual": (i, [P, i, vp, vp, vp, vp, vp, vp, i, i, vp]),
             "fcuda_conv_can_pool": (i, [P, i]),

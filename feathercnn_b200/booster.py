@@ -8,10 +8,11 @@ every call goes through ``libfcuda.so`` (no torch ops on the data path).
 from __future__ import annotations
 
 import ctypes
+import math
 
 import torch
 
-from ._lib import FcudaConvParam, fcuda
+from ._lib import FcudaConvOptions, FcudaConvParam, fcuda
 from ._lib import FcudaDeconvParam as DeconvParam
 from ._lib import FcudaInterpParam as InterpParam
 from ._lib import FcudaPriorBoxParam as PriorBoxParam
@@ -114,6 +115,18 @@ class ConvBooster:
         _check("fcuda_conv_init",
                fcuda().fcuda_conv_init(ctypes.byref(param), self.algo, _ptr(processed_kernel), kp, _stream()))
 
+    def ForwardOpts(self, param: ConvParam, output, input, kernel, buffer, bias_arr, residual=None, relu_after_add=False,
+                    clip: tuple[float, float] | None = None, dilation: int = 1, pool: bool = False, batch: int = 1) -> None:
+        """Forward with everything the epilogue can fuse (fcuda.h, FcudaConvOptions).  `clip` = (min, max) are the bounds
+        of param.activation == ACT_CLIP; a Clip without them is refused (-200), as are bounds without a Clip."""
+        if clip is None:
+            clip = (math.nan, math.nan) if param.activation == ACT_CLIP else (0.0, 0.0)
+        o = FcudaConvOptions(residual=None if residual is None else _ptr(residual).value, relu_after_add=int(relu_after_add),
+                             clip_min=clip[0], clip_max=clip[1], dilation_h=dilation, dilation_w=dilation, pool=int(pool))
+        _check("fcuda_conv_forward_opts",
+               fcuda().fcuda_conv_forward_opts(ctypes.byref(param), self.algo, _ptr(output), _ptr(input), _ptr(kernel),
+                                               _ptr(buffer), _ptr(bias_arr), ctypes.byref(o), batch, _stream()))
+
     def ForwardResidual(self, param: ConvParam, output, input, kernel, buffer, bias_arr, residual, relu_after_add,
                         batch: int = 1) -> None:
         _check("fcuda_conv_forward_residual",
@@ -140,9 +153,8 @@ def conv_forward(param: ConvParam, x: torch.Tensor, w: torch.Tensor, b: torch.Te
                  relu_after_add: bool = False, dilation: int = 1, tuned: bool = False,
                  pool: bool = False, clip: tuple[float, float] | None = None) -> tuple[torch.Tensor, int]:
     """Whole ConvBooster protocol for a batch x (N, IC, H, W) -> (N, OC, OH, OW).  Returns (output, algo).
-    With `residual` (shaped like the output) the fused Eltwise-SUM entry point is used instead of Forward.
-    With `clip` = (min, max) ForwardClip runs instead (param.activation must be ACT_CLIP).
-    `dilation` > 1 goes through fcuda_conv_forward_ext (the caller sets param.output_h/w for the dilated extent)."""
+    `residual` (shaped like the output), `clip` = (min, max) (param.activation must be ACT_CLIP), `dilation` (the caller
+    sets param.output_h/w for the dilated extent) and `pool` (the output is the pooled blob) are ForwardOpts's."""
     cb = ConvBooster()
     if algo is None:
         rc = cb.SelectAlgoTuned(param) if tuned else cb.SelectAlgo(param)
@@ -155,25 +167,10 @@ def conv_forward(param: ConvParam, x: torch.Tensor, w: torch.Tensor, b: torch.Te
     packed = torch.empty(max(packed_n, 1), device=x.device, dtype=torch.float32)
     scratch = torch.empty(max(scratch_n, 1), device=x.device, dtype=torch.float32)
     cb.Init(param, packed, w.contiguous())
-    if pool:  # fused trailing 2x2 / stride-2 max pooling: the output is the pooled blob
-        out = torch.empty((n, param.output_channels, (param.output_h + 1) // 2, (param.output_w + 1) // 2), device=x.device,
-                          dtype=torch.float32)
-        _check("fcuda_conv_forward_pool",
-               fcuda().fcuda_conv_forward_pool(ctypes.byref(param), cb.algo, _ptr(out), _ptr(x.contiguous()), _ptr(packed),
-                                               _ptr(scratch), _ptr(b), n, _stream()))
-        return out, cb.algo
-    out = torch.empty((n, param.output_channels, param.output_h, param.output_w), device=x.device, dtype=torch.float32)
-    if dilation > 1:
-        _check("fcuda_conv_forward_ext",
-               fcuda().fcuda_conv_forward_ext(ctypes.byref(param), cb.algo, _ptr(out), _ptr(x.contiguous()), _ptr(packed),
-                                              _ptr(scratch), _ptr(b), _ptr(residual.contiguous()) if residual is not None else None,
-                                              int(relu_after_add), dilation, dilation, n, _stream()))
-    elif clip is not None:
-        cb.ForwardClip(param, out, x.contiguous(), packed, scratch, b, clip[0], clip[1], n)
-    elif residual is None:
-        cb.Forward(param, out, x.contiguous(), packed, scratch, b, n)
-    else:
-        cb.ForwardResidual(param, out, x.contiguous(), packed, scratch, b, residual.contiguous(), relu_after_add, n)
+    oh, ow = ((param.output_h + 1) // 2, (param.output_w + 1) // 2) if pool else (param.output_h, param.output_w)
+    out = torch.empty((n, param.output_channels, oh, ow), device=x.device, dtype=torch.float32)
+    cb.ForwardOpts(param, out, x.contiguous(), packed, scratch, b, None if residual is None else residual.contiguous(),
+                   relu_after_add, clip, dilation, pool, n)
     return out, cb.algo
 
 

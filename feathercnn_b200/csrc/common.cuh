@@ -2,6 +2,7 @@
 #pragma once
 
 #include <cuda_runtime.h>
+#include <math.h>
 #include <stdint.h>
 #include <stdio.h>
 
@@ -26,6 +27,32 @@ namespace fcuda {
 static inline int ceil_div(int a, int b) { return (a + b - 1) / b; }
 static inline size_t ceil_div_sz(size_t a, size_t b) { return (a + b - 1) / b; }
 static inline size_t round_up_sz(size_t a, size_t b) { return ceil_div_sz(a, b) * b; }
+
+// What a convolution does to each output value after its contraction, in this order.  Built once per call by
+// conv_epilogue() and handed to every kernel launcher; a launcher reads the fields its kernels have.
+struct ConvEpilogue {
+    const float* bias;      // OC floats or null
+    const float* residual;  // fused Eltwise SUM (implicit GEMM only) or null
+    int act;                // 0 none, 1 ReLU: fmaxf(v, 0), 2 Clip: fminf(fmaxf(v, lo), hi) in the Clip instantiations
+    float lo, hi;
+    int pool;               // 1: the output is the pooled (N, OC, (OH+1)/2, (OW+1)/2) blob (Winograd, implicit GEMM)
+};
+
+// `activation` is an FcudaActivation (the same numbering as `act`).  With a residual the convolution has no activation
+// of its own and the one applied, after the sum, is the ReLU of relu_after_add.  Without Clip the bounds are [0, +inf],
+// which stand for the ReLU where a kernel takes them at run time: fminf(fmaxf(v, 0), +inf) is fmaxf(v, 0) bit for bit,
+// NaN included.
+static inline ConvEpilogue conv_epilogue(int activation, bool bias_term, const float* bias, float clip_min, float clip_max,
+                                         const float* residual, int relu_after_add, int pool) {
+    ConvEpilogue e;
+    e.bias = bias_term ? bias : nullptr;
+    e.residual = residual;
+    e.act = residual ? (relu_after_add ? 1 : 0) : (activation == 1 || activation == 2) ? activation : 0;
+    e.lo = e.act == 2 ? clip_min : 0.f;
+    e.hi = e.act == 2 ? clip_max : INFINITY;
+    e.pool = pool ? 1 : 0;
+    return e;
+}
 
 // Launch accounting for bench.py's gpu_launches (fcuda_launch_count).
 void count_launch(int n = 1);

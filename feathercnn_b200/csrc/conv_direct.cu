@@ -74,11 +74,11 @@ conv_direct_kernel(const float* __restrict__ in, const float* __restrict__ w, co
     }
 }
 
-int conv_direct(const float* in, const float* w, const float* bias, float* out, const PackGeom& g, int OC, int act,
-                float lo, float hi, int batch, cudaStream_t s) {
+int conv_direct(const float* in, const float* w, float* out, const PackGeom& g, int OC, const ConvEpilogue& e, int batch,
+                cudaStream_t s) {
     dim3 grid(ceil_div(g.OH * g.OW, 64), ceil_div(OC, 64), batch);
-    if (act == 2) conv_direct_kernel<true><<<grid, 256, 0, s>>>(in, w, bias, out, g, OC, act, lo, hi);
-    else conv_direct_kernel<false><<<grid, 256, 0, s>>>(in, w, bias, out, g, OC, act, lo, hi);
+    if (e.act == 2) conv_direct_kernel<true><<<grid, 256, 0, s>>>(in, w, e.bias, out, g, OC, e.act, e.lo, e.hi);
+    else conv_direct_kernel<false><<<grid, 256, 0, s>>>(in, w, e.bias, out, g, OC, e.act, e.lo, e.hi);
     FCUDA_CHECK_LAUNCH();
     count_launch();
     return 0;

@@ -367,7 +367,7 @@ static int prof_igemm(const IgemmProblem& p, cudaStream_t stream, long long tile
     const double mma = 2.0 * static_cast<double>(tile_pixels) * n_cols * (kblocks * 32) * (p.planes >= 2 ? 3 : 1);
     return prof_begin(stream, PROF_IGEMM, 2.0 * macs, mma,
                       4.0 * (static_cast<double>(p.N) * p.IC * p.H * p.W + static_cast<double>(p.OC) * taps * p.IC +
-                             static_cast<double>(p.N) * p.OC * p.OH * p.OW * (p.residual ? 2 : 1)));
+                             static_cast<double>(p.N) * p.OC * p.OH * p.OW * (p.epi.residual ? 2 : 1)));
 }
 
 template <int BN, int PLANES, bool CLIP>
@@ -382,7 +382,7 @@ int launch_igemm(const IgemmProblem& p, cudaStream_t stream) {
     IgemmArgs a;
     a.wbf = reinterpret_cast<const unsigned char*>(p.w_hi);
     a.wbf_kb_bytes = 2u * static_cast<unsigned>(igemm_ocpad(p.OC)) * 64u;
-    a.in = p.input; a.out = p.output; a.bias = p.bias; a.residual = p.residual;
+    a.in = p.input; a.out = p.output; a.bias = p.epi.bias; a.residual = p.epi.residual;
     a.N = p.N; a.IC = p.IC; a.H = p.H; a.W = p.W; a.OC = p.OC; a.OH = p.OH; a.OW = p.OW;
     a.KH = p.KH; a.KW = p.KW; a.pad_top = p.pad_top; a.pad_left = p.pad_left;
     a.stride_h = p.stride_h; a.stride_w = p.stride_w;
@@ -395,8 +395,8 @@ int launch_igemm(const IgemmProblem& p, cudaStream_t stream) {
     a.taps = taps;
     a.num_n = ceil_div(p.OC, BN);
     a.total_pix = static_cast<long long>(p.N) * p.OH * p.OW;
-    a.act = p.act; a.lo = p.lo; a.hi = p.hi;
-    a.pool = p.pool ? 1 : 0;
+    a.act = p.epi.act; a.lo = p.epi.lo; a.hi = p.epi.hi;
+    a.pool = p.epi.pool;
     a.tiles_x = ceil_div(p.OW, 64);
     a.tiles_y = ceil_div(p.OH, 2);
     const long long pixel_tiles = a.pool ? static_cast<long long>(p.N) * a.tiles_x * a.tiles_y : (a.total_pix + 127) / 128;
@@ -1120,7 +1120,7 @@ __device__ __forceinline__ void wide_body(const CUtensorMap& tmX, const HaloArgs
 }
 
 // The wide kernel without / with a Clip: conv_igemm_wide_kernel serves no activation and ReLU with the ReLU epilogue of
-// the other kernels (fmaxf(v, 0)); conv_igemm_wide_clip_kernel clamps to [args.lo, args.hi] (fcuda_conv_forward_clip).
+// the other kernels (fmaxf(v, 0)); conv_igemm_wide_clip_kernel clamps to [args.lo, args.hi].
 template <int BN>
 __global__ void __launch_bounds__(kThreadsIg, 1)
 conv_igemm_wide_kernel(const __grid_constant__ CUtensorMap tmX, const HaloArgs args) {
@@ -1241,13 +1241,13 @@ static int halo_input_map(const IgemmProblem& p, const HaloGeom& hg, int chans, 
 static HaloArgs halo_args(const IgemmProblem& p, const HaloGeom& hg, int BN) {
     const int taps = p.KH * p.KW;
     HaloArgs a;
-    a.residual = p.residual; a.out = p.output; a.bias = p.bias;
+    a.residual = p.epi.residual; a.out = p.output; a.bias = p.epi.bias;
     a.OC = p.OC; a.OH = p.OH; a.OW = p.OW; a.KW = p.KW; a.taps = taps;
     a.out_img_c = p.out_c_total > 0 ? p.out_c_total : p.OC;
     a.kblocks = ceil_div(taps * p.IC, 32);
     a.num_n = ceil_div(p.OC, BN);
-    a.act = p.act; a.lo = p.lo; a.hi = p.hi;
-    a.pool = p.pool ? 1 : 0;
+    a.act = p.epi.act; a.lo = p.epi.lo; a.hi = p.epi.hi;
+    a.pool = p.epi.pool;
     a.R = hg.R; a.C = hg.C;
     a.tiles_x = ceil_div(p.OW, hg.C);
     a.tiles_y = ceil_div(p.OH, hg.R);
@@ -1289,7 +1289,7 @@ int launch_halo_family(const IgemmProblem& p, const HaloGeom& hg, int BN, int sm
 // The kernel a layer takes for one N tile and operand format: the gathering kernel, or with switch igemm_halo on a
 // layer halo_geometry accepts the per-tap halo kernel, in BF16x3 mode the pre-split kernel (switch igemm_presplit) and
 // the wide one (switch igemm_wide).
-// CLIP: the Clip instantiations (IgemmProblem::act == 2); the others apply a ReLU as fmaxf(v, 0).
+// CLIP: the Clip instantiations (ConvEpilogue::act == 2); the others apply a ReLU as fmaxf(v, 0).
 template <int BN, int PLANES, bool CLIP>
 int launch_conv(const IgemmProblem& p, cudaStream_t stream) {
     HaloGeom hg;
@@ -1366,13 +1366,13 @@ int conv_igemm_pack_weights(const float* w, float* w_hi, float* w_lo, int OC, in
 // (VGG-style stacks); the other layers keep a separate pooling launch.
 bool conv_igemm_can_pool(const IgemmProblem& p) {
     return p.KH == 3 && p.KW == 3 && p.stride_h == 1 && p.stride_w == 1 && p.dil_h <= 1 && p.dil_w <= 1 && p.IC % 32 == 0 &&
-           p.pad_top <= 2 && p.pad_left <= 2 && p.W % 4 == 0 && p.residual == nullptr &&
+           p.pad_top <= 2 && p.pad_left <= 2 && p.W % 4 == 0 && p.epi.residual == nullptr &&
            (p.input == nullptr || (reinterpret_cast<uintptr_t>(p.input) & 15) == 0);
 }
 
 int conv_igemm_forward(const IgemmProblem& p, cudaStream_t stream) {
     if (!conv_igemm_supported(p.IC, p.KH, p.KW)) return -1;
-    if (p.pool && !conv_igemm_can_pool(p)) return -200;
+    if (p.epi.pool && !conv_igemm_can_pool(p)) return -200;
     using Launch = int (*)(const IgemmProblem&, cudaStream_t);
     static const Launch kLaunch[2][3][3] = {  // [Clip][N tile 32, 64, 128][planes 1, 2, 3]
         {{launch_conv<32, 1, false>, launch_conv<32, 2, false>, launch_conv<32, 3, false>},
@@ -1381,7 +1381,7 @@ int conv_igemm_forward(const IgemmProblem& p, cudaStream_t stream) {
         {{launch_conv<32, 1, true>, launch_conv<32, 2, true>, launch_conv<32, 3, true>},
          {launch_conv<64, 1, true>, launch_conv<64, 2, true>, launch_conv<64, 3, true>},
          {launch_conv<128, 1, true>, launch_conv<128, 2, true>, launch_conv<128, 3, true>}}};
-    return kLaunch[p.act == 2][igemm_bn_for(p.OC) / 64][p.planes == 3 ? 2 : p.planes == 2 ? 1 : 0](p, stream);
+    return kLaunch[p.epi.act == 2][igemm_bn_for(p.OC) / 64][p.planes == 3 ? 2 : p.planes == 2 ? 1 : 0](p, stream);
 }
 
 }  // namespace fcuda

@@ -1,6 +1,6 @@
 // Implicit-GEMM convolution on Hopper warpgroup MMA (see conv_igemm.cu).
 #pragma once
-#include <cuda_runtime.h>
+#include "common.cuh"
 
 namespace fcuda {
 
@@ -8,19 +8,15 @@ struct IgemmProblem {
     const float* input;   // (N, IC, H, W) fp32 NCHW
     const float* w_hi;    // packed filters [OC][Kf], k = tap*IC + ic, TF32-exact plane
     const float* w_lo;    // fp32 remainder plane (planes == 2) or null
-    const float* bias;    // OC floats or null
     float* output;        // (N, OC, OH, OW)
     int N, IC, H, W, OC, OH, OW;
     int KH, KW, pad_top, pad_left, stride_h, stride_w;
     int planes;           // 1 = TF32, 2 = 3xTF32, 3 = BF16x3 (w_hi / w_lo then hold the two bf16 planes)
-    int act;              // 0 none, 1 ReLU, 2 Clip: clamp to [lo, hi] (the Clip instantiations of every kernel)
-    float lo, hi;
-    const float* residual;  // optional (N, OC, OH, OW) tensor added before the activation (fused Eltwise SUM), or null
+    ConvEpilogue epi;     // every field is read; with epi.pool `output` is (N, OC, (OH+1)/2, (OW+1)/2)
     // Extensions beyond the reference (it rejects both: conv_layer.h:43-47, avx/booster.cpp:304-308); 0 = default.
     int dil_h, dil_w;       // dilation (0 or 1 = dense taps)
     int in_c_total;         // channels per image of the INPUT tensor when `input` addresses a channel slice of it
     int out_c_total;        // same for output / residual (grouped convolution = one launch per group on slices)
-    int pool;               // fuse a following 2x2 / stride-2 max pooling (pad 0): `output` is (N, OC, (OH+1)/2, (OW+1)/2)
 };
 
 // KH*KW <= 63 and, unless IC % 32 == 0, KH*KW*IC <= 8192 (shared-memory k-table).

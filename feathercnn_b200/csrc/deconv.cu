@@ -358,13 +358,12 @@ int fcuda_deconv_forward(const FcudaDeconvParam* p, float* output, const float* 
     size_t conv_scratch = 0;
     if ((rc = conv_scratch_floats(pl, batch, &conv_scratch))) return rc;
     if ((conv_scratch || pl.path == PATH_SUBPIXEL) && !scratch) return -100;
+    FcudaConvOptions o{};
+    o.dilation_h = pl.dil_h; o.dilation_w = pl.dil_w;
     if (pl.path == PATH_DIRECT)
-        return fcuda_conv_forward_ext(&pl.eq, pl.algo, output, input, packed, scratch, b, nullptr, 0, pl.dil_h, pl.dil_w,
-                                      batch, stream);
+        return fcuda_conv_forward_opts(&pl.eq, pl.algo, output, input, packed, scratch, b, &o, batch, stream);
     float* P = scratch + conv_scratch;
-    if ((rc = fcuda_conv_forward_ext(&pl.eq, pl.algo, P, input, packed, scratch, nullptr, nullptr, 0, pl.dil_h, pl.dil_w,
-                                     batch, stream)))
-        return rc;
+    if ((rc = fcuda_conv_forward_opts(&pl.eq, pl.algo, P, input, packed, scratch, nullptr, &o, batch, stream))) return rc;
     DeconvScatterGeom g;
     g.OC = q.output_channels; g.group = q.group; g.stride_h = q.stride_h; g.stride_w = q.stride_w;
     g.Hc = pl.eq.output_h; g.Wc = pl.eq.output_w; g.OH = q.output_h; g.OW = q.output_w;

@@ -393,8 +393,8 @@ dw_generic_kernel(const float* __restrict__ in, const float* __restrict__ w, con
 
 // The kernel choice of depthwise_forward; CLIP selects the Clip instantiations (act == 2).
 template <bool CLIP>
-static void dw_launch(const float* in, const float* w, const float* bias, float* out, const DwGeom& g, int act, float lo,
-                      float hi, int batch, cudaStream_t s) {
+static void dw_launch(const float* in, const float* w, float* out, const DwGeom& g, const ConvEpilogue& e, int batch,
+                      cudaStream_t s) {
     const bool k3 = g.KH == 3 && g.KW == 3 && g.pad_top == 1 && g.pad_left == 1 && g.stride_h == g.stride_w &&
                     (g.stride_h == 1 || g.stride_h == 2) && g.OW >= 24;
     // vector width: the widest VEC whose strips (32 * VEC outputs) still fill most lanes and keep accesses aligned
@@ -413,7 +413,7 @@ static void dw_launch(const float* in, const float* w, const float* bias, float*
         const int xstrips = ceil_div(g.OW, 32 * vec), ystrips = ceil_div(g.OH, kDwRows);
         const long long items = static_cast<long long>(batch) * g.C * xstrips * ystrips;
         const unsigned blocks = static_cast<unsigned>((items + 3) / 4);
-#define DW_VEC_LAUNCH(S, V) dw3x3_vec_kernel<S, V, CLIP><<<blocks, 128, 0, s>>>(in, w, bias, out, g.C, g.H, g.W, g.OH, g.OW, act, lo, hi, items, xstrips, ystrips)
+#define DW_VEC_LAUNCH(S, V) dw3x3_vec_kernel<S, V, CLIP><<<blocks, 128, 0, s>>>(in, w, e.bias, out, g.C, g.H, g.W, g.OH, g.OW, e.act, e.lo, e.hi, items, xstrips, ystrips)
         if (g.stride_h == 1 && vec == 4) DW_VEC_LAUNCH(1, 4);
         else if (g.stride_h == 1) DW_VEC_LAUNCH(1, 2);
         else DW_VEC_LAUNCH(2, 2);
@@ -423,20 +423,20 @@ static void dw_launch(const float* in, const float* w, const float* bias, float*
         const long long items = static_cast<long long>(batch) * g.C * xstrips * ystrips;
         const unsigned blocks = static_cast<unsigned>((items + 3) / 4);
         if (g.stride_h == 1)
-            dw3x3_shuffle_kernel<1, CLIP><<<blocks, 128, 0, s>>>(in, w, bias, out, g.C, g.H, g.W, g.OH, g.OW, act, lo, hi, items,
+            dw3x3_shuffle_kernel<1, CLIP><<<blocks, 128, 0, s>>>(in, w, e.bias, out, g.C, g.H, g.W, g.OH, g.OW, e.act, e.lo, e.hi, items,
                                                             xstrips, ystrips);
         else
-            dw3x3_shuffle_kernel<2, CLIP><<<blocks, 128, 0, s>>>(in, w, bias, out, g.C, g.H, g.W, g.OH, g.OW, act, lo, hi, items,
+            dw3x3_shuffle_kernel<2, CLIP><<<blocks, 128, 0, s>>>(in, w, e.bias, out, g.C, g.H, g.W, g.OH, g.OW, e.act, e.lo, e.hi, items,
                                                             xstrips, ystrips);
     } else if (!vec_off && g.KH == 3 && g.KW == 3 && g.pad_top == 1 && g.pad_left == 1 && g.stride_h == 1 && g.stride_w == 1 &&
                g.H <= 16 && g.W <= 16 && g.OH == g.H && g.OW == g.W) {
         const long long planes_ll = static_cast<long long>(batch) * g.C;
         if (g.W <= 8) {
             const unsigned blocks = static_cast<unsigned>((planes_ll + 15) / 16);
-            dw3x3_cols_kernel<8, CLIP><<<blocks, 128, 0, s>>>(in, w, bias, out, g.C, g.H, g.W, act, lo, hi, planes_ll);
+            dw3x3_cols_kernel<8, CLIP><<<blocks, 128, 0, s>>>(in, w, e.bias, out, g.C, g.H, g.W, e.act, e.lo, e.hi, planes_ll);
         } else {
             const unsigned blocks = static_cast<unsigned>((planes_ll + 7) / 8);
-            dw3x3_cols_kernel<16, CLIP><<<blocks, 128, 0, s>>>(in, w, bias, out, g.C, g.H, g.W, act, lo, hi, planes_ll);
+            dw3x3_cols_kernel<16, CLIP><<<blocks, 128, 0, s>>>(in, w, e.bias, out, g.C, g.H, g.W, e.act, e.lo, e.hi, planes_ll);
         }
     } else if (g.KH == 3 && g.KW == 3 && (g.pad_top == 0 || g.pad_top == 1) && (g.pad_left == 0 || g.pad_left == 1) &&
                g.stride_h == g.stride_w && (g.stride_h == 1 || g.stride_h == 2) && g.H <= 34 && g.W <= 34 &&
@@ -446,24 +446,24 @@ static void dw_launch(const float* in, const float* w, const float* bias, float*
         const unsigned blocks = static_cast<unsigned>((planes_ll + 3) / 4);
         const int smem = 4 * (g.H + 2) * (g.W + 2) * static_cast<int>(sizeof(float));
         if (g.stride_h == 1)
-            dw3x3_plane_kernel<1, CLIP><<<blocks, 128, smem, s>>>(in, w, bias, out, g.C, g.H, g.W, g.OH, g.OW, g.pad_top,
-                                                             g.pad_left, act, lo, hi, planes_ll);
+            dw3x3_plane_kernel<1, CLIP><<<blocks, 128, smem, s>>>(in, w, e.bias, out, g.C, g.H, g.W, g.OH, g.OW, g.pad_top,
+                                                             g.pad_left, e.act, e.lo, e.hi, planes_ll);
         else
-            dw3x3_plane_kernel<2, CLIP><<<blocks, 128, smem, s>>>(in, w, bias, out, g.C, g.H, g.W, g.OH, g.OW, g.pad_top,
-                                                             g.pad_left, act, lo, hi, planes_ll);
+            dw3x3_plane_kernel<2, CLIP><<<blocks, 128, smem, s>>>(in, w, e.bias, out, g.C, g.H, g.W, g.OH, g.OW, g.pad_top,
+                                                             g.pad_left, e.act, e.lo, e.hi, planes_ll);
     } else {
         const long long total = static_cast<long long>(batch) * g.C * g.OH * g.OW;
-        dw_generic_kernel<CLIP><<<static_cast<unsigned>((total + 255) / 256), 256, 0, s>>>(in, w, bias, out, g, act, lo, hi, total);
+        dw_generic_kernel<CLIP><<<static_cast<unsigned>((total + 255) / 256), 256, 0, s>>>(in, w, e.bias, out, g, e.act, e.lo, e.hi, total);
     }
 }
 
-int depthwise_forward(const float* in, const float* w, const float* bias, float* out, const DwGeom& g, int act, float lo,
-                      float hi, int batch, cudaStream_t s) {
+int depthwise_forward(const float* in, const float* w, float* out, const DwGeom& g, const ConvEpilogue& e, int batch,
+                      cudaStream_t s) {
     const double planes = static_cast<double>(batch) * g.C;
     const int prof = prof_begin(s, PROF_DEPTHWISE, 2.0 * planes * g.OH * g.OW * g.KH * g.KW, 0,
                                 4.0 * planes * (static_cast<double>(g.H) * g.W + static_cast<double>(g.OH) * g.OW));
-    if (act == 2) dw_launch<true>(in, w, bias, out, g, act, lo, hi, batch, s);
-    else dw_launch<false>(in, w, bias, out, g, act, lo, hi, batch, s);
+    if (e.act == 2) dw_launch<true>(in, w, out, g, e, batch, s);
+    else dw_launch<false>(in, w, out, g, e, batch, s);
     prof_end(prof, s);
     FCUDA_CHECK_LAUNCH();
     count_launch();

@@ -383,68 +383,13 @@ int fcuda_conv_init(const FcudaConvParam* p, int algo, float* packed, const floa
     return rc;
 }
 
-static int conv_forward_impl(const FcudaConvParam* p, int algo, float* output, const float* input, const float* packed,
-                             float* scratch, const float* bias, const float* residual, int relu_after_add, int batch,
-                             void* stream, int dil_h = 1, int dil_w = 1, int pool = 0, const float* clip = nullptr);
-
-int fcuda_conv_forward_ext(const FcudaConvParam* p, int algo, float* output, const float* input, const float* packed,
-                           float* scratch, const float* bias, const float* residual, int relu_after_add, int dilation_h,
-                           int dilation_w, int batch, void* stream) {
-    if (!p || dilation_h < 1 || dilation_w < 1) return -100;
-    if ((dilation_h > 1 || dilation_w > 1) && algo != FCUDA_SGECONV) return -200;  // only the implicit GEMM spaces its taps
-    if (residual && !(algo == FCUDA_SGECONV && p->activation == FCUDA_ACT_NONE)) {
-        if (dilation_h > 1 || dilation_w > 1) return -200;
-        return fcuda_conv_forward_residual(p, algo, output, input, packed, scratch, bias, residual, relu_after_add, batch, stream);
-    }
-    return conv_forward_impl(p, algo, output, input, packed, scratch, bias, residual, relu_after_add, batch, stream,
-                             dilation_h, dilation_w);
-}
-
-int fcuda_conv_forward(const FcudaConvParam* p, int algo, float* output, const float* input, const float* packed,
-                       float* scratch, const float* bias, int batch, void* stream) {
-    return conv_forward_impl(p, algo, output, input, packed, scratch, bias, nullptr, 0, batch, stream);
-}
-
-int fcuda_conv_forward_clip(const FcudaConvParam* p, int algo, float* output, const float* input, const float* packed,
-                            float* scratch, const float* bias, float clip_min, float clip_max, int batch, void* stream) {
-    if (!p) return -100;
-    if (p->activation != FCUDA_ACT_CLIP || !(clip_min <= clip_max)) return -200;
-    const float clip[2] = {clip_min, clip_max};
-    return conv_forward_impl(p, algo, output, input, packed, scratch, bias, nullptr, 0, batch, stream, 1, 1, 0, clip);
-}
-
-int fcuda_conv_forward_residual(const FcudaConvParam* p, int algo, float* output, const float* input, const float* packed,
-                                float* scratch, const float* bias, const float* residual, int relu_after_add, int batch,
-                                void* stream) {
-    if (!p || !residual) return -100;
-    if (algo == FCUDA_SGECONV && p->activation == FCUDA_ACT_NONE)  // fused into the implicit-GEMM epilogue
-        return conv_forward_impl(p, algo, output, input, packed, scratch, bias, residual, relu_after_add, batch, stream);
-    // every other algorithm: the convolution, then the reference's add_relu in place
-    int rc = conv_forward_impl(p, algo, output, input, packed, scratch, bias, nullptr, 0, batch, stream);
-    if (rc) return rc;
-    const size_t n = static_cast<size_t>(batch) * p->output_channels * p->output_h * p->output_w;
-    return add_relu(output, residual, output, n, relu_after_add, as_stream(stream));
-}
-
-static int conv_forward_impl(const FcudaConvParam* p, int algo, float* output, const float* input, const float* packed,
-                             float* scratch, const float* bias, const float* residual, int relu_after_add, int batch,
-                             void* stream, int dil_h, int dil_w, int pool, const float* clip) {
-    ConvPlan pl;
-    int rc = make_plan(p, algo, batch, &pl);
-    if (rc) return rc;
-    if (p->activation == FCUDA_ACT_CLIP && !clip) return -200;  // only fcuda_conv_forward_clip carries the bounds
-    if (!output || !input || !packed) return -100;
-    if (pl.scratch_floats && !scratch) return -100;
-    cudaStream_t s = as_stream(stream);
+// The launches of one planned convolution; `epi` is what every kernel applies after its contraction (epi.pool only on
+// the algorithms of fcuda_conv_can_pool).
+static int conv_launch(const FcudaConvParam* p, const ConvPlan& pl, float* output, const float* input, const float* packed,
+                       float* scratch, const ConvEpilogue& epi, int dil_h, int dil_w, int batch, cudaStream_t s) {
+    int rc;
     const int IC = p->input_channels, OC = p->output_channels;
-    const float* b = p->bias_term ? bias : nullptr;
-    // epilogue activation: 0 none, 1 ReLU (fmaxf(v, 0)), 2 Clip: min(max(v, lo), hi) in the Clip instantiations of the
-    // kernels.  [0, +inf] stands for a ReLU where a kernel takes the bounds at run time (fminf(fmaxf(v, 0), +inf) is
-    // fmaxf(v, 0) bit for bit, NaN included).
-    const int act = p->activation == FCUDA_ACT_RELU ? 1 : p->activation == FCUDA_ACT_CLIP ? 2 : 0;
-    const float lo = act == 2 ? clip[0] : 0.f;
-    const float hi = act == 2 ? clip[1] : INFINITY;
-    switch (algo) {
+    switch (pl.algo) {
         case FCUDA_WINOGRADF63:
         case FCUDA_WINOGRADF23: {
             const size_t v_plane = static_cast<size_t>(pl.TT) * pl.Tc_max * IC;
@@ -465,12 +410,11 @@ static int conv_forward_impl(const FcudaConvParam* p, int algo, float* output, c
                 g.algo_flops = 2.0 * OC * IC * 9.0 * p->output_h * p->output_w * batch *
                                (static_cast<double>(R1 - R0) / pl.total_tile_rows);
                 if ((rc = tensor_gemm(g, s))) return rc;
-                if ((rc = wino_output_transform(pl.tile, Mbuf, output, b, pl.wg, R0, R1, act, lo, hi, pool, s))) return rc;
+                if ((rc = wino_output_transform(pl.tile, Mbuf, output, pl.wg, R0, R1, epi, s))) return rc;
             }
             return 0;
         }
         case FCUDA_IM2COL: {
-            if (pool) return -200;
             const size_t w_plane = static_cast<size_t>(OC) * pl.pg.Kp;
             float* P = scratch;
             for (long long m0 = 0; m0 < pl.total_pixels; m0 += pl.pixels_per_chunk) {
@@ -483,8 +427,7 @@ static int conv_forward_impl(const FcudaConvParam* p, int algo, float* output, c
                 g.D = output;
                 g.M = rows; g.N = OC; g.K = pl.pg.Kp; g.G = 1;
                 g.planes = pl.np; g.epilogue = EPI_NCHW; g.P = p->output_h * p->output_w; g.m_offset = m0;
-                g.bias = b; g.relu = act != 0; g.split_k = 1;
-                g.clip = act == 2; g.clip_lo = lo; g.clip_hi = hi;
+                g.epi = epi; g.split_k = 1;
                 g.algo_flops = 2.0 * OC * pl.pg.K * static_cast<double>(rows);
                 if ((rc = tensor_gemm(g, s))) return rc;
             }
@@ -497,16 +440,18 @@ static int conv_forward_impl(const FcudaConvParam* p, int algo, float* output, c
             const size_t wplane = conv_igemm_packed_floats(OCg, ICg, taps, 1);
             const size_t wgroup = conv_igemm_packed_floats(OCg, ICg, taps, pl.np);
             const size_t in_plane = static_cast<size_t>(p->input_h) * p->input_w;
-            const size_t out_plane = static_cast<size_t>(p->output_h) * p->output_w;
+            const size_t out_plane = epi.pool ? static_cast<size_t>((p->output_h + 1) / 2) * ((p->output_w + 1) / 2)
+                                              : static_cast<size_t>(p->output_h) * p->output_w;
             for (int gi = 0; gi < G; ++gi) {  // one launch per group on channel slices (G == 1: the whole tensor)
                 IgemmProblem g{};
                 const float* wg = packed + static_cast<size_t>(gi) * wgroup;
                 g.input = input + static_cast<size_t>(gi) * ICg * in_plane;
                 g.w_hi = wg;
                 g.w_lo = pl.np == 2 ? wg + wplane : nullptr;
-                g.bias = b ? b + static_cast<size_t>(gi) * OCg : nullptr;
                 g.output = output + static_cast<size_t>(gi) * OCg * out_plane;
-                g.residual = residual ? residual + static_cast<size_t>(gi) * OCg * out_plane : nullptr;
+                g.epi = epi;
+                if (epi.bias) g.epi.bias += static_cast<size_t>(gi) * OCg;
+                if (epi.residual) g.epi.residual += static_cast<size_t>(gi) * OCg * out_plane;
                 g.N = batch; g.IC = ICg; g.OC = OCg;
                 g.in_c_total = IC; g.out_c_total = OC;
                 g.KH = p->kernel_h; g.KW = p->kernel_w; g.pad_top = p->pad_top; g.pad_left = p->pad_left;
@@ -519,29 +464,96 @@ static int conv_forward_impl(const FcudaConvParam* p, int algo, float* output, c
                     g.H = p->input_h; g.W = p->input_w; g.OH = p->output_h; g.OW = p->output_w;
                 }
                 g.planes = igemm_planes();
-                if (residual) {  // the convolution has no activation of its own (see fcuda_conv_forward_residual)
-                    g.act = relu_after_add; g.lo = 0.f; g.hi = INFINITY;
-                } else {
-                    g.act = act; g.lo = lo; g.hi = hi;
-                }
-                g.pool = pool;
-                if (pool) {  // pooled output planes
-                    g.output = output + static_cast<size_t>(gi) * OCg * (static_cast<size_t>((p->output_h + 1) / 2) * ((p->output_w + 1) / 2));
-                    g.out_c_total = OC;
-                }
                 if ((rc = conv_igemm_forward(g, s))) return rc;
             }
             return 0;
         }
         case FCUDA_NAIVE:
-            if (pool) return -200;
-            return conv_direct(input, packed, b, output, pl.pg, OC, act, lo, hi, batch, s);
+            return conv_direct(input, packed, output, pl.pg, OC, epi, batch, s);
         case FCUDA_DEPTHWISE:
-            if (pool) return -200;
-            return depthwise_forward(input, packed, b, output, pl.dg, act, lo, hi, batch, s);
+            return depthwise_forward(input, packed, output, pl.dg, epi, batch, s);
         default:
             return -1;
     }
+}
+
+// The one forward path: fcuda_conv_forward_opts, and the five older entry points with the options their signatures carry
+// (include/fcuda.h, FcudaConvOptions).  clip_bounds_given is false from the entry points without clip bounds: for them a
+// Clip activation is refused, after the plan's own error and before the tensor checks.
+static int conv_forward(const FcudaConvParam* p, int algo, float* output, const float* input, const float* packed,
+                        float* scratch, const float* bias, const FcudaConvOptions& o, bool clip_bounds_given, int batch,
+                        void* stream) {
+    if (!p || o.dilation_h < 0 || o.dilation_w < 0) return -100;
+    const int dil_h = o.dilation_h ? o.dilation_h : 1, dil_w = o.dilation_w ? o.dilation_w : 1;
+    const bool dilated = dil_h > 1 || dil_w > 1;
+    const bool clip = clip_bounds_given && p->activation == FCUDA_ACT_CLIP;
+    if (clip && !(o.clip_min <= o.clip_max)) return -200;  // (a NaN bound too)
+    if (clip_bounds_given && !clip && (o.clip_min != 0.f || o.clip_max != 0.f)) return -200;  // bounds without a Clip
+    if (dilated && algo != FCUDA_SGECONV) return -200;  // only the implicit GEMM spaces its taps
+    // The implicit GEMM adds the residual in its epilogue when the convolution has no activation of its own; every other
+    // case is the convolution, then the reference's add_relu in place.
+    const bool fuse_residual = o.residual && algo == FCUDA_SGECONV && p->activation == FCUDA_ACT_NONE;
+    if (dilated && o.residual && !fuse_residual) return -200;
+    if (o.pool && !fcuda_conv_can_pool(p, algo)) return -200;
+    if ((clip && (o.residual || dilated || o.pool)) || (o.pool && (o.residual || dilated))) return -200;  // not built
+    ConvPlan pl;
+    int rc = make_plan(p, algo, batch, &pl);
+    if (rc) return rc;
+    if (p->activation == FCUDA_ACT_CLIP && !clip_bounds_given) return -200;
+    if (!output || !input || !packed) return -100;
+    if (pl.scratch_floats && !scratch) return -100;
+    const ConvEpilogue epi = conv_epilogue(p->activation, p->bias_term, bias, o.clip_min, o.clip_max,
+                                           fuse_residual ? o.residual : nullptr, o.relu_after_add, o.pool);
+    if ((rc = conv_launch(p, pl, output, input, packed, scratch, epi, dil_h, dil_w, batch, as_stream(stream)))) return rc;
+    if (!o.residual || fuse_residual) return 0;
+    const size_t n = static_cast<size_t>(batch) * p->output_channels * p->output_h * p->output_w;
+    return add_relu(output, o.residual, output, n, o.relu_after_add, as_stream(stream));
+}
+
+int fcuda_conv_forward_opts(const FcudaConvParam* p, int algo, float* output, const float* input, const float* packed,
+                            float* scratch, const float* bias, const FcudaConvOptions* options, int batch, void* stream) {
+    return conv_forward(p, algo, output, input, packed, scratch, bias, options ? *options : FcudaConvOptions{}, true, batch,
+                        stream);
+}
+
+int fcuda_conv_forward(const FcudaConvParam* p, int algo, float* output, const float* input, const float* packed,
+                       float* scratch, const float* bias, int batch, void* stream) {
+    return conv_forward(p, algo, output, input, packed, scratch, bias, FcudaConvOptions{}, false, batch, stream);
+}
+
+int fcuda_conv_forward_clip(const FcudaConvParam* p, int algo, float* output, const float* input, const float* packed,
+                            float* scratch, const float* bias, float clip_min, float clip_max, int batch, void* stream) {
+    if (!p) return -100;
+    if (p->activation != FCUDA_ACT_CLIP) return -200;
+    FcudaConvOptions o{};
+    o.clip_min = clip_min; o.clip_max = clip_max;
+    return conv_forward(p, algo, output, input, packed, scratch, bias, o, true, batch, stream);
+}
+
+int fcuda_conv_forward_residual(const FcudaConvParam* p, int algo, float* output, const float* input, const float* packed,
+                                float* scratch, const float* bias, const float* residual, int relu_after_add, int batch,
+                                void* stream) {
+    if (!p || !residual) return -100;
+    FcudaConvOptions o{};
+    o.residual = residual; o.relu_after_add = relu_after_add;
+    return conv_forward(p, algo, output, input, packed, scratch, bias, o, false, batch, stream);
+}
+
+int fcuda_conv_forward_pool(const FcudaConvParam* p, int algo, float* output, const float* input, const float* packed,
+                            float* scratch, const float* bias, int batch, void* stream) {
+    FcudaConvOptions o{};
+    o.pool = 1;
+    return conv_forward(p, algo, output, input, packed, scratch, bias, o, false, batch, stream);
+}
+
+int fcuda_conv_forward_ext(const FcudaConvParam* p, int algo, float* output, const float* input, const float* packed,
+                           float* scratch, const float* bias, const float* residual, int relu_after_add, int dilation_h,
+                           int dilation_w, int batch, void* stream) {
+    if (!p || dilation_h < 1 || dilation_w < 1) return -100;
+    FcudaConvOptions o{};
+    o.residual = residual; o.relu_after_add = relu_after_add;
+    o.dilation_h = dilation_h; o.dilation_w = dilation_w;
+    return conv_forward(p, algo, output, input, packed, scratch, bias, o, false, batch, stream);
 }
 
 // The implicit-GEMM problem of one group of a layer, without tensors (N = 1): what the tile and pooling queries read
@@ -556,7 +568,7 @@ static IgemmProblem igemm_problem(const FcudaConvParam* p) {
     return g;
 }
 
-// Can fcuda_conv_forward_pool fuse the pooling for this layer?  Winograd: always (the output tile starts at an even
+// Can the epilogue fuse the pooling (FcudaConvOptions::pool) for this layer?  Winograd: always (the output tile starts at an even
 // coordinate); implicit GEMM: the 3x3 / stride-1 slab kernel (group 1).
 int fcuda_conv_can_pool(const FcudaConvParam* p, int algo) {
     if (!p) return 0;
@@ -576,13 +588,6 @@ static int igemm_tile(const FcudaConvParam* p, int* geom, bool (*geometry)(const
 int fcuda_igemm_halo_tile(const FcudaConvParam* p, int* geom) { return igemm_tile(p, geom, conv_igemm_halo_geometry); }
 int fcuda_igemm_presplit_tile(const FcudaConvParam* p, int* geom) { return igemm_tile(p, geom, conv_igemm_presplit_geometry); }
 int fcuda_igemm_wide_tile(const FcudaConvParam* p, int* geom) { return igemm_tile(p, geom, conv_igemm_wide_geometry); }
-
-int fcuda_conv_forward_pool(const FcudaConvParam* p, int algo, float* output, const float* input, const float* packed,
-                            float* scratch, const float* bias, int batch, void* stream) {
-    if (!p) return -100;
-    if (!fcuda_conv_can_pool(p, algo)) return -200;
-    return conv_forward_impl(p, algo, output, input, packed, scratch, bias, nullptr, 0, batch, stream, 1, 1, 1);
-}
 
 int fcuda_tensor_gemm(float* d, const float* a, const float* b_hi, const float* b_lo, int m, int n, int k, int g,
                       void* stream) {

@@ -459,18 +459,11 @@ bool tensor_gemm_supported(const GemmProblem& p) {
     return true;
 }
 
-// The epilogue clamp of a problem: its Clip bounds, or [0, +inf] for a ReLU (fmaxf(v, 0) bit for bit, NaN included)
-static void set_activation(const GemmProblem& p, int* act, float* lo, float* hi) {
-    *act = p.clip || p.relu;
-    *lo = p.clip ? p.clip_lo : 0.f;
-    *hi = p.clip ? p.clip_hi : INFINITY;
-}
-
 static void fill_kernel_args(const GemmProblem& p, int bn, GemmKernelArgs* a) {
-    a->D = p.D; a->bias = p.bias;
+    a->D = p.D; a->bias = p.epi.bias;
     a->M = p.M; a->N = p.N; a->K = p.K; a->G = p.G;
     a->epilogue = p.epilogue; a->ldd = p.ldd; a->P = p.P > 0 ? p.P : 1;
-    set_activation(p, &a->act, &a->lo, &a->hi);
+    a->act = p.epi.act; a->lo = p.epi.lo; a->hi = p.epi.hi;
     a->m_offset = p.m_offset;
     a->split_stride = p.split_stride;
     a->num_m = ceil_div(p.M, kBM);
@@ -528,7 +521,7 @@ static int launch(const GemmProblem& p, cudaStream_t stream) {
 }
 
 // N tile: the smallest supported tile that covers N (fewer wasted MMA columns), capped at 128.  CLIP: the instantiations
-// whose EPI_NCHW epilogue clamps to [clip_lo, clip_hi]; the others apply a ReLU as fmaxf(v, 0).
+// whose EPI_NCHW epilogue clamps to [epi.lo, epi.hi]; the others apply a ReLU as fmaxf(v, 0).
 template <bool CLIP>
 static int launch_tile(const GemmProblem& p, cudaStream_t stream) {
     if (p.planes == 2) {
@@ -544,7 +537,7 @@ static int launch_tile(const GemmProblem& p, cudaStream_t stream) {
 int tensor_gemm(const GemmProblem& p, cudaStream_t stream) {
     if (!tensor_gemm_supported(p)) return -1;
     if (p.split_k > 1 && p.epilogue != EPI_COLMAJOR_PARTIAL) return -1;
-    return p.clip ? launch_tile<true>(p, stream) : launch_tile<false>(p, stream);
+    return p.epi.act == 2 ? launch_tile<true>(p, stream) : launch_tile<false>(p, stream);
 }
 
 // --------------------------------------------------------------------------------------------
@@ -616,11 +609,11 @@ simt_gemm_kernel(const float* __restrict__ A_hi, const float* __restrict__ A_lo,
 
 int simt_gemm(const GemmProblem& p, cudaStream_t stream) {
     GemmKernelArgs a;
-    a.D = p.D; a.bias = p.bias;
+    a.D = p.D; a.bias = p.epi.bias;
     a.M = p.M; a.N = p.N; a.K = p.K; a.G = p.G;
     a.epilogue = p.epilogue; a.ldd = p.ldd; a.P = p.P > 0 ? p.P : 1; a.split_k = 1; a.m_offset = p.m_offset; a.split_stride = 0;
     a.num_m = ceil_div(p.M, 64); a.num_n = ceil_div(p.N, 64); a.k_blocks_total = 0;
-    set_activation(p, &a.act, &a.lo, &a.hi);
+    a.act = p.epi.act; a.lo = p.epi.lo; a.hi = p.epi.hi;
     const long long as = p.a_batch_stride ? p.a_batch_stride : static_cast<long long>(p.M) * p.K;
     const long long bs = p.b_batch_stride ? p.b_batch_stride : static_cast<long long>(p.N) * p.K;
     dim3 grid(a.num_n, a.num_m, p.G);

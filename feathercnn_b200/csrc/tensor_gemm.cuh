@@ -15,8 +15,8 @@
 #pragma once
 
 #include <cuda.h>
-#include <cuda_runtime.h>
-#include <stdint.h>
+
+#include "common.cuh"
 
 namespace fcuda {
 
@@ -43,10 +43,7 @@ struct GemmProblem {
     int ldd;           // EPI_ROWMAJOR / EPI_COLMAJOR_PARTIAL leading dimension (floats)
     int P;             // EPI_NCHW: pixels per image
     long long m_offset;  // EPI_NCHW: global pixel index of row 0 (chunked im2col); image = (m_offset + m) / P
-    const float* bias; // EPI_NCHW: per-n bias or null
-    int relu;          // EPI_NCHW: fuse max(0, .)
-    int clip;          // EPI_NCHW: fuse min(max(., clip_lo), clip_hi) instead of the ReLU
-    float clip_lo, clip_hi;
+    ConvEpilogue epi;  // EPI_NCHW: per-n bias and activation (bias, act, lo, hi; the other fields are not read)
     int split_k;       // >=1; only with EPI_COLMAJOR_PARTIAL
     long long split_stride;  // EPI_COLMAJOR_PARTIAL: floats between the partial planes of consecutive k-splits
     long long a_batch_stride;  // floats between consecutive g in A; 0 => dense (M*K)

@@ -428,24 +428,24 @@ int wino_input_transform(int tile, const float* in, float* V, const WinoGeom& g,
 }
 
 template <bool CLIP>
-static void wino_output_launch(int tile, int pool, bool mlp, dim3 grid, const float* M, float* out, const float* bias,
-                               const WinoGeom& g, int R0, int Tc, int act, float lo, float hi, int ncb, cudaStream_t s) {
+static void wino_output_launch(int tile, bool mlp, dim3 grid, const float* M, float* out, const WinoGeom& g, int R0, int Tc,
+                               const ConvEpilogue& e, int ncb, cudaStream_t s) {
     if (tile == 8) {
         if (mlp) {
-            if (pool) wino_output_kernel<8, true, true, CLIP><<<grid, kXformThreads, 0, s>>>(M, out, bias, g, R0, Tc, act, lo, hi, ncb);
-            else wino_output_kernel<8, false, true, CLIP><<<grid, kXformThreads, 0, s>>>(M, out, bias, g, R0, Tc, act, lo, hi, ncb);
+            if (e.pool) wino_output_kernel<8, true, true, CLIP><<<grid, kXformThreads, 0, s>>>(M, out, e.bias, g, R0, Tc, e.act, e.lo, e.hi, ncb);
+            else wino_output_kernel<8, false, true, CLIP><<<grid, kXformThreads, 0, s>>>(M, out, e.bias, g, R0, Tc, e.act, e.lo, e.hi, ncb);
         } else {
-            if (pool) wino_output_kernel<8, true, false, CLIP><<<grid, kXformThreads, 0, s>>>(M, out, bias, g, R0, Tc, act, lo, hi, ncb);
-            else wino_output_kernel<8, false, false, CLIP><<<grid, kXformThreads, 0, s>>>(M, out, bias, g, R0, Tc, act, lo, hi, ncb);
+            if (e.pool) wino_output_kernel<8, true, false, CLIP><<<grid, kXformThreads, 0, s>>>(M, out, e.bias, g, R0, Tc, e.act, e.lo, e.hi, ncb);
+            else wino_output_kernel<8, false, false, CLIP><<<grid, kXformThreads, 0, s>>>(M, out, e.bias, g, R0, Tc, e.act, e.lo, e.hi, ncb);
         }
     } else {
-        if (pool) wino_output_kernel<4, true, false, CLIP><<<grid, kXformThreads, 0, s>>>(M, out, bias, g, R0, Tc, act, lo, hi, ncb);
-        else wino_output_kernel<4, false, false, CLIP><<<grid, kXformThreads, 0, s>>>(M, out, bias, g, R0, Tc, act, lo, hi, ncb);
+        if (e.pool) wino_output_kernel<4, true, false, CLIP><<<grid, kXformThreads, 0, s>>>(M, out, e.bias, g, R0, Tc, e.act, e.lo, e.hi, ncb);
+        else wino_output_kernel<4, false, false, CLIP><<<grid, kXformThreads, 0, s>>>(M, out, e.bias, g, R0, Tc, e.act, e.lo, e.hi, ncb);
     }
 }
 
-int wino_output_transform(int tile, const float* M, float* out, const float* bias, const WinoGeom& g, int R0, int R1,
-                          int act, float lo, float hi, int pool, cudaStream_t s) {
+int wino_output_transform(int tile, const float* M, float* out, const WinoGeom& g, int R0, int R1, const ConvEpilogue& e,
+                          cudaStream_t s) {
     const int segs = ceil_div(g.tilesX, kSegTiles);
     const int Tc = (R1 - R0) * g.tilesX;
     dim3 grid(static_cast<unsigned>(segs) * (R1 - R0), ceil_div(g.C_out, kChBlock));
@@ -455,12 +455,12 @@ int wino_output_transform(int tile, const float* M, float* out, const float* bia
         grid = dim3(grid.x * grid.y, 1);
     }
     const double imgs = static_cast<double>(R1 - R0) / g.tilesY;  // tile-rows of the chunk, in images
-    const double out_px = pool ? static_cast<double>((g.OH + 1) / 2) * ((g.OW + 1) / 2) : static_cast<double>(g.OH) * g.OW;
+    const double out_px = e.pool ? static_cast<double>((g.OH + 1) / 2) * ((g.OW + 1) / 2) : static_cast<double>(g.OH) * g.OW;
     const int prof = prof_begin(s, PROF_WINO_OUTPUT, 0, 0,
                                 4.0 * (imgs * g.C_out * out_px + static_cast<double>(tile) * tile * Tc * g.C_out));
     const bool mlp = tune_get(TUNE_WINO_MLP) != 0;
-    if (act == 2) wino_output_launch<true>(tile, pool, mlp, grid, M, out, bias, g, R0, Tc, act, lo, hi, ncb, s);
-    else wino_output_launch<false>(tile, pool, mlp, grid, M, out, bias, g, R0, Tc, act, lo, hi, ncb, s);
+    if (e.act == 2) wino_output_launch<true>(tile, mlp, grid, M, out, g, R0, Tc, e, ncb, s);
+    else wino_output_launch<false>(tile, mlp, grid, M, out, g, R0, Tc, e, ncb, s);
     prof_end(prof, s);
     FCUDA_CHECK_LAUNCH();
     count_launch();

@@ -204,29 +204,19 @@ public:
     int Forward() {
         float* buffer = NULL;
         MEMPOOL_CHECK_RETURN(this->common_mempool->GetPtr(&buffer));
-        if (fused_pool) {
-            const int batch = static_cast<int>(bottoms[0]->num());
-            if (pool_in_epilogue)
-                return fcuda_conv_forward_pool(&conv_param, conv_booster.GetAlgo(), tops[0]->data(), bottoms[0]->data(),
-                                               processed_kernel, buffer, bias_data, batch, stream());
-            int rc = fcuda_conv_forward_ext(&conv_param, conv_booster.GetAlgo(), pre_pool->data(), bottoms[0]->data(),
-                                            processed_kernel, buffer, bias_data, NULL, 0, dilation_h, dilation_w, batch, stream());
-            if (rc) return rc;
-            return fcuda_pooling_forward(tops[0]->data(), pre_pool->data(), conv_param.output_channels, conv_param.output_h,
-                                         conv_param.output_w, 0, 2, 2, 2, 2, 0, 0, 0, 0, 0, batch, stream());
-        }
-        if (dilation_h > 1 || dilation_w > 1)
-            return fcuda_conv_forward_ext(&conv_param, conv_booster.GetAlgo(), tops[0]->data(), bottoms[0]->data(),
-                                          processed_kernel, buffer, bias_data, residual ? residual->data() : NULL,
-                                          relu_after_add, dilation_h, dilation_w, bottoms[0]->num(), stream());
-        if (conv_param.activation == booster::Clip)
-            return conv_booster.ForwardClip(&conv_param, tops[0]->data(), bottoms[0]->data(), processed_kernel, buffer,
-                                            bias_data, clip_min, clip_max, bottoms[0]->num(), stream());
-        if (residual != NULL)
-            return conv_booster.ForwardResidual(&conv_param, tops[0]->data(), bottoms[0]->data(), processed_kernel, buffer,
-                                                bias_data, residual->data(), relu_after_add, bottoms[0]->num(), stream());
-        return conv_booster.Forward(&conv_param, tops[0]->data(), bottoms[0]->data(), processed_kernel, buffer, bias_data,
-                                    bottoms[0]->num(), stream());
+        const int batch = static_cast<int>(bottoms[0]->num());
+        FcudaConvOptions o = FcudaConvOptions();
+        o.residual = residual ? residual->data() : NULL;
+        o.relu_after_add = relu_after_add;
+        o.clip_min = clip_min; o.clip_max = clip_max;
+        o.dilation_h = dilation_h; o.dilation_w = dilation_w;
+        o.pool = fused_pool && pool_in_epilogue;
+        const bool pool_after = fused_pool && !pool_in_epilogue;
+        const int rc = conv_booster.ForwardOpts(&conv_param, pool_after ? pre_pool->data() : tops[0]->data(), bottoms[0]->data(),
+                                                processed_kernel, buffer, bias_data, o, batch, stream());
+        if (rc || !pool_after) return rc;
+        return fcuda_pooling_forward(tops[0]->data(), pre_pool->data(), conv_param.output_channels, conv_param.output_h,
+                                     conv_param.output_w, 0, 2, 2, 2, 2, 0, 0, 0, 0, 0, batch, stream());
     }
 
     // Net::ApplyFusion: absorb `Eltwise SUM(this->top, other) [+ReLU]` (a ResNet shortcut) into this layer's epilogue.
@@ -242,8 +232,7 @@ public:
         if (fused_pool) return 0;  // the pooling is always last
         if (next_layer->type.compare("Pooling") == 0) {
             PoolingLayer* pl = dynamic_cast<PoolingLayer*>(next_layer);
-            // A clamped convolution keeps its pooling separate: the pooled epilogue entry point
-            // (fcuda_conv_forward_pool) has no clip bounds, and fcuda_conv_forward_clip does not pool.
+            // A clamped convolution keeps its pooling separate: a Clip followed by the pooling in one epilogue is not built.
             if (!pl || !pl->IsMax2x2Stride2() || residual != NULL || conv_param.activation == booster::Clip) return 0;
             fused_pool = true;
             return 1;
@@ -254,8 +243,8 @@ public:
             return 1;
         }
         if (next_layer->type.compare("Clip") == 0) {
-            // after any BatchNorm / Scale folding, so conv -> BN -> Scale -> Clip is one kernel.  Dilated convolutions run
-            // through fcuda_conv_forward_ext, which has no clip bounds: their Clip stays a layer of its own.
+            // after any BatchNorm / Scale folding, so conv -> BN -> Scale -> Clip is one kernel.  A Clip in the epilogue of a
+            // dilated convolution, or before a residual sum, is not built: there the Clip stays a layer of its own.
             const ClipLayer* cl = dynamic_cast<const ClipLayer*>(next_layer);
             if (!cl || residual != NULL || dilation_h > 1 || dilation_w > 1) return 0;
             conv_param.activation = booster::Clip;

@@ -34,8 +34,8 @@ enum FcudaConvAlgo {
 };
 
 /* booster::ActivationType, booster.h:53-57, plus FCUDA_ACT_CLIP (ncnn's Clip / Caffe's ReLU6, an extension): a clamp to
- * [clip_min, clip_max] whose bounds only fcuda_conv_forward_clip carries — every other convolution entry point returns -200
- * for it. */
+ * [clip_min, clip_max] whose bounds fcuda_conv_forward_opts and fcuda_conv_forward_clip carry — every other convolution
+ * entry point returns -200 for it. */
 enum FcudaActivation { FCUDA_ACT_NONE = 0, FCUDA_ACT_RELU = 1, FCUDA_ACT_CLIP = 2 };
 
 /* Field-compatible with booster::ConvParam (booster.h:59-77): 15 ints, bool, enum. */
@@ -104,12 +104,40 @@ int fcuda_conv_init(const FcudaConvParam* param, int algo, float* packed_kernel,
 int fcuda_conv_forward(const FcudaConvParam* param, int algo, float* output, const float* input,
                        const float* packed_kernel, float* scratch, const float* bias, int batch, void* stream);
 
-/* fcuda_conv_forward with param->activation == FCUDA_ACT_CLIP (-200 otherwise, and for clip_min > clip_max or a NaN
- * bound): output = min(max(conv(input) [+bias], clip_min), clip_max), the clamp applied in the epilogue of the same
- * kernels every algorithm runs (Caffe's ReLU6 is clip_min = 0, clip_max = 6).  The bits before the clamp are those of
- * fcuda_conv_forward with FCUDA_ACT_NONE.  NaN maps to clip_min (fmaxf returns the non-NaN operand); ncnn's
- * compare-and-assign Clip passes NaN through.  Runs the Clip instantiations of the kernels; the ReLU and plain launches
- * of the other entry points are unchanged. */
+/* What a convolution does beyond fcuda_conv_forward, which is the all-zero struct.  Per output value, in this order:
+ * + bias, param->activation (or, with a residual, + residual then relu_after_add), the pooling.
+ *   residual        a tensor shaped like the output, added to conv(input) [+bias]: a fused Eltwise SUM (ResNet shortcuts;
+ *                   ConvLayer::Forward then EltwiseLayer::Forward, src/layers/eltwise_layer.h:68-82 -> booster::add_relu<>).
+ *                   FCUDA_SGECONV with FCUDA_ACT_NONE adds it in its epilogue; every other case runs the convolution with
+ *                   its own activation and then add_relu in place.  NULL = none.
+ *   relu_after_add  a ReLU after that sum; read only with a residual.
+ *   clip_min/max    the bounds of FCUDA_ACT_CLIP: output = min(max(conv(input) [+bias], clip_min), clip_max), the clamp
+ *                   applied in the epilogue of the same kernels every algorithm runs, by their Clip instantiations (Caffe's
+ *                   ReLU6 is 0, 6).  The bits before the clamp are those of FCUDA_ACT_NONE.  NaN maps to clip_min (fmaxf
+ *                   returns the non-NaN operand); ncnn's compare-and-assign Clip passes NaN through.  -200 for
+ *                   clip_min > clip_max or a NaN bound, and for a non-zero bound with any other activation.
+ *   dilation_h/w    tap spacing, 0 meaning 1 (the reference rejects it, src/layers/conv_layer.h:43-47).  > 1:
+ *                   FCUDA_SGECONV only (-200 otherwise, and with a residual it cannot add in its epilogue); the caller sets
+ *                   param->output_h/w for the dilated extent out = (in + pads - dilation*(k-1) - 1) / stride + 1.  < 0: -100.
+ *   pool            non-zero: a FOLLOWING 2x2 / stride-2 / pad-0 max pooling (ConvLayer::Forward then PoolingLayer::Forward,
+ *                   src/layers/pooling_layer.h:38-91): `output` is the pooled blob (batch, OC, (OH+1)/2, (OW+1)/2), ceil
+ *                   mode, windows clipped at the border like the reference.  -200 unless fcuda_conv_can_pool.
+ * Not built, -200: Clip together with a residual, a dilation or the pooling; the pooling together with a residual or a
+ * dilation. */
+typedef struct FcudaConvOptions {
+    const float* residual;
+    int relu_after_add;
+    float clip_min, clip_max;
+    int dilation_h, dilation_w;
+    int pool;
+} FcudaConvOptions;
+/* fcuda_conv_forward with `options` (NULL = the all-zero struct).  The entry points fcuda_conv_forward_clip, _residual,
+ * _pool and _ext below are this call with some of the options set. */
+int fcuda_conv_forward_opts(const FcudaConvParam* param, int algo, float* output, const float* input,
+                            const float* packed_kernel, float* scratch, const float* bias, const FcudaConvOptions* options,
+                            int batch, void* stream);
+
+/* fcuda_conv_forward_opts with only clip_min / clip_max set; -200 unless param->activation == FCUDA_ACT_CLIP. */
 int fcuda_conv_forward_clip(const FcudaConvParam* param, int algo, float* output, const float* input,
                             const float* packed_kernel, float* scratch, const float* bias, float clip_min, float clip_max,
                             int batch, void* stream);
@@ -173,20 +201,13 @@ int fcuda_dropout_forward(float* output, const float* input, size_t n, float sca
 int fcuda_copy_channels(float* dst, int dst_channels, int dst_channel_offset, const float* src, int channels,
                         size_t stride, int batch, void* stream);
 
-/* Convolution with a fused Eltwise SUM (+ReLU): output = act(conv(input) [+bias] + residual), `residual` shaped like the
- * output.  Replaces ConvLayer::Forward followed by EltwiseLayer::Forward (src/layers/eltwise_layer.h:68-82 ->
- * booster::add_relu<>) when the Eltwise is the only reader of the convolution's top (ResNet shortcuts).  SGECONV adds the
- * residual in its epilogue; every other algorithm runs the convolution and then add_relu in place.  The convolution's
- * own activation (param->activation) is applied before the sum, relu_after_add after it. */
+/* fcuda_conv_forward_opts with only residual / relu_after_add set; -100 for a NULL residual. */
 int fcuda_conv_forward_residual(const FcudaConvParam* param, int algo, float* output, const float* input,
                                 const float* packed_kernel, float* scratch, const float* bias, const float* residual,
                                 int relu_after_add, int batch, void* stream);
 
-/* Convolution (+bias, +ReLU per param->activation) with a FOLLOWING 2x2 / stride-2 / pad-0 max pooling fused into its
- * epilogue (ConvLayer::Forward then PoolingLayer::Forward, src/layers/pooling_layer.h:38-91): `output` is the pooled blob
- * (batch, OC, (OH+1)/2, (OW+1)/2) — ceil mode, windows clipped at the border like the reference.  fcuda_conv_can_pool
- * says whether the algorithm can do it (Winograd F(6,3)/F(2,3): the output tile is pooled in registers; FCUDA_SGECONV:
- * 3x3 / stride-1 layers with IC % 32 == 0, pooled by two shuffles per value); otherwise the call returns -200. */
+/* Whether the algorithm can apply FcudaConvOptions::pool in its epilogue (Winograd F(6,3)/F(2,3): the output tile is pooled
+ * in registers; FCUDA_SGECONV: 3x3 / stride-1 layers with IC % 32 == 0, pooled by two shuffles per value). */
 int fcuda_conv_can_pool(const FcudaConvParam* param, int algo);
 
 /* FCUDA_SGECONV in the current arithmetic mode: 1 when the layer (output_h / output_w assigned) runs on the halo kernel
@@ -203,6 +224,7 @@ int fcuda_igemm_presplit_tile(const FcudaConvParam* param, int* geom);
  * 1 with geom[0..3] = tile rows (28), tile columns (16 for a 64-channel N tile, 8 for 128), fp32 box rows, box columns;
  * 0 otherwise.  The switches themselves are not consulted. */
 int fcuda_igemm_wide_tile(const FcudaConvParam* param, int* geom);
+/* fcuda_conv_forward_opts with only pool set. */
 int fcuda_conv_forward_pool(const FcudaConvParam* param, int algo, float* output, const float* input,
                             const float* packed_kernel, float* scratch, const float* bias, int batch, void* stream);
 
@@ -219,13 +241,11 @@ int fcuda_pixel_channels(int type, int* src_channels, int* out_channels);
 int fcuda_from_pixels(float* output, const unsigned char* pixels, int type, int w, int h, int target_w, int target_h,
                       const float* mean_vals, const float* norm_vals, int batch, void* stream);
 
-/* Extended forward (beyond the reference, which rejects both: dilation at src/layers/conv_layer.h:43-47, partial groups at
- * avx/booster.cpp:304-308).  Same as fcuda_conv_forward[_residual] (`residual` may be NULL) plus a tap spacing.
- *   dilation: FCUDA_SGECONV only (-200 otherwise); the caller sets param->output_h/w for the dilated extent
- *             out = (in + pads - dilation*(k-1) - 1) / stride + 1.
- *   groups  : with FCUDA_SGECONV and param->group > 1 (also through the plain entry points) input_channels and
- *             output_channels are the TOTAL channel counts, the raw kernel is (OC, IC/group, KH, KW) and group g
- *             maps input channels [g*IC/G, (g+1)*IC/G) to output channels [g*OC/G, (g+1)*OC/G). */
+/* fcuda_conv_forward_opts with only residual / relu_after_add (`residual` may be NULL) and the dilations set; -100 for a
+ * dilation < 1.
+ * Groups (the reference rejects partial groups, avx/booster.cpp:304-308): with FCUDA_SGECONV and param->group > 1, through
+ * every entry point, input_channels and output_channels are the TOTAL channel counts, the raw kernel is
+ * (OC, IC/group, KH, KW) and group g maps input channels [g*IC/G, (g+1)*IC/G) to output channels [g*OC/G, (g+1)*OC/G). */
 int fcuda_conv_forward_ext(const FcudaConvParam* param, int algo, float* output, const float* input,
                            const float* packed_kernel, float* scratch, const float* bias, const float* residual,
                            int relu_after_add, int dilation_h, int dilation_w, int batch, void* stream);

@@ -12,7 +12,7 @@ namespace booster {
 inline namespace b200 {  // ABI tag: keeps these symbols apart from the reference build when both are loaded
 
 enum ConvAlgo { NAIVE, IM2COL, SGECONV, DEPTHWISE, WINOGRADF63, WINOGRADF63FUSED, WINOGRADF23 };
-enum ActivationType { None, ReLU, Clip };  // Clip == FCUDA_ACT_CLIP: bounds passed to ForwardClip
+enum ActivationType { None, ReLU, Clip };  // Clip == FCUDA_ACT_CLIP: bounds passed to ForwardOpts / ForwardClip
 
 struct ConvParam : FcudaConvParam {
     ConvParam() { *static_cast<FcudaConvParam*>(this) = FcudaConvParam(); }
@@ -53,6 +53,11 @@ public:
     int Forward(ConvParam* param, float* output, const float* input, const float* kernel, float* buffer,
                 const float* bias_arr, int batch = 1, void* stream = nullptr) const {
         return fcuda_conv_forward(param, algo, output, input, kernel, buffer, bias_arr, batch, stream);
+    }
+    // Forward with everything the epilogue can fuse (fcuda.h, FcudaConvOptions); the two below carry one option each
+    int ForwardOpts(ConvParam* param, float* output, const float* input, const float* kernel, float* buffer,
+                    const float* bias_arr, const FcudaConvOptions& options, int batch = 1, void* stream = nullptr) const {
+        return fcuda_conv_forward_opts(param, algo, output, input, kernel, buffer, bias_arr, &options, batch, stream);
     }
     // Forward + fused Eltwise SUM (+ReLU) of `residual` (same shape as the output)
     int ForwardResidual(ConvParam* param, float* output, const float* input, const float* kernel, float* buffer,

@@ -74,7 +74,8 @@ static int run_case(const Case& c, int planes, bool bench) {
     CK(cudaMemcpy(dAh, A.data(), nA * 4, cudaMemcpyHostToDevice));  // A goes in as plain fp32
     p.A = dAh; p.B_hi = dBh; p.B_lo = dBl; p.D = dD;
     p.M = c.M; p.N = c.N; p.K = c.K; p.G = c.G; p.planes = planes; p.epilogue = c.epi; p.ldd = ldd;
-    p.P = c.P; p.bias = (c.epi == EPI_NCHW) ? dbias : nullptr; p.relu = (c.epi == EPI_NCHW) ? 1 : 0;
+    p.P = c.P;
+    if (c.epi == EPI_NCHW) p.epi = conv_epilogue(/*activation=*/1, true, dbias, 0.f, 0.f, nullptr, 0, 0);  // bias + ReLU
     p.split_k = c.split_k;
     p.split_stride = (long long)nD;
     int rc = tensor_gemm(p, 0);
