@@ -179,12 +179,12 @@ decode_kernel(float* __restrict__ boxes, const float* __restrict__ loc, const fl
     b[3] = __fadd_rn(cy, __fmul_rn(h, 0.5f));
 }
 
+// -0 takes the image of +0: the two are equal scores, ordered by class and prior like any other tie.  So the image does
+// not give back the score's bits; the output row reads the score from conf.
 __device__ __forceinline__ uint32_t orderable(float f) {
-    const uint32_t b = __float_as_uint(f);
+    uint32_t b = __float_as_uint(f);
+    if (b == 0x80000000u) b = 0u;
     return (b & 0x80000000u) ? ~b : (b | 0x80000000u);
-}
-__device__ __forceinline__ float from_orderable(uint32_t u) {
-    return __uint_as_float((u & 0x80000000u) ? (u & 0x7fffffffu) : ~u);
 }
 __device__ __forceinline__ unsigned long long make_key(uint32_t u, int i) {
     return (static_cast<unsigned long long>(u) << 32) | (0xffffffffu - static_cast<uint32_t>(i));
@@ -365,8 +365,9 @@ nms_class_kernel(const float* __restrict__ conf, const float* __restrict__ boxes
 }
 
 __global__ void __launch_bounds__(kDetThreads)
-merge_kernel(float* __restrict__ out, const float* __restrict__ boxes, const unsigned long long* __restrict__ kept,
-             const int* __restrict__ kept_count, int P, int C, int top_k, int keep_top_k) {
+merge_kernel(float* __restrict__ out, const float* __restrict__ conf, const float* __restrict__ boxes,
+             const unsigned long long* __restrict__ kept, const int* __restrict__ kept_count, int P, int C, int top_k,
+             int keep_top_k) {
     __shared__ SelectSmem sm;
     const int n = blockIdx.x;
     const unsigned long long* lists = kept + static_cast<size_t>(n) * C * top_k;
@@ -384,10 +385,10 @@ merge_kernel(float* __restrict__ out, const float* __restrict__ boxes, const uns
         float* row = o + static_cast<size_t>(r) * 6;
         if (r < m) {
             const int v = key_index(sm.keys[r]);
-            const unsigned long long k = lists[v];
-            const float* b = ib + static_cast<size_t>(key_index(k)) * 4;
-            row[0] = static_cast<float>(v / top_k);
-            row[1] = from_orderable(static_cast<uint32_t>(k >> 32));
+            const int c = v / top_k, prior = key_index(lists[v]);
+            const float* b = ib + static_cast<size_t>(prior) * 4;
+            row[0] = static_cast<float>(c);
+            row[1] = conf[(static_cast<size_t>(n) * P + prior) * C + c];
             row[2] = b[0];
             row[3] = b[1];
             row[4] = b[2];
@@ -497,8 +498,8 @@ int detection_output(float* out, const float* loc, const float* conf, const floa
     prof_end(prof, s);
     count_launch();
     prof = prof_begin(s, PROF_DETECTION, 0, 0, 24.0 * batch * keep_top_k);
-    merge_kernel<<<static_cast<unsigned>(batch), kDetThreads, 0, s>>>(out, w.boxes, w.kept, w.counts, P, C, nms_top_k,
-                                                                       keep_top_k);
+    merge_kernel<<<static_cast<unsigned>(batch), kDetThreads, 0, s>>>(out, conf, w.boxes, w.kept, w.counts, P, C,
+                                                                       nms_top_k, keep_top_k);
     FCUDA_CHECK_LAUNCH();
     prof_end(prof, s);
     count_launch();

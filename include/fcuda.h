@@ -374,7 +374,8 @@ int fcuda_ssd_decode(float* boxes, const float* loc, const float* priors, int nu
  *   union  = (area_b + area_a) - inter
  *   IoU    = inter / union                       a NaN IoU (0 / 0 of two empty boxes) suppresses nothing.
  * The kept boxes of all classes are merged, ordered by (score descending, class ascending, prior ascending), and the first
- * keep_top_k written.  output: (batch, keep_top_k, 6) rows [label, score, xmin, ymin, xmax, ymax] with the boxes of
+ * keep_top_k written.  Scores compare as floats: -0 and +0 are equal (ordered by class, then prior), and the row carries
+ * the score's own bits.  output: (batch, keep_top_k, 6) rows [label, score, xmin, ymin, xmax, ymax] with the boxes of
  * fcuda_ssd_decode; rows past an image's count are [-1, 0, 0, 0, 0, 0].
  * Limits (else -200): 1 <= nms_top_k <= 1024, 1 <= keep_top_k <= 1024, 1 <= C <= 1024, 1 <= P < 2^24, batch <= 65535,
  * nms_threshold not NaN.  `workspace` holds fcuda_detection_output_workspace_size floats, 8-byte aligned (else -100). */

@@ -15,7 +15,7 @@
     8 U (|pcx| + |pw| (1 + |var0 l0|) + |p0| + |p2|) + (6 + |var2 l2|) U w / 2 + U |box| per coordinate.
   - DetectionOutput decision by decision against test_ssd_host.detection_ref fed the boxes of fcuda_ssd_decode, bit for
     bit, over: no candidates, every score above the threshold at P = 8732 and C = 81, nms_top_k / keep_top_k truncation,
-    exact score ties, zero-area boxes and one survivor per class.  Each case (but the first) asserts suppression happened.
+    exact score ties, zero-area boxes, one survivor per class and -0 / +0 scores under a negative threshold.  Each case (but the first) asserts suppression happened.
   - Batch independence, and modelgen's MobileNet-SSD end to end with fusion and CUDA graphs on and off: the backbone per
     layer within test_gpu_net_bounds's bounds, every head blob against the checks above from the net's own blobs, and the
     detections bit-identical with CUDA graphs on and off.  Fusion folds BatchNorm / Scale into the convolution weights,
@@ -255,10 +255,17 @@ def _case(name, rng):
         pri = np.tile(_random_priors(rng, 1).reshape(2, 1, 4), (1, P, 1)).reshape(2, -1)
         return (np.zeros((2, 4 * P), np.float32), rng.uniform(0.3, 1.0, (2, P * C)).astype(np.float32), pri, C, 0.2,
                 0.5, 200, 100)
+    if name == "signed_zero":
+        # -0 and +0 scores above a negative threshold are equal: ordered by prior within a class and by class in the
+        # merge, and each row keeps its score's sign; duplicated priors give suppression
+        P, C = 64, 3
+        conf = np.float32([-0.0, 0.0, -0.25])[rng.integers(0, 3, (2, P * C))]
+        pri = np.tile(_random_priors(rng, 16).reshape(2, 16, 4), (1, 4, 1)).reshape(2, -1)
+        return (np.zeros((2, 4 * P), np.float32), conf, pri, C, -0.5, 0.45, 40, 60)
     raise AssertionError(name)
 
 
-DET_CASES = ["no_candidates", "all_above_8732x81", "truncation", "ties", "zero_area", "one_survivor"]
+DET_CASES = ["no_candidates", "all_above_8732x81", "truncation", "ties", "zero_area", "one_survivor", "signed_zero"]
 
 
 @gpu
