@@ -80,6 +80,16 @@ class FcudaPriorBoxParam(ctypes.Structure):
                  ("offset", ctypes.c_float)])
 
 
+class FcudaYoloParam(ctypes.Structure):
+    """include/fcuda.h FcudaYoloParam (up to 4 scales of 16 boxes, 128 bias floats)."""
+
+    _fields_ = ([(n, ctypes.c_int) for n in "version num_class num_box num_scales".split()] +
+                [("confidence_threshold", ctypes.c_float), ("nms_threshold", ctypes.c_float), ("nms_top_k", ctypes.c_int),
+                 ("keep_top_k", ctypes.c_int), ("num_biases", ctypes.c_int), ("biases", ctypes.c_float * 128),
+                 ("mask", ctypes.c_int * 64), ("anchors_scale", ctypes.c_float * 4), ("grid_h", ctypes.c_int * 4),
+                 ("grid_w", ctypes.c_int * 4)])
+
+
 def fcuda() -> ctypes.CDLL:
     global _fcuda
     if _fcuda is None:
@@ -90,6 +100,7 @@ def fcuda() -> ctypes.CDLL:
         D = ctypes.POINTER(FcudaDeconvParam)
         R = ctypes.POINTER(FcudaInterpParam)
         PB = ctypes.POINTER(FcudaPriorBoxParam)
+        Y = ctypes.POINTER(FcudaYoloParam)
         f = ctypes.c_float
         sigs = {
             "fcuda_permute_forward": (i, [vp, vp, i, i, i, i, i, vp]),
@@ -99,6 +110,9 @@ def fcuda() -> ctypes.CDLL:
             "fcuda_ssd_decode": (i, [vp, vp, vp, i, i, vp]),
             "fcuda_detection_output_workspace_size": (i, [i, i, i, i, szp]),
             "fcuda_detection_output_forward": (i, [vp, vp, vp, vp, i, i, f, f, i, i, vp, i, vp]),
+            "fcuda_yolo_decode": (i, [vp, vp, vp, vp, Y, i, vp]),
+            "fcuda_yolo_detection_workspace_size": (i, [Y, i, szp]),
+            "fcuda_yolo_detection_forward": (i, [vp, vp, Y, vp, i, vp]),
             "fcuda_interp_output_dim": (i, [R]),
             "fcuda_interp_forward": (i, [R, vp, vp, i, i, vp]),
             "fcuda_crop_forward": (i, [vp, vp] + [i] * 10 + [vp]),

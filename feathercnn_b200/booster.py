@@ -16,6 +16,7 @@ from ._lib import FcudaConvOptions, FcudaConvParam, fcuda
 from ._lib import FcudaDeconvParam as DeconvParam
 from ._lib import FcudaInterpParam as InterpParam
 from ._lib import FcudaPriorBoxParam as PriorBoxParam
+from ._lib import FcudaYoloParam as YoloParam
 
 NAIVE, IM2COL, SGECONV, DEPTHWISE, WINOGRADF63, WINOGRADF63FUSED, WINOGRADF23 = range(7)
 ALGO_NAMES = ["NAIVE", "IM2COL", "SGECONV", "DEPTHWISE", "WINOGRADF63", "WINOGRADF63FUSED", "WINOGRADF23"]
@@ -336,6 +337,64 @@ def detection_output(loc: torch.Tensor, conf: torch.Tensor, priors: torch.Tensor
            lib.fcuda_detection_output_forward(_ptr(out), _ptr(loc.contiguous()), _ptr(conf.contiguous()),
                                               _ptr(priors.contiguous()), num, num_classes, float(conf_threshold),
                                               float(nms_threshold), nms_top_k, keep_top_k, _ptr(workspace), n, _stream()))
+    return out
+
+
+# ---- YOLO detection head ---------------------------------------------------------------------------
+def yolo_param(version: int, num_class: int, num_box: int, grids, biases, mask=(), anchors_scale=(),
+               confidence_threshold: float = 0.01, nms_threshold: float = 0.45, nms_top_k: int = 1024,
+               keep_top_k: int = 1024) -> YoloParam:
+    """FcudaYoloParam: version 2 (YoloDetectionOutput) or 3 (Yolov3DetectionOutput); grids = [(h, w)] per scale."""
+    p = YoloParam()
+    p.version, p.num_class, p.num_box, p.num_scales = version, num_class, num_box, len(grids)
+    p.confidence_threshold, p.nms_threshold = float(confidence_threshold), float(nms_threshold)
+    p.nms_top_k, p.keep_top_k, p.num_biases = nms_top_k, keep_top_k, len(biases)
+    for dst, src in ((p.biases, biases), (p.mask, mask), (p.anchors_scale, anchors_scale),
+                     (p.grid_h, [g[0] for g in grids]), (p.grid_w, [g[1] for g in grids])):
+        for k, v in enumerate(list(src)[:len(dst)]):
+            dst[k] = v
+    return p
+
+
+def _yolo_inputs(inputs, p: YoloParam):
+    """The inputs as the C side reads them: p.num_scales float32 CUDA tensors of one batch, scale b shaped
+    (N, num_box * (5 + num_class), grid_h[b], grid_w[b])."""
+    xs = [x.contiguous() for x in inputs]
+    assert len(xs) == p.num_scales >= 1, (len(xs), p.num_scales)
+    n = xs[0].shape[0]
+    for b, x in enumerate(xs):
+        want = (n, p.num_box * (5 + p.num_class), p.grid_h[b], p.grid_w[b])
+        assert x.is_cuda and x.dtype == torch.float32 and tuple(x.shape) == want, (b, tuple(x.shape), want)
+    arr = (ctypes.c_void_p * len(xs))(*[x.data_ptr() for x in xs])
+    return xs, arr
+
+
+def yolo_decode(inputs, p: YoloParam):
+    """inputs: one (N, num_box * (5 + C), h, w) tensor per scale -> (scores (N, S), classes (N, S) int32,
+    boxes (N, S, 4)) for every slot S, candidate or not."""
+    xs, arr = _yolo_inputs(inputs, p)
+    n = xs[0].shape[0]
+    slots = sum(p.num_box * x.shape[2] * x.shape[3] for x in xs)
+    scores = torch.empty((n, slots), device=xs[0].device, dtype=torch.float32)
+    classes = torch.empty((n, slots), device=xs[0].device, dtype=torch.int32)
+    boxes = torch.empty((n, slots, 4), device=xs[0].device, dtype=torch.float32)
+    _check("fcuda_yolo_decode", fcuda().fcuda_yolo_decode(_ptr(scores), ctypes.c_void_p(classes.data_ptr()), _ptr(boxes),
+                                                          arr, ctypes.byref(p), n, _stream()))
+    return scores, classes, boxes
+
+
+def yolo_detection(inputs, p: YoloParam) -> torch.Tensor:
+    """inputs as yolo_decode -> (N, keep_top_k, 6) rows [class + 1, confidence, xmin, ymin, xmax, ymax]."""
+    lib = fcuda()
+    xs, arr = _yolo_inputs(inputs, p)
+    n = xs[0].shape[0]
+    ws = ctypes.c_size_t(0)
+    _check("fcuda_yolo_detection_workspace_size", lib.fcuda_yolo_detection_workspace_size(ctypes.byref(p), n,
+                                                                                          ctypes.byref(ws)))
+    workspace = torch.empty(max(ws.value, 1), device=xs[0].device, dtype=torch.float32)
+    out = torch.empty((n, p.keep_top_k, 6), device=xs[0].device, dtype=torch.float32)
+    _check("fcuda_yolo_detection_forward", lib.fcuda_yolo_detection_forward(_ptr(out), arr, ctypes.byref(p),
+                                                                            _ptr(workspace), n, _stream()))
     return out
 
 

@@ -13,6 +13,7 @@
 #include "common.cuh"
 #include "detection.cuh"
 
+#include <float.h>
 #include <math.h>
 #include <stdint.h>
 
@@ -416,6 +417,262 @@ DetWorkspace carve(float* ws, int P, int C, int top_k, int batch) {
     return w;
 }
 
+// ---- YOLO (YoloDetectionOutput, Yolov3DetectionOutput) --------------------------------------------------------------
+// decode  one thread per (image, slot): confidence, class and box of every slot;
+// select  one CTA per image: select_top_k over the candidates (score >= threshold), their sorted keys, boxes and areas;
+// mask    CTAs over (32-row block, image): word w of row i has bit b set iff j = 32 w + b > i and IoU(i, j) > threshold;
+// sweep   one CTA per image: the mask in shared memory, one warp walks the candidates in order (lane l owns the removal
+//         word l: no barrier and no global load in the loop), then the output rows.
+// Switch yolo_nms = 0 replaces mask + sweep by one CTA per image that builds the mask in its own shared memory.
+constexpr int kYoloMaskWords = kMaxTopK / 32;
+constexpr int kYoloMaskRows = 32;  // rows of one mask CTA: 8 warps x 4
+
+// Per-scale geometry, by value: the bottom, its grid, its first slot and, per box, the anchor and its normaliser
+// (version 3: (int)(anchors_scale * w); version 2: the grid side).
+struct YoloScale {
+    const float* in;
+    int h, w, slot0;
+    float norm_w, norm_h;
+    float bias_w[FCUDA_YOLO_MAX_BOXES], bias_h[FCUDA_YOLO_MAX_BOXES];
+};
+struct YoloGeom {
+    int version, num_class, num_box, num_scales, slots;
+    YoloScale scale[FCUDA_YOLO_MAX_SCALES];
+};
+
+__device__ __forceinline__ float sigm(float t) { return __fdiv_rn(1.f, __fadd_rn(1.f, expf(-t))); }
+
+__global__ void __launch_bounds__(256)
+yolo_decode_kernel(float* __restrict__ scores, int* __restrict__ classes, float* __restrict__ boxes, const YoloGeom g,
+                   long long total) {
+    const int stride = 5 + g.num_class;
+    for (long long t = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x; t < total;
+         t += static_cast<long long>(gridDim.x) * blockDim.x) {
+        const long long n = t / g.slots;
+        const int slot = static_cast<int>(t - n * g.slots);
+        int b = 0;
+        while (b + 1 < g.num_scales && slot >= g.scale[b + 1].slot0) ++b;
+        const YoloScale& sc = g.scale[b];
+        const int hw = sc.h * sc.w;
+        const int r = slot - sc.slot0, pp = r / hw, cell = r - pp * hw;
+        const int i = cell / sc.w, j = cell - i * sc.w;
+        const float* p = sc.in + (static_cast<size_t>(n) * g.num_box + pp) * stride * hw + cell;
+        const float tx = p[0], ty = p[static_cast<size_t>(hw)], tw = p[2 * static_cast<size_t>(hw)];
+        const float th = p[3 * static_cast<size_t>(hw)], obj = p[4 * static_cast<size_t>(hw)];
+        const float* logit = p + 5 * static_cast<size_t>(hw);
+        int cls = 0;
+        float conf;
+        if (g.version == 3) {
+            float m = -FLT_MAX;
+            for (int k = 0; k < g.num_class; ++k) {
+                const float v = logit[static_cast<size_t>(k) * hw];
+                if (v > m) {
+                    m = v;
+                    cls = k;
+                }
+            }
+            conf = __fdiv_rn(1.f, __fadd_rn(1.f, __fmul_rn(expf(-obj), __fadd_rn(1.f, expf(-m)))));
+        } else {
+            float m = -FLT_MAX;  // ncnn's Softmax: a NaN logit does not become the max
+            for (int k = 0; k < g.num_class; ++k) m = fmaxf(m, logit[static_cast<size_t>(k) * hw]);
+            float sum = 0.f;
+            for (int k = 0; k < g.num_class; ++k) sum = __fadd_rn(sum, expf(__fsub_rn(logit[static_cast<size_t>(k) * hw], m)));
+            float best = 0.f;
+            for (int k = 0; k < g.num_class; ++k) {
+                const float pk = __fdiv_rn(expf(__fsub_rn(logit[static_cast<size_t>(k) * hw], m)), sum);
+                if (pk > best) {
+                    best = pk;
+                    cls = k;
+                }
+            }
+            conf = __fmul_rn(sigm(obj), best);
+        }
+        const float cx = __fdiv_rn(__fadd_rn(static_cast<float>(j), sigm(tx)), static_cast<float>(sc.w));
+        const float cy = __fdiv_rn(__fadd_rn(static_cast<float>(i), sigm(ty)), static_cast<float>(sc.h));
+        const float bw = __fdiv_rn(__fmul_rn(expf(tw), sc.bias_w[pp]), sc.norm_w);
+        const float bh = __fdiv_rn(__fmul_rn(expf(th), sc.bias_h[pp]), sc.norm_h);
+        scores[t] = conf;
+        classes[t] = cls;
+        float* o = boxes + static_cast<size_t>(t) * 4;
+        o[0] = __fsub_rn(cx, __fmul_rn(bw, 0.5f));
+        o[1] = __fsub_rn(cy, __fmul_rn(bh, 0.5f));
+        o[2] = __fadd_rn(cx, __fmul_rn(bw, 0.5f));
+        o[3] = __fadd_rn(cy, __fmul_rn(bh, 0.5f));
+    }
+}
+
+struct YoloWorkspace {
+    unsigned long long* keys;  // (batch, kMaxTopK)
+    uint32_t* mask;            // (batch, kMaxTopK, kYoloMaskWords)
+    float* sel_box;            // (batch, kMaxTopK, 4)
+    float* sel_area;           // (batch, kMaxTopK)
+    float* boxes;              // (batch, slots, 4)
+    float* scores;             // (batch, slots)
+    int* classes;              // (batch, slots)
+    int* counts;               // (batch)
+};
+
+YoloWorkspace yolo_carve(float* ws, int slots, int batch) {
+    YoloWorkspace w;
+    const size_t n = static_cast<size_t>(batch);
+    w.keys = reinterpret_cast<unsigned long long*>(ws);
+    ws += n * kMaxTopK * 2;
+    w.mask = reinterpret_cast<uint32_t*>(ws);
+    ws += n * kMaxTopK * kYoloMaskWords;
+    w.sel_box = ws;
+    ws += n * kMaxTopK * 4;
+    w.sel_area = ws;
+    ws += n * kMaxTopK;
+    w.boxes = ws;
+    ws += n * slots * 4;
+    w.scores = ws;
+    ws += n * slots;
+    w.classes = reinterpret_cast<int*>(ws);
+    ws += n * slots;
+    w.counts = reinterpret_cast<int*>(ws);
+    return w;
+}
+
+__global__ void __launch_bounds__(kDetThreads)
+yolo_select_kernel(const YoloWorkspace w, int slots, float thr, int top_k) {
+    __shared__ SelectSmem sm;
+    const int n = blockIdx.x;
+    const float* sc = w.scores + static_cast<size_t>(n) * slots;
+    const int m = select_top_k(slots, top_k, [&](int i, uint32_t& u) {
+        const float s = sc[i];
+        u = orderable(s);
+        return s >= thr;
+    }, sm);
+    const float* ib = w.boxes + static_cast<size_t>(n) * slots * 4;
+    for (int j = threadIdx.x; j < m; j += kDetThreads) {
+        const unsigned long long key = sm.keys[j];
+        const float* b = ib + static_cast<size_t>(key_index(key)) * 4;
+        float* o = w.sel_box + (static_cast<size_t>(n) * kMaxTopK + j) * 4;
+#pragma unroll
+        for (int q = 0; q < 4; ++q) o[q] = b[q];
+        w.sel_area[static_cast<size_t>(n) * kMaxTopK + j] = __fmul_rn(__fsub_rn(b[2], b[0]), __fsub_rn(b[3], b[1]));
+        w.keys[static_cast<size_t>(n) * kMaxTopK + j] = key;
+    }
+    if (threadIdx.x == 0) w.counts[n] = m;
+}
+
+// Row i of the suppression mask over m candidates staged in sb / sarea: every lane of the warp calls it and gets word
+// `lane` (bit b set iff j = 32 lane + b > i and IoU(i, j) > nms_thr).
+__device__ __forceinline__ uint32_t yolo_mask_row(int i, int m, const float (*sb)[4], const float* sarea, float nms_thr,
+                                                  int lane) {
+    uint32_t mine = 0;
+    const int words = (m + 31) >> 5;
+    for (int wd = i >> 5; wd < words; ++wd) {
+        const int j = (wd << 5) + lane;
+        const bool hit = j > i && j < m && box_iou(sb[i], sarea[i], sb[j], sarea[j]) > nms_thr;
+        const uint32_t bits = __ballot_sync(0xffffffffu, hit);
+        if (lane == wd) mine = bits;
+    }
+    return mine;
+}
+
+// Stage the selected boxes and areas j in [from, m) of image n.  The caller synchronises.
+__device__ __forceinline__ void yolo_stage_boxes(const YoloWorkspace& w, int n, int from, int m, float (*sb)[4],
+                                                 float* sarea) {
+    const float* gb = w.sel_box + static_cast<size_t>(n) * kMaxTopK * 4;
+    const float* ga = w.sel_area + static_cast<size_t>(n) * kMaxTopK;
+    for (int j = from + threadIdx.x; j < m; j += blockDim.x) {
+#pragma unroll
+        for (int q = 0; q < 4; ++q) sb[j][q] = gb[static_cast<size_t>(j) * 4 + q];
+        sarea[j] = ga[j];
+    }
+}
+
+// The greedy walk over the shared-memory mask (m rows of kYoloMaskWords words) and the output rows of image n.  One warp
+// walks the candidates in order, lane l owning removal word l: no barrier and no global load in the loop; it stops at
+// keep_top_k kept boxes.  Every thread of the CTA calls it.
+__device__ __forceinline__ void yolo_sweep_rows(float* __restrict__ out, const YoloWorkspace& w, int n, int m, int slots,
+                                                int keep_top_k, const uint32_t* smask, int* keep, int* kept_count) {
+    if (threadIdx.x < 32) {
+        const int lane = threadIdx.x;
+        uint32_t removed = 0;  // lane l: candidates 32 l .. 32 l + 31 suppressed by a kept box
+        int kept = 0;
+        for (int i = 0; i < m && kept < keep_top_k; ++i) {
+            const uint32_t word = __shfl_sync(0xffffffffu, removed, i >> 5);
+            if (!((word >> (i & 31)) & 1u)) {  // uniform over the warp
+                if (lane == 0) keep[kept] = i;
+                ++kept;
+                removed |= smask[i * kYoloMaskWords + lane];
+            }
+        }
+        if (lane == 0) *kept_count = kept;
+    }
+    __syncthreads();
+    const int kept = *kept_count;
+    const unsigned long long* keys = w.keys + static_cast<size_t>(n) * kMaxTopK;
+    const float* sel = w.sel_box + static_cast<size_t>(n) * kMaxTopK * 4;
+    float* o = out + static_cast<size_t>(n) * keep_top_k * 6;
+    for (int r = threadIdx.x; r < keep_top_k; r += blockDim.x) {
+        float* row = o + static_cast<size_t>(r) * 6;
+        if (r < kept) {
+            const int c = keep[r];
+            const size_t slot = static_cast<size_t>(n) * slots + key_index(keys[c]);
+            row[0] = static_cast<float>(w.classes[slot] + 1);
+            row[1] = w.scores[slot];
+#pragma unroll
+            for (int q = 0; q < 4; ++q) row[2 + q] = sel[static_cast<size_t>(c) * 4 + q];
+        } else {
+            row[0] = -1.f;
+            row[1] = row[2] = row[3] = row[4] = row[5] = 0.f;
+        }
+    }
+}
+
+// Split NMS, first half: CTAs over (32-row block, image) write the mask to the workspace.
+__global__ void __launch_bounds__(256)
+yolo_mask_kernel(const YoloWorkspace w, float nms_thr) {
+    __shared__ float sb[kMaxTopK][4];
+    __shared__ float sarea[kMaxTopK];
+    const int n = blockIdx.y, row0 = blockIdx.x * kYoloMaskRows;
+    const int m = w.counts[n];
+    if (row0 >= m) return;
+    yolo_stage_boxes(w, n, row0, m, sb, sarea);  // only columns >= row0 can be set
+    __syncthreads();
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    uint32_t* out = w.mask + static_cast<size_t>(n) * kMaxTopK * kYoloMaskWords;
+    for (int i = row0 + warp; i < row0 + kYoloMaskRows && i < m; i += 8)
+        out[static_cast<size_t>(i) * kYoloMaskWords + lane] = yolo_mask_row(i, m, sb, sarea, nms_thr, lane);
+}
+
+// Split NMS, second half: one CTA per image stages the mask (16-byte loads: the workspace is 16-byte aligned and every
+// offset into it is a multiple of 16 bytes) and sweeps it.
+__global__ void __launch_bounds__(kDetThreads)
+yolo_sweep_kernel(float* __restrict__ out, const YoloWorkspace w, int slots, int keep_top_k) {
+    extern __shared__ uint4 yolo_smem[];
+    __shared__ int keep[kMaxTopK];
+    __shared__ int kept_count;
+    const int n = blockIdx.x;
+    const int m = w.counts[n];
+    const uint4* gm = reinterpret_cast<const uint4*>(w.mask + static_cast<size_t>(n) * kMaxTopK * kYoloMaskWords);
+    for (int v = threadIdx.x; v < m * (kYoloMaskWords / 4); v += kDetThreads) yolo_smem[v] = gm[v];
+    __syncthreads();
+    yolo_sweep_rows(out, w, n, m, slots, keep_top_k, reinterpret_cast<const uint32_t*>(yolo_smem), keep, &kept_count);
+}
+
+// Single-CTA NMS (switch yolo_nms = 0): one CTA per image builds the whole mask in shared memory, then sweeps it.
+__global__ void __launch_bounds__(kDetThreads)
+yolo_nms_fused_kernel(float* __restrict__ out, const YoloWorkspace w, int slots, float nms_thr, int keep_top_k) {
+    extern __shared__ uint4 yolo_smem[];
+    uint32_t* smask = reinterpret_cast<uint32_t*>(yolo_smem);
+    __shared__ float sb[kMaxTopK][4];
+    __shared__ float sarea[kMaxTopK];
+    __shared__ int keep[kMaxTopK];
+    __shared__ int kept_count;
+    const int n = blockIdx.x;
+    const int m = w.counts[n];
+    yolo_stage_boxes(w, n, 0, m, sb, sarea);
+    __syncthreads();
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    for (int i = warp; i < m; i += kDetWarps) smask[i * kYoloMaskWords + lane] = yolo_mask_row(i, m, sb, sarea, nms_thr, lane);
+    __syncthreads();
+    yolo_sweep_rows(out, w, n, m, slots, keep_top_k, smask, keep, &kept_count);
+}
+
 }  // namespace
 
 int permute_forward(const float* in, float* out, int c, int h, int w, int order, int batch, cudaStream_t s) {
@@ -500,6 +757,107 @@ int detection_output(float* out, const float* loc, const float* conf, const floa
     prof = prof_begin(s, PROF_DETECTION, 0, 0, 24.0 * batch * keep_top_k);
     merge_kernel<<<static_cast<unsigned>(batch), kDetThreads, 0, s>>>(out, conf, w.boxes, w.kept, w.counts, P, C,
                                                                        nms_top_k, keep_top_k);
+    FCUDA_CHECK_LAUNCH();
+    prof_end(prof, s);
+    count_launch();
+    return 0;
+}
+
+namespace {
+
+YoloGeom yolo_geom(const float* const* inputs, const FcudaYoloParam& p) {
+    YoloGeom g{};
+    g.version = p.version;
+    g.num_class = p.num_class;
+    g.num_box = p.num_box;
+    g.num_scales = p.num_scales;
+    int slot0 = 0;
+    for (int b = 0; b < p.num_scales; ++b) {
+        YoloScale& sc = g.scale[b];
+        sc.in = inputs[b];
+        sc.h = p.grid_h[b];
+        sc.w = p.grid_w[b];
+        sc.slot0 = slot0;
+        slot0 += p.num_box * sc.h * sc.w;
+        if (p.version == 3) {
+            sc.norm_w = static_cast<float>(static_cast<int>(p.anchors_scale[b] * static_cast<float>(sc.w)));
+            sc.norm_h = static_cast<float>(static_cast<int>(p.anchors_scale[b] * static_cast<float>(sc.h)));
+        } else {
+            sc.norm_w = static_cast<float>(sc.w);
+            sc.norm_h = static_cast<float>(sc.h);
+        }
+        for (int pp = 0; pp < p.num_box; ++pp) {
+            const int k = p.version == 3 ? p.mask[b * p.num_box + pp] : pp;
+            sc.bias_w[pp] = p.biases[2 * k];
+            sc.bias_h[pp] = p.biases[2 * k + 1];
+        }
+    }
+    g.slots = slot0;
+    return g;
+}
+
+int yolo_decode_launch(float* scores, int* classes, float* boxes, const YoloGeom& g, int batch, cudaStream_t s) {
+    const long long total = static_cast<long long>(batch) * g.slots;
+    const int prof = prof_begin(s, PROF_DETECTION, 0, 0, 4.0 * (5 + g.num_class) * total + 24.0 * total);
+    const long long blocks = (total + 255) / 256;
+    yolo_decode_kernel<<<static_cast<unsigned>(blocks < 65536 * 16 ? blocks : 65536 * 16), 256, 0, s>>>(scores, classes,
+                                                                                                        boxes, g, total);
+    FCUDA_CHECK_LAUNCH();
+    prof_end(prof, s);
+    count_launch();
+    return 0;
+}
+
+SmemAttrCache yolo_sweep_smem, yolo_fused_smem;
+
+}  // namespace
+
+int yolo_decode(float* scores, int* classes, float* boxes, const float* const* inputs, const FcudaYoloParam& p, int batch,
+                cudaStream_t s) {
+    return yolo_decode_launch(scores, classes, boxes, yolo_geom(inputs, p), batch, s);
+}
+
+size_t yolo_detection_workspace(int slots, int batch) {
+    return static_cast<size_t>(batch) * (6 * static_cast<size_t>(slots) + 2 * kMaxTopK + kMaxTopK * kYoloMaskWords +
+                                         5 * kMaxTopK + 1);
+}
+
+int yolo_detection(float* out, const float* const* inputs, const FcudaYoloParam& p, float* workspace, int batch,
+                   cudaStream_t s) {
+    const YoloGeom g = yolo_geom(inputs, p);
+    const YoloWorkspace w = yolo_carve(workspace, g.slots, batch);
+    int rc = yolo_decode_launch(w.scores, w.classes, w.boxes, g, batch, s);
+    if (rc) return rc;
+    const double slots = static_cast<double>(batch) * g.slots;
+    int prof = prof_begin(s, PROF_DETECTION, 0, 0, 4.0 * slots + 24.0 * batch * p.nms_top_k);
+    yolo_select_kernel<<<static_cast<unsigned>(batch), kDetThreads, 0, s>>>(w, g.slots, p.confidence_threshold,
+                                                                             p.nms_top_k);
+    FCUDA_CHECK_LAUNCH();
+    prof_end(prof, s);
+    count_launch();
+    const int smem = p.nms_top_k * kYoloMaskWords * static_cast<int>(sizeof(uint32_t));
+    if (!tune_get(TUNE_YOLO_NMS)) {
+        rc = ensure_dynamic_smem(yolo_nms_fused_kernel, smem, yolo_fused_smem);
+        if (rc) return rc;
+        prof = prof_begin(s, PROF_DETECTION, 0, 0, 20.0 * batch * p.nms_top_k + 24.0 * batch * p.keep_top_k);
+        yolo_nms_fused_kernel<<<static_cast<unsigned>(batch), kDetThreads, smem, s>>>(out, w, g.slots, p.nms_threshold,
+                                                                                       p.keep_top_k);
+        FCUDA_CHECK_LAUNCH();
+        prof_end(prof, s);
+        count_launch();
+        return 0;
+    }
+    const int row_blocks = ceil_div(p.nms_top_k, kYoloMaskRows);
+    prof = prof_begin(s, PROF_DETECTION, 0, 0, 20.0 * batch * p.nms_top_k + 4.0 * batch * p.nms_top_k * kYoloMaskWords);
+    yolo_mask_kernel<<<dim3(static_cast<unsigned>(row_blocks), static_cast<unsigned>(batch)), 256, 0, s>>>(w,
+                                                                                                        p.nms_threshold);
+    FCUDA_CHECK_LAUNCH();
+    prof_end(prof, s);
+    count_launch();
+    rc = ensure_dynamic_smem(yolo_sweep_kernel, smem, yolo_sweep_smem);
+    if (rc) return rc;
+    prof = prof_begin(s, PROF_DETECTION, 0, 0, 4.0 * batch * p.nms_top_k * kYoloMaskWords + 24.0 * batch * p.keep_top_k);
+    yolo_sweep_kernel<<<static_cast<unsigned>(batch), kDetThreads, smem, s>>>(out, w, g.slots, p.keep_top_k);
     FCUDA_CHECK_LAUNCH();
     prof_end(prof, s);
     count_launch();

@@ -19,4 +19,12 @@ size_t detection_output_workspace(int num_priors, int num_classes, int nms_top_k
 int detection_output(float* out, const float* loc, const float* conf, const float* priors, int num_priors, int num_classes,
                      float conf_threshold, float nms_threshold, int nms_top_k, int keep_top_k, float* workspace, int batch,
                      cudaStream_t s);
+// YOLO head (include/fcuda.h, FcudaYoloParam); the parameters are checked by the caller.
+int yolo_decode(float* scores, int* classes, float* boxes, const float* const* inputs, const FcudaYoloParam& p, int batch,
+                cudaStream_t s);
+// Workspace (floats) of yolo_detection.
+size_t yolo_detection_workspace(int slots, int batch);
+// decode, select, suppression mask, sweep: four launches.
+int yolo_detection(float* out, const float* const* inputs, const FcudaYoloParam& p, float* workspace, int batch,
+                   cudaStream_t s);
 }  // namespace fcuda

@@ -105,6 +105,36 @@ int detection_limits(int P, int C, int nms_top_k, int batch) {
     return 0;
 }
 
+// Limits of the YOLO head (include/fcuda.h, FcudaYoloParam): -100 / -200, and the slot count when both pass.
+int yolo_limits(const FcudaYoloParam* p, int batch, int* slots) {
+    if (!p) return -100;
+    const bool v3 = p->version == 3;
+    if ((p->version != 2 && !v3) || p->num_class < 1 || p->num_class > 1024 || p->num_box < 1 ||
+        p->num_box > FCUDA_YOLO_MAX_BOXES || p->num_scales < 1 || p->num_scales > (v3 ? FCUDA_YOLO_MAX_SCALES : 1) ||
+        p->num_biases < 0 || p->num_biases > FCUDA_YOLO_MAX_BIASES || (!v3 && p->num_biases < 2 * p->num_box) ||
+        p->nms_top_k < 1 || p->nms_top_k > 1024 || p->keep_top_k < 1 || p->keep_top_k > 1024 || isnan(p->nms_threshold))
+        return -200;
+    if (v3) {
+        for (int k = 0; k < p->num_scales * p->num_box; ++k)
+            if (p->mask[k] < 0 || p->mask[k] >= p->num_biases / 2) return -200;
+        for (int b = 0; b < p->num_scales; ++b)
+            if (!(p->anchors_scale[b] > 0.f)) return -200;
+    }
+    if (batch < 1) return -100;
+    if (batch > 65535) return -200;
+    long long total = 0;
+    for (int b = 0; b < p->num_scales; ++b) {
+        if (p->grid_h[b] < 1 || p->grid_w[b] < 1) return -100;
+        // the fp32 products anchors_scale * side must truncate to an int (NaN and inf fail too)
+        const int side = p->grid_h[b] > p->grid_w[b] ? p->grid_h[b] : p->grid_w[b];
+        if (v3 && !(p->anchors_scale[b] * static_cast<float>(side) < 2147483520.f)) return -200;
+        total += static_cast<long long>(p->num_box) * p->grid_h[b] * p->grid_w[b];
+        if (total >= kMaxPriors) return -200;
+    }
+    *slots = static_cast<int>(total);
+    return 0;
+}
+
 struct ConvPlan {
     int algo = -1;
     int np = 1;  // operand planes (1 = TF32, 2 = 3xTF32)
@@ -853,6 +883,41 @@ int fcuda_detection_output_forward(float* output, const float* loc, const float*
     if (!output || !loc || !conf || !priors || !workspace || (reinterpret_cast<uintptr_t>(workspace) & 7)) return -100;
     return detection_output(output, loc, conf, priors, num_priors, num_classes, conf_threshold, nms_threshold, nms_top_k,
                             keep_top_k, workspace, batch, as_stream(stream));
+}
+
+static bool yolo_inputs_ok(const float* const* inputs, int scales) {
+    if (!inputs) return false;
+    for (int b = 0; b < scales; ++b)
+        if (!inputs[b]) return false;
+    return true;
+}
+
+int fcuda_yolo_decode(float* scores, int* classes, float* boxes, const float* const* inputs, const FcudaYoloParam* param,
+                      int batch, void* stream) {
+    int slots = 0;
+    const int rc = yolo_limits(param, batch, &slots);
+    if (rc) return rc;
+    if (!scores || !classes || !boxes || !yolo_inputs_ok(inputs, param->num_scales)) return -100;
+    return yolo_decode(scores, classes, boxes, inputs, *param, batch, as_stream(stream));
+}
+
+int fcuda_yolo_detection_workspace_size(const FcudaYoloParam* param, int batch, size_t* floats) {
+    if (!floats) return -100;
+    int slots = 0;
+    const int rc = yolo_limits(param, batch, &slots);
+    if (rc) return rc;
+    *floats = yolo_detection_workspace(slots, batch);
+    return 0;
+}
+
+int fcuda_yolo_detection_forward(float* output, const float* const* inputs, const FcudaYoloParam* param, float* workspace,
+                                 int batch, void* stream) {
+    int slots = 0;
+    const int rc = yolo_limits(param, batch, &slots);
+    if (rc) return rc;
+    if (!output || !workspace || (reinterpret_cast<uintptr_t>(workspace) & 15) || !yolo_inputs_ok(inputs, param->num_scales))
+        return -100;
+    return yolo_detection(output, inputs, *param, workspace, batch, as_stream(stream));
 }
 
 int fcuda_pixel_channels(int type, int* src_channels, int* out_channels) { return pixel_channels(type, src_channels, out_channels); }

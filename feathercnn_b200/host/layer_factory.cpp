@@ -1,6 +1,6 @@
 // Built-in layer registrations: the 13 ncnn type names the reference serves (/root/reference/src/layer_factory.cpp:53-68)
-// plus Deconvolution / DeconvolutionDepthWise, Interp, Crop, Clip, PReLU and SSD's Permute, Flatten, Reshape, PriorBox and
-// DetectionOutput, 24 in all, mapped onto this host's layer classes.  A table of {type name, factory} pairs instead of one macro line per layer; the
+// plus Deconvolution / DeconvolutionDepthWise, Interp, Crop, Clip, PReLU, SSD's Permute, Flatten, Reshape, PriorBox and
+// DetectionOutput, and YOLO's YoloDetectionOutput and Yolov3DetectionOutput, 26 in all, mapped onto this host's layer classes.  A table of {type name, factory} pairs instead of one macro line per layer; the
 // DEFINE_LAYER_CREATOR / REGISTER_LAYER_CREATOR macros of <feather/layer_factory.h> remain the plugin API for user layers.
 #include <feather/layer_factory.h>
 
@@ -18,6 +18,7 @@
 #include "layers/relu_layer.h"
 #include "layers/resize_layers.h"
 #include "layers/scale_layer.h"
+#include "layers/yolo_layers.h"
 
 namespace feather {
 inline namespace b200 {  // ABI tag: keeps these symbols apart from the reference build when both are loaded
@@ -61,6 +62,8 @@ const BuiltIn kBuiltIns[] = {
     {"Reshape", make_layer<ReshapeLayer>},
     {"PriorBox", make_layer<PriorBoxLayer>},
     {"DetectionOutput", make_layer<DetectionOutputLayer>},
+    {"YoloDetectionOutput", make_layer<YoloDetectionOutputLayer>},
+    {"Yolov3DetectionOutput", make_layer<Yolov3DetectionOutputLayer>},
 };
 
 }  // namespace

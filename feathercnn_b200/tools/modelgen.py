@@ -6,7 +6,8 @@ weight blobs, raw fp32 for bias/BN/Scale blobs) — /root/reference/src/net.cpp:
 snapshot, and there is no network for pretrained checkpoints, so benchmarks and tests use random-init
 models of the architectures BASELINE.json names: a single 3x3 conv, VGG-16, ResNet-50 (Caffe topology:
 BN + Scale + ReLU as separate layers, Split/Eltwise residuals), MobileNet-v1, MobileNet-v2 (ReLU6 as Clip), plus a small "mini" net
-that exercises every layer type, and single-shot detectors (MobileNet-SSD, a two-head tiny SSD).  Weight statistics follow
+that exercises every layer type, single-shot detectors (MobileNet-SSD, a two-head tiny SSD) and YOLO detectors
+(MobileNet-YOLOv2, MobileNet-v2 YOLOv3, a two-scale tiny YOLOv3).  Weight statistics follow
 SURVEY.md §8(d).
 """
 from __future__ import annotations
@@ -46,7 +47,9 @@ class ModelWriter:
         self.shape = {name: (c, h, w)}
         return name
 
-    def conv(self, name, bottom, oc, k, stride=1, pad=0, bias=True, group=1, top=None, gain=None, dilation=1):
+    def conv(self, name, bottom, oc, k, stride=1, pad=0, bias=True, group=1, top=None, gain=None, dilation=1,
+             bias_values=None):
+        """bias_values: the bias as given instead of uniform(-0.1, 0.1) draws."""
         top = top or name
         ic, h, w = self.shape[bottom]
         icg = ic // group
@@ -61,7 +64,9 @@ class ModelWriter:
             params[2] = dilation
         self._layer(ltype, name, [bottom], [top], params)
         self._weights(wts, True)
-        if bias:
+        if bias and bias_values is not None:
+            self._weights(np.asarray(bias_values, np.float32).reshape(oc), False)
+        elif bias:
             self._weights(self.rng.uniform(-0.1, 0.1, oc).astype(np.float32), False)
         oh = (h + 2 * pad - dilation * (k - 1) - 1) // stride + 1
         ow = (w + 2 * pad - dilation * (k - 1) - 1) // stride + 1
@@ -299,6 +304,39 @@ class ModelWriter:
         self._layer("DetectionOutput", name, [loc, conf, priors], [top],
                     {0: num_classes, 1: f"{nms_threshold:e}", 2: nms_top_k, 3: keep_top_k, 4: f"{conf_threshold:e}"})
         self.shape[top] = (1, keep_top_k, 6)
+        self.rank[top] = 2
+        return top
+
+    def yolo_detection_output(self, name, bottom, num_class, num_box, biases, confidence_threshold=0.01,
+                              nms_threshold=0.45, nms_top_k=None, keep_top_k=None, top=None):
+        """ncnn YoloDetectionOutput (YOLOv2): biases are num_box (w, h) anchor pairs in grid cells; 20= / 21= (nms_top_k /
+        keep_top_k, default 1024) only when given.  Rank-2 (keep_top_k, 6) top."""
+        return self._yolo("YoloDetectionOutput", name, [bottom], num_class, num_box, biases, None, None,
+                          confidence_threshold, nms_threshold, nms_top_k, keep_top_k, top)
+
+    def yolov3_detection_output(self, name, bottoms, num_class, num_box, biases, mask, anchors_scale,
+                                confidence_threshold=0.01, nms_threshold=0.45, nms_top_k=None, keep_top_k=None, top=None):
+        """ncnn Yolov3DetectionOutput: one bottom per scale; biases are anchor (w, h) pairs in input pixels, mask the anchor
+        index of each (scale, box), anchors_scale the stride of each scale."""
+        return self._yolo("Yolov3DetectionOutput", name, list(bottoms), num_class, num_box, biases, mask, anchors_scale,
+                          confidence_threshold, nms_threshold, nms_top_k, keep_top_k, top)
+
+    def _yolo(self, type_, name, bottoms, num_class, num_box, biases, mask, anchors_scale, confidence_threshold,
+              nms_threshold, nms_top_k, keep_top_k, top):
+        top = top or name
+        for b in bottoms:
+            assert self.shape[b][0] == num_box * (5 + num_class), (name, b, self.shape[b])
+        params = {0: num_class, 1: num_box, 2: f"{confidence_threshold:e}", 3: f"{nms_threshold:e}",
+                  -23304: self._floats(biases)}
+        if mask is not None:
+            params[-23305] = self._floats(mask)
+            params[-23306] = self._floats(anchors_scale)
+        if nms_top_k is not None:
+            params[20] = nms_top_k
+        if keep_top_k is not None:
+            params[21] = keep_top_k
+        self._layer(type_, name, bottoms, [top], params)
+        self.shape[top] = (1, keep_top_k or 1024, 6)
         self.rank[top] = 2
         return top
 
@@ -668,9 +706,112 @@ def ssd_tiny(seed=0, size=64, num_classes=5, conf_threshold=0.05, conf_gain=3.0)
     return m
 
 
+VOC_ANCHORS = [1.08, 1.19, 3.42, 4.41, 6.63, 11.38, 9.42, 5.11, 16.62, 10.52]  # YOLOv2 VOC, grid cells
+COCO_ANCHORS = [10, 13, 16, 30, 33, 23, 30, 61, 62, 45, 59, 119, 116, 90, 156, 198, 373, 326]  # YOLOv3, input pixels
+
+
+def _yolo_out(m: ModelWriter, name: str, x: str, num_box: int, num_class: int, head_gain: float, obj_bias: float) -> str:
+    """The 1x1 output convolution of a YOLO head: num_box * (5 + num_class) channels, weights head_gain times He init, bias
+    0 except obj_bias on each box's objectness channel (so the synthetic weights give many candidates)."""
+    fan_in = m.shape[x][0]
+    bias = np.zeros((num_box, 5 + num_class), np.float32)
+    bias[:, 4] = obj_bias
+    return m.conv(name, x, num_box * (5 + num_class), 1, 1, 0, True, gain=head_gain * np.sqrt(2.0 / fan_in),
+                  bias_values=bias.reshape(-1))
+
+
+def _dw_pw(m: ModelWriter, tag: str, x: str, oc: int, act) -> str:
+    """Depthwise 3x3 + BatchNorm + Scale + activation, then pointwise 1x1 to oc + BatchNorm + Scale + activation."""
+    ic = m.shape[x][0]
+    x = act(m, f"_{tag}_dw", m.conv(f"{tag}_dw", x, ic, 3, 1, 1, False, group=ic))
+    return act(m, f"_{tag}_pw", m.conv(f"{tag}_pw", x, oc, 1, 1, 0, False))
+
+
+def mobilenet_yolov2(seed=0, size=416, num_classes=20, confidence_threshold=0.01, head_gain=1.0,
+                     obj_bias=-3.0) -> ModelWriter:
+    """MobileNet-YOLO (YOLOv2 head): the MobileNet-v1 body (conv1 .. conv14, BatchNorm + Scale + ReLU) at 416 x 416, one more
+    depthwise / pointwise 1024 block on the 13 x 13 map, a 1x1 convolution to 5 x (5 + 20) channels and
+    YoloDetectionOutput with the 5 VOC anchors: 845 slots."""
+    m = ModelWriter(seed)
+    x = m.input("data", 3, size, size)
+    x = _bn_scale_relu(m, "_conv1", m.conv("conv1", x, 32, 3, 2, 1, False))
+    cfg = [(64, 1), (128, 2), (128, 1), (256, 2), (256, 1), (512, 2), (512, 1), (512, 1), (512, 1), (512, 1), (512, 1),
+           (1024, 2), (1024, 1)]
+    for i, (oc, s) in enumerate(cfg, 2):
+        ic = m.shape[x][0]
+        x = _bn_scale_relu(m, f"_conv{i}_dw", m.conv(f"conv{i}_dw", x, ic, 3, s, 1, False, group=ic))
+        x = _bn_scale_relu(m, f"_conv{i}_pw", m.conv(f"conv{i}_pw", x, oc, 1, 1, 0, False))
+    x = _dw_pw(m, "yolo_conv", x, 1024, _bn_scale_relu)
+    x = _yolo_out(m, "yolo_out", x, 5, num_classes, head_gain, obj_bias)
+    m.yolo_detection_output("detection_out", x, num_classes, 5, VOC_ANCHORS, confidence_threshold, 0.45)
+    return m
+
+
+def mobilenetv2_yolov3(seed=0, size=416, num_classes=80, confidence_threshold=0.01, head_gain=1.0,
+                       obj_bias=-5.0) -> ModelWriter:
+    """MobileNet-v2 YOLOv3: the MobileNet-v2 body (ReLU6 as Clip) at 416 x 416 up to conv_last (1280 x 13 x 13); heads on
+    13 x 13 (conv_last), 26 x 26 (a 1x1 reduction of the 13 x 13 branch, nearest Interp x2, channel Concat with the
+    96-channel stride-16 block) and 52 x 52 (likewise with the 32-channel stride-8 block), each a depthwise / pointwise
+    block and a 1x1 convolution to 3 x (5 + 80); Yolov3DetectionOutput with the 9 COCO anchors, mask 6,7,8 / 3,4,5 / 0,1,2
+    and anchors_scale 32, 16, 8: 10647 slots."""
+    m = ModelWriter(seed)
+    x = m.input("data", 3, size, size)
+    x = _bn_scale_clip(m, "_conv1", m.conv("conv1", x, 32, 3, 2, 1, False))
+    table = [(1, 16, 1, 1), (6, 24, 2, 2), (6, 32, 3, 2), (6, 64, 4, 2), (6, 96, 3, 1), (6, 160, 3, 2), (6, 320, 1, 1)]
+    taps = {}
+    for bi, (t, c, n, s) in enumerate(table, 2):
+        for i in range(n):
+            tag = f"{bi}_{i + 1}"
+            stride = s if i == 0 else 1
+            ic = m.shape[x][0]
+            shortcut = stride == 1 and ic == c
+            if shortcut:
+                sc, x = m.split(f"block{tag}_split", x, [f"block{tag}_in_a", f"block{tag}_in_b"])
+            y = x
+            if t != 1:
+                y = _bn_scale_clip(m, f"_conv{tag}_expand", m.conv(f"conv{tag}_expand", y, ic * t, 1, 1, 0, False))
+            y = _bn_scale_clip(m, f"_conv{tag}_dw", m.conv(f"conv{tag}_dw", y, ic * t, 3, stride, 1, False, group=ic * t))
+            y = m.conv(f"conv{tag}_linear", y, c, 1, 1, 0, False)
+            y = _bn_scale_clip(m, f"_conv{tag}_linear", y, clip=False, center=0.3 if shortcut else 1.0)
+            x = m.eltwise(f"block{tag}", [sc, y]) if shortcut else y
+        taps[bi] = x
+    x = _bn_scale_clip(m, "_conv_last", m.conv("conv_last", x, 1280, 1, 1, 0, False))
+    anchors_mask = [6, 7, 8, 3, 4, 5, 0, 1, 2]
+    outs = []
+    h = _dw_pw(m, "yolo13", x, 512, _bn_scale_clip)
+    outs.append(_yolo_out(m, "yolo13_out", h, 3, num_classes, head_gain, obj_bias))
+    for grid, tap, mid, width in ((26, taps[6], 128, 192), (52, taps[4], 64, 96)):
+        u = _bn_scale_clip(m, f"_up{grid}_reduce", m.conv(f"up{grid}_reduce", x, mid, 1, 1, 0, False))
+        u = m.interp(f"up{grid}", u, 1, scale=2.0)
+        x = m.concat(f"cat{grid}", [u, tap])
+        h = _dw_pw(m, f"yolo{grid}", x, width, _bn_scale_clip)
+        outs.append(_yolo_out(m, f"yolo{grid}_out", h, 3, num_classes, head_gain, obj_bias))
+    m.yolov3_detection_output("detection_out", outs, num_classes, 3, COCO_ANCHORS, anchors_mask, [32.0, 16.0, 8.0],
+                              confidence_threshold, 0.45)
+    return m
+
+
+def yolo_tiny(seed=0, size=64, num_classes=5, confidence_threshold=0.05, head_gain=1.0, obj_bias=-2.0) -> ModelWriter:
+    """Two-scale YOLOv3 head at small size: 8 x 8 and 16 x 16 maps (the second through nearest Interp x2 and Concat),
+    3 anchors each, 5 classes, anchors_scale 8 and 4: 960 slots at 64 x 64."""
+    m = ModelWriter(seed)
+    x = m.input("data", 3, size, size)
+    x = m.relu("relu1", m.conv("conv1", x, 16, 3, 2, 1, True))
+    a = m.relu("relu2", m.conv("conv2", x, 32, 3, 2, 1, True))
+    b = m.relu("relu3", m.conv("conv3", a, 64, 3, 2, 1, True))
+    o8 = _yolo_out(m, "yolo8_out", b, 3, num_classes, head_gain, obj_bias)
+    u = m.interp("up16", m.relu("up16_relu", m.conv("up16_reduce", b, 16, 1, 1, 0, True)), 1, scale=2.0)
+    x = m.relu("yolo16_relu", m.conv("yolo16_conv", m.concat("cat16", [u, a]), 32, 3, 1, 1, True))
+    o16 = _yolo_out(m, "yolo16_out", x, 3, num_classes, head_gain, obj_bias)
+    m.yolov3_detection_output("detection_out", [o8, o16], num_classes, 3, [4, 6, 8, 10, 12, 9, 16, 20, 24, 18, 32, 40],
+                              [3, 4, 5, 0, 1, 2], [8.0, 4.0], confidence_threshold, 0.45)
+    return m
+
+
 ZOO = {"single_conv": single_conv, "vgg16": vgg16, "resnet50": resnet50, "mobilenet_v1": mobilenet_v1, "mini": mini,
        "decoder_tiny": decoder_tiny, "fcn8s_tiny": fcn8s_tiny, "deeplab_head_tiny": deeplab_head_tiny,
-       "mobilenet_v2": mobilenet_v2, "prelu_tiny": prelu_tiny, "mobilenet_ssd": mobilenet_ssd, "ssd_tiny": ssd_tiny}
+       "mobilenet_v2": mobilenet_v2, "prelu_tiny": prelu_tiny, "mobilenet_ssd": mobilenet_ssd, "ssd_tiny": ssd_tiny,
+       "mobilenet_yolov2": mobilenet_yolov2, "mobilenetv2_yolov3": mobilenetv2_yolov3, "yolo_tiny": yolo_tiny}
 
 
 def synthetic_input(shape, index: int = 0) -> np.ndarray:

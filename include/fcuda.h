@@ -384,6 +384,66 @@ int fcuda_detection_output_forward(float* output, const float* loc, const float*
                                    int num_classes, float conf_threshold, float nms_threshold, int nms_top_k, int keep_top_k,
                                    float* workspace, int batch, void* stream);
 
+/* ---- YOLO detection head (the reference has none of these layers) --------------------------------------------------
+ * ncnn's YoloDetectionOutput (YOLOv2, version 2) and Yolov3DetectionOutput (version 3), with a fixed-shape output.
+ * Stream-ordered like the SSD calls above: nothing allocates, synchronises or copies to the host.
+ *
+ * Inputs: one (batch, num_box * (5 + C), h, w) blob per scale b (exactly one for version 2), in mask-group order; for box
+ * pp the channels pp * (5 + C) + {0: x, 1: y, 2: w, 3: h, 4: objectness, 5..: class logits}.  A slot is one (scale, box,
+ * row, column) in that order (ncnn's gather order); slots = sum over scales of num_box * h * w.
+ *
+ * Decode of the cell (i, j) of box pp on scale b, in fp32, every operation rounded on its own (no FMA), s(t) =
+ * 1 / (1 + expf(-t)):
+ *   cx = (j + s(x)) / w, cy = (i + s(y)) / h, bw = expf(tw) * bias_w / norm_w, bh = expf(th) * bias_h / norm_h,
+ *   box = (cx - bw * 0.5, cy - bh * 0.5, cx + bw * 0.5, cy + bh * 0.5)
+ *   version 3: k = mask[b * num_box + pp], bias = (biases[2k], biases[2k + 1]) in input pixels, norm_w =
+ *     (int)(anchors_scale[b] * w) (fp32 product, truncated), norm_h likewise.  class = the argmax of the raw logits
+ *     (strict >, from -FLT_MAX, so the first maximum wins; all -inf / NaN logits give class 0 with -FLT_MAX), and
+ *       confidence = 1 / (1 + expf(-obj) * (1 + expf(-logit_max)))
+ *     which is ncnn's expression as written.  ncnn's comment calls it s(obj) * s(logit_max), but the parentheses make it
+ *     a different function; it is kept because thresholds shipped with ncnn models were tuned against it.
+ *   version 2: bias = (biases[2pp], biases[2pp + 1]) in grid cells, norm_w = w, norm_h = h.  p = the max-subtracted
+ *     softmax of the C logits, p_k = expf(l_k - max) / sum (sum in class order), computed without writing the input
+ *     (ncnn's layer overwrites its bottom); class = the argmax of p (strict >, from 0), confidence = s(obj) * p_class.
+ * A slot is a candidate iff confidence >= confidence_threshold (>=, where SSD's DetectionOutput takes >).
+ *
+ * Selection, NMS and output: the candidates of each image are ordered by (confidence descending, slot ascending) and the
+ * first nms_top_k kept; then one greedy class-agnostic NMS over them in that order: a candidate is kept iff no earlier kept
+ * box has IoU > nms_threshold, the IoU being DetectionOutput's above (areas from the corners; a NaN IoU suppresses
+ * nothing).  output: (batch, keep_top_k, 6), rows [class + 1, confidence, xmin, ymin, xmax, ymax] in kept order (the + 1
+ * is ncnn's prepended background label), then [-1, 0, 0, 0, 0, 0].  ncnn's output has one row per kept box and no cap, so
+ * with nms_top_k = keep_top_k = 1024 the rows equal ncnn's whenever at most 1024 slots pass the threshold; past that
+ * the lowest-ranked candidates are dropped before NMS, and past keep_top_k kept boxes the rest are dropped.
+ *
+ * Limits (else -200): version 2 or 3; 1 <= num_class <= 1024; 1 <= num_box <= 16; 1..4 scales (1 for version 2);
+ * num_biases <= 128, and >= 2 * num_box for version 2; version 3: every mask index k in 0 <= k < num_biases / 2, and
+ * on every scale anchors_scale > 0 with anchors_scale * (the longer grid side) < 2^31 in fp32; slots < 2^24;
+ * 1 <= nms_top_k, keep_top_k <= 1024; batch <= 65535; nms_threshold not NaN.  -100: a NULL pointer, batch < 1, a grid
+ * side < 1, or a workspace that is not 16-byte aligned (fcuda_yolo_detection_forward). */
+#define FCUDA_YOLO_MAX_SCALES 4
+#define FCUDA_YOLO_MAX_BOXES 16
+#define FCUDA_YOLO_MAX_BIASES 128
+typedef struct FcudaYoloParam {
+    int version;                                           /* 2: YoloDetectionOutput, 3: Yolov3DetectionOutput */
+    int num_class, num_box, num_scales;
+    float confidence_threshold, nms_threshold;
+    int nms_top_k, keep_top_k;
+    int num_biases;                                        /* floats in biases */
+    float biases[FCUDA_YOLO_MAX_BIASES];
+    int mask[FCUDA_YOLO_MAX_SCALES * FCUDA_YOLO_MAX_BOXES]; /* version 3: num_box per scale */
+    float anchors_scale[FCUDA_YOLO_MAX_SCALES];            /* version 3 */
+    int grid_h[FCUDA_YOLO_MAX_SCALES], grid_w[FCUDA_YOLO_MAX_SCALES];
+} FcudaYoloParam;
+/* Decode alone: for every slot of every image, scores (batch, slots) the confidence, classes (batch, slots) the class
+ * (without the + 1) and boxes (batch, slots, 4), whether or not the slot is a candidate.  The boxes and confidences
+ * fcuda_yolo_detection_forward uses are these bits.  inputs: num_scales device pointers. */
+int fcuda_yolo_decode(float* scores, int* classes, float* boxes, const float* const* inputs, const FcudaYoloParam* param,
+                      int batch, void* stream);
+/* Workspace in floats: batch * (6 * slots + 39937). */
+int fcuda_yolo_detection_workspace_size(const FcudaYoloParam* param, int batch, size_t* floats);
+int fcuda_yolo_detection_forward(float* output, const float* const* inputs, const FcudaYoloParam* param, float* workspace,
+                                 int batch, void* stream);
+
 /* Kernel-variant switches for A/B measurements and tests.  Defaults are the measured-best configuration; the environment
  * variable FCUDA_<NAME> sets the initial value.  Names (value range, default):
  *   dw_vec (0-1, 1)           vectorised depthwise kernel on wide planes
@@ -403,6 +463,9 @@ int fcuda_detection_output_forward(float* output, const float* loc, const float*
  *                             GEMM turned around (output channels on the wgmma M side, 224 pixels per warpgroup on N,
  *                             read from the split planes by descriptor), so each filter byte serves 1.75x (N tile 128)
  *                             or 3.5x (N tile 64) as many pixels.  Bit-identical to 0 = the pre-split kernel
+ *   yolo_nms (0-1, 1)         YOLO NMS: CTAs over (32-row block, image) write the suppression mask, then one CTA per
+ *                             image sweeps it.  0 = one CTA per image builds the whole mask in its own shared memory
+ *                             and sweeps it.  Bit-identical
  * Every variant computes the same result (tests/test_gpu_variants.py).  Returns 0 / the value, -200 for an unknown name or value. */
 int fcuda_set_tuning(const char* name, int value);
 int fcuda_get_tuning(const char* name);
@@ -416,7 +479,7 @@ int fcuda_profile_collect(double* total_ms, double* algo_flops, double* mma_flop
 /* Same, per kernel class, for every instrumented launch (the enable switch above covers all of them):
  * kind 0 TensorGEMM, 1 implicit-GEMM conv, 2 Winograd input transform, 3 Winograd output transform, 4 pooling,
  * 5 depthwise, 6 element-wise (BN/Scale/Eltwise/Clip/PReLU), 7 deconvolution scatter / depthwise gather, 8 resize / crop (Interp,
- * Crop), 9 detection (Permute, axis Softmax, PriorBox, decode, NMS, merge), < 0 all.  algo_bytes = the bytes the operation must move (inputs
+ * Crop), 9 detection (Permute, axis Softmax, PriorBox, decode, NMS, merge; YOLO decode, select, mask, sweep), < 0 all.  algo_bytes = the bytes the operation must move (inputs
  * read once + outputs written once). */
 int fcuda_profile_collect_kind(int kind, double* total_ms, double* algo_flops, double* mma_flops, double* algo_bytes,
                                long long* launches);
