@@ -138,6 +138,7 @@ def fcuda() -> ctypes.CDLL:
             "fcuda_igemm_halo_tile": (i, [P, ctypes.POINTER(i)]),
             "fcuda_igemm_presplit_tile": (i, [P, ctypes.POINTER(i)]),
             "fcuda_igemm_wide_tile": (i, [P, ctypes.POINTER(i)]),
+            "fcuda_igemm_stem_supported": (i, [P, ctypes.POINTER(FcudaConvOptions)]),
             "fcuda_conv_forward_pool": (i, [P, i, vp, vp, vp, vp, vp, i, vp]),
             "fcuda_conv_forward_ext": (i, [P, i, vp, vp, vp, vp, vp, vp, i, i, i, i, vp]),
             "fcuda_eltwise_forward": (i, [vp, vp, vp, sz, i, ctypes.c_float, ctypes.c_float, i, vp]),

@@ -424,6 +424,230 @@ int launch_igemm(const IgemmProblem& p, cudaStream_t stream) {
 }
 
 // ===================================================================================================================
+// Stem kernel (BF16x3, switch igemm_stem): the short-K k-table layers (IC % 32 != 0, K <= 256, OC <= 128, no residual,
+// pooling or dilation), e.g. IC = 3 first layers, whose time is their output written to HBM, not their few MMAs.
+//   CTAs       = persistent, 8 consumer warps, no producer warp; static stride over the tiles.
+//   M tile     = 128 consecutive output pixels of ONE image (the last tile of an image is partial), one N tile (BN >= OC).
+//   B operand  = every k-block of the pre-tiled filter planes, fetched once per CTA by one bulk copy each and resident
+//                (8 KB for a 3x3x3 -> 64 layer); the k-table is built once per CTA as well.
+//   A operand  = gathered into registers as in conv_igemm_kernel; the next k-block's (or the next tile's first k-block's)
+//                loads are issued before the current one is multiplied, so they land during its MMAs and its epilogue.
+//   epilogue   = +bias -> ReLU / Clip into a staging tile [BN channels][128 pixels] in shared memory (two buffers when
+//                they fit, so one CTA barrier per tile suffices), then each warp writes whole channel runs: 128 pixels =
+//                32 lanes x one 16-byte store, or per-lane 4-byte stores where the output is not 16-byte aligned or
+//                OH * OW % 4 != 0.  The stores drain while the CTA computes the next tile.
+// Per k-block the operand values, the k order, the split, the wgmma sequence (p2*q1, p1*q2, p1*q1 per k-step) and the
+// fp32 epilogue are those of conv_igemm_kernel<BN, 3>: the result is bit-identical to it.
+constexpr int kStemThreads = kConsumerWarps * 32;
+constexpr int kStemPitch = 132;  // floats per staging row: fragment writes hit 32 banks, rows stay 16-byte aligned
+constexpr int kStemMaxK = 256;
+
+struct StemArgs {
+    const float* in;
+    float* out;
+    const float* bias;
+    int IC, H, W, OC, OW, oplane;  // oplane = OH * OW
+    int pad_top, pad_left, stride_h, stride_w;
+    int in_img_c, out_img_c;
+    int K, kblocks, KW;
+    int act;                       // 0 none, 1 ReLU, 2 Clip: clamp to [lo, hi]
+    float lo, hi;
+    int tiles_per_img;             // ceil(oplane / 128)
+    long long tiles;               // N * tiles_per_img
+    int nbuf;                      // staging buffers: 2, or 1 where two do not fit beside the filters
+    int vec;                       // 16-byte stores: `out` 16-byte aligned and oplane % 4 == 0
+    const unsigned char* wbf;
+    unsigned wbf_kb_bytes;
+};
+
+template <int BN, bool CLIP>
+__global__ void __launch_bounds__(kStemThreads, BN == 128 ? 1 : 2)
+conv_igemm_stem_kernel(const StemArgs args) {
+    constexpr int kBTile = BN * 32 * 2;
+    constexpr int kStage = 2 * kBTile;  // both bf16 planes of one k-block
+    extern __shared__ uint8_t smem_raw[];
+    uint8_t* smem = smem_raw + ((1024u - (ptx::smem_u32(smem_raw) & 1023u)) & 1023u);
+    // [k-block][q1, q2] filters, the staging buffers, the k-table
+    float* staging = reinterpret_cast<float*>(smem + args.kblocks * kStage);
+    int2* ktab = reinterpret_cast<int2*>(staging + args.nbuf * BN * kStemPitch);
+    __shared__ uint64_t wbar;
+
+    const int warp = threadIdx.x >> 5;
+    const int lane = threadIdx.x & 31;
+    const int kblocks = args.kblocks;
+    const int plane = args.H * args.W;
+
+    if (threadIdx.x == 0) {
+        ptx::mbar_init(&wbar, 1);
+        ptx::fence_barrier_init();
+    }
+    for (int k = threadIdx.x; k < kblocks * 32; k += kStemThreads) {
+        int2 e = make_int2(0, 0);
+        if (k < args.K) {
+            const int tap = k / args.IC, ic = k - tap * args.IC;
+            const int dy = tap / args.KW, dx = tap % args.KW;
+            e = make_int2(ic * plane + dy * args.W + dx, (dy << 16) | dx);
+        }
+        ktab[k] = e;
+    }
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        ptx::mbar_arrive_expect_tx(&wbar, static_cast<uint32_t>(kblocks * kStage));
+        for (int kb = 0; kb < kblocks; ++kb)
+            ptx::bulk_load_1d(smem + kb * kStage, args.wbf + static_cast<size_t>(kb) * args.wbf_kb_bytes, kStage, &wbar);
+    }
+
+    const int gq = lane >> 2, c = lane & 3;
+    const float* __restrict__ in = args.in;
+    // gather state: the two pixels (fragment rows gq, gq + 8 of this warp's 16) of the tile being gathered
+    int iy0[2], ix0[2];
+    long long ibase[2];
+    bool valid[2];
+    auto locate = [&](long long t) {
+        const int img = static_cast<int>(t / args.tiles_per_img);
+        const int p0 = static_cast<int>(t - static_cast<long long>(img) * args.tiles_per_img) * 128;
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+            const int pix = p0 + warp * 16 + 8 * h + gq;
+            valid[h] = pix < args.oplane;
+            const int pc = valid[h] ? pix : 0;
+            const int oy = pc / args.OW, ox = pc - oy * args.OW;
+            iy0[h] = oy * args.stride_h - args.pad_top;
+            ix0[h] = ox * args.stride_w - args.pad_left;
+            ibase[h] = static_cast<long long>(img) * args.in_img_c * plane + static_cast<long long>(iy0[h]) * args.W + ix0[h];
+        }
+    };
+    auto gather = [&](int kb, float (&raw)[2][8]) {
+#pragma unroll
+        for (int j = 0; j < 8; ++j) {
+            const int k = kb * 32 + frag_k<true>(j, c);
+            int2 e;
+            asm volatile("ld.shared.v2.s32 {%0, %1}, [%2];" : "=r"(e.x), "=r"(e.y) : "r"(ptx::smem_u32(ktab + k)));
+            const int dy = e.y >> 16, dx = e.y & 0xFFFF;
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+                const bool ok = valid[h] && k < args.K && static_cast<unsigned>(iy0[h] + dy) < static_cast<unsigned>(args.H) &&
+                                static_cast<unsigned>(ix0[h] + dx) < static_cast<unsigned>(args.W);
+                raw[h][j] = ok ? __ldg(in + ibase[h] + e.x) : 0.f;
+            }
+        }
+    };
+
+    float raw[2][8];
+    locate(blockIdx.x);  // grid <= tiles: every CTA has a first tile
+    gather(0, raw);
+    const uint32_t filters = ptx::smem_u32(smem);
+    ptx::mbar_wait_nocall(&wbar, 0);
+    int buf = 0;
+    for (long long t = blockIdx.x; t < args.tiles; t += gridDim.x) {
+        const int img = static_cast<int>(t / args.tiles_per_img);
+        const int p0 = static_cast<int>(t - static_cast<long long>(img) * args.tiles_per_img) * 128;
+        float acc[BN / 2];
+#pragma unroll
+        for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+        for (int kb = 0; kb < kblocks; ++kb) {
+            uint32_t f1[4][4], f2[4][4];
+            split_fragments<3>(raw, f1, f2);
+            if (kb + 1 < kblocks) {
+                gather(kb + 1, raw);
+            } else if (t + gridDim.x < args.tiles) {
+                locate(t + gridDim.x);
+                gather(0, raw);
+            }
+            const uint32_t b_base = filters + kb * kStage;
+            ptx::wgmma_fence();
+            mma_kblock<BN, 3>(acc, f1, f2, b_base, b_base + kBTile);
+            ptx::wgmma_commit();
+            ptx::wgmma_wait<0>();
+        }
+
+        // epilogue: the fragment values (conv_igemm_kernel's order) into staging rows [channel][pixel] ...
+        float* st = staging + buf * BN * kStemPitch;
+        const int prow = warp * 16 + gq;
+#pragma unroll
+        for (int j = 0; j < BN / 8; ++j) {
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {
+                const int oc = 8 * j + 2 * c + e;
+                const float bv = (args.bias != nullptr && oc < args.OC) ? __ldg(args.bias + oc) : 0.f;
+#pragma unroll
+                for (int h = 0; h < 2; ++h) {
+                    float v = acc[4 * j + 2 * h + e] + bv;
+                    if (args.act) v = act_clamp<CLIP>(v, args.lo, args.hi);
+                    st[oc * kStemPitch + prow + 8 * h] = v;
+                }
+            }
+        }
+        __syncthreads();
+        // ... and out as whole channel runs: warp w writes channels w, w + 8, ...
+        const int npix = min(128, args.oplane - p0);
+        float* obase = args.out + static_cast<size_t>(img) * args.out_img_c * args.oplane + p0;
+        for (int oc = warp; oc < args.OC; oc += kConsumerWarps) {
+            const float* row = st + oc * kStemPitch;
+            float* dst = obase + static_cast<size_t>(oc) * args.oplane;
+            if (args.vec) {
+                if (4 * lane < npix)
+                    *reinterpret_cast<float4*>(dst + 4 * lane) = *reinterpret_cast<const float4*>(row + 4 * lane);
+            } else {
+                for (int i = lane; i < npix; i += 32) dst[i] = row[i];
+            }
+        }
+        if (args.nbuf == 1) __syncthreads();  // every run read before the next tile's values overwrite the buffer
+        else buf ^= 1;
+    }
+}
+
+// Shared memory of the stem kernel: resident filters, staging buffers, k-table, alignment slack
+static int stem_smem_bytes(int BN, int kblocks, int nbuf) {
+    return kblocks * 2 * BN * 64 + nbuf * BN * kStemPitch * 4 + kblocks * 32 * 8 + 1024;
+}
+
+static bool stem_supported(const IgemmProblem& p) {
+    const int K = p.KH * p.KW * p.IC;
+    if (!conv_igemm_supported(p.IC, p.KH, p.KW) || p.planes != 3 || p.IC % 32 == 0 || K > kStemMaxK || p.OC > 128 ||
+        p.epi.residual != nullptr || p.epi.pool ||
+        p.dil_h > 1 || p.dil_w > 1 || p.OH < 1 || p.OW < 1)
+        return false;
+    // 32-bit planes, packed tap offsets (dy << 16 | dx) and k-table offsets ic * H * W + dy * W + dx
+    const long long table_max = static_cast<long long>(p.IC - 1) * p.H * p.W + static_cast<long long>(p.KH - 1) * p.W + p.KW - 1;
+    return static_cast<long long>(p.H) * p.W < (1ll << 30) && static_cast<long long>(p.OH) * p.OW < (1ll << 30) &&
+           p.KH - 1 < (1 << 15) && p.KW - 1 < (1 << 16) && table_max < (1ll << 31);
+}
+
+template <int BN, bool CLIP>
+int launch_stem(const IgemmProblem& p, cudaStream_t stream) {
+    if (!bf16_filters_fit(p, BN)) return -1;
+    StemArgs a;
+    a.in = p.input; a.out = p.output; a.bias = p.epi.bias;
+    a.IC = p.IC; a.H = p.H; a.W = p.W; a.OC = p.OC; a.OW = p.OW; a.oplane = p.OH * p.OW;
+    a.pad_top = p.pad_top; a.pad_left = p.pad_left; a.stride_h = p.stride_h; a.stride_w = p.stride_w;
+    a.in_img_c = p.in_c_total > 0 ? p.in_c_total : p.IC;
+    a.out_img_c = p.out_c_total > 0 ? p.out_c_total : p.OC;
+    a.K = p.KH * p.KW * p.IC;
+    a.kblocks = ceil_div(a.K, 32);
+    a.KW = p.KW;
+    a.act = p.epi.act; a.lo = p.epi.lo; a.hi = p.epi.hi;
+    a.tiles_per_img = ceil_div(a.oplane, 128);
+    a.tiles = static_cast<long long>(p.N) * a.tiles_per_img;
+    a.nbuf = stem_smem_bytes(BN, a.kblocks, 2) <= 227 * 1024 ? 2 : 1;
+    a.vec = (reinterpret_cast<uintptr_t>(p.output) & 15) == 0 && a.oplane % 4 == 0;
+    a.wbf = reinterpret_cast<const unsigned char*>(p.w_hi);
+    a.wbf_kb_bytes = 2u * static_cast<unsigned>(igemm_ocpad(p.OC)) * 64u;
+    const int smem = stem_smem_bytes(BN, a.kblocks, a.nbuf);
+    auto kern = conv_igemm_stem_kernel<BN, CLIP>;
+    static SmemAttrCache attr_cache;
+    if (int rc = ensure_dynamic_smem(kern, smem, attr_cache)) return rc;
+    unsigned grid = 0;
+    if (int rc = persistent_grid(kern, kStemThreads, smem, a.tiles, &grid)) return rc;
+    const int prof = prof_igemm(p, stream, a.tiles * 128, BN, a.kblocks);
+    kern<<<grid, kStemThreads, smem, stream>>>(a);
+    prof_end(prof, stream);
+    FCUDA_CHECK_LAUNCH();
+    count_launch();
+    return 0;
+}
+
+// ===================================================================================================================
 // Halo kernel: stride-1, dense layers with IC % 32 == 0 (k = ((ic/32)*taps + tap)*32 + ic%32, as above).
 //
 //   M tile     = an R x C patch of output pixels inside one image (R * C = 128, C in {8, 16, 32, 64}); warp w covers rows
@@ -1288,10 +1512,13 @@ int launch_halo_family(const IgemmProblem& p, const HaloGeom& hg, int BN, int sm
 
 // The kernel a layer takes for one N tile and operand format: the gathering kernel, or with switch igemm_halo on a
 // layer halo_geometry accepts the per-tap halo kernel, in BF16x3 mode the pre-split kernel (switch igemm_presplit) and
-// the wide one (switch igemm_wide).
+// the wide one (switch igemm_wide).  In BF16x3 mode the short-K layers stem_supported accepts take the stem kernel
+// (switch igemm_stem); they never qualify for the halo family (IC % 32 != 0).
 // CLIP: the Clip instantiations (ConvEpilogue::act == 2); the others apply a ReLU as fmaxf(v, 0).
 template <int BN, int PLANES, bool CLIP>
 int launch_conv(const IgemmProblem& p, cudaStream_t stream) {
+    if constexpr (PLANES == 3)
+        if (tune_get(TUNE_IGEMM_STEM) != 0 && stem_supported(p)) return launch_stem<BN, CLIP>(p, stream);
     HaloGeom hg;
     if (tune_get(TUNE_IGEMM_HALO) == 0 || !halo_geometry(p, hg)) return launch_igemm<BN, PLANES, CLIP>(p, stream);
     if constexpr (PLANES == 3) {
@@ -1329,6 +1556,7 @@ static bool geometry_query(bool (*geometry)(const IgemmProblem&, HaloGeom&), con
 bool conv_igemm_halo_geometry(const IgemmProblem& p, HaloGeom* g) { return geometry_query(halo_geometry, p, g); }
 bool conv_igemm_presplit_geometry(const IgemmProblem& p, HaloGeom* g) { return geometry_query(presplit_geometry, p, g); }
 bool conv_igemm_wide_geometry(const IgemmProblem& p, HaloGeom* g) { return geometry_query(wide_geometry, p, g); }
+bool conv_igemm_stem_supported(const IgemmProblem& p) { return stem_supported(p); }
 
 bool conv_igemm_supported(int IC, int KH, int KW) {
     if (KH * KW > 63) return false;                               // per-pixel tap validity mask is 64-bit

@@ -41,6 +41,9 @@ bool conv_igemm_presplit_geometry(const IgemmProblem& p, HaloGeom* g);
 // Tile (28 x 16 pixels with a 64-channel N tile, 28 x 8 with a 128-channel one) and box of the wide pre-split kernel
 // (switch igemm_wide) on a layer that takes the pre-split kernel; false when the layer keeps the pre-split kernel.
 bool conv_igemm_wide_geometry(const IgemmProblem& p, HaloGeom* g);
+// True when the layer takes the persistent stem kernel (switch igemm_stem): BF16x3 mode, IC % 32 != 0, KH*KW*IC <= 256,
+// OC <= 128, no residual, pooling or dilation.  Reads planes, IC, OC, H, W, OH, OW, KH, KW, dilation and epi.
+bool conv_igemm_stem_supported(const IgemmProblem& p);
 int conv_igemm_forward(const IgemmProblem& p, cudaStream_t stream);
 
 }  // namespace fcuda

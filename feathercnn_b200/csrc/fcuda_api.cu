@@ -619,6 +619,17 @@ int fcuda_igemm_halo_tile(const FcudaConvParam* p, int* geom) { return igemm_til
 int fcuda_igemm_presplit_tile(const FcudaConvParam* p, int* geom) { return igemm_tile(p, geom, conv_igemm_presplit_geometry); }
 int fcuda_igemm_wide_tile(const FcudaConvParam* p, int* geom) { return igemm_tile(p, geom, conv_igemm_wide_geometry); }
 
+int fcuda_igemm_stem_supported(const FcudaConvParam* p, const FcudaConvOptions* o) {
+    if (!p) return 0;
+    IgemmProblem g = igemm_problem(p);
+    if (o) {
+        g.epi.residual = o->residual;
+        g.epi.pool = o->pool ? 1 : 0;
+        g.dil_h = o->dilation_h; g.dil_w = o->dilation_w;
+    }
+    return conv_igemm_stem_supported(g) ? 1 : 0;
+}
+
 int fcuda_tensor_gemm(float* d, const float* a, const float* b_hi, const float* b_lo, int m, int n, int k, int g,
                       void* stream) {
     GemmProblem p{};

@@ -224,6 +224,11 @@ int fcuda_igemm_presplit_tile(const FcudaConvParam* param, int* geom);
  * 1 with geom[0..3] = tile rows (28), tile columns (16 for a 64-channel N tile, 8 for 128), fp32 box rows, box columns;
  * 0 otherwise.  The switches themselves are not consulted. */
 int fcuda_igemm_wide_tile(const FcudaConvParam* param, int* geom);
+/* FCUDA_SGECONV in the current arithmetic mode: 1 when the layer (output_h / output_w assigned) with `options` (NULL = the
+ * all-zero struct) runs on the persistent stem kernel (switch igemm_stem below: fp32split mode, input_channels / group
+ * % 32 != 0, kernel_h * kernel_w * input_channels / group <= 256, output_channels / group <= 128, no residual, pooling or
+ * dilation); 0 when it keeps the gathering kernel.  The switch itself is not consulted. */
+int fcuda_igemm_stem_supported(const FcudaConvParam* param, const FcudaConvOptions* options);
 /* fcuda_conv_forward_opts with only pool set. */
 int fcuda_conv_forward_pool(const FcudaConvParam* param, int algo, float* output, const float* input,
                             const float* packed_kernel, float* scratch, const float* bias, int batch, void* stream);
@@ -466,6 +471,10 @@ int fcuda_yolo_detection_forward(float* output, const float* const* inputs, cons
  *   yolo_nms (0-1, 1)         YOLO NMS: CTAs over (32-row block, image) write the suppression mask, then one CTA per
  *                             image sweeps it.  0 = one CTA per image builds the whole mask in its own shared memory
  *                             and sweeps it.  Bit-identical
+ *   igemm_stem (0-1, 1)       fp32split mode: the layers fcuda_igemm_stem_supported names (short K, e.g. IC = 3 first
+ *                             layers) run on persistent CTAs that keep every filter k-block resident, gather the next
+ *                             tile during the current one and write whole channel runs from a shared-memory staging
+ *                             tile.  Bit-identical to 0 = the gathering kernel, one CTA per 128-pixel tile
  * Every variant computes the same result (tests/test_gpu_variants.py).  Returns 0 / the value, -200 for an unknown name or value. */
 int fcuda_set_tuning(const char* name, int value);
 int fcuda_get_tuning(const char* name);

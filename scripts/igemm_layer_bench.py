@@ -1,15 +1,18 @@
 """Per-layer timing of the implicit-GEMM convolution (SGECONV), switch --switch at 0 against 1: igemm_presplit (default:
 the pre-split halo kernel against the per-tap split), igemm_wide (the wide pre-split kernel against the pre-split kernel)
-or igemm_halo (the halo kernel against the gathering kernel), for
+igemm_halo (the halo kernel against the gathering kernel) or igemm_stem (the persistent stem kernel against the
+gathering kernel), for
 every layer of the benchmark nets that fcuda_conv_select_algo_tuned sends to SGECONV, at the nets' benchmark batch sizes.
 
-    python scripts/igemm_layer_bench.py --out DIR [--reps 5] [--iters 20] [--switch igemm_presplit|igemm_wide|igemm_halo]
+    python scripts/igemm_layer_bench.py --out DIR [--reps 5] [--iters 20] [--switch igemm_presplit|igemm_wide|igemm_halo|igemm_stem]
 
 For each layer: CUDA-event time per launch of both kernels (alternated over --reps repetitions; median and every value),
 the algorithmic rate (direct-convolution FLOPs), the issued tensor-pipe rate (padded patch pixels, N tiles and the three
 MMAs per product of the split modes) and that rate's fraction of the H100 SXM data-sheet dense BF16 rate, and for the
 halo kernels the bytes one launch moves from L2 to the SMs (filter ring stages + input boxes, from the geometry).  The Winograd
-F(6,3) time of the same shape is listed for reference only.  Writes DIR/igemm_layer_bench.json with the card's name and
+F(6,3) time of the same shape is listed for reference only.  For the layers the stem kernel takes: the algorithmic bytes
+(input + filters read once, output written once, fp32) per second of both kernels, next to the H100 SXM data-sheet HBM3
+rate.  Writes DIR/igemm_layer_bench.json with the card's name and
 power limit.  Needs a CUDA device."""
 from __future__ import annotations
 
@@ -26,6 +29,7 @@ if str(ROOT) not in sys.path:
     sys.path.insert(0, str(ROOT))
 
 DATASHEET_BF16_DENSE = 989e12  # H100 SXM data sheet, dense BF16 (not a measured figure)
+DATASHEET_HBM = 3.35e12        # H100 SXM data sheet, HBM3 bytes/s (not a measured figure)
 BATCH = {"vgg16": 64, "resnet50": 128, "mobilenet_v1": 256}
 
 
@@ -78,7 +82,7 @@ def main() -> None:
     ap.add_argument("--reps", type=int, default=5)
     ap.add_argument("--iters", type=int, default=20, help="launches per timed repetition")
     ap.add_argument("--models", default="vgg16,resnet50,mobilenet_v1")
-    ap.add_argument("--switch", default="igemm_presplit", choices=["igemm_presplit", "igemm_wide", "igemm_halo"])
+    ap.add_argument("--switch", default="igemm_presplit", choices=["igemm_presplit", "igemm_wide", "igemm_halo", "igemm_stem"])
     args = ap.parse_args()
 
     import torch
@@ -131,7 +135,7 @@ def main() -> None:
         return e0.elapsed_time(e1) / iters
 
     result = {"card": card(), "switch": args.switch, "reps": args.reps, "iters": args.iters,
-              "datasheet_bf16_dense_tflops": DATASHEET_BF16_DENSE / 1e12,
+              "datasheet_bf16_dense_tflops": DATASHEET_BF16_DENSE / 1e12, "datasheet_hbm_tbps": DATASHEET_HBM / 1e12,
               "precision": {0: "tf32x3", 1: "tf32", 2: "fp32split"}[lib.fcuda_get_precision()], "layers": []}
     try:
         for model in args.models.split(","):
@@ -148,6 +152,7 @@ def main() -> None:
                 presplit = lib.fcuda_igemm_presplit_tile(ctypes.byref(p), pgeom) == 1
                 wgeom = (ctypes.c_int * 4)()
                 wide = lib.fcuda_igemm_wide_tile(ctypes.byref(p), wgeom) == 1
+                stem = lib.fcuda_igemm_stem_supported(ctypes.byref(p), None) == 1
                 t = {0: [], 1: []}
                 outs = {}
                 for _ in range(args.reps):
@@ -184,6 +189,7 @@ def main() -> None:
                     return tiles * ((kpad // 32) * stage + (ic // group // 32) * 32 * rb * cb * 4)
                 issued_new = 2.0 * pix * ocp * kpad * mult
                 old_ms, new_ms = statistics.median(t[0]), statistics.median(t[1])
+                algo_bytes = 4.0 * (n * ic * ih * iw + oc * (ic // group) * k * k + n * oc * p.output_h * p.output_w)
                 wino_ms = None  # Winograd F(6,3) on the same shape (3x3, stride 1), for reference only
                 if k == 3 and s == 1 and group == 1:
                     del launch, out
@@ -206,11 +212,15 @@ def main() -> None:
                        "l2_to_sm_bytes_halo": l2_to_sm_bytes(geom) if halo else None,
                        "l2_to_sm_bytes_presplit": l2_to_sm_bytes(pgeom) if presplit else None,
                        "wide_tile_rows_cols_box": list(wgeom) if wide else None,
-                       "l2_to_sm_bytes_wide": l2_to_sm_bytes(wgeom) if wide else None}
+                       "l2_to_sm_bytes_wide": l2_to_sm_bytes(wgeom) if wide else None,
+                       "stem_eligible": stem, "algo_bytes": algo_bytes,
+                       "algo_tbps_old": algo_bytes / old_ms / 1e9, "algo_tbps_new": algo_bytes / new_ms / 1e9,
+                       "algo_fraction_of_datasheet_hbm_new": algo_bytes / new_ms / 1e-3 / DATASHEET_HBM}
                 result["layers"].append(rec)
                 print(json.dumps({k2: rec[k2] for k2 in ("model", "layer", "old_ms_median", "new_ms_median", "speedup",
                                                           "bit_identical", "algo_tflops_new", "issued_tflops_new",
-                                                          "l2_to_sm_bytes_presplit", "l2_to_sm_bytes_wide")}),
+                                                          "l2_to_sm_bytes_presplit", "l2_to_sm_bytes_wide",
+                                                          "stem_eligible", "algo_tbps_old", "algo_tbps_new")}),
                       flush=True)
                 torch.cuda.empty_cache()
     finally:
