@@ -90,6 +90,15 @@ class FcudaYoloParam(ctypes.Structure):
                  ("grid_w", ctypes.c_int * 4)])
 
 
+class FcudaRoute(ctypes.Structure):
+    """include/fcuda.h FcudaRoute (up to FCUDA_ROUTE_MAX = 8 sources and destinations)."""
+
+    _fields_ = [("outer", ctypes.c_int), ("inner", ctypes.c_int), ("num_src", ctypes.c_int),
+                ("src", ctypes.c_void_p * 8), ("src_extent", ctypes.c_int * 8), ("group", ctypes.c_int),
+                ("reverse", ctypes.c_int), ("dst_begin", ctypes.c_int), ("num_dst", ctypes.c_int),
+                ("dst", ctypes.c_void_p * 8), ("dst_extent", ctypes.c_int * 8)]
+
+
 def fcuda() -> ctypes.CDLL:
     global _fcuda
     if _fcuda is None:
@@ -113,6 +122,8 @@ def fcuda() -> ctypes.CDLL:
             "fcuda_yolo_decode": (i, [vp, vp, vp, vp, Y, i, vp]),
             "fcuda_yolo_detection_workspace_size": (i, [Y, i, szp]),
             "fcuda_yolo_detection_forward": (i, [vp, vp, Y, vp, i, vp]),
+            "fcuda_route_forward": (i, [ctypes.POINTER(FcudaRoute), i, vp]),
+            "fcuda_slice_plan": (i, [i, i, ctypes.POINTER(i), ctypes.POINTER(i), i, ctypes.POINTER(i), ctypes.POINTER(i)]),
             "fcuda_interp_output_dim": (i, [R]),
             "fcuda_interp_forward": (i, [R, vp, vp, i, i, vp]),
             "fcuda_crop_forward": (i, [vp, vp] + [i] * 10 + [vp]),

@@ -261,6 +261,57 @@ def crop(x: torch.Tensor, coff: int, hoff: int, woff: int, oc: int, oh: int, ow:
     return out
 
 
+# ---- channel routing -------------------------------------------------------------------------------
+def route(sources, sizes, group: int = 1, reverse: int = 0, begin: int = 0, axis: int = 1, outs=None) -> list:
+    """fcuda_route_forward: `sources` (same shape but along `axis`, a dimension of the (N, ...) tensors) concatenated
+    along `axis`, ShuffleChannel(group, reverse) on it, and positions [begin, begin + sum(sizes)) written to one new
+    tensor per size (or into `outs`).  At most 8 sources and 8 sizes: one launch."""
+    from ._lib import FcudaRoute
+    x0 = sources[0]
+    shape = list(x0.shape)
+    r = FcudaRoute()
+    r.outer, r.inner = math.prod(shape[1:axis]), math.prod(shape[axis + 1:])
+    r.num_src, r.num_dst = len(sources), len(sizes)
+    r.group, r.reverse, r.dst_begin = group, reverse, begin
+    if outs is None:
+        outs = [torch.empty(shape[:axis] + [s] + shape[axis + 1:], device=x0.device, dtype=torch.float32) for s in sizes]
+    for k, x in enumerate(sources[:8]):
+        r.src[k], r.src_extent[k] = _ptr(x).value, x.shape[axis]
+    for k, (o, s) in enumerate(list(zip(outs, sizes))[:8]):
+        r.dst[k], r.dst_extent[k] = _ptr(o).value, s
+    _check("fcuda_route_forward", fcuda().fcuda_route_forward(ctypes.byref(r), x0.shape[0], _stream()))
+    return outs
+
+
+def shuffle_channel(x: torch.Tensor, group: int, reverse: int = 0) -> torch.Tensor:
+    """ncnn ShuffleChannel of x (N, C, H, W) (include/fcuda.h, fcuda_route_forward)."""
+    return route([x.contiguous()], [x.shape[1]], group, reverse)[0]
+
+
+def slice_plan(shape, axis: int, slices) -> tuple[int, list[int]]:
+    """fcuda_slice_plan for one image of ncnn rank len(shape): (storage axis 0..2 of (c, h, w), the tops' sizes)."""
+    rank = len(shape)
+    chw = (ctypes.c_int * 3)(*([1] * (3 - rank) + list(shape)))
+    sl = (ctypes.c_int * len(slices))(*slices)
+    sizes = (ctypes.c_int * len(slices))()
+    sa = ctypes.c_int()
+    _check("fcuda_slice_plan", fcuda().fcuda_slice_plan(rank, axis, chw, sl, len(slices), ctypes.byref(sa), sizes))
+    return sa.value, list(sizes)
+
+
+def slice(x: torch.Tensor, slices, axis: int = 0) -> list:
+    """ncnn Slice of x (N, ...), each image of rank x.dim() - 1 (1..3), along ncnn's per-rank `axis`; -233 takes an
+    even share of what is left.  One launch per 8 tops."""
+    x = x.contiguous()
+    sa, sizes = slice_plan(tuple(x.shape[1:]), axis, slices)
+    dim = 1 + sa - (4 - x.dim())
+    outs, begin = [], 0
+    for t0 in range(0, len(sizes), 8):
+        outs += route([x], sizes[t0:t0 + 8], begin=begin, axis=dim)
+        begin += sum(sizes[t0:t0 + 8])
+    return outs
+
+
 # ---- SSD detection head ----------------------------------------------------------------------------
 def permute(x: torch.Tensor, order: int) -> torch.Tensor:
     """ncnn Permute of x (N, C, H, W): order 0 (c,h,w) 1 (c,w,h) 2 (h,c,w) 3 (h,w,c) 4 (w,c,h) 5 (w,h,c)."""

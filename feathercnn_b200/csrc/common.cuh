@@ -111,7 +111,7 @@ __device__ __forceinline__ void split_tf32(float v, float& hi, float& lo) {
 // Kernel-variant switches (defaults = the measured-best configuration; FCUDA_<NAME> in the environment or
 // fcuda_set_tuning() override them — the variants stay testable and benchmarkable side by side).
 enum TuneKey { TUNE_DW_VEC = 0, TUNE_WINO_MLP, TUNE_IGEMM_HALO, TUNE_GEMM_PIPE, TUNE_IGEMM_PRESPLIT, TUNE_IGEMM_WIDE,
-               TUNE_YOLO_NMS, TUNE_IGEMM_STEM, TUNE_COUNT };
+               TUNE_YOLO_NMS, TUNE_IGEMM_STEM, TUNE_ROUTE_FUSE, TUNE_COUNT };
 int tune_get(int key);
 const char* tune_name(int key);             // registry name of a key (fcuda_set_tuning / fcuda_get_tuning)
 int tune_set(const char* name, int value);  // 0, or -200 for an unknown name / value
@@ -119,7 +119,7 @@ int tune_set(const char* name, int value);  // 0, or -200 for an unknown name / 
 // Per-launch profiling (tensor_gemm.cu): kernel classes for bench.py's roofline legs.
 enum ProfKind { PROF_TENSOR_GEMM = 0, PROF_IGEMM = 1, PROF_WINO_INPUT = 2, PROF_WINO_OUTPUT = 3, PROF_POOL = 4,
                 PROF_DEPTHWISE = 5, PROF_ELEMENTWISE = 6, PROF_DECONV = 7, PROF_RESIZE = 8, PROF_DETECTION = 9,
-                PROF_KINDS = 10 };
+                PROF_ROUTE = 10, PROF_KINDS = 11 };
 int prof_begin(cudaStream_t s, int kind, double algo_flops, double mma_flops, double algo_bytes);  // -1 when off
 void prof_end(int idx, cudaStream_t s);
 void profile_collect_kind(int kind, double* total_ms, double* algo_flops, double* mma_flops, double* algo_bytes,

@@ -12,6 +12,7 @@
 #include "pack.cuh"
 #include "preprocess.cuh"
 #include "resize.cuh"
+#include "route.cuh"
 #include "tensor_gemm.cuh"
 #include "winograd.cuh"
 
@@ -929,6 +930,64 @@ int fcuda_yolo_detection_forward(float* output, const float* const* inputs, cons
     if (!output || !workspace || (reinterpret_cast<uintptr_t>(workspace) & 15) || !yolo_inputs_ok(inputs, param->num_scales))
         return -100;
     return yolo_detection(output, inputs, *param, workspace, batch, as_stream(stream));
+}
+
+static const long long kRouteMaxPositions = 1ll << 31;  // positions of the concatenated axis fit an int
+
+int fcuda_route_forward(const FcudaRoute* route, int batch, void* stream) {
+    if (!route) return -100;
+    const FcudaRoute& r = *route;
+    if (r.num_src < 1 || r.num_src > FCUDA_ROUTE_MAX || r.num_dst < 1 || r.num_dst > FCUDA_ROUTE_MAX) return -200;
+    if (batch < 1 || r.outer < 1 || r.inner < 1 || r.dst_begin < 0) return -100;
+    RouteGeom g;
+    memset(&g, 0, sizeof(g));
+    long long mid = 0, span = 0;
+    for (int k = 0; k < r.num_src; ++k) {
+        if (!r.src[k] || r.src_extent[k] < 1) return -100;
+        g.src[k] = r.src[k];
+        g.src_begin[k] = static_cast<int>(mid);
+        mid += r.src_extent[k];
+        if (mid >= kRouteMaxPositions) return -200;
+    }
+    for (int k = 0; k < r.num_dst; ++k) {
+        if (!r.dst[k] || r.dst_extent[k] < 1) return -100;
+        g.dst[k] = r.dst[k];
+        g.dst_begin[k] = static_cast<int>(span);
+        span += r.dst_extent[k];
+        if (span >= kRouteMaxPositions) return -200;
+    }
+    g.src_begin[r.num_src] = static_cast<int>(mid);
+    g.dst_begin[r.num_dst] = static_cast<int>(span);
+    if (r.dst_begin + span > mid) return -100;
+    if (r.group < 1 || mid % r.group != 0) return -200;
+    if (static_cast<long long>(r.outer) * r.inner * span >= (1ll << 31)) return -200;
+    g.num_src = r.num_src;
+    g.num_dst = r.num_dst;
+    g.first = r.dst_begin;
+    g.g = r.reverse ? static_cast<int>(mid / r.group) : r.group;
+    g.cpg = static_cast<int>(mid / g.g);
+    g.outer = r.outer;
+    g.inner = r.inner;
+    return route_forward(g, batch, as_stream(stream));
+}
+
+int fcuda_slice_plan(int rank, int axis, const int* shape, const int* slices, int count, int* storage_axis, int* sizes) {
+    if (!shape || !slices || !storage_axis || !sizes || count < 1 || rank < 1 || rank > 3) return -100;
+    for (int k = 0; k < 3; ++k)
+        if (shape[k] < 1) return -100;
+    const int a = axis < 0 ? axis + rank : axis;
+    if (a < 0 || a >= rank) return -200;
+    const int sa = a + 3 - rank;
+    const long long extent = shape[sa];
+    long long taken = 0;
+    for (int i = 0; i < count; ++i) {
+        const long long n = slices[i] == -233 ? (extent - taken) / (count - i) : slices[i];
+        if (n < 1 || taken + n > extent) return -200;
+        sizes[i] = static_cast<int>(n);
+        taken += n;
+    }
+    *storage_axis = sa;
+    return 0;
 }
 
 int fcuda_pixel_channels(int type, int* src_channels, int* out_channels) { return pixel_channels(type, src_channels, out_channels); }

@@ -333,6 +333,7 @@ TuneEntry g_tune[TUNE_COUNT] = {
     {"igemm_wide", "FCUDA_IGEMM_WIDE", 1, 0, 1, 0, false},           // pre-split kernel: 224-pixel N side, filters on M
     {"yolo_nms", "FCUDA_YOLO_NMS", 1, 0, 1, 0, false},               // YOLO NMS: mask CTAs + sweep CTA (0: one CTA per image)
     {"igemm_stem", "FCUDA_IGEMM_STEM", 1, 0, 1, 0, false},           // short-K k-table layers: persistent, resident filters
+    {"route_fuse", "FCUDA_ROUTE_FUSE", 1, 0, 1, 0, false},           // Net fusion: Concat -> ShuffleChannel -> Slice in one launch
 };
 }  // namespace
 const char* tune_name(int key) { return key >= 0 && key < TUNE_COUNT ? g_tune[key].name : nullptr; }

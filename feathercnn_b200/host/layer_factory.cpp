@@ -1,6 +1,7 @@
 // Built-in layer registrations: the 13 ncnn type names the reference serves (/root/reference/src/layer_factory.cpp:53-68)
 // plus Deconvolution / DeconvolutionDepthWise, Interp, Crop, Clip, PReLU, SSD's Permute, Flatten, Reshape, PriorBox and
-// DetectionOutput, and YOLO's YoloDetectionOutput and Yolov3DetectionOutput, 26 in all, mapped onto this host's layer classes.  A table of {type name, factory} pairs instead of one macro line per layer; the
+// DetectionOutput, YOLO's YoloDetectionOutput and Yolov3DetectionOutput, and ShuffleNet's ShuffleChannel and Slice, 28 in
+// all, mapped onto this host's layer classes.  A table of {type name, factory} pairs instead of one macro line per layer; the
 // DEFINE_LAYER_CREATOR / REGISTER_LAYER_CREATOR macros of <feather/layer_factory.h> remain the plugin API for user layers.
 #include <feather/layer_factory.h>
 
@@ -17,6 +18,7 @@
 #include "layers/pooling_layer.h"
 #include "layers/relu_layer.h"
 #include "layers/resize_layers.h"
+#include "layers/route_layers.h"
 #include "layers/scale_layer.h"
 #include "layers/yolo_layers.h"
 
@@ -64,6 +66,8 @@ const BuiltIn kBuiltIns[] = {
     {"DetectionOutput", make_layer<DetectionOutputLayer>},
     {"YoloDetectionOutput", make_layer<YoloDetectionOutputLayer>},
     {"Yolov3DetectionOutput", make_layer<Yolov3DetectionOutputLayer>},
+    {"ShuffleChannel", make_layer<ShuffleChannelLayer>},
+    {"Slice", make_layer<SliceLayer>},
 };
 
 }  // namespace

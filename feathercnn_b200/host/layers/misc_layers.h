@@ -93,6 +93,7 @@ public:
         }
         return rc;
     }
+    int param_axis() const { return axis; }
 
 private:
     int axis;

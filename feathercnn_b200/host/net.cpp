@@ -16,6 +16,7 @@
 #include "layers/eltwise_layer.h"
 #include "layers/misc_layers.h"
 #include "layers/resize_layers.h"
+#include "layers/route_layers.h"
 
 namespace feather {
 inline namespace b200 {  // ABI tag: keeps these symbols apart from the reference build when both are loaded
@@ -603,6 +604,34 @@ int Net::ApplyFusion() {
         c->tops.clear();
         c->bottoms.clear();
         c->_fused_away = true;
+    }
+    // Fourth pass: channel routing.  Concat (axis 0) -> ShuffleChannel -> Slice (axis 0), or any two adjacent of them,
+    // run as one fcuda_route_forward launch by the chain's last layer (ShuffleNet-v2 units: one read and one write of
+    // the activation instead of three of each).  Every intermediate blob must have that layer as its only reader.  A
+    // layer absorbs its producer's bottoms, so a ShuffleChannel that took a Concat passes both on to a Slice.
+    if (fcuda_get_tuning("route_fuse") != 1) return 0;
+    std::map<Blob<float>*, Layer*> made_by;
+    for (size_t i = 0; i < layers.size(); ++i)
+        for (size_t j = 0; j < layers[i]->tops.size(); ++j) made_by[layers[i]->tops[j]] = layers[i];
+    for (size_t j = 0; j < layers.size(); ++j) {
+        RouteLayer* r = dynamic_cast<RouteLayer*>(layers[j]);
+        if (!r || r->_fused_away || r->absorbed() || r->bottoms.size() != 1) continue;
+        SliceLayer* slice = dynamic_cast<SliceLayer*>(r);
+        if (slice && slice->axis() != 0) continue;
+        Blob<float>* mine = r->bottoms[0];
+        if (readers[mine] != 1 || !made_by.count(mine)) continue;
+        Layer* p = made_by[mine];
+        if (p->_fused_away || p->tops.size() != 1) continue;
+        ConcatLayer* cat = dynamic_cast<ConcatLayer*>(p);
+        ShuffleChannelLayer* sh = slice ? dynamic_cast<ShuffleChannelLayer*>(p) : nullptr;
+        if (cat && (cat->param_axis() != 0 || cat->bottoms.empty() || cat->bottoms.size() > FCUDA_ROUTE_MAX)) continue;
+        if (!cat && !sh) continue;
+        r->Absorb(p->bottoms, sh != nullptr, sh ? sh->group() : 1, sh ? sh->reverse() : 0);
+        blob_map.erase(mine->name);
+        delete mine;
+        p->tops.clear();
+        p->bottoms.clear();
+        p->_fused_away = true;
     }
     return 0;
 }

@@ -8,7 +8,10 @@ no caffe / protobuf-generated code is needed — and writes the ncnn text ``.par
 
 * layer grammar and parameter ids as ``ConvLayer::LoadParam`` & co. read them (``src/layers/*.h``; ids follow ncnn's
   caffe2ncnn): Convolution / ConvolutionDepthWise, Deconvolution / DeconvolutionDepthWise, InnerProduct, Pooling, ReLU, BatchNorm, Scale, Eltwise, Concat, Dropout,
-  Softmax, Split, Input, Crop, Clip, PReLU;
+  Softmax, Split, Input, Crop, Clip, PReLU, Slice;
+* Slice (``slice_param``: ``axis`` or the older ``slice_dim``, ``slice_point``) becomes ncnn's Slice: the cut points become
+  sizes with ``-233`` (the rest) for the last top, and no cut points an even split (``-233`` for every top).  Caffe has no
+  ShuffleChannel in its upstream ``caffe.proto``, so that type keeps the "no counterpart" error;
 * ReLU6 (the type MobileNet-v2 Caffe ports use) becomes ``Clip 0=0 1=6``, Caffe's Clip (``clip_param.min / max``) Clip with its
   bounds, PReLU ``PReLU 0=num_slope`` with its slopes (one, ``channel_shared``, or one per channel) raw in the ``.bin``;
 * Crop (``axis`` 2 or 3, FCN's score crops) becomes ncnn's two-bottom Crop: the output height and width are the reference
@@ -306,6 +309,23 @@ def convert(caffemodel: bytes) -> tuple[str, bytes]:
             p = parse_message(_first(L, 104, b""))
             axis = int(_first(p, 2, _first(p, 1, 1)))
             out.layer("Concat", name, bottoms, tops, f"0={axis - 1}")
+        elif type_ == "Slice":
+            # slice_param = 126: axis = 3 (default 1), slice_point = 2 (repeated), slice_dim = 1 (deprecated axis)
+            p = parse_message(_first(L, 126, b""))
+            axis = int(_first(p, 3, _first(p, 1, 1)))
+            if axis >= 1 << 63:  # a negative int32 on the wire
+                axis -= 1 << 64
+            axis = axis + 4 if axis < 0 else axis
+            points = _ints(p.get(2, []))
+            if axis not in (1, 2, 3):
+                raise ValueError(f"layer {name}: Slice along axis {axis} (the batch) has no FeatherCNN counterpart")
+            if points and (len(points) != len(tops) - 1 or any(b <= a for a, b in zip([0] + points, points))):
+                raise ValueError(f"layer {name}: Slice needs {len(tops) - 1} increasing positive slice points, "
+                                 f"not {points}")
+            # cut points become sizes, the last top takes the rest; none: an even split (every entry -233)
+            sizes = [b - a for a, b in zip([0] + points, points)] + [-233] if points else [-233] * len(tops)
+            ps = f"-23300={len(sizes)}," + ",".join(str(s) for s in sizes)
+            out.layer("Slice", name, bottoms, tops, ps + (f" 1={axis - 1}" if axis != 1 else ""))
         elif type_ == "Dropout":
             out.layer("Dropout", name, bottoms, tops)   # identity at test time (dropout_layer.h:40-43)
         elif type_ == "Softmax":

@@ -6,8 +6,8 @@ weight blobs, raw fp32 for bias/BN/Scale blobs) — /root/reference/src/net.cpp:
 snapshot, and there is no network for pretrained checkpoints, so benchmarks and tests use random-init
 models of the architectures BASELINE.json names: a single 3x3 conv, VGG-16, ResNet-50 (Caffe topology:
 BN + Scale + ReLU as separate layers, Split/Eltwise residuals), MobileNet-v1, MobileNet-v2 (ReLU6 as Clip), plus a small "mini" net
-that exercises every layer type, single-shot detectors (MobileNet-SSD, a two-head tiny SSD) and YOLO detectors
-(MobileNet-YOLOv2, MobileNet-v2 YOLOv3, a two-scale tiny YOLOv3).  Weight statistics follow
+that exercises every layer type, single-shot detectors (MobileNet-SSD, a two-head tiny SSD), YOLO detectors
+(MobileNet-YOLOv2, MobileNet-v2 YOLOv3, a two-scale tiny YOLOv3) and ShuffleNet-v2 with a small routing probe net.  Weight statistics follow
 SURVEY.md §8(d).
 """
 from __future__ import annotations
@@ -231,6 +231,32 @@ class ModelWriter:
         self.shape[top] = tuple(shape)
         self.rank[top] = rank
         return top
+
+    def shuffle_channel(self, name, bottom, group, reverse=0, top=None):
+        """ncnn ShuffleChannel 0=group 1=reverse (1= only when set)."""
+        top = top or name
+        self._layer("ShuffleChannel", name, [bottom], [top], {0: group, 1: 1} if reverse else {0: group})
+        self.shape[top] = self.shape[bottom]
+        return top
+
+    def slice(self, name, bottom, slices, axis=0, tops=None):
+        """ncnn Slice -23300=slices 1=axis (1= only when not 0); -233 takes (extent - taken) / (tops left)."""
+        tops = tops or [f"{name}_{i}" for i in range(len(slices))]
+        params = {-23300: f"{len(slices)}," + ",".join(str(v) for v in slices)}
+        if axis:
+            params[1] = axis
+        self._layer("Slice", name, [bottom], tops, params)
+        rank = self.rank.get(bottom, 3)
+        a = (axis + rank if axis < 0 else axis) + 3 - rank
+        taken = 0
+        for i, (t, v) in enumerate(zip(tops, slices)):
+            n = (self.shape[bottom][a] - taken) // (len(slices) - i) if v == -233 else v
+            shape = list(self.shape[bottom])
+            shape[a] = n
+            self.shape[t] = tuple(shape)
+            self.rank[t] = rank
+            taken += n
+        return tops
 
     def softmax(self, name, bottom, top=None, axis=None):
         """Without `axis` (no 0= emitted): over each image's whole blob; with it, ncnn's softmax over that axis."""
@@ -514,6 +540,80 @@ def mobilenet_v2(seed=0, num_classes=1000, size=224, wide_stats=False) -> ModelW
     x = _bn_scale_clip(m, "_conv_last", x)
     x = m.pool("pool_last", x, 1, 7, 1, 0, global_pooling=True)
     x = m.conv("fc", x, num_classes, 1, 1, 0, True)
+    m.softmax("prob", x)
+    return m
+
+
+SHUFFLENET_V2_STAGES = {0.5: (48, 96, 192), 1.0: (116, 232, 464), 1.5: (176, 352, 704), 2.0: (244, 488, 976)}
+
+
+def shufflenet_v2(seed=0, num_classes=1000, size=224, width=1.0, wide_stats=False) -> ModelWriter:
+    """ShuffleNet-v2 (Ma et al. 2018) as ncnn's converted models lay it out: a 3x3 / 2 stem (24 channels) with BatchNorm +
+    Scale + ReLU and a 3x3 / 2 max pool, three stages of 4 / 8 / 4 units, conv5 (1024 channels, 2048 at 2.0x), global
+    average pool, InnerProduct and Softmax.  A downsampling unit Splits its input into two stride-2 branches (3x3 depthwise
+    + 1x1; 1x1 + 3x3 depthwise + 1x1); a stride-1 unit Slices its input into two halves and runs the second through the
+    1x1 / depthwise / 1x1 branch.  Both Concat their halves and ShuffleChannel with group 2."""
+    m = ModelWriter(seed, wide_stats)
+    x = m.input("data", 3, size, size)
+    x = m.conv("conv1", x, 24, 3, 2, 1, False)
+    x = _bn_scale_relu(m, "_conv1", x)
+    x = m.pool("pool1", x, 0, 3, 2, 0)
+    for si, (oc, n) in enumerate(zip(SHUFFLENET_V2_STAGES[width], (4, 8, 4)), 2):
+        half = oc // 2
+        for u in range(1, n + 1):
+            tag = f"stage{si}_{u}"
+            ic = m.shape[x][0]
+            if u == 1:
+                a, b = m.split(f"{tag}_split", x, [f"{tag}_in_a", f"{tag}_in_b"])
+                a = m.conv(f"{tag}_b1_dw", a, ic, 3, 2, 1, False, group=ic)
+                a = _bn_scale_relu(m, f"_{tag}_b1_dw", a, relu=False)
+                a = m.conv(f"{tag}_b1_pw", a, half, 1, 1, 0, False)
+                a = _bn_scale_relu(m, f"_{tag}_b1_pw", a)
+                stride = 2
+            else:
+                a, b = m.slice(f"{tag}_slice", x, [-233, -233])
+                stride = 1
+            b = m.conv(f"{tag}_b2_pw1", b, half, 1, 1, 0, False)
+            b = _bn_scale_relu(m, f"_{tag}_b2_pw1", b)
+            b = m.conv(f"{tag}_b2_dw", b, half, 3, stride, 1, False, group=half)
+            b = _bn_scale_relu(m, f"_{tag}_b2_dw", b, relu=False)
+            b = m.conv(f"{tag}_b2_pw2", b, half, 1, 1, 0, False)
+            b = _bn_scale_relu(m, f"_{tag}_b2_pw2", b)
+            x = m.concat(f"{tag}_concat", [a, b])
+            x = m.shuffle_channel(f"{tag}_shuffle", x, 2)
+    x = m.conv("conv5", x, 2048 if width == 2.0 else 1024, 1, 1, 0, False)
+    x = _bn_scale_relu(m, "_conv5", x)
+    x = m.pool("pool5", x, 1, 7, 1, 0, global_pooling=True)
+    x = m.fc("fc", x, num_classes)
+    m.softmax("prob", x)
+    return m
+
+
+def shuffle_tiny(seed=0, size=15, classes=10, wide_stats=False) -> ModelWriter:
+    """What ShuffleNet-v2 does not route: ShuffleChannel group 3 after a grouped 1x1 convolution (ShuffleNet-v1's
+    pattern) fused into an uneven Slice that drops a remainder, a reverse ShuffleChannel in a Concat -> ShuffleChannel ->
+    Slice chain, a Concat -> Slice pair, and Slices on h and w.  The 15 x 15 planes take the 4-byte path."""
+    m = ModelWriter(seed, wide_stats)
+    x = m.input("data", 3, size, size)
+    x = m.relu("relu1", m.conv("conv1", x, 12, 3, 1, 1, True))
+    x = m.relu("gconv_relu", m.conv("gconv", x, 12, 1, 1, 0, True, group=3))
+    x = m.shuffle_channel("shuffle_g3", x, 3)
+    a, b = m.slice("slice_uneven", x, [5, 4])                 # channels 9..11 are dropped
+    a = m.relu("conv_a_relu", m.conv("conv_a", a, 6, 1, 1, 0, True))
+    b, bs = m.split("split_b", b, ["b_conv", "b_rows"])
+    h0, h1 = m.slice("slice_h", bs, [-233, -233], axis=1)      # rows 7 + 8
+    m.slice("slice_w", h1, [3, -233, 5], axis=2)               # columns 3 + 6 + 5, one dropped
+    b = m.relu("conv_b_relu", m.conv("conv_b", b, 6, 1, 1, 0, True))
+    x = m.concat("cat1", [a, b])
+    x = m.shuffle_channel("shuffle_rev", x, 4, reverse=1)     # 12 channels: 3 groups of 4
+    c, d = m.slice("slice_even", x, [-233, -233])
+    c = m.relu("conv_c_relu", m.conv("conv_c", c, 6, 3, 1, 1, True))
+    x = m.concat("cat2", [d, c])
+    e, f = m.slice("slice_cat", x, [4, -233])
+    e = m.relu("conv_e_relu", m.conv("conv_e", e, 4, 1, 1, 0, True))
+    x = m.concat("cat3", [e, f])
+    x = m.pool("pool", x, 1, 2, 2, 0, global_pooling=True)
+    x = m.conv("fc", x, classes, 1, 1, 0, True)
     m.softmax("prob", x)
     return m
 
@@ -811,7 +911,8 @@ def yolo_tiny(seed=0, size=64, num_classes=5, confidence_threshold=0.05, head_ga
 ZOO = {"single_conv": single_conv, "vgg16": vgg16, "resnet50": resnet50, "mobilenet_v1": mobilenet_v1, "mini": mini,
        "decoder_tiny": decoder_tiny, "fcn8s_tiny": fcn8s_tiny, "deeplab_head_tiny": deeplab_head_tiny,
        "mobilenet_v2": mobilenet_v2, "prelu_tiny": prelu_tiny, "mobilenet_ssd": mobilenet_ssd, "ssd_tiny": ssd_tiny,
-       "mobilenet_yolov2": mobilenet_yolov2, "mobilenetv2_yolov3": mobilenetv2_yolov3, "yolo_tiny": yolo_tiny}
+       "mobilenet_yolov2": mobilenet_yolov2, "mobilenetv2_yolov3": mobilenetv2_yolov3, "yolo_tiny": yolo_tiny,
+       "shufflenet_v2": shufflenet_v2, "shuffle_tiny": shuffle_tiny}
 
 
 def synthetic_input(shape, index: int = 0) -> np.ndarray:

@@ -449,6 +449,39 @@ int fcuda_yolo_detection_workspace_size(const FcudaYoloParam* param, int batch, 
 int fcuda_yolo_detection_forward(float* output, const float* const* inputs, const FcudaYoloParam* param, float* workspace,
                                  int batch, void* stream);
 
+/* ---- Channel routing: ncnn's ShuffleChannel and Slice, and Concat -> ShuffleChannel -> Slice fused (the reference has
+ * neither layer) ------------------------------------------------------------------------------------------------------
+ * Every image of every blob is viewed as [outer][extent][inner].  The sources, concatenated along the middle axis, form
+ * mid = sum of src_extent positions.  ShuffleChannel with k = reverse ? mid / group : group and cpg = mid / k puts
+ * concatenated position cpg * i + j at shuffled position k * j + i (i < k, j < cpg); group 1 leaves the order alone.
+ * Shuffled positions [dst_begin, dst_begin + sum of dst_extent) go to the destinations in order; the rest are not
+ * written.  Each destination is (batch, outer, dst_extent[k], inner), each source (batch, outer, src_extent[k], inner).
+ * Every output element is a bit copy of one input element; no input element is read twice.  One launch (one per 2^31
+ * output elements of whole images), stream-ordered, nothing allocated: capturable in a CUDA graph.  16-byte accesses when
+ * inner % 4 == 0 and every pointer is 16-byte aligned, 4-byte ones otherwise.
+ * -100: a NULL route or pointer, batch < 1, outer, inner or an extent < 1, dst_begin < 0 or destinations past mid;
+ * -200: num_src or num_dst outside 1..8, group < 1, mid % group != 0, or outer * inner * (sum of dst_extent) >= 2^31. */
+#define FCUDA_ROUTE_MAX 8
+typedef struct FcudaRoute {
+    int outer, inner;
+    int num_src;
+    const float* src[FCUDA_ROUTE_MAX];
+    int src_extent[FCUDA_ROUTE_MAX];
+    int group, reverse;
+    int dst_begin;
+    int num_dst;
+    float* dst[FCUDA_ROUTE_MAX];
+    int dst_extent[FCUDA_ROUTE_MAX];
+} FcudaRoute;
+int fcuda_route_forward(const FcudaRoute* route, int batch, void* stream);
+/* ncnn's Slice rule, host only.  A blob of ncnn rank `rank` (1..3) is stored as (c, h, w) = shape[0..2] (rank 2: c = 1;
+ * rank 1: c = h = 1).  `axis` is the per-rank axis (rank 3: 0 = c, 1 = h, 2 = w; rank 2: 0 = h, 1 = w; rank 1: 0 = w; a
+ * negative axis adds the rank); *storage_axis gets its index in (c, h, w).  Top i takes sizes[i] = slices[i], or for
+ * slices[i] == -233 (extent - taken) / (count - i) where taken is what tops 0..i-1 took; the tops may leave a remainder.
+ * -100: NULL pointers, count < 1, rank outside 1..3, a shape entry < 1; -200: the axis out of range, a size below 1, or
+ * sizes past the extent. */
+int fcuda_slice_plan(int rank, int axis, const int* shape, const int* slices, int count, int* storage_axis, int* sizes);
+
 /* Kernel-variant switches for A/B measurements and tests.  Defaults are the measured-best configuration; the environment
  * variable FCUDA_<NAME> sets the initial value.  Names (value range, default):
  *   dw_vec (0-1, 1)           vectorised depthwise kernel on wide planes
@@ -475,6 +508,10 @@ int fcuda_yolo_detection_forward(float* output, const float* const* inputs, cons
  *                             layers) run on persistent CTAs that keep every filter k-block resident, gather the next
  *                             tile during the current one and write whole channel runs from a shared-memory staging
  *                             tile.  Bit-identical to 0 = the gathering kernel, one CTA per 128-pixel tile
+ *   route_fuse (0-1, 1)       read by feather::Net's fusion pass when a net first fuses: Concat (axis 0) ->
+ *                             ShuffleChannel -> Slice (axis 0) chains, or any two adjacent of them, run as one
+ *                             fcuda_route_forward launch.  Bit-identical to 0 = every routing layer on its own, while
+ *                             the net's other fusions stay as they are
  * Every variant computes the same result (tests/test_gpu_variants.py).  Returns 0 / the value, -200 for an unknown name or value. */
 int fcuda_set_tuning(const char* name, int value);
 int fcuda_get_tuning(const char* name);
@@ -488,7 +525,8 @@ int fcuda_profile_collect(double* total_ms, double* algo_flops, double* mma_flop
 /* Same, per kernel class, for every instrumented launch (the enable switch above covers all of them):
  * kind 0 TensorGEMM, 1 implicit-GEMM conv, 2 Winograd input transform, 3 Winograd output transform, 4 pooling,
  * 5 depthwise, 6 element-wise (BN/Scale/Eltwise/Clip/PReLU), 7 deconvolution scatter / depthwise gather, 8 resize / crop (Interp,
- * Crop), 9 detection (Permute, axis Softmax, PriorBox, decode, NMS, merge; YOLO decode, select, mask, sweep), < 0 all.  algo_bytes = the bytes the operation must move (inputs
+ * Crop), 9 detection (Permute, axis Softmax, PriorBox, decode, NMS, merge; YOLO decode, select, mask, sweep), 10 channel
+ * routing (fcuda_route_forward), < 0 all.  algo_bytes = the bytes the operation must move (inputs
  * read once + outputs written once). */
 int fcuda_profile_collect_kind(int kind, double* total_ms, double* algo_flops, double* mma_flops, double* algo_bytes,
                                long long* launches);
