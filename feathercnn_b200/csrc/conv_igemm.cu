@@ -359,68 +359,89 @@ static bool bf16_filters_fit(const IgemmProblem& p, int BN) {
            static_cast<unsigned long long>(ceil_div(p.KH * p.KW * p.IC, 32)) * igemm_ocpad(p.OC) * 128ull < (1ull << 31);
 }
 
-// Profile record of an implicit-GEMM launch: the layer's algorithmic work (direct-convolution FLOPs; input + filters read
-// once, output written once) and the MMA work issued over `tile_pixels` (padded) pixels x `n_cols` channels x `kblocks`.
-static int prof_igemm(const IgemmProblem& p, cudaStream_t stream, long long tile_pixels, int n_cols, int kblocks) {
+// The fields every implicit-GEMM kernel's arguments (IgemmArgs, StemArgs, HaloArgs) hold: the output and its fused
+// epilogue, and the source of the filters.  Each struct keeps its own field order: ptxas allocates registers by the
+// kernel's parameter offsets, and a common leading block changed the register counts of the gathering, halo and
+// pre-split kernels and gave some of them stack frames.
+template <class Args>
+static void fill_common(Args& a, const IgemmProblem& p) {
+    a.residual = p.epi.residual; a.out = p.output; a.bias = p.epi.bias;
+    a.wbf = reinterpret_cast<const unsigned char*>(p.w_hi);
+    a.OC = p.OC; a.OH = p.OH; a.OW = p.OW;
+    a.out_img_c = p.out_c_total > 0 ? p.out_c_total : p.OC;
+    a.kblocks = ceil_div(p.KH * p.KW * p.IC, 32);
+    a.act = p.epi.act; a.lo = p.epi.lo; a.hi = p.epi.hi;
+    a.pool = p.epi.pool;
+    a.wbf_kb_bytes = 2u * static_cast<unsigned>(igemm_ocpad(p.OC)) * 64u;
+}
+
+// The gathering and stem kernels index in 32 bits: input and output planes, the packed tap offsets dy << 16 | dx and,
+// unless IC % 32 == 0, the k-table's element offsets ic * H * W + dy * W + dx
+static bool igemm_offsets_fit(const IgemmProblem& p) {
+    const int dil_h = p.dil_h > 1 ? p.dil_h : 1, dil_w = p.dil_w > 1 ? p.dil_w : 1;
+    const long long table_max = static_cast<long long>(p.IC - 1) * p.H * p.W + static_cast<long long>(p.KH - 1) * dil_h * p.W +
+                                static_cast<long long>(p.KW - 1) * dil_w;
+    return static_cast<long long>(p.H) * p.W < (1ll << 30) && static_cast<long long>(p.OH) * p.OW < (1ll << 30) &&
+           (p.KH - 1) * dil_h < (1 << 15) && (p.KW - 1) * dil_w < (1 << 16) && (p.IC % 32 == 0 || table_max < (1ll << 31));
+}
+
+// Launch of an implicit-GEMM kernel with `smem` bytes of dynamic shared memory: `ctas` CTAs, or with `persistent` as
+// many as fit on the device at once, at most `ctas`.  Its profile record holds the layer's algorithmic work
+// (direct-convolution FLOPs; input + filters read once, output written once) and the MMA work issued over
+// `tile_pixels` (padded) pixels x `n_cols` channels x `kblocks`.
+template <auto Kernel, class... Params>
+int launch_igemm_kernel(const IgemmProblem& p, cudaStream_t stream, int threads, int smem, long long ctas, bool persistent,
+                        long long tile_pixels, int n_cols, int kblocks, const Params&... params) {
+    static SmemAttrCache attr_cache;
+    if (int rc = ensure_dynamic_smem(Kernel, smem, attr_cache)) return rc;
+    unsigned grid = static_cast<unsigned>(ctas);
+    if (persistent)
+        if (int rc = persistent_grid(Kernel, threads, smem, ctas, &grid)) return rc;
     const int taps = p.KH * p.KW;
     const double macs = static_cast<double>(p.N) * p.OC * p.OH * p.OW * p.IC * taps;
     const double mma = 2.0 * static_cast<double>(tile_pixels) * n_cols * (kblocks * 32) * (p.planes >= 2 ? 3 : 1);
-    return prof_begin(stream, PROF_IGEMM, 2.0 * macs, mma,
-                      4.0 * (static_cast<double>(p.N) * p.IC * p.H * p.W + static_cast<double>(p.OC) * taps * p.IC +
-                             static_cast<double>(p.N) * p.OC * p.OH * p.OW * (p.epi.residual ? 2 : 1)));
+    const int prof = prof_begin(stream, PROF_IGEMM, 2.0 * macs, mma,
+                                4.0 * (static_cast<double>(p.N) * p.IC * p.H * p.W + static_cast<double>(p.OC) * taps * p.IC +
+                                       static_cast<double>(p.N) * p.OC * p.OH * p.OW * (p.epi.residual ? 2 : 1)));
+    Kernel<<<grid, threads, smem, stream>>>(params...);
+    prof_end(prof, stream);
+    FCUDA_CHECK_LAUNCH();
+    count_launch();
+    return 0;
 }
 
 template <int BN, int PLANES, bool CLIP>
 int launch_igemm(const IgemmProblem& p, cudaStream_t stream) {
     constexpr bool BF = PLANES == 3;
     constexpr int NPL = BF ? 2 : PLANES;
-    const int taps = p.KH * p.KW;
-    const int K = taps * p.IC;
     CUtensorMap tmW, tmWlo;
     if (int rc = filter_maps(p, BN, PLANES, &tmW, &tmWlo)) return rc;
     if (BF && !bf16_filters_fit(p, BN)) return -1;
     IgemmArgs a;
-    a.wbf = reinterpret_cast<const unsigned char*>(p.w_hi);
-    a.wbf_kb_bytes = 2u * static_cast<unsigned>(igemm_ocpad(p.OC)) * 64u;
-    a.in = p.input; a.out = p.output; a.bias = p.epi.bias; a.residual = p.epi.residual;
-    a.N = p.N; a.IC = p.IC; a.H = p.H; a.W = p.W; a.OC = p.OC; a.OH = p.OH; a.OW = p.OW;
-    a.KH = p.KH; a.KW = p.KW; a.pad_top = p.pad_top; a.pad_left = p.pad_left;
+    fill_common(a, p);
+    a.in = p.input;
+    a.N = p.N; a.KH = p.KH;
+    a.IC = p.IC; a.H = p.H; a.W = p.W;
+    a.KW = p.KW; a.pad_top = p.pad_top; a.pad_left = p.pad_left;
     a.stride_h = p.stride_h; a.stride_w = p.stride_w;
     a.dil_h = p.dil_h > 1 ? p.dil_h : 1; a.dil_w = p.dil_w > 1 ? p.dil_w : 1;
     a.in_img_c = p.in_c_total > 0 ? p.in_c_total : p.IC;
-    a.out_img_c = p.out_c_total > 0 ? p.out_c_total : p.OC;
-    a.K = K;
-    a.kblocks = ceil_div(K, 32);
+    a.taps = p.KH * p.KW;
+    a.K = a.taps * p.IC;
     a.use_table = (p.IC % 32 == 0) ? 0 : 1;
-    a.taps = taps;
     a.num_n = ceil_div(p.OC, BN);
     a.total_pix = static_cast<long long>(p.N) * p.OH * p.OW;
-    a.act = p.epi.act; a.lo = p.epi.lo; a.hi = p.epi.hi;
-    a.pool = p.epi.pool;
     a.tiles_x = ceil_div(p.OW, 64);
     a.tiles_y = ceil_div(p.OH, 2);
     const long long pixel_tiles = a.pool ? static_cast<long long>(p.N) * a.tiles_x * a.tiles_y : (a.total_pix + 127) / 128;
     const long long total = pixel_tiles * a.num_n;
-    // 32-bit plane strides and packed tap offsets (dy << 16 | dx) inside the kernel; the k-table's element offsets
-    // ic * H * W + dy * W + dx are 32-bit as well
-    const long long table_max = static_cast<long long>(p.IC - 1) * p.H * p.W + static_cast<long long>(p.KH - 1) * a.dil_h * p.W +
-                                static_cast<long long>(p.KW - 1) * a.dil_w;
-    if (total >= (1ll << 31) || static_cast<long long>(p.H) * p.W >= (1ll << 30) || static_cast<long long>(p.OH) * p.OW >= (1ll << 30) ||
-        (p.KH - 1) * a.dil_h >= (1 << 15) || (p.KW - 1) * a.dil_w >= (1 << 16) || (a.use_table && table_max >= (1ll << 31)))
-        return -1;
+    if (total >= (1ll << 31) || !igemm_offsets_fit(p)) return -1;
     constexpr int kStage = NPL * BN * 32 * (BF ? 2 : 4);
     const int table_bytes = a.use_table ? a.kblocks * 32 * 8 : 0;
     const int smem = kStagesIg * kStage + table_bytes + 1024;
     if (smem > 227 * 1024) return -1;
-    auto kern = conv_igemm_kernel<BN, PLANES, CLIP>;
-    static SmemAttrCache attr_cache;
-    if (int rc = ensure_dynamic_smem(kern, smem, attr_cache)) return rc;
-    const int prof = prof_igemm(p, stream, pixel_tiles * 128, a.num_n * BN, a.kblocks);
-    kern<<<static_cast<unsigned>(total), kThreadsIg, smem, stream>>>(tmW, tmWlo, a);
-    prof_end(prof, stream);
-    FCUDA_CHECK_LAUNCH();
-    count_launch();
-    return 0;
+    return launch_igemm_kernel<conv_igemm_kernel<BN, PLANES, CLIP>>(p, stream, kThreadsIg, smem, total, false,
+                                                                    pixel_tiles * 128, a.num_n * BN, a.kblocks, tmW, tmWlo, a);
 }
 
 // ===================================================================================================================
@@ -458,6 +479,8 @@ struct StemArgs {
     int vec;                       // 16-byte stores: `out` 16-byte aligned and oplane % 4 == 0
     const unsigned char* wbf;
     unsigned wbf_kb_bytes;
+    const float* residual;         // the fields below are not read: the stem kernel fuses no residual or pooling
+    int OH, pool;
 };
 
 template <int BN, bool CLIP>
@@ -604,47 +627,29 @@ static int stem_smem_bytes(int BN, int kblocks, int nbuf) {
 
 static bool stem_supported(const IgemmProblem& p) {
     const int K = p.KH * p.KW * p.IC;
-    if (!conv_igemm_supported(p.IC, p.KH, p.KW) || p.planes != 3 || p.IC % 32 == 0 || K > kStemMaxK || p.OC > 128 ||
-        p.epi.residual != nullptr || p.epi.pool ||
-        p.dil_h > 1 || p.dil_w > 1 || p.OH < 1 || p.OW < 1)
-        return false;
-    // 32-bit planes, packed tap offsets (dy << 16 | dx) and k-table offsets ic * H * W + dy * W + dx
-    const long long table_max = static_cast<long long>(p.IC - 1) * p.H * p.W + static_cast<long long>(p.KH - 1) * p.W + p.KW - 1;
-    return static_cast<long long>(p.H) * p.W < (1ll << 30) && static_cast<long long>(p.OH) * p.OW < (1ll << 30) &&
-           p.KH - 1 < (1 << 15) && p.KW - 1 < (1 << 16) && table_max < (1ll << 31);
+    return conv_igemm_supported(p.IC, p.KH, p.KW) && p.planes == 3 && p.IC % 32 != 0 && K <= kStemMaxK && p.OC <= 128 &&
+           p.epi.residual == nullptr && !p.epi.pool && p.dil_h <= 1 && p.dil_w <= 1 && p.OH >= 1 && p.OW >= 1 &&
+           igemm_offsets_fit(p);
 }
 
 template <int BN, bool CLIP>
 int launch_stem(const IgemmProblem& p, cudaStream_t stream) {
     if (!bf16_filters_fit(p, BN)) return -1;
     StemArgs a;
-    a.in = p.input; a.out = p.output; a.bias = p.epi.bias;
-    a.IC = p.IC; a.H = p.H; a.W = p.W; a.OC = p.OC; a.OW = p.OW; a.oplane = p.OH * p.OW;
+    fill_common(a, p);
+    a.in = p.input;
+    a.IC = p.IC; a.H = p.H; a.W = p.W; a.oplane = p.OH * p.OW;
     a.pad_top = p.pad_top; a.pad_left = p.pad_left; a.stride_h = p.stride_h; a.stride_w = p.stride_w;
     a.in_img_c = p.in_c_total > 0 ? p.in_c_total : p.IC;
-    a.out_img_c = p.out_c_total > 0 ? p.out_c_total : p.OC;
     a.K = p.KH * p.KW * p.IC;
-    a.kblocks = ceil_div(a.K, 32);
     a.KW = p.KW;
-    a.act = p.epi.act; a.lo = p.epi.lo; a.hi = p.epi.hi;
     a.tiles_per_img = ceil_div(a.oplane, 128);
     a.tiles = static_cast<long long>(p.N) * a.tiles_per_img;
     a.nbuf = stem_smem_bytes(BN, a.kblocks, 2) <= 227 * 1024 ? 2 : 1;
     a.vec = (reinterpret_cast<uintptr_t>(p.output) & 15) == 0 && a.oplane % 4 == 0;
-    a.wbf = reinterpret_cast<const unsigned char*>(p.w_hi);
-    a.wbf_kb_bytes = 2u * static_cast<unsigned>(igemm_ocpad(p.OC)) * 64u;
     const int smem = stem_smem_bytes(BN, a.kblocks, a.nbuf);
-    auto kern = conv_igemm_stem_kernel<BN, CLIP>;
-    static SmemAttrCache attr_cache;
-    if (int rc = ensure_dynamic_smem(kern, smem, attr_cache)) return rc;
-    unsigned grid = 0;
-    if (int rc = persistent_grid(kern, kStemThreads, smem, a.tiles, &grid)) return rc;
-    const int prof = prof_igemm(p, stream, a.tiles * 128, BN, a.kblocks);
-    kern<<<grid, kStemThreads, smem, stream>>>(a);
-    prof_end(prof, stream);
-    FCUDA_CHECK_LAUNCH();
-    count_launch();
-    return 0;
+    return launch_igemm_kernel<conv_igemm_stem_kernel<BN, CLIP>>(p, stream, kStemThreads, smem, a.tiles, true, a.tiles * 128,
+                                                                 BN, a.kblocks, a);
 }
 
 // ===================================================================================================================
@@ -921,18 +926,12 @@ __device__ __forceinline__ void halo_body(const CUtensorMap& tmX, const CUtensor
     }
 }
 
-// The per-tap halo kernel without / with a Clip (see conv_igemm_wide_kernel below).
-template <int BN, int PLANES>
+// The per-tap halo kernel (CLIP: see conv_igemm_wide_kernel below).
+template <int BN, int PLANES, bool CLIP>
 __global__ void __launch_bounds__(kThreadsIg, 1)
 conv_igemm_halo_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__ CUtensorMap tmW,
                        const __grid_constant__ CUtensorMap tmWlo, const HaloArgs args) {
-    halo_body<BN, PLANES, false>(tmX, tmW, tmWlo, args);
-}
-template <int BN, int PLANES>
-__global__ void __launch_bounds__(kThreadsIg, 1)
-conv_igemm_halo_clip_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__ CUtensorMap tmW,
-                            const __grid_constant__ CUtensorMap tmWlo, const HaloArgs args) {
-    halo_body<BN, PLANES, true>(tmX, tmW, tmWlo, args);
+    halo_body<BN, PLANES, CLIP>(tmX, tmW, tmWlo, args);
 }
 
 // Pre-split halo kernel (BF16x3, switch igemm_presplit): the producer and the filter ring of conv_igemm_halo_kernel, but
@@ -1091,16 +1090,11 @@ __device__ __forceinline__ void presplit_body(const CUtensorMap& tmX, const Halo
     }
 }
 
-// The pre-split kernel without / with a Clip (see conv_igemm_wide_kernel below).
-template <int BN>
+// The pre-split kernel (CLIP: see conv_igemm_wide_kernel below).
+template <int BN, bool CLIP>
 __global__ void __launch_bounds__(kThreadsIg, 1)
 conv_igemm_presplit_kernel(const __grid_constant__ CUtensorMap tmX, const HaloArgs args) {
-    presplit_body<BN, false>(tmX, args);
-}
-template <int BN>
-__global__ void __launch_bounds__(kThreadsIg, 1)
-conv_igemm_presplit_clip_kernel(const __grid_constant__ CUtensorMap tmX, const HaloArgs args) {
-    presplit_body<BN, true>(tmX, args);
+    presplit_body<BN, CLIP>(tmX, args);
 }
 
 // Wide pre-split kernel (BF16x3, switch igemm_wide): the GEMM of conv_igemm_presplit_kernel turned around,
@@ -1343,17 +1337,13 @@ __device__ __forceinline__ void wide_body(const CUtensorMap& tmX, const HaloArgs
     }
 }
 
-// The wide kernel without / with a Clip: conv_igemm_wide_kernel serves no activation and ReLU with the ReLU epilogue of
-// the other kernels (fmaxf(v, 0)); conv_igemm_wide_clip_kernel clamps to [args.lo, args.hi].
-template <int BN>
+// The wide kernel.  Without CLIP it serves no activation and ReLU with the ReLU epilogue of the other kernels
+// (fmaxf(v, 0)); the CLIP instantiation clamps to [args.lo, args.hi].  The two stay separate instantiations, so the
+// ReLU kernels keep their own code and registers.
+template <int BN, bool CLIP>
 __global__ void __launch_bounds__(kThreadsIg, 1)
 conv_igemm_wide_kernel(const __grid_constant__ CUtensorMap tmX, const HaloArgs args) {
-    wide_body<BN, false>(tmX, args);
-}
-template <int BN>
-__global__ void __launch_bounds__(kThreadsIg, 1)
-conv_igemm_wide_clip_kernel(const __grid_constant__ CUtensorMap tmX, const HaloArgs args) {
-    wide_body<BN, true>(tmX, args);
+    wide_body<BN, CLIP>(tmX, args);
 }
 
 // Bank model of one ld.shared of the halo gather: lane l reads column l / 4 of channel plane (l % 4) * (2 for the bf16
@@ -1462,31 +1452,6 @@ static int halo_input_map(const IgemmProblem& p, const HaloGeom& hg, int chans, 
     return 0;
 }
 
-static HaloArgs halo_args(const IgemmProblem& p, const HaloGeom& hg, int BN) {
-    const int taps = p.KH * p.KW;
-    HaloArgs a;
-    a.residual = p.epi.residual; a.out = p.output; a.bias = p.epi.bias;
-    a.OC = p.OC; a.OH = p.OH; a.OW = p.OW; a.KW = p.KW; a.taps = taps;
-    a.out_img_c = p.out_c_total > 0 ? p.out_c_total : p.OC;
-    a.kblocks = ceil_div(taps * p.IC, 32);
-    a.num_n = ceil_div(p.OC, BN);
-    a.act = p.epi.act; a.lo = p.epi.lo; a.hi = p.epi.hi;
-    a.pool = p.epi.pool;
-    a.R = hg.R; a.C = hg.C;
-    a.tiles_x = ceil_div(p.OW, hg.C);
-    a.tiles_y = ceil_div(p.OH, hg.R);
-    a.Rb = hg.Rb; a.Cb = hg.Cb;
-    a.pad_top = p.pad_top;
-    a.xpad = (p.pad_left + 3) & ~3;
-    a.xshift = a.xpad - p.pad_left;
-    a.tiles = static_cast<long long>(p.N) * a.tiles_x * a.tiles_y * a.num_n;
-    a.wbf = reinterpret_cast<const unsigned char*>(p.w_hi);
-    a.wbf_kb_bytes = 2u * static_cast<unsigned>(igemm_ocpad(p.OC)) * 64u;
-    a.pr = hg.R + p.KH - 1;
-    a.pc = hg.C + p.KW - 1;
-    return a;
-}
-
 // Launch of a halo-family kernel on tile geometry hg: input boxes of `box_chans` channels, `smem` bytes of dynamic shared
 // memory, persistent CTAs.  `wmaps` are the filter tensor maps conv_igemm_halo_kernel takes.
 template <auto Kernel, class... Maps>
@@ -1495,19 +1460,24 @@ int launch_halo_family(const IgemmProblem& p, const HaloGeom& hg, int BN, int sm
     CUtensorMap tmX;
     if (int rc = halo_input_map(p, hg, box_chans, &tmX)) return rc;
     if (p.planes == 3 && !bf16_filters_fit(p, BN)) return -1;
-    const HaloArgs a = halo_args(p, hg, BN);
+    HaloArgs a;
+    fill_common(a, p);
+    a.KW = p.KW; a.taps = p.KH * p.KW;
+    a.num_n = ceil_div(p.OC, BN);
+    a.R = hg.R; a.C = hg.C;
+    a.tiles_x = ceil_div(p.OW, hg.C);
+    a.tiles_y = ceil_div(p.OH, hg.R);
+    a.Rb = hg.Rb; a.Cb = hg.Cb;
+    a.pad_top = p.pad_top;
+    a.xpad = (p.pad_left + 3) & ~3;
+    a.xshift = a.xpad - p.pad_left;
+    a.tiles = static_cast<long long>(p.N) * a.tiles_x * a.tiles_y * a.num_n;
+    a.pr = hg.R + p.KH - 1;
+    a.pc = hg.C + p.KW - 1;
     if (static_cast<long long>(p.OH) * p.OW >= (1ll << 30) || a.tiles * a.kblocks >= (1ll << 31)) return -1;
-    static SmemAttrCache attr_cache;
-    if (int rc = ensure_dynamic_smem(Kernel, smem, attr_cache)) return rc;
-    unsigned grid = 0;
-    if (int rc = persistent_grid(Kernel, kThreadsIg, smem, a.tiles, &grid)) return rc;
     // the issued MMA work includes the padded tile pixels
-    const int prof = prof_igemm(p, stream, a.tiles / a.num_n * hg.R * hg.C, a.num_n * BN, a.kblocks);
-    Kernel<<<grid, kThreadsIg, smem, stream>>>(tmX, wmaps..., a);
-    prof_end(prof, stream);
-    FCUDA_CHECK_LAUNCH();
-    count_launch();
-    return 0;
+    return launch_igemm_kernel<Kernel>(p, stream, kThreadsIg, smem, a.tiles, true, a.tiles / a.num_n * hg.R * hg.C,
+                                       a.num_n * BN, a.kblocks, tmX, wmaps..., a);
 }
 
 // The kernel a layer takes for one N tile and operand format: the gathering kernel, or with switch igemm_halo on a
@@ -1526,21 +1496,15 @@ int launch_conv(const IgemmProblem& p, cudaStream_t stream) {
         if (tune_get(TUNE_IGEMM_PRESPLIT) != 0 && presplit_geometry(p, pg)) {
             HaloGeom wg;
             if constexpr (BN != 32)  // wide_geometry takes N tiles of 64 and 128 channels only
-                if (tune_get(TUNE_IGEMM_WIDE) != 0 && wide_geometry(p, wg)) {
-                    if constexpr (CLIP)
-                        return launch_halo_family<conv_igemm_wide_clip_kernel<BN>>(p, wg, BN, wide_smem_bytes(p, wg), 16, stream);
-                    return launch_halo_family<conv_igemm_wide_kernel<BN>>(p, wg, BN, wide_smem_bytes(p, wg), 16, stream);
-                }
-            if constexpr (CLIP)
-                return launch_halo_family<conv_igemm_presplit_clip_kernel<BN>>(p, pg, BN, presplit_smem_bytes(p, pg), 32, stream);
-            return launch_halo_family<conv_igemm_presplit_kernel<BN>>(p, pg, BN, presplit_smem_bytes(p, pg), 32, stream);
+                if (tune_get(TUNE_IGEMM_WIDE) != 0 && wide_geometry(p, wg))
+                    return launch_halo_family<conv_igemm_wide_kernel<BN, CLIP>>(p, wg, BN, wide_smem_bytes(p, wg), 16, stream);
+            return launch_halo_family<conv_igemm_presplit_kernel<BN, CLIP>>(p, pg, BN, presplit_smem_bytes(p, pg), 32, stream);
         }
     }
     CUtensorMap tmW, tmWlo;
     if (int rc = filter_maps(p, BN, PLANES, &tmW, &tmWlo)) return rc;
     const int smem = halo_smem_bytes(p.OC, PLANES, hg.Rb, hg.Cb);
-    if constexpr (CLIP) return launch_halo_family<conv_igemm_halo_clip_kernel<BN, PLANES>>(p, hg, BN, smem, 32, stream, tmW, tmWlo);
-    return launch_halo_family<conv_igemm_halo_kernel<BN, PLANES>>(p, hg, BN, smem, 32, stream, tmW, tmWlo);
+    return launch_halo_family<conv_igemm_halo_kernel<BN, PLANES, CLIP>>(p, hg, BN, smem, 32, stream, tmW, tmWlo);
 }
 
 // The geometry query behind the exported conv_igemm_*_geometry: g is written only when the layer takes the kernel

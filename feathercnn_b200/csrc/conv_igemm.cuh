@@ -11,7 +11,7 @@ struct IgemmProblem {
     float* output;        // (N, OC, OH, OW)
     int N, IC, H, W, OC, OH, OW;
     int KH, KW, pad_top, pad_left, stride_h, stride_w;
-    int planes;           // 1 = TF32, 2 = 3xTF32, 3 = BF16x3 (w_hi / w_lo then hold the two bf16 planes)
+    int planes;           // 1 = TF32, 2 = 3xTF32, 3 = BF16x3 (w_hi then holds both pre-tiled bf16 planes)
     ConvEpilogue epi;     // every field is read; with epi.pool `output` is (N, OC, (OH+1)/2, (OW+1)/2)
     // Extensions beyond the reference (it rejects both: conv_layer.h:43-47, avx/booster.cpp:304-308); 0 = default.
     int dil_h, dil_w;       // dilation (0 or 1 = dense taps)
@@ -19,16 +19,18 @@ struct IgemmProblem {
     int out_c_total;        // same for output / residual (grouped convolution = one launch per group on slices)
 };
 
-// KH*KW <= 63 and, unless IC % 32 == 0, KH*KW*IC <= 8192 (shared-memory k-table).
+// KH*KW <= 63 and, unless IC % 32 == 0, KH*KW*IC <= 6144 (shared-memory k-table).
 bool conv_igemm_supported(int IC, int KH, int KW);
-// Floats of the packed filter buffer ([OC][Kf] per plane, Kf = KH*KW*IC rounded up to 4).
+// Floats of the packed filter buffer: [OC][Kf] per plane (Kf = KH*KW*IC rounded up to 4), or with planes >= 2 at
+// least the pre-tiled BF16x3 planes.
 size_t conv_igemm_packed_floats(int OC, int IC, int taps, int planes);
 // raw (OC, IC, KH, KW) -> [OC][Kf] hi (+ lo) planes.
-// bf16x3 != 0: w_hi / w_lo receive the two bf16 planes q1 = RN(w), q2 = RN(w - q1), rows of Kf8 = K rounded up to 8
-// (they fit the float planes sized above).
+// bf16x3 != 0: w_hi receives both bf16 planes q1 = RN(w), q2 = RN(w - q1), pre-tiled per (32-wide k-block, N tile) in
+// the un-swizzled core-matrix order of wgmma, so that one bulk copy fetches a filter stage; w_lo is not written.
 int conv_igemm_pack_weights(const float* w, float* w_hi, float* w_lo, int OC, int IC, int taps, cudaStream_t s,
                             int bf16x3 = 0);
-// True when the launch can apply a fused 2x2 / stride-2 max pooling (the 3x3 stride-1 slab kernel without a residual).
+// True when the launch can apply a fused 2x2 / stride-2 max pooling: 3x3, stride 1, no dilation, IC % 32 == 0, pads
+// <= 2, W % 4 == 0, a 16-byte aligned (or not yet known) input and no residual.
 bool conv_igemm_can_pool(const IgemmProblem& p);
 // Output patch (R x C pixels) and shared-memory halo box (Rb x Cb) of the halo kernel conv_igemm_forward uses for
 // stride-1, dense layers with IC % 32 == 0 and W % 4 == 0 (switch igemm_halo); false when the layer keeps the

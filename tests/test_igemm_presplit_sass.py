@@ -13,8 +13,8 @@ from pathlib import Path
 import pytest
 
 ROOT = Path(__file__).resolve().parents[1]
-NEW = r"conv_igemm_presplit_kernelILi(32|64|128)EE"
-OLD = r"conv_igemm_halo_kernelILi(32|64|128)ELi3EE"
+NEW = r"conv_igemm_presplit_kernelILi(32|64|128)ELb0EE"
+OLD = r"conv_igemm_halo_kernelILi(32|64|128)ELi3ELb0EE"
 
 
 def _functions():

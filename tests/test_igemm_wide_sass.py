@@ -5,7 +5,7 @@ import collections
 
 from test_igemm_presplit_sass import _functions, _kernels, main_loop
 
-NEW = r"conv_igemm_wide_kernelILi(64|128)EE"
+NEW = r"conv_igemm_wide_kernelILi(64|128)ELb0EE"
 
 
 def test_wide_switch_is_registered():

@@ -45,7 +45,8 @@ def _kernels(ops, pattern):
     (r"tensor_gemm_pipe_kernelILi(32|64|128)ELi1E", 4),    # TF32 TensorGEMM
     (r"conv_igemm_kernelILi(32|64|128)ELi3E", 6),          # BF16x3 gathering implicit GEMM: 3 MMAs x 2 k-steps
     (r"conv_igemm_kernelILi(32|64|128)ELi1E", 4),          # TF32 gathering implicit GEMM
-    (r"conv_igemm_halo_kernelILi(32|64|128)ELi3E", 6),     # BF16x3 per-tap halo implicit GEMM
+    pytest.param(r"conv_igemm_halo_kernelILi(32|64|128)ELi3ELb0E", 6,  # BF16x3 per-tap halo implicit GEMM
+                 id="conv_igemm_halo_kernelILi(32|64|128)ELi3E-6"),
 ])
 def test_wgmma_are_not_serialised(pattern, per_group):
     ops = _sass_ops()
