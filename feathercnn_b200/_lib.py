@@ -170,6 +170,8 @@ def fcuda() -> ctypes.CDLL:
             "fcuda_relu_forward": (i, [vp, vp, sz, vp]),
             "fcuda_clip_forward": (i, [vp, vp, sz, ctypes.c_float, ctypes.c_float, vp]),
             "fcuda_prelu_forward": (i, [vp, vp, i, sz, vp, i, i, vp]),
+            "fcuda_normalize_workspace_size": (i, [i, i, i, sz, i, szp]),
+            "fcuda_normalize_forward": (i, [vp, vp, i, sz, vp, i, i, i, f, i, vp, i, vp]),
             "fcuda_softmax_forward": (i, [vp, vp, sz, i, vp]),
             "fcuda_dropout_forward": (i, [vp, vp, sz, ctypes.c_float, vp]),
             "fcuda_copy_channels": (i, [vp, i, i, vp, i, sz, i, vp]),

@@ -564,6 +564,25 @@ def prelu(x, slope, out=None):
     return out
 
 
+def normalize(x, scale, across_spatial=0, across_channel=1, eps=1e-4, eps_mode=0, out=None):
+    """ncnn Normalize over (N, C, ...): y = (x * a) * scale[c], a from the sum of squares over each pixel's channels
+    (across_spatial 0), the whole image (1, 1) or each channel plane (1, 0); a one-element `scale` is shared
+    (include/fcuda.h).  The workspace comes from torch.  `out` may be `x`."""
+    lib = fcuda()
+    n, c = x.shape[:2]
+    plane = x[0, 0].numel()
+    ws = ctypes.c_size_t(0)
+    _check("fcuda_normalize_workspace_size",
+           lib.fcuda_normalize_workspace_size(int(across_spatial), int(across_channel), c, plane, n, ctypes.byref(ws)))
+    workspace = torch.empty(ws.value, device=x.device, dtype=torch.float32) if ws.value else None
+    out = torch.empty_like(x) if out is None else out
+    _check("fcuda_normalize_forward",
+           lib.fcuda_normalize_forward(_ptr(out), _ptr(x.contiguous()), c, plane, _ptr(scale.contiguous()), scale.numel(),
+                                       int(across_spatial), int(across_channel), float(eps), int(eps_mode),
+                                       _ptr(workspace), n, _stream()))
+    return out
+
+
 def softmax(x):
     out = torch.empty_like(x)
     _check("fcuda_softmax_forward",

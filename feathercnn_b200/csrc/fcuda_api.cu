@@ -9,6 +9,7 @@
 #include "depthwise.cuh"
 #include "detection.cuh"
 #include "layers.cuh"
+#include "normalize.cuh"
 #include "pack.cuh"
 #include "preprocess.cuh"
 #include "resize.cuh"
@@ -790,6 +791,37 @@ int fcuda_prelu_forward(float* output, const float* input, int channels, size_t 
     if (!output || !input || !slope || channels <= 0 || plane == 0 || batch < 1) return -100;
     if (num_slope != 1 && num_slope != channels) return -200;
     return prelu(input, output, slope, channels, plane, num_slope == 1, batch, as_stream(stream));
+}
+
+static int normalize_params_ok(int across_spatial, int across_channel, float eps, int eps_mode) {
+    return (across_spatial || across_channel) && eps_mode >= 0 && eps_mode <= 2 && eps >= 0.f;  // NaN eps fails >=
+}
+
+int fcuda_normalize_workspace_size(int across_spatial, int across_channel, int channels, size_t plane, int batch,
+                                   size_t* floats) {
+    if (!floats || channels < 1 || plane == 0 || batch < 1) return -100;
+    if (!across_spatial && !across_channel) return -200;
+    *floats = normalize_workspace_floats(across_spatial != 0, across_channel != 0, channels, plane, batch);
+    return 0;
+}
+
+int fcuda_normalize_forward(float* output, const float* input, int channels, size_t plane, const float* scale,
+                            int num_scale, int across_spatial, int across_channel, float eps, int eps_mode,
+                            float* workspace, int batch, void* stream) {
+    if (!output || !input || !scale || channels < 1 || plane == 0 || batch < 1) return -100;
+    if ((num_scale != 1 && num_scale != channels) || !normalize_params_ok(across_spatial, across_channel, eps, eps_mode))
+        return -200;
+    if (across_spatial && !workspace) return -100;
+    NormalizeGeom g;
+    g.channels = channels;
+    g.plane = plane;
+    g.batch = batch;
+    g.across_spatial = across_spatial != 0;
+    g.across_channel = across_channel != 0;
+    g.shared = num_scale == 1;
+    g.eps = eps;
+    g.eps_mode = eps_mode;
+    return normalize_forward(input, output, scale, g, workspace, as_stream(stream));
 }
 
 int fcuda_softmax_forward(float* output, const float* input, size_t n_per_image, int batch, void* stream) {

@@ -1,7 +1,7 @@
 // Built-in layer registrations: the 13 ncnn type names the reference serves (/root/reference/src/layer_factory.cpp:53-68)
 // plus Deconvolution / DeconvolutionDepthWise, Interp, Crop, Clip, PReLU, SSD's Permute, Flatten, Reshape, PriorBox and
-// DetectionOutput, YOLO's YoloDetectionOutput and Yolov3DetectionOutput, and ShuffleNet's ShuffleChannel and Slice, 28 in
-// all, mapped onto this host's layer classes.  A table of {type name, factory} pairs instead of one macro line per layer; the
+// DetectionOutput, VGG-SSD's Normalize, YOLO's YoloDetectionOutput and Yolov3DetectionOutput, and ShuffleNet's ShuffleChannel
+// and Slice, 29 in all, mapped onto this host's layer classes.  A table of {type name, factory} pairs instead of one macro line per layer; the
 // DEFINE_LAYER_CREATOR / REGISTER_LAYER_CREATOR macros of <feather/layer_factory.h> remain the plugin API for user layers.
 #include <feather/layer_factory.h>
 
@@ -15,6 +15,7 @@
 #include "layers/eltwise_layer.h"
 #include "layers/inner_product_layer.h"
 #include "layers/misc_layers.h"
+#include "layers/normalize_layer.h"
 #include "layers/pooling_layer.h"
 #include "layers/relu_layer.h"
 #include "layers/resize_layers.h"
@@ -64,6 +65,7 @@ const BuiltIn kBuiltIns[] = {
     {"Reshape", make_layer<ReshapeLayer>},
     {"PriorBox", make_layer<PriorBoxLayer>},
     {"DetectionOutput", make_layer<DetectionOutputLayer>},
+    {"Normalize", make_layer<NormalizeLayer>},
     {"YoloDetectionOutput", make_layer<YoloDetectionOutputLayer>},
     {"Yolov3DetectionOutput", make_layer<Yolov3DetectionOutputLayer>},
     {"ShuffleChannel", make_layer<ShuffleChannelLayer>},

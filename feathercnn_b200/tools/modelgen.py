@@ -6,7 +6,7 @@ weight blobs, raw fp32 for bias/BN/Scale blobs) — /root/reference/src/net.cpp:
 snapshot, and there is no network for pretrained checkpoints, so benchmarks and tests use random-init
 models of the architectures BASELINE.json names: a single 3x3 conv, VGG-16, ResNet-50 (Caffe topology:
 BN + Scale + ReLU as separate layers, Split/Eltwise residuals), MobileNet-v1, MobileNet-v2 (ReLU6 as Clip), plus a small "mini" net
-that exercises every layer type, single-shot detectors (MobileNet-SSD, a two-head tiny SSD), YOLO detectors
+that exercises every layer type, single-shot detectors (MobileNet-SSD, VGG-SSD 300, a two-head tiny SSD), YOLO detectors
 (MobileNet-YOLOv2, MobileNet-v2 YOLOv3, a two-scale tiny YOLOv3) and ShuffleNet-v2 with a small routing probe net.  Weight statistics follow
 SURVEY.md §8(d).
 """
@@ -121,6 +121,25 @@ class ModelWriter:
         assert slopes.shape == (n,), slopes.shape
         self._layer("PReLU", name, [bottom], [top], {0: n})
         self._weights(slopes, False)
+        self.shape[top] = self.shape[bottom]
+        return top
+
+    def normalize(self, name, bottom, across_spatial=0, channel_shared=0, eps=1e-10, scale=20.0, across_channel=1,
+                  eps_mode=0, top=None):
+        """ncnn Normalize 0=across_spatial 1=channel_shared 2=eps 3=scale_data_size (4=across_channel, 9=eps_mode only
+        when not the defaults 1 / 0); the scales, raw fp32 in the bin, are all `scale` (SSD's initial value) or the array
+        given."""
+        top = top or name
+        c = self.shape[bottom][0]
+        n = 1 if channel_shared else c
+        scales = np.ascontiguousarray(np.broadcast_to(np.asarray(scale, np.float32), (n,)), np.float32)
+        params = {0: int(across_spatial), 1: int(channel_shared), 2: f"{eps:e}", 3: n}
+        if across_channel != 1:
+            params[4] = int(across_channel)
+        if eps_mode != 0:
+            params[9] = int(eps_mode)
+        self._layer("Normalize", name, [bottom], [top], params)
+        self._weights(scales, False)
         self.shape[top] = self.shape[bottom]
         return top
 
@@ -743,18 +762,19 @@ def deeplab_head_tiny(seed=0, size=32, classes=5) -> ModelWriter:
 
 def _ssd_heads(m: ModelWriter, data: str, sources, num_classes: int, conf_gain: float, conf_threshold: float,
                nms_top_k: int = 100, keep_top_k: int = 100):
-    """3x3 loc / conf heads and PriorBoxes on each (blob, min_sizes, max_sizes, aspect_ratios) source; Permute 0=3 ->
-    Flatten -> Concat, the conf branch through Reshape (w = classes) -> Softmax over the class axis -> Flatten; and
-    DetectionOutput (nms 0.45)."""
+    """3x3 loc / conf heads and PriorBoxes on each (blob, min_sizes, max_sizes, aspect_ratios[, step]) source (a step
+    writes PriorBox keys 11 / 12; without one the step is image / feature size); Permute 0=3 -> Flatten -> Concat, the
+    conf branch through Reshape (w = classes) -> Softmax over the class axis -> Flatten; and DetectionOutput (nms 0.45)."""
     locs, confs, priors = [], [], []
-    for src, mins, maxs, ars in sources:
+    for src, mins, maxs, ars, *step in sources:
         per_loc = len(mins) * (1 + (1 if maxs else 0) + 2 * sum(abs(a - 1) >= 1e-6 for a in ars))
         fan_in = m.shape[src][0] * 9
         x = m.conv(f"{src}_mbox_loc", src, per_loc * 4, 3, 1, 1, True)
         locs.append(m.flatten(f"{src}_mbox_loc_flat", m.permute(f"{src}_mbox_loc_perm", x, 3)))
         x = m.conv(f"{src}_mbox_conf", src, per_loc * num_classes, 3, 1, 1, True, gain=conf_gain * np.sqrt(2.0 / fan_in))
         confs.append(m.flatten(f"{src}_mbox_conf_flat", m.permute(f"{src}_mbox_conf_perm", x, 3)))
-        priors.append(m.priorbox(f"{src}_mbox_priorbox", src, data, mins, maxs, ars, flip=True, clip=False))
+        priors.append(m.priorbox(f"{src}_mbox_priorbox", src, data, mins, maxs, ars, flip=True, clip=False,
+                                 step=(step[0], step[0]) if step else None))
     loc = m.concat("mbox_loc", locs, axis=0)
     conf = m.concat("mbox_conf", confs, axis=0)
     pri = m.concat("mbox_priorbox", priors, axis=1)
@@ -803,6 +823,40 @@ def ssd_tiny(seed=0, size=64, num_classes=5, conf_threshold=0.05, conf_gain=3.0)
     a = m.relu("relu2", m.conv("conv2", x, 32, 3, 2, 1, True))
     b = m.relu("relu3", m.conv("conv3", a, 32, 3, 2, 1, True))
     _ssd_heads(m, data, [(a, [12.0], [], [2.0]), (b, [24.0], [40.0], [2.0, 3.0])], num_classes, conf_gain, conf_threshold)
+    return m
+
+
+def vgg_ssd(seed=0, size=300, num_classes=21, conf_threshold=0.01, conf_gain=1.0) -> ModelWriter:
+    """VGG-SSD 300 in weiliu89's Caffe layout: VGG-16 conv1_1 .. conv5_3 with ReLU, 2x2 / 2 pool1-4 (pool3 75 -> 38 by
+    ceil mode) and a 3x3 / 1 / pad 1 pool5; fc6 as a 3x3 convolution of 1024 channels with dilation 6 and pad 6, fc7 as a
+    1x1 of 1024; extras conv6_1/2 (1x1 256, 3x3 / 2 / pad 1 512: 10 x 10), conv7_1/2 (128, 256 / 2: 5 x 5), conv8_1/2 and
+    conv9_1/2 (128, 256 3x3 unpadded: 3 x 3, then 1 x 1); conv4_3_norm, a per-pixel Normalize of relu4_3 (eps 1e-10,
+    scales 20); 3x3 loc and conf heads with PriorBoxes (flip, no clip) on conv4_3_norm (min 30, max 60, aspect ratio 2,
+    step 8), fc7 (60 / 111, 2 and 3, 16), conv6_2 (111 / 162, 2 and 3, 32), conv7_2 (162 / 213, 2 and 3, 64), conv8_2
+    (213 / 264, 2, 100) and conv9_2 (264 / 315, 2, 300); DetectionOutput 0=21 1=0.45 2=400 3=200.  8732 priors at
+    300 x 300.  conf_gain scales the spread of the conf head's logits."""
+    m = ModelWriter(seed)
+    data = m.input("data", 3, size, size)
+    x = data
+    for si, (ch, n) in enumerate([(64, 2), (128, 2), (256, 3), (512, 3), (512, 3)], 1):
+        for li in range(1, n + 1):
+            x = m.relu(f"relu{si}_{li}", m.conv(f"conv{si}_{li}", x, ch, 3, 1, 1, True))
+        if si == 4:
+            conv4_3 = x
+        x = m.pool(f"pool{si}", x, 0, 3, 1, 1) if si == 5 else m.pool(f"pool{si}", x, 0, 2, 2)
+    x = m.relu("relu6", m.conv("fc6", x, 1024, 3, 1, 6, True, dilation=6))
+    fc7 = x = m.relu("relu7", m.conv("fc7", x, 1024, 1, 1, 0, True))
+    extras = []
+    for i, (mid, oc, stride, pad) in enumerate([(256, 512, 2, 1), (128, 256, 2, 1), (128, 256, 1, 0), (128, 256, 1, 0)], 6):
+        x = m.relu(f"conv{i}_1_relu", m.conv(f"conv{i}_1", x, mid, 1, 1, 0, True))
+        x = m.relu(f"conv{i}_2_relu", m.conv(f"conv{i}_2", x, oc, 3, stride, pad, True))
+        extras.append(x)
+    norm = m.normalize("conv4_3_norm", conv4_3, across_spatial=0, channel_shared=0, eps=1e-10, scale=20.0)
+    sources = [(norm, [30.0], [60.0], [2.0], 8.0), (fc7, [60.0], [111.0], [2.0, 3.0], 16.0)]
+    sources += [(e, [float(a)], [float(b)], ars, float(st)) for e, (a, b, ars, st) in
+                zip(extras, [(111, 162, [2.0, 3.0], 32), (162, 213, [2.0, 3.0], 64), (213, 264, [2.0], 100),
+                             (264, 315, [2.0], 300)])]
+    _ssd_heads(m, data, sources, num_classes, conf_gain, conf_threshold, nms_top_k=400, keep_top_k=200)
     return m
 
 
@@ -911,6 +965,7 @@ def yolo_tiny(seed=0, size=64, num_classes=5, confidence_threshold=0.05, head_ga
 ZOO = {"single_conv": single_conv, "vgg16": vgg16, "resnet50": resnet50, "mobilenet_v1": mobilenet_v1, "mini": mini,
        "decoder_tiny": decoder_tiny, "fcn8s_tiny": fcn8s_tiny, "deeplab_head_tiny": deeplab_head_tiny,
        "mobilenet_v2": mobilenet_v2, "prelu_tiny": prelu_tiny, "mobilenet_ssd": mobilenet_ssd, "ssd_tiny": ssd_tiny,
+       "vgg_ssd": vgg_ssd,
        "mobilenet_yolov2": mobilenet_yolov2, "mobilenetv2_yolov3": mobilenetv2_yolov3, "yolo_tiny": yolo_tiny,
        "shufflenet_v2": shufflenet_v2, "shuffle_tiny": shuffle_tiny}
 

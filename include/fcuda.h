@@ -192,6 +192,35 @@ int fcuda_clip_forward(float* output, const float* input, size_t n, float min, f
  * through.  `slope` is a device pointer.  In-place (output == input) is allowed. */
 int fcuda_prelu_forward(float* output, const float* input, int channels, size_t plane, const float* slope, int num_slope,
                         int batch, void* stream);
+/* ncnn's Normalize (the reference has none; SSD's conv4_3_norm) over (batch, channels, plane).  Per image, the reduction
+ * set R is: across_spatial 0 (across_channel must be 1): the `channels` values of one pixel; across_spatial 1,
+ * across_channel 1: the whole image; across_spatial 1, across_channel 0: the plane of one channel.  ssum = sum of x^2
+ * over R in fp32, and
+ *   eps_mode 0 (Caffe / MXNet)  a = 1 / sqrt(ssum + eps)
+ *   eps_mode 1 (PyTorch)        a = 1 / max(sqrt(ssum), eps)
+ *   eps_mode 2 (TensorFlow)     a = 1 / sqrt(max(ssum, eps))
+ * each operation rounded in fp32 (IEEE sqrt and division); then y = fl(fl(x * a) * s_c): the factor first, the scale
+ * second, with s_c = scale[0] when num_scale == 1 (shared) or scale[c] when num_scale == channels.  Nothing else is
+ * special-cased: an all-zero R gives 0 when eps > 0, and NaN (0 * inf) when eps == 0, in every eps_mode.
+ * Summation order (a result depends on its reduction set's values only: the same bits for any batch split, pointer
+ * alignment, in or out of place, eager or in a CUDA graph):
+ *   per pixel    warp w (0..7) adds the terms of channels w, w + 8, w + 16, ... in increasing order, one fmaf each,
+ *                then the eight warp partials are added in warp order;
+ *   across_spatial  the set, as one contiguous run of n floats, is cut into chunks of 8192; in a chunk thread t (0..255)
+ *                adds the terms of elements t, t + 256, ... in order by fmaf, a 32-lane xor-shuffle tree sums each
+ *                warp and the eight warp partials are added in warp order; the chunk sums are added lane-strided (lane
+ *                l: chunks l, l + 32, ... in order) and by a 32-lane xor-shuffle tree.
+ * The per-pixel mode is one launch that reads the blob once and writes it once (the tile of consecutive pixels stays in
+ * shared memory for C <= 1024; past that the write pass re-reads it, from L2) and needs no workspace.  The across_spatial
+ * modes take two launches through `workspace`: fcuda_normalize_workspace_size floats, written before they are read.
+ * No atomics.  In-place (output == input) is allowed.  Stream-ordered: allocates and synchronises nothing.
+ * -100: a NULL pointer (workspace only where its size is not 0), channels, plane or batch < 1.  -200: num_scale other
+ * than 1 or channels, eps_mode outside 0..2, across_spatial == across_channel == 0, a negative or NaN eps. */
+int fcuda_normalize_workspace_size(int across_spatial, int across_channel, int channels, size_t plane, int batch,
+                                   size_t* floats);
+int fcuda_normalize_forward(float* output, const float* input, int channels, size_t plane, const float* scale,
+                            int num_scale, int across_spatial, int across_channel, float eps, int eps_mode,
+                            float* workspace, int batch, void* stream);
 /* SoftmaxLayer::Forward (src/layers/softmax_layer.h:32-55): over each image's whole blob. */
 int fcuda_softmax_forward(float* output, const float* input, size_t n_per_image, int batch, void* stream);
 /* DropoutLayer::Forward (src/layers/dropout_layer.h:36-57): y = x*scale (copy when scale == 1). */
@@ -524,7 +553,7 @@ void fcuda_profile_tensor_gemm(int enable);
 int fcuda_profile_collect(double* total_ms, double* algo_flops, double* mma_flops, long long* launches);
 /* Same, per kernel class, for every instrumented launch (the enable switch above covers all of them):
  * kind 0 TensorGEMM, 1 implicit-GEMM conv, 2 Winograd input transform, 3 Winograd output transform, 4 pooling,
- * 5 depthwise, 6 element-wise (BN/Scale/Eltwise/Clip/PReLU), 7 deconvolution scatter / depthwise gather, 8 resize / crop (Interp,
+ * 5 depthwise, 6 element-wise (BN/Scale/Eltwise/Clip/PReLU/Normalize), 7 deconvolution scatter / depthwise gather, 8 resize / crop (Interp,
  * Crop), 9 detection (Permute, axis Softmax, PriorBox, decode, NMS, merge; YOLO decode, select, mask, sweep), 10 channel
  * routing (fcuda_route_forward), < 0 all.  algo_bytes = the bytes the operation must move (inputs
  * read once + outputs written once). */
