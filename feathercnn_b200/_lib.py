@@ -172,6 +172,7 @@ def fcuda() -> ctypes.CDLL:
             "fcuda_prelu_forward": (i, [vp, vp, i, sz, vp, i, i, vp]),
             "fcuda_normalize_workspace_size": (i, [i, i, i, sz, i, szp]),
             "fcuda_normalize_forward": (i, [vp, vp, i, sz, vp, i, i, i, f, i, vp, i, vp]),
+            "fcuda_lrn_forward": (i, [vp, vp, i, i, i, i, i, f, f, f, i, vp]),
             "fcuda_softmax_forward": (i, [vp, vp, sz, i, vp]),
             "fcuda_dropout_forward": (i, [vp, vp, sz, ctypes.c_float, vp]),
             "fcuda_copy_channels": (i, [vp, i, i, vp, i, sz, i, vp]),

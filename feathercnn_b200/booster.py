@@ -583,6 +583,19 @@ def normalize(x, scale, across_spatial=0, across_channel=1, eps=1e-4, eps_mode=0
     return out
 
 
+def lrn(x, region_type=0, local_size=5, alpha=1.0, beta=0.75, bias=1.0, out=None):
+    """ncnn LRN over (N, C, H, W): y = x * (bias + alpha / n * ss)^-beta, ss the sum of squares over `local_size`
+    neighbouring channels (region_type 0) or a local_size x local_size window of the plane (1; n = local_size^2)
+    (include/fcuda.h).  Out of place: `out` may not be `x`."""
+    n, c, h, w = x.shape
+    x = x.contiguous()
+    out = torch.empty_like(x) if out is None else out
+    _check("fcuda_lrn_forward",
+           fcuda().fcuda_lrn_forward(_ptr(out), _ptr(x), c, h, w, int(region_type), int(local_size), float(alpha),
+                                     float(beta), float(bias), n, _stream()))
+    return out
+
+
 def softmax(x):
     out = torch.empty_like(x)
     _check("fcuda_softmax_forward",

@@ -9,6 +9,7 @@
 #include "depthwise.cuh"
 #include "detection.cuh"
 #include "layers.cuh"
+#include "lrn.cuh"
 #include "normalize.cuh"
 #include "pack.cuh"
 #include "preprocess.cuh"
@@ -822,6 +823,23 @@ int fcuda_normalize_forward(float* output, const float* input, int channels, siz
     g.eps = eps;
     g.eps_mode = eps_mode;
     return normalize_forward(input, output, scale, g, workspace, as_stream(stream));
+}
+
+int fcuda_lrn_forward(float* output, const float* input, int channels, int h, int w, int region_type, int local_size,
+                      float alpha, float beta, float bias, int batch, void* stream) {
+    if (!output || !input || channels < 1 || h < 1 || w < 1 || batch < 1) return -100;
+    if (region_type < 0 || region_type > 1 || local_size < 1 || local_size % 2 == 0 || output == input) return -200;
+    LrnGeom g;
+    g.channels = channels;
+    g.h = h;
+    g.w = w;
+    g.batch = batch;
+    g.region = region_type;
+    g.local_size = local_size;
+    g.alpha = alpha;
+    g.beta = beta;
+    g.bias = bias;
+    return lrn_forward(input, output, g, as_stream(stream));
 }
 
 int fcuda_softmax_forward(float* output, const float* input, size_t n_per_image, int batch, void* stream) {

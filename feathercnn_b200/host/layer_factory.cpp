@@ -1,7 +1,8 @@
 // Built-in layer registrations: the 13 ncnn type names the reference serves (/root/reference/src/layer_factory.cpp:53-68)
 // plus Deconvolution / DeconvolutionDepthWise, Interp, Crop, Clip, PReLU, SSD's Permute, Flatten, Reshape, PriorBox and
-// DetectionOutput, VGG-SSD's Normalize, YOLO's YoloDetectionOutput and Yolov3DetectionOutput, and ShuffleNet's ShuffleChannel
-// and Slice, 29 in all, mapped onto this host's layer classes.  A table of {type name, factory} pairs instead of one macro line per layer; the
+// DetectionOutput, VGG-SSD's Normalize, YOLO's YoloDetectionOutput and Yolov3DetectionOutput, ShuffleNet's ShuffleChannel
+// and Slice, and AlexNet's and GoogLeNet's LRN, 30 in all, mapped onto this host's layer classes.  A table of {type name,
+// factory} pairs instead of one macro line per layer; the
 // DEFINE_LAYER_CREATOR / REGISTER_LAYER_CREATOR macros of <feather/layer_factory.h> remain the plugin API for user layers.
 #include <feather/layer_factory.h>
 
@@ -14,6 +15,7 @@
 #include "layers/detection_layers.h"
 #include "layers/eltwise_layer.h"
 #include "layers/inner_product_layer.h"
+#include "layers/lrn_layer.h"
 #include "layers/misc_layers.h"
 #include "layers/normalize_layer.h"
 #include "layers/pooling_layer.h"
@@ -70,6 +72,7 @@ const BuiltIn kBuiltIns[] = {
     {"Yolov3DetectionOutput", make_layer<Yolov3DetectionOutputLayer>},
     {"ShuffleChannel", make_layer<ShuffleChannelLayer>},
     {"Slice", make_layer<SliceLayer>},
+    {"LRN", make_layer<LRNLayer>},
 };
 
 }  // namespace

@@ -8,7 +8,10 @@ no caffe / protobuf-generated code is needed — and writes the ncnn text ``.par
 
 * layer grammar and parameter ids as ``ConvLayer::LoadParam`` & co. read them (``src/layers/*.h``; ids follow ncnn's
   caffe2ncnn): Convolution / ConvolutionDepthWise, Deconvolution / DeconvolutionDepthWise, InnerProduct, Pooling, ReLU, BatchNorm, Scale, Eltwise, Concat, Dropout,
-  Softmax, Split, Input, Crop, Clip, PReLU, Slice;
+  Softmax, Split, Input, Crop, Clip, PReLU, Slice, LRN;
+* LRN (``lrn_param``: ``local_size``, ``alpha``, ``beta``, ``norm_region``, ``k``) becomes ncnn's LRN
+  ``0=region 1=local_size 2=alpha 3=beta 4=bias``.  Caffe's WITHIN_CHANNEL LRN divides by a fixed ``1 + alpha / n * ss``
+  and ignores ``k``, so that region is written with ``4=1``; an even ``local_size`` (which Caffe rejects) is an error;
 * Slice (``slice_param``: ``axis`` or the older ``slice_dim``, ``slice_point``) becomes ncnn's Slice: the cut points become
   sizes with ``-233`` (the rest) for the last top, and no cut points an even split (``-233`` for every top).  Caffe has no
   ShuffleChannel in its upstream ``caffe.proto``, so that type keeps the "no counterpart" error;
@@ -326,6 +329,18 @@ def convert(caffemodel: bytes) -> tuple[str, bytes]:
             sizes = [b - a for a, b in zip([0] + points, points)] + [-233] if points else [-233] * len(tops)
             ps = f"-23300={len(sizes)}," + ",".join(str(s) for s in sizes)
             out.layer("Slice", name, bottoms, tops, ps + (f" 1={axis - 1}" if axis != 1 else ""))
+        elif type_ == "LRN":
+            # lrn_param = 118: local_size = 1 (5), alpha = 2 (1), beta = 3 (0.75), norm_region = 4 (ACROSS_CHANNELS), k = 5 (1)
+            p = parse_message(_first(L, 118, b""))
+            size = int(_first(p, 1, 5))
+            region = int(_first(p, 4, 0))
+            if size % 2 == 0:
+                raise ValueError(f"layer {name}: LRN local_size {size} is even (Caffe accepts odd sizes only)")
+            if region not in (0, 1):
+                raise ValueError(f"layer {name}: LRN norm_region {region} has no FeatherCNN counterpart")
+            bias = 1.0 if region == 1 else _f32(_first(p, 5), 1.0)  # Caffe's WITHIN_CHANNEL shifts by 1, not k
+            out.layer("LRN", name, bottoms, tops, f"0={region} 1={size} 2={_f32(_first(p, 2), 1.0):.8e} "
+                                                  f"3={_f32(_first(p, 3), 0.75):.8e} 4={bias:.8e}")
         elif type_ == "Dropout":
             out.layer("Dropout", name, bottoms, tops)   # identity at test time (dropout_layer.h:40-43)
         elif type_ == "Softmax":

@@ -5,7 +5,8 @@ weight blobs, raw fp32 for bias/BN/Scale blobs) — /root/reference/src/net.cpp:
 /root/reference/src/ncnn/modelbin.cpp:47-197.  Its own converter (``tools/``) is absent from the
 snapshot, and there is no network for pretrained checkpoints, so benchmarks and tests use random-init
 models of the architectures BASELINE.json names: a single 3x3 conv, VGG-16, ResNet-50 (Caffe topology:
-BN + Scale + ReLU as separate layers, Split/Eltwise residuals), MobileNet-v1, MobileNet-v2 (ReLU6 as Clip), plus a small "mini" net
+BN + Scale + ReLU as separate layers, Split/Eltwise residuals), MobileNet-v1, MobileNet-v2 (ReLU6 as Clip), GoogLeNet and
+AlexNet (BVLC's deploy nets, with LRN), plus a small "mini" net
 that exercises every layer type, single-shot detectors (MobileNet-SSD, VGG-SSD 300, a two-head tiny SSD), YOLO detectors
 (MobileNet-YOLOv2, MobileNet-v2 YOLOv3, a two-scale tiny YOLOv3) and ShuffleNet-v2 with a small routing probe net.  Weight statistics follow
 SURVEY.md §8(d).
@@ -140,6 +141,14 @@ class ModelWriter:
             params[9] = int(eps_mode)
         self._layer("Normalize", name, [bottom], [top], params)
         self._weights(scales, False)
+        self.shape[top] = self.shape[bottom]
+        return top
+
+    def lrn(self, name, bottom, local_size=5, alpha=1e-4, beta=0.75, bias=1.0, region=0, top=None):
+        """ncnn LRN 0=region_type 1=local_size 2=alpha 3=beta 4=bias (every key written); no weights."""
+        top = top or name
+        self._layer("LRN", name, [bottom], [top],
+                    {0: int(region), 1: int(local_size), 2: f"{alpha:e}", 3: f"{beta:e}", 4: f"{bias:e}"})
         self.shape[top] = self.shape[bottom]
         return top
 
@@ -860,6 +869,72 @@ def vgg_ssd(seed=0, size=300, num_classes=21, conf_threshold=0.01, conf_gain=1.0
     return m
 
 
+# BVLC GoogLeNet's inception modules: name, 1x1, 3x3 reduce, 3x3, 5x5 reduce, 5x5, pool projection
+GOOGLENET_INCEPTIONS = [("3a", 64, 96, 128, 16, 32, 32), ("3b", 128, 128, 192, 32, 96, 64),
+                        ("4a", 192, 96, 208, 16, 48, 64), ("4b", 160, 112, 224, 24, 64, 64),
+                        ("4c", 128, 128, 256, 24, 64, 64), ("4d", 112, 144, 288, 32, 64, 64),
+                        ("4e", 256, 160, 320, 32, 128, 128), ("5a", 256, 160, 320, 32, 128, 128),
+                        ("5b", 384, 192, 384, 48, 128, 128)]
+
+
+def googlenet(seed=0, num_classes=1000, size=224, lrn_alpha=1e-4) -> ModelWriter:
+    """BVLC GoogLeNet (Inception-v1), deploy net without the training-only auxiliary heads: conv1/7x7_s2 (pad 3) -> ReLU ->
+    pool1 3x3 / 2 -> norm1 (LRN 5, beta 0.75) -> conv2/3x3_reduce 1x1 64 -> ReLU -> conv2/3x3 192 -> ReLU -> norm2 -> pool2
+    3x3 / 2; nine inception modules (GOOGLENET_INCEPTIONS: outputs 256, 480, 512, 512, 512, 528, 832, 832, 1024), each
+    reading its input through an explicit 4-top Split (1x1; 3x3 reduce -> 3x3; 5x5 reduce -> 5x5; 3x3 / 1 / pad 1 max
+    pool -> 1x1 projection, every convolution with a ReLU) into a 4-bottom Concat; pool3 and pool4 3x3 / 2 after 3b and
+    4e; a 7x7 average pool, Dropout, the 1024 -> num_classes classifier and Softmax.  56 / 28 / 14 / 7 planes at 224.
+    lrn_alpha is both LRNs' alpha (the zoo's 1e-4 barely changes the activations; near 1 the factor varies widely)."""
+    m = ModelWriter(seed)
+    x = m.input("data", 3, size, size)
+    x = m.relu("conv1/relu_7x7", m.conv("conv1/7x7_s2", x, 64, 7, 2, 3, True))
+    x = m.pool("pool1/3x3_s2", x, 0, 3, 2)
+    x = m.lrn("pool1/norm1", x, 5, lrn_alpha, 0.75)
+    x = m.relu("conv2/relu_3x3_reduce", m.conv("conv2/3x3_reduce", x, 64, 1, 1, 0, True))
+    x = m.relu("conv2/relu_3x3", m.conv("conv2/3x3", x, 192, 3, 1, 1, True))
+    x = m.lrn("conv2/norm2", x, 5, lrn_alpha, 0.75)
+    x = m.pool("pool2/3x3_s2", x, 0, 3, 2)
+    for tag, c1, r3, c3, r5, c5, pp in GOOGLENET_INCEPTIONS:
+        if tag in ("4a", "5a"):
+            x = m.pool(f"pool{int(tag[0]) - 1}/3x3_s2", x, 0, 3, 2)
+        t = f"inception_{tag}"
+        a, b, c, d = m.split(f"{t}/split", x, [f"{t}/split_{i}" for i in range(4)])
+        a = m.relu(f"{t}/relu_1x1", m.conv(f"{t}/1x1", a, c1, 1, 1, 0, True))
+        b = m.relu(f"{t}/relu_3x3_reduce", m.conv(f"{t}/3x3_reduce", b, r3, 1, 1, 0, True))
+        b = m.relu(f"{t}/relu_3x3", m.conv(f"{t}/3x3", b, c3, 3, 1, 1, True))
+        c = m.relu(f"{t}/relu_5x5_reduce", m.conv(f"{t}/5x5_reduce", c, r5, 1, 1, 0, True))
+        c = m.relu(f"{t}/relu_5x5", m.conv(f"{t}/5x5", c, c5, 5, 1, 2, True))
+        d = m.pool(f"{t}/pool", d, 0, 3, 1, 1)
+        d = m.relu(f"{t}/relu_pool_proj", m.conv(f"{t}/pool_proj", d, pp, 1, 1, 0, True))
+        x = m.concat(f"{t}/output", [a, b, c, d])
+    x = m.pool("pool5/7x7_s1", x, 1, 7, 1)
+    x = m.dropout("pool5/drop_7x7_s1", x)
+    x = m.fc("loss3/classifier", x, num_classes)
+    m.softmax("prob", x)
+    return m
+
+
+def alexnet(seed=0, num_classes=1000, size=227, lrn_alpha=1e-4) -> ModelWriter:
+    """BVLC AlexNet, deploy net: conv1 11x11 / 4 96 -> ReLU -> norm1 (LRN 5, beta 0.75) -> pool1 3x3 / 2; conv2 5x5 pad 2
+    256 in 2 groups -> ReLU -> norm2 -> pool2; conv3 3x3 384, conv4 3x3 384 in 2 groups, conv5 3x3 256 in 2 groups (each
+    with a ReLU) -> pool5 3x3 / 2; fc6 9216 -> 4096, fc7 4096 (ReLU and Dropout after each), fc8 and Softmax.  55 / 27 /
+    13 / 6 planes at 227.  lrn_alpha as in googlenet()."""
+    m = ModelWriter(seed)
+    x = m.input("data", 3, size, size)
+    x = m.relu("relu1", m.conv("conv1", x, 96, 11, 4, 0, True))
+    x = m.pool("pool1", m.lrn("norm1", x, 5, lrn_alpha, 0.75), 0, 3, 2)
+    x = m.relu("relu2", m.conv("conv2", x, 256, 5, 1, 2, True, group=2))
+    x = m.pool("pool2", m.lrn("norm2", x, 5, lrn_alpha, 0.75), 0, 3, 2)
+    x = m.relu("relu3", m.conv("conv3", x, 384, 3, 1, 1, True))
+    x = m.relu("relu4", m.conv("conv4", x, 384, 3, 1, 1, True, group=2))
+    x = m.relu("relu5", m.conv("conv5", x, 256, 3, 1, 1, True, group=2))
+    x = m.pool("pool5", x, 0, 3, 2)
+    x = m.dropout("drop6", m.relu("relu6", m.fc("fc6", x, 4096)))
+    x = m.dropout("drop7", m.relu("relu7", m.fc("fc7", x, 4096)))
+    m.softmax("prob", m.fc("fc8", x, num_classes))
+    return m
+
+
 VOC_ANCHORS = [1.08, 1.19, 3.42, 4.41, 6.63, 11.38, 9.42, 5.11, 16.62, 10.52]  # YOLOv2 VOC, grid cells
 COCO_ANCHORS = [10, 13, 16, 30, 33, 23, 30, 61, 62, 45, 59, 119, 116, 90, 156, 198, 373, 326]  # YOLOv3, input pixels
 
@@ -965,7 +1040,7 @@ def yolo_tiny(seed=0, size=64, num_classes=5, confidence_threshold=0.05, head_ga
 ZOO = {"single_conv": single_conv, "vgg16": vgg16, "resnet50": resnet50, "mobilenet_v1": mobilenet_v1, "mini": mini,
        "decoder_tiny": decoder_tiny, "fcn8s_tiny": fcn8s_tiny, "deeplab_head_tiny": deeplab_head_tiny,
        "mobilenet_v2": mobilenet_v2, "prelu_tiny": prelu_tiny, "mobilenet_ssd": mobilenet_ssd, "ssd_tiny": ssd_tiny,
-       "vgg_ssd": vgg_ssd,
+       "vgg_ssd": vgg_ssd, "googlenet": googlenet, "alexnet": alexnet,
        "mobilenet_yolov2": mobilenet_yolov2, "mobilenetv2_yolov3": mobilenetv2_yolov3, "yolo_tiny": yolo_tiny,
        "shufflenet_v2": shufflenet_v2, "shuffle_tiny": shuffle_tiny}
 

@@ -221,6 +221,25 @@ int fcuda_normalize_workspace_size(int across_spatial, int across_channel, int c
 int fcuda_normalize_forward(float* output, const float* input, int channels, size_t plane, const float* scale,
                             int num_scale, int across_spatial, int across_channel, float eps, int eps_mode,
                             float* workspace, int batch, void* stream);
+/* ncnn's LRN (the reference has none; Caffe's local response normalisation in AlexNet, CaffeNet and GoogLeNet) over
+ * (batch, channels, h, w) with dense planes.  r = local_size / 2, sq(v) = fl(v * v), each square rounded on its own.
+ *   region_type 0 (ACROSS_CHANNELS)  ss(q, i, j) = sum of sq(x[p][i][j]) for p = max(0, q - r) .. min(C - 1, q + r) in
+ *                                    ascending p, one rounded add per term; a = fl(alpha / local_size).
+ *   region_type 1 (WITHIN_CHANNEL)   ss(q, i, j) = sum of sq(x[q][i + di][j + dj]) for di = -r .. r (outer) and
+ *                                    dj = -r .. r (inner), a term outside the plane being 0; a = fl(alpha / local_size^2).
+ * Then s = fl(bias + fl(a * ss)) and y = fl(x * powf(s, -beta)), each operation rounded in fp32 with no contraction and
+ * CUDA's full-precision powf.  Nothing is special-cased: s = 0 gives x * inf.  This is the order ncnn's CPU loop adds
+ * in, so the only difference from it is powf; a result depends only on the values in its window: the same bits for any
+ * batch split, pointer alignment, eager or in a CUDA graph.
+ * One launch, no workspace.  ACROSS_CHANNELS reads each input element from HBM once and writes each output once (every
+ * thread walks the channels of its pixels through a cp.async ring, 16-byte accesses when h * w % 4 == 0 and both
+ * pointers are 16-byte aligned); local_size 1, 3, 5 and 7 are compiled specialisations, larger sizes a generic kernel
+ * that reads each window through the cache.  WITHIN_CHANNEL squares a 2D tile and its r-wide halo once in shared memory.
+ * Out of place only.  Stream-ordered: allocates and synchronises nothing.
+ * -100: a NULL pointer, batch, channels, h or w < 1.  -200: region_type outside 0..1, local_size < 1 or even,
+ * output == input. */
+int fcuda_lrn_forward(float* output, const float* input, int channels, int h, int w, int region_type, int local_size,
+                      float alpha, float beta, float bias, int batch, void* stream);
 /* SoftmaxLayer::Forward (src/layers/softmax_layer.h:32-55): over each image's whole blob. */
 int fcuda_softmax_forward(float* output, const float* input, size_t n_per_image, int batch, void* stream);
 /* DropoutLayer::Forward (src/layers/dropout_layer.h:36-57): y = x*scale (copy when scale == 1). */
@@ -553,7 +572,7 @@ void fcuda_profile_tensor_gemm(int enable);
 int fcuda_profile_collect(double* total_ms, double* algo_flops, double* mma_flops, long long* launches);
 /* Same, per kernel class, for every instrumented launch (the enable switch above covers all of them):
  * kind 0 TensorGEMM, 1 implicit-GEMM conv, 2 Winograd input transform, 3 Winograd output transform, 4 pooling,
- * 5 depthwise, 6 element-wise (BN/Scale/Eltwise/Clip/PReLU/Normalize), 7 deconvolution scatter / depthwise gather, 8 resize / crop (Interp,
+ * 5 depthwise, 6 element-wise (BN/Scale/Eltwise/Clip/PReLU/Normalize/LRN), 7 deconvolution scatter / depthwise gather, 8 resize / crop (Interp,
  * Crop), 9 detection (Permute, axis Softmax, PriorBox, decode, NMS, merge; YOLO decode, select, mask, sweep), 10 channel
  * routing (fcuda_route_forward), < 0 all.  algo_bytes = the bytes the operation must move (inputs
  * read once + outputs written once). */
