@@ -117,13 +117,15 @@ class ConvBooster:
                fcuda().fcuda_conv_init(ctypes.byref(param), self.algo, _ptr(processed_kernel), kp, _stream()))
 
     def ForwardOpts(self, param: ConvParam, output, input, kernel, buffer, bias_arr, residual=None, relu_after_add=False,
-                    clip: tuple[float, float] | None = None, dilation: int = 1, pool: bool = False, batch: int = 1) -> None:
+                    clip: tuple[float, float] | None = None, dilation=1, pool: bool = False, batch: int = 1) -> None:
         """Forward with everything the epilogue can fuse (fcuda.h, FcudaConvOptions).  `clip` = (min, max) are the bounds
-        of param.activation == ACT_CLIP; a Clip without them is refused (-200), as are bounds without a Clip."""
+        of param.activation == ACT_CLIP; a Clip without them is refused (-200), as are bounds without a Clip.  `dilation`
+        is an int or an (h, w) pair."""
         if clip is None:
             clip = (math.nan, math.nan) if param.activation == ACT_CLIP else (0.0, 0.0)
+        dh, dw = _hw(dilation)
         o = FcudaConvOptions(residual=None if residual is None else _ptr(residual).value, relu_after_add=int(relu_after_add),
-                             clip_min=clip[0], clip_max=clip[1], dilation_h=dilation, dilation_w=dilation, pool=int(pool))
+                             clip_min=clip[0], clip_max=clip[1], dilation_h=dh, dilation_w=dw, pool=int(pool))
         _check("fcuda_conv_forward_opts",
                fcuda().fcuda_conv_forward_opts(ctypes.byref(param), self.algo, _ptr(output), _ptr(input), _ptr(kernel),
                                                _ptr(buffer), _ptr(bias_arr), ctypes.byref(o), batch, _stream()))
@@ -151,11 +153,12 @@ class ConvBooster:
 
 def conv_forward(param: ConvParam, x: torch.Tensor, w: torch.Tensor, b: torch.Tensor | None = None,
                  algo: int | None = None, residual: torch.Tensor | None = None,
-                 relu_after_add: bool = False, dilation: int = 1, tuned: bool = False,
+                 relu_after_add: bool = False, dilation=1, tuned: bool = False,
                  pool: bool = False, clip: tuple[float, float] | None = None) -> tuple[torch.Tensor, int]:
     """Whole ConvBooster protocol for a batch x (N, IC, H, W) -> (N, OC, OH, OW).  Returns (output, algo).
-    `residual` (shaped like the output), `clip` = (min, max) (param.activation must be ACT_CLIP), `dilation` (the caller
-    sets param.output_h/w for the dilated extent) and `pool` (the output is the pooled blob) are ForwardOpts's."""
+    `residual` (shaped like the output), `clip` = (min, max) (param.activation must be ACT_CLIP), `dilation` (an int or
+    an (h, w) pair; the caller sets param.output_h/w for the dilated extent) and `pool` (the output is the pooled blob)
+    are ForwardOpts's."""
     cb = ConvBooster()
     if algo is None:
         rc = cb.SelectAlgoTuned(param) if tuned else cb.SelectAlgo(param)

@@ -11,7 +11,10 @@
 #include "depthwise.cuh"
 #include "common.cuh"
 
+#include <stdint.h>
 #include <stdlib.h>
+
+#include <algorithm>
 
 namespace fcuda {
 
@@ -362,7 +365,122 @@ dw3x3_cols_kernel(const float* __restrict__ in, const float* __restrict__ w, con
     }
 }
 
-// Generic k x k / any stride / any padding depthwise: one thread per output element.
+// Dilated 3x3 / stride 1 depthwise (DeepLab's atrous backbones: pad = dilation on 33x33 or 65x65 planes, dilations 2 to 18).
+// One CTA per strip of up to kDilRows output rows of one plane.  The CTA stages the strip's input box, (rows + 2 dh) x
+// (OW + 2 dw), in shared memory with zeros where the box leaves the image, so the compute loop has no bounds checks.  The
+// image rows of the box are one contiguous span of the input: it is read with 16-byte loads between a scalar head and tail
+// whatever the plane width or pointer alignment, and each element is scattered to its box row by a reciprocal multiply.
+// Each input element comes from HBM once per layer; the 2 dh halo rows shared by neighbouring strips come again from L2.
+// A thread then marches one chain of outputs dh rows apart (rows rho, rho + dh, ...): consecutive outputs of a chain share
+// two of their three window rows, so each step reads one new window row (3 VEC values) from shared memory.  VEC = 4: a
+// thread owns four consecutive columns and stores them as one float4 (OW % 4 == 0 and a 16-byte aligned output).
+constexpr int kDilThreads = 128;
+constexpr int kDilRows = 64;       // output rows per strip, before balancing the strips of a plane
+constexpr int kDilChain = 4;       // outputs per chain segment: one thread's work item
+constexpr int kDilMaxBox = 12288;  // floats of the staged box (48 KB: no dynamic shared-memory opt-in)
+
+template <int VEC, bool CLIP>
+__global__ void __launch_bounds__(kDilThreads)
+dw3x3_dilated_kernel(const float* __restrict__ in, const float* __restrict__ w, const float* __restrict__ bias,
+                     float* __restrict__ out, DwGeom g, int TH, int strips, int BW, unsigned w_rcp, int act, float lo,
+                     float hi) {
+    extern __shared__ float box[];
+    const int tid = threadIdx.x;
+    const long long plane = blockIdx.x / strips;  // n * C + c
+    const int strip = static_cast<int>(blockIdx.x - plane * strips);
+    const int c = static_cast<int>(plane % g.C);
+    const int dh = g.dil_h, dw = g.dil_w;
+    const int oy0 = strip * TH, th = min(TH, g.OH - oy0);
+    const int BH = th + 2 * dh;
+    const int by0 = oy0 - g.pad_top;  // image row of box row 0
+    // box rows [r_lo, r_hi) hold image rows; the others, and the pad columns of these, are zero
+    const int r_lo = min(max(0, -by0), BH), r_hi = max(r_lo, min(BH, g.H - by0));
+    for (int i = tid; i < r_lo * BW; i += kDilThreads) box[i] = 0.f;
+    for (int i = r_hi * BW + tid; i < BH * BW; i += kDilThreads) box[i] = 0.f;
+    const int padl = min(g.pad_left, BW), padr = max(0, BW - g.pad_left - g.W), pc = padl + padr;
+    for (int i = tid; i < (r_hi - r_lo) * pc; i += kDilThreads) {
+        const int r = r_lo + i / pc, x = i % pc;
+        box[r * BW + (x < padl ? x : g.pad_left + g.W + x - padl)] = 0.f;
+    }
+    const float* src = in + plane * g.H * g.W + static_cast<long long>(by0 + r_lo) * g.W;
+    const int n = (r_hi - r_lo) * g.W;
+    // e < n <= kDilMaxBox keeps e * W far below 2^32: __umulhi(e, ceil(2^32 / W)) is exactly e / W
+    auto put = [&](int e, float v) {
+        const int r = static_cast<int>(__umulhi(static_cast<unsigned>(e), w_rcp));
+        const int col = g.pad_left + e - r * g.W;
+        if (col < BW) box[(r_lo + r) * BW + col] = v;
+    };
+    const int head = min(n, static_cast<int>(((16u - (static_cast<unsigned>(reinterpret_cast<uintptr_t>(src)) & 15u)) & 15u) >> 2));
+    if (tid < head) put(tid, __ldg(src + tid));
+    const int nq = (n - head) >> 2;
+    const float4* s4 = reinterpret_cast<const float4*>(src + head);
+    for (int q0 = tid; q0 < nq; q0 += 4 * kDilThreads) {
+        float4 v[4];  // four 16-byte loads in flight before the first shared-memory store
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+            const int q = q0 + j * kDilThreads;
+            v[j] = q < nq ? __ldg(s4 + q) : make_float4(0.f, 0.f, 0.f, 0.f);
+        }
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+            const int q = q0 + j * kDilThreads;
+            if (q < nq) {
+                const int e = head + 4 * q;
+                put(e, v[j].x); put(e + 1, v[j].y); put(e + 2, v[j].z); put(e + 3, v[j].w);
+            }
+        }
+    }
+    const int tail = head + 4 * nq + tid;
+    if (tail < n) put(tail, __ldg(src + tail));
+    float k[9];
+#pragma unroll
+    for (int i = 0; i < 9; ++i) k[i] = __ldg(w + c * 9 + i);
+    const float bv = bias ? __ldg(bias + c) : 0.f;
+    __syncthreads();
+
+    const int chains = min(dh, th), segs = ((th + dh - 1) / dh + kDilChain - 1) / kDilChain, xq = g.OW / VEC;
+    float* op = out + plane * g.OH * g.OW + static_cast<long long>(oy0) * g.OW;
+    for (int it = tid; it < xq * chains * segs; it += kDilThreads) {
+        const int ox = (it % xq) * VEC, rest = it / xq, rho = rest % chains, m0 = rest / chains * kDilChain;
+        const int len = (th - rho + dh - 1) / dh;  // outputs of chain rho
+        if (m0 >= len) continue;
+        const int m1 = min(m0 + kDilChain, len);
+        float a[3][VEC], b[3][VEC], cur[3][VEC];
+        auto row = [&](int m, float (&v)[3][VEC]) {  // box row rho + m * dh, columns ox + j * dw + i
+            const float* p = box + (rho + m * dh) * BW + ox;
+#pragma unroll
+            for (int j = 0; j < 3; ++j)
+#pragma unroll
+                for (int i = 0; i < VEC; ++i) v[j][i] = p[j * dw + i];
+        };
+        row(m0, a);
+        row(m0 + 1, b);
+        for (int m = m0; m < m1; ++m) {
+            row(m + 2, cur);
+            __align__(16) float o[VEC];
+#pragma unroll
+            for (int i = 0; i < VEC; ++i) {
+                float v = bv;
+#pragma unroll
+                for (int j = 0; j < 3; ++j) v = fmaf(k[j], a[j][i], v);
+#pragma unroll
+                for (int j = 0; j < 3; ++j) v = fmaf(k[3 + j], b[j][i], v);
+#pragma unroll
+                for (int j = 0; j < 3; ++j) v = fmaf(k[6 + j], cur[j][i], v);
+                o[i] = act ? act_clamp<CLIP>(v, lo, hi) : v;
+            }
+            float* dst = op + static_cast<long long>(rho + m * dh) * g.OW + ox;
+            if (VEC == 4) *reinterpret_cast<float4*>(dst) = *reinterpret_cast<const float4*>(o);
+            else dst[0] = o[0];
+#pragma unroll
+            for (int j = 0; j < 3; ++j)
+#pragma unroll
+                for (int i = 0; i < VEC; ++i) { a[j][i] = b[j][i]; b[j][i] = cur[j][i]; }
+        }
+    }
+}
+
+// Generic k x k / any stride / any padding / any dilation depthwise: one thread per output element.
 template <bool CLIP>
 __global__ void __launch_bounds__(256)
 dw_generic_kernel(const float* __restrict__ in, const float* __restrict__ w, const float* __restrict__ bias,
@@ -378,10 +496,10 @@ dw_generic_kernel(const float* __restrict__ in, const float* __restrict__ w, con
     const float* kp = w + static_cast<size_t>(c) * g.KH * g.KW;
     float v = 0.f;
     for (int u = 0; u < g.KH; ++u) {
-        const int iy = oy * g.stride_h - g.pad_top + u;
+        const int iy = oy * g.stride_h - g.pad_top + u * g.dil_h;
         if (iy < 0 || iy >= g.H) continue;
         for (int x = 0; x < g.KW; ++x) {
-            const int ix = ox * g.stride_w - g.pad_left + x;
+            const int ix = ox * g.stride_w - g.pad_left + x * g.dil_w;
             if (ix < 0 || ix >= g.W) continue;
             v = fmaf(__ldg(ip + static_cast<long long>(iy) * g.W + ix), __ldg(kp + u * g.KW + x), v);
         }
@@ -391,10 +509,45 @@ dw_generic_kernel(const float* __restrict__ in, const float* __restrict__ w, con
     out[idx] = v;
 }
 
+template <bool CLIP>
+static void dw_generic_launch(const float* in, const float* w, float* out, const DwGeom& g, const ConvEpilogue& e, int batch,
+                              cudaStream_t s) {
+    const long long total = static_cast<long long>(batch) * g.C * g.OH * g.OW;
+    dw_generic_kernel<CLIP><<<static_cast<unsigned>((total + 255) / 256), 256, 0, s>>>(in, w, e.bias, out, g, e.act, e.lo, e.hi, total);
+}
+
+// Strip height and box width of dw3x3_dilated_kernel for a dilated layer; false when the layer is not 3x3 / stride 1 or a
+// strip of one output row would not fit the box.
+static bool dil_strips(const DwGeom& g, int* TH, int* strips, int* BW) {
+    if (g.KH != 3 || g.KW != 3 || g.stride_h != 1 || g.stride_w != 1 || g.W < 2) return false;
+    const int bw = g.OW + 2 * g.dil_w;
+    const int fit = kDilMaxBox / bw - 2 * g.dil_h;  // most output rows whose box fits
+    if (fit < 1) return false;
+    const int n = ceil_div(g.OH, std::min(kDilRows, fit));
+    *strips = n;
+    *TH = ceil_div(g.OH, n);  // balanced strips
+    *BW = bw;
+    return true;
+}
+
 // The kernel choice of depthwise_forward; CLIP selects the Clip instantiations (act == 2).
 template <bool CLIP>
 static void dw_launch(const float* in, const float* w, float* out, const DwGeom& g, const ConvEpilogue& e, int batch,
                       cudaStream_t s) {
+    if (g.dil_h > 1 || g.dil_w > 1) {
+        int TH, strips, BW;
+        if (!dil_strips(g, &TH, &strips, &BW)) return dw_generic_launch<CLIP>(in, w, out, g, e, batch, s);
+        const unsigned blocks = static_cast<unsigned>(static_cast<long long>(batch) * g.C * strips);
+        const int smem = (TH + 2 * g.dil_h) * BW * static_cast<int>(sizeof(float));
+        const unsigned w_rcp = static_cast<unsigned>(((1ull << 32) + g.W - 1) / g.W);
+        if (g.OW % 4 == 0 && (reinterpret_cast<uintptr_t>(out) & 15) == 0)
+            dw3x3_dilated_kernel<4, CLIP><<<blocks, kDilThreads, smem, s>>>(in, w, e.bias, out, g, TH, strips, BW, w_rcp, e.act,
+                                                                          e.lo, e.hi);
+        else
+            dw3x3_dilated_kernel<1, CLIP><<<blocks, kDilThreads, smem, s>>>(in, w, e.bias, out, g, TH, strips, BW, w_rcp, e.act,
+                                                                          e.lo, e.hi);
+        return;
+    }
     const bool k3 = g.KH == 3 && g.KW == 3 && g.pad_top == 1 && g.pad_left == 1 && g.stride_h == g.stride_w &&
                     (g.stride_h == 1 || g.stride_h == 2) && g.OW >= 24;
     // vector width: the widest VEC whose strips (32 * VEC outputs) still fill most lanes and keep accesses aligned
@@ -452,13 +605,15 @@ static void dw_launch(const float* in, const float* w, float* out, const DwGeom&
             dw3x3_plane_kernel<2, CLIP><<<blocks, 128, smem, s>>>(in, w, e.bias, out, g.C, g.H, g.W, g.OH, g.OW, g.pad_top,
                                                              g.pad_left, e.act, e.lo, e.hi, planes_ll);
     } else {
-        const long long total = static_cast<long long>(batch) * g.C * g.OH * g.OW;
-        dw_generic_kernel<CLIP><<<static_cast<unsigned>((total + 255) / 256), 256, 0, s>>>(in, w, e.bias, out, g, e.act, e.lo, e.hi, total);
+        dw_generic_launch<CLIP>(in, w, out, g, e, batch, s);
     }
 }
 
-int depthwise_forward(const float* in, const float* w, float* out, const DwGeom& g, const ConvEpilogue& e, int batch,
+int depthwise_forward(const float* in, const float* w, float* out, const DwGeom& geom, const ConvEpilogue& e, int batch,
                       cudaStream_t s) {
+    DwGeom g = geom;
+    g.dil_h = std::max(g.dil_h, 1);
+    g.dil_w = std::max(g.dil_w, 1);
     const double planes = static_cast<double>(batch) * g.C;
     const int prof = prof_begin(s, PROF_DEPTHWISE, 2.0 * planes * g.OH * g.OW * g.KH * g.KW, 0,
                                 4.0 * planes * (static_cast<double>(g.H) * g.W + static_cast<double>(g.OH) * g.OW));

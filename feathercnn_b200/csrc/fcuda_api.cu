@@ -248,6 +248,7 @@ int make_plan(const FcudaConvParam* p, int algo, int batch, ConvPlan* plan) {
             g.C = IC; g.H = p->input_h; g.W = p->input_w; g.KH = p->kernel_h; g.KW = p->kernel_w;
             g.OH = p->output_h; g.OW = p->output_w; g.stride_h = p->stride_h; g.stride_w = p->stride_w;
             g.pad_top = p->pad_top; g.pad_left = p->pad_left;
+            g.dil_h = 1; g.dil_w = 1;  // conv_launch sets the layer's
             pl.scratch_floats = 0;
             pl.packed_floats = static_cast<size_t>(IC) * p->kernel_h * p->kernel_w;
             return 0;
@@ -503,8 +504,11 @@ static int conv_launch(const FcudaConvParam* p, const ConvPlan& pl, float* outpu
         }
         case FCUDA_NAIVE:
             return conv_direct(input, packed, output, pl.pg, OC, epi, batch, s);
-        case FCUDA_DEPTHWISE:
-            return depthwise_forward(input, packed, output, pl.dg, epi, batch, s);
+        case FCUDA_DEPTHWISE: {
+            DwGeom g = pl.dg;
+            g.dil_h = dil_h; g.dil_w = dil_w;
+            return depthwise_forward(input, packed, output, g, epi, batch, s);
+        }
         default:
             return -1;
     }
@@ -522,13 +526,14 @@ static int conv_forward(const FcudaConvParam* p, int algo, float* output, const 
     const bool clip = clip_bounds_given && p->activation == FCUDA_ACT_CLIP;
     if (clip && !(o.clip_min <= o.clip_max)) return -200;  // (a NaN bound too)
     if (clip_bounds_given && !clip && (o.clip_min != 0.f || o.clip_max != 0.f)) return -200;  // bounds without a Clip
-    if (dilated && algo != FCUDA_SGECONV) return -200;  // only the implicit GEMM spaces its taps
+    if (dilated && algo != FCUDA_SGECONV && algo != FCUDA_DEPTHWISE) return -200;  // only these space their taps
     // The implicit GEMM adds the residual in its epilogue when the convolution has no activation of its own; every other
     // case is the convolution, then the reference's add_relu in place.
     const bool fuse_residual = o.residual && algo == FCUDA_SGECONV && p->activation == FCUDA_ACT_NONE;
     if (dilated && o.residual && !fuse_residual) return -200;
     if (o.pool && !fcuda_conv_can_pool(p, algo)) return -200;
-    if ((clip && (o.residual || dilated || o.pool)) || (o.pool && (o.residual || dilated))) return -200;  // not built
+    // not built (a dilated depthwise clamps in its epilogue like an undilated one)
+    if ((clip && (o.residual || (dilated && algo != FCUDA_DEPTHWISE) || o.pool)) || (o.pool && (o.residual || dilated))) return -200;
     ConvPlan pl;
     int rc = make_plan(p, algo, batch, &pl);
     if (rc) return rc;

@@ -28,7 +28,7 @@ public:
     }
 
     int LoadParam(const ncnn::ParamDict& pd) {
-        // The reference rejects dilation > 1 (conv_layer.h:41-47); here the implicit-GEMM kernel spaces its taps (§8f rank 4)
+        // The reference rejects dilation > 1 (conv_layer.h:41-47); here the implicit-GEMM and depthwise kernels space their taps
         dilation_w = pd.get(2, 1);
         dilation_h = pd.get(12, dilation_w);
         if (dilation_w < 1 || dilation_h < 1) return FEATHER_ERR_UNSUPPORTED;
@@ -128,10 +128,8 @@ public:
         int rc = (reference_policy && !extension) ? conv_booster.SelectAlgo(&this->conv_param)
                                                   : conv_booster.SelectAlgoTuned(&this->conv_param);
         if (rc) return rc;
-        if (dilation_h > 1 || dilation_w > 1) {
-            if (conv_param.group > 1 && is_depthwise) return FEATHER_ERR_UNSUPPORTED;  // dilated depthwise: not built
-            conv_booster.ForceSelectAlgo(booster::SGECONV);
-        }
+        if (dilation_h > 1 || dilation_w > 1)  // the depthwise kernels and the implicit GEMM space their taps
+            conv_booster.ForceSelectAlgo(is_depthwise ? booster::DEPTHWISE : booster::SGECONV);
         if (const char* force = extension ? NULL : getenv("FEATHER_FORCE_CONV_ALGO")) {  // ForceSelectAlgo hook, avx/booster.cpp:313-317
             booster::ConvBooster forced;
             forced.ForceSelectAlgo(static_cast<booster::ConvAlgo>(atoi(force)));
@@ -221,7 +219,7 @@ public:
 
     // Net::ApplyFusion: absorb `Eltwise SUM(this->top, other) [+ReLU]` (a ResNet shortcut) into this layer's epilogue.
     int FuseResidual(Blob<float>* other, int relu) {
-        if (residual != NULL || fused_pool) return 0;
+        if (residual != NULL || fused_pool || (is_depthwise && (dilation_h > 1 || dilation_w > 1))) return 0;
         residual = other;
         relu_after_add = relu;
         return 1;
@@ -244,9 +242,10 @@ public:
         }
         if (next_layer->type.compare("Clip") == 0) {
             // after any BatchNorm / Scale folding, so conv -> BN -> Scale -> Clip is one kernel.  A Clip in the epilogue of a
-            // dilated convolution, or before a residual sum, is not built: there the Clip stays a layer of its own.
+            // dilated ordinary convolution, or before a residual sum, is not built: there the Clip stays a layer of its own.
+            // A dilated depthwise layer clamps in its epilogue like an undilated one.
             const ClipLayer* cl = dynamic_cast<const ClipLayer*>(next_layer);
-            if (!cl || residual != NULL || dilation_h > 1 || dilation_w > 1) return 0;
+            if (!cl || residual != NULL || (!is_depthwise && (dilation_h > 1 || dilation_w > 1))) return 0;
             conv_param.activation = booster::Clip;
             clip_min = cl->min_value;
             clip_max = cl->max_value;

@@ -769,6 +769,73 @@ def deeplab_head_tiny(seed=0, size=32, classes=5) -> ModelWriter:
     return m
 
 
+def _deeplabv3(m: ModelWriter, x: str, table, output_stride: int, aspp: int, num_classes: int, size: int) -> str:
+    """DeepLab-v3's atrous backbone and mobile ASPP head on `x` (after a stride-2 stem).  The MobileNet-v2 blocks of `table`
+    ((t, c, n, s, k) rows) follow TF-DeepLab's rule: once the stride so far equals `output_stride`, a block's stride becomes
+    1, that layer keeps the current rate, and every later depthwise layer runs at the rate times that stride (pad = rate,
+    pad = rate * (k - 1) / 2 for k != 3)."""
+    stride_so_far, rate = 2, 1
+    for bi, (t, c, n, s, k) in enumerate(table, 2):
+        for i in range(n):
+            tag = f"{bi}_{i + 1}"
+            stride, layer_rate = s if i == 0 else 1, rate
+            if stride_so_far == output_stride:
+                rate *= stride
+                stride = 1
+            else:
+                stride_so_far *= stride
+            ic = m.shape[x][0]
+            shortcut = stride == 1 and ic == c
+            if shortcut:
+                sc, x = m.split(f"block{tag}_split", x, [f"block{tag}_in_a", f"block{tag}_in_b"])
+            y = x
+            if t != 1:
+                y = m.conv(f"conv{tag}_expand", y, ic * t, 1, 1, 0, False)
+                y = _bn_scale_clip(m, f"_conv{tag}_expand", y)
+            y = m.conv(f"conv{tag}_dw", y, ic * t, k, stride, layer_rate * (k - 1) // 2, False, group=ic * t,
+                       dilation=layer_rate)
+            y = _bn_scale_clip(m, f"_conv{tag}_dw", y)
+            y = m.conv(f"conv{tag}_linear", y, c, 1, 1, 0, False)
+            y = _bn_scale_clip(m, f"_conv{tag}_linear", y, clip=False, center=0.3 if shortcut else 1.0)
+            x = m.eltwise(f"block{tag}", [sc, y]) if shortcut else y
+    _, fh, fw = m.shape[x]
+    feat_a, feat_b = m.split("aspp_split", x, ["aspp_in_a", "aspp_in_b"])
+    p = m.pool("image_pool", feat_a, 1, 1, 1, 0, global_pooling=True)
+    p = _bn_scale_relu(m, "_image_pool_conv", m.conv("image_pool_conv", p, aspp, 1, 1, 0, False))
+    p = m.interp("image_pool_up", p, 2, out_h=fh, out_w=fw)
+    b = _bn_scale_relu(m, "_aspp0", m.conv("aspp0", feat_b, aspp, 1, 1, 0, False))
+    y = m.concat("aspp_concat", [p, b])
+    y = _bn_scale_relu(m, "_aspp_proj", m.conv("aspp_proj", y, aspp, 1, 1, 0, False))
+    y = m.conv("logits", y, num_classes, 1, 1, 0, True)
+    return m.interp("logits_up", y, 2, out_h=size, out_w=size, align_corner=1)
+
+
+def deeplabv3_mobilenet_v2(seed=0, size=513, num_classes=21, output_stride=16) -> ModelWriter:
+    """DeepLab-v3 (Chen et al. 2017) on MobileNet-v2, as TF-DeepLab's mobilenet_v2 variant: `mobilenet_v2`'s stem and
+    blocks up to the 320 one, with the last strides turned into depthwise dilations so the features stay at
+    `output_stride` 8 (65 x 65 for a 513 input) or 16 (33 x 33), then the mobile ASPP head (image pooling and a 1x1 branch,
+    256 channels) and a bilinear Interp (align_corner) of the logits back to `size`."""
+    assert output_stride in (8, 16), output_stride
+    m = ModelWriter(seed)
+    x = m.input("data", 3, size, size)
+    x = _bn_scale_clip(m, "_conv1", m.conv("conv1", x, 32, 3, 2, 1, False))
+    table = [(1, 16, 1, 1, 3), (6, 24, 2, 2, 3), (6, 32, 3, 2, 3), (6, 64, 4, 2, 3), (6, 96, 3, 1, 3), (6, 160, 3, 2, 3),
+             (6, 320, 1, 1, 3)]
+    _deeplabv3(m, x, table, output_stride, 256, num_classes, size)
+    return m
+
+
+def deeplabv3_tiny(seed=0, size=65, num_classes=5) -> ModelWriter:
+    """A small DeepLab-v3 for fast tests: 65 x 65 input, at most 48 channels, output stride 8.  Its dilated depthwise
+    layers run at dilation 2 and 4 (3x3, the shared-memory kernel) and one 5x5 layer at dilation 2 takes the generic one."""
+    m = ModelWriter(seed)
+    x = m.input("data", 3, size, size)
+    x = _bn_scale_clip(m, "_conv1", m.conv("conv1", x, 8, 3, 2, 1, False))
+    table = [(1, 8, 1, 1, 3), (2, 8, 1, 2, 3), (2, 16, 2, 2, 3), (2, 16, 2, 2, 3), (2, 24, 1, 1, 5), (2, 24, 2, 2, 3)]
+    _deeplabv3(m, x, table, 8, 16, num_classes, size)
+    return m
+
+
 def _ssd_heads(m: ModelWriter, data: str, sources, num_classes: int, conf_gain: float, conf_threshold: float,
                nms_top_k: int = 100, keep_top_k: int = 100):
     """3x3 loc / conf heads and PriorBoxes on each (blob, min_sizes, max_sizes, aspect_ratios[, step]) source (a step
@@ -1042,7 +1109,8 @@ ZOO = {"single_conv": single_conv, "vgg16": vgg16, "resnet50": resnet50, "mobile
        "mobilenet_v2": mobilenet_v2, "prelu_tiny": prelu_tiny, "mobilenet_ssd": mobilenet_ssd, "ssd_tiny": ssd_tiny,
        "vgg_ssd": vgg_ssd, "googlenet": googlenet, "alexnet": alexnet,
        "mobilenet_yolov2": mobilenet_yolov2, "mobilenetv2_yolov3": mobilenetv2_yolov3, "yolo_tiny": yolo_tiny,
-       "shufflenet_v2": shufflenet_v2, "shuffle_tiny": shuffle_tiny}
+       "shufflenet_v2": shufflenet_v2, "shuffle_tiny": shuffle_tiny, "deeplabv3_mobilenet_v2": deeplabv3_mobilenet_v2,
+       "deeplabv3_tiny": deeplabv3_tiny}
 
 
 def synthetic_input(shape, index: int = 0) -> np.ndarray:

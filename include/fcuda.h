@@ -117,13 +117,20 @@ int fcuda_conv_forward(const FcudaConvParam* param, int algo, float* output, con
  *                   returns the non-NaN operand); ncnn's compare-and-assign Clip passes NaN through.  -200 for
  *                   clip_min > clip_max or a NaN bound, and for a non-zero bound with any other activation.
  *   dilation_h/w    tap spacing, 0 meaning 1 (the reference rejects it, src/layers/conv_layer.h:43-47).  > 1:
- *                   FCUDA_SGECONV only (-200 otherwise, and with a residual it cannot add in its epilogue); the caller sets
- *                   param->output_h/w for the dilated extent out = (in + pads - dilation*(k-1) - 1) / stride + 1.  < 0: -100.
+ *                   FCUDA_SGECONV and FCUDA_DEPTHWISE only (-200 otherwise, and -200 with a residual that the algorithm
+ *                   cannot add in its epilogue, which FCUDA_DEPTHWISE never does); the caller sets param->output_h/w for the
+ *                   dilated extent out = (in + pads - dilation*(k-1) - 1) / stride + 1.  < 0: -100.
+ *                   FCUDA_DEPTHWISE with a dilation: a 3x3 / stride-1 layer (DeepLab's atrous backbone, pad = dilation)
+ *                   computes each output as v = bias, then the nine taps in row-major order, each v = fmaf(w, x, v) with
+ *                   x = 0 outside the image, then the activation's clamp.  Every other kernel size or stride adds the taps
+ *                   inside the image in row-major order by fmaf from 0, then the bias, then the clamp.  Either way an
+ *                   output depends only on its own window, so the bits do not change with the batch split, the pointers'
+ *                   alignment or CUDA-graph replay.  A dilation of 1 runs the undilated depthwise kernels unchanged.
  *   pool            non-zero: a FOLLOWING 2x2 / stride-2 / pad-0 max pooling (ConvLayer::Forward then PoolingLayer::Forward,
  *                   src/layers/pooling_layer.h:38-91): `output` is the pooled blob (batch, OC, (OH+1)/2, (OW+1)/2), ceil
  *                   mode, windows clipped at the border like the reference.  -200 unless fcuda_conv_can_pool.
- * Not built, -200: Clip together with a residual, a dilation or the pooling; the pooling together with a residual or a
- * dilation. */
+ * Not built, -200: Clip together with a residual or the pooling, or with a dilation outside FCUDA_DEPTHWISE; the pooling
+ * together with a residual or a dilation. */
 typedef struct FcudaConvOptions {
     const float* residual;
     int relu_after_add;
