@@ -81,16 +81,6 @@ static inline int ensure_dynamic_smem(Kernel kern, int bytes, SmemAttrCache& cac
     return 0;
 }
 
-// Grid of a persistent kernel: as many CTAs as fit on the device at once (occupancy x SMs), at most one per tile.
-template <class Kernel>
-static inline int persistent_grid(Kernel kern, int threads, int smem, long long tiles, unsigned* grid) {
-    int per_sm = 0;
-    FCUDA_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, threads, smem));
-    const long long slots = static_cast<long long>(sm_count()) * (per_sm > 0 ? per_sm : 1);
-    *grid = static_cast<unsigned>(tiles < slots ? tiles : slots);
-    return 0;
-}
-
 // Split an fp32 value into a TF32-representable "hi" (round-to-nearest on the 13 dropped
 // mantissa bits) and the exact fp32 remainder "lo".  hi + lo == v exactly; the tensor
 // core then truncates lo to TF32, leaving a relative error of ~2^-22 per operand.
@@ -111,10 +101,23 @@ __device__ __forceinline__ void split_tf32(float v, float& hi, float& lo) {
 // Kernel-variant switches (defaults = the measured-best configuration; FCUDA_<NAME> in the environment or
 // fcuda_set_tuning() override them — the variants stay testable and benchmarkable side by side).
 enum TuneKey { TUNE_DW_VEC = 0, TUNE_WINO_MLP, TUNE_IGEMM_HALO, TUNE_GEMM_PIPE, TUNE_IGEMM_PRESPLIT, TUNE_IGEMM_WIDE,
-               TUNE_YOLO_NMS, TUNE_IGEMM_STEM, TUNE_ROUTE_FUSE, TUNE_COUNT };
+               TUNE_YOLO_NMS, TUNE_IGEMM_STEM, TUNE_ROUTE_FUSE, TUNE_PERSISTENT_CTAS, TUNE_COUNT };
 int tune_get(int key);
 const char* tune_name(int key);             // registry name of a key (fcuda_set_tuning / fcuda_get_tuning)
 int tune_set(const char* name, int value);  // 0, or -200 for an unknown name / value
+
+// Grid of a persistent kernel: as many CTAs as fit on the device at once (occupancy x SMs), at most one per tile.  The
+// switch persistent_ctas = n > 0 caps it at n CTAs, so tests can set how many tiles each CTA runs whatever the card.
+template <class Kernel>
+static inline int persistent_grid(Kernel kern, int threads, int smem, long long tiles, unsigned* grid) {
+    int per_sm = 0;
+    FCUDA_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, threads, smem));
+    long long slots = static_cast<long long>(sm_count()) * (per_sm > 0 ? per_sm : 1);
+    const int cap = tune_get(TUNE_PERSISTENT_CTAS);
+    if (cap > 0 && cap < slots) slots = cap;
+    *grid = static_cast<unsigned>(tiles < slots ? tiles : slots);
+    return 0;
+}
 
 // Per-launch profiling (tensor_gemm.cu): kernel classes for bench.py's roofline legs.
 enum ProfKind { PROF_TENSOR_GEMM = 0, PROF_IGEMM = 1, PROF_WINO_INPUT = 2, PROF_WINO_OUTPUT = 3, PROF_POOL = 4,

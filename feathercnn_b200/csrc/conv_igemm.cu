@@ -45,6 +45,8 @@ constexpr int kConsumerWarps = 8;                      // two warpgroups x 64 pi
 constexpr int kThreadsIg = (kConsumerWarps + 1) * 32;  // + the filter producer warp
 constexpr int kStagesIg = 4;
 constexpr int kMaxTableK = 6144;                       // k-table entries that fit beside the filter ring
+// Dynamic shared memory a CTA may take: the 227 KB opt-in less the kernels' static mbarriers (at most 96 bytes)
+constexpr int kSmemBudget = 227 * 1024 - 128;
 
 struct IgemmArgs {
     const float* residual;   // added to the output before the activation, or null
@@ -439,7 +441,7 @@ int launch_igemm(const IgemmProblem& p, cudaStream_t stream) {
     constexpr int kStage = NPL * BN * 32 * (BF ? 2 : 4);
     const int table_bytes = a.use_table ? a.kblocks * 32 * 8 : 0;
     const int smem = kStagesIg * kStage + table_bytes + 1024;
-    if (smem > 227 * 1024) return -1;
+    if (smem > kSmemBudget) return -1;
     return launch_igemm_kernel<conv_igemm_kernel<BN, PLANES, CLIP>>(p, stream, kThreadsIg, smem, total, false,
                                                                     pixel_tiles * 128, a.num_n * BN, a.kblocks, tmW, tmWlo, a);
 }
@@ -645,7 +647,7 @@ int launch_stem(const IgemmProblem& p, cudaStream_t stream) {
     a.KW = p.KW;
     a.tiles_per_img = ceil_div(a.oplane, 128);
     a.tiles = static_cast<long long>(p.N) * a.tiles_per_img;
-    a.nbuf = stem_smem_bytes(BN, a.kblocks, 2) <= 227 * 1024 ? 2 : 1;
+    a.nbuf = stem_smem_bytes(BN, a.kblocks, 2) <= kSmemBudget ? 2 : 1;
     a.vec = (reinterpret_cast<uintptr_t>(p.output) & 15) == 0 && a.oplane % 4 == 0;
     const int smem = stem_smem_bytes(BN, a.kblocks, a.nbuf);
     return launch_igemm_kernel<conv_igemm_stem_kernel<BN, CLIP>>(p, stream, kStemThreads, smem, a.tiles, true, a.tiles * 128,
@@ -1383,7 +1385,7 @@ static bool halo_geometry(const IgemmProblem& p, HaloGeom& g) {
                 if (r > 256 || cc > 256 || !halo_banks_conflict_free(r * cc, p.planes == 3)) continue;
                 if (rb == 0 || r * cc < rb * cbx) { rb = r; cbx = cc; }
             }
-        if (rb == 0 || halo_smem_bytes(p.OC, p.planes, rb, cbx) > 227 * 1024) continue;
+        if (rb == 0 || halo_smem_bytes(p.OC, p.planes, rb, cbx) > kSmemBudget) continue;
         if (best < 0 || cost < best) {
             best = cost;
             g.R = R; g.C = C; g.Rb = rb; g.Cb = cbx;
@@ -1407,7 +1409,7 @@ static bool presplit_geometry(const IgemmProblem& p, HaloGeom& g) {
     g.R = h.R; g.C = h.C;
     g.Rb = h.R + p.KH - 1;
     g.Cb = (h.C + p.KW - 1 + xshift + 3) & ~3;
-    return presplit_smem_bytes(p, g) <= 227 * 1024;
+    return presplit_smem_bytes(p, g) <= kSmemBudget;
 }
 
 // Filter ring, one fp32 half box, two plane buffers and the unit table of conv_igemm_wide_kernel
@@ -1429,7 +1431,7 @@ static bool wide_geometry(const IgemmProblem& p, HaloGeom& g) {
     g.R = R; g.C = C;
     g.Rb = R + p.KH - 1;
     g.Cb = (C + p.KW - 1 + xshift + 3) & ~3;
-    return wide_smem_bytes(p, g) <= 227 * 1024;
+    return wide_smem_bytes(p, g) <= kSmemBudget;
 }
 
 // The input blob [N][in_img_c][H][W] (the IC channels of this slice) in boxes of hg.Cb x hg.Rb x `chans` channels; boxes

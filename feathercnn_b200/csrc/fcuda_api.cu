@@ -491,8 +491,9 @@ static int conv_launch(const FcudaConvParam* p, const ConvPlan& pl, float* outpu
                 g.KH = p->kernel_h; g.KW = p->kernel_w; g.pad_top = p->pad_top; g.pad_left = p->pad_left;
                 g.stride_h = p->stride_h; g.stride_w = p->stride_w;
                 g.dil_h = dil_h; g.dil_w = dil_w;
-                if (taps == 1 && p->pad_top == 0 && p->pad_left == 0 && p->stride_h == 1 && p->stride_w == 1) {
-                    // pointwise stride 1: address each image as one H*W-long row (fuller 32-pixel boxes)
+                if (taps == 1 && p->pad_top == 0 && p->pad_left == 0 && p->stride_h == 1 && p->stride_w == 1 &&
+                    p->output_h == p->input_h && p->output_w == p->input_w) {
+                    // pointwise stride 1, no padding: address each image as one H*W-long row (fuller 32-pixel boxes)
                     g.H = 1; g.W = p->input_h * p->input_w; g.OH = 1; g.OW = p->output_h * p->output_w;
                 } else {
                     g.H = p->input_h; g.W = p->input_w; g.OH = p->output_h; g.OW = p->output_w;

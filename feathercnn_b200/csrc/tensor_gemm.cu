@@ -334,6 +334,7 @@ TuneEntry g_tune[TUNE_COUNT] = {
     {"yolo_nms", "FCUDA_YOLO_NMS", 1, 0, 1, 0, false},               // YOLO NMS: mask CTAs + sweep CTA (0: one CTA per image)
     {"igemm_stem", "FCUDA_IGEMM_STEM", 1, 0, 1, 0, false},           // short-K k-table layers: persistent, resident filters
     {"route_fuse", "FCUDA_ROUTE_FUSE", 1, 0, 1, 0, false},           // Net fusion: Concat -> ShuffleChannel -> Slice in one launch
+    {"persistent_ctas", "FCUDA_PERSISTENT_CTAS", 0, 0, 65536, 0, false},  // n > 0: persistent kernels run at most n CTAs
 };
 }  // namespace
 const char* tune_name(int key) { return key >= 0 && key < TUNE_COUNT ? g_tune[key].name : nullptr; }

@@ -567,6 +567,10 @@ int fcuda_slice_plan(int rank, int axis, const int* shape, const int* slices, in
  *                             ShuffleChannel -> Slice (axis 0) chains, or any two adjacent of them, run as one
  *                             fcuda_route_forward launch.  Bit-identical to 0 = every routing layer on its own, while
  *                             the net's other fusions stay as they are
+ *   persistent_ctas (0-65536, 0)  n > 0: every persistent kernel (stem, halo / pre-split / wide implicit GEMM, pipelined
+ *                             TensorGEMM) runs at most n CTAs, so each CTA walks ceil(tiles / n) or fewer tiles whatever
+ *                             the card's SM count.  For tests; feather::Net captures grids in its CUDA graphs, so set it
+ *                             before a Net first runs.  Bit-identical to 0 = as many CTAs as fit on the device
  * Every variant computes the same result (tests/test_gpu_variants.py).  Returns 0 / the value, -200 for an unknown name or value. */
 int fcuda_set_tuning(const char* name, int value);
 int fcuda_get_tuning(const char* name);

@@ -27,7 +27,8 @@ Depthwise and pooling cases also run on views that start 0..3 floats past an ali
 separately), through the C ABI: the vector kernels must then give way to the scalar ones.  The output view sits in a
 NaN-filled buffer and the floats around it must stay NaN.
 
-Every case is labelled with the kernel it reaches (the implicit-GEMM tile queries for gather / halo / presplit / wide, a
+Every case is labelled with the kernel it reaches (the implicit-GEMM stem and tile queries for stem / gather / halo /
+presplit / wide, a
 restatement of dw_launch and of pooling_forward, the Winograd chunk plan); the CPU tests below check that the generated
 list hits every reachable (kernel, epilogue, mode) cell and both sides of every predicate boundary, and that the checker
 rejects simulated defects on the sweep's own shapes.  A failing case prints a ready-to-paste Conv(...) literal, to be
@@ -344,13 +345,18 @@ def _set_mode(mode):
 
 
 def igemm_kernel(c: Conv, mode: int) -> str:
-    """gather / halo / presplit / wide from the tile queries of the per-group problem in `mode` (launch_conv's order)."""
-    if c.dil > 1:
-        return "gather"          # the queries do not see dilation; halo_geometry rejects it
+    """stem / gather / halo / presplit / wide from the queries of the per-group problem in `mode`, in launch_conv's
+    order: the stem query (with the case's residual, pooling and dilation), then the tile queries."""
+    from feathercnn_b200._lib import FcudaConvOptions
     lib, p, g = _lib(), conv_param(c), (ctypes.c_int * 4)()
     old = lib.fcuda_get_precision()
     _set_mode(mode)
     try:
+        o = FcudaConvOptions(residual=1 if c.res else None, pool=int(c.pool), dilation_h=c.dil, dilation_w=c.dil)
+        if lib.fcuda_igemm_stem_supported(ctypes.byref(p), ctypes.byref(o)):
+            return "stem"
+        if c.dil > 1:
+            return "gather"      # the tile queries do not see dilation; halo_geometry rejects it
         if lib.fcuda_igemm_wide_tile(ctypes.byref(p), g):
             return "wide"
         if lib.fcuda_igemm_presplit_tile(ctypes.byref(p), g):
@@ -589,7 +595,8 @@ def _guard_ok(buf, off, n) -> bool:
     return bool(torch.isnan(buf[:off]).all() and torch.isnan(buf[off + n:]).all())
 
 
-def run_conv_case(case: Case, algo: int):
+def forward_conv_case(case: Case, algo: int):
+    """Runs case on `algo` through its entry point; returns (x, w, b, r, the output (N, OC, OH, OW), guard ok)."""
     from feathercnn_b200 import booster
     c, mode = case.conv, case.mode
     booster.set_precision(mode)
@@ -632,8 +639,12 @@ def run_conv_case(case: Case, algo: int):
     finally:
         booster.set_l2_chunk_bytes(default_chunk)
     assert rc == 0, (booster.ALGO_NAMES[algo], rc)
-    guard = _guard_ok(obuf, case.out_off, n_out)
-    got = out.view(n, c.oc, oh, ow)
+    return x, w, b, r, out.view(n, c.oc, oh, ow), _guard_ok(obuf, case.out_off, n_out)
+
+
+def run_conv_case(case: Case, algo: int):
+    c, mode = case.conv, case.mode
+    x, w, b, r, got, guard = forward_conv_case(case, algo)
     coef = conv_coef(c, algo, mode, x, w, b)
     ref, bound, s = conv_expect(c, x, w, b, r, coef, wino_tile(algo))
     used, rel = check_conv(got, ref, bound, s)
@@ -695,8 +706,11 @@ def test_dispatch_sweep(cuda, i):
 #     the fused pool, which needs 3x3 taps;
 #   - im2col / naive / depthwise with a fused pool (fcuda_conv_forward_pool rejects them);
 #   - naive and depthwise in a given mode: fp32 FMA kernels, mode-independent ("any").
+#   - stem outside fp32split (it reads the BF16x3 split planes), and with a residual or pool: fcuda_igemm_stem_supported
+#     rejects both (the kernel fuses neither), and res / res_relu carry a residual;
 EXPECTED_CELLS = (
     [("gather", e, m) for e in EPILOGUES if e != "pool" for m in MODE_NAME.values()]
+    + [("stem", e, "fp32split") for e in ("none", "relu", "clip")]
     + [("halo", e, m) for e in EPILOGUES for m in MODE_NAME.values() if (e, m) != ("pool", "fp32split")]
     + [(k, e, "fp32split") for k in ("presplit", "wide") for e in EPILOGUES]
     + [(k, e, m) for k in ("f63", "f63-chunked", "f23", "f23-chunked") for e in EPILOGUES for m in MODE_NAME.values()]

@@ -384,6 +384,11 @@ SGECONV_SWEEP = (
        Conv("sg_stride_2x1", 40, 12, 13, 17, sh=2, sw=1),
        Conv("sg_pad_top2_left0", 40, 32, 11, 12, pad=(0, 1, 2, 2)),
        Conv("sg_pad_asym_br", 36, 20, 10, 13, pad=(1, 0, 2, 1)),            # bottom 0, right 2
+       # a 1x1 / stride 1 layer padded only at the bottom and right is not the pointwise H * W-row layout (OH > H)
+       Conv("psweep854", 62, 514, 40, 40, kh=1, kw=1, pad=(0, 2, 2, 0), group=2),
+       Conv("sg_1x1_pad_br_table", 31, 33, 9, 10, 1, pad=(0, 1, 2, 0), batch=3),
+       # a halo patch whose TF32 box and filter ring fill the 227 KB but for the kernel's static mbarriers
+       Conv("psweep981", 96, 32, 7, 32, kh=7, kw=1, pad=(2, 0, 2, 0), bias=False, batch=1, clip=(-0.125, 0.25)),
        Conv("sg_dil2", 40, 32, 14, 13, dil=2, pad=2),
        Conv("sg_dil3_table", 24, 12, 15, 16, dil=3, pad=(3, 1, 2, 3)),
        Conv("sg_group4_table", 96, 64, 9, 10, group=4),                    # 16 channels per group: channel slices
