@@ -100,8 +100,8 @@ __device__ __forceinline__ void split_tf32(float v, float& hi, float& lo) {
 
 // Kernel-variant switches (defaults = the measured-best configuration; FCUDA_<NAME> in the environment or
 // fcuda_set_tuning() override them — the variants stay testable and benchmarkable side by side).
-enum TuneKey { TUNE_DW_VEC = 0, TUNE_WINO_MLP, TUNE_IGEMM_HALO, TUNE_GEMM_PIPE, TUNE_IGEMM_PRESPLIT, TUNE_IGEMM_WIDE,
-               TUNE_YOLO_NMS, TUNE_IGEMM_STEM, TUNE_ROUTE_FUSE, TUNE_PERSISTENT_CTAS, TUNE_COUNT };
+enum TuneKey { TUNE_DW_VEC = 0, TUNE_IGEMM_HALO, TUNE_IGEMM_PRESPLIT, TUNE_IGEMM_WIDE, TUNE_IGEMM_STEM, TUNE_ROUTE_FUSE,
+               TUNE_PERSISTENT_CTAS, TUNE_COUNT };
 int tune_get(int key);
 const char* tune_name(int key);             // registry name of a key (fcuda_set_tuning / fcuda_get_tuning)
 int tune_set(const char* name, int value);  // 0, or -200 for an unknown name / value

@@ -87,7 +87,7 @@ __device__ __forceinline__ void load_filter_stage(uint8_t* smem, uint64_t* full_
     constexpr int kBTile = BN * 32 * (PLANES == 3 ? 2 : 4);
     constexpr int kStage = (PLANES == 3 ? 2 : PLANES) * kBTile;
     const int stage = kbg % kStagesIg;
-    if (kbg >= kStagesIg) ptx::mbar_wait_nocall(&empty_bar[stage], ((kbg / kStagesIg) - 1) & 1);
+    if (kbg >= kStagesIg) ptx::mbar_wait(&empty_bar[stage], ((kbg / kStagesIg) - 1) & 1);
     uint8_t* st = smem + stage * kStage;
     ptx::mbar_arrive_expect_tx(&full_bar[stage], kStage);
     if (PLANES == 3) {
@@ -230,7 +230,7 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tmW, const __grid_constant
         uint32_t f1[4][4], f2[4][4];  // [k-step][a0..a3]: hi / p1 and lo / p2
         split_fragments<PLANES>(raw, f1, f2);
         if (kb + 1 < kblocks) gather(kb + 1, raw);
-        ptx::mbar_wait_nocall(&full_bar[stage], (kb / kStagesIg) & 1);
+        ptx::mbar_wait(&full_bar[stage], (kb / kStagesIg) & 1);
         const uint32_t b_base = ptx::smem_u32(smem + stage * kStage);
         ptx::wgmma_fence();
         mma_kblock<BN, PLANES>(acc, f1, f2, b_base, b_base + kBTile);
@@ -562,7 +562,7 @@ conv_igemm_stem_kernel(const StemArgs args) {
     locate(blockIdx.x);  // grid <= tiles: every CTA has a first tile
     gather(0, raw);
     const uint32_t filters = ptx::smem_u32(smem);
-    ptx::mbar_wait_nocall(&wbar, 0);
+    ptx::mbar_wait(&wbar, 0);
     int buf = 0;
     for (long long t = blockIdx.x; t < args.tiles; t += gridDim.x) {
         const int img = static_cast<int>(t / args.tiles_per_img);
@@ -792,7 +792,7 @@ __device__ __forceinline__ void halo_producer(const CUtensorMap* tmX, const CUte
     auto load_halo = [&](long long t, int cb) {
         const HaloTile h = halo_tile(args, per_img, t);
         const int hs = hb % HS;
-        if (hb >= HS) ptx::mbar_wait_nocall(&hempty_bar[hs], ((hb / HS) - 1) & 1);
+        if (hb >= HS) ptx::mbar_wait(&hempty_bar[hs], ((hb / HS) - 1) & 1);
         ptx::mbar_arrive_expect_tx(&hfull_bar[hs], static_cast<uint32_t>(hstage) * 4u);
         ptx::tma_load_4d(halo + hs * hstage, tmX, &hfull_bar[hs], h.tx * args.C - args.xpad, h.ty * args.R - args.pad_top,
                          cb * 32, h.img);
@@ -888,7 +888,7 @@ __device__ __forceinline__ void halo_body(const CUtensorMap& tmX, const CUtensor
         float raw[2][8];
         uint32_t fa1[4][4], fa2[4][4], fb1[4][4], fb2[4][4];  // two fragment sets: [k-step][a0..a3], hi / p1 and lo / p2
         int tap = 0, dy = 0, dx = 0;                          // tap of the k-block in `raw`
-        ptx::mbar_wait_nocall(&hfull_bar[hb % kHaloStages], (hb / kHaloStages) & 1);
+        ptx::mbar_wait(&hfull_bar[hb % kHaloStages], (hb / kHaloStages) & 1);
         gather(halo + (hb % kHaloStages) * hstage, 0, raw);
 
         auto step = [&](uint32_t (&f1)[4][4], uint32_t (&f2)[4][4], int kb) {
@@ -903,11 +903,11 @@ __device__ __forceinline__ void halo_body(const CUtensorMap& tmX, const CUtensor
                 ++dy;
             }
             if (kb + 1 < kblocks) {
-                if (tap == 0) ptx::mbar_wait_nocall(&hfull_bar[hb % kHaloStages], (hb / kHaloStages) & 1);
+                if (tap == 0) ptx::mbar_wait(&hfull_bar[hb % kHaloStages], (hb / kHaloStages) & 1);
                 gather(halo + (hb % kHaloStages) * hstage, dy * args.Cb + dx, raw);
             }
             const int stage = kbg % kStagesIg;
-            ptx::mbar_wait_nocall(&full_bar[stage], (kbg / kStagesIg) & 1);
+            ptx::mbar_wait(&full_bar[stage], (kbg / kStagesIg) & 1);
             const uint32_t b_base = ptx::smem_u32(smem + stage * kStage);
             ptx::wgmma_fence();
             mma_kblock<BN, PLANES>(acc, f1, f2, b_base, b_base + kBTile);
@@ -1008,7 +1008,7 @@ __device__ __forceinline__ void presplit_body(const CUtensorMap& tmX, const Halo
     // split box hb into plane buffer hb & 1 and hand the fp32 box back
     auto convert_next = [&]() {
         const int hs = hb % HS;
-        ptx::mbar_wait_nocall(&hfull_bar[hs], (hb / HS) & 1);
+        ptx::mbar_wait(&hfull_bar[hs], (hb / HS) & 1);
         split_box(halo + hs * hstage, utab, cstride, units, planes + static_cast<uint32_t>(hb & 1) * 2u * pbytes, pbytes);
         __syncwarp();
         ptx::mbar_arrive_if(&hempty_bar[hs], lane == 0);
@@ -1046,7 +1046,7 @@ __device__ __forceinline__ void presplit_body(const CUtensorMap& tmX, const Halo
                 toff += 16u * static_cast<uint32_t>(args.pc - KW);
             }
             const int stage = kbg & (kStagesIg - 1);
-            ptx::mbar_wait_nocall(&full_bar[stage], (kbg / kStagesIg) & 1);
+            ptx::mbar_wait(&full_bar[stage], (kbg / kStagesIg) & 1);
             const uint32_t b_base = ptx::smem_u32(smem) + stage * kStage;
             ptx::wgmma_fence();
             mma_kblock<BN, 3>(acc, f1, f2, b_base, b_base + kBTile);
@@ -1139,7 +1139,7 @@ __device__ __forceinline__ void wide_producer(const CUtensorMap* tmX, const Halo
     int kbg = 0;  // filter stages issued
     auto load_half = [&](long long t, int cb, int h) {
         const HaloTile tile = halo_tile(args, per_img, t);
-        if (nh > 0) ptx::mbar_wait_nocall(hempty_bar, (nh - 1) & 1);
+        if (nh > 0) ptx::mbar_wait(hempty_bar, (nh - 1) & 1);
         ptx::mbar_arrive_expect_tx(hfull_bar, static_cast<uint32_t>(hstage) * 4u);
         ptx::tma_load_4d(halo, tmX, hfull_bar, tile.tx * args.C - args.xpad, tile.ty * args.R - args.pad_top,
                          cb * 32 + 16 * h, tile.img);
@@ -1265,7 +1265,7 @@ __device__ __forceinline__ void wide_body(const CUtensorMap& tmX, const HaloArgs
     int kbg = 0;  // filter stages consumed
     // split half h of box nc / 2 into plane buffer (nc / 2) & 1 and hand the fp32 half box back
     auto convert_half = [&](int h) {
-        ptx::mbar_wait_nocall(&hfull_bar, nc & 1);
+        ptx::mbar_wait(&hfull_bar, nc & 1);
         split_box(halo, utab, cstride, hunits,
                   planes + static_cast<uint32_t>((nc >> 1) & 1) * 2u * pbytes + 16u * static_cast<uint32_t>(h * hunits), pbytes);
         ptx::fence_proxy_async_smem();
@@ -1289,7 +1289,7 @@ __device__ __forceinline__ void wide_body(const CUtensorMap& tmX, const HaloArgs
         // one k-block: the six MMAs, then (half >= 0) the split of that half of the next box behind them
         auto step = [&](int half) {
             const int stage = kbg & (kStagesIg - 1);
-            ptx::mbar_wait_nocall(&full_bar[stage], (kbg / kStagesIg) & 1);
+            ptx::mbar_wait(&full_bar[stage], (kbg / kStagesIg) & 1);
             const uint32_t a_base = ptx::smem_u32(smem) + stage * kStage + a_off;
             const uint64_t dQ1 = make_smem_desc_none(a_base, 128, 512);
             const uint64_t dQ2 = make_smem_desc_none(a_base + kBTile, 128, 512);

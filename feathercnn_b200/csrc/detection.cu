@@ -423,7 +423,6 @@ DetWorkspace carve(float* ws, int P, int C, int top_k, int batch) {
 // mask    CTAs over (32-row block, image): word w of row i has bit b set iff j = 32 w + b > i and IoU(i, j) > threshold;
 // sweep   one CTA per image: the mask in shared memory, one warp walks the candidates in order (lane l owns the removal
 //         word l: no barrier and no global load in the loop), then the output rows.
-// Switch yolo_nms = 0 replaces mask + sweep by one CTA per image that builds the mask in its own shared memory.
 constexpr int kYoloMaskWords = kMaxTopK / 32;
 constexpr int kYoloMaskRows = 32;  // rows of one mask CTA: 8 warps x 4
 
@@ -654,25 +653,6 @@ yolo_sweep_kernel(float* __restrict__ out, const YoloWorkspace w, int slots, int
     yolo_sweep_rows(out, w, n, m, slots, keep_top_k, reinterpret_cast<const uint32_t*>(yolo_smem), keep, &kept_count);
 }
 
-// Single-CTA NMS (switch yolo_nms = 0): one CTA per image builds the whole mask in shared memory, then sweeps it.
-__global__ void __launch_bounds__(kDetThreads)
-yolo_nms_fused_kernel(float* __restrict__ out, const YoloWorkspace w, int slots, float nms_thr, int keep_top_k) {
-    extern __shared__ uint4 yolo_smem[];
-    uint32_t* smask = reinterpret_cast<uint32_t*>(yolo_smem);
-    __shared__ float sb[kMaxTopK][4];
-    __shared__ float sarea[kMaxTopK];
-    __shared__ int keep[kMaxTopK];
-    __shared__ int kept_count;
-    const int n = blockIdx.x;
-    const int m = w.counts[n];
-    yolo_stage_boxes(w, n, 0, m, sb, sarea);
-    __syncthreads();
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    for (int i = warp; i < m; i += kDetWarps) smask[i * kYoloMaskWords + lane] = yolo_mask_row(i, m, sb, sarea, nms_thr, lane);
-    __syncthreads();
-    yolo_sweep_rows(out, w, n, m, slots, keep_top_k, smask, keep, &kept_count);
-}
-
 }  // namespace
 
 int permute_forward(const float* in, float* out, int c, int h, int w, int order, int batch, cudaStream_t s) {
@@ -808,7 +788,7 @@ int yolo_decode_launch(float* scores, int* classes, float* boxes, const YoloGeom
     return 0;
 }
 
-SmemAttrCache yolo_sweep_smem, yolo_fused_smem;
+SmemAttrCache yolo_sweep_smem;
 
 }  // namespace
 
@@ -836,17 +816,6 @@ int yolo_detection(float* out, const float* const* inputs, const FcudaYoloParam&
     prof_end(prof, s);
     count_launch();
     const int smem = p.nms_top_k * kYoloMaskWords * static_cast<int>(sizeof(uint32_t));
-    if (!tune_get(TUNE_YOLO_NMS)) {
-        rc = ensure_dynamic_smem(yolo_nms_fused_kernel, smem, yolo_fused_smem);
-        if (rc) return rc;
-        prof = prof_begin(s, PROF_DETECTION, 0, 0, 20.0 * batch * p.nms_top_k + 24.0 * batch * p.keep_top_k);
-        yolo_nms_fused_kernel<<<static_cast<unsigned>(batch), kDetThreads, smem, s>>>(out, w, g.slots, p.nms_threshold,
-                                                                                       p.keep_top_k);
-        FCUDA_CHECK_LAUNCH();
-        prof_end(prof, s);
-        count_launch();
-        return 0;
-    }
     const int row_blocks = ceil_div(p.nms_top_k, kYoloMaskRows);
     prof = prof_begin(s, PROF_DETECTION, 0, 0, 20.0 * batch * p.nms_top_k + 4.0 * batch * p.nms_top_k * kYoloMaskWords);
     yolo_mask_kernel<<<dim3(static_cast<unsigned>(row_blocks), static_cast<unsigned>(batch)), 256, 0, s>>>(w,

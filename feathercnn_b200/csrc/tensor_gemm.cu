@@ -1,17 +1,17 @@
 // TensorGEMM on Hopper warpgroup MMA (sm_90a).  See tensor_gemm.cuh for the contract.
 //
-// tensor_gemm_kernel<BN, PLANES>: one CTA per 128 x BN output tile (and k-split), 288 threads:
+// tensor_gemm_kernel<BN, PLANES, CLIP>: persistent CTAs of 288 threads walk the 128 x BN output tiles (and k-splits) with
+// a static stride:
 //   warp 8        TMA producer : per 32-wide k-block the raw fp32 A tile (128 rows) and the B_hi (+ B_lo) tiles
-//                                (cp.async.bulk.tensor 3-D boxes, 128-byte swizzle) into a kStages-deep smem ring
+//                                (cp.async.bulk.tensor 3-D boxes, 128-byte swizzle) into a kStages-deep smem ring.  It
+//                                keeps a running k-block count across tiles, so it fills the next tile's stages while
+//                                the consumers run the epilogue.
 //   warps 0..7    two consumer warpgroups, 64 rows each: a thread reads its A fragment from the swizzled tile, splits it
 //                 into TF32 hi + fp32 lo (PLANES == 2) in registers and issues wgmma.mma_async with A from registers and B
 //                 from shared memory: A_lo*B_hi + A_hi*B_lo + A_hi*B_hi per k-step of 8 into fp32 register
 //                 accumulators; then the fused store (row-major / NCHW+bias+ReLU / k-split partial planes).
 // A is ONE fp32 plane in HBM (the split happens on chip); full / empty mbarriers hand the ring slots over, and a bounded
 // wait traps instead of hanging the GPU.
-//
-// tensor_gemm_pipe_kernel<BN, PLANES> (switch gemm_pipe, the default) runs the same tiles and MMA sequence with
-// persistent CTAs and overlapped k-blocks; see its comment below.
 #include "tensor_gemm.cuh"
 #include "common.cuh"
 #include "wgmma.cuh"
@@ -134,88 +134,17 @@ __device__ __forceinline__ void load_a_fragments(uint32_t a_base, int row0, int 
     }
 }
 
+// Two A-fragment sets overlap the k-blocks: k-block kb + 1 is read from the swizzled tile and split while kb's commit
+// group runs (wgmma_wait<1>); a ring stage is released once the group that read its B planes retired.
 template <int BN, int PLANES, bool CLIP>
 __global__ void __launch_bounds__(kThreads, 1)
 tensor_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
-                   const __grid_constant__ CUtensorMap tmBlo, const GemmKernelArgs args) {
-    constexpr int kATile = kBM * kBK * 4;  // 16 KB raw A
-    constexpr int kBTile = BN * kBK * 4;
-    constexpr int kStage = kATile + PLANES * kBTile;  // [A raw][B_hi][B_lo]
-    extern __shared__ uint8_t smem_raw[];
-    // SWIZZLE_128B tiles need 1024-byte alignment.
-    uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-    __shared__ uint64_t full_bar[kStages];
-    __shared__ uint64_t empty_bar[kStages];
-
-    const int warp = threadIdx.x >> 5;
-    const int lane = threadIdx.x & 31;
-
-    const TileCoord tc = tile_coord(args, blockIdx.x);
-
-    if (threadIdx.x == 0) {
-        ptx::mbar_init_ring(full_bar, empty_bar, kStages, kConsumerWarps);
-        ptx::fence_barrier_init();
-    }
-    __syncthreads();
-
-    if (warp == kConsumerWarps) {
-        // ===================== TMA producer =====================
-        if (lane == 0) {
-            ptx::prefetch_tensormap(&tmA);
-            ptx::prefetch_tensormap(&tmB);
-            if (PLANES == 2) ptx::prefetch_tensormap(&tmBlo);
-            for (int i = 0; i < tc.nk; ++i) {
-                const int stage = i % kStages;
-                if (i >= kStages) ptx::mbar_wait(&empty_bar[stage], ((i / kStages) - 1) & 1);
-                uint8_t* st = smem + stage * kStage;
-                const int kc = (tc.kb0 + i) * kBK;
-                ptx::mbar_arrive_expect_tx(&full_bar[stage], kStage);
-                ptx::tma_load_3d(st, &tmA, &full_bar[stage], kc, tc.m_blk * kBM, tc.g);
-                ptx::tma_load_3d(st + kATile, &tmB, &full_bar[stage], kc, tc.n_blk * BN, tc.g);
-                if (PLANES == 2) ptx::tma_load_3d(st + kATile + kBTile, &tmBlo, &full_bar[stage], kc, tc.n_blk * BN, tc.g);
-            }
-        }
-        return;
-    }
-
-    // ===================== consumers: two warpgroups of 64 rows =====================
-    const int gq = lane >> 2, c = lane & 3;
-    const int row0 = warp * 16 + gq;  // tile rows row0 and row0 + 8; row & 7 == gq for both (128B swizzle phase)
-    float acc[BN / 2];
-#pragma unroll
-    for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
-
-    for (int i = 0; i < tc.nk; ++i) {
-        const int stage = i % kStages;
-        ptx::mbar_wait(&full_bar[stage], (i / kStages) & 1);
-        const uint32_t a_base = ptx::smem_u32(smem + stage * kStage);
-        uint32_t ahi[4][4], alo[4][4];
-        load_a_fragments<PLANES>(a_base, row0, gq, c, ahi, alo);
-        ptx::wgmma_fence();
-        mma_kblock<BN, PLANES>(acc, ahi, alo, a_base + kATile, a_base + kATile + kBTile);
-        ptx::wgmma_commit();
-        ptx::wgmma_wait<0>();
-        __syncwarp();
-        if (lane == 0) ptx::mbar_arrive(&empty_bar[stage]);
-    }
-    epilogue_store<BN, CLIP>(args, acc, tc.g, tc.m_blk * kBM + row0, tc.n_blk * BN, c, tc.ks);
-}
-
-// tensor_gemm_pipe_kernel<BN, PLANES>: the same tiles, k-blocks, wgmma sequence and epilogue as tensor_gemm_kernel, so the
-// result is bit-identical to it, with
-//   - two A-fragment sets: k-block kb + 1 is read from the swizzled tile and split while kb's commit group runs
-//     (wgmma_wait<1>); a ring stage is released once the group that read its B planes retired;
-//   - call-free bounded waits: a call inside the pipeline would make ptxas serialise every wgmma;
-//   - persistent CTAs that walk the tile order with a static stride; the producer keeps a running k-block count across
-//     tiles, so it fills the next tile's stages while the consumers run the epilogue.
-template <int BN, int PLANES, bool CLIP>
-__global__ void __launch_bounds__(kThreads, 1)
-tensor_gemm_pipe_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
-                        const __grid_constant__ CUtensorMap tmBlo, const GemmKernelArgs args, int tiles) {
+                   const __grid_constant__ CUtensorMap tmBlo, const GemmKernelArgs args, int tiles) {
     constexpr int kATile = kBM * kBK * 4;
     constexpr int kBTile = BN * kBK * 4;
     constexpr int kStage = kATile + PLANES * kBTile;  // [A raw][B_hi][B_lo]
     extern __shared__ uint8_t smem_raw[];
+    // SWIZZLE_128B tiles need 1024-byte alignment.
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
     __shared__ uint64_t full_bar[kStages];
     __shared__ uint64_t empty_bar[kStages];
@@ -240,7 +169,7 @@ tensor_gemm_pipe_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_co
                 const TileCoord tc = tile_coord(args, tile);
                 for (int i = 0; i < tc.nk; ++i, ++kbg) {
                     const int stage = kbg % kStages;
-                    if (kbg >= kStages) ptx::mbar_wait_nocall(&empty_bar[stage], ((kbg / kStages) - 1) & 1);
+                    if (kbg >= kStages) ptx::mbar_wait(&empty_bar[stage], ((kbg / kStages) - 1) & 1);
                     uint8_t* st = smem + stage * kStage;
                     const int kc = (tc.kb0 + i) * kBK;
                     ptx::mbar_arrive_expect_tx(&full_bar[stage], kStage);
@@ -266,7 +195,7 @@ tensor_gemm_pipe_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_co
 
         auto step = [&](uint32_t (&f1)[4][4], uint32_t (&f2)[4][4], int i) {
             const int stage = kbg % kStages;
-            ptx::mbar_wait_nocall(&full_bar[stage], (kbg / kStages) & 1);
+            ptx::mbar_wait(&full_bar[stage], (kbg / kStages) & 1);
             const uint32_t a_base = ptx::smem_u32(smem + stage * kStage);
             load_a_fragments<PLANES>(a_base, row0, gq, c, f1, f2);
             ptx::wgmma_fence();
@@ -326,12 +255,9 @@ namespace {
 struct TuneEntry { const char* name; const char* env; int def, lo, hi; int value; bool init; };
 TuneEntry g_tune[TUNE_COUNT] = {
     {"dw_vec", "FCUDA_DW_VEC", 1, 0, 1, 0, false},                   // vectorised depthwise kernel on wide planes
-    {"wino_mlp", "FCUDA_WINO_MLP", 2, 0, 2, 0, false},               // Winograd transforms: slab copies / all plane loads in flight
     {"igemm_halo", "FCUDA_IGEMM_HALO", 1, 0, 1, 0, false},           // implicit GEMM: TMA halo tiles + pipelined wgmma (stride 1)
-    {"gemm_pipe", "FCUDA_GEMM_PIPE", 1, 0, 1, 0, false},             // TensorGEMM: persistent CTAs + pipelined wgmma
     {"igemm_presplit", "FCUDA_IGEMM_PRESPLIT", 1, 0, 1, 0, false},   // BF16x3 halo kernel: one split per box, ldmatrix fragments
     {"igemm_wide", "FCUDA_IGEMM_WIDE", 1, 0, 1, 0, false},           // pre-split kernel: 224-pixel N side, filters on M
-    {"yolo_nms", "FCUDA_YOLO_NMS", 1, 0, 1, 0, false},               // YOLO NMS: mask CTAs + sweep CTA (0: one CTA per image)
     {"igemm_stem", "FCUDA_IGEMM_STEM", 1, 0, 1, 0, false},           // short-K k-table layers: persistent, resident filters
     {"route_fuse", "FCUDA_ROUTE_FUSE", 1, 0, 1, 0, false},           // Net fusion: Concat -> ShuffleChannel -> Slice in one launch
     {"persistent_ctas", "FCUDA_PERSISTENT_CTAS", 0, 0, 65536, 0, false},  // n > 0: persistent kernels run at most n CTAs
@@ -503,21 +429,15 @@ static int launch(const GemmProblem& p, cudaStream_t stream) {
     const long long total = static_cast<long long>(a.num_m) * a.num_n * a.G * a.split_k;
     if (total > 0x7fffffffLL) return -1;
     const int smem = kStages * kStage + 1024;
-    const bool pipe = tune_get(TUNE_GEMM_PIPE) != 0;
     auto kern = tensor_gemm_kernel<BN, PLANES, CLIP>;
-    auto pkern = tensor_gemm_pipe_kernel<BN, PLANES, CLIP>;
-    static SmemAttrCache attr_cache, pattr_cache;
-    if (int rc2 = pipe ? ensure_dynamic_smem(pkern, smem, pattr_cache) : ensure_dynamic_smem(kern, smem, attr_cache))
-        return rc2;
-    unsigned grid = static_cast<unsigned>(total);
-    if (pipe) {
-        if (int rc2 = persistent_grid(pkern, kThreads, smem, total, &grid)) return rc2;
-    }
+    static SmemAttrCache attr_cache;
+    if (int rc2 = ensure_dynamic_smem(kern, smem, attr_cache)) return rc2;
+    unsigned grid = 0;
+    if (int rc2 = persistent_grid(kern, kThreads, smem, total, &grid)) return rc2;
     const double dense = 2.0 * p.M * static_cast<double>(p.N) * p.K * p.G;
     const int prof = prof_begin(stream, PROF_TENSOR_GEMM, p.algo_flops > 0 ? p.algo_flops : dense,
                                 dense * (PLANES == 2 ? 3.0 : 1.0), gemm_algo_bytes(p));
-    if (pipe) pkern<<<grid, kThreads, smem, stream>>>(tmA, tmB, tmBlo, a, static_cast<int>(total));
-    else kern<<<grid, kThreads, smem, stream>>>(tmA, tmB, tmBlo, a);
+    kern<<<grid, kThreads, smem, stream>>>(tmA, tmB, tmBlo, a, static_cast<int>(total));
     FCUDA_CHECK_LAUNCH();
     count_launch();
     prof_end(prof, stream);

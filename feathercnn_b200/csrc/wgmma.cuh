@@ -7,7 +7,6 @@
 #include <cuda.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
-#include <stdio.h>
 
 namespace fcuda {
 
@@ -47,26 +46,9 @@ __device__ __forceinline__ bool mbar_try_wait(uint64_t* bar, uint32_t parity) {
     return ok != 0;
 }
 // Bounded wait: a protocol bug must fail the launch (trap) instead of hanging the GPU.  The clock is read every 64th
-// failed poll only.
-static __device__ __noinline__ void mbar_timeout_trap() {
-    printf("fcuda: mbarrier wait timed out (block %d thread %d)\n", blockIdx.x, threadIdx.x);
-    __trap();
-}
+// failed poll only.  It traps silently and makes no function call: ptxas serialises every wgmma of a function whose
+// pipeline crosses a call (a diagnostic printf would be one).
 __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
-    if (mbar_try_wait(bar, parity)) return;
-    long long t0 = 0;
-    for (uint32_t spins = 1; !mbar_try_wait(bar, parity); ++spins) {
-        if ((spins & 63u) == 0) {
-            const long long now = clock64();
-            if (t0 == 0) t0 = now;
-            else if (now - t0 > 4000000000LL) mbar_timeout_trap();  // ~2 s at 2 GHz
-        }
-    }
-}
-
-// The same bounded wait without a function call, for waits inside a running wgmma pipeline: ptxas serialises every
-// wgmma of a function whose pipeline crosses a call (the diagnostic's printf is one).  Traps silently.
-__device__ __forceinline__ void mbar_wait_nocall(uint64_t* bar, uint32_t parity) {
     if (mbar_try_wait(bar, parity)) return;
     long long t0 = 0;
     for (uint32_t spins = 1; !mbar_try_wait(bar, parity); ++spins) {

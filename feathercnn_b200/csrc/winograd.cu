@@ -161,7 +161,7 @@ __device__ __forceinline__ void cp_async4_zfill(float* smem_dst, const float* gm
                  : "memory");
 }
 
-template <int T, bool ASYNC>
+template <int T>
 __global__ void __launch_bounds__(kXformThreads)
 wino_input_kernel(const float* __restrict__ in, float* __restrict__ V, WinoGeom g, int R0, int Tc, int ncb) {
     using W = Wino<T>;
@@ -183,9 +183,9 @@ wino_input_kernel(const float* __restrict__ in, float* __restrict__ V, WinoGeom 
     const int gy0 = ty * OT - g.pad_top, gx0 = tx0 * OT - g.pad_left;
     const int w = threadIdx.x >> 5, lane = threadIdx.x & 31;
 
-    // slab load: warp w takes channels w, w+5, ...; per channel the T rows are unrolled (T loads in flight per lane,
-    // one IMAD.WIDE + LDG + STS per line; the first version spent 31 instructions per line on index arithmetic and
-    // that loop was 64% of the kernel's instructions); lane = column.
+    // Slab load: warp w takes channels w, w+5, ...; lane = column.  Every line of the slab is an asynchronous 4-byte
+    // copy: all ~52 loads of a lane are in flight at once (one memory latency per block), no staging registers, no STS;
+    // padding = zero-fill copies that do not touch global memory.
     {
         const size_t plane = static_cast<size_t>(g.H) * g.W;
         const float* img = in + static_cast<size_t>(n) * g.C_in * plane;
@@ -195,49 +195,20 @@ wino_input_kernel(const float* __restrict__ in, float* __restrict__ V, WinoGeom 
 #pragma unroll
         for (int r = 0; r < T; ++r)
             if (static_cast<unsigned>(gy0 + r) < static_cast<unsigned>(g.H)) row_ok |= 1u << r;
-        if (ASYNC) {
-            // Every line of the slab as an asynchronous 4-byte copy: all ~52 loads of a lane are in flight at once (one
-            // memory latency per block instead of four dependent rounds of 16 register-staged loads), no staging registers,
-            // no STS; padding = zero-fill copies that do not touch global memory.
-            if (lane < COLS) {
-                for (int c = w; c < kChBlock; c += kSegTiles) {
-                    const int ic = c0 + c;
-                    const bool c_ok = x_ok && ic < g.C_in;
-                    const float* p = c_ok ? img + static_cast<size_t>(ic) * plane + static_cast<long long>(gy0) * g.W + gx : in;
-                    float* sp = slab + c * CH_STRIDE + lane;
+        if (lane < COLS) {
+            for (int c = w; c < kChBlock; c += kSegTiles) {
+                const int ic = c0 + c;
+                const bool c_ok = x_ok && ic < g.C_in;
+                const float* p = c_ok ? img + static_cast<size_t>(ic) * plane + static_cast<long long>(gy0) * g.W + gx : in;
+                float* sp = slab + c * CH_STRIDE + lane;
 #pragma unroll
-                    for (int r = 0; r < T; ++r) {
-                        const bool ok = c_ok && ((row_ok >> r) & 1u);
-                        cp_async4_zfill(sp + r * COLS, ok ? p + r * g.W : in, ok);
-                    }
-                }
-            }
-            asm volatile("cp.async.wait_all;" ::: "memory");
-        }
-        // Channels w, w+5, ..., two per iteration: 2*T row loads are in flight per lane before the first shared-memory store
-        // (ncu r02h: the kernel waits on global loads — long-scoreboard stalls, 37 % warp occupancy, 0.59 of HBM bandwidth)
-        for (int c = w; !ASYNC && c < kChBlock; c += 2 * kSegTiles) {
-            float v[2][T];
-#pragma unroll
-            for (int h = 0; h < 2; ++h) {
-                const int cc = c + h * kSegTiles;
-                const int ic = c0 + cc;
-                const bool c_ok = x_ok && cc < kChBlock && ic < g.C_in;
-                // may point outside the image when gy0 < 0: only dereferenced under row_ok
-                const float* p = img + static_cast<size_t>(ic) * plane + static_cast<long long>(gy0) * g.W + gx;
-#pragma unroll
-                for (int r = 0; r < T; ++r) v[h][r] = (c_ok && ((row_ok >> r) & 1u)) ? __ldg(p + r * g.W) : 0.f;
-            }
-#pragma unroll
-            for (int h = 0; h < 2; ++h) {
-                const int cc = c + h * kSegTiles;
-                if (lane < COLS && cc < kChBlock) {
-                    float* sp = slab + cc * CH_STRIDE + lane;
-#pragma unroll
-                    for (int r = 0; r < T; ++r) sp[r * COLS] = v[h][r];
+                for (int r = 0; r < T; ++r) {
+                    const bool ok = c_ok && ((row_ok >> r) & 1u);
+                    cp_async4_zfill(sp + r * COLS, ok ? p + r * g.W : in, ok);
                 }
             }
         }
+        asm volatile("cp.async.wait_all;" ::: "memory");
     }
     __syncthreads();
 
@@ -274,7 +245,7 @@ wino_input_kernel(const float* __restrict__ in, float* __restrict__ V, WinoGeom 
 // (pooling_layer.h:38-91, pad 0) is applied to the tile in registers — the 6x6 (2x2) output tile starts at an even
 // coordinate, so no window straddles two tiles — and only the pooled (OH+1)/2 x (OW+1)/2 blob is written.
 // ------------------------------------------------------------------------------------------------
-template <int T, bool POOL, bool MLP, bool CLIP>
+template <int T, bool POOL, bool CLIP>
 __global__ void __launch_bounds__(kXformThreads)
 wino_output_kernel(const float* __restrict__ M, float* __restrict__ out, const float* __restrict__ bias, WinoGeom g,
                    int R0, int Tc, int act, float lo, float hi, int ncb) {
@@ -305,7 +276,7 @@ wino_output_kernel(const float* __restrict__ M, float* __restrict__ out, const f
         for (int a = 0; a < T; ++a)
 #pragma unroll
             for (int b = 0; b < T; ++b)
-                if (MLP) {
+                if (T == 8) {
                     // all T*T plane loads issued back to back (volatile: nvcc otherwise interleaves them column by column with
                     // the transform to save registers — 56 registers, eight dependent rounds of memory latency per tile)
                     asm volatile("ld.volatile.global.f32 %0, [%1];"
@@ -405,7 +376,7 @@ int wino_input_transform(int tile, const float* in, float* V, const WinoGeom& g,
     const int Tc = (R1 - R0) * g.tilesX;
     dim3 grid(static_cast<unsigned>(segs) * (R1 - R0), ceil_div(g.C_in, kChBlock));
     int ncb = 0;
-    if (tune_get(TUNE_WINO_MLP) >= 2 && static_cast<unsigned long long>(grid.x) * grid.y < 0x7fffffffULL) {
+    if (static_cast<unsigned long long>(grid.x) * grid.y < 0x7fffffffULL) {
         ncb = static_cast<int>(grid.y);
         grid = dim3(grid.x * grid.y, 1);
     }
@@ -413,14 +384,8 @@ int wino_input_transform(int tile, const float* in, float* V, const WinoGeom& g,
     const double imgs = static_cast<double>(R1 - R0) / g.tilesY;  // tile-rows of the chunk, in images
     const int prof = prof_begin(s, PROF_WINO_INPUT, 0, 0,
                                 4.0 * (imgs * g.C_in * g.H * g.W + static_cast<double>(tile) * tile * Tc * g.C_in));
-    const bool mlp = tune_get(TUNE_WINO_MLP) != 0;
-    if (tile == 8) {
-        if (mlp) wino_input_kernel<8, true><<<grid, kXformThreads, 0, s>>>(in, V, g, R0, Tc, ncb);
-        else wino_input_kernel<8, false><<<grid, kXformThreads, 0, s>>>(in, V, g, R0, Tc, ncb);
-    } else {
-        if (mlp) wino_input_kernel<4, true><<<grid, kXformThreads, 0, s>>>(in, V, g, R0, Tc, ncb);
-        else wino_input_kernel<4, false><<<grid, kXformThreads, 0, s>>>(in, V, g, R0, Tc, ncb);
-    }
+    if (tile == 8) wino_input_kernel<8><<<grid, kXformThreads, 0, s>>>(in, V, g, R0, Tc, ncb);
+    else wino_input_kernel<4><<<grid, kXformThreads, 0, s>>>(in, V, g, R0, Tc, ncb);
     prof_end(prof, s);
     FCUDA_CHECK_LAUNCH();
     count_launch();
@@ -428,19 +393,14 @@ int wino_input_transform(int tile, const float* in, float* V, const WinoGeom& g,
 }
 
 template <bool CLIP>
-static void wino_output_launch(int tile, bool mlp, dim3 grid, const float* M, float* out, const WinoGeom& g, int R0, int Tc,
+static void wino_output_launch(int tile, dim3 grid, const float* M, float* out, const WinoGeom& g, int R0, int Tc,
                                const ConvEpilogue& e, int ncb, cudaStream_t s) {
     if (tile == 8) {
-        if (mlp) {
-            if (e.pool) wino_output_kernel<8, true, true, CLIP><<<grid, kXformThreads, 0, s>>>(M, out, e.bias, g, R0, Tc, e.act, e.lo, e.hi, ncb);
-            else wino_output_kernel<8, false, true, CLIP><<<grid, kXformThreads, 0, s>>>(M, out, e.bias, g, R0, Tc, e.act, e.lo, e.hi, ncb);
-        } else {
-            if (e.pool) wino_output_kernel<8, true, false, CLIP><<<grid, kXformThreads, 0, s>>>(M, out, e.bias, g, R0, Tc, e.act, e.lo, e.hi, ncb);
-            else wino_output_kernel<8, false, false, CLIP><<<grid, kXformThreads, 0, s>>>(M, out, e.bias, g, R0, Tc, e.act, e.lo, e.hi, ncb);
-        }
+        if (e.pool) wino_output_kernel<8, true, CLIP><<<grid, kXformThreads, 0, s>>>(M, out, e.bias, g, R0, Tc, e.act, e.lo, e.hi, ncb);
+        else wino_output_kernel<8, false, CLIP><<<grid, kXformThreads, 0, s>>>(M, out, e.bias, g, R0, Tc, e.act, e.lo, e.hi, ncb);
     } else {
-        if (e.pool) wino_output_kernel<4, true, false, CLIP><<<grid, kXformThreads, 0, s>>>(M, out, e.bias, g, R0, Tc, e.act, e.lo, e.hi, ncb);
-        else wino_output_kernel<4, false, false, CLIP><<<grid, kXformThreads, 0, s>>>(M, out, e.bias, g, R0, Tc, e.act, e.lo, e.hi, ncb);
+        if (e.pool) wino_output_kernel<4, true, CLIP><<<grid, kXformThreads, 0, s>>>(M, out, e.bias, g, R0, Tc, e.act, e.lo, e.hi, ncb);
+        else wino_output_kernel<4, false, CLIP><<<grid, kXformThreads, 0, s>>>(M, out, e.bias, g, R0, Tc, e.act, e.lo, e.hi, ncb);
     }
 }
 
@@ -450,7 +410,7 @@ int wino_output_transform(int tile, const float* M, float* out, const WinoGeom& 
     const int Tc = (R1 - R0) * g.tilesX;
     dim3 grid(static_cast<unsigned>(segs) * (R1 - R0), ceil_div(g.C_out, kChBlock));
     int ncb = 0;
-    if (tune_get(TUNE_WINO_MLP) >= 2 && static_cast<unsigned long long>(grid.x) * grid.y < 0x7fffffffULL) {
+    if (static_cast<unsigned long long>(grid.x) * grid.y < 0x7fffffffULL) {
         ncb = static_cast<int>(grid.y);
         grid = dim3(grid.x * grid.y, 1);
     }
@@ -458,9 +418,8 @@ int wino_output_transform(int tile, const float* M, float* out, const WinoGeom& 
     const double out_px = e.pool ? static_cast<double>((g.OH + 1) / 2) * ((g.OW + 1) / 2) : static_cast<double>(g.OH) * g.OW;
     const int prof = prof_begin(s, PROF_WINO_OUTPUT, 0, 0,
                                 4.0 * (imgs * g.C_out * out_px + static_cast<double>(tile) * tile * Tc * g.C_out));
-    const bool mlp = tune_get(TUNE_WINO_MLP) != 0;
-    if (e.act == 2) wino_output_launch<true>(tile, mlp, grid, M, out, g, R0, Tc, e, ncb, s);
-    else wino_output_launch<false>(tile, mlp, grid, M, out, g, R0, Tc, e, ncb, s);
+    if (e.act == 2) wino_output_launch<true>(tile, grid, M, out, g, R0, Tc, e, ncb, s);
+    else wino_output_launch<false>(tile, grid, M, out, g, R0, Tc, e, ncb, s);
     prof_end(prof, s);
     FCUDA_CHECK_LAUNCH();
     count_launch();

@@ -540,15 +540,9 @@ int fcuda_slice_plan(int rank, int axis, const int* shape, const int* slices, in
 /* Kernel-variant switches for A/B measurements and tests.  Defaults are the measured-best configuration; the environment
  * variable FCUDA_<NAME> sets the initial value.  Names (value range, default):
  *   dw_vec (0-1, 1)           vectorised depthwise kernel on wide planes
- *   wino_mlp (0-2, 2)         Winograd transforms: 1 = every global load of a block in flight at once (cp.async slab /
- *                             back-to-back plane loads) instead of register-staged rounds; 2 = also launch the channel
- *                             blocks of a tile group next to each other (whole 1 KB rows of V / M in flight together)
  *   igemm_halo (0-1, 1)       implicit GEMM on stride-1, dense layers with IC % 32 == 0 (per group) and W % 4 == 0: the
  *                             input patch of 32 channels plus its halo arrives by one TMA load and serves every tap;
  *                             persistent CTAs, split and MMA of neighbouring k-blocks overlap.  0 = the gathering kernel
- *   gemm_pipe (0-1, 1)        TensorGEMM (Winograd, im2col, InnerProduct): persistent CTAs that fill the next tile's ring
- *                             stages during the epilogue; the split and MMAs of neighbouring k-blocks overlap and no wgmma
- *                             waits for the one before it.  Bit-identical to 0 = one CTA per tile, drained per k-block
  *   igemm_presplit (0-1, 1)   halo kernel in fp32split mode: each 32-channel input box is split into its two bf16 planes
  *                             once instead of once per tap and the A fragments are loaded by ldmatrix (128-pixel
  *                             tiles).  Bit-identical to 0 = the per-tap split
@@ -556,9 +550,6 @@ int fcuda_slice_plan(int rank, int axis, const int* shape, const int* slices, in
  *                             GEMM turned around (output channels on the wgmma M side, 224 pixels per warpgroup on N,
  *                             read from the split planes by descriptor), so each filter byte serves 1.75x (N tile 128)
  *                             or 3.5x (N tile 64) as many pixels.  Bit-identical to 0 = the pre-split kernel
- *   yolo_nms (0-1, 1)         YOLO NMS: CTAs over (32-row block, image) write the suppression mask, then one CTA per
- *                             image sweeps it.  0 = one CTA per image builds the whole mask in its own shared memory
- *                             and sweeps it.  Bit-identical
  *   igemm_stem (0-1, 1)       fp32split mode: the layers fcuda_igemm_stem_supported names (short K, e.g. IC = 3 first
  *                             layers) run on persistent CTAs that keep every filter k-block resident, gather the next
  *                             tile during the current one and write whole channel runs from a shared-memory staging
@@ -567,11 +558,13 @@ int fcuda_slice_plan(int rank, int axis, const int* shape, const int* slices, in
  *                             ShuffleChannel -> Slice (axis 0) chains, or any two adjacent of them, run as one
  *                             fcuda_route_forward launch.  Bit-identical to 0 = every routing layer on its own, while
  *                             the net's other fusions stay as they are
- *   persistent_ctas (0-65536, 0)  n > 0: every persistent kernel (stem, halo / pre-split / wide implicit GEMM, pipelined
+ *   persistent_ctas (0-65536, 0)  n > 0: every persistent kernel (stem, halo / pre-split / wide implicit GEMM,
  *                             TensorGEMM) runs at most n CTAs, so each CTA walks ceil(tiles / n) or fewer tiles whatever
  *                             the card's SM count.  For tests; feather::Net captures grids in its CUDA graphs, so set it
  *                             before a Net first runs.  Bit-identical to 0 = as many CTAs as fit on the device
- * Every variant computes the same result (tests/test_gpu_variants.py).  Returns 0 / the value, -200 for an unknown name or value. */
+ * Every variant computes the same result (tests/test_gpu_variants.py).  Returns 0 / the value, -200 for an unknown name or value.
+ * The retired names wino_mlp, gemm_pipe and yolo_nms are unknown names like any other: they return -200, and
+ * FCUDA_WINO_MLP, FCUDA_GEMM_PIPE and FCUDA_YOLO_NMS are not read. */
 int fcuda_set_tuning(const char* name, int value);
 int fcuda_get_tuning(const char* name);
 

@@ -1,14 +1,13 @@
-"""Per-layer timing of the TensorGEMM: the persistent, pipelined kernel (gemm_pipe = 1) against the one-tile-per-CTA
-kernel (gemm_pipe = 0), for every layer of VGG-16 (b64) and ResNet-50 (b128) that fcuda_conv_select_algo_tuned sends to
-Winograd, and for VGG-16's three InnerProduct layers at b64.
+"""Per-layer timing of the TensorGEMM, for every layer of VGG-16 (b64) and ResNet-50 (b128) that
+fcuda_conv_select_algo_tuned sends to Winograd, and for VGG-16's three InnerProduct layers at b64.
 
     python scripts/gemm_layer_bench.py --out DIR [--reps 5] [--iters 20]
 
-For each layer, with the two switch values alternated over --reps repetitions (median and every value): the CUDA-event
-time of the whole layer per forward, the time of its TensorGEMM launches alone (the per-launch profile hooks, a separate
-pass), the issued tensor-pipe rate of the GEMM (TF32 MMA FLOPs of the launches: M, N, K as launched, x3 in the split
-modes) and its fraction of the H100 SXM data-sheet dense TF32 rate, and whether both outputs are bit-identical.  Writes
-DIR/gemm_layer_bench.json with the card's name and power limit.  Needs a CUDA device."""
+For each layer, over --reps repetitions (median and every value): the CUDA-event time of the whole layer per forward,
+the time of its TensorGEMM launches alone (the per-launch profile hooks, a separate pass), the issued tensor-pipe rate of
+the GEMM (TF32 MMA FLOPs of the launches: M, N, K as launched, x3 in the split modes) and its fraction of the H100 SXM
+data-sheet dense TF32 rate.  Two builds are compared by running the script on each.  Writes DIR/gemm_layer_bench.json
+with the card's name and power limit.  Needs a CUDA device."""
 from __future__ import annotations
 
 import argparse
@@ -92,7 +91,6 @@ def main() -> None:
         raise SystemExit("gemm_layer_bench needs a CUDA device")
     torch.cuda.set_device(0)
     lib = fcuda()
-    saved = lib.fcuda_get_tuning(b"gemm_pipe")
     stream = booster._stream
     ptr = lambda t: ctypes.c_void_p(t.data_ptr())  # noqa: E731
 
@@ -169,63 +167,44 @@ def main() -> None:
     result = {"card": card(), "reps": args.reps, "iters": args.iters,
               "datasheet_tf32_dense_tflops": DATASHEET_TF32_DENSE / 1e12,
               "precision": {0: "tf32x3", 1: "tf32", 2: "fp32split"}[lib.fcuda_get_precision()], "layers": []}
-    try:
-        for model in args.models.split(","):
-            n = BATCH[model]
-            convs, fcs = winograd_layers(model)
-            jobs = {}
-            for name, pf, algo, pool in convs:  # one measurement per distinct shape
-                jobs.setdefault(("conv", pf, algo, pool), []).append(name)
-            if model == "vgg16":
-                for name, n_in, n_out in fcs:
-                    jobs.setdefault(("ip", n_in, n_out), []).append(name)
-            for key, names in jobs.items():
-                if key[0] == "conv":
-                    launch, out = prepare_conv(key[1], key[2], n, key[3])
-                    desc = {"kind": booster.ALGO_NAMES[key[2]] if hasattr(booster, "ALGO_NAMES") else key[2],
-                            "oc_ic_h_w_k_s_pad_group": list(key[1]), "fused_pool": key[3]}
-                else:
-                    launch, out = prepare_ip(key[1], key[2], n)
-                    desc = {"kind": "InnerProduct", "in": key[1], "out": key[2]}
-                layer_t, gemm_t, issued = {0: [], 1: []}, {0: [], 1: []}, {}
-                outs, launches = {}, {}
-                for _ in range(args.reps):
-                    for sw in (0, 1):
-                        assert lib.fcuda_set_tuning(b"gemm_pipe", sw) == 0
-                        layer_t[sw].append(time_ms(launch, args.iters))
-                        outs[sw] = out.clone()
-                        ms, mf, nl = gemm_ms(launch, args.iters)
-                        gemm_t[sw].append(ms)
-                        issued[sw], launches[sw] = mf, nl
-                identical = bool(torch.equal(outs[0], outs[1]))
-                del outs
-                med = {sw: (statistics.median(layer_t[sw]), statistics.median(gemm_t[sw])) for sw in (0, 1)}
-                rec = {"model": model, "layer": ",".join(names), "count": len(names), "batch": n, **desc,
-                       "gemm_launches_per_forward": launches[1], "issued_mma_gflop": issued[1] / 1e9,
-                       "layer_ms_median": {str(sw): med[sw][0] for sw in (0, 1)},
-                       "gemm_ms_median": {str(sw): med[sw][1] for sw in (0, 1)},
-                       "layer_ms": {str(sw): layer_t[sw] for sw in (0, 1)},
-                       "gemm_ms": {str(sw): gemm_t[sw] for sw in (0, 1)},
-                       "gemm_speedup": med[0][1] / med[1][1], "layer_speedup": med[0][0] / med[1][0],
-                       "issued_tf32_tflops": {str(sw): issued[sw] / med[sw][1] / 1e9 for sw in (0, 1)},
-                       "issued_fraction_of_datasheet_tf32": {str(sw): issued[sw] / med[sw][1] / 1e-3 / DATASHEET_TF32_DENSE
-                                                             for sw in (0, 1)},
-                       "bit_identical": identical}
-                result["layers"].append(rec)
-                print(json.dumps({k2: rec[k2] for k2 in ("model", "layer", "layer_ms_median", "gemm_ms_median",
-                                                          "gemm_speedup", "issued_tf32_tflops", "bit_identical")}),
-                      flush=True)
-                del launch, out
-                torch.cuda.empty_cache()
-    finally:
-        lib.fcuda_set_tuning(b"gemm_pipe", saved)
+    for model in args.models.split(","):
+        n = BATCH[model]
+        convs, fcs = winograd_layers(model)
+        jobs = {}
+        for name, pf, algo, pool in convs:  # one measurement per distinct shape
+            jobs.setdefault(("conv", pf, algo, pool), []).append(name)
+        if model == "vgg16":
+            for name, n_in, n_out in fcs:
+                jobs.setdefault(("ip", n_in, n_out), []).append(name)
+        for key, names in jobs.items():
+            if key[0] == "conv":
+                launch, out = prepare_conv(key[1], key[2], n, key[3])
+                desc = {"kind": booster.ALGO_NAMES[key[2]] if hasattr(booster, "ALGO_NAMES") else key[2],
+                        "oc_ic_h_w_k_s_pad_group": list(key[1]), "fused_pool": key[3]}
+            else:
+                launch, out = prepare_ip(key[1], key[2], n)
+                desc = {"kind": "InnerProduct", "in": key[1], "out": key[2]}
+            layer_t, gemm_t = [], []
+            for _ in range(args.reps):
+                layer_t.append(time_ms(launch, args.iters))
+                ms, issued, launches = gemm_ms(launch, args.iters)
+                gemm_t.append(ms)
+            layer_med, gemm_med = statistics.median(layer_t), statistics.median(gemm_t)
+            rec = {"model": model, "layer": ",".join(names), "count": len(names), "batch": n, **desc,
+                   "gemm_launches_per_forward": launches, "issued_mma_gflop": issued / 1e9,
+                   "layer_ms_median": layer_med, "gemm_ms_median": gemm_med, "layer_ms": layer_t, "gemm_ms": gemm_t,
+                   "issued_tf32_tflops": issued / gemm_med / 1e9,
+                   "issued_fraction_of_datasheet_tf32": issued / gemm_med / 1e-3 / DATASHEET_TF32_DENSE}
+            result["layers"].append(rec)
+            print(json.dumps({k2: rec[k2] for k2 in ("model", "layer", "layer_ms_median", "gemm_ms_median",
+                                                      "issued_tf32_tflops")}), flush=True)
+            del launch, out
+            torch.cuda.empty_cache()
     for model in BATCH:
         rows = [r for r in result["layers"] if r["model"] == model]
-        for sw in ("0", "1"):
-            if rows:
-                result[f"{model}_gemm_total_ms_{sw}"] = sum(r["gemm_ms_median"][sw] * r["count"] for r in rows)
-                result[f"{model}_layer_total_ms_{sw}"] = sum(r["layer_ms_median"][sw] * r["count"] for r in rows)
-    result["all_bit_identical"] = all(r["bit_identical"] for r in result["layers"])
+        if rows:
+            result[f"{model}_gemm_total_ms"] = sum(r["gemm_ms_median"] * r["count"] for r in rows)
+            result[f"{model}_layer_total_ms"] = sum(r["layer_ms_median"] * r["count"] for r in rows)
     out_dir = Path(args.out)
     out_dir.mkdir(parents=True, exist_ok=True)
     (out_dir / "gemm_layer_bench.json").write_text(json.dumps(result, indent=1))

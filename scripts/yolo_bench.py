@@ -6,10 +6,9 @@ Models (modelgen.mobilenet_yolov2 and mobilenetv2_yolov3, 416 x 416, fusion and 
 images/s at --batch, latency at batch 1, launches per forward, and the share of each kernel class in an eager forward
 (kind 9 is the detection head: YOLO decode, select, mask, sweep).  The head alone (fcuda_yolo_detection_forward, 80
 classes, 3 anchors per scale, nms_top_k = keep_top_k = 1024) at 416 (13 / 26 / 52: 10647 slots) and 608 (19 / 38 / 76:
-22743 slots), with hundreds of candidates and with more than 1024, at batch 1 and --batch, for both NMS variants of the
-yolo_nms switch (1: CTAs over (32-row block, image) write the suppression mask, then one sweep CTA per image; 0: one CTA
-per image builds the mask in its own shared memory and sweeps it): the whole head timed with CUDA events (--reps windows
-of --head-iters calls, the median), and each kernel from a torch.profiler run of its own over --head-iters calls.
+22743 slots), with hundreds of candidates and with more than 1024, at batch 1 and --batch: the whole head timed with
+CUDA events (--reps windows of --head-iters calls, the median), and each kernel from a torch.profiler run of its own over
+--head-iters calls.
 Writes DIR/yolo_bench.json and .md with the card's name and power limit, read in the same run.  Needs a CUDA device."""
 from __future__ import annotations
 
@@ -30,8 +29,7 @@ from mobilenet_v2_bench import load  # noqa: E402
 from ssd_bench import kind_shares, timed  # noqa: E402
 
 COCO = [10, 13, 16, 30, 33, 23, 30, 61, 62, 45, 59, 119, 116, 90, 156, 198, 373, 326]
-KERNELS = ["yolo_decode_kernel", "yolo_select_kernel", "yolo_mask_kernel", "yolo_sweep_kernel", "yolo_nms_fused_kernel"]
-VARIANTS = {1: "split", 0: "single CTA"}  # fcuda_set_tuning("yolo_nms", v)
+KERNELS = ["yolo_decode_kernel", "yolo_select_kernel", "yolo_mask_kernel", "yolo_sweep_kernel"]
 
 
 class Head:
@@ -66,11 +64,6 @@ class Head:
         rc = self.lib.fcuda_yolo_detection_forward(ctypes.c_void_p(self.out.data_ptr()), self.arr, ctypes.byref(self.p),
                                                    ctypes.c_void_p(self.ws.data_ptr()), self.batch, self.stream)
         assert rc == 0, rc
-
-
-def booster_lib():
-    from feathercnn_b200 import booster
-    return booster.fcuda()
 
 
 def time_calls(fn, reps: int, iters: int) -> float:
@@ -145,19 +138,15 @@ def main() -> None:
                         "kind_shares_eager": shares}
         del net_b, net_1
     heads = []
-    lib = booster_lib()
     for size in (416, 608):
         for label, obj in (("hundreds", -8.0), ("many", 0.0)):
             for b in (1, args.batch):
                 h = Head(size, b, obj)
-                for v, vname in VARIANTS.items():
-                    assert lib.fcuda_set_tuning(b"yolo_nms", v) == 0
-                    row = {"size": size, "slots": h.slots, "candidates_per_image": h.candidates, "label": label,
-                           "batch": b, "nms": vname, "ms": time_calls(h, args.reps, args.head_iters)}
-                    row.update(kernel_times(h, args.head_iters))
-                    heads.append(row)
+                row = {"size": size, "slots": h.slots, "candidates_per_image": h.candidates, "label": label,
+                       "batch": b, "ms": time_calls(h, args.reps, args.head_iters)}
+                row.update(kernel_times(h, args.head_iters))
+                heads.append(row)
                 del h
-    lib.fcuda_set_tuning(b"yolo_nms", 1)
     info = card()
     res = {"card": info, "fusion": True, "cuda_graph": True, "models": models, "head_alone": heads}
     out = Path(args.out)
@@ -169,9 +158,9 @@ def main() -> None:
                   f"{r['launches_per_forward']} launches / forward; batch 1 latency {r['batch1_latency_ms']:.3f} ms; "
                   f"detection head (kind 9) {r['head_kind9_share_eager']:.1%} of an eager forward")
     md += ["", "Head alone (80 classes, nms_top_k = keep_top_k = 1024), ms per call; kernels from torch.profiler:", "",
-           "| slots | candidates / image | batch | NMS | head | decode | select | mask | sweep | single-CTA NMS |",
-           "|---|---|---|---|---|---|---|---|---|---|"]
-    md += [f"| {r['slots']} ({r['size']}) | {r['candidates_per_image']:.0f} | {r['batch']} | {r['nms']} | {r['ms']:.4f} | "
+           "| slots | candidates / image | batch | head | decode | select | mask | sweep |",
+           "|---|---|---|---|---|---|---|---|"]
+    md += [f"| {r['slots']} ({r['size']}) | {r['candidates_per_image']:.0f} | {r['batch']} | {r['ms']:.4f} | "
            + " | ".join(f"{r[k]:.4f}" for k in KERNELS) + " |" for r in heads]
     (out / "yolo_bench.md").write_text("\n".join(md) + "\n")
     print("\n".join(md))

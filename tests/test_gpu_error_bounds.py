@@ -448,6 +448,7 @@ WINO_SWEEP = [
     Conv("w_pool", 40, 16, 15, 13, pool=True, relu=True),
     Conv("w_chunked", 32, 32, 60, 120, batch=2, chunk=1),          # one chunk holds a few tile rows of an image
     Conv("w_res_relu", 48, 32, 12, 14, res=True, relu_after_add=True),
+    Conv("w_oc40_ic48", 40, 48, 26, 22, batch=3, relu=True),       # OC 40: a partial BN 64 tile; IC 48: K % 32 = 16
 ]
 
 
@@ -497,6 +498,8 @@ GEMM_CASES = (
     [(2, 129, n, 44) for n in (32, 33, 64, 65, 128, 129, 300)]     # N tiles; K % 32 = 12
     + [(3, m, 65, 60) for m in (127, 128, 129)]                    # M tiles; K % 32 = 28
     + [(64, 127, 33, 36), (64, 64, 64, 100), (1, 128, 300, 228)]   # G up to 64; K % 32 = 4
+    + [(64, 1024, 256, 128),                                       # 1024 tiles: several per persistent CTA
+       (7, 127, 65, 1000)]                                         # 32 k-blocks (K % 32 = 8) per tile, odd G
 )
 
 
@@ -563,6 +566,9 @@ IP_CASES = [
     (4096, 1000, 256, False),   # several k-splits, two N tiles
     (36, 65, 129, False),       # K % 32 = 4
     (998, 40, 7, True),         # input_size % 4 != 0: SIMT fallback
+    (25088, 4096, 64, True),    # VGG-16 fc6: 784 k-blocks in 9 splits of 88; the last owns 80
+    (1316, 200, 129, True),     # 42 k-blocks in 5 splits of 9; the last owns 6
+    (4096, 1000, 1, True),      # batch 1: one partial N tile
 ]
 
 

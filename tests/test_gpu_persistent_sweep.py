@@ -1,7 +1,7 @@
 """Seeded random shapes across the persistent tensor-core kernels, with a set number of CTAs, against float64.
 
 Five kernels run on persistent CTAs that walk the tile list with a static stride: the stem kernel, the halo, pre-split
-and wide implicit-GEMM kernels (conv_igemm.cu, launch_igemm_kernel(..., persistent=true)) and tensor_gemm_pipe_kernel
+and wide implicit-GEMM kernels (conv_igemm.cu, launch_igemm_kernel(..., persistent=true)) and tensor_gemm_kernel
 (Winograd, im2col, InnerProduct, the raw TensorGEMM).  Most of their hardest code runs only when a CTA gets a second
 tile: ring slots and mbarrier phases carried over from one tile to the next (the TensorGEMM's running k-block count,
 the halo family's 4-deep filter and 2-deep box rings), the next tile's loads or gather issued during the current tile's

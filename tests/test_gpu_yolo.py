@@ -18,8 +18,7 @@
   - Selection, NMS and output decision by decision, bit for bit, against test_yolo_host.yolo_ref fed the kernel's own
     decoded candidates (fcuda_yolo_decode): no candidates; exactly 32 / 33 / 1023 / 1024 / 1025; nms_top_k / keep_top_k
     truncation; exact confidence ties; zero-area boxes; one survivor; all 10647 slots of the 416 x 416 YOLOv3 geometry
-    above the threshold.  Every case but the first asserts that NMS suppressed something.  Each case runs both NMS
-    variants of the yolo_nms switch (mask CTAs + sweep CTA, and one CTA per image), so the two are bit-identical.
+    above the threshold.  Every case but the first asserts that NMS suppressed something.
   - A seeded sweep of random geometries across the decode (scale boundaries, grid sides, C, num_box), select (candidate
     counts around 32 and 1024, nms_top_k), mask (row blocks of 32) and sweep (keep_top_k) boundaries.
   - Batch independence of the layer and of the nets; a channel-count mismatch fails at Reshape.
@@ -200,21 +199,9 @@ def run_and_check(xs, p):
     return want, suppressed, candidates, s
 
 
-@pytest.fixture
-def yolo_nms():
-    """Sets the yolo_nms switch (1: mask CTAs + sweep CTA, 0: one CTA per image) and restores it."""
-    from feathercnn_b200._lib import fcuda
-    lib = fcuda()
-    saved = lib.fcuda_get_tuning(b"yolo_nms")
-    yield lambda v: lib.fcuda_set_tuning(b"yolo_nms", v)
-    lib.fcuda_set_tuning(b"yolo_nms", saved)
-
-
 @gpu
-@pytest.mark.parametrize("variant", [1, 0], ids=["split", "single_cta"])
 @pytest.mark.parametrize("name", SEL_CASES)
-def test_selection_nms_decisions(cuda, yolo_nms, name, variant):
-    assert yolo_nms(variant) == 0
+def test_selection_nms_decisions(cuda, name):
     rng = np.random.default_rng(SEL_CASES.index(name) + 31)
     xs, p = _sel_case(name, rng)
     want, suppressed, candidates, s = run_and_check(xs, p)
@@ -290,10 +277,8 @@ def test_sweep_cases_cover_the_boundaries():
 
 @gpu
 @pytest.mark.parametrize("i", range(SWEEP_N))
-def test_random_geometry(cuda, yolo_nms, i):
-    """Odd cases run the single-CTA NMS, even ones the split one."""
+def test_random_geometry_matches_reference(cuda, i):
     from feathercnn_b200 import booster
-    assert yolo_nms(1 - i % 2) == 0
     xs, p = _sweep_case(i)
     dev = _cuda(xs)
     check_decode(xs, p, booster.yolo_decode(dev, p))

@@ -41,8 +41,8 @@ def _kernels(ops, pattern):
 
 
 @pytest.mark.parametrize("pattern, per_group", [
-    (r"tensor_gemm_pipe_kernelILi(32|64|128)ELi2E", 12),   # 3xTF32 TensorGEMM: 3 MMAs x 4 k-steps per k-block
-    (r"tensor_gemm_pipe_kernelILi(32|64|128)ELi1E", 4),    # TF32 TensorGEMM
+    (r"tensor_gemm_kernelILi(32|64|128)ELi2E", 12),        # 3xTF32 TensorGEMM: 3 MMAs x 4 k-steps per k-block
+    (r"tensor_gemm_kernelILi(32|64|128)ELi1E", 4),         # TF32 TensorGEMM
     (r"conv_igemm_kernelILi(32|64|128)ELi3E", 6),          # BF16x3 gathering implicit GEMM: 3 MMAs x 2 k-steps
     (r"conv_igemm_kernelILi(32|64|128)ELi1E", 4),          # TF32 gathering implicit GEMM
     pytest.param(r"conv_igemm_halo_kernelILi(32|64|128)ELi3ELb0E", 6,  # BF16x3 per-tap halo implicit GEMM
@@ -57,10 +57,3 @@ def test_wgmma_are_not_serialised(pattern, per_group):
         # at most one wait per commit group plus the drain at the end of a tile (serialised code has one per HGMMA)
         assert 1 <= depbar <= hgmma // per_group + 1 and depbar < hgmma, (k, hgmma, depbar)
 
-
-def test_gemm_pipe_switch_is_registered():
-    from feathercnn_b200._lib import fcuda
-    lib = fcuda()
-    assert lib.fcuda_get_tuning(b"gemm_pipe") == 1
-    assert lib.fcuda_set_tuning(b"gemm_pipe", 2) == -200
-    assert lib.fcuda_set_tuning(b"gemm_pipe", -1) == -200
