@@ -90,6 +90,13 @@ class FcudaYoloParam(ctypes.Structure):
                  ("grid_w", ctypes.c_int * 4)])
 
 
+class FcudaProposalParam(ctypes.Structure):
+    """include/fcuda.h FcudaProposalParam."""
+
+    _fields_ = [("feat_stride", ctypes.c_int), ("base_size", ctypes.c_int), ("pre_nms_topN", ctypes.c_int),
+                ("after_nms_topN", ctypes.c_int), ("nms_thresh", ctypes.c_float), ("min_size", ctypes.c_int)]
+
+
 class FcudaRoute(ctypes.Structure):
     """include/fcuda.h FcudaRoute (up to FCUDA_ROUTE_MAX = 8 sources and destinations)."""
 
@@ -110,6 +117,7 @@ def fcuda() -> ctypes.CDLL:
         R = ctypes.POINTER(FcudaInterpParam)
         PB = ctypes.POINTER(FcudaPriorBoxParam)
         Y = ctypes.POINTER(FcudaYoloParam)
+        PP = ctypes.POINTER(FcudaProposalParam)
         f = ctypes.c_float
         sigs = {
             "fcuda_permute_forward": (i, [vp, vp, i, i, i, i, i, vp]),
@@ -122,6 +130,11 @@ def fcuda() -> ctypes.CDLL:
             "fcuda_yolo_decode": (i, [vp, vp, vp, vp, Y, i, vp]),
             "fcuda_yolo_detection_workspace_size": (i, [Y, i, szp]),
             "fcuda_yolo_detection_forward": (i, [vp, vp, Y, vp, i, vp]),
+            "fcuda_proposal_anchors": (i, [PP, vp]),
+            "fcuda_proposal_decode": (i, [vp, vp, vp, vp, PP, i, i, i, vp]),
+            "fcuda_proposal_workspace_size": (i, [PP, i, i, i, szp]),
+            "fcuda_proposal_forward": (i, [vp, vp, vp, vp, vp, PP, i, i, vp, i, vp]),
+            "fcuda_roi_pooling_forward": (i, [vp, vp, vp, i, i, i, i, i, i, f, i, vp]),
             "fcuda_route_forward": (i, [ctypes.POINTER(FcudaRoute), i, vp]),
             "fcuda_slice_plan": (i, [i, i, ctypes.POINTER(i), ctypes.POINTER(i), i, ctypes.POINTER(i), ctypes.POINTER(i)]),
             "fcuda_interp_output_dim": (i, [R]),

@@ -16,6 +16,7 @@ from ._lib import FcudaConvOptions, FcudaConvParam, fcuda
 from ._lib import FcudaDeconvParam as DeconvParam
 from ._lib import FcudaInterpParam as InterpParam
 from ._lib import FcudaPriorBoxParam as PriorBoxParam
+from ._lib import FcudaProposalParam as ProposalParam
 from ._lib import FcudaYoloParam as YoloParam
 
 NAIVE, IM2COL, SGECONV, DEPTHWISE, WINOGRADF63, WINOGRADF63FUSED, WINOGRADF23 = range(7)
@@ -626,3 +627,79 @@ def tensor_gemm(a: torch.Tensor, b: torch.Tensor, x3: bool = True) -> torch.Tens
     else:
         _check("fcuda_tensor_gemm", lib.fcuda_tensor_gemm(_ptr(d), _ptr(a), _ptr(b), None, m, n, k, g, _stream()))
     return d
+
+
+# ---- Faster R-CNN: Proposal and ROIPooling ------------------------------------------------------------------------
+PROPOSAL_ANCHORS = 9
+
+
+def proposal_param(feat_stride: int = 16, base_size: int = 16, pre_nms_topN: int = 6000, after_nms_topN: int = 300,
+                   nms_thresh: float = 0.7, min_size: int = 16) -> ProposalParam:
+    """FcudaProposalParam with ncnn's defaults."""
+    p = ProposalParam()
+    p.feat_stride, p.base_size, p.pre_nms_topN, p.after_nms_topN = feat_stride, base_size, pre_nms_topN, after_nms_topN
+    p.nms_thresh, p.min_size = float(nms_thresh), min_size
+    return p
+
+
+def proposal_anchors(p: ProposalParam) -> list[tuple[float, float, float, float]]:
+    """The 9 anchors of p as (ax1, ay1, aw, ah), from the library."""
+    table = (ctypes.c_float * (4 * PROPOSAL_ANCHORS))()
+    _check("fcuda_proposal_anchors", fcuda().fcuda_proposal_anchors(ctypes.byref(p), table))
+    return [tuple(table[4 * q:4 * q + 4]) for q in range(PROPOSAL_ANCHORS)]
+
+
+def _proposal_inputs(score: torch.Tensor, bbox: torch.Tensor, im_info: torch.Tensor):
+    """The bottoms as the C side reads them: float32 CUDA tensors of one batch, score (N, 18, H, W), bbox (N, 36, H, W),
+    im_info 3 values per image."""
+    score, bbox, im_info = score.contiguous(), bbox.contiguous(), im_info.contiguous()
+    for t in (score, bbox, im_info):
+        assert t.is_cuda and t.dtype == torch.float32, (t.device, t.dtype)
+    assert score.dim() == 4 and score.shape[1] == 2 * PROPOSAL_ANCHORS, tuple(score.shape)
+    n, _, h, w = score.shape
+    assert tuple(bbox.shape) == (n, 4 * PROPOSAL_ANCHORS, h, w), (tuple(bbox.shape), tuple(score.shape))
+    assert im_info.shape[0] == n and im_info.numel() == 3 * n, tuple(im_info.shape)
+    return score, bbox, im_info, n, h, w
+
+
+def proposal_decode(score: torch.Tensor, bbox: torch.Tensor, im_info: torch.Tensor, p: ProposalParam) -> torch.Tensor:
+    """-> (N, 9 * H * W, 4) clipped boxes of every anchor and cell, index q * H * W + y * W + x, candidate or not."""
+    score, bbox, im_info, n, h, w = _proposal_inputs(score, bbox, im_info)
+    boxes = torch.empty((n, PROPOSAL_ANCHORS * h * w, 4), device=score.device, dtype=torch.float32)
+    _check("fcuda_proposal_decode", fcuda().fcuda_proposal_decode(_ptr(boxes), _ptr(score), _ptr(bbox), _ptr(im_info),
+                                                                  ctypes.byref(p), h, w, n, _stream()))
+    return boxes
+
+
+def proposal(score: torch.Tensor, bbox: torch.Tensor, im_info: torch.Tensor, p: ProposalParam):
+    """-> (rois (N, after_nms_topN, 4) [x1, y1, x2, y2], zero rows past each image's count; scores (N, after_nms_topN),
+    -1 past the count)."""
+    lib = fcuda()
+    score, bbox, im_info, n, h, w = _proposal_inputs(score, bbox, im_info)
+    ws = ctypes.c_size_t(0)
+    _check("fcuda_proposal_workspace_size", lib.fcuda_proposal_workspace_size(ctypes.byref(p), h, w, n, ctypes.byref(ws)))
+    workspace = torch.empty(max(ws.value, 1), device=score.device, dtype=torch.float32)
+    rois = torch.empty((n, p.after_nms_topN, 4), device=score.device, dtype=torch.float32)
+    scores = torch.empty((n, p.after_nms_topN), device=score.device, dtype=torch.float32)
+    _check("fcuda_proposal_forward", lib.fcuda_proposal_forward(_ptr(rois), _ptr(scores), _ptr(score), _ptr(bbox),
+                                                                _ptr(im_info), ctypes.byref(p), h, w, _ptr(workspace), n,
+                                                                _stream()))
+    return rois, scores
+
+
+def roi_pooling(x: torch.Tensor, rois: torch.Tensor, pooled_h: int = 7, pooled_w: int = 7,
+                spatial_scale: float = 0.0625) -> torch.Tensor:
+    """x (N, C, H, W), rois (N, R, 4) or (N, R, 1, 4) -> (N * R, C, pooled_h, pooled_w); RoI r of image n pools image n."""
+    x, rois = x.contiguous(), rois.contiguous()
+    for t in (x, rois):
+        assert t.is_cuda and t.dtype == torch.float32, (t.device, t.dtype)
+    assert x.dim() == 4 and rois.shape[0] == x.shape[0] and rois.shape[-1] == 4 and rois.dim() in (3, 4), \
+        (tuple(x.shape), tuple(rois.shape))
+    n, c, h, w = x.shape
+    r = rois.shape[1]
+    assert rois.numel() == 4 * n * r, tuple(rois.shape)
+    out = torch.empty((n * r, c, pooled_h, pooled_w), device=x.device, dtype=torch.float32)
+    _check("fcuda_roi_pooling_forward", fcuda().fcuda_roi_pooling_forward(_ptr(out), _ptr(x), _ptr(rois), c, h, w, r,
+                                                                          pooled_h, pooled_w, float(spatial_scale), n,
+                                                                          _stream()))
+    return out

@@ -24,6 +24,7 @@ namespace {
 constexpr int kDetThreads = 512;
 constexpr int kDetWarps = kDetThreads / 32;
 constexpr int kMaxTopK = 1024;  // nms_top_k and keep_top_k limit: the candidates of one CTA live in shared memory
+constexpr int kProposalMaxTopK = 8192;  // pre_nms_topN / after_nms_topN limit: 64 KB of keys in dynamic shared memory
 
 // ---- Permute --------------------------------------------------------------------------------------------------------
 // Input axis (0 = c, 1 = h, 2 = w) of each output axis, per ncnn order_type.
@@ -194,15 +195,20 @@ __device__ __forceinline__ int key_index(unsigned long long k) {
     return static_cast<int>(0xffffffffu - static_cast<uint32_t>(k));
 }
 
-struct SelectSmem {
-    unsigned long long keys[kMaxTopK];
+// The scratch of select_top_k; the keys live apart, so their capacity is the caller's: SSD's and YOLO's CTAs hold
+// kMaxTopK of them in SelectSmem, Proposal's up to kProposalMaxTopK in dynamic shared memory.
+struct SelectScratch {
     int hist[256];
     int warp_sums[kDetWarps];
     int bcast[2];
 };
+struct SelectSmem {
+    unsigned long long keys[kMaxTopK];
+    SelectScratch s;
+};
 
 // Exclusive prefix of a 0/1 flag over the CTA in thread order; *total gets the CTA's sum.  Every thread calls it.
-__device__ __forceinline__ int block_scan(int flag, int* total, SelectSmem& sm) {
+__device__ __forceinline__ int block_scan(int flag, int* total, SelectScratch& sm) {
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     const unsigned m = __ballot_sync(0xffffffffu, flag);
     if (lane == 0) sm.warp_sums[warp] = __popc(m);
@@ -219,7 +225,7 @@ __device__ __forceinline__ int block_scan(int flag, int* total, SelectSmem& sm) 
     return before + __popc(m & ((1u << lane) - 1u));
 }
 
-__device__ __forceinline__ int block_sum(int v, SelectSmem& sm) {
+__device__ __forceinline__ int block_sum(int v, SelectScratch& sm) {
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
     if (threadIdx.x == 0) sm.bcast[0] = 0;
@@ -232,11 +238,12 @@ __device__ __forceinline__ int block_sum(int v, SelectSmem& sm) {
 }
 
 // The k largest keys (score image u descending, then index ascending) among the valid elements 0..n-1 of get(i, u):
-// their keys go to sm.keys[0..m) sorted descending, m = min(k, number valid) is returned.  An exact radix select of the
+// their keys go to keys[0..m) sorted descending, m = min(k, number valid) is returned.  `keys` (shared memory) holds the
+// next power of two >= k keys: the bitonic sort pads to it.  An exact radix select of the
 // k-th largest u (four 8-bit passes) gives the threshold T; every element above T is taken, and of those equal to T the
 // ones with the smallest indices (an ordered scan).  Every thread calls it.
 template <class Get>
-__device__ int select_top_k(int n, int k, Get get, SelectSmem& sm) {
+__device__ int select_top_k(int n, int k, Get get, unsigned long long* keys, SelectScratch& sm) {
     const int tid = threadIdx.x;
     int local = 0;
     for (int i = tid; i < n; i += kDetThreads) {
@@ -284,24 +291,24 @@ __device__ int select_top_k(int n, int k, Get get, SelectSmem& sm) {
         const bool eq = v && !all && u == prefix;
         int chunk_ties;
         const int before = block_scan(eq, &chunk_ties, sm);
-        if (v && (all || u > prefix || (eq && ties + before < need))) sm.keys[atomicAdd(&sm.bcast[1], 1)] = make_key(u, i);
+        if (v && (all || u > prefix || (eq && ties + before < need))) keys[atomicAdd(&sm.bcast[1], 1)] = make_key(u, i);
         ties += chunk_ties;
     }
     // bitonic sort, descending, over the next power of two (padding keys 0 sort last: a real key is >= 1)
     int len = 1;
     while (len < m) len <<= 1;
     __syncthreads();
-    for (int i = m + tid; i < len; i += kDetThreads) sm.keys[i] = 0;
+    for (int i = m + tid; i < len; i += kDetThreads) keys[i] = 0;
     __syncthreads();
     for (int size = 2; size <= len; size <<= 1)
         for (int stride = size >> 1; stride > 0; stride >>= 1) {
             for (int t = tid; t < (len >> 1); t += kDetThreads) {
                 const int lo = (t / stride) * stride * 2 + (t % stride), hi = lo + stride;
                 const bool desc = (lo & size) == 0;
-                const unsigned long long a = sm.keys[lo], b = sm.keys[hi];
+                const unsigned long long a = keys[lo], b = keys[hi];
                 if (desc ? a < b : a > b) {
-                    sm.keys[lo] = b;
-                    sm.keys[hi] = a;
+                    keys[lo] = b;
+                    keys[hi] = a;
                 }
             }
             __syncthreads();
@@ -309,10 +316,19 @@ __device__ int select_top_k(int n, int k, Get get, SelectSmem& sm) {
     return m;
 }
 
-// IoU of two boxes, operation by operation as include/fcuda.h states it (no contraction into FMA)
+// IoU of two boxes, operation by operation as include/fcuda.h states it (no contraction into FMA).  PLUS_ONE is
+// Proposal's pixel convention: each side of the overlap is min - max + 1 (and the caller's areas carry the same + 1);
+// without it the operations are DetectionOutput's and YOLO's.
+template <bool PLUS_ONE = false>
 __device__ __forceinline__ float box_iou(const float* a, float area_a, const float* b, float area_b) {
-    const float iw = fmaxf(__fsub_rn(fminf(a[2], b[2]), fmaxf(a[0], b[0])), 0.f);
-    const float ih = fmaxf(__fsub_rn(fminf(a[3], b[3]), fmaxf(a[1], b[1])), 0.f);
+    float iw = __fsub_rn(fminf(a[2], b[2]), fmaxf(a[0], b[0]));
+    float ih = __fsub_rn(fminf(a[3], b[3]), fmaxf(a[1], b[1]));
+    if (PLUS_ONE) {
+        iw = __fadd_rn(iw, 1.f);
+        ih = __fadd_rn(ih, 1.f);
+    }
+    iw = fmaxf(iw, 0.f);
+    ih = fmaxf(ih, 0.f);
     const float inter = __fmul_rn(iw, ih);
     return __fdiv_rn(inter, __fsub_rn(__fadd_rn(area_a, area_b), inter));
 }
@@ -336,7 +352,7 @@ nms_class_kernel(const float* __restrict__ conf, const float* __restrict__ boxes
         const float s = cf[static_cast<size_t>(i) * C];
         u = orderable(s);
         return s > conf_thr;
-    }, sm);
+    }, sm.keys, sm.s);
     const float* ib = boxes + static_cast<size_t>(n) * P * 4;
     for (int j = tid; j < m; j += kDetThreads) {
         const float* b = ib + static_cast<size_t>(key_index(sm.keys[j])) * 4;
@@ -358,7 +374,7 @@ nms_class_kernel(const float* __restrict__ conf, const float* __restrict__ boxes
         const int j = base + tid;
         const int keep = j < m && !sup[j];
         int total;
-        const int pos = block_scan(keep, &total, sm);
+        const int pos = block_scan(keep, &total, sm.s);
         if (keep) out[written + pos] = sm.keys[j];
         written += total;
     }
@@ -379,7 +395,7 @@ merge_kernel(float* __restrict__ out, const float* __restrict__ conf, const floa
         if (c == 0 || v - c * top_k >= counts[c]) return false;
         u = static_cast<uint32_t>(lists[v] >> 32);
         return true;
-    }, sm);
+    }, sm.keys, sm.s);
     const float* ib = boxes + static_cast<size_t>(n) * P * 4;
     float* o = out + static_cast<size_t>(n) * keep_top_k * 6;
     for (int r = threadIdx.x; r < keep_top_k; r += kDetThreads) {
@@ -541,7 +557,7 @@ yolo_select_kernel(const YoloWorkspace w, int slots, float thr, int top_k) {
         const float s = sc[i];
         u = orderable(s);
         return s >= thr;
-    }, sm);
+    }, sm.keys, sm.s);
     const float* ib = w.boxes + static_cast<size_t>(n) * slots * 4;
     for (int j = threadIdx.x; j < m; j += kDetThreads) {
         const unsigned long long key = sm.keys[j];
@@ -827,6 +843,369 @@ int yolo_detection(float* out, const float* const* inputs, const FcudaYoloParam&
     if (rc) return rc;
     prof = prof_begin(s, PROF_DETECTION, 0, 0, 4.0 * batch * p.nms_top_k * kYoloMaskWords + 24.0 * batch * p.keep_top_k);
     yolo_sweep_kernel<<<static_cast<unsigned>(batch), kDetThreads, smem, s>>>(out, w, g.slots, p.keep_top_k);
+    FCUDA_CHECK_LAUNCH();
+    prof_end(prof, s);
+    count_launch();
+    return 0;
+}
+
+namespace {
+
+// ---- Faster R-CNN: Proposal and ROIPooling -------------------------------------------------------------------------
+// decode    one thread per (image, anchor, cell): the clipped box and the candidate key (the orderable image of the
+//           foreground score, 0 for a box below min_size or a NaN score) into the workspace;
+// select    one CTA per image: select_top_k over the A * H * W keys, up to kProposalMaxTopK of them sorted in dynamic
+//           shared memory; the selected boxes, their + 1 areas and anchor-cell indices go to the workspace;
+// mask      CTAs over (32-row block, image): word w of row i has bit b set iff j = 32 w + b > i and IoU(i, j) > thresh,
+//           the columns staged through shared memory 1024 at a time; K x ceil(K / 32) words in global memory;
+// sweep     one warp per image: the removal bitmap in shared memory; find-first-set over the live bits of one word at a
+//           time, each kept box ORs its mask row (from L2) into the bitmap and writes its output row; stops at
+//           after_nms_topN.
+// roi_pool  one thread per output element, pooled x fastest.
+constexpr int kProposalAnchors = 9;  // ratios {0.5, 1, 2} x scales {8, 16, 32}
+constexpr int kMaskChunk = 1024;     // columns of the mask staged per pass
+
+struct ProposalGeom {
+    int A, H, W, P;  // anchors, feature map, A * H * W
+    float stride, min_size;
+    float ax1[kProposalAnchors], ay1[kProposalAnchors], aw[kProposalAnchors], ah[kProposalAnchors];
+};
+
+struct ProposalWorkspace {
+    float* boxes;     // (batch, P, 4) clipped boxes
+    uint32_t* keys;   // (batch, P4) orderable score, 0 = not a candidate
+    float* sel_box;   // (batch, K, 4)
+    float* sel_area;  // (batch, K4)
+    int* sel_idx;     // (batch, K4)
+    int* counts;      // (batch4)
+    uint32_t* mask;   // (batch, K, words)
+    int P4, K, K4, words;
+};
+
+size_t round4(size_t v) { return round_up_sz(v, 4); }
+
+ProposalWorkspace proposal_carve(float* ws, int P, int K, int batch) {
+    ProposalWorkspace w;
+    const size_t n = static_cast<size_t>(batch);
+    w.P4 = static_cast<int>(round4(P));
+    w.K = K;
+    w.K4 = static_cast<int>(round4(K));
+    w.words = ceil_div(K, 32);
+    w.boxes = ws;
+    ws += n * P * 4;
+    w.keys = reinterpret_cast<uint32_t*>(ws);
+    ws += n * w.P4;
+    w.sel_box = ws;
+    ws += n * K * 4;
+    w.sel_area = ws;
+    ws += n * w.K4;
+    w.sel_idx = reinterpret_cast<int*>(ws);
+    ws += n * w.K4;
+    w.counts = reinterpret_cast<int*>(ws);
+    ws += round4(n);
+    w.mask = reinterpret_cast<uint32_t*>(ws);
+    return w;
+}
+
+// boxes: (batch, P, 4); keys: (batch, key_stride) or null (decode alone)
+__global__ void __launch_bounds__(256)
+proposal_decode_kernel(float4* __restrict__ boxes, uint32_t* __restrict__ keys, int key_stride,
+                       const float* __restrict__ score, const float* __restrict__ bbox, const float* __restrict__ im_info,
+                       const ProposalGeom g, long long total) {
+    const int hw = g.H * g.W;
+    for (long long t = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x; t < total;
+         t += static_cast<long long>(gridDim.x) * blockDim.x) {
+        const long long n = t / g.P;
+        const int i = static_cast<int>(t - n * g.P);
+        const int q = i / hw, cell = i - q * hw;
+        const int y = cell / g.W, x = cell - y * g.W;
+        const float* d = bbox + (static_cast<size_t>(n) * 4 * g.A + 4 * q) * hw + cell;
+        const float dx = d[0], dy = d[static_cast<size_t>(hw)], dw = d[2 * static_cast<size_t>(hw)];
+        const float dh = d[3 * static_cast<size_t>(hw)];
+        const float aw = g.aw[q], ah = g.ah[q];
+        const float ax = __fadd_rn(g.ax1[q], __fmul_rn(static_cast<float>(x), g.stride));
+        const float ay = __fadd_rn(g.ay1[q], __fmul_rn(static_cast<float>(y), g.stride));
+        const float pcx = __fadd_rn(__fadd_rn(ax, __fmul_rn(aw, 0.5f)), __fmul_rn(aw, dx));
+        const float pcy = __fadd_rn(__fadd_rn(ay, __fmul_rn(ah, 0.5f)), __fmul_rn(ah, dy));
+        const float pw = __fmul_rn(aw, expf(dw)), ph = __fmul_rn(ah, expf(dh));
+        const float* info = im_info + static_cast<size_t>(n) * 3;
+        const float xmax = __fsub_rn(info[1], 1.f), ymax = __fsub_rn(info[0], 1.f);
+        float4 b;
+        b.x = fmaxf(fminf(__fsub_rn(pcx, __fmul_rn(pw, 0.5f)), xmax), 0.f);
+        b.y = fmaxf(fminf(__fsub_rn(pcy, __fmul_rn(ph, 0.5f)), ymax), 0.f);
+        b.z = fmaxf(fminf(__fadd_rn(pcx, __fmul_rn(pw, 0.5f)), xmax), 0.f);
+        b.w = fmaxf(fminf(__fadd_rn(pcy, __fmul_rn(ph, 0.5f)), ymax), 0.f);
+        boxes[t] = b;
+        if (keys) {
+            const float s = score[(static_cast<size_t>(n) * 2 * g.A + g.A + q) * hw + cell];
+            const float thr = __fmul_rn(g.min_size, info[2]);
+            const bool ok = !isnan(s) && __fadd_rn(__fsub_rn(b.z, b.x), 1.f) >= thr &&
+                            __fadd_rn(__fsub_rn(b.w, b.y), 1.f) >= thr;
+            keys[static_cast<size_t>(n) * key_stride + i] = ok ? orderable(s) : 0u;  // a non-NaN image is never 0
+        }
+    }
+}
+
+__device__ __forceinline__ float area_plus_one(float4 b) {
+    return __fmul_rn(__fadd_rn(__fsub_rn(b.z, b.x), 1.f), __fadd_rn(__fsub_rn(b.w, b.y), 1.f));
+}
+
+__global__ void __launch_bounds__(kDetThreads)
+proposal_select_kernel(const ProposalWorkspace w, int P) {
+    extern __shared__ unsigned long long proposal_keys[];
+    __shared__ SelectScratch sm;
+    const int n = blockIdx.x;
+    const uint32_t* ku = w.keys + static_cast<size_t>(n) * w.P4;
+    const int m = select_top_k(P, w.K, [&](int i, uint32_t& u) {
+        u = ku[i];
+        return u != 0u;
+    }, proposal_keys, sm);
+    const float4* ib = reinterpret_cast<const float4*>(w.boxes) + static_cast<size_t>(n) * P;
+    float4* ob = reinterpret_cast<float4*>(w.sel_box) + static_cast<size_t>(n) * w.K;
+    for (int j = threadIdx.x; j < m; j += kDetThreads) {
+        const int idx = key_index(proposal_keys[j]);
+        const float4 b = ib[idx];
+        ob[j] = b;
+        w.sel_area[static_cast<size_t>(n) * w.K4 + j] = area_plus_one(b);
+        w.sel_idx[static_cast<size_t>(n) * w.K4 + j] = idx;
+    }
+    if (threadIdx.x == 0) w.counts[n] = m;
+}
+
+// 8 warps x 4 rows; every row's words from its own word on, a chunk of 32 words (1024 columns) per staging pass
+__global__ void __launch_bounds__(256)
+proposal_mask_kernel(const ProposalWorkspace w, float nms_thr) {
+    __shared__ float4 sb[kMaskChunk];
+    __shared__ float sa[kMaskChunk];
+    const int n = blockIdx.y, row0 = blockIdx.x * 32;
+    const int m = w.counts[n];
+    if (row0 >= m) return;
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const int words = (m + 31) >> 5;
+    const float4* gb = reinterpret_cast<const float4*>(w.sel_box) + static_cast<size_t>(n) * w.K;
+    const float* ga = w.sel_area + static_cast<size_t>(n) * w.K4;
+    float rb[4][4], ra[4];
+#pragma unroll
+    for (int r = 0; r < 4; ++r) {
+        const int i = min(row0 + warp + 8 * r, m - 1);
+        const float4 b = gb[i];
+        rb[r][0] = b.x;
+        rb[r][1] = b.y;
+        rb[r][2] = b.z;
+        rb[r][3] = b.w;
+        ra[r] = ga[i];
+    }
+    uint32_t* out = w.mask + static_cast<size_t>(n) * w.K * w.words;
+    for (int c0 = row0; c0 < m; c0 += kMaskChunk) {  // row0 is a multiple of 32: chunks start on a word
+        const int cn = min(kMaskChunk, m - c0);
+        __syncthreads();
+        for (int j = threadIdx.x; j < cn; j += blockDim.x) {
+            sb[j] = gb[c0 + j];
+            sa[j] = ga[c0 + j];
+        }
+        __syncthreads();
+        const int w0 = c0 >> 5, nw = min(32, words - w0);
+#pragma unroll
+        for (int r = 0; r < 4; ++r) {
+            const int i = row0 + warp + 8 * r;
+            if (i >= m) break;  // uniform over the warp
+            uint32_t mine = 0;
+            for (int k = 0; k < nw; ++k) {
+                const int j = c0 + 32 * k + lane;
+                if (c0 + 32 * k + 31 <= i) continue;  // the whole word is at or before row i: never read
+                const bool hit = j > i && j < m &&
+                                 box_iou<true>(rb[r], ra[r], reinterpret_cast<const float*>(&sb[j - c0]), sa[j - c0]) >
+                                     nms_thr;
+                const uint32_t bits = __ballot_sync(0xffffffffu, hit);
+                if (lane == k) mine = bits;
+            }
+            if (lane < nw && w0 + lane >= (i >> 5)) out[static_cast<size_t>(i) * w.words + w0 + lane] = mine;
+        }
+    }
+}
+
+// rois: (batch, post, 4); scores: (batch, post) or null
+__global__ void __launch_bounds__(32)
+proposal_sweep_kernel(float4* __restrict__ rois, float* __restrict__ scores, const float* __restrict__ score,
+                      const ProposalWorkspace w, int A, int hw, int post) {
+    __shared__ uint32_t removed[kProposalMaxTopK / 32];
+    const int n = blockIdx.x, lane = threadIdx.x;
+    const int m = w.counts[n];
+    const int words = (m + 31) >> 5;
+    for (int v = lane; v < words; v += 32) removed[v] = 0u;
+    __syncwarp();
+    const float4* sel = reinterpret_cast<const float4*>(w.sel_box) + static_cast<size_t>(n) * w.K;
+    const int* sel_idx = w.sel_idx + static_cast<size_t>(n) * w.K4;
+    const uint32_t* mask = w.mask + static_cast<size_t>(n) * w.K * w.words;
+    const float* fg = score + (static_cast<size_t>(n) * 2 * A + A) * hw;
+    float4* orow = rois + static_cast<size_t>(n) * post;
+    float* srow = scores ? scores + static_cast<size_t>(n) * post : nullptr;
+    int kept = 0;
+    for (int wd = 0; wd < words && kept < post; ++wd) {
+        const uint32_t valid = (wd == words - 1 && (m & 31)) ? (1u << (m & 31)) - 1u : 0xffffffffu;
+        uint32_t live = ~removed[wd] & valid;
+        while (live && kept < post) {  // uniform: every lane reads the same words
+            const int b = __ffs(live) - 1, i = (wd << 5) + b;
+            if (lane == 0) {
+                orow[kept] = sel[i];
+                if (srow) srow[kept] = fg[sel_idx[i]];
+            }
+            ++kept;
+            const uint32_t* row = mask + static_cast<size_t>(i) * w.words;
+            for (int v = wd + lane; v < words; v += 32) removed[v] |= row[v];
+            __syncwarp();
+            live = ~removed[wd] & valid & (b == 31 ? 0u : 0xffffffffu << (b + 1));
+        }
+    }
+    for (int r = kept + lane; r < post; r += 32) {
+        orow[r] = make_float4(0.f, 0.f, 0.f, 0.f);
+        if (srow) srow[r] = -1.f;
+    }
+}
+
+__global__ void __launch_bounds__(256)
+roi_pool_kernel(float* __restrict__ out, const float* __restrict__ in, const float* __restrict__ rois, int C, int H,
+                int W, int R, int PH, int PW, float scale, long long total) {
+    for (long long t = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x; t < total;
+         t += static_cast<long long>(gridDim.x) * blockDim.x) {
+        long long r = t;
+        const int pw = static_cast<int>(r % PW);
+        r /= PW;
+        const int ph = static_cast<int>(r % PH);
+        r /= PH;
+        const int c = static_cast<int>(r % C);
+        const long long item = r / C, n = item / R;
+        const float* roi = rois + item * 4;
+        // (int)roundf: half away from zero, converted saturating (a NaN corner reads as 0)
+        const long long x1 = static_cast<int>(roundf(__fmul_rn(roi[0], scale)));
+        const long long y1 = static_cast<int>(roundf(__fmul_rn(roi[1], scale)));
+        const long long x2 = static_cast<int>(roundf(__fmul_rn(roi[2], scale)));
+        const long long y2 = static_cast<int>(roundf(__fmul_rn(roi[3], scale)));
+        const long long rw = max(x2 - x1 + 1, 1ll), rh = max(y2 - y1 + 1, 1ll);
+        const float bin_w = __fdiv_rn(static_cast<float>(rw), static_cast<float>(PW));
+        const float bin_h = __fdiv_rn(static_cast<float>(rh), static_cast<float>(PH));
+        const long long ws = min(max(static_cast<long long>(floorf(__fmul_rn(static_cast<float>(pw), bin_w))) + x1, 0ll),
+                                 static_cast<long long>(W));
+        const long long we = min(max(static_cast<long long>(ceilf(__fmul_rn(static_cast<float>(pw + 1), bin_w))) + x1, 0ll),
+                                 static_cast<long long>(W));
+        const long long hs = min(max(static_cast<long long>(floorf(__fmul_rn(static_cast<float>(ph), bin_h))) + y1, 0ll),
+                                 static_cast<long long>(H));
+        const long long he = min(max(static_cast<long long>(ceilf(__fmul_rn(static_cast<float>(ph + 1), bin_h))) + y1, 0ll),
+                                 static_cast<long long>(H));
+        float v = 0.f;
+        if (we > ws && he > hs) {
+            const float* plane = in + (static_cast<size_t>(n) * C + c) * H * W;
+            v = -FLT_MAX;
+            for (long long h = hs; h < he; ++h)
+                for (long long x = ws; x < we; ++x) v = fmaxf(v, __ldg(plane + h * W + x));
+        }
+        out[t] = v;
+    }
+}
+
+ProposalGeom proposal_geom(const FcudaProposalParam& p, int feat_h, int feat_w) {
+    ProposalGeom g{};
+    g.A = kProposalAnchors;
+    g.H = feat_h;
+    g.W = feat_w;
+    g.P = kProposalAnchors * feat_h * feat_w;
+    g.stride = static_cast<float>(p.feat_stride);
+    g.min_size = static_cast<float>(p.min_size);
+    float table[kProposalAnchors * 4];
+    proposal_anchors(p, table);
+    for (int q = 0; q < kProposalAnchors; ++q) {
+        g.ax1[q] = table[4 * q];
+        g.ay1[q] = table[4 * q + 1];
+        g.aw[q] = table[4 * q + 2];
+        g.ah[q] = table[4 * q + 3];
+    }
+    return g;
+}
+
+int proposal_decode_launch(float* boxes, uint32_t* keys, int key_stride, const float* score, const float* bbox,
+                           const float* im_info, const ProposalGeom& g, int batch, cudaStream_t s) {
+    const long long total = static_cast<long long>(batch) * g.P;
+    const int prof = prof_begin(s, PROF_RCNN, 0, 0, (keys ? 40.0 : 36.0) * total);
+    const long long blocks = (total + 255) / 256;
+    proposal_decode_kernel<<<static_cast<unsigned>(blocks < 65536 * 16 ? blocks : 65536 * 16), 256, 0, s>>>(
+        reinterpret_cast<float4*>(boxes), keys, key_stride, score, bbox, im_info, g, total);
+    FCUDA_CHECK_LAUNCH();
+    prof_end(prof, s);
+    count_launch();
+    return 0;
+}
+
+SmemAttrCache proposal_select_smem;
+
+}  // namespace
+
+void proposal_anchors(const FcudaProposalParam& p, float* table) {
+    const float ratios[3] = {0.5f, 1.f, 2.f}, scales[3] = {8.f, 16.f, 32.f};
+    const float base = static_cast<float>(p.base_size);
+    for (int r = 0; r < 3; ++r) {
+        const float rw = roundf(base / sqrtf(ratios[r]));
+        const float rh = roundf(rw * ratios[r]);
+        for (int k = 0; k < 3; ++k) {
+            const float aw = rw * scales[k], ah = rh * scales[k];
+            float* a = table + 4 * (r * 3 + k);
+            a[0] = base * 0.5f - aw * 0.5f;
+            a[1] = base * 0.5f - ah * 0.5f;
+            a[2] = aw;
+            a[3] = ah;
+        }
+    }
+}
+
+int proposal_decode(float* boxes, const float* score, const float* bbox, const float* im_info, const FcudaProposalParam& p,
+                    int feat_h, int feat_w, int batch, cudaStream_t s) {
+    return proposal_decode_launch(boxes, nullptr, 0, score, bbox, im_info, proposal_geom(p, feat_h, feat_w), batch, s);
+}
+
+size_t proposal_workspace(const FcudaProposalParam& p, int feat_h, int feat_w, int batch) {
+    const size_t P = static_cast<size_t>(kProposalAnchors) * feat_h * feat_w, K = static_cast<size_t>(p.pre_nms_topN);
+    const size_t n = static_cast<size_t>(batch);
+    return n * (4 * P + round4(P) + 4 * K + 2 * round4(K) + K * ceil_div_sz(K, 32)) + round4(n);
+}
+
+int proposal_forward(float* rois, float* scores, const float* score, const float* bbox, const float* im_info,
+                     const FcudaProposalParam& p, int feat_h, int feat_w, float* workspace, int batch, cudaStream_t s) {
+    const ProposalGeom g = proposal_geom(p, feat_h, feat_w);
+    const ProposalWorkspace w = proposal_carve(workspace, g.P, p.pre_nms_topN, batch);
+    int rc = proposal_decode_launch(w.boxes, w.keys, w.P4, score, bbox, im_info, g, batch, s);
+    if (rc) return rc;
+    const double n = batch, K = p.pre_nms_topN;
+    int len = 1;
+    while (len < p.pre_nms_topN) len <<= 1;
+    const int smem = len * static_cast<int>(sizeof(unsigned long long));
+    rc = ensure_dynamic_smem(proposal_select_kernel, smem, proposal_select_smem);
+    if (rc) return rc;
+    int prof = prof_begin(s, PROF_RCNN, 0, 0, n * (4.0 * g.P + 40.0 * K));
+    proposal_select_kernel<<<static_cast<unsigned>(batch), kDetThreads, smem, s>>>(w, g.P);
+    FCUDA_CHECK_LAUNCH();
+    prof_end(prof, s);
+    count_launch();
+    prof = prof_begin(s, PROF_RCNN, 0, 0, n * (20.0 * K + 2.0 * K * w.words));
+    proposal_mask_kernel<<<dim3(static_cast<unsigned>(ceil_div(p.pre_nms_topN, 32)), static_cast<unsigned>(batch)), 256, 0,
+                           s>>>(w, p.nms_thresh);
+    FCUDA_CHECK_LAUNCH();
+    prof_end(prof, s);
+    count_launch();
+    prof = prof_begin(s, PROF_RCNN, 0, 0, n * p.after_nms_topN * (20.0 + 4.0 * w.words));
+    proposal_sweep_kernel<<<static_cast<unsigned>(batch), 32, 0, s>>>(reinterpret_cast<float4*>(rois), scores, score, w,
+                                                                      g.A, feat_h * feat_w, p.after_nms_topN);
+    FCUDA_CHECK_LAUNCH();
+    prof_end(prof, s);
+    count_launch();
+    return 0;
+}
+
+int roi_pooling_forward(float* out, const float* in, const float* rois, int C, int H, int W, int R, int pooled_h,
+                        int pooled_w, float spatial_scale, int batch, cudaStream_t s) {
+    const long long total = static_cast<long long>(batch) * R * C * pooled_h * pooled_w;
+    const int prof = prof_begin(s, PROF_RCNN, 0, 0, 4.0 * batch * C * H * W + 16.0 * batch * R + 4.0 * total);
+    const long long blocks = (total + 255) / 256;
+    roi_pool_kernel<<<static_cast<unsigned>(blocks < 65536 * 16 ? blocks : 65536 * 16), 256, 0, s>>>(
+        out, in, rois, C, H, W, R, pooled_h, pooled_w, spatial_scale, total);
     FCUDA_CHECK_LAUNCH();
     prof_end(prof, s);
     count_launch();

@@ -27,4 +27,16 @@ size_t yolo_detection_workspace(int slots, int batch);
 // decode, select, suppression mask, sweep: four launches.
 int yolo_detection(float* out, const float* const* inputs, const FcudaYoloParam& p, float* workspace, int batch,
                    cudaStream_t s);
+// Faster R-CNN (include/fcuda.h, FcudaProposalParam); the parameters are checked by the caller.  The 9 anchors of p as
+// (x1, y1, w, h) rows, host only.
+void proposal_anchors(const FcudaProposalParam& p, float* table);
+int proposal_decode(float* boxes, const float* score, const float* bbox, const float* im_info, const FcudaProposalParam& p,
+                    int feat_h, int feat_w, int batch, cudaStream_t s);
+// Workspace (floats) of proposal_forward.
+size_t proposal_workspace(const FcudaProposalParam& p, int feat_h, int feat_w, int batch);
+// decode, select, suppression mask, sweep: four launches.
+int proposal_forward(float* rois, float* scores, const float* score, const float* bbox, const float* im_info,
+                     const FcudaProposalParam& p, int feat_h, int feat_w, float* workspace, int batch, cudaStream_t s);
+int roi_pooling_forward(float* out, const float* in, const float* rois, int channels, int height, int width, int num_rois,
+                        int pooled_h, int pooled_w, float spatial_scale, int batch, cudaStream_t s);
 }  // namespace fcuda

@@ -988,6 +988,59 @@ int fcuda_yolo_detection_forward(float* output, const float* const* inputs, cons
     return yolo_detection(output, inputs, *param, workspace, batch, as_stream(stream));
 }
 
+static int proposal_limits(const FcudaProposalParam* p, int feat_h, int feat_w, int batch) {
+    if (!p) return -100;
+    if (p->feat_stride < 1 || p->base_size < 1 || p->pre_nms_topN < 1 || p->pre_nms_topN > 8192 || p->after_nms_topN < 1 ||
+        p->after_nms_topN > 8192 || isnan(p->nms_thresh))
+        return -200;
+    if (batch < 1 || feat_h < 1 || feat_w < 1) return -100;
+    if (batch > 65535 || feat_h >= kMaxPriors || feat_w >= kMaxPriors ||
+        static_cast<long long>(FCUDA_PROPOSAL_ANCHORS) * feat_h * feat_w >= kMaxPriors)
+        return -200;
+    return 0;
+}
+
+int fcuda_proposal_anchors(const FcudaProposalParam* param, float* table) {
+    const int rc = proposal_limits(param, 1, 1, 1);
+    if (rc) return rc;
+    if (!table) return -100;
+    proposal_anchors(*param, table);
+    return 0;
+}
+
+int fcuda_proposal_decode(float* boxes, const float* score, const float* bbox, const float* im_info,
+                          const FcudaProposalParam* param, int feat_h, int feat_w, int batch, void* stream) {
+    const int rc = proposal_limits(param, feat_h, feat_w, batch);
+    if (rc) return rc;
+    if (!boxes || !score || !bbox || !im_info) return -100;
+    return proposal_decode(boxes, score, bbox, im_info, *param, feat_h, feat_w, batch, as_stream(stream));
+}
+
+int fcuda_proposal_workspace_size(const FcudaProposalParam* param, int feat_h, int feat_w, int batch, size_t* floats) {
+    if (!floats) return -100;
+    const int rc = proposal_limits(param, feat_h, feat_w, batch);
+    if (rc) return rc;
+    *floats = proposal_workspace(*param, feat_h, feat_w, batch);
+    return 0;
+}
+
+int fcuda_proposal_forward(float* rois, float* scores, const float* score, const float* bbox, const float* im_info,
+                           const FcudaProposalParam* param, int feat_h, int feat_w, float* workspace, int batch,
+                           void* stream) {
+    const int rc = proposal_limits(param, feat_h, feat_w, batch);
+    if (rc) return rc;
+    if (!rois || !score || !bbox || !im_info || !workspace || (reinterpret_cast<uintptr_t>(workspace) & 15)) return -100;
+    return proposal_forward(rois, scores, score, bbox, im_info, *param, feat_h, feat_w, workspace, batch, as_stream(stream));
+}
+
+int fcuda_roi_pooling_forward(float* output, const float* input, const float* rois, int channels, int height, int width,
+                              int num_rois, int pooled_h, int pooled_w, float spatial_scale, int batch, void* stream) {
+    if (pooled_h < 1 || pooled_w < 1 || !isfinite(spatial_scale) || !(spatial_scale > 0.f)) return -200;
+    if (!output || !input || !rois || channels < 1 || height < 1 || width < 1 || num_rois < 1 || batch < 1) return -100;
+    return roi_pooling_forward(output, input, rois, channels, height, width, num_rois, pooled_h, pooled_w, spatial_scale,
+                               batch, as_stream(stream));
+}
+
 static const long long kRouteMaxPositions = 1ll << 31;  // positions of the concatenated axis fit an int
 
 int fcuda_route_forward(const FcudaRoute* route, int batch, void* stream) {

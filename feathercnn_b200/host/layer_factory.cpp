@@ -1,7 +1,8 @@
 // Built-in layer registrations: the 13 ncnn type names the reference serves (/root/reference/src/layer_factory.cpp:53-68)
 // plus Deconvolution / DeconvolutionDepthWise, Interp, Crop, Clip, PReLU, SSD's Permute, Flatten, Reshape, PriorBox and
 // DetectionOutput, VGG-SSD's Normalize, YOLO's YoloDetectionOutput and Yolov3DetectionOutput, ShuffleNet's ShuffleChannel
-// and Slice, and AlexNet's and GoogLeNet's LRN, 30 in all, mapped onto this host's layer classes.  A table of {type name,
+// and Slice, AlexNet's and GoogLeNet's LRN, and Faster R-CNN's Proposal and ROIPooling, 32 in all, mapped onto this
+// host's layer classes.  A table of {type name,
 // factory} pairs instead of one macro line per layer; the
 // DEFINE_LAYER_CREATOR / REGISTER_LAYER_CREATOR macros of <feather/layer_factory.h> remain the plugin API for user layers.
 #include <feather/layer_factory.h>
@@ -19,6 +20,7 @@
 #include "layers/misc_layers.h"
 #include "layers/normalize_layer.h"
 #include "layers/pooling_layer.h"
+#include "layers/rcnn_layers.h"
 #include "layers/relu_layer.h"
 #include "layers/resize_layers.h"
 #include "layers/route_layers.h"
@@ -73,6 +75,8 @@ const BuiltIn kBuiltIns[] = {
     {"ShuffleChannel", make_layer<ShuffleChannelLayer>},
     {"Slice", make_layer<SliceLayer>},
     {"LRN", make_layer<LRNLayer>},
+    {"Proposal", make_layer<ProposalLayer>},
+    {"ROIPooling", make_layer<ROIPoolingLayer>},
 };
 
 }  // namespace

@@ -8,7 +8,8 @@ models of the architectures BASELINE.json names: a single 3x3 conv, VGG-16, ResN
 BN + Scale + ReLU as separate layers, Split/Eltwise residuals), MobileNet-v1, MobileNet-v2 (ReLU6 as Clip), GoogLeNet and
 AlexNet (BVLC's deploy nets, with LRN), plus a small "mini" net
 that exercises every layer type, single-shot detectors (MobileNet-SSD, VGG-SSD 300, a two-head tiny SSD), YOLO detectors
-(MobileNet-YOLOv2, MobileNet-v2 YOLOv3, a two-scale tiny YOLOv3) and ShuffleNet-v2 with a small routing probe net.  Weight statistics follow
+(MobileNet-YOLOv2, MobileNet-v2 YOLOv3, a two-scale tiny YOLOv3), two-stage detectors (py-faster-rcnn's VGG-16 Faster
+R-CNN and a tiny one) and ShuffleNet-v2 with a small routing probe net.  Weight statistics follow
 SURVEY.md §8(d).
 """
 from __future__ import annotations
@@ -392,6 +393,32 @@ class ModelWriter:
         self._layer(type_, name, bottoms, [top], params)
         self.shape[top] = (1, keep_top_k or 1024, 6)
         self.rank[top] = 2
+        return top
+
+    def extra_input(self, name, c=1, h=1, w=3):
+        """A further Input after the first (input() starts a new net): Faster R-CNN's im_info, 3 values per image."""
+        self._layer("Input", name, [], [name], {0: w, 1: h, 2: c})
+        self.shape[name] = (c, h, w)
+        return name
+
+    def proposal(self, name, score, bbox, im_info, feat_stride=16, base_size=16, pre_nms_top_n=6000, post_nms_top_n=300,
+                 nms_thresh=0.7, min_size=16, tops=None):
+        """ncnn Proposal, every key written: rois (post_nms_top_n, 1, 4) per image and, with a second top, scores
+        (post_nms_top_n, 1, 1).  Returns the rois top."""
+        tops = tops or [name]
+        self._layer("Proposal", name, [score, bbox, im_info], tops,
+                    {0: feat_stride, 1: base_size, 2: pre_nms_top_n, 3: post_nms_top_n, 4: f"{nms_thresh:e}", 5: min_size})
+        self.shape[tops[0]] = (post_nms_top_n, 1, 4)
+        if len(tops) > 1:
+            self.shape[tops[1]] = (post_nms_top_n, 1, 1)
+        return tops[0]
+
+    def roi_pooling(self, name, bottom, rois, pooled_w=7, pooled_h=7, spatial_scale=0.0625, top=None):
+        """ncnn ROIPooling 0=pooled_w 1=pooled_h 2=spatial_scale.  The top has one item per RoI of every image; its shape
+        here is one item's (C, pooled_h, pooled_w)."""
+        top = top or name
+        self._layer("ROIPooling", name, [bottom, rois], [top], {0: pooled_w, 1: pooled_h, 2: f"{spatial_scale:e}"})
+        self.shape[top] = (self.shape[bottom][0], pooled_h, pooled_w)
         return top
 
     def dropout(self, name, bottom, top=None, scale=None):
@@ -1104,13 +1131,72 @@ def yolo_tiny(seed=0, size=64, num_classes=5, confidence_threshold=0.05, head_ga
     return m
 
 
+def _faster_rcnn_head(m: ModelWriter, feat: str, num_classes: int, rpn_width: int, fc_width: int, feat_stride: int,
+                      base_size: int, pre_nms_top_n: int, post_nms_top_n: int, min_size: int, pooled: int,
+                      rpn_cls_gain: float, rpn_bbox_gain: float):
+    """py-faster-rcnn's test net after the backbone: rpn_conv/3x3 + ReLU; rpn_cls_score (2 x 9) and rpn_bbox_pred (4 x 9)
+    1x1 convolutions; Reshape (2, -1, W) -> Softmax over the channel axis -> Reshape (18, -1, W); Proposal; ROIPooling
+    pooled x pooled at 1 / feat_stride; fc6 and fc7 (ReLU, Dropout); cls_score -> Softmax (cls_prob) and bbox_pred.  The
+    RPN gains multiply He init: rpn_cls_gain spreads the objectness logits, rpn_bbox_gain keeps the box deltas small so
+    the boxes stay finite and neighbouring anchors overlap."""
+    fan_in = rpn_width
+    x = m.relu("rpn_relu/3x3", m.conv("rpn_conv/3x3", feat, rpn_width, 3, 1, 1, True))
+    cls = m.conv("rpn_cls_score", x, 18, 1, 1, 0, True, gain=rpn_cls_gain * np.sqrt(2.0 / fan_in))
+    bbox = m.conv("rpn_bbox_pred", x, 36, 1, 1, 0, True, gain=rpn_bbox_gain * np.sqrt(2.0 / fan_in),
+                  bias_values=np.zeros(36, np.float32))
+    cls = m.reshape("rpn_cls_score_reshape", cls, 0, -1, 2)
+    cls = m.softmax("rpn_cls_prob", cls, axis=0)
+    cls = m.reshape("rpn_cls_prob_reshape", cls, 0, -1, 18)
+    rois = m.proposal("proposal", cls, bbox, "im_info", feat_stride, base_size, pre_nms_top_n, post_nms_top_n, 0.7,
+                      min_size, tops=["rois"])
+    x = m.roi_pooling("roi_pool5", feat, rois, pooled, pooled, 1.0 / feat_stride, top="pool5")
+    x = m.dropout("drop6", m.relu("relu6", m.fc("fc6", x, fc_width)))
+    x = m.dropout("drop7", m.relu("relu7", m.fc("fc7", x, fc_width)))
+    m.softmax("cls_prob", m.fc("cls_score", x, num_classes))
+    m.fc("bbox_pred", x, 4 * num_classes)
+
+
+def faster_rcnn_vgg16(seed=0, height=600, width=800, num_classes=21, pre_nms_top_n=6000, post_nms_top_n=300,
+                      rpn_cls_gain=1.0, rpn_bbox_gain=0.1) -> ModelWriter:
+    """py-faster-rcnn's VGG-16 Faster R-CNN test net: Input data (3, height, width) and Input im_info (3 values per image:
+    height, width, scale), VGG-16 conv1_1 .. conv5_3 with ReLU and the four 2x2 / 2 pools (conv5_3 at 1 / 16: 38 x 50 at
+    600 x 800, 17,100 anchors), then _faster_rcnn_head: RPN 512 wide, Proposal 16 / 16 / pre_nms_top_n / post_nms_top_n /
+    0.7 / 16, ROIPooling 7 x 7, fc6 25088 -> 4096, fc7 4096, cls_score num_classes and bbox_pred 4 x num_classes.  fc6
+    to bbox_pred run once over batch x post_nms_top_n RoIs."""
+    m = ModelWriter(seed)
+    x = m.input("data", 3, height, width)
+    m.extra_input("im_info")
+    for si, (ch, n) in enumerate([(64, 2), (128, 2), (256, 3), (512, 3), (512, 3)], 1):
+        for li in range(1, n + 1):
+            x = m.relu(f"relu{si}_{li}", m.conv(f"conv{si}_{li}", x, ch, 3, 1, 1, True))
+        if si < 5:
+            x = m.pool(f"pool{si}", x, 0, 2, 2)
+    _faster_rcnn_head(m, x, num_classes, 512, 4096, 16, 16, pre_nms_top_n, post_nms_top_n, 16, 7, rpn_cls_gain,
+                      rpn_bbox_gain)
+    return m
+
+
+def faster_rcnn_tiny(seed=0, height=96, width=128, num_classes=5, pre_nms_top_n=2000, post_nms_top_n=64,
+                     rpn_cls_gain=1.0, rpn_bbox_gain=0.1) -> ModelWriter:
+    """Faster R-CNN at float64-checkable size: two 3x3 / 2 convolutions (16, 32 channels, ReLU) to a 1 / 4 map (24 x 32 at
+    96 x 128: 6,912 anchors), then _faster_rcnn_head with RPN width 32, Proposal feat_stride 4, base_size 2 (anchors 24 to
+    96 pixels wide), min_size 4, ROIPooling 4 x 4 at 1 / 4, fc6 / fc7 64 wide."""
+    m = ModelWriter(seed)
+    x = m.input("data", 3, height, width)
+    m.extra_input("im_info")
+    x = m.relu("relu1", m.conv("conv1", x, 16, 3, 2, 1, True))
+    x = m.relu("relu2", m.conv("conv2", x, 32, 3, 2, 1, True))
+    _faster_rcnn_head(m, x, num_classes, 32, 64, 4, 2, pre_nms_top_n, post_nms_top_n, 4, 4, rpn_cls_gain, rpn_bbox_gain)
+    return m
+
+
 ZOO = {"single_conv": single_conv, "vgg16": vgg16, "resnet50": resnet50, "mobilenet_v1": mobilenet_v1, "mini": mini,
        "decoder_tiny": decoder_tiny, "fcn8s_tiny": fcn8s_tiny, "deeplab_head_tiny": deeplab_head_tiny,
        "mobilenet_v2": mobilenet_v2, "prelu_tiny": prelu_tiny, "mobilenet_ssd": mobilenet_ssd, "ssd_tiny": ssd_tiny,
        "vgg_ssd": vgg_ssd, "googlenet": googlenet, "alexnet": alexnet,
        "mobilenet_yolov2": mobilenet_yolov2, "mobilenetv2_yolov3": mobilenetv2_yolov3, "yolo_tiny": yolo_tiny,
        "shufflenet_v2": shufflenet_v2, "shuffle_tiny": shuffle_tiny, "deeplabv3_mobilenet_v2": deeplabv3_mobilenet_v2,
-       "deeplabv3_tiny": deeplabv3_tiny}
+       "deeplabv3_tiny": deeplabv3_tiny, "faster_rcnn_vgg16": faster_rcnn_vgg16, "faster_rcnn_tiny": faster_rcnn_tiny}
 
 
 def synthetic_input(shape, index: int = 0) -> np.ndarray:

@@ -504,6 +504,62 @@ int fcuda_yolo_detection_workspace_size(const FcudaYoloParam* param, int batch, 
 int fcuda_yolo_detection_forward(float* output, const float* const* inputs, const FcudaYoloParam* param, float* workspace,
                                  int batch, void* stream);
 
+/* ---- Faster R-CNN: Proposal and ROIPooling (the reference has neither layer) ---------------------------------------
+ * Stream-ordered like the detection calls above: nothing allocates, synchronises or copies to the host.
+ *
+ * Proposal (ncnn's layer, py-faster-rcnn's proposal_layer.py arithmetic) in fp32, every operation rounded on its own (no
+ * FMA).  A = 9 anchors, q = ratio * 3 + scale over ratios {0.5, 1, 2} and scales {8, 16, 32}:
+ *   rw = roundf(base_size / sqrtf(ratio)), rh = roundf(rw * ratio)       (half away from zero)
+ *   aw = rw * scale, ah = rh * scale, ax1 = base_size * 0.5 - aw * 0.5, ay1 = base_size * 0.5 - ah * 0.5
+ * With the defaults (ax1, ay1, ax1 + aw - 1, ay1 + ah - 1) is py-faster-rcnn's anchor table.
+ * Inputs, per image of `batch`: score (2A, H, W), the foreground score of anchor q at channel A + q; bbox (4A, H, W),
+ * channels 4q + {0: dx, 1: dy, 2: dw, 3: dh}; im_info 3 floats (height, width, scale).  Decode of anchor q at cell (y, x):
+ *   ax = ax1 + x * feat_stride, ay = ay1 + y * feat_stride
+ *   pcx = (ax + aw * 0.5) + aw * dx, pcy likewise, pw = aw * expf(dw), ph = ah * expf(dh)
+ *   box = (pcx - pw * 0.5, pcy - ph * 0.5, pcx + pw * 0.5, pcy + ph * 0.5), each x clipped as fmaxf(fminf(x, width - 1), 0)
+ *   and each y with height - 1.
+ * A box is a candidate iff x2 - x1 + 1 >= min_size * scale, y2 - y1 + 1 >= min_size * scale and its score is not NaN.
+ * The candidates are ordered by (score descending, index ascending), index = q * H * W + y * W + x (-0 and +0 are equal
+ * scores), and the first pre_nms_topN kept; then greedy NMS in that order: a candidate is kept iff no earlier kept box has
+ * IoU > nms_thresh, with the + 1 pixel convention:
+ *   iw = fmaxf((min(x2) - max(x1)) + 1, 0), ih likewise, inter = iw * ih, area = (x2 - x1 + 1) * (y2 - y1 + 1)
+ *   IoU = inter / ((area_a + area_b) - inter)                a NaN IoU suppresses nothing
+ * and it stops at after_nms_topN kept boxes.  rois: (batch, after_nms_topN, 4) rows [x1, y1, x2, y2] in kept order, then
+ * [0, 0, 0, 0]; scores (may be NULL): (batch, after_nms_topN), the kept boxes' score bits, then -1.
+ * Limits (else -200): feat_stride, base_size >= 1; 1 <= pre_nms_topN, after_nms_topN <= 8192; nms_thresh not NaN;
+ * A * H * W < 2^24; batch <= 65535.  -100: a NULL pointer, batch < 1, H or W < 1, or a workspace that is not 16-byte
+ * aligned (fcuda_proposal_forward). */
+#define FCUDA_PROPOSAL_ANCHORS 9
+typedef struct FcudaProposalParam {
+    int feat_stride, base_size;      /* ncnn 0= (16), 1= (16) */
+    int pre_nms_topN, after_nms_topN; /* 2= (6000), 3= (300) */
+    float nms_thresh;                 /* 4= (0.7) */
+    int min_size;                     /* 5= (16) */
+} FcudaProposalParam;
+/* The 9 anchors as (ax1, ay1, aw, ah) rows, anchor q at table[4q..4q+3]; host only, after the limits above. */
+int fcuda_proposal_anchors(const FcudaProposalParam* param, float* table);
+/* Decode alone: boxes (batch, A * H * W, 4), clipped, for every anchor and cell whether or not it is a candidate.  The
+ * boxes fcuda_proposal_forward uses are these bits. */
+int fcuda_proposal_decode(float* boxes, const float* score, const float* bbox, const float* im_info,
+                          const FcudaProposalParam* param, int feat_h, int feat_w, int batch, void* stream);
+/* Workspace in floats: with P = 9 * H * W, K = pre_nms_topN and r4(v) = v rounded up to a multiple of 4,
+ * batch * (4 P + r4(P) + 4 K + 2 r4(K) + K * ceil(K / 32)) + r4(batch). */
+int fcuda_proposal_workspace_size(const FcudaProposalParam* param, int feat_h, int feat_w, int batch, size_t* floats);
+int fcuda_proposal_forward(float* rois, float* scores, const float* score, const float* bbox, const float* im_info,
+                           const FcudaProposalParam* param, int feat_h, int feat_w, float* workspace, int batch,
+                           void* stream);
+
+/* ROIPooling (Caffe's and ncnn's arithmetic): input (batch, C, H, W), rois (batch, num_rois, 4) [x1, y1, x2, y2] in input
+ * pixels; output (batch * num_rois, C, pooled_h, pooled_w), RoI r of image n at item n * num_rois + r pooling image n.
+ *   x1 = (int)roundf(roi[0] * spatial_scale), likewise y1, x2, y2 (half away from zero, converted saturating)
+ *   roi_w = max(x2 - x1 + 1, 1), bin_w = (float)roi_w / pooled_w      (roi_h, bin_h likewise)
+ *   wstart = floorf(pw * bin_w) + x1, wend = ceilf((pw + 1) * bin_w) + x1, both clamped to [0, W]   (h likewise)
+ *   value = 0 for an empty bin, else the fmaxf over the bin from -FLT_MAX: bit-exact.
+ * Limits: -200 for pooled_w or pooled_h < 1 or spatial_scale not finite and > 0; -100 for a NULL pointer or a size < 1.
+ * Every RoI row is pooled, the [0, 0, 0, 0] padding of fcuda_proposal_forward included. */
+int fcuda_roi_pooling_forward(float* output, const float* input, const float* rois, int channels, int height, int width,
+                              int num_rois, int pooled_h, int pooled_w, float spatial_scale, int batch, void* stream);
+
 /* ---- Channel routing: ncnn's ShuffleChannel and Slice, and Concat -> ShuffleChannel -> Slice fused (the reference has
  * neither layer) ------------------------------------------------------------------------------------------------------
  * Every image of every blob is viewed as [outer][extent][inner].  The sources, concatenated along the middle axis, form
@@ -578,7 +634,7 @@ int fcuda_profile_collect(double* total_ms, double* algo_flops, double* mma_flop
  * kind 0 TensorGEMM, 1 implicit-GEMM conv, 2 Winograd input transform, 3 Winograd output transform, 4 pooling,
  * 5 depthwise, 6 element-wise (BN/Scale/Eltwise/Clip/PReLU/Normalize/LRN), 7 deconvolution scatter / depthwise gather, 8 resize / crop (Interp,
  * Crop), 9 detection (Permute, axis Softmax, PriorBox, decode, NMS, merge; YOLO decode, select, mask, sweep), 10 channel
- * routing (fcuda_route_forward), < 0 all.  algo_bytes = the bytes the operation must move (inputs
+ * routing (fcuda_route_forward), 11 two-stage detection (Proposal decode, select, mask, sweep; ROIPooling), < 0 all.  algo_bytes = the bytes the operation must move (inputs
  * read once + outputs written once). */
 int fcuda_profile_collect_kind(int kind, double* total_ms, double* algo_flops, double* mma_flops, double* algo_bytes,
                                long long* launches);
