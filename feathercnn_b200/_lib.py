@@ -135,6 +135,7 @@ def fcuda() -> ctypes.CDLL:
             "fcuda_proposal_workspace_size": (i, [PP, i, i, i, szp]),
             "fcuda_proposal_forward": (i, [vp, vp, vp, vp, vp, PP, i, i, vp, i, vp]),
             "fcuda_roi_pooling_forward": (i, [vp, vp, vp, i, i, i, i, i, i, f, i, vp]),
+            "fcuda_psroi_pooling_forward": (i, [vp, vp, vp, i, i, i, i, i, i, i, f, i, vp]),
             "fcuda_route_forward": (i, [ctypes.POINTER(FcudaRoute), i, vp]),
             "fcuda_slice_plan": (i, [i, i, ctypes.POINTER(i), ctypes.POINTER(i), i, ctypes.POINTER(i), ctypes.POINTER(i)]),
             "fcuda_interp_output_dim": (i, [R]),

@@ -687,9 +687,8 @@ def proposal(score: torch.Tensor, bbox: torch.Tensor, im_info: torch.Tensor, p: 
     return rois, scores
 
 
-def roi_pooling(x: torch.Tensor, rois: torch.Tensor, pooled_h: int = 7, pooled_w: int = 7,
-                spatial_scale: float = 0.0625) -> torch.Tensor:
-    """x (N, C, H, W), rois (N, R, 4) or (N, R, 1, 4) -> (N * R, C, pooled_h, pooled_w); RoI r of image n pools image n."""
+def _roi_inputs(x: torch.Tensor, rois: torch.Tensor):
+    """The bottoms as the C side reads them: float32 CUDA tensors, x (N, C, H, W) and rois (N, R, 4) or (N, R, 1, 4)."""
     x, rois = x.contiguous(), rois.contiguous()
     for t in (x, rois):
         assert t.is_cuda and t.dtype == torch.float32, (t.device, t.dtype)
@@ -698,8 +697,27 @@ def roi_pooling(x: torch.Tensor, rois: torch.Tensor, pooled_h: int = 7, pooled_w
     n, c, h, w = x.shape
     r = rois.shape[1]
     assert rois.numel() == 4 * n * r, tuple(rois.shape)
+    return x, rois, n, c, h, w, r
+
+
+def roi_pooling(x: torch.Tensor, rois: torch.Tensor, pooled_h: int = 7, pooled_w: int = 7,
+                spatial_scale: float = 0.0625) -> torch.Tensor:
+    """x (N, C, H, W), rois (N, R, 4) or (N, R, 1, 4) -> (N * R, C, pooled_h, pooled_w); RoI r of image n pools image n."""
+    x, rois, n, c, h, w, r = _roi_inputs(x, rois)
     out = torch.empty((n * r, c, pooled_h, pooled_w), device=x.device, dtype=torch.float32)
     _check("fcuda_roi_pooling_forward", fcuda().fcuda_roi_pooling_forward(_ptr(out), _ptr(x), _ptr(rois), c, h, w, r,
                                                                           pooled_h, pooled_w, float(spatial_scale), n,
                                                                           _stream()))
+    return out
+
+
+def psroi_pooling(x: torch.Tensor, rois: torch.Tensor, pooled_h: int = 7, pooled_w: int = 7, output_dim: int = 21,
+                  spatial_scale: float = 0.0625) -> torch.Tensor:
+    """R-FCN's position-sensitive RoI average pooling: x (N, output_dim * pooled_h * pooled_w, H, W), rois (N, R, 4) or
+    (N, R, 1, 4) -> (N * R, output_dim, pooled_h, pooled_w); RoI r of image n pools image n."""
+    x, rois, n, c, h, w, r = _roi_inputs(x, rois)
+    out = torch.empty((n * r, output_dim, pooled_h, pooled_w), device=x.device, dtype=torch.float32)
+    _check("fcuda_psroi_pooling_forward", fcuda().fcuda_psroi_pooling_forward(_ptr(out), _ptr(x), _ptr(rois), c, h, w, r,
+                                                                              pooled_h, pooled_w, output_dim,
+                                                                              float(spatial_scale), n, _stream()))
     return out

@@ -862,6 +862,8 @@ namespace {
 //           time, each kept box ORs its mask row (from L2) into the bitmap and writes its output row; stops at
 //           after_nms_topN.
 // roi_pool  one thread per output element, pooled x fastest.
+// psroi     R-FCN's position-sensitive average pooling: one thread per output element, pooled x fastest; bin (ph, pw) of
+//           output channel q reads input channel (q * PH + ph) * PW + pw.
 constexpr int kProposalAnchors = 9;  // ratios {0.5, 1, 2} x scales {8, 16, 32}
 constexpr int kMaskChunk = 1024;     // columns of the mask staged per pass
 
@@ -1103,6 +1105,44 @@ roi_pool_kernel(float* __restrict__ out, const float* __restrict__ in, const flo
     }
 }
 
+// (int)floorf / ceilf converted saturating (a NaN reads as 0), then clamped to [0, hi]
+__device__ __forceinline__ int psroi_edge(float v, int hi) { return min(max(static_cast<int>(v), 0), hi); }
+
+__global__ void __launch_bounds__(256)
+psroi_pool_kernel(float* __restrict__ out, const float* __restrict__ in, const float* __restrict__ rois, int C, int H,
+                  int W, int R, int PH, int PW, int D, float scale, long long total) {
+    for (long long t = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x; t < total;
+         t += static_cast<long long>(gridDim.x) * blockDim.x) {
+        long long r = t;
+        const int pw = static_cast<int>(r % PW);
+        r /= PW;
+        const int ph = static_cast<int>(r % PH);
+        r /= PH;
+        const int q = static_cast<int>(r % D);
+        const long long item = r / D, n = item / R;
+        const float* roi = rois + item * 4;
+        const float x1 = __fmul_rn(roundf(roi[0]), scale), y1 = __fmul_rn(roundf(roi[1]), scale);
+        const float x2 = __fmul_rn(roundf(__fadd_rn(roi[2], 1.f)), scale);
+        const float y2 = __fmul_rn(roundf(__fadd_rn(roi[3], 1.f)), scale);
+        const float bin_w = __fdiv_rn(fmaxf(__fsub_rn(x2, x1), 0.1f), static_cast<float>(PW));
+        const float bin_h = __fdiv_rn(fmaxf(__fsub_rn(y2, y1), 0.1f), static_cast<float>(PH));
+        const int ws = psroi_edge(floorf(__fadd_rn(x1, __fmul_rn(static_cast<float>(pw), bin_w))), W);
+        const int we = psroi_edge(ceilf(__fadd_rn(x1, __fmul_rn(static_cast<float>(pw + 1), bin_w))), W);
+        const int hs = psroi_edge(floorf(__fadd_rn(y1, __fmul_rn(static_cast<float>(ph), bin_h))), H);
+        const int he = psroi_edge(ceilf(__fadd_rn(y1, __fmul_rn(static_cast<float>(ph + 1), bin_h))), H);
+        float v = 0.f;
+        if (we > ws && he > hs) {
+            const int c = (q * PH + ph) * PW + pw;
+            const float* plane = in + (static_cast<size_t>(n) * C + c) * H * W;
+            float sum = 0.f;
+            for (int h = hs; h < he; ++h)
+                for (int x = ws; x < we; ++x) sum = __fadd_rn(sum, __ldg(plane + static_cast<size_t>(h) * W + x));
+            v = __fdiv_rn(sum, static_cast<float>((he - hs) * (we - ws)));
+        }
+        out[t] = v;
+    }
+}
+
 ProposalGeom proposal_geom(const FcudaProposalParam& p, int feat_h, int feat_w) {
     ProposalGeom g{};
     g.A = kProposalAnchors;
@@ -1206,6 +1246,19 @@ int roi_pooling_forward(float* out, const float* in, const float* rois, int C, i
     const long long blocks = (total + 255) / 256;
     roi_pool_kernel<<<static_cast<unsigned>(blocks < 65536 * 16 ? blocks : 65536 * 16), 256, 0, s>>>(
         out, in, rois, C, H, W, R, pooled_h, pooled_w, spatial_scale, total);
+    FCUDA_CHECK_LAUNCH();
+    prof_end(prof, s);
+    count_launch();
+    return 0;
+}
+
+int psroi_pooling_forward(float* out, const float* in, const float* rois, int C, int H, int W, int R, int pooled_h,
+                          int pooled_w, int output_dim, float spatial_scale, int batch, cudaStream_t s) {
+    const long long total = static_cast<long long>(batch) * R * C;  // C = output_dim * pooled_h * pooled_w
+    const int prof = prof_begin(s, PROF_RCNN, 0, 0, 4.0 * batch * C * H * W + 16.0 * batch * R + 4.0 * total);
+    const long long blocks = (total + 255) / 256;
+    psroi_pool_kernel<<<static_cast<unsigned>(blocks < 65536 * 16 ? blocks : 65536 * 16), 256, 0, s>>>(
+        out, in, rois, C, H, W, R, pooled_h, pooled_w, output_dim, spatial_scale, total);
     FCUDA_CHECK_LAUNCH();
     prof_end(prof, s);
     count_launch();

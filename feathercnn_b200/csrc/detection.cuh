@@ -39,4 +39,8 @@ int proposal_forward(float* rois, float* scores, const float* score, const float
                      const FcudaProposalParam& p, int feat_h, int feat_w, float* workspace, int batch, cudaStream_t s);
 int roi_pooling_forward(float* out, const float* in, const float* rois, int channels, int height, int width, int num_rois,
                         int pooled_h, int pooled_w, float spatial_scale, int batch, cudaStream_t s);
+// R-FCN; channels == output_dim * pooled_h * pooled_w, checked by the caller.
+int psroi_pooling_forward(float* out, const float* in, const float* rois, int channels, int height, int width,
+                          int num_rois, int pooled_h, int pooled_w, int output_dim, float spatial_scale, int batch,
+                          cudaStream_t s);
 }  // namespace fcuda

@@ -1041,6 +1041,17 @@ int fcuda_roi_pooling_forward(float* output, const float* input, const float* ro
                                batch, as_stream(stream));
 }
 
+int fcuda_psroi_pooling_forward(float* output, const float* input, const float* rois, int channels, int height,
+                                int width, int num_rois, int pooled_h, int pooled_w, int output_dim, float spatial_scale,
+                                int batch, void* stream) {
+    if (pooled_h < 1 || pooled_w < 1 || output_dim < 1 || !isfinite(spatial_scale) || !(spatial_scale > 0.f) ||
+        static_cast<long long>(output_dim) * pooled_h * pooled_w != channels)
+        return -200;
+    if (!output || !input || !rois || channels < 1 || height < 1 || width < 1 || num_rois < 1 || batch < 1) return -100;
+    return psroi_pooling_forward(output, input, rois, channels, height, width, num_rois, pooled_h, pooled_w, output_dim,
+                                 spatial_scale, batch, as_stream(stream));
+}
+
 static const long long kRouteMaxPositions = 1ll << 31;  // positions of the concatenated axis fit an int
 
 int fcuda_route_forward(const FcudaRoute* route, int batch, void* stream) {

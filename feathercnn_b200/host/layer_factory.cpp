@@ -1,7 +1,8 @@
 // Built-in layer registrations: the 13 ncnn type names the reference serves (/root/reference/src/layer_factory.cpp:53-68)
 // plus Deconvolution / DeconvolutionDepthWise, Interp, Crop, Clip, PReLU, SSD's Permute, Flatten, Reshape, PriorBox and
 // DetectionOutput, VGG-SSD's Normalize, YOLO's YoloDetectionOutput and Yolov3DetectionOutput, ShuffleNet's ShuffleChannel
-// and Slice, AlexNet's and GoogLeNet's LRN, and Faster R-CNN's Proposal and ROIPooling, 32 in all, mapped onto this
+// and Slice, AlexNet's and GoogLeNet's LRN, Faster R-CNN's Proposal and ROIPooling, and R-FCN's PSROIPooling, 33 in all,
+// mapped onto this
 // host's layer classes.  A table of {type name,
 // factory} pairs instead of one macro line per layer; the
 // DEFINE_LAYER_CREATOR / REGISTER_LAYER_CREATOR macros of <feather/layer_factory.h> remain the plugin API for user layers.
@@ -77,6 +78,7 @@ const BuiltIn kBuiltIns[] = {
     {"LRN", make_layer<LRNLayer>},
     {"Proposal", make_layer<ProposalLayer>},
     {"ROIPooling", make_layer<ROIPoolingLayer>},
+    {"PSROIPooling", make_layer<PSROIPoolingLayer>},
 };
 
 }  // namespace

@@ -1,11 +1,12 @@
-// ProposalLayer and ROIPoolingLayer — ncnn's Proposal and ROIPooling, the two layers of a Faster R-CNN the other layers
-// do not cover; the reference has neither.  Parameter ids and defaults follow ncnn: Proposal 0=feat_stride (16)
-// 1=base_size (16) 2=pre_nms_topN (6000) 3=after_nms_topN (300) 4=nms_thresh (0.7) 5=min_size (16); ROIPooling 0=pooled_w
-// (7) 1=pooled_h (7) 2=spatial_scale (0.0625).  Proposal's output has a fixed shape (include/fcuda.h): rois
+// ProposalLayer, ROIPoolingLayer and PSROIPoolingLayer — ncnn's Proposal, ROIPooling and PSROIPooling, the layers of a
+// Faster R-CNN and an R-FCN the other layers do not cover; the reference has none of them.  Parameter ids and defaults
+// follow ncnn: Proposal 0=feat_stride (16) 1=base_size (16) 2=pre_nms_topN (6000) 3=after_nms_topN (300) 4=nms_thresh
+// (0.7) 5=min_size (16); ROIPooling 0=pooled_w (7) 1=pooled_h (7) 2=spatial_scale (0.0625); PSROIPooling the same and
+// 3=output_dim (0, which is rejected: a net must give it).  Proposal's output has a fixed shape (include/fcuda.h): rois
 // (after_nms_topN, 1, 4) per image, zero rows past the kept count, and an optional second top of scores (after_nms_topN,
-// 1, 1), -1 past the count.  ROIPooling pools every RoI of image n from image n's map, so its top has
-// batch * after_nms_topN items and the layers after it (fc6, fc7, ...) run once over all of them.  Neither layer takes
-// part in fusion.
+// 1, 1), -1 past the count.  ROIPooling and PSROIPooling pool every RoI of image n from image n's map, so their tops have
+// batch * after_nms_topN items and the layers after them (fc6, fc7, ...; R-FCN's average-pooling vote) run once over all
+// of them.  None of these layers takes part in fusion.
 #pragma once
 
 #include <math.h>
@@ -107,6 +108,50 @@ public:
 
 private:
     int pooled_w = 7, pooled_h = 7;
+    float spatial_scale = 0.0625f;
+};
+
+class PSROIPoolingLayer : public Layer {
+public:
+    explicit PSROIPoolingLayer(RuntimeParameter<float>* rt_param) : Layer(rt_param) {}
+    int LoadParam(const ncnn::ParamDict& pd) {
+        pooled_w = pd.get(0, 7);
+        pooled_h = pd.get(1, 7);
+        spatial_scale = pd.get(2, 0.0625f);
+        output_dim = pd.get(3, 0);
+        if (bottoms.size() != 2 || pooled_w < 1 || pooled_h < 1 || output_dim < 1 || !isfinite(spatial_scale) ||
+            !(spatial_scale > 0.f)) {
+            LOGE("Layer %s: PSROIPooling needs 2 bottoms (score maps, rois), pooled_w, pooled_h and output_dim >= 1 and "
+                 "a finite spatial_scale > 0", this->name.c_str());
+            return FEATHER_ERR_UNSUPPORTED;
+        }
+        return 0;
+    }
+    int Reshape() {
+        const Blob<float>* x = bottoms[0];
+        const Blob<float>* rois = bottoms[1];
+        if (x->channels() != static_cast<size_t>(output_dim) * pooled_h * pooled_w) {
+            LOGE("Layer %s: PSROIPooling needs output_dim x pooled_h x pooled_w = %d x %d x %d channels, not %zu",
+                 this->name.c_str(), output_dim, pooled_h, pooled_w, x->channels());
+            return FEATHER_ERR_TOPOLOGY;
+        }
+        if (rois->num() != x->num() || rois->height() * rois->width() != 4) {
+            LOGE("Layer %s: PSROIPooling needs rois (R, 1, 4) per image of the score maps' batch", this->name.c_str());
+            return FEATHER_ERR_TOPOLOGY;
+        }
+        tops[0]->ReshapeWithRealloc(x->num() * rois->channels(), output_dim, pooled_h, pooled_w);
+        return 0;
+    }
+    int Forward() {
+        const Blob<float>* x = bottoms[0];
+        return fcuda_psroi_pooling_forward(tops[0]->data(), x->data(), bottoms[1]->data(), static_cast<int>(x->channels()),
+                                           static_cast<int>(x->height()), static_cast<int>(x->width()),
+                                           static_cast<int>(bottoms[1]->channels()), pooled_h, pooled_w, output_dim,
+                                           spatial_scale, static_cast<int>(x->num()), stream());
+    }
+
+private:
+    int pooled_w = 7, pooled_h = 7, output_dim = 0;
     float spatial_scale = 0.0625f;
 };
 

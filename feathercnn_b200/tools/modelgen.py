@@ -9,8 +9,8 @@ BN + Scale + ReLU as separate layers, Split/Eltwise residuals), MobileNet-v1, Mo
 AlexNet (BVLC's deploy nets, with LRN), plus a small "mini" net
 that exercises every layer type, single-shot detectors (MobileNet-SSD, VGG-SSD 300, a two-head tiny SSD), YOLO detectors
 (MobileNet-YOLOv2, MobileNet-v2 YOLOv3, a two-scale tiny YOLOv3), two-stage detectors (py-faster-rcnn's VGG-16 Faster
-R-CNN and a tiny one) and ShuffleNet-v2 with a small routing probe net.  Weight statistics follow
-SURVEY.md §8(d).
+R-CNN, py-R-FCN's ResNet-50 R-FCN and a tiny one of each) and ShuffleNet-v2 with a small routing probe net.  Weight
+statistics follow SURVEY.md §8(d).
 """
 from __future__ import annotations
 
@@ -421,6 +421,17 @@ class ModelWriter:
         self.shape[top] = (self.shape[bottom][0], pooled_h, pooled_w)
         return top
 
+    def psroi_pooling(self, name, bottom, rois, output_dim, pooled_w=7, pooled_h=7, spatial_scale=0.0625, top=None):
+        """ncnn PSROIPooling 0=pooled_w 1=pooled_h 2=spatial_scale 3=output_dim on output_dim x pooled_h x pooled_w score
+        maps.  One item per RoI of every image, as roi_pooling; its shape here is one item's (output_dim, pooled_h,
+        pooled_w)."""
+        top = top or name
+        assert self.shape[bottom][0] == output_dim * pooled_h * pooled_w, (name, self.shape[bottom])
+        self._layer("PSROIPooling", name, [bottom, rois], [top],
+                    {0: pooled_w, 1: pooled_h, 2: f"{spatial_scale:e}", 3: output_dim})
+        self.shape[top] = (output_dim, pooled_h, pooled_w)
+        return top
+
     def dropout(self, name, bottom, top=None, scale=None):
         top = top or name
         self._layer("Dropout", name, [bottom], [top], {} if scale is None else {0: f"{scale:e}"})
@@ -506,15 +517,14 @@ def _bn_scale_relu(m: ModelWriter, tag: str, x: str, relu=True, center=1.0):
     return x
 
 
-def resnet50(seed=0, num_classes=1000, size=224, wide_stats=False) -> ModelWriter:
-    """Caffe ResNet-50 layout: stride on the first 1x1 of each stage, BN/Scale/ReLU layers, Split/Eltwise."""
-    m = ModelWriter(seed, wide_stats)
-    x = m.input("data", 3, size, size)
+def _resnet50_trunk(m: ModelWriter, x: str, strides=(1, 2, 2, 2), dilations=(1, 1, 1, 1)) -> str:
+    """Caffe ResNet-50 conv1 .. res5c_relu: stride on the first 1x1 of each stage (strides[i] for res2 .. res5), every
+    3x3 branch2b of stage i at dilation and pad dilations[i], BN/Scale/ReLU layers, Split/Eltwise."""
     x = m.conv("conv1", x, 64, 7, 2, 3, True)
     x = _bn_scale_relu(m, "_conv1", x)
     x = m.pool("pool1", x, 0, 3, 2, 0)
-    stages = [(2, 3, 64, 1), (3, 4, 128, 2), (4, 6, 256, 2), (5, 3, 512, 2)]
-    for sid, nblocks, width, stride in stages:
+    stages = [(2, 3, 64), (3, 4, 128), (4, 6, 256), (5, 3, 512)]
+    for (sid, nblocks, width), stride, dil in zip(stages, strides, dilations):
         for b in range(nblocks):
             blk = f"{sid}{chr(ord('a') + b)}"
             s = stride if b == 0 else 1
@@ -526,12 +536,19 @@ def resnet50(seed=0, num_classes=1000, size=224, wide_stats=False) -> ModelWrite
                 sc = a
             y = m.conv(f"res{blk}_branch2a", c, width, 1, s, 0, False)
             y = _bn_scale_relu(m, f"{blk}_branch2a", y)
-            y = m.conv(f"res{blk}_branch2b", y, width, 3, 1, 1, False)
+            y = m.conv(f"res{blk}_branch2b", y, width, 3, 1, dil, False, dilation=dil)
             y = _bn_scale_relu(m, f"{blk}_branch2b", y)
             y = m.conv(f"res{blk}_branch2c", y, width * 4, 1, 1, 0, False)
             y = _bn_scale_relu(m, f"{blk}_branch2c", y, relu=False, center=0.3)  # keep residual sums O(1)
             x = m.eltwise(f"res{blk}", [sc, y])
             x = m.relu(f"res{blk}_relu", x)
+    return x
+
+
+def resnet50(seed=0, num_classes=1000, size=224, wide_stats=False) -> ModelWriter:
+    """Caffe ResNet-50 layout: stride on the first 1x1 of each stage, BN/Scale/ReLU layers, Split/Eltwise."""
+    m = ModelWriter(seed, wide_stats)
+    x = _resnet50_trunk(m, m.input("data", 3, size, size))
     x = m.pool("pool5", x, 1, 7, 1, 0, global_pooling=True)
     x = m.fc("fc1000", x, num_classes)
     m.softmax("prob", x)
@@ -1131,14 +1148,12 @@ def yolo_tiny(seed=0, size=64, num_classes=5, confidence_threshold=0.05, head_ga
     return m
 
 
-def _faster_rcnn_head(m: ModelWriter, feat: str, num_classes: int, rpn_width: int, fc_width: int, feat_stride: int,
-                      base_size: int, pre_nms_top_n: int, post_nms_top_n: int, min_size: int, pooled: int,
-                      rpn_cls_gain: float, rpn_bbox_gain: float):
-    """py-faster-rcnn's test net after the backbone: rpn_conv/3x3 + ReLU; rpn_cls_score (2 x 9) and rpn_bbox_pred (4 x 9)
-    1x1 convolutions; Reshape (2, -1, W) -> Softmax over the channel axis -> Reshape (18, -1, W); Proposal; ROIPooling
-    pooled x pooled at 1 / feat_stride; fc6 and fc7 (ReLU, Dropout); cls_score -> Softmax (cls_prob) and bbox_pred.  The
-    RPN gains multiply He init: rpn_cls_gain spreads the objectness logits, rpn_bbox_gain keeps the box deltas small so
-    the boxes stay finite and neighbouring anchors overlap."""
+def _rpn(m: ModelWriter, feat: str, rpn_width: int, feat_stride: int, base_size: int, pre_nms_top_n: int,
+         post_nms_top_n: int, min_size: int, rpn_cls_gain: float, rpn_bbox_gain: float) -> str:
+    """py-faster-rcnn's region proposal network on `feat`: rpn_conv/3x3 + ReLU; rpn_cls_score (2 x 9) and rpn_bbox_pred
+    (4 x 9) 1x1 convolutions; Reshape (2, -1, W) -> Softmax over the channel axis -> Reshape (18, -1, W); Proposal (nms
+    0.7) on im_info.  The gains multiply He init: rpn_cls_gain spreads the objectness logits, rpn_bbox_gain keeps the box
+    deltas small so the boxes stay finite and neighbouring anchors overlap.  Returns the rois blob."""
     fan_in = rpn_width
     x = m.relu("rpn_relu/3x3", m.conv("rpn_conv/3x3", feat, rpn_width, 3, 1, 1, True))
     cls = m.conv("rpn_cls_score", x, 18, 1, 1, 0, True, gain=rpn_cls_gain * np.sqrt(2.0 / fan_in))
@@ -1147,8 +1162,17 @@ def _faster_rcnn_head(m: ModelWriter, feat: str, num_classes: int, rpn_width: in
     cls = m.reshape("rpn_cls_score_reshape", cls, 0, -1, 2)
     cls = m.softmax("rpn_cls_prob", cls, axis=0)
     cls = m.reshape("rpn_cls_prob_reshape", cls, 0, -1, 18)
-    rois = m.proposal("proposal", cls, bbox, "im_info", feat_stride, base_size, pre_nms_top_n, post_nms_top_n, 0.7,
+    return m.proposal("proposal", cls, bbox, "im_info", feat_stride, base_size, pre_nms_top_n, post_nms_top_n, 0.7,
                       min_size, tops=["rois"])
+
+
+def _faster_rcnn_head(m: ModelWriter, feat: str, num_classes: int, rpn_width: int, fc_width: int, feat_stride: int,
+                      base_size: int, pre_nms_top_n: int, post_nms_top_n: int, min_size: int, pooled: int,
+                      rpn_cls_gain: float, rpn_bbox_gain: float):
+    """py-faster-rcnn's test net after the backbone: _rpn; ROIPooling pooled x pooled at 1 / feat_stride; fc6 and fc7
+    (ReLU, Dropout); cls_score -> Softmax (cls_prob) and bbox_pred."""
+    rois = _rpn(m, feat, rpn_width, feat_stride, base_size, pre_nms_top_n, post_nms_top_n, min_size, rpn_cls_gain,
+                rpn_bbox_gain)
     x = m.roi_pooling("roi_pool5", feat, rois, pooled, pooled, 1.0 / feat_stride, top="pool5")
     x = m.dropout("drop6", m.relu("relu6", m.fc("fc6", x, fc_width)))
     x = m.dropout("drop7", m.relu("relu7", m.fc("fc7", x, fc_width)))
@@ -1190,13 +1214,62 @@ def faster_rcnn_tiny(seed=0, height=96, width=128, num_classes=5, pre_nms_top_n=
     return m
 
 
+def _rfcn_head(m: ModelWriter, feat: str, rois: str, num_classes: int, width: int, pooled: int, feat_stride: int):
+    """py-R-FCN's test net after the trunk: conv_new_1 (1x1, width) + ReLU; the position-sensitive score maps rfcn_cls
+    (pooled^2 x num_classes) and rfcn_bbox (pooled^2 x 8: class-agnostic boxes) as 1x1 convolutions; PSROIPooling of both
+    pooled x pooled at 1 / feat_stride; the vote, a pooled x pooled / pooled average Pooling, to cls_score and bbox_pred;
+    cls_score -> Softmax (cls_prob)."""
+    x = m.relu("conv_new_1_relu", m.conv("conv_new_1", feat, width, 1, 1, 0, True))
+    cls = m.conv("rfcn_cls", x, pooled * pooled * num_classes, 1, 1, 0, True)
+    loc = m.conv("rfcn_bbox", x, pooled * pooled * 8, 1, 1, 0, True)
+    cls = m.psroi_pooling("psroipooled_cls_rois", cls, rois, num_classes, pooled, pooled, 1.0 / feat_stride)
+    loc = m.psroi_pooling("psroipooled_loc_rois", loc, rois, 8, pooled, pooled, 1.0 / feat_stride)
+    cls = m.pool("ave_cls_score_rois", cls, 1, pooled, pooled, top="cls_score")
+    m.pool("ave_bbox_pred_rois", loc, 1, pooled, pooled, top="bbox_pred")
+    m.softmax("cls_prob", cls)
+
+
+def rfcn_resnet50(seed=0, height=600, width=800, num_classes=21, pre_nms_top_n=6000, post_nms_top_n=300,
+                  rpn_cls_gain=1.0, rpn_bbox_gain=0.1) -> ModelWriter:
+    """py-R-FCN's ResNet-50 rfcn_end2end test net: Input data (3, height, width) and Input im_info; Caffe ResNet-50 with
+    res5 at stride 1 (res5a_branch1 and res5a_branch2a stride 1, every res5 3x3 at dilation 2 and pad 2), so res4f and
+    res5c are both at 1 / 16 (38 x 50 at 600 x 800); _rpn on res4f (512 wide, Proposal 16 / 16 / pre_nms_top_n /
+    post_nms_top_n / 0.7 / 16); _rfcn_head on res5c: conv_new_1 1024, rfcn_cls 7 x 7 x num_classes, rfcn_bbox 7 x 7 x 8,
+    PSROIPooling 7 x 7 at 1 / 16 and the 7 x 7 average vote, over batch x post_nms_top_n RoIs."""
+    m = ModelWriter(seed)
+    x = m.input("data", 3, height, width)
+    m.extra_input("im_info")
+    x = _resnet50_trunk(m, x, strides=(1, 2, 2, 1), dilations=(1, 1, 1, 2))
+    rois = _rpn(m, "res4f_relu", 512, 16, 16, pre_nms_top_n, post_nms_top_n, 16, rpn_cls_gain, rpn_bbox_gain)
+    _rfcn_head(m, x, rois, num_classes, 1024, 7, 16)
+    return m
+
+
+def rfcn_tiny(seed=0, height=96, width=128, num_classes=5, pre_nms_top_n=2000, post_nms_top_n=64, rpn_cls_gain=1.0,
+              rpn_bbox_gain=0.1) -> ModelWriter:
+    """R-FCN at float64-checkable size: two 3x3 / 2 convolutions (16, 32 channels, ReLU) to a 1 / 4 map (24 x 32 at
+    96 x 128: 6,912 anchors) and a 3x3 convolution at dilation 2 (32 channels, ReLU); _rpn on it (32 wide, feat_stride 4,
+    base_size 2, min_size 4); _rfcn_head with conv_new_1 64 wide, PSROIPooling 3 x 3 at 1 / 4 (rfcn_cls 9 x num_classes,
+    rfcn_bbox 72 channels) and the 3 x 3 vote."""
+    m = ModelWriter(seed)
+    x = m.input("data", 3, height, width)
+    m.extra_input("im_info")
+    x = m.relu("relu1", m.conv("conv1", x, 16, 3, 2, 1, True))
+    x = m.relu("relu2", m.conv("conv2", x, 32, 3, 2, 1, True))
+    x = m.relu("relu3", m.conv("conv3", x, 32, 3, 1, 2, True, dilation=2))
+    rois = _rpn(m, x, 32, 4, 2, pre_nms_top_n, post_nms_top_n, 4, rpn_cls_gain, rpn_bbox_gain)
+    _rfcn_head(m, x, rois, num_classes, 64, 3, 4)
+    return m
+
+
 ZOO = {"single_conv": single_conv, "vgg16": vgg16, "resnet50": resnet50, "mobilenet_v1": mobilenet_v1, "mini": mini,
        "decoder_tiny": decoder_tiny, "fcn8s_tiny": fcn8s_tiny, "deeplab_head_tiny": deeplab_head_tiny,
        "mobilenet_v2": mobilenet_v2, "prelu_tiny": prelu_tiny, "mobilenet_ssd": mobilenet_ssd, "ssd_tiny": ssd_tiny,
        "vgg_ssd": vgg_ssd, "googlenet": googlenet, "alexnet": alexnet,
        "mobilenet_yolov2": mobilenet_yolov2, "mobilenetv2_yolov3": mobilenetv2_yolov3, "yolo_tiny": yolo_tiny,
        "shufflenet_v2": shufflenet_v2, "shuffle_tiny": shuffle_tiny, "deeplabv3_mobilenet_v2": deeplabv3_mobilenet_v2,
-       "deeplabv3_tiny": deeplabv3_tiny, "faster_rcnn_vgg16": faster_rcnn_vgg16, "faster_rcnn_tiny": faster_rcnn_tiny}
+       "deeplabv3_tiny": deeplabv3_tiny, "faster_rcnn_vgg16": faster_rcnn_vgg16, "faster_rcnn_tiny": faster_rcnn_tiny,
+       "rfcn_resnet50": rfcn_resnet50, "rfcn_tiny": rfcn_tiny}
 
 
 def synthetic_input(shape, index: int = 0) -> np.ndarray:

@@ -504,7 +504,7 @@ int fcuda_yolo_detection_workspace_size(const FcudaYoloParam* param, int batch, 
 int fcuda_yolo_detection_forward(float* output, const float* const* inputs, const FcudaYoloParam* param, float* workspace,
                                  int batch, void* stream);
 
-/* ---- Faster R-CNN: Proposal and ROIPooling (the reference has neither layer) ---------------------------------------
+/* ---- Faster R-CNN and R-FCN: Proposal, ROIPooling and PSROIPooling (the reference has none of them) ----------------
  * Stream-ordered like the detection calls above: nothing allocates, synchronises or copies to the host.
  *
  * Proposal (ncnn's layer, py-faster-rcnn's proposal_layer.py arithmetic) in fp32, every operation rounded on its own (no
@@ -559,6 +559,23 @@ int fcuda_proposal_forward(float* rois, float* scores, const float* score, const
  * Every RoI row is pooled, the [0, 0, 0, 0] padding of fcuda_proposal_forward included. */
 int fcuda_roi_pooling_forward(float* output, const float* input, const float* rois, int channels, int height, int width,
                               int num_rois, int pooled_h, int pooled_w, float spatial_scale, int batch, void* stream);
+
+/* PSROIPooling (R-FCN's position-sensitive RoI average pooling; ncnn's and R-FCN Caffe's arithmetic) in fp32, every
+ * operation rounded on its own (no FMA): input (batch, C, H, W) with C = output_dim * pooled_h * pooled_w, rois and item
+ * layout as ROIPooling; output (batch * num_rois, output_dim, pooled_h, pooled_w).  For output (item, q, ph, pw):
+ *   x1 = roundf(roi[0]) * spatial_scale, y1 likewise          (roundf: half away from zero)
+ *   x2 = roundf(roi[2] + 1) * spatial_scale, y2 likewise with roi[3]
+ *   roi_w = fmaxf(x2 - x1, 0.1), bin_w = roi_w / pooled_w     (roi_h, bin_h likewise)
+ *   wstart = (int)floorf(x1 + pw * bin_w), wend = (int)ceilf(x1 + (pw + 1) * bin_w), converted saturating (NaN -> 0),
+ *   then clamped to [0, W]                                    (h likewise)
+ *   c = (q * pooled_h + ph) * pooled_w + pw
+ *   value = 0 for an empty bin, else (the sum over the bin of plane c, row-major from 0) / (float)area: bit-exact.
+ * Limits: -200 for pooled_h, pooled_w or output_dim < 1, spatial_scale not finite and > 0, or channels !=
+ * output_dim * pooled_h * pooled_w; -100 for a NULL pointer or a size < 1.  Every RoI row is pooled, the [0, 0, 0, 0]
+ * padding of fcuda_proposal_forward included. */
+int fcuda_psroi_pooling_forward(float* output, const float* input, const float* rois, int channels, int height,
+                                int width, int num_rois, int pooled_h, int pooled_w, int output_dim, float spatial_scale,
+                                int batch, void* stream);
 
 /* ---- Channel routing: ncnn's ShuffleChannel and Slice, and Concat -> ShuffleChannel -> Slice fused (the reference has
  * neither layer) ------------------------------------------------------------------------------------------------------
@@ -634,7 +651,7 @@ int fcuda_profile_collect(double* total_ms, double* algo_flops, double* mma_flop
  * kind 0 TensorGEMM, 1 implicit-GEMM conv, 2 Winograd input transform, 3 Winograd output transform, 4 pooling,
  * 5 depthwise, 6 element-wise (BN/Scale/Eltwise/Clip/PReLU/Normalize/LRN), 7 deconvolution scatter / depthwise gather, 8 resize / crop (Interp,
  * Crop), 9 detection (Permute, axis Softmax, PriorBox, decode, NMS, merge; YOLO decode, select, mask, sweep), 10 channel
- * routing (fcuda_route_forward), 11 two-stage detection (Proposal decode, select, mask, sweep; ROIPooling), < 0 all.  algo_bytes = the bytes the operation must move (inputs
+ * routing (fcuda_route_forward), 11 two-stage detection (Proposal decode, select, mask, sweep; ROIPooling; PSROIPooling), < 0 all.  algo_bytes = the bytes the operation must move (inputs
  * read once + outputs written once). */
 int fcuda_profile_collect_kind(int kind, double* total_ms, double* algo_flops, double* mma_flops, double* algo_bytes,
                                long long* launches);
