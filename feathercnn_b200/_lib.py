@@ -70,6 +70,12 @@ class FcudaInterpParam(ctypes.Structure):
                 [(n, ctypes.c_int) for n in "output_height output_width input_h input_w output_h output_w".split()])
 
 
+class FcudaPad(ctypes.Structure):
+    """include/fcuda.h FcudaPad: type 0 constant, 1 replicate, 2 reflect."""
+
+    _fields_ = [(n, ctypes.c_int) for n in "top bottom left right type".split()] + [("value", ctypes.c_float)]
+
+
 class FcudaPriorBoxParam(ctypes.Structure):
     """include/fcuda.h FcudaPriorBoxParam (fixed arrays of FCUDA_PRIORBOX_MAX = 16)."""
 
@@ -186,6 +192,9 @@ def fcuda() -> ctypes.CDLL:
             "fcuda_prelu_forward": (i, [vp, vp, i, sz, vp, i, i, vp]),
             "fcuda_normalize_workspace_size": (i, [i, i, i, sz, i, szp]),
             "fcuda_normalize_forward": (i, [vp, vp, i, sz, vp, i, i, i, f, i, vp, i, vp]),
+            "fcuda_instance_norm_workspace_size": (i, [i, sz, i, szp]),
+            "fcuda_instance_norm_forward": (i, [vp, vp, i, i, i, vp, vp, f, i, vp, vp, i, vp]),
+            "fcuda_padding_forward": (i, [vp, vp, i, i, i, vp, i, vp]),
             "fcuda_lrn_forward": (i, [vp, vp, i, i, i, i, i, f, f, f, i, vp]),
             "fcuda_softmax_forward": (i, [vp, vp, sz, i, vp]),
             "fcuda_dropout_forward": (i, [vp, vp, sz, ctypes.c_float, vp]),

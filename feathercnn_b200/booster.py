@@ -15,6 +15,7 @@ import torch
 from ._lib import FcudaConvOptions, FcudaConvParam, fcuda
 from ._lib import FcudaDeconvParam as DeconvParam
 from ._lib import FcudaInterpParam as InterpParam
+from ._lib import FcudaPad
 from ._lib import FcudaPriorBoxParam as PriorBoxParam
 from ._lib import FcudaProposalParam as ProposalParam
 from ._lib import FcudaYoloParam as YoloParam
@@ -584,6 +585,47 @@ def normalize(x, scale, across_spatial=0, across_channel=1, eps=1e-4, eps_mode=0
            lib.fcuda_normalize_forward(_ptr(out), _ptr(x.contiguous()), c, plane, _ptr(scale.contiguous()), scale.numel(),
                                        int(across_spatial), int(across_channel), float(eps), int(eps_mode),
                                        _ptr(workspace), n, _stream()))
+    return out
+
+
+def _pad(top, bottom, left, right, type_, value) -> FcudaPad:
+    return FcudaPad(int(top), int(bottom), int(left), int(right), int(type_), float(value))
+
+
+def _padded_shape(x, p: FcudaPad | None):
+    n, c, h, w = x.shape
+    return (n, c, h + p.top + p.bottom, w + p.left + p.right) if p is not None else (n, c, h, w)
+
+
+def instance_norm(x, gamma, beta, eps, relu=False, pad=None, out=None):
+    """ncnn InstanceNorm over (N, C, H, W): y = fmaf(x, a, b) per plane from its mean and biased variance, a ReLU with
+    `relu`, and with `pad` = (top, bottom, left, right, type, value) the output plane padded in the same pass
+    (include/fcuda.h).  gamma = beta = None: affine 0.  The workspace comes from torch.  `out` may be `x` when unpadded."""
+    lib = fcuda()
+    assert x.dim() == 4, x.shape
+    n, c, h, w = x.shape
+    p = _pad(*pad) if pad is not None else None
+    ws = ctypes.c_size_t(0)
+    _check("fcuda_instance_norm_workspace_size", lib.fcuda_instance_norm_workspace_size(c, h * w, n, ctypes.byref(ws)))
+    workspace = torch.empty(ws.value, device=x.device, dtype=torch.float32)
+    out = torch.empty(_padded_shape(x, p), device=x.device, dtype=torch.float32) if out is None else out
+    assert tuple(out.shape) == _padded_shape(x, p), (out.shape, x.shape)
+    _check("fcuda_instance_norm_forward",
+           lib.fcuda_instance_norm_forward(_ptr(out), _ptr(x), c, h, w,
+                                           _ptr(gamma.contiguous()) if gamma is not None else None,
+                                           _ptr(beta.contiguous()) if beta is not None else None, float(eps), int(relu),
+                                           ctypes.byref(p) if p is not None else None, _ptr(workspace), n, _stream()))
+    return out
+
+
+def padding(x, top, bottom, left, right, type=0, value=0.0, out=None):
+    """ncnn Padding of every (N, C) plane of x: type 0 constant `value`, 1 replicate, 2 reflect (include/fcuda.h)."""
+    p = _pad(top, bottom, left, right, type, value)
+    n, c, h, w = x.shape
+    out = torch.empty(_padded_shape(x, p), device=x.device, dtype=torch.float32) if out is None else out
+    assert tuple(out.shape) == _padded_shape(x, p), (out.shape, x.shape)
+    _check("fcuda_padding_forward",
+           fcuda().fcuda_padding_forward(_ptr(out), _ptr(x), c, h, w, ctypes.byref(p), n, _stream()))
     return out
 
 

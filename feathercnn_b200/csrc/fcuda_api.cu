@@ -8,6 +8,7 @@
 #include "conv_igemm.cuh"
 #include "depthwise.cuh"
 #include "detection.cuh"
+#include "instance_norm.cuh"
 #include "layers.cuh"
 #include "lrn.cuh"
 #include "normalize.cuh"
@@ -829,6 +830,55 @@ int fcuda_normalize_forward(float* output, const float* input, int channels, siz
     g.eps = eps;
     g.eps_mode = eps_mode;
     return normalize_forward(input, output, scale, g, workspace, as_stream(stream));
+}
+
+// -200 for a pad fcuda.h rejects; *padded tells whether any side is non-zero.
+static int plane_pad_check(const FcudaPad* pad, int h, int w, PlanePad* out, int* padded) {
+    *out = PlanePad{0, 0, 0, 0, 0, 0.f};
+    *padded = 0;
+    if (!pad) return 0;
+    if (pad->top < 0 || pad->bottom < 0 || pad->left < 0 || pad->right < 0 || pad->type < 0 || pad->type > 2) return -200;
+    if (pad->type == 2 && (pad->top >= h || pad->bottom >= h || pad->left >= w || pad->right >= w)) return -200;
+    const long long ho = static_cast<long long>(h) + pad->top + pad->bottom;
+    const long long wo = static_cast<long long>(w) + pad->left + pad->right;
+    if (ho * wo > 0x7fffffffll) return -200;
+    *out = PlanePad{pad->top, pad->bottom, pad->left, pad->right, pad->type, pad->value};
+    *padded = (pad->top | pad->bottom | pad->left | pad->right) != 0;
+    return 0;
+}
+
+// InstanceNorm's input and padded output planes: float(S) is exact, and the per-CTA re-combination of a plane's partials
+// stays bounded (instance_norm.cu).
+static const long long kMaxNormPlane = 1ll << 24;
+
+int fcuda_instance_norm_workspace_size(int channels, size_t plane, int batch, size_t* floats) {
+    if (!floats || channels < 1 || plane == 0 || batch < 1) return -100;
+    *floats = instance_norm_workspace_floats(channels, plane, batch);
+    return 0;
+}
+
+int fcuda_instance_norm_forward(float* output, const float* input, int channels, int h, int w, const float* gamma,
+                                const float* beta, float eps, int relu, const FcudaPad* pad, float* workspace,
+                                int batch, void* stream) {
+    if (!output || !input || !workspace || !gamma != !beta || channels < 1 || h < 1 || w < 1 || batch < 1) return -100;
+    if (!(eps >= 0.f) || static_cast<long long>(h) * w > kMaxNormPlane) return -200;  // NaN eps fails >=
+    PlanePad pd;
+    int padded = 0;
+    if (plane_pad_check(pad, h, w, &pd, &padded)) return -200;
+    if (static_cast<long long>(h + pd.top + pd.bottom) * (w + pd.left + pd.right) > kMaxNormPlane) return -200;
+    if (padded && output == input) return -200;
+    return instance_norm_forward(input, output, channels, h, w, gamma, beta, eps, relu != 0, padded ? &pd : NULL,
+                                 workspace, batch, as_stream(stream));
+}
+
+int fcuda_padding_forward(float* output, const float* input, int channels, int h, int w, const FcudaPad* pad, int batch,
+                          void* stream) {
+    if (!output || !input || !pad || channels < 1 || h < 1 || w < 1 || batch < 1) return -100;
+    PlanePad pd;
+    int padded = 0;
+    if (static_cast<long long>(h) * w > 0x7fffffffll || plane_pad_check(pad, h, w, &pd, &padded)) return -200;
+    if (padded && output == input) return -200;
+    return padding_forward(input, output, channels, h, w, pd, batch, as_stream(stream));
 }
 
 int fcuda_lrn_forward(float* output, const float* input, int channels, int h, int w, int region_type, int local_size,

@@ -1,8 +1,8 @@
 // Built-in layer registrations: the 13 ncnn type names the reference serves (/root/reference/src/layer_factory.cpp:53-68)
 // plus Deconvolution / DeconvolutionDepthWise, Interp, Crop, Clip, PReLU, SSD's Permute, Flatten, Reshape, PriorBox and
 // DetectionOutput, VGG-SSD's Normalize, YOLO's YoloDetectionOutput and Yolov3DetectionOutput, ShuffleNet's ShuffleChannel
-// and Slice, AlexNet's and GoogLeNet's LRN, Faster R-CNN's Proposal and ROIPooling, and R-FCN's PSROIPooling, 33 in all,
-// mapped onto this
+// and Slice, AlexNet's and GoogLeNet's LRN, Faster R-CNN's Proposal and ROIPooling, R-FCN's PSROIPooling, and fast neural
+// style's InstanceNorm and Padding, 35 in all, mapped onto this
 // host's layer classes.  A table of {type name,
 // factory} pairs instead of one macro line per layer; the
 // DEFINE_LAYER_CREATOR / REGISTER_LAYER_CREATOR macros of <feather/layer_factory.h> remain the plugin API for user layers.
@@ -26,6 +26,7 @@
 #include "layers/resize_layers.h"
 #include "layers/route_layers.h"
 #include "layers/scale_layer.h"
+#include "layers/style_layers.h"
 #include "layers/yolo_layers.h"
 
 namespace feather {
@@ -79,6 +80,8 @@ const BuiltIn kBuiltIns[] = {
     {"Proposal", make_layer<ProposalLayer>},
     {"ROIPooling", make_layer<ROIPoolingLayer>},
     {"PSROIPooling", make_layer<PSROIPoolingLayer>},
+    {"InstanceNorm", make_layer<InstanceNormLayer>},
+    {"Padding", make_layer<PaddingLayer>},
 };
 
 }  // namespace

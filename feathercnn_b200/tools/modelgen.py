@@ -9,7 +9,8 @@ BN + Scale + ReLU as separate layers, Split/Eltwise residuals), MobileNet-v1, Mo
 AlexNet (BVLC's deploy nets, with LRN), plus a small "mini" net
 that exercises every layer type, single-shot detectors (MobileNet-SSD, VGG-SSD 300, a two-head tiny SSD), YOLO detectors
 (MobileNet-YOLOv2, MobileNet-v2 YOLOv3, a two-scale tiny YOLOv3), two-stage detectors (py-faster-rcnn's VGG-16 Faster
-R-CNN, py-R-FCN's ResNet-50 R-FCN and a tiny one of each) and ShuffleNet-v2 with a small routing probe net.  Weight
+R-CNN, py-R-FCN's ResNet-50 R-FCN and a tiny one of each), fast neural style transfer (TransformerNet, with a tiny
+one) and ShuffleNet-v2 with a small routing probe net.  Weight
 statistics follow SURVEY.md §8(d).
 """
 from __future__ import annotations
@@ -431,6 +432,30 @@ class ModelWriter:
                     {0: pooled_w, 1: pooled_h, 2: f"{spatial_scale:e}", 3: output_dim})
         self.shape[top] = (output_dim, pooled_h, pooled_w)
         return top
+
+    def instance_norm(self, name, bottom, eps=1e-5, affine=True, top=None):
+        """ncnn InstanceNorm 0=channels 1=eps 2=affine; with affine, gamma (uniform(0.8, 1.2)) then beta (uniform(-0.1,
+        0.1)), raw fp32 in the bin."""
+        top = top or name
+        c = self.shape[bottom][0]
+        self._layer("InstanceNorm", name, [bottom], [top], {0: c, 1: f"{eps:e}", 2: int(affine)})
+        if affine:
+            self._weights(self.rng.uniform(0.8, 1.2, c).astype(np.float32), False)
+            self._weights(self.rng.uniform(-0.1, 0.1, c).astype(np.float32), False)
+        self.shape[top] = self.shape[bottom]
+        return top
+
+    def padding(self, name, bottom, top, bottom_, left, right, type_=2, value=0.0):
+        """ncnn Padding 0=top 1=bottom 2=left 3=right 4=type (0 constant, 1 replicate, 2 reflect) 5=value (written when
+        not 0).  The output blob is `name`."""
+        c, h, w = self.shape[bottom]
+        assert type_ != 2 or (max(top, bottom_) < h and max(left, right) < w), (name, self.shape[bottom])
+        params = {0: top, 1: bottom_, 2: left, 3: right, 4: type_}
+        if value:
+            params[5] = f"{value:e}"
+        self._layer("Padding", name, [bottom], [name], params)
+        self.shape[name] = (c, h + top + bottom_, w + left + right)
+        return name
 
     def dropout(self, name, bottom, top=None, scale=None):
         top = top or name
@@ -1262,6 +1287,48 @@ def rfcn_tiny(seed=0, height=96, width=128, num_classes=5, pre_nms_top_n=2000, p
     return m
 
 
+def _style_conv(m: ModelWriter, name: str, x: str, oc: int, k: int, stride: int = 1) -> str:
+    """TransformerNet's ConvLayer: a reflect Padding of k // 2 on every side, then the convolution with pad 0."""
+    return m.conv(name, m.padding(name + "_pad", x, k // 2, k // 2, k // 2, k // 2), oc, k, stride, 0, True)
+
+
+def _transformer_net(m: ModelWriter, x: str, widths, blocks: int) -> str:
+    """The PyTorch examples' fast-neural-style TransformerNet on widths (w1, w2, w3): conv 9x9 3 -> w1, conv 3x3 / 2 to
+    w2 and to w3, `blocks` residual blocks (conv, IN, ReLU, conv, IN, then the Eltwise SUM skip), twice nearest x2
+    Interp, conv 3x3 and IN (w3 -> w2 -> w1), and a 9x9 w1 -> 3 output convolution.  Every convolution but the last is
+    followed by an affine InstanceNorm, and every InstanceNorm by a ReLU except the second of each residual block."""
+    w1, w2, w3 = widths
+    for i, (oc, k, s) in enumerate(((w1, 9, 1), (w2, 3, 2), (w3, 3, 2)), 1):
+        x = m.relu(f"relu{i}", m.instance_norm(f"in{i}", _style_conv(m, f"conv{i}", x, oc, k, s)))
+    for b in range(1, blocks + 1):
+        a, c = m.split(f"res{b}_split", x, [f"res{b}_in_a", f"res{b}_in_b"])
+        y = m.relu(f"res{b}_relu1", m.instance_norm(f"res{b}_in1", _style_conv(m, f"res{b}_conv1", c, w3, 3)))
+        y = m.instance_norm(f"res{b}_in2", _style_conv(m, f"res{b}_conv2", y, w3, 3))
+        x = m.eltwise(f"res{b}", [a, y])
+    for i, oc in ((4, w2), (5, w1)):
+        x = m.interp(f"up{i}", x, resize_type=1, scale=2.0)
+        x = m.relu(f"relu{i}", m.instance_norm(f"in{i}", _style_conv(m, f"conv{i}", x, oc, 3)))
+    return _style_conv(m, "conv6", x, 3, 9)
+
+
+def fast_neural_style(seed=0, height=512, width=512) -> ModelWriter:
+    """Johnson et al.'s fast neural style transfer network in the layout of the PyTorch examples' TransformerNet: 32,
+    64 and 128 channels, five residual blocks, nearest x2 upsampling.  The output (`conv6`) is shaped like the input."""
+    assert height % 4 == 0 and width % 4 == 0, (height, width)
+    m = ModelWriter(seed)
+    _transformer_net(m, m.input("data", 3, height, width), (32, 64, 128), 5)
+    return m
+
+
+def style_tiny(seed=0, height=32, width=32) -> ModelWriter:
+    """fast_neural_style's layout at float64-checkable size: 8, 16 and 16 channels, two residual blocks (the second
+    block's first Padding reads an Eltwise), both upsamples."""
+    assert height % 4 == 0 and width % 4 == 0, (height, width)
+    m = ModelWriter(seed)
+    _transformer_net(m, m.input("data", 3, height, width), (8, 16, 16), 2)
+    return m
+
+
 ZOO = {"single_conv": single_conv, "vgg16": vgg16, "resnet50": resnet50, "mobilenet_v1": mobilenet_v1, "mini": mini,
        "decoder_tiny": decoder_tiny, "fcn8s_tiny": fcn8s_tiny, "deeplab_head_tiny": deeplab_head_tiny,
        "mobilenet_v2": mobilenet_v2, "prelu_tiny": prelu_tiny, "mobilenet_ssd": mobilenet_ssd, "ssd_tiny": ssd_tiny,
@@ -1269,7 +1336,8 @@ ZOO = {"single_conv": single_conv, "vgg16": vgg16, "resnet50": resnet50, "mobile
        "mobilenet_yolov2": mobilenet_yolov2, "mobilenetv2_yolov3": mobilenetv2_yolov3, "yolo_tiny": yolo_tiny,
        "shufflenet_v2": shufflenet_v2, "shuffle_tiny": shuffle_tiny, "deeplabv3_mobilenet_v2": deeplabv3_mobilenet_v2,
        "deeplabv3_tiny": deeplabv3_tiny, "faster_rcnn_vgg16": faster_rcnn_vgg16, "faster_rcnn_tiny": faster_rcnn_tiny,
-       "rfcn_resnet50": rfcn_resnet50, "rfcn_tiny": rfcn_tiny}
+       "rfcn_resnet50": rfcn_resnet50, "rfcn_tiny": rfcn_tiny, "fast_neural_style": fast_neural_style,
+       "style_tiny": style_tiny}
 
 
 def synthetic_input(shape, index: int = 0) -> np.ndarray:

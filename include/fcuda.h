@@ -247,6 +247,61 @@ int fcuda_normalize_forward(float* output, const float* input, int channels, siz
  * output == input. */
 int fcuda_lrn_forward(float* output, const float* input, int channels, int h, int w, int region_type, int local_size,
                       float alpha, float beta, float bias, int batch, void* stream);
+/* A padding of each (n, c) plane (ncnn's Padding with front = behind = 0; PyTorch's ConstantPad2d, ReplicationPad2d and
+ * ReflectionPad2d): top / bottom rows and left / right columns added, all >= 0.  type 0 constant (`value`), 1 replicate
+ * (the edge element), 2 reflect (mirrored about the edge, the edge itself excluded: pads < the dimension they pad).
+ * Output element (oy, ox) of the (h + top + bottom) x (w + left + right) plane reads input row sy = src(oy, h, top) and
+ * column sx = src(ox, w, left), src(o, n, before) = i = o - before when 0 <= i < n, else: constant none (the element
+ * is `value`), replicate clamp(i, 0, n - 1), reflect -i when i < 0 and 2 (n - 1) - i when i >= n. */
+typedef struct FcudaPad {
+    int top, bottom, left, right;
+    int type;
+    float value;
+} FcudaPad;
+/* ncnn's InstanceNorm over (batch, channels, h, w) (PyTorch's InstanceNorm2d in eval without running statistics).  Per
+ * (n, c) plane of S = h * w floats, in fp32:
+ *   mean = sum(x) / S,  var = sum((x - mean)^2) / S  (biased; never E[x^2] - mean^2),
+ *   a = gamma[c] / sqrtf(var + eps), or 1 / sqrtf(var + eps) when gamma == beta == NULL (affine 0),
+ *   b = fmaf(-mean, a, beta[c]) (beta 0 without affine),
+ *   y = fmaf(x, a, b): one fused multiply-add, one rounding; then with `relu` y = fmaxf(y, 0.f) (the ReLU kernel's
+ *   expression, so a NaN y gives 0 there too); then, with a non-zero `pad`, the output plane is padded as
+ *   fcuda_padding_forward does: border elements are a * x_src + b (with the ReLU) of the element src() maps them to, and
+ *   constant borders are `value` with no ReLU.  So IN, then ReLU, then Padding as separate calls give the same bits.
+ * IEEE sqrtf and division.  S is converted to float (exact: S <= 2^24).
+ * Order (a plane's result depends on its own values only: the same bits for any batch split, pointer offset, in or out
+ * of place, eager or in a CUDA graph; the vector width and alignment change loads, never the order):
+ *   the plane is cut into chunks of 8192 floats (n_k the size of chunk k, K = ceil(S / 8192) chunks).  In a chunk,
+ *   thread t (0..255) adds its elements 4t + 1024j + q (j = 0..7 outer, q = 0..3 inner, those < n_k) in that order
+ *   from 0.f, a 32-lane xor-shuffle tree sums each warp and the eight warp partials are added in warp order: sum_k.
+ *   m_k = sum_k / n_k, and M2_k = sum of (x - m_k)^2 in the same order, each term one fmaf.  Then lane l (0..31) adds
+ *   sum_k for chunks k = l, l + 32, ... in order from 0.f and a 32-lane xor-shuffle tree gives the total: mean = total
+ *   / S; lane l adds fmaf(n_k d, d, M2_k) with d = sum_k / n_k - mean over the same chunks, a shuffle tree gives M2 and
+ *   var = M2 / S (Chan et al.'s combination).
+ * Error bound (first order; float64 quantities of the plane: mean mu, biased variance s2, X = max |x|, A = |a| with
+ * the exact mean and variance; U = 2^-24, D = 64 + ceil(K / 32)):
+ *   dmu = D U X,  V = (D + 8) U s2 + 4 D U X sqrt(s2) + 6 D^2 U^2 X^2,  rho = V / (s2 + eps) + 6 U,
+ *   |y - y64| <= A (rho |x - mu| + (1 + 2 rho) dmu) + U (|beta| + (1 + rho) A (|mu| + dmu) + |y64|)
+ * per element before the ReLU and the padding (which change no bound: fmaxf is non-expansive, padding copies).
+ * Two launches through `workspace` (fcuda_instance_norm_workspace_size floats: 2 per chunk of every plane, written
+ * before they are read), no atomics.  Launch 1 reads each chunk once into registers; launch 2 has one CTA per chunk of
+ * the output plane, reads its source elements again and writes them.  Stream-ordered: allocates and synchronises
+ * nothing.  In place (output == input) is allowed without a padding.
+ * Every launch-2 CTA re-reads its plane's K partials, so a plane costs K * K2 * 8 bytes of workspace reads (K2 the
+ * chunks of the output plane); the 2^24-float limits below keep that under 32 MB per plane.
+ * -100: a NULL output, input or workspace, exactly one of gamma / beta NULL, channels, h, w or batch < 1.  -200: a
+ * negative pad, a type outside 0..2, a reflect pad >= the dimension it pads, a negative or NaN eps, h * w or the padded
+ * plane over 2^24 floats, a non-zero pad with output == input.  `pad` NULL or all zero: no padding. */
+int fcuda_instance_norm_workspace_size(int channels, size_t plane, int batch, size_t* floats);
+int fcuda_instance_norm_forward(float* output, const float* input, int channels, int h, int w, const float* gamma,
+                                const float* beta, float eps, int relu, const FcudaPad* pad, float* workspace,
+                                int batch, void* stream);
+/* ncnn's Padding (front = behind = 0, one pad value) of each (n, c) plane: a pure copy through the index function of
+ * FcudaPad, bit-exact; coalesced stores, 16 bytes wide when the padded plane is a multiple of 4 floats and the
+ * pointers are 16-byte aligned.  In place (output == input) only with every pad 0.  -100: a NULL pointer (pad
+ * included), channels, h, w or batch < 1.  -200: a negative pad, a type outside 0..2, a reflect pad >= the dimension
+ * it pads, h * w or the padded plane over 2^31 - 1 floats, a non-zero pad with output == input. */
+int fcuda_padding_forward(float* output, const float* input, int channels, int h, int w, const FcudaPad* pad, int batch,
+                          void* stream);
 /* SoftmaxLayer::Forward (src/layers/softmax_layer.h:32-55): over each image's whole blob. */
 int fcuda_softmax_forward(float* output, const float* input, size_t n_per_image, int batch, void* stream);
 /* DropoutLayer::Forward (src/layers/dropout_layer.h:36-57): y = x*scale (copy when scale == 1). */
@@ -651,7 +706,8 @@ int fcuda_profile_collect(double* total_ms, double* algo_flops, double* mma_flop
  * kind 0 TensorGEMM, 1 implicit-GEMM conv, 2 Winograd input transform, 3 Winograd output transform, 4 pooling,
  * 5 depthwise, 6 element-wise (BN/Scale/Eltwise/Clip/PReLU/Normalize/LRN), 7 deconvolution scatter / depthwise gather, 8 resize / crop (Interp,
  * Crop), 9 detection (Permute, axis Softmax, PriorBox, decode, NMS, merge; YOLO decode, select, mask, sweep), 10 channel
- * routing (fcuda_route_forward), 11 two-stage detection (Proposal decode, select, mask, sweep; ROIPooling; PSROIPooling), < 0 all.  algo_bytes = the bytes the operation must move (inputs
+ * routing (fcuda_route_forward), 11 two-stage detection (Proposal decode, select, mask, sweep; ROIPooling; PSROIPooling),
+ * 12 instance normalisation / padding (InstanceNorm, Padding), < 0 all.  algo_bytes = the bytes the operation must move (inputs
  * read once + outputs written once). */
 int fcuda_profile_collect_kind(int kind, double* total_ms, double* algo_flops, double* mma_flops, double* algo_bytes,
                                long long* launches);
