@@ -257,6 +257,28 @@ def interp(x: torch.Tensor, out_h: int, out_w: int, mode: str = "bilinear", alig
     return out
 
 
+def pixel_shuffle(x: torch.Tensor, r: int, mode: int = 0, addend: torch.Tensor | None = None, addend_scale=None,
+                  out: torch.Tensor | None = None) -> torch.Tensor:
+    """ncnn PixelShuffle of x (N, C, H, W) to (N, C / r^2, H r, W r): mode 0 PyTorch's channel order, 1 ONNX
+    DepthToSpace DCR (include/fcuda.h).  With `addend` (N, C / r^2, h, w) its nearest Interp to the output size is added
+    in the same pass; `addend_scale` (a float or (h, w), ncnn's Interp scales) maps it, or by default the explicit
+    output size."""
+    n, c, h, w = x.shape
+    amap = None
+    if addend is not None:
+        ah, aw = addend.shape[2:]
+        amap = (interp_param(ah, aw, 0, 0, "nearest", scale=addend_scale) if addend_scale is not None
+                else interp_param(ah, aw, h * r, w * r, "nearest"))
+        addend = addend.contiguous()
+    oc = c // (r * r) if r > 0 else c
+    out = torch.empty((n, oc, h * r, w * r), device=x.device, dtype=torch.float32) if out is None else out
+    _check("fcuda_pixel_shuffle_forward",
+           fcuda().fcuda_pixel_shuffle_forward(_ptr(out), _ptr(x.contiguous()), c, h, w, r, mode,
+                                               _ptr(addend) if addend is not None else None,
+                                               ctypes.byref(amap) if amap is not None else None, n, _stream()))
+    return out
+
+
 def crop(x: torch.Tensor, coff: int, hoff: int, woff: int, oc: int, oh: int, ow: int) -> torch.Tensor:
     """out[n][c][y][x] = x[n][c + coff][y + hoff][x + woff], shape (N, oc, oh, ow)."""
     n, c, h, w = x.shape

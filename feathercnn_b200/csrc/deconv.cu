@@ -8,11 +8,17 @@
 // phases into the cropped output, adding the bias once and applying the ReLU.  Stride 1 needs no phases: the flipped
 // filter with dilation d and pads d*(K-1) - pad writes the output directly.  True depthwise layers have one input channel
 // per filter, too little work for the tensor cores, and run as a CUDA-core gather.
+//
+// The scatter with stride r, no pads, no bias and no ReLU is ncnn's PixelShuffle (fcuda_pixel_shuffle_forward), and its
+// ADD variant also adds a nearest-upsampled blob to each output: SRVGGNetCompact's tail, pixel_shuffle(conv) +
+// nearest_upsample(x), as one read of each input and one write of the output.
 #include "fcuda.h"
 
 #include "common.cuh"
 #include "deconv.cuh"
+#include "resize.cuh"
 
+#include <stdint.h>
 #include <string.h>
 
 #include <vector>
@@ -22,29 +28,82 @@ namespace fcuda {
 constexpr int kDeconvThreads = 256;
 constexpr int kDeconvMaxGridY = 65535;
 
+constexpr int kScatterVec = 4;  // consecutive outputs of one row per thread
+
+// One thread writes kScatterVec consecutive outputs of a row in every plane it visits: the row's phase ry, the columns'
+// phases, source offsets and validity are worked out once per thread, so a plane costs the thread one 32-bit division
+// (its group) and four independent loads before its stores.  Planes advance by gridDim.y with (n, oc) carried along,
+// so no 64-bit division runs on the device.  ADD: the PixelShuffle tail's nearest-upsampled addend (deconv.cuh).
+// VEC: OW % 4 == 0 and `out` 16-byte aligned, so the four outputs are one float4 store.
+template <bool ADD, bool VEC>
 __global__ void __launch_bounds__(kDeconvThreads)
 deconv_scatter_kernel(const float* __restrict__ P, const float* __restrict__ bias, float* __restrict__ out,
-                      DeconvScatterGeom g, int relu, long long planes) {
-    const int OHW = g.OH * g.OW;
-    const int idx = blockIdx.x * kDeconvThreads + threadIdx.x;
-    if (idx >= OHW) return;
-    const int oy = idx / g.OW, ox = idx - oy * g.OW;
-    const int Y = oy + g.pad_top, X = ox + g.pad_left;
+                      DeconvScatterGeom g, int relu, long long planes, ScatterAddend a) {
+    const int groups = (g.OW + kScatterVec - 1) / kScatterVec;  // per output row
+    const int item = blockIdx.x * kDeconvThreads + threadIdx.x;
+    if (item >= g.OH * groups) return;
+    const int oy = item / groups, ox0 = (item - oy * groups) * kScatterVec;
+    const int Y = oy + g.pad_top;
     const int ty = Y / g.stride_h, ry = Y - ty * g.stride_h;
-    const int tx = X / g.stride_w, rx = X - tx * g.stride_w;
-    const bool inside = ty < g.Hc && tx < g.Wc;
     const int OCg = g.OC / g.group;
     const int OCp = g.OC * g.stride_h * g.stride_w;
     const size_t pc = static_cast<size_t>(g.Hc) * g.Wc;
+    size_t off[kScatterVec];  // source offset of each output within its phase row: rx * OCg * pc + tx
+    bool in[kScatterVec];     // a source element exists (0 in its place otherwise) and the output is inside the row
+    bool col[kScatterVec];    // the output is inside the row
+    int sx[kScatterVec];      // the addend's source column (the nearest Interp's map)
+    {
+        const int X = ox0 + g.pad_left;
+        int tx = X / g.stride_w, rx = X - tx * g.stride_w;
+#pragma unroll
+        for (int k = 0; k < kScatterVec; ++k) {
+            col[k] = VEC || ox0 + k < g.OW;
+            in[k] = col[k] && ty < g.Hc && tx < g.Wc;
+            off[k] = static_cast<size_t>(rx) * OCg * pc + tx;
+            if constexpr (ADD) sx[k] = nearest_coord(ox0 + k, a.W, a.scale_w);
+            if (++rx == g.stride_w) {
+                rx = 0;
+                ++tx;
+            }
+        }
+    }
+    const int sy = ADD ? nearest_coord(oy, a.H, a.scale_h) : 0;
+    const size_t src_row = static_cast<size_t>(ty) * g.Wc;
+    const size_t OHW = static_cast<size_t>(g.OH) * g.OW;
+    const int step_n = gridDim.y / g.OC, step_oc = gridDim.y - step_n * g.OC;
+    long long n = blockIdx.y / g.OC;
+    int oc = blockIdx.y - static_cast<int>(n) * g.OC;
     for (long long plane = blockIdx.y; plane < planes; plane += gridDim.y) {  // plane = n * OC + oc
-        const long long n = plane / g.OC;
-        const int oc = static_cast<int>(plane - n * g.OC);
         const int grp = oc / OCg, ocg = oc - grp * OCg;
-        const int ch = ((grp * g.stride_h + ry) * g.stride_w + rx) * OCg + ocg;
-        float v = inside ? __ldg(P + (static_cast<size_t>(n) * OCp + ch) * pc + static_cast<size_t>(ty) * g.Wc + tx) : 0.f;
-        if (bias) v += __ldg(bias + oc);
-        if (relu) v = v > 0 ? v : 0.f;  // the ReLU layer's comparison (layers.cu scale_relu_kernel)
-        out[static_cast<size_t>(plane) * OHW + idx] = v;
+        const float* src = P + (static_cast<size_t>(n) * OCp + static_cast<size_t>(grp * g.stride_h + ry) * g.stride_w * OCg +
+                                ocg) * pc + src_row;
+        float v[kScatterVec];
+#pragma unroll
+        for (int k = 0; k < kScatterVec; ++k) v[k] = in[k] ? __ldg(src + off[k]) : 0.f;
+        const float b = bias ? __ldg(bias + oc) : 0.f;
+        const float* base = ADD ? a.base + (static_cast<size_t>(plane) * a.H + sy) * a.W : nullptr;
+#pragma unroll
+        for (int k = 0; k < kScatterVec; ++k) {
+            if (bias) v[k] += b;
+            if (relu) v[k] = v[k] > 0 ? v[k] : 0.f;  // the ReLU layer's comparison (layers.cu scale_relu_kernel)
+            if constexpr (ADD) {
+                if (col[k]) v[k] += __ldg(base + sx[k]);
+            }
+        }
+        float* dst = out + static_cast<size_t>(plane) * OHW + static_cast<size_t>(oy) * g.OW + ox0;
+        if constexpr (VEC) {
+            *reinterpret_cast<float4*>(dst) = make_float4(v[0], v[1], v[2], v[3]);
+        } else {
+#pragma unroll
+            for (int k = 0; k < kScatterVec; ++k)
+                if (col[k]) dst[k] = v[k];
+        }
+        oc += step_oc;
+        n += step_n;
+        if (oc >= g.OC) {
+            oc -= g.OC;
+            ++n;
+        }
     }
 }
 
@@ -89,13 +148,20 @@ static dim3 plane_grid(int per_plane, long long planes) {
                 static_cast<unsigned>(planes < kDeconvMaxGridY ? planes : kDeconvMaxGridY));
 }
 
-int deconv_scatter(const float* P, const float* bias, float* out, const DeconvScatterGeom& g, int relu, int batch,
-                   cudaStream_t s) {
+int deconv_scatter(const float* P, const float* bias, float* out, const DeconvScatterGeom& g, int relu,
+                   const ScatterAddend* add, int kind, int batch, cudaStream_t s) {
     const long long planes = static_cast<long long>(batch) * g.OC;
     const double out_n = static_cast<double>(planes) * g.OH * g.OW;
     const double p_n = static_cast<double>(batch) * g.OC * g.stride_h * g.stride_w * g.Hc * g.Wc;
-    const int prof = prof_begin(s, PROF_DECONV, 0, 0, 4.0 * (out_n + p_n));
-    deconv_scatter_kernel<<<plane_grid(g.OH * g.OW, planes), kDeconvThreads, 0, s>>>(P, bias, out, g, relu, planes);
+    const double add_n = add ? static_cast<double>(planes) * add->H * add->W : 0.0;
+    const int prof = prof_begin(s, kind, 0, 0, 4.0 * (out_n + p_n + add_n));
+    const dim3 grid = plane_grid(g.OH * ceil_div(g.OW, kScatterVec), planes);
+    const bool vec = g.OW % kScatterVec == 0 && (reinterpret_cast<uintptr_t>(out) & 15) == 0;
+    const ScatterAddend a = add ? *add : ScatterAddend{};
+    if (add && vec) deconv_scatter_kernel<true, true><<<grid, kDeconvThreads, 0, s>>>(P, bias, out, g, relu, planes, a);
+    else if (add) deconv_scatter_kernel<true, false><<<grid, kDeconvThreads, 0, s>>>(P, bias, out, g, relu, planes, a);
+    else if (vec) deconv_scatter_kernel<false, true><<<grid, kDeconvThreads, 0, s>>>(P, bias, out, g, relu, planes, a);
+    else deconv_scatter_kernel<false, false><<<grid, kDeconvThreads, 0, s>>>(P, bias, out, g, relu, planes, a);
     prof_end(prof, s);
     FCUDA_CHECK_LAUNCH();
     count_launch();
@@ -368,7 +434,7 @@ int fcuda_deconv_forward(const FcudaDeconvParam* p, float* output, const float* 
     g.OC = q.output_channels; g.group = q.group; g.stride_h = q.stride_h; g.stride_w = q.stride_w;
     g.Hc = pl.eq.output_h; g.Wc = pl.eq.output_w; g.OH = q.output_h; g.OW = q.output_w;
     g.pad_top = q.pad_top; g.pad_left = q.pad_left;
-    return deconv_scatter(P, b, output, g, relu, batch, s);
+    return deconv_scatter(P, b, output, g, relu, nullptr, PROF_DECONV, batch, s);
 }
 
 }  // extern "C"

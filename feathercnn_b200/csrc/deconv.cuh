@@ -7,8 +7,16 @@ namespace fcuda {
 struct DeconvScatterGeom {
     int OC, group, stride_h, stride_w, Hc, Wc, OH, OW, pad_top, pad_left;
 };
-int deconv_scatter(const float* P, const float* bias, float* out, const DeconvScatterGeom& g, int relu, int batch,
-                   cudaStream_t s);
+// With `add` (the PixelShuffle tail), the scatter then adds add.base[n][oc][nearest_coord(oy, H, scale_h)]
+// [nearest_coord(ox, W, scale_w)], one fp32 add, as a nearest Interp of base followed by an Eltwise SUM.  `kind` is
+// the profiling kind the launch is counted under.
+struct ScatterAddend {
+    const float* base;
+    int H, W;
+    float scale_h, scale_w;
+};
+int deconv_scatter(const float* P, const float* bias, float* out, const DeconvScatterGeom& g, int relu,
+                   const ScatterAddend* add, int kind, int batch, cudaStream_t s);
 
 // Depthwise deconvolution (one filter per channel, w is (C, KH, KW)): every output gathers its taps in ascending
 // (ky, kx) order with fp32 FMAs, starting from the bias; stride > 1 and dilation > 1 never share a direction.

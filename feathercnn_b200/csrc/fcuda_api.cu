@@ -6,6 +6,7 @@
 #include "common.cuh"
 #include "conv_direct.cuh"
 #include "conv_igemm.cuh"
+#include "deconv.cuh"
 #include "depthwise.cuh"
 #include "detection.cuh"
 #include "instance_norm.cuh"
@@ -932,6 +933,33 @@ int fcuda_interp_forward(const FcudaInterpParam* param, float* output, const flo
     g.scale_h = interp_scale(p, p.input_h, p.output_h, p.output_height, p.height_scale);
     g.scale_w = interp_scale(p, p.input_w, p.output_w, p.output_width, p.width_scale);
     return interp_forward(input, output, g, static_cast<long long>(batch) * channels, as_stream(stream));
+}
+
+int fcuda_pixel_shuffle_forward(float* output, const float* input, int channels, int h, int w, int r, int mode,
+                                const float* addend, const FcudaInterpParam* addend_map, int batch, void* stream) {
+    if (!output || !input || (addend && !addend_map) || channels < 1 || h < 1 || w < 1 || batch < 1) return -100;
+    if (r < 1 || (mode != 0 && mode != 1) || static_cast<long long>(r) * r > channels || channels % (r * r)) return -200;
+    const long long oh = static_cast<long long>(h) * r, ow = static_cast<long long>(w) * r;
+    if (oh * ow > 0x7fffffffLL || output == input || (addend && output == addend)) return -200;
+    const int oc = channels / (r * r);
+    ScatterAddend add{};
+    if (addend) {
+        FcudaInterpParam p = *addend_map;
+        if (p.resize_type != 1) return -200;
+        const int rc = interp_check_and_size(&p);
+        if (rc) return rc;
+        if (p.output_h != oh || p.output_w != ow) return -200;
+        add = ScatterAddend{addend, p.input_h, p.input_w, interp_scale(p, p.input_h, p.output_h, p.output_height,
+                                                                      p.height_scale),
+                            interp_scale(p, p.input_w, p.output_w, p.output_width, p.width_scale)};
+    }
+    // the sub-pixel scatter of a deconvolution with stride r and no pads, bias or ReLU; mode 0 is group = OC (channel
+    // p * r^2 + i * r + j), mode 1 group = 1 (channel (i * r + j) * OC + p)
+    DeconvScatterGeom g;
+    g.OC = oc; g.group = mode == 0 ? oc : 1; g.stride_h = g.stride_w = r;
+    g.Hc = h; g.Wc = w; g.OH = static_cast<int>(oh); g.OW = static_cast<int>(ow); g.pad_top = g.pad_left = 0;
+    return deconv_scatter(input, nullptr, output, g, 0, addend ? &add : nullptr, PROF_PIXEL_SHUFFLE, batch,
+                          as_stream(stream));
 }
 
 int fcuda_crop_forward(float* output, const float* input, int channels, int in_h, int in_w, int coff, int hoff, int woff,

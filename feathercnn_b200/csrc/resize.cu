@@ -30,11 +30,6 @@ __device__ __forceinline__ void bilinear_coord(int d, int in, float scale, int a
     a = f - static_cast<float>(i0);
 }
 
-// ncnn's nearest index: min((int)(d * scale), in - 1) with the fp32 product
-__device__ __forceinline__ int nearest_coord(int d, int in, float scale) {
-    return min(static_cast<int>(__fmul_rn(static_cast<float>(d), scale)), in - 1);
-}
-
 template <int MODE, bool VEC>  // MODE 1 nearest, 2 bilinear; VEC: 4 outputs per thread, one float4 store
 __global__ void __launch_bounds__(kResizeThreads)
 interp_kernel(const float* __restrict__ in, float* __restrict__ out, InterpGeom g, int band, long long planes) {

@@ -11,6 +11,12 @@ struct InterpGeom {
 };
 int interp_forward(const float* in, float* out, const InterpGeom& g, long long planes, cudaStream_t s);
 
+// ncnn's nearest index: min((int)(d * scale), in - 1) with the fp32 product.  Shared by Interp and the PixelShuffle
+// tail that adds a nearest-upsampled blob (deconv.cu), so both read the same source element.
+__device__ __forceinline__ int nearest_coord(int d, int in, float scale) {
+    return min(static_cast<int>(__fmul_rn(static_cast<float>(d), scale)), in - 1);
+}
+
 // out[n][c][y][x] = in[n][c + coff][y + hoff][x + woff] for an out_c x out_h x out_w window of each image.
 struct CropGeom {
     int C, H, W, coff, hoff, woff, OC, OH, OW;

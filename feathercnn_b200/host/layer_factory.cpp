@@ -1,8 +1,8 @@
 // Built-in layer registrations: the 13 ncnn type names the reference serves (/root/reference/src/layer_factory.cpp:53-68)
 // plus Deconvolution / DeconvolutionDepthWise, Interp, Crop, Clip, PReLU, SSD's Permute, Flatten, Reshape, PriorBox and
 // DetectionOutput, VGG-SSD's Normalize, YOLO's YoloDetectionOutput and Yolov3DetectionOutput, ShuffleNet's ShuffleChannel
-// and Slice, AlexNet's and GoogLeNet's LRN, Faster R-CNN's Proposal and ROIPooling, R-FCN's PSROIPooling, and fast neural
-// style's InstanceNorm and Padding, 35 in all, mapped onto this
+// and Slice, AlexNet's and GoogLeNet's LRN, Faster R-CNN's Proposal and ROIPooling, R-FCN's PSROIPooling, fast neural
+// style's InstanceNorm and Padding, and super-resolution's PixelShuffle, 36 in all, mapped onto this
 // host's layer classes.  A table of {type name,
 // factory} pairs instead of one macro line per layer; the
 // DEFINE_LAYER_CREATOR / REGISTER_LAYER_CREATOR macros of <feather/layer_factory.h> remain the plugin API for user layers.
@@ -20,6 +20,7 @@
 #include "layers/lrn_layer.h"
 #include "layers/misc_layers.h"
 #include "layers/normalize_layer.h"
+#include "layers/pixel_shuffle_layer.h"
 #include "layers/pooling_layer.h"
 #include "layers/rcnn_layers.h"
 #include "layers/relu_layer.h"
@@ -82,6 +83,7 @@ const BuiltIn kBuiltIns[] = {
     {"PSROIPooling", make_layer<PSROIPoolingLayer>},
     {"InstanceNorm", make_layer<InstanceNormLayer>},
     {"Padding", make_layer<PaddingLayer>},
+    {"PixelShuffle", make_layer<PixelShuffleLayer>},
 };
 
 }  // namespace

@@ -52,6 +52,9 @@ public:
                                     static_cast<int>(bottom->num()), stream());
     }
 
+    // ncnn's parameters; input_h / input_w and the output size are those of the last Reshape
+    const FcudaInterpParam& interp_param() const { return param; }
+
 private:
     FcudaInterpParam param;
 };

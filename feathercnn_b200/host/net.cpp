@@ -15,6 +15,7 @@
 #include "layers/deconv_layer.h"
 #include "layers/eltwise_layer.h"
 #include "layers/misc_layers.h"
+#include "layers/pixel_shuffle_layer.h"
 #include "layers/resize_layers.h"
 #include "layers/route_layers.h"
 
@@ -604,6 +605,46 @@ int Net::ApplyFusion() {
         c->tops.clear();
         c->bottoms.clear();
         c->_fused_away = true;
+    }
+    // Super-resolution tail pass (ahead of the routing pass, which ends early when its tuning switch is off): a plain
+    // two-input Eltwise SUM of a PixelShuffle's top and a nearest Interp's top, each read only by the Eltwise, becomes
+    // the PixelShuffle's tail (SRVGGNetCompact's out = pixel_shuffle(conv) + nearest_upsample(x): two full-size blobs
+    // neither written nor read back).  Like the residual addend, the Interp's input must already exist when the
+    // PixelShuffle runs.
+    for (size_t j = 0; j < layers.size(); ++j) {
+        EltwiseLayer* e = dynamic_cast<EltwiseLayer*>(layers[j]);
+        if (!e || e->_fused_away || e->bottoms.size() != 2 || e->tops.size() != 1 || !e->plain_sum() || e->fused_relu())
+            continue;
+        for (int k = 0; k < 2; ++k) {
+            Blob<float>* mine = e->bottoms[k];
+            Blob<float>* other = e->bottoms[1 - k];
+            if (mine == other || readers[mine] != 1 || readers[other] != 1 || !producer.count(mine) ||
+                !producer.count(other))
+                continue;
+            const size_t i = producer[mine], m = producer[other];
+            PixelShuffleLayer* ps = dynamic_cast<PixelShuffleLayer*>(layers[i]);
+            InterpLayer* up = dynamic_cast<InterpLayer*>(layers[m]);
+            if (!ps || !up || i >= j || m >= j || ps->_fused_away || up->_fused_away || ps->tops.size() != 1 ||
+                up->tops.size() != 1 || up->bottoms.size() != 1)
+                continue;
+            Blob<float>* base = up->bottoms[0];
+            if (producer.count(base) && producer[base] >= i) continue;  // not computed yet when the PixelShuffle runs
+            if (ps->FuseUpsampledAdd(up->interp_param(), base) != 1) continue;
+            for (Blob<float>* dead : {mine, other}) {
+                blob_map.erase(dead->name);
+                producer.erase(dead);
+                delete dead;
+            }
+            ps->tops[0] = e->tops[0];
+            producer[ps->tops[0]] = i;
+            up->tops.clear();
+            up->bottoms.clear();
+            up->_fused_away = true;
+            e->tops.clear();
+            e->bottoms.clear();
+            e->_fused_away = true;
+            break;
+        }
     }
     // Fourth pass: channel routing.  Concat (axis 0) -> ShuffleChannel -> Slice (axis 0), or any two adjacent of them,
     // run as one fcuda_route_forward launch by the chain's last layer (ShuffleNet-v2 units: one read and one write of

@@ -10,7 +10,8 @@ AlexNet (BVLC's deploy nets, with LRN), plus a small "mini" net
 that exercises every layer type, single-shot detectors (MobileNet-SSD, VGG-SSD 300, a two-head tiny SSD), YOLO detectors
 (MobileNet-YOLOv2, MobileNet-v2 YOLOv3, a two-scale tiny YOLOv3), two-stage detectors (py-faster-rcnn's VGG-16 Faster
 R-CNN, py-R-FCN's ResNet-50 R-FCN and a tiny one of each), fast neural style transfer (TransformerNet, with a tiny
-one) and ShuffleNet-v2 with a small routing probe net.  Weight
+one), super-resolution (Real-ESRGAN's SRVGGNetCompact and EDSR baseline, with a tiny PixelShuffle net) and ShuffleNet-v2
+with a small routing probe net.  Weight
 statistics follow SURVEY.md §8(d).
 """
 from __future__ import annotations
@@ -480,6 +481,29 @@ class ModelWriter:
         else:  # fp32 products, truncated (fcuda_interp_output_dim)
             s = np.float32(1.0 if scale is None else scale)
             self.shape[top] = (c, int(np.float32(h) * s), int(np.float32(w) * s))
+        return top
+
+    def pixel_shuffle(self, name, bottom, r, mode=0, top=None):
+        """ncnn PixelShuffle 0=upscale_factor 1=mode (0 PyTorch's channel order, 1 DepthToSpace DCR; written when 1)."""
+        top = top or name
+        c, h, w = self.shape[bottom]
+        assert c % (r * r) == 0, (name, self.shape[bottom], r)
+        self._layer("PixelShuffle", name, [bottom], [top], {0: r, 1: mode} if mode else {0: r})
+        self.shape[top] = (c // (r * r), h * r, w * r)
+        return top
+
+    def fixed_conv1x1(self, name, bottom, weights, bias, top=None):
+        """A 1x1 Convolution with the given (oc, ic) weights and oc biases (EDSR's MeanShift)."""
+        top = top or name
+        wts = np.ascontiguousarray(weights, np.float32)
+        oc, ic = wts.shape
+        c, h, w = self.shape[bottom]
+        assert ic == c, (name, self.shape[bottom])
+        self._layer("Convolution", name, [bottom], [top], {0: oc, 1: 1, 3: 1, 4: 0, 5: 1, 6: wts.size})
+        self._weights(wts, True)
+        self._weights(np.asarray(bias, np.float32).reshape(oc), False)
+        self.shape[top] = (oc, h, w)
+        self.flops += 2.0 * oc * ic * h * w
         return top
 
     def crop(self, name, bottom, woff=0, hoff=0, reference=None, coff=0, outc=0, outh=0, outw=0, top=None):
@@ -1329,6 +1353,73 @@ def style_tiny(seed=0, height=32, width=32) -> ModelWriter:
     return m
 
 
+def srvgg_compact(seed=0, scale=4, num_conv=16, num_feat=64, height=270, width=480) -> ModelWriter:
+    """Real-ESRGAN's SRVGGNetCompact (basicsr): conv 3 -> num_feat and PReLU, num_conv x (conv num_feat -> num_feat,
+    PReLU), conv num_feat -> 3 scale^2 and PixelShuffle(scale), plus the input upsampled by a nearest Interp x scale,
+    added by an Eltwise SUM.  The defaults are realesr-animevideov3; num_conv=32 gives realesr-general-x4v3.  The output
+    (`output`) is (3, height * scale, width * scale)."""
+    m = ModelWriter(seed)
+    x, skip = m.split("data_split", m.input("data", 3, height, width), ["data_body", "data_skip"])
+    x = m.prelu("prelu0", m.conv("conv0", x, num_feat, 3, 1, 1), slopes=np.full(num_feat, 0.25))
+    for i in range(1, num_conv + 1):
+        x = m.prelu(f"prelu{i}", m.conv(f"conv{i}", x, num_feat, 3, 1, 1), slopes=np.full(num_feat, 0.25))
+    x = m.pixel_shuffle("upsample", m.conv("conv_last", x, 3 * scale * scale, 3, 1, 1), scale)
+    base = m.interp("base", skip, resize_type=1, scale=float(scale))
+    m.eltwise("output", [x, base])
+    return m
+
+
+EDSR_RGB_MEAN = (0.4488, 0.4371, 0.4040)
+
+
+def _edsr_upsampler(m: ModelWriter, x: str, scale: int, n_feats: int) -> str:
+    """EDSR's Upsampler: log2(scale) x (conv n_feats -> 4 n_feats, PixelShuffle 2) for 2, 4, 8; conv to 9 n_feats and
+    PixelShuffle 3 for 3."""
+    if scale == 3:
+        return m.pixel_shuffle("up_shuffle1", m.conv("up_conv1", x, 9 * n_feats, 3, 1, 1), 3)
+    assert scale in (2, 4, 8), scale
+    for i in range(1, int(math.log2(scale)) + 1):
+        x = m.pixel_shuffle(f"up_shuffle{i}", m.conv(f"up_conv{i}", x, 4 * n_feats, 3, 1, 1), 2)
+    return x
+
+
+def edsr_baseline(seed=0, scale=4, n_resblocks=16, n_feats=64, height=270, width=480, rgb_range=255.0,
+                  res_gain=0.1) -> ModelWriter:
+    """EDSR baseline (Lim et al. 2017): MeanShift (sub_mean) as a fixed 1x1 convolution, the head conv 3 -> n_feats,
+    n_resblocks x (conv, ReLU, conv, + skip), a conv plus the global skip, the upsampler (_edsr_upsampler), the tail conv
+    n_feats -> 3 and add_mean.  Each residual block's second convolution draws its weights at res_gain times He init, so
+    the activations stay in range over depth as trained weights keep them.  The output (`add_mean`) is
+    (3, height * scale, width * scale)."""
+    m = ModelWriter(seed)
+    mean = rgb_range * np.asarray(EDSR_RGB_MEAN)
+    x = m.fixed_conv1x1("sub_mean", m.input("data", 3, height, width), np.eye(3), -mean)
+    x, head = m.split("head_split", m.conv("head", x, n_feats, 3, 1, 1), ["body_in", "head_skip"])
+    for b in range(1, n_resblocks + 1):
+        a, c = m.split(f"res{b}_split", x, [f"res{b}_in", f"res{b}_skip"])
+        y = m.relu(f"res{b}_relu", m.conv(f"res{b}_conv1", a, n_feats, 3, 1, 1))
+        y = m.conv(f"res{b}_conv2", y, n_feats, 3, 1, 1, gain=res_gain * np.sqrt(2.0 / (9 * n_feats)))
+        x = m.eltwise(f"res{b}", [c, y])
+    x = m.eltwise("body", [head, m.conv("body_conv", x, n_feats, 3, 1, 1)])
+    x = m.conv("tail", _edsr_upsampler(m, x, scale, n_feats), 3, 3, 1, 1)
+    m.fixed_conv1x1("add_mean", x, np.eye(3), mean)
+    return m
+
+
+def sr_tiny(seed=0, height=9, width=11) -> ModelWriter:
+    """PixelShuffle at float64-checkable size, odd height and width: conv 3 -> 8 and PReLU, conv to 32 and PixelShuffle 2
+    in mode 1 (DepthToSpace DCR) feeding conv 8 -> 27, PixelShuffle 3 in mode 0, and SRVGGNetCompact's tail: the input
+    upsampled x 6 by a nearest Interp and added by an Eltwise SUM, which fuses into the second PixelShuffle.  The output
+    (`output`) is (3, 6 height, 6 width)."""
+    m = ModelWriter(seed)
+    x, skip = m.split("data_split", m.input("data", 3, height, width), ["data_body", "data_skip"])
+    x = m.prelu("prelu0", m.conv("conv0", x, 8, 3, 1, 1))
+    x = m.pixel_shuffle("shuffle1", m.conv("conv1", x, 32, 3, 1, 1), 2, mode=1)
+    x = m.pixel_shuffle("shuffle2", m.conv("conv2", x, 27, 3, 1, 1), 3)
+    base = m.interp("base", skip, resize_type=1, scale=6.0)
+    m.eltwise("output", [x, base])
+    return m
+
+
 ZOO = {"single_conv": single_conv, "vgg16": vgg16, "resnet50": resnet50, "mobilenet_v1": mobilenet_v1, "mini": mini,
        "decoder_tiny": decoder_tiny, "fcn8s_tiny": fcn8s_tiny, "deeplab_head_tiny": deeplab_head_tiny,
        "mobilenet_v2": mobilenet_v2, "prelu_tiny": prelu_tiny, "mobilenet_ssd": mobilenet_ssd, "ssd_tiny": ssd_tiny,
@@ -1337,7 +1428,7 @@ ZOO = {"single_conv": single_conv, "vgg16": vgg16, "resnet50": resnet50, "mobile
        "shufflenet_v2": shufflenet_v2, "shuffle_tiny": shuffle_tiny, "deeplabv3_mobilenet_v2": deeplabv3_mobilenet_v2,
        "deeplabv3_tiny": deeplabv3_tiny, "faster_rcnn_vgg16": faster_rcnn_vgg16, "faster_rcnn_tiny": faster_rcnn_tiny,
        "rfcn_resnet50": rfcn_resnet50, "rfcn_tiny": rfcn_tiny, "fast_neural_style": fast_neural_style,
-       "style_tiny": style_tiny}
+       "style_tiny": style_tiny, "srvgg_compact": srvgg_compact, "edsr_baseline": edsr_baseline, "sr_tiny": sr_tiny}
 
 
 def synthetic_input(shape, index: int = 0) -> np.ndarray:

@@ -428,6 +428,25 @@ int fcuda_interp_output_dim(FcudaInterpParam* param);
 /* output <- input for `channels` planes of each of `batch` images.  Allocates nothing and does not synchronise. */
 int fcuda_interp_forward(const FcudaInterpParam* param, float* output, const float* input, int channels, int batch,
                          void* stream);
+/* ncnn's PixelShuffle (sub-pixel convolution upsampling; the reference has no such layer): input (batch, C, h, w) ->
+ * output (batch, C / r^2, h * r, w * r), with OC = C / r^2 and output element (p, y, x), y = h' * r + i, x = w' * r + j
+ * (0 <= i, j < r), read from input channel
+ *   mode 0:  q = p * r^2 + i * r + j      (PyTorch's nn.PixelShuffle, ONNX DepthToSpace CRD)
+ *   mode 1:  q = (i * r + j) * OC + p     (ONNX DepthToSpace DCR, TensorFlow's depth_to_space)
+ * at (h', w').  Without an addend this is a pure copy, bit-exact, NaN payloads included.
+ * With `addend` (batch, OC, addend_map->input_h, addend_map->input_w), each output element becomes
+ *   out = shuffled + addend[n][p][min((int)(y * hs), input_h - 1)][min((int)(x * ws), input_w - 1)],
+ * one fp32 add (round to nearest), hs / ws the fp32 scales fcuda_interp_forward derives from `addend_map`: the bits of
+ * PixelShuffle, then a nearest Interp of the addend, then an Eltwise SUM of the two (fp32 addition commutes, so either
+ * bottom order), as three calls.  A NaN sum is the canonical NaN, as the Eltwise kernel writes it.
+ * One launch through the deconvolution's sub-pixel scatter kernel (profiling kind 13); it reads the input and the
+ * addend once and writes the output once.  Allocates nothing and does not synchronise.
+ * -100: a NULL output or input, an addend without addend_map, C, h, w or batch < 1, or an addend_map that
+ * fcuda_interp_output_dim rejects with -100.  -200: r < 1, mode other than 0 or 1, C % r^2 != 0, an output plane over
+ * 2^31 - 1 floats, output == input or output == addend, an addend_map that is not nearest (resize_type 1) or whose
+ * output size is not (h * r, w * r). */
+int fcuda_pixel_shuffle_forward(float* output, const float* input, int channels, int h, int w, int r, int mode,
+                                const float* addend, const FcudaInterpParam* addend_map, int batch, void* stream);
 /* ncnn / Caffe Crop: output (batch, out_c, out_h, out_w)[n][c][y][x] = input (batch, channels, in_h, in_w)
  * [n][c + coff][y + hoff][x + woff].  -100 for empty sizes, a negative offset or a window outside the input.  Allocates
  * nothing and does not synchronise. */
@@ -707,7 +726,8 @@ int fcuda_profile_collect(double* total_ms, double* algo_flops, double* mma_flop
  * 5 depthwise, 6 element-wise (BN/Scale/Eltwise/Clip/PReLU/Normalize/LRN), 7 deconvolution scatter / depthwise gather, 8 resize / crop (Interp,
  * Crop), 9 detection (Permute, axis Softmax, PriorBox, decode, NMS, merge; YOLO decode, select, mask, sweep), 10 channel
  * routing (fcuda_route_forward), 11 two-stage detection (Proposal decode, select, mask, sweep; ROIPooling; PSROIPooling),
- * 12 instance normalisation / padding (InstanceNorm, Padding), < 0 all.  algo_bytes = the bytes the operation must move (inputs
+ * 12 instance normalisation / padding (InstanceNorm, Padding), 13 pixel shuffle (PixelShuffle, alone or with its fused
+ * upsampled-input add), < 0 all.  algo_bytes = the bytes the operation must move (inputs
  * read once + outputs written once). */
 int fcuda_profile_collect_kind(int kind, double* total_ms, double* algo_flops, double* mma_flops, double* algo_bytes,
                                long long* launches);
