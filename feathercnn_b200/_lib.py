@@ -148,6 +148,8 @@ def fcuda() -> ctypes.CDLL:
             "fcuda_interp_forward": (i, [R, vp, vp, i, i, vp]),
             "fcuda_crop_forward": (i, [vp, vp] + [i] * 10 + [vp]),
             "fcuda_pixel_shuffle_forward": (i, [vp, vp, i, i, i, i, i, vp, R, i, vp]),
+            "fcuda_binary_op_shape": (i, [i, ctypes.POINTER(i), i] + [ctypes.POINTER(i)] * 5),
+            "fcuda_binary_op_forward": (i, [vp, vp, ctypes.POINTER(i), vp, ctypes.POINTER(i), f, i, i, vp]),
             "fcuda_deconv_output_dim": (i, [D]),
             "fcuda_deconv_plan": (i, [D, P, ctypes.POINTER(i)]),
             "fcuda_deconv_get_buffer_size": (i, [D, i, szp, szp]),

@@ -279,6 +279,34 @@ def pixel_shuffle(x: torch.Tensor, r: int, mode: int = 0, addend: torch.Tensor |
     return out
 
 
+BINARY_OPS = ["ADD", "SUB", "MUL", "DIV", "MAX", "MIN", "POW", "RSUB", "RDIV", "RPOW", "ATAN2", "RATAN2"]  # FcudaBinaryOp
+
+
+def binary_op_shape(a_rank: int, a_shape, b_rank: int, b_shape):
+    """fcuda_binary_op_shape for two images of ncnn ranks a_rank, b_rank stored as (c, h, w): (output rank, output
+    (c, h, w), a's and b's extents along the output's axes)."""
+    i3 = ctypes.c_int * 3
+    rank, out, aa, ba = ctypes.c_int(), i3(), i3(), i3()
+    _check("fcuda_binary_op_shape", fcuda().fcuda_binary_op_shape(a_rank, i3(*a_shape), b_rank, i3(*b_shape),
+                                                                   ctypes.byref(rank), out, aa, ba))
+    return rank.value, tuple(out), tuple(aa), tuple(ba)
+
+
+def binary_op(a: torch.Tensor, b, op: int, relu: bool = False, out: torch.Tensor | None = None) -> torch.Tensor:
+    """ncnn BinaryOp `op` (0..11, BINARY_OPS) of a (N, C, H, W) and b: a tensor of the same rank that broadcasts
+    against a on C, H and W (either side may be 1 there; N equal), or a float scalar.  Optional ReLU (include/fcuda.h)."""
+    i4 = ctypes.c_int * 4
+    if torch.is_tensor(b):
+        shape = (a.shape[0],) + tuple(max(x, y) if 1 in (x, y) else x for x, y in zip(a.shape[1:], b.shape[1:]))
+        bp, bshape, scalar = _ptr(b.contiguous()), i4(*b.shape), 0.0
+    else:
+        shape, bp, bshape, scalar = tuple(a.shape), None, None, float(b)
+    out = torch.empty(shape, device=a.device, dtype=torch.float32) if out is None else out
+    _check("fcuda_binary_op_forward", fcuda().fcuda_binary_op_forward(_ptr(out), _ptr(a.contiguous()), i4(*a.shape), bp,
+                                                                      bshape, scalar, op, int(relu), _stream()))
+    return out
+
+
 def crop(x: torch.Tensor, coff: int, hoff: int, woff: int, oc: int, oh: int, ow: int) -> torch.Tensor:
     """out[n][c][y][x] = x[n][c + coff][y + hoff][x + woff], shape (N, oc, oh, ow)."""
     n, c, h, w = x.shape

@@ -3,6 +3,7 @@
 // (/root/reference/src/booster/avx/booster.cpp:283-355).
 #include "fcuda.h"
 
+#include "binary_op.cuh"
 #include "common.cuh"
 #include "conv_direct.cuh"
 #include "conv_igemm.cuh"
@@ -782,6 +783,84 @@ int fcuda_eltwise_forward(float* output, const float* a, const float* b, size_t 
     if (op < 0 || op > 2) return -200;
     if (op == 1 && coeff_a == 1.f && coeff_b == 1.f) return add_relu(a, b, output, n, relu, as_stream(stream));
     return eltwise(a, b, output, n, op, coeff_a, coeff_b, relu, as_stream(stream));
+}
+
+int fcuda_binary_op_shape(int a_rank, const int* a_shape, int b_rank, const int* b_shape, int* out_rank, int* out_shape,
+                          int* a_aligned, int* b_aligned) {
+    if (!a_shape || !b_shape || !out_rank || !out_shape || !a_aligned || !b_aligned) return -100;
+    int a[3], b[3];
+    for (int k = 0; k < 3; ++k) {
+        a[k] = a_shape[k];
+        b[k] = b_shape[k];
+        if (a[k] < 1 || b[k] < 1) return -100;
+    }
+    if (a_rank < 1 || a_rank > 3 || b_rank < 1 || b_rank > 3) return -100;
+    if ((a_rank < 3 && a[0] != 1) || (a_rank < 2 && a[1] != 1) || (b_rank < 3 && b[0] != 1) || (b_rank < 2 && b[1] != 1))
+        return -100;
+    const bool equal = a[0] == b[0] && a[1] == b[1] && a[2] == b[2];
+    const bool a_one = a[0] == 1 && a[1] == 1 && a[2] == 1, b_one = b[0] == 1 && b[1] == 1 && b[2] == 1;
+    int rank = a_rank > b_rank ? a_rank : b_rank;
+    if (equal) {
+    } else if (a_one) {
+        rank = b_rank;
+    } else if (b_one) {
+        rank = a_rank;
+    } else if (a_rank == 3 && b_rank == 1 && b[2] == a[0]) {  // ncnn's per-channel operand
+        b[0] = b[2];
+        b[2] = 1;
+    } else if (b_rank == 3 && a_rank == 1 && a[2] == b[0]) {
+        a[0] = a[2];
+        a[2] = 1;
+    }
+    int out[3];
+    for (int k = 0; k < 3; ++k) {
+        if (a[k] != b[k] && a[k] != 1 && b[k] != 1) return -200;
+        out[k] = a[k] == 1 ? b[k] : a[k];
+    }
+    *out_rank = rank;
+    for (int k = 0; k < 3; ++k) {
+        out_shape[k] = out[k];
+        a_aligned[k] = a[k];
+        b_aligned[k] = b[k];
+    }
+    return 0;
+}
+
+// Element strides of an NCHW operand of shape s along the output's axes: 0 where it broadcasts (extent 1).
+static BinaryOperand binary_operand(const float* p, const int* s) {
+    const long long w = s[3], hw = static_cast<long long>(s[2]) * w;
+    return BinaryOperand{p, s[1] * hw, s[1] == 1 ? 0 : hw, s[2] == 1 ? 0 : w, s[3] == 1 ? 0 : 1};
+}
+
+int fcuda_binary_op_forward(float* output, const float* a, const int* a_shape, const float* b, const int* b_shape,
+                            float b_scalar, int op, int relu, void* stream) {
+    if (!output || !a || !a_shape || (b && !b_shape)) return -100;
+    int as[4], bs[4], os[4];
+    for (int k = 0; k < 4; ++k) {
+        as[k] = a_shape[k];
+        bs[k] = b ? b_shape[k] : (k == 0 ? as[0] : 1);
+        if (as[k] < 1 || bs[k] < 1) return -100;
+    }
+    if (op < FCUDA_BINARY_ADD || op > FCUDA_BINARY_RATAN2 || as[0] != bs[0]) return -200;
+    os[0] = as[0];
+    bool a_bc = false, b_bc = false;
+    for (int k = 1; k < 4; ++k) {
+        if (as[k] != bs[k] && as[k] != 1 && bs[k] != 1) return -200;
+        os[k] = as[k] == 1 ? bs[k] : as[k];
+        a_bc = a_bc || as[k] != os[k];
+        b_bc = b_bc || bs[k] != os[k];
+    }
+    if (static_cast<long long>(os[2]) * os[3] > 0x7fffffffLL) return -200;
+    if ((output == a && a_bc) || (b && output == b && b_bc)) return -200;
+    relu = relu ? 1 : 0;
+    const cudaStream_t s = as_stream(stream);
+    if (!a_bc && (!b || !b_bc)) {
+        const size_t n = static_cast<size_t>(os[0]) * os[1] * os[2] * os[3];
+        if (b && op == FCUDA_BINARY_ADD) return add_relu(a, b, output, n, relu, s);  // Eltwise SUM
+        return binary_op_same(output, a, b, b_scalar, n, op, relu, s);
+    }
+    return binary_op_broadcast(output, binary_operand(a, as), binary_operand(b, bs), os[1], os[2], os[3], op, relu, os[0],
+                               s);
 }
 
 int fcuda_relu_forward(float* output, const float* input, size_t n, void* stream) {

@@ -3,6 +3,7 @@
 #pragma once
 
 #include <cuda_runtime_api.h>
+#include <fcuda.h>
 #include <feather/booster.h>
 #include <feather/layer.h>
 #include <stdlib.h>
@@ -114,6 +115,10 @@ public:
             if (conv_param.output_h <= 0 || conv_param.output_w <= 0) return FEATHER_ERR_WEIGHTS;
         }
         const int batch = bottom_blob->num();
+        if (residual) {
+            const int rc = CheckResidual(batch);
+            if (rc) return rc;
+        }
         if (fused_pool)  // the top is the pooled blob (ceil mode, pooling_layer.h:129-130 with k = s = 2, pad 0)
             tops[0]->ReshapeWithRealloc(batch, conv_param.output_channels, (conv_param.output_h + 1) / 2, (conv_param.output_w + 1) / 2);
         else
@@ -204,7 +209,7 @@ public:
         MEMPOOL_CHECK_RETURN(this->common_mempool->GetPtr(&buffer));
         const int batch = static_cast<int>(bottoms[0]->num());
         FcudaConvOptions o = FcudaConvOptions();
-        o.residual = residual ? residual->data() : NULL;
+        o.residual = residual && !residual_broadcast ? residual->data() : NULL;
         o.relu_after_add = relu_after_add;
         o.clip_min = clip_min; o.clip_max = clip_max;
         o.dilation_h = dilation_h; o.dilation_w = dilation_w;
@@ -212,17 +217,50 @@ public:
         const bool pool_after = fused_pool && !pool_in_epilogue;
         const int rc = conv_booster.ForwardOpts(&conv_param, pool_after ? pre_pool->data() : tops[0]->data(), bottoms[0]->data(),
                                                 processed_kernel, buffer, bias_data, o, batch, stream());
+        if (!rc && residual_broadcast) {  // a broadcast addend: the BinaryOp ADD (+ReLU) in place after the convolution
+            const int out[4] = {batch, conv_param.output_channels, conv_param.output_h, conv_param.output_w};
+            return fcuda_binary_op_forward(tops[0]->data(), tops[0]->data(), out, residual->data(), residual_shape, 0.f,
+                                           FCUDA_BINARY_ADD, relu_after_add, stream());
+        }
         if (rc || !pool_after) return rc;
         return fcuda_pooling_forward(tops[0]->data(), pre_pool->data(), conv_param.output_channels, conv_param.output_h,
                                      conv_param.output_w, 0, 2, 2, 2, 2, 0, 0, 0, 0, 0, batch, stream());
     }
 
-    // Net::ApplyFusion: absorb `Eltwise SUM(this->top, other) [+ReLU]` (a ResNet shortcut) into this layer's epilogue.
-    int FuseResidual(Blob<float>* other, int relu) {
+    // Net::ApplyFusion: absorb `Eltwise SUM(this->top, other) [+ReLU]` (a ResNet shortcut), or the same add written as a
+    // BinaryOp ADD (`broadcast`: `other` may broadcast against this layer's output), into this layer's epilogue.
+    int FuseResidual(Blob<float>* other, int relu, bool broadcast) {
         if (residual != NULL || fused_pool || (is_depthwise && (dilation_h > 1 || dilation_w > 1))) return 0;
         residual = other;
         relu_after_add = relu;
+        residual_may_broadcast = broadcast;
         return 1;
+    }
+
+    // Reshape with a fused residual, whose shape is only known now: an addend shaped like the output goes to the
+    // epilogue; a BinaryOp addend that broadcasts onto the output (fcuda_binary_op_shape, the output on the left) is
+    // added after the convolution by fcuda_binary_op_forward; anything else is the topology error the unfused layer
+    // would report.
+    int CheckResidual(int batch) {
+        const int oc = conv_param.output_channels, oh = conv_param.output_h, ow = conv_param.output_w;
+        const Blob<float>* r = residual;
+        residual_broadcast = false;
+        if (r->num() == static_cast<size_t>(batch) && r->channels() == static_cast<size_t>(oc) &&
+            r->height() == static_cast<size_t>(oh) && r->width() == static_cast<size_t>(ow))
+            return 0;
+        const int mine[3] = {oc, oh, ow};
+        const int theirs[3] = {static_cast<int>(r->channels()), static_cast<int>(r->height()), static_cast<int>(r->width())};
+        int rank = 0, out[3], a[3];
+        if (residual_may_broadcast && r->num() == static_cast<size_t>(batch) &&
+            fcuda_binary_op_shape(3, mine, r->dims(), theirs, &rank, out, a, residual_shape + 1) == 0 && rank == 3 &&
+            out[0] == oc && out[1] == oh && out[2] == ow) {
+            residual_shape[0] = batch;
+            residual_broadcast = true;
+            return 0;
+        }
+        LOGE("Convolution layer %s: the added blob %s (%zu, %zu, %zu, %zu) does not fit its output (%d, %d, %d, %d)",
+             this->name.c_str(), r->name.c_str(), r->num(), r->channels(), r->height(), r->width(), batch, oc, oh, ow);
+        return FEATHER_ERR_TOPOLOGY;
     }
 
     // conv_layer.h:174-185, extended to BatchNorm, Scale, Clip and a trailing 2x2 max pooling
@@ -298,9 +336,12 @@ protected:
     Blob<float>* folded_bias = NULL;
     // fused Clip (ConvLayer::Fuse): the epilogue's clamp bounds when conv_param.activation == booster::Clip
     float clip_min = 0.f, clip_max = 0.f;
-    // fused Eltwise SUM (Net::ApplyFusion)
+    // fused Eltwise SUM or BinaryOp ADD (Net::ApplyFusion); a BinaryOp addend may broadcast, and when it does
+    // (CheckResidual) residual_shape holds its (n, c, h, w) along the output's axes
     Blob<float>* residual = NULL;
     int relu_after_add = 0;
+    bool residual_may_broadcast = false, residual_broadcast = false;
+    int residual_shape[4] = {0, 0, 0, 0};
     // fused trailing 2x2 / stride-2 max pooling (Net::ApplyFusion)
     bool fused_pool = false;
     bool pool_in_epilogue = false;

@@ -12,6 +12,7 @@
 #include <feather/layer_factory.h>
 
 #include "layers/conv_layer.h"
+#include "layers/binary_op_layer.h"
 #include "layers/deconv_layer.h"
 #include "layers/eltwise_layer.h"
 #include "layers/misc_layers.h"
@@ -526,6 +527,24 @@ int Net::RunLayers() {
     return 0;
 }
 
+// A two-input sum the residual and super-resolution tail passes may absorb: a plain Eltwise SUM (Caffe's layout), or a
+// BinaryOp ADD of two bottoms without a scalar (how onnx2ncnn and pnnx write the same add).  *relu gets the ReLU it has
+// absorbed; *broadcast whether its addends may broadcast (BinaryOp), which Reshape of the absorbing layer then checks.
+static bool two_input_sum(Layer* l, int* relu, bool* broadcast) {
+    if (l->_fused_away || l->bottoms.size() != 2 || l->tops.size() != 1) return false;
+    if (const EltwiseLayer* e = dynamic_cast<const EltwiseLayer*>(l)) {
+        *relu = e->fused_relu();
+        *broadcast = false;
+        return e->plain_sum();
+    }
+    if (const BinaryOpLayer* b = dynamic_cast<const BinaryOpLayer*>(l)) {
+        *relu = b->fused_relu();
+        *broadcast = true;
+        return b->plain_add();
+    }
+    return false;
+}
+
 // The live version of the reference's dead TryFuse/Fuse hooks (layer.h:61-68, SURVEY.md §8f rank 1):
 // a fusible producer absorbs its consumer when that consumer is the only reader of the producer's top.
 int Net::ApplyFusion() {
@@ -551,15 +570,17 @@ int Net::ApplyFusion() {
             b->_fused_away = true;
         }
     }
-    // Second pass: a two-input Eltwise SUM (+ReLU, absorbed above) whose one addend is a convolution's otherwise unread
-    // top becomes that convolution's epilogue (ResNet shortcuts: 16 add_relu passes over the activations in ResNet-50).
-    // The other addend must already exist when the convolution runs.
+    // Second pass: a two-input sum (two_input_sum, +ReLU absorbed above) whose one addend is a convolution's otherwise
+    // unread top becomes that convolution's epilogue (ResNet shortcuts: 16 add_relu passes over the activations in
+    // ResNet-50).  The other addend must already exist when the convolution runs.
     std::map<Blob<float>*, size_t> producer;
     for (size_t i = 0; i < layers.size(); ++i)
         for (size_t j = 0; j < layers[i]->tops.size(); ++j) producer[layers[i]->tops[j]] = i;
     for (size_t j = 0; j < layers.size(); ++j) {
-        EltwiseLayer* e = dynamic_cast<EltwiseLayer*>(layers[j]);
-        if (!e || e->_fused_away || e->bottoms.size() != 2 || e->tops.size() != 1 || !e->plain_sum()) continue;
+        Layer* e = layers[j];
+        int relu = 0;
+        bool broadcast = false;
+        if (!two_input_sum(e, &relu, &broadcast)) continue;
         for (int k = 1; k >= 0; --k) {
             Blob<float>* mine = e->bottoms[k];
             Blob<float>* other = e->bottoms[1 - k];
@@ -569,7 +590,7 @@ int Net::ApplyFusion() {
             if (!conv || i >= j || conv->_fused_away || conv->tops.size() != 1) continue;
             if (producer.count(other) && producer[other] >= i) continue;  // not computed yet when the conv runs
             if (conv->param().activation != booster::None) continue;      // its own ReLU would have to precede the sum
-            if (conv->FuseResidual(other, e->fused_relu()) != 1) continue;
+            if (conv->FuseResidual(other, relu, broadcast) != 1) continue;
             Blob<float>* dead = conv->tops[0];
             blob_map.erase(dead->name);
             producer.erase(dead);
@@ -606,15 +627,16 @@ int Net::ApplyFusion() {
         c->bottoms.clear();
         c->_fused_away = true;
     }
-    // Super-resolution tail pass (ahead of the routing pass, which ends early when its tuning switch is off): a plain
-    // two-input Eltwise SUM of a PixelShuffle's top and a nearest Interp's top, each read only by the Eltwise, becomes
-    // the PixelShuffle's tail (SRVGGNetCompact's out = pixel_shuffle(conv) + nearest_upsample(x): two full-size blobs
-    // neither written nor read back).  Like the residual addend, the Interp's input must already exist when the
-    // PixelShuffle runs.
+    // Super-resolution tail pass (ahead of the routing pass, which ends early when its tuning switch is off): a
+    // two-input sum (two_input_sum) without a ReLU of a PixelShuffle's top and a nearest Interp's top, each read only by
+    // the sum, becomes the PixelShuffle's tail (SRVGGNetCompact's out = pixel_shuffle(conv) + nearest_upsample(x): two
+    // full-size blobs neither written nor read back).  Like the residual addend, the Interp's input must already exist
+    // when the PixelShuffle runs.  PixelShuffleLayer::Reshape rejects a tail whose addends do not have one shape.
     for (size_t j = 0; j < layers.size(); ++j) {
-        EltwiseLayer* e = dynamic_cast<EltwiseLayer*>(layers[j]);
-        if (!e || e->_fused_away || e->bottoms.size() != 2 || e->tops.size() != 1 || !e->plain_sum() || e->fused_relu())
-            continue;
+        Layer* e = layers[j];
+        int relu = 0;
+        bool broadcast = false;
+        if (!two_input_sum(e, &relu, &broadcast) || relu) continue;
         for (int k = 0; k < 2; ++k) {
             Blob<float>* mine = e->bottoms[k];
             Blob<float>* other = e->bottoms[1 - k];

@@ -24,8 +24,10 @@ import numpy as np
 
 
 class ModelWriter:
-    def __init__(self, seed: int = 0, wide_stats: bool = False):
+    def __init__(self, seed: int = 0, wide_stats: bool = False, adds: str = "eltwise"):
+        assert adds in ("eltwise", "binaryop"), adds
         self.rng = np.random.default_rng(seed)
+        self.adds = adds  # how add() writes a two-input sum: Caffe's Eltwise SUM, or BinaryOp ADD as onnx2ncnn / pnnx do
         self.wide_stats = wide_stats       # BatchNorm / Scale statistics of _batchnorm_wide (default: mild, near identity)
         self._bn_mul: dict[str, np.ndarray] = {}
         self.lines: list[str] = []
@@ -250,6 +252,24 @@ class ModelWriter:
         self._layer("Eltwise", name, bottoms, [top], {0: 1})
         self.shape[top] = self.shape[bottoms[0]]
         return top
+
+    def binary_op(self, name, bottoms, op, scalar=None, top=None):
+        """ncnn BinaryOp 0=op (0 ADD .. 11 RATAN2) of two bottoms, or of one bottom and `scalar` (1=1 2=scalar).  Two
+        bottoms broadcast by numpy's rule on their (c, h, w)."""
+        top = top or name
+        if scalar is None:
+            assert len(bottoms) == 2, (name, bottoms)
+            self._layer("BinaryOp", name, bottoms, [top], {0: op})
+            self.shape[top] = tuple(np.broadcast_shapes(*(self.shape[b] for b in bottoms)))
+        else:
+            assert len(bottoms) == 1, (name, bottoms)
+            self._layer("BinaryOp", name, bottoms, [top], {0: op, 1: 1, 2: f"{float(scalar):e}"})
+            self.shape[top] = self.shape[bottoms[0]]
+        return top
+
+    def add(self, name, bottoms, top=None):
+        """A two-input sum in the writer's `adds` layout: Eltwise SUM, or BinaryOp ADD."""
+        return self.eltwise(name, bottoms, top) if self.adds == "eltwise" else self.binary_op(name, bottoms, 0, top=top)
 
     def concat(self, name, bottoms, top=None, axis=0):
         """ncnn Concat over `axis` of the bottoms' rank (rank 1: 0 = w; rank 2: 0 = h, 1 = w; rank 3: 0 = c, 1 = h, 2 = w)."""
@@ -589,14 +609,15 @@ def _resnet50_trunk(m: ModelWriter, x: str, strides=(1, 2, 2, 2), dilations=(1, 
             y = _bn_scale_relu(m, f"{blk}_branch2b", y)
             y = m.conv(f"res{blk}_branch2c", y, width * 4, 1, 1, 0, False)
             y = _bn_scale_relu(m, f"{blk}_branch2c", y, relu=False, center=0.3)  # keep residual sums O(1)
-            x = m.eltwise(f"res{blk}", [sc, y])
+            x = m.add(f"res{blk}", [sc, y])
             x = m.relu(f"res{blk}_relu", x)
     return x
 
 
-def resnet50(seed=0, num_classes=1000, size=224, wide_stats=False) -> ModelWriter:
-    """Caffe ResNet-50 layout: stride on the first 1x1 of each stage, BN/Scale/ReLU layers, Split/Eltwise."""
-    m = ModelWriter(seed, wide_stats)
+def resnet50(seed=0, num_classes=1000, size=224, wide_stats=False, adds="eltwise") -> ModelWriter:
+    """Caffe ResNet-50 layout: stride on the first 1x1 of each stage, BN/Scale/ReLU layers, Split/Eltwise.  adds=
+    "binaryop" writes each shortcut sum as BinaryOp ADD (onnx2ncnn's and pnnx's layout), the same .bin."""
+    m = ModelWriter(seed, wide_stats, adds)
     x = _resnet50_trunk(m, m.input("data", 3, size, size))
     x = m.pool("pool5", x, 1, 7, 1, 0, global_pooling=True)
     x = m.fc("fc1000", x, num_classes)
@@ -631,11 +652,12 @@ def _bn_scale_clip(m: ModelWriter, tag: str, x: str, clip=True, center=1.0):
     return x
 
 
-def mobilenet_v2(seed=0, num_classes=1000, size=224, wide_stats=False) -> ModelWriter:
+def mobilenet_v2(seed=0, num_classes=1000, size=224, wide_stats=False, adds="eltwise") -> ModelWriter:
     """MobileNet-v2 (Sandler et al. 2018): inverted residual blocks from the (t, c, n, s) table, every convolution followed
     by BatchNorm + Scale, ReLU6 as ncnn's Clip 0..6 after the stem, expansion and depthwise convolutions, linear
-    projections, and an Eltwise SUM shortcut (through a Split) where the stride is 1 and the channel count is kept."""
-    m = ModelWriter(seed, wide_stats)
+    projections, and an Eltwise SUM shortcut (through a Split) where the stride is 1 and the channel count is kept.
+    adds="binaryop" writes each shortcut as BinaryOp ADD, the same .bin."""
+    m = ModelWriter(seed, wide_stats, adds)
     x = m.input("data", 3, size, size)
     x = m.conv("conv1", x, 32, 3, 2, 1, False)
     x = _bn_scale_clip(m, "_conv1", x)
@@ -656,7 +678,7 @@ def mobilenet_v2(seed=0, num_classes=1000, size=224, wide_stats=False) -> ModelW
             y = _bn_scale_clip(m, f"_conv{tag}_dw", y)
             y = m.conv(f"conv{tag}_linear", y, c, 1, 1, 0, False)
             y = _bn_scale_clip(m, f"_conv{tag}_linear", y, clip=False, center=0.3 if shortcut else 1.0)
-            x = m.eltwise(f"block{tag}", [sc, y]) if shortcut else y
+            x = m.add(f"block{tag}", [sc, y]) if shortcut else y
     x = m.conv("conv_last", x, 1280, 1, 1, 0, False)
     x = _bn_scale_clip(m, "_conv_last", x)
     x = m.pool("pool_last", x, 1, 7, 1, 0, global_pooling=True)
@@ -1328,44 +1350,46 @@ def _transformer_net(m: ModelWriter, x: str, widths, blocks: int) -> str:
         a, c = m.split(f"res{b}_split", x, [f"res{b}_in_a", f"res{b}_in_b"])
         y = m.relu(f"res{b}_relu1", m.instance_norm(f"res{b}_in1", _style_conv(m, f"res{b}_conv1", c, w3, 3)))
         y = m.instance_norm(f"res{b}_in2", _style_conv(m, f"res{b}_conv2", y, w3, 3))
-        x = m.eltwise(f"res{b}", [a, y])
+        x = m.add(f"res{b}", [a, y])
     for i, oc in ((4, w2), (5, w1)):
         x = m.interp(f"up{i}", x, resize_type=1, scale=2.0)
         x = m.relu(f"relu{i}", m.instance_norm(f"in{i}", _style_conv(m, f"conv{i}", x, oc, 3)))
     return _style_conv(m, "conv6", x, 3, 9)
 
 
-def fast_neural_style(seed=0, height=512, width=512) -> ModelWriter:
+def fast_neural_style(seed=0, height=512, width=512, adds="eltwise") -> ModelWriter:
     """Johnson et al.'s fast neural style transfer network in the layout of the PyTorch examples' TransformerNet: 32,
-    64 and 128 channels, five residual blocks, nearest x2 upsampling.  The output (`conv6`) is shaped like the input."""
+    64 and 128 channels, five residual blocks, nearest x2 upsampling.  The output (`conv6`) is shaped like the input.
+    adds="binaryop" writes the residual sums as BinaryOp ADD (an ONNX export's layout), the same .bin."""
     assert height % 4 == 0 and width % 4 == 0, (height, width)
-    m = ModelWriter(seed)
+    m = ModelWriter(seed, adds=adds)
     _transformer_net(m, m.input("data", 3, height, width), (32, 64, 128), 5)
     return m
 
 
-def style_tiny(seed=0, height=32, width=32) -> ModelWriter:
+def style_tiny(seed=0, height=32, width=32, adds="eltwise") -> ModelWriter:
     """fast_neural_style's layout at float64-checkable size: 8, 16 and 16 channels, two residual blocks (the second
     block's first Padding reads an Eltwise), both upsamples."""
     assert height % 4 == 0 and width % 4 == 0, (height, width)
-    m = ModelWriter(seed)
+    m = ModelWriter(seed, adds=adds)
     _transformer_net(m, m.input("data", 3, height, width), (8, 16, 16), 2)
     return m
 
 
-def srvgg_compact(seed=0, scale=4, num_conv=16, num_feat=64, height=270, width=480) -> ModelWriter:
+def srvgg_compact(seed=0, scale=4, num_conv=16, num_feat=64, height=270, width=480, adds="eltwise") -> ModelWriter:
     """Real-ESRGAN's SRVGGNetCompact (basicsr): conv 3 -> num_feat and PReLU, num_conv x (conv num_feat -> num_feat,
     PReLU), conv num_feat -> 3 scale^2 and PixelShuffle(scale), plus the input upsampled by a nearest Interp x scale,
     added by an Eltwise SUM.  The defaults are realesr-animevideov3; num_conv=32 gives realesr-general-x4v3.  The output
-    (`output`) is (3, height * scale, width * scale)."""
-    m = ModelWriter(seed)
+    (`output`) is (3, height * scale, width * scale).  adds="binaryop" writes the tail's sum as BinaryOp ADD (a pnnx or
+    ONNX export's layout), the same .bin."""
+    m = ModelWriter(seed, adds=adds)
     x, skip = m.split("data_split", m.input("data", 3, height, width), ["data_body", "data_skip"])
     x = m.prelu("prelu0", m.conv("conv0", x, num_feat, 3, 1, 1), slopes=np.full(num_feat, 0.25))
     for i in range(1, num_conv + 1):
         x = m.prelu(f"prelu{i}", m.conv(f"conv{i}", x, num_feat, 3, 1, 1), slopes=np.full(num_feat, 0.25))
     x = m.pixel_shuffle("upsample", m.conv("conv_last", x, 3 * scale * scale, 3, 1, 1), scale)
     base = m.interp("base", skip, resize_type=1, scale=float(scale))
-    m.eltwise("output", [x, base])
+    m.add("output", [x, base])
     return m
 
 
@@ -1384,13 +1408,13 @@ def _edsr_upsampler(m: ModelWriter, x: str, scale: int, n_feats: int) -> str:
 
 
 def edsr_baseline(seed=0, scale=4, n_resblocks=16, n_feats=64, height=270, width=480, rgb_range=255.0,
-                  res_gain=0.1) -> ModelWriter:
+                  res_gain=0.1, adds="eltwise") -> ModelWriter:
     """EDSR baseline (Lim et al. 2017): MeanShift (sub_mean) as a fixed 1x1 convolution, the head conv 3 -> n_feats,
     n_resblocks x (conv, ReLU, conv, + skip), a conv plus the global skip, the upsampler (_edsr_upsampler), the tail conv
     n_feats -> 3 and add_mean.  Each residual block's second convolution draws its weights at res_gain times He init, so
     the activations stay in range over depth as trained weights keep them.  The output (`add_mean`) is
-    (3, height * scale, width * scale)."""
-    m = ModelWriter(seed)
+    (3, height * scale, width * scale).  adds="binaryop" writes the residual sums as BinaryOp ADD, the same .bin."""
+    m = ModelWriter(seed, adds=adds)
     mean = rgb_range * np.asarray(EDSR_RGB_MEAN)
     x = m.fixed_conv1x1("sub_mean", m.input("data", 3, height, width), np.eye(3), -mean)
     x, head = m.split("head_split", m.conv("head", x, n_feats, 3, 1, 1), ["body_in", "head_skip"])
@@ -1398,25 +1422,25 @@ def edsr_baseline(seed=0, scale=4, n_resblocks=16, n_feats=64, height=270, width
         a, c = m.split(f"res{b}_split", x, [f"res{b}_in", f"res{b}_skip"])
         y = m.relu(f"res{b}_relu", m.conv(f"res{b}_conv1", a, n_feats, 3, 1, 1))
         y = m.conv(f"res{b}_conv2", y, n_feats, 3, 1, 1, gain=res_gain * np.sqrt(2.0 / (9 * n_feats)))
-        x = m.eltwise(f"res{b}", [c, y])
-    x = m.eltwise("body", [head, m.conv("body_conv", x, n_feats, 3, 1, 1)])
+        x = m.add(f"res{b}", [c, y])
+    x = m.add("body", [head, m.conv("body_conv", x, n_feats, 3, 1, 1)])
     x = m.conv("tail", _edsr_upsampler(m, x, scale, n_feats), 3, 3, 1, 1)
     m.fixed_conv1x1("add_mean", x, np.eye(3), mean)
     return m
 
 
-def sr_tiny(seed=0, height=9, width=11) -> ModelWriter:
+def sr_tiny(seed=0, height=9, width=11, adds="eltwise") -> ModelWriter:
     """PixelShuffle at float64-checkable size, odd height and width: conv 3 -> 8 and PReLU, conv to 32 and PixelShuffle 2
     in mode 1 (DepthToSpace DCR) feeding conv 8 -> 27, PixelShuffle 3 in mode 0, and SRVGGNetCompact's tail: the input
     upsampled x 6 by a nearest Interp and added by an Eltwise SUM, which fuses into the second PixelShuffle.  The output
     (`output`) is (3, 6 height, 6 width)."""
-    m = ModelWriter(seed)
+    m = ModelWriter(seed, adds=adds)
     x, skip = m.split("data_split", m.input("data", 3, height, width), ["data_body", "data_skip"])
     x = m.prelu("prelu0", m.conv("conv0", x, 8, 3, 1, 1))
     x = m.pixel_shuffle("shuffle1", m.conv("conv1", x, 32, 3, 1, 1), 2, mode=1)
     x = m.pixel_shuffle("shuffle2", m.conv("conv2", x, 27, 3, 1, 1), 3)
     base = m.interp("base", skip, resize_type=1, scale=6.0)
-    m.eltwise("output", [x, base])
+    m.add("output", [x, base])
     return m
 
 

@@ -188,6 +188,51 @@ int fcuda_eltwise_add_forward(float* output, const float* a, const float* b, siz
  * op 0 PROD a*b, op 1 SUM coeff_a*a + coeff_b*b, op 2 MAX max(a,b); optional ReLU.  In-place (output == a) is allowed. */
 int fcuda_eltwise_forward(float* output, const float* a, const float* b, size_t n, int op, float coeff_a, float coeff_b,
                           int relu, void* stream);
+/* ncnn's BinaryOp (what onnx2ncnn writes for ONNX Add / Sub / Mul / Div / Max / Min / Pow and pnnx for torch.add, x + y,
+ * x * 0.5; the reference has no such layer), in ncnn's op numbering.  All arithmetic is fp32, one operation per element:
+ * IEEE division and round-to-nearest add / sub / mul.  MAX and MIN are fmaxf / fminf, so a NaN operand yields the other
+ * operand (the NaN rule of the Eltwise MAX); the rest propagate NaN.  POW, RPOW, ATAN2 and RATAN2 are CUDA's powf /
+ * atan2f, within the ulp bounds the CUDA C Programming Guide lists for them. */
+enum FcudaBinaryOp {
+    FCUDA_BINARY_ADD = 0,    /* a + b */
+    FCUDA_BINARY_SUB = 1,    /* a - b */
+    FCUDA_BINARY_MUL = 2,    /* a * b */
+    FCUDA_BINARY_DIV = 3,    /* a / b */
+    FCUDA_BINARY_MAX = 4,    /* fmaxf(a, b) */
+    FCUDA_BINARY_MIN = 5,    /* fminf(a, b) */
+    FCUDA_BINARY_POW = 6,    /* powf(a, b) */
+    FCUDA_BINARY_RSUB = 7,   /* b - a */
+    FCUDA_BINARY_RDIV = 8,   /* b / a */
+    FCUDA_BINARY_RPOW = 9,   /* powf(b, a) */
+    FCUDA_BINARY_ATAN2 = 10, /* atan2f(a, b) */
+    FCUDA_BINARY_RATAN2 = 11 /* atan2f(b, a) */
+};
+/* ncnn's BinaryOp operand rule, host only.  Each operand is one image of ncnn rank 1..3 stored as (c, h, w) (rank 2:
+ * c = 1; rank 1: c = h = 1).  In this order:
+ *   1. equal (c, h, w): the output is that shape;
+ *   2. a one-element operand is a scalar: the output is the other operand's shape;
+ *   3. a rank-3 blob with a rank-1 operand whose w equals its c broadcasts that operand per channel, as (c, 1, 1): ncnn's
+ *      per-channel convention, which wins where numpy alignment would disagree (a rank-1 operand of c values next to a
+ *      (c, h, c) blob);
+ *   4. otherwise both operands, padded to (c, h, w) with leading 1s, follow numpy's rule on each axis: equal, or 1 on one
+ *      side, which broadcasts.
+ * The output rank is the larger of the two.  out_shape gets the output (c, h, w); a_aligned and b_aligned get each
+ * operand's extent along the output's (c, h, w) axes (the output's extent, or 1 where it broadcasts); the operand's
+ * storage read in that shape is unchanged.  -100: a NULL pointer, a rank outside 1..3, a shape entry < 1, or c > 1 with
+ * rank < 3, h > 1 with rank 1.  -200: a pair outside the rule. */
+int fcuda_binary_op_shape(int a_rank, const int* a_shape, int b_rank, const int* b_shape, int* out_rank, int* out_shape,
+                          int* a_aligned, int* b_aligned);
+/* out = op(a, b) [then fmaxf(., 0): the Eltwise ReLU, NaN becomes 0] over NCHW fp32 blobs.  a_shape and b_shape are
+ * (n, c, h, w); on each of c, h, w the two are equal or one of them is 1, which broadcasts (stride 0) and may be either
+ * side; n must be equal.  The output takes the broadcast shape.  With b NULL, b_shape is ignored and every b is
+ * b_scalar.  The same-shape ADD is the Eltwise SUM kernel (fcuda_eltwise_add_forward) bit for bit; every other case is
+ * one launch of the BinaryOp kernels (profiling kind 6).  output == a is allowed when a broadcasts on no axis, likewise
+ * output == b.  Allocates nothing and does not synchronise.
+ * -100: NULL output, a or a_shape, b without b_shape, or a size < 1.  -200: op outside 0..11, shapes that do not
+ * broadcast, unequal n, an output plane of 2^31 floats or more, or output equal to an operand that broadcasts.  Both are
+ * decided before any launch. */
+int fcuda_binary_op_forward(float* output, const float* a, const int* a_shape, const float* b, const int* b_shape,
+                            float b_scalar, int op, int relu, void* stream);
 /* ReluLayer::Forward (src/layers/relu_layer.h:29-41). */
 int fcuda_relu_forward(float* output, const float* input, size_t n, void* stream);
 /* ncnn's Clip (the reference has no such layer; Caffe's ReLU6 is min 0, max 6): y = min(max(x, min), max) over n
@@ -723,7 +768,7 @@ void fcuda_profile_tensor_gemm(int enable);
 int fcuda_profile_collect(double* total_ms, double* algo_flops, double* mma_flops, long long* launches);
 /* Same, per kernel class, for every instrumented launch (the enable switch above covers all of them):
  * kind 0 TensorGEMM, 1 implicit-GEMM conv, 2 Winograd input transform, 3 Winograd output transform, 4 pooling,
- * 5 depthwise, 6 element-wise (BN/Scale/Eltwise/Clip/PReLU/Normalize/LRN), 7 deconvolution scatter / depthwise gather, 8 resize / crop (Interp,
+ * 5 depthwise, 6 element-wise (BN/Scale/Eltwise/BinaryOp/Clip/PReLU/Normalize/LRN), 7 deconvolution scatter / depthwise gather, 8 resize / crop (Interp,
  * Crop), 9 detection (Permute, axis Softmax, PriorBox, decode, NMS, merge; YOLO decode, select, mask, sweep), 10 channel
  * routing (fcuda_route_forward), 11 two-stage detection (Proposal decode, select, mask, sweep; ROIPooling; PSROIPooling),
  * 12 instance normalisation / padding (InstanceNorm, Padding), 13 pixel shuffle (PixelShuffle, alone or with its fused
