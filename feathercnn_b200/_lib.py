@@ -192,6 +192,7 @@ def fcuda() -> ctypes.CDLL:
             "fcuda_eltwise_add_forward": (i, [vp, vp, vp, sz, i, vp]),
             "fcuda_relu_forward": (i, [vp, vp, sz, vp]),
             "fcuda_clip_forward": (i, [vp, vp, sz, ctypes.c_float, ctypes.c_float, vp]),
+            "fcuda_activation_forward": (i, [vp, vp, sz, i, ctypes.c_float, ctypes.c_float, vp]),
             "fcuda_prelu_forward": (i, [vp, vp, i, sz, vp, i, i, vp]),
             "fcuda_normalize_workspace_size": (i, [i, i, i, sz, i, szp]),
             "fcuda_normalize_forward": (i, [vp, vp, i, sz, vp, i, i, i, f, i, vp, i, vp]),

@@ -609,6 +609,20 @@ def clip(x, lo, hi, out=None):
     return out
 
 
+ACTIVATIONS = ["Sigmoid", "TanH", "Swish", "HardSigmoid", "HardSwish"]  # FcudaActivationType, ncnn's layer type names
+
+
+def activation(x, kind, alpha: float = 0.2, beta: float = 0.5, out=None):
+    """ncnn activation `kind` (0..4 or a name of ACTIVATIONS) over every element of x; alpha / beta are read by
+    HardSigmoid / HardSwish only (ncnn's defaults 0.2 / 0.5).  `out` may be `x` (in place).  Definitions, roundings and
+    bounds: include/fcuda.h."""
+    kind = ACTIVATIONS.index(kind) if isinstance(kind, str) else int(kind)
+    out = torch.empty_like(x) if out is None else out
+    _check("fcuda_activation_forward", fcuda().fcuda_activation_forward(_ptr(out), _ptr(x.contiguous()), x.numel(), kind,
+                                                                        float(alpha), float(beta), _stream()))
+    return out
+
+
 def prelu(x, slope, out=None):
     """ncnn PReLU over (N, C, ...): x < 0 ? x * slope[c] : x; a one-element `slope` is shared.  `out` may be `x`."""
     n, c = x.shape[:2]

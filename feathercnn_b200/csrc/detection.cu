@@ -10,6 +10,7 @@
 //   merge      one CTA per image: the same select and sort over the kept lists of all classes, then the output rows.
 // Keys are 64 bits: an order-preserving image of the fp32 score above 32 bits of (0xffffffff - index), so one descending
 // sort gives score descending and index ascending.
+#include "activation.cuh"
 #include "common.cuh"
 #include "detection.cuh"
 
@@ -454,8 +455,6 @@ struct YoloGeom {
     int version, num_class, num_box, num_scales, slots;
     YoloScale scale[FCUDA_YOLO_MAX_SCALES];
 };
-
-__device__ __forceinline__ float sigm(float t) { return __fdiv_rn(1.f, __fadd_rn(1.f, expf(-t))); }
 
 __global__ void __launch_bounds__(256)
 yolo_decode_kernel(float* __restrict__ scores, int* __restrict__ classes, float* __restrict__ boxes, const YoloGeom g,

@@ -3,6 +3,7 @@
 // (/root/reference/src/booster/avx/booster.cpp:283-355).
 #include "fcuda.h"
 
+#include "activation.cuh"
 #include "binary_op.cuh"
 #include "common.cuh"
 #include "conv_direct.cuh"
@@ -872,6 +873,18 @@ int fcuda_clip_forward(float* output, const float* input, size_t n, float min, f
     if (!output || !input) return -100;
     if (!(min <= max)) return -200;
     return clip(input, output, n, min, max, as_stream(stream));
+}
+
+int fcuda_activation_forward(float* output, const float* input, size_t n, int type, float alpha, float beta,
+                             void* stream) {
+    if (!output || !input || n == 0) return -100;
+    if (type < FCUDA_ACTIVATION_SIGMOID || type > FCUDA_ACTIVATION_HARDSWISH) return -200;
+    const bool hard = type == FCUDA_ACTIVATION_HARDSIGMOID || type == FCUDA_ACTIVATION_HARDSWISH;
+    if (hard && (alpha == 0.f || !isfinite(alpha) || !isfinite(beta))) return -200;
+    // ncnn's HardSigmoid / HardSwish load_param, in fp32
+    const float lower = hard ? -beta / alpha : 0.f;
+    const float upper = hard ? 1.f / alpha + lower : 0.f;
+    return activation(output, input, n, type, alpha, beta, lower, upper, as_stream(stream));
 }
 
 int fcuda_prelu_forward(float* output, const float* input, int channels, size_t plane, const float* slope, int num_slope,

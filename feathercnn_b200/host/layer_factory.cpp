@@ -2,14 +2,16 @@
 // plus Deconvolution / DeconvolutionDepthWise, Interp, Crop, Clip, PReLU, SSD's Permute, Flatten, Reshape, PriorBox and
 // DetectionOutput, VGG-SSD's Normalize, YOLO's YoloDetectionOutput and Yolov3DetectionOutput, ShuffleNet's ShuffleChannel
 // and Slice, AlexNet's and GoogLeNet's LRN, Faster R-CNN's Proposal and ROIPooling, R-FCN's PSROIPooling, fast neural
-// style's InstanceNorm and Padding, super-resolution's PixelShuffle, and BinaryOp (the element-wise ops onnx2ncnn and
-// pnnx write, residual adds among them), 37 in all, mapped onto this host's layer classes.  A table of {type name,
+// style's InstanceNorm and Padding, super-resolution's PixelShuffle, BinaryOp (the element-wise ops onnx2ncnn and pnnx
+// write, residual adds among them), and the activations Sigmoid, TanH, Swish, HardSigmoid and HardSwish (MobileNet-v3,
+// EfficientNet, ESPCN), 42 in all, mapped onto this host's layer classes.  A table of {type name,
 // factory} pairs instead of one macro line per layer; the
 // DEFINE_LAYER_CREATOR / REGISTER_LAYER_CREATOR macros of <feather/layer_factory.h> remain the plugin API for user layers.
 #include <feather/layer_factory.h>
 
 #include <stdio.h>
 
+#include "layers/activation_layers.h"
 #include "layers/batchnorm_layer.h"
 #include "layers/binary_op_layer.h"
 #include "layers/clip_prelu_layers.h"
@@ -86,6 +88,11 @@ const BuiltIn kBuiltIns[] = {
     {"Padding", make_layer<PaddingLayer>},
     {"PixelShuffle", make_layer<PixelShuffleLayer>},
     {"BinaryOp", make_layer<BinaryOpLayer>},
+    {"Sigmoid", make_layer<ActivationLayer>},
+    {"TanH", make_layer<ActivationLayer>},
+    {"Swish", make_layer<ActivationLayer>},
+    {"HardSigmoid", make_layer<ActivationLayer>},
+    {"HardSwish", make_layer<ActivationLayer>},
 };
 
 }  // namespace

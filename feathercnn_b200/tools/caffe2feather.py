@@ -8,13 +8,14 @@ no caffe / protobuf-generated code is needed — and writes the ncnn text ``.par
 
 * layer grammar and parameter ids as ``ConvLayer::LoadParam`` & co. read them (``src/layers/*.h``; ids follow ncnn's
   caffe2ncnn): Convolution / ConvolutionDepthWise, Deconvolution / DeconvolutionDepthWise, InnerProduct, Pooling, ReLU, BatchNorm, Scale, Eltwise, Concat, Dropout,
-  Softmax, Split, Input, Crop, Clip, PReLU, Slice, LRN;
+  Softmax, Split, Input, Crop, Clip, PReLU, Slice, LRN, Sigmoid, TanH;
 * LRN (``lrn_param``: ``local_size``, ``alpha``, ``beta``, ``norm_region``, ``k``) becomes ncnn's LRN
   ``0=region 1=local_size 2=alpha 3=beta 4=bias``.  Caffe's WITHIN_CHANNEL LRN divides by a fixed ``1 + alpha / n * ss``
   and ignores ``k``, so that region is written with ``4=1``; an even ``local_size`` (which Caffe rejects) is an error;
 * Slice (``slice_param``: ``axis`` or the older ``slice_dim``, ``slice_point``) becomes ncnn's Slice: the cut points become
   sizes with ``-233`` (the rest) for the last top, and no cut points an even split (``-233`` for every top).  Caffe has no
   ShuffleChannel in its upstream ``caffe.proto``, so that type keeps the "no counterpart" error;
+* Sigmoid and TanH keep their names; ``sigmoid_param`` / ``tanh_param`` only choose Caffe's compute engine;
 * ReLU6 (the type MobileNet-v2 Caffe ports use) becomes ``Clip 0=0 1=6``, Caffe's Clip (``clip_param.min / max``) Clip with its
   bounds, PReLU ``PReLU 0=num_slope`` with its slopes (one, ``channel_shared``, or one per channel) raw in the ``.bin``;
 * Crop (``axis`` 2 or 3, FCN's score crops) becomes ncnn's two-bottom Crop: the output height and width are the reference
@@ -269,6 +270,8 @@ def convert(caffemodel: bytes) -> tuple[str, bytes]:
         elif type_ == "ReLU":
             slope = _f32(_first(parse_message(_first(L, 123, b"")), 1), 0.0)
             out.layer("ReLU", name, bottoms, tops, f"0={slope:e}" if slope else "")
+        elif type_ in ("Sigmoid", "TanH"):
+            out.layer(type_, name, bottoms, tops, "")
         elif type_ == "ReLU6":
             out.layer("Clip", name, bottoms, tops, f"0={0.0:e} 1={6.0:e}")
         elif type_ == "Clip":

@@ -10,8 +10,9 @@ AlexNet (BVLC's deploy nets, with LRN), plus a small "mini" net
 that exercises every layer type, single-shot detectors (MobileNet-SSD, VGG-SSD 300, a two-head tiny SSD), YOLO detectors
 (MobileNet-YOLOv2, MobileNet-v2 YOLOv3, a two-scale tiny YOLOv3), two-stage detectors (py-faster-rcnn's VGG-16 Faster
 R-CNN, py-R-FCN's ResNet-50 R-FCN and a tiny one of each), fast neural style transfer (TransformerNet, with a tiny
-one), super-resolution (Real-ESRGAN's SRVGGNetCompact and EDSR baseline, with a tiny PixelShuffle net) and ShuffleNet-v2
-with a small routing probe net.  Weight
+one), super-resolution (Real-ESRGAN's SRVGGNetCompact and EDSR baseline, with a tiny PixelShuffle net, and ESPCN), ShuffleNet-v2
+with a small routing probe net, and the nets of ncnn's activation layers (MobileNet-v3 Large / Small and EfficientNet-B0
+in torchvision's layouts, with a small squeeze-and-excitation net).  Weight
 statistics follow SURVEY.md §8(d).
 """
 from __future__ import annotations
@@ -502,6 +503,20 @@ class ModelWriter:
             s = np.float32(1.0 if scale is None else scale)
             self.shape[top] = (c, int(np.float32(h) * s), int(np.float32(w) * s))
         return top
+
+    def activation(self, type_, name, bottom, alpha=None, beta=None, top=None):
+        """ncnn Sigmoid / TanH / Swish (no parameters), HardSigmoid / HardSwish 0=alpha 1=beta (each written when given;
+        pnnx writes PyTorch's 1/6 and 0.5 as 0=1.666667e-01 1=5.000000e-01)."""
+        assert type_ in ("Sigmoid", "TanH", "Swish", "HardSigmoid", "HardSwish"), type_
+        top = top or name
+        params = {k: f"{v:e}" for k, v in ((0, alpha), (1, beta)) if v is not None}
+        self._layer(type_, name, [bottom], [top], params)
+        self.shape[top] = self.shape[bottom]
+        return top
+
+    def hard(self, type_, name, bottom, top=None):
+        """HardSigmoid / HardSwish with PyTorch's alpha 1/6 and beta 0.5, as pnnx writes them."""
+        return self.activation(type_, name, bottom, 1.0 / 6.0, 0.5, top)
 
     def pixel_shuffle(self, name, bottom, r, mode=0, top=None):
         """ncnn PixelShuffle 0=upscale_factor 1=mode (0 PyTorch's channel order, 1 DepthToSpace DCR; written when 1)."""
@@ -1444,6 +1459,154 @@ def sr_tiny(seed=0, height=9, width=11, adds="eltwise") -> ModelWriter:
     return m
 
 
+def make_divisible(v: float, divisor: int = 8) -> int:
+    """torchvision's _make_divisible: the nearest multiple of divisor, at least divisor and not below 90 % of v."""
+    new_v = max(divisor, int(v + divisor / 2) // divisor * divisor)
+    return new_v + divisor if new_v < 0.9 * v else new_v
+
+
+def _conv_bn(m: ModelWriter, name: str, x: str, oc: int, k: int, stride: int, eps: float, group: int = 1,
+             act: str | None = None) -> str:
+    """torchvision's Conv2dNormActivation as pnnx exports it: a convolution without bias, BatchNorm + Scale with eps, then
+    the activation layer ("ReLU", or an ncnn activation type)."""
+    x = m.conv(name, x, oc, k, stride, (k - 1) // 2, False, group=group)
+    x = m.scale(name + "_scale", m.batchnorm(name + "_bn", x, eps=eps), True)
+    if act == "ReLU":
+        x = m.relu(name + "_relu", x)
+    elif act in ("HardSwish", "HardSigmoid"):
+        x = m.hard(act, name + "_hs", x)
+    elif act is not None:
+        x = m.activation(act, name + "_" + act.lower(), x)
+    return x
+
+
+def _squeeze_excitation(m: ModelWriter, name: str, x: str, squeeze: int, act: str, gate: str) -> str:
+    """SE block: Split, global average Pooling, 1 x 1 Convolution (bias), `act`, 1 x 1 Convolution (bias), `gate`, and
+    BinaryOp MUL of the (C, 1, 1) gate and the block's activation, the gate first (torchvision's `scale * input`)."""
+    c = m.shape[x][0]
+    a, b = m.split(name + "_split", x, [name + "_in", name + "_sq"])
+    g = m.pool(name + "_pool", b, 1, 1, 1, 0, global_pooling=True)
+    g = m.conv(name + "_fc1", g, squeeze, 1, 1, 0, True)
+    g = m.relu(name + "_relu", g) if act == "ReLU" else m.activation(act, name + "_" + act.lower(), g)
+    g = m.conv(name + "_fc2", g, c, 1, 1, 0, True)
+    g = m.hard(gate, name + "_gate", g) if gate == "HardSigmoid" else m.activation(gate, name + "_gate", g)
+    return m.binary_op(name + "_mul", [g, a], 2)
+
+
+# (input_c, kernel, expanded_c, out_c, use_se, activation, stride) of torchvision's _mobilenet_v3_conf
+MOBILENET_V3_LARGE = [(16, 3, 16, 16, False, "RE", 1), (16, 3, 64, 24, False, "RE", 2), (24, 3, 72, 24, False, "RE", 1),
+                      (24, 5, 72, 40, True, "RE", 2), (40, 5, 120, 40, True, "RE", 1), (40, 5, 120, 40, True, "RE", 1),
+                      (40, 3, 240, 80, False, "HS", 2), (80, 3, 200, 80, False, "HS", 1),
+                      (80, 3, 184, 80, False, "HS", 1), (80, 3, 184, 80, False, "HS", 1),
+                      (80, 3, 480, 112, True, "HS", 1), (112, 3, 672, 112, True, "HS", 1),
+                      (112, 5, 672, 160, True, "HS", 2), (160, 5, 960, 160, True, "HS", 1),
+                      (160, 5, 960, 160, True, "HS", 1)]
+MOBILENET_V3_SMALL = [(16, 3, 16, 16, True, "RE", 2), (16, 3, 72, 24, False, "RE", 2), (24, 3, 88, 24, False, "RE", 1),
+                      (24, 5, 96, 40, True, "HS", 2), (40, 5, 240, 40, True, "HS", 1), (40, 5, 240, 40, True, "HS", 1),
+                      (40, 5, 120, 48, True, "HS", 1), (48, 5, 144, 48, True, "HS", 1), (48, 5, 288, 96, True, "HS", 2),
+                      (96, 5, 576, 96, True, "HS", 1), (96, 5, 576, 96, True, "HS", 1)]
+
+
+def _mobilenet_v3(table, last_channel: int, seed: int, num_classes: int, size: int) -> ModelWriter:
+    m = ModelWriter(seed)
+    x = _conv_bn(m, "conv_stem", m.input("data", 3, size, size), 16, 3, 2, 1e-3, act="HardSwish")
+    for i, (ic, k, exp, oc, se, act, stride) in enumerate(table, 1):
+        act = "ReLU" if act == "RE" else "HardSwish"
+        res = stride == 1 and ic == oc
+        if res:
+            sc, x = m.split(f"block{i}_split", x, [f"block{i}_skip", f"block{i}_body"])
+        y = x
+        if exp != ic:
+            y = _conv_bn(m, f"block{i}_expand", y, exp, 1, 1, 1e-3, act=act)
+        y = _conv_bn(m, f"block{i}_dw", y, exp, k, stride, 1e-3, group=exp, act=act)
+        if se:
+            y = _squeeze_excitation(m, f"block{i}_se", y, make_divisible(exp / 4), "ReLU", "HardSigmoid")
+        y = _conv_bn(m, f"block{i}_project", y, oc, 1, 1, 1e-3)
+        x = m.binary_op(f"block{i}_add", [sc, y], 0) if res else y
+    x = _conv_bn(m, "conv_last", x, 6 * m.shape[x][0], 1, 1, 1e-3, act="HardSwish")
+    x = m.pool("pool", x, 1, 1, 1, 0, global_pooling=True)
+    x = m.hard("HardSwish", "fc1_hs", m.fc("fc1", x, last_channel))
+    x = m.fc("fc2", x, num_classes)
+    m.softmax("prob", x)
+    return m
+
+
+def mobilenet_v3_large(seed=0, num_classes=1000, size=224) -> ModelWriter:
+    """MobileNet-v3 Large (Howard et al. 2019) in torchvision's layout as pnnx exports it: every convolution followed by
+    BatchNorm + Scale (eps 1e-3), HardSwish / ReLU as the block table says, squeeze-and-excitation with a
+    make_divisible(expanded / 4, 8) squeeze, ReLU and a HardSigmoid gate, BinaryOp ADD shortcuts, and the classifier
+    InnerProduct 1280, HardSwish, InnerProduct, Softmax."""
+    return _mobilenet_v3(MOBILENET_V3_LARGE, 1280, seed, num_classes, size)
+
+
+def mobilenet_v3_small(seed=0, num_classes=1000, size=224) -> ModelWriter:
+    """MobileNet-v3 Small, as mobilenet_v3_large with the small block table and a 1024-wide classifier."""
+    return _mobilenet_v3(MOBILENET_V3_SMALL, 1024, seed, num_classes, size)
+
+
+# (expand_ratio, kernel, stride, input_channels, out_channels, num_layers) of torchvision's efficientnet_b0
+EFFICIENTNET_B0 = [(1, 3, 1, 32, 16, 1), (6, 3, 2, 16, 24, 2), (6, 5, 2, 24, 40, 2), (6, 3, 2, 40, 80, 3),
+                   (6, 5, 1, 80, 112, 3), (6, 5, 2, 112, 192, 4), (6, 3, 1, 192, 320, 1)]
+
+
+def efficientnet_b0(seed=0, num_classes=1000, size=224) -> ModelWriter:
+    """EfficientNet-B0 (Tan & Le 2019) in torchvision's layout as pnnx exports it: SiLU as Swish, every convolution
+    followed by BatchNorm + Scale (eps 1e-5), seven MBConv stages (3 x 3 and 5 x 5 depthwise), squeeze-and-excitation
+    with a max(1, input / 4) squeeze of the block input, Swish and a Sigmoid gate, BinaryOp ADD shortcuts, a 1280-channel
+    head, global average pooling, InnerProduct and Softmax."""
+    m = ModelWriter(seed)
+    x = _conv_bn(m, "conv_stem", m.input("data", 3, size, size), 32, 3, 2, 1e-5, act="Swish")
+    i = 0
+    for t, k, s, ic0, oc, n in EFFICIENTNET_B0:
+        for j in range(n):
+            i += 1
+            ic, stride = (ic0, s) if j == 0 else (oc, 1)
+            exp = make_divisible(ic * t)
+            res = stride == 1 and ic == oc
+            if res:
+                sc, x = m.split(f"block{i}_split", x, [f"block{i}_skip", f"block{i}_body"])
+            y = x
+            if exp != ic:
+                y = _conv_bn(m, f"block{i}_expand", y, exp, 1, 1, 1e-5, act="Swish")
+            y = _conv_bn(m, f"block{i}_dw", y, exp, k, stride, 1e-5, group=exp, act="Swish")
+            y = _squeeze_excitation(m, f"block{i}_se", y, max(1, ic // 4), "Swish", "Sigmoid")
+            y = _conv_bn(m, f"block{i}_project", y, oc, 1, 1, 1e-5)
+            x = m.binary_op(f"block{i}_add", [sc, y], 0) if res else y
+    x = _conv_bn(m, "conv_last", x, 1280, 1, 1, 1e-5, act="Swish")
+    x = m.pool("pool", x, 1, 1, 1, 0, global_pooling=True)
+    x = m.fc("fc", x, num_classes)
+    m.softmax("prob", x)
+    return m
+
+
+def espcn(seed=0, scale=3, height=360, width=640) -> ModelWriter:
+    """ESPCN (Shi et al. 2016) on the Y channel: 5 x 5 / 64 + TanH, 3 x 3 / 32 + TanH, 3 x 3 / scale^2, PixelShuffle
+    scale.  The output (`output`) is (1, scale height, scale width)."""
+    m = ModelWriter(seed)
+    x = m.input("data", 1, height, width)
+    x = m.activation("TanH", "tanh1", m.conv("conv1", x, 64, 5, 1, 2))
+    x = m.activation("TanH", "tanh2", m.conv("conv2", x, 32, 3, 1, 1))
+    m.pixel_shuffle("output", m.conv("conv3", x, scale * scale, 3, 1, 1), scale)
+    return m
+
+
+def se_tiny(seed=0, size=16, classes=10) -> ModelWriter:
+    """All five activation types at float64-checkable size: a 3 x 3 stem with BatchNorm + Scale + HardSwish, a 5 x 5
+    stride-2 depthwise layer + Swish, an SE gate (ReLU, HardSigmoid), a linear projection, a block with a Sigmoid branch
+    added back by BinaryOp ADD, TanH, global pooling, InnerProduct and Softmax."""
+    m = ModelWriter(seed)
+    x = _conv_bn(m, "stem", m.input("data", 3, size, size), 16, 3, 1, 1e-3, act="HardSwish")
+    x = _conv_bn(m, "dw", x, 16, 5, 2, 1e-3, group=16, act="Swish")
+    x = _squeeze_excitation(m, "se", x, 8, "ReLU", "HardSigmoid")
+    x = _conv_bn(m, "project", x, 16, 1, 1, 1e-3)
+    sc, x = m.split("block_split", x, ["block_skip", "block_body"])
+    x = _conv_bn(m, "branch", x, 16, 1, 1, 1e-3, act="Sigmoid")
+    x = m.activation("TanH", "tanh", m.binary_op("add", [sc, x], 0))
+    x = m.pool("pool", x, 1, 1, 1, 0, global_pooling=True)
+    m.softmax("prob", m.fc("fc", x, classes))
+    return m
+
+
 ZOO = {"single_conv": single_conv, "vgg16": vgg16, "resnet50": resnet50, "mobilenet_v1": mobilenet_v1, "mini": mini,
        "decoder_tiny": decoder_tiny, "fcn8s_tiny": fcn8s_tiny, "deeplab_head_tiny": deeplab_head_tiny,
        "mobilenet_v2": mobilenet_v2, "prelu_tiny": prelu_tiny, "mobilenet_ssd": mobilenet_ssd, "ssd_tiny": ssd_tiny,
@@ -1452,7 +1615,9 @@ ZOO = {"single_conv": single_conv, "vgg16": vgg16, "resnet50": resnet50, "mobile
        "shufflenet_v2": shufflenet_v2, "shuffle_tiny": shuffle_tiny, "deeplabv3_mobilenet_v2": deeplabv3_mobilenet_v2,
        "deeplabv3_tiny": deeplabv3_tiny, "faster_rcnn_vgg16": faster_rcnn_vgg16, "faster_rcnn_tiny": faster_rcnn_tiny,
        "rfcn_resnet50": rfcn_resnet50, "rfcn_tiny": rfcn_tiny, "fast_neural_style": fast_neural_style,
-       "style_tiny": style_tiny, "srvgg_compact": srvgg_compact, "edsr_baseline": edsr_baseline, "sr_tiny": sr_tiny}
+       "style_tiny": style_tiny, "srvgg_compact": srvgg_compact, "edsr_baseline": edsr_baseline, "sr_tiny": sr_tiny,
+       "mobilenet_v3_large": mobilenet_v3_large, "mobilenet_v3_small": mobilenet_v3_small,
+       "efficientnet_b0": efficientnet_b0, "espcn": espcn, "se_tiny": se_tiny}
 
 
 def synthetic_input(shape, index: int = 0) -> np.ndarray:

@@ -239,6 +239,44 @@ int fcuda_relu_forward(float* output, const float* input, size_t n, void* stream
  * floats.  NaN maps to min (ncnn's compare-and-assign passes it through).  -200 for min > max or a NaN bound.  In-place
  * (output == input) is allowed. */
 int fcuda_clip_forward(float* output, const float* input, size_t n, float min, float max, void* stream);
+/* ncnn's element-wise activation layers (the reference has none; MobileNet-v3, EfficientNet and ESPCN use them), in a
+ * numbering of their own: FcudaActivation names the convolution epilogues' activations, which stay 0..2.
+ * Definitions, every operation in fp32 and rounded once (IEEE division; no FMA contraction), x the input:
+ *   SIGMOID      y = fl(1 / fl(1 + expf(-x)))                      (the statement YOLO's decode uses, bit for bit)
+ *   TANH         y = tanhf(x)
+ *   SWISH        y = fl(x / fl(1 + expf(-x)))
+ *   HARDSIGMOID  y = x < lower ? 0 : x > upper ? 1 : fl(fl(x * alpha) + beta)
+ *   HARDSWISH    y = x < lower ? 0 : x > upper ? x : fl(x * fl(fl(x * alpha) + beta))
+ * with lower = fl(-beta / alpha) and upper = fl(fl(1 / alpha) + lower), computed once in fp32 on the host as ncnn's
+ * load_param does.  ncnn's defaults are alpha 0.2, beta 0.5; PyTorch's hardswish / hardsigmoid are alpha 1/6, beta 0.5,
+ * which pnnx writes as 0=1.666667e-01.
+ * NaN propagates through every type: both comparisons of the hard types are false for NaN, so it reaches the linear
+ * branch.  (Clip differs: fmaxf maps NaN to its min.)  SWISH(-inf) is NaN (-inf / inf), as in ncnn; SWISH(+inf) = +inf.
+ * Bounds against the exact value f(x) (float64), from the CUDA C Programming Guide's ulp table (expf and tanhf: 2 ulp;
+ * one ulp of v is at most 2^-23 |v|) and 2^-24 relative per rounding:
+ *   SIGMOID      |y - f| <= 2^-21 |f| + 2^-126    SWISH  |y - f| <= 2^-21 |f| + 2^-118
+ *   TANH         |y - f| <= 2^-22 |f| + 2^-148
+ * The relative term is 3 ulp of first order (expf's 2 ulp carried through 1 + e, which does not amplify it, and two
+ * roundings), with headroom.  The absolute term covers x below about -87.3, where the true value is subnormal, and below
+ * -88.72, where expf(-x) overflows to +inf and SIGMOID / SWISH return +-0 while f is a tiny normal or subnormal
+ * (|SWISH| <= 88.8 e^-88.72 < 2^-118 there).  TANH's absolute term is two subnormal spacings.
+ * The hard types, against f evaluated in float64 with the same fp32 lower / upper (so the same branch); the 2^-149 terms
+ * are the subnormal rounding of products near zero:
+ *   HARDSIGMOID  |y - f| <= 2^-23 (|x alpha| + |f|) + 2^-149
+ *   HARDSWISH    |y - f| <= 2^-23 (|x| (|x alpha| + |x alpha + beta|) + |f|) + 2^-149 (|x| + 1) */
+enum FcudaActivationType {
+    FCUDA_ACTIVATION_SIGMOID = 0,
+    FCUDA_ACTIVATION_TANH = 1,
+    FCUDA_ACTIVATION_SWISH = 2,
+    FCUDA_ACTIVATION_HARDSIGMOID = 3,
+    FCUDA_ACTIVATION_HARDSWISH = 4
+};
+/* y = act(x) over n floats, `type` an FcudaActivationType; alpha and beta are read by HARDSIGMOID / HARDSWISH only.  One
+ * launch (profiling kind 14).  output == input is allowed.  Allocates nothing and does not synchronise.
+ * -100: NULL output or input, or n == 0.  -200: a type outside 0..4, or, for HARDSIGMOID / HARDSWISH, alpha 0 or not
+ * finite, or beta not finite.  Both are decided before any launch. */
+int fcuda_activation_forward(float* output, const float* input, size_t n, int type, float alpha, float beta,
+                             void* stream);
 /* ncnn's PReLU (the reference has none): y = x < 0 ? x * slope[c] : x over (batch, channels, plane) with num_slope ==
  * channels slopes, or one slope shared by every channel (num_slope == 1); -200 for any other num_slope.  NaN passes
  * through.  `slope` is a device pointer.  In-place (output == input) is allowed. */
@@ -772,7 +810,7 @@ int fcuda_profile_collect(double* total_ms, double* algo_flops, double* mma_flop
  * Crop), 9 detection (Permute, axis Softmax, PriorBox, decode, NMS, merge; YOLO decode, select, mask, sweep), 10 channel
  * routing (fcuda_route_forward), 11 two-stage detection (Proposal decode, select, mask, sweep; ROIPooling; PSROIPooling),
  * 12 instance normalisation / padding (InstanceNorm, Padding), 13 pixel shuffle (PixelShuffle, alone or with its fused
- * upsampled-input add), < 0 all.  algo_bytes = the bytes the operation must move (inputs
+ * upsampled-input add), 14 activation (Sigmoid, TanH, Swish, HardSigmoid, HardSwish), < 0 all.  algo_bytes = the bytes the operation must move (inputs
  * read once + outputs written once). */
 int fcuda_profile_collect_kind(int kind, double* total_ms, double* algo_flops, double* mma_flops, double* algo_bytes,
                                long long* launches);
