@@ -99,6 +99,29 @@ def test_fused_chain_equals_layers_one_by_one(cuda, hw, group, reverse, batch):
     assert np.array_equal(_bits(part[1]), want[:, 14:16].view(np.uint32))
 
 
+ROUTE_CASES = [
+    # (source channels, destination sizes, group, reverse, begin, inner, batch): one fcuda_route_forward launch
+    ([3, 1, 4, 1, 5, 9, 2, 6], [31], 1, 0, 0, 7, 2),          # Concat of eight unequal bottoms
+    ([30], [30], 5, 1, 0, 4, 3),                             # ShuffleChannel, group != C / group
+    ([5, 7], [3, 4, 2], 4, 0, 3, 1, 7),                      # Concat -> ShuffleChannel -> Slice from position 3, inner 1
+]
+
+
+@gpu
+@pytest.mark.parametrize("srcs, sizes, group, reverse, begin, inner, batch", ROUTE_CASES)
+@pytest.mark.parametrize("misalign", [False, True])
+def test_route_cases_bit_exact(cuda, srcs, sizes, group, reverse, begin, inner, batch, misalign):
+    from feathercnn_b200 import booster
+    rng = np.random.default_rng(sum(srcs) + inner)
+    xs = [rng.standard_normal((batch, c, inner)).astype(np.float32) for c in srcs]
+    got = booster.route([_dev(x, misalign and k == 0) for k, x in enumerate(xs)], sizes, group, reverse, begin)
+    torch.cuda.synchronize()
+    want = np.concatenate(xs, 1)
+    want = shuffle_ref(want, group, reverse) if group > 1 else want
+    for t, s0, n in zip(got, np.cumsum([begin] + sizes), sizes):
+        assert np.array_equal(_bits(t), want[:, s0:s0 + n].view(np.uint32))
+
+
 HEAD = "Input data 0 1 data 0=6 1=5 2=12\n"
 
 

@@ -4,7 +4,8 @@ within the per-element bound include/fcuda.h states, and the naive E[x^2] - mean
 offset plane; the C ABI's rejections and workspace size (every call here fails its checks before a launch); the loader's
 ids, defaults and rejections; and the blob shapes of modelgen's style models.
 
-pad_ref, instance_norm64 and instance_norm_bound are what tests/test_gpu_style.py holds the kernels to."""
+pad_ref, instance_norm64 and instance_norm_bound are what tests/test_gpu_style.py holds the kernels to;
+tests/test_gpu_memory_bound_sweep.py also holds InstanceNorm to instance_norm32 bit for bit."""
 from __future__ import annotations
 
 import ctypes
@@ -62,9 +63,21 @@ def instance_norm_bound(x, gamma=None, beta=None, eps=1e-5):
 
 
 def _fmaf(a, b, c):
-    """fmaf of float32 operands: the product is exact in float64, one rounding there and one to float32 (the second
-    changes nothing except in rare double-rounding ties, which the bound does not care about)."""
-    return (np.asarray(a, np.float64) * np.asarray(b, np.float64) + np.asarray(c, np.float64)).astype(np.float32)
+    """fmaf of float32 operands, correctly rounded: the product is exact in float64 and s = p + c rounds once there, with
+    e = (p + c) - s exact (TwoSum).  Rounding s to float32 is right unless s sits exactly halfway between two floats while
+    e != 0; then the exact sum lies on e's side of the midpoint.  Bit for bit what the GPU's fmaf gives."""
+    p = np.asarray(a, np.float64) * np.asarray(b, np.float64)
+    c = np.asarray(c, np.float64)
+    s = p + c
+    t = s - p
+    e = (p - (s - t)) + (c - t)
+    r = s.astype(np.float32)
+    r64 = r.astype(np.float64)
+    other = np.nextafter(r, np.where(s > r64, np.float32(np.inf), np.float32(-np.inf))).astype(np.float32)
+    with np.errstate(invalid="ignore", over="ignore"):
+        tie = (s != r64) & ((r64 + other.astype(np.float64)) / 2 == s) & (e != 0)
+        toward = np.where((e > 0) == (other.astype(np.float64) > r64), other, r)
+    return np.where(tie, toward, r).astype(np.float32)
 
 
 def _block_sum(v):
