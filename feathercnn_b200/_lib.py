@@ -193,6 +193,8 @@ def fcuda() -> ctypes.CDLL:
             "fcuda_relu_forward": (i, [vp, vp, sz, vp]),
             "fcuda_clip_forward": (i, [vp, vp, sz, ctypes.c_float, ctypes.c_float, vp]),
             "fcuda_activation_forward": (i, [vp, vp, sz, i, ctypes.c_float, ctypes.c_float, vp]),
+            "fcuda_layer_norm_forward": (i, [vp, vp, i, ctypes.c_longlong, vp, vp, f, vp]),
+            "fcuda_attention_forward": (i, [vp, vp, i, vp, i, vp, i, i, i, i, i, i, f, vp]),
             "fcuda_prelu_forward": (i, [vp, vp, i, sz, vp, i, i, vp]),
             "fcuda_normalize_workspace_size": (i, [i, i, i, sz, i, szp]),
             "fcuda_normalize_forward": (i, [vp, vp, i, sz, vp, i, i, i, f, i, vp, i, vp]),

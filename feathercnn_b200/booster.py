@@ -610,13 +610,16 @@ def clip(x, lo, hi, out=None):
 
 
 ACTIVATIONS = ["Sigmoid", "TanH", "Swish", "HardSigmoid", "HardSwish"]  # FcudaActivationType, ncnn's layer type names
+GELU_TYPES = {"GELU": 6, "GELU_TANH": 7}  # FcudaActivationType of GELU with fast_gelu 0 / 1
 
 
 def activation(x, kind, alpha: float = 0.2, beta: float = 0.5, out=None):
-    """ncnn activation `kind` (0..4 or a name of ACTIVATIONS) over every element of x; alpha / beta are read by
-    HardSigmoid / HardSwish only (ncnn's defaults 0.2 / 0.5).  `out` may be `x` (in place).  Definitions, roundings and
-    bounds: include/fcuda.h."""
-    kind = ACTIVATIONS.index(kind) if isinstance(kind, str) else int(kind)
+    """ncnn activation `kind` (an FcudaActivationType, a name of ACTIVATIONS, or "GELU" / "GELU_TANH") over every
+    element of x; alpha / beta are read by HardSigmoid / HardSwish only (ncnn's defaults 0.2 / 0.5).  `out` may be `x`
+    (in place).  Definitions, roundings and bounds: include/fcuda.h."""
+    if isinstance(kind, str):
+        kind = GELU_TYPES[kind] if kind in GELU_TYPES else ACTIVATIONS.index(kind)
+    kind = int(kind)
     out = torch.empty_like(x) if out is None else out
     _check("fcuda_activation_forward", fcuda().fcuda_activation_forward(_ptr(out), _ptr(x.contiguous()), x.numel(), kind,
                                                                         float(alpha), float(beta), _stream()))
@@ -679,6 +682,41 @@ def instance_norm(x, gamma, beta, eps, relu=False, pad=None, out=None):
                                            _ptr(gamma.contiguous()) if gamma is not None else None,
                                            _ptr(beta.contiguous()) if beta is not None else None, float(eps), int(relu),
                                            ctypes.byref(p) if p is not None else None, _ptr(workspace), n, _stream()))
+    return out
+
+
+def layer_norm(x, n, gamma=None, beta=None, eps=1e-3, out=None):
+    """ncnn LayerNorm: every run of n contiguous floats of x (a row, or a channel plane) normalised with its mean and
+    biased variance, then * gamma + beta (n floats each, or both None).  `out` may be `x`.  Rounding order and bound:
+    include/fcuda.h."""
+    assert x.numel() % n == 0, (x.shape, n)
+    out = torch.empty_like(x) if out is None else out
+    _check("fcuda_layer_norm_forward",
+           fcuda().fcuda_layer_norm_forward(_ptr(out), _ptr(x.contiguous()), int(n), x.numel() // n,
+                                            _ptr(gamma.contiguous()) if gamma is not None else None,
+                                            _ptr(beta.contiguous()) if beta is not None else None, float(eps),
+                                            _stream()))
+    return out
+
+
+def attention(q, k, v, heads, scale=None, out=None):
+    """Scaled dot-product attention per head of fcuda_attention_forward.  q (N, Lq, >= E), k and v (N, Lk, >= E), each
+    with unit stride in its last dimension and any row stride (a slice of a fused [N, L, 3E] projection is read in
+    place); E = heads * head_dim is taken from `out`'s width, or q's when `out` is None.  Returns (N, Lq, E).  scale
+    defaults to 1 / sqrt(head_dim)."""
+    n, lq = q.shape[:2]
+    lk = k.shape[1]
+    e = out.shape[2] if out is not None else q.shape[2]
+    d = e // heads
+    scale = 1.0 / math.sqrt(d) if scale is None else scale
+    for t in (q, k, v):  # row-strided: a column slice of a contiguous buffer is read in place
+        assert t.is_cuda and t.dtype == torch.float32, (t.device, t.dtype)
+        assert t.stride(2) == 1 and t.stride(0) == t.shape[1] * t.stride(1), t.stride()
+    rows = [ctypes.c_void_p(t.data_ptr()) for t in (q, k, v)]
+    out = torch.empty((n, lq, e), device=q.device, dtype=torch.float32) if out is None else out
+    _check("fcuda_attention_forward",
+           fcuda().fcuda_attention_forward(_ptr(out), rows[0], q.stride(1), rows[1], k.stride(1), rows[2], v.stride(1),
+                                           n, heads, d, lq, lk, float(scale), _stream()))
     return out
 
 

@@ -1,4 +1,4 @@
-// ncnn's element-wise activation layers Sigmoid, TanH, Swish, HardSigmoid and HardSwish (fcuda_activation_forward).
+// ncnn's element-wise activation layers Sigmoid, TanH, Swish, HardSigmoid, HardSwish and GELU (fcuda_activation_forward).
 //
 // One flat grid-stride kernel per type, so the loop body is that type's arithmetic alone: float4 loads and stores where
 // both pointers are 16-byte aligned, then a scalar tail.  Every rounding is written out (__fmul_rn / __fadd_rn /
@@ -29,8 +29,14 @@ __device__ __forceinline__ float act_apply(float x, const HardParams& p) {
     } else if constexpr (TYPE == FCUDA_ACTIVATION_HARDSIGMOID) {
         // NaN fails both comparisons and reaches the linear branch, which propagates it
         return x < p.lower ? 0.f : x > p.upper ? 1.f : __fadd_rn(__fmul_rn(x, p.alpha), p.beta);
-    } else {  // FCUDA_ACTIVATION_HARDSWISH
+    } else if constexpr (TYPE == FCUDA_ACTIVATION_HARDSWISH) {
         return x < p.lower ? 0.f : x > p.upper ? x : __fmul_rn(x, __fadd_rn(__fmul_rn(x, p.alpha), p.beta));
+    } else if constexpr (TYPE == FCUDA_ACTIVATION_GELU) {
+        return __fmul_rn(__fmul_rn(0.5f, x), __fadd_rn(1.f, erff(__fmul_rn(x, 0.70710678118654752f))));
+    } else {  // FCUDA_ACTIVATION_GELU_TANH
+        const float x3 = __fmul_rn(__fmul_rn(x, x), x);
+        const float z = __fmul_rn(0.79788456080286536f, __fadd_rn(x, __fmul_rn(0.044715f, x3)));
+        return __fmul_rn(__fmul_rn(0.5f, x), __fadd_rn(1.f, tanhf(z)));
     }
 }
 
@@ -54,7 +60,9 @@ using ActKernel = void (*)(float*, const float*, size_t, HardParams);
 constexpr ActKernel kActKernels[] = {activation_kernel<FCUDA_ACTIVATION_SIGMOID>, activation_kernel<FCUDA_ACTIVATION_TANH>,
                                      activation_kernel<FCUDA_ACTIVATION_SWISH>,
                                      activation_kernel<FCUDA_ACTIVATION_HARDSIGMOID>,
-                                     activation_kernel<FCUDA_ACTIVATION_HARDSWISH>};
+                                     activation_kernel<FCUDA_ACTIVATION_HARDSWISH>, nullptr,
+                                     activation_kernel<FCUDA_ACTIVATION_GELU>,
+                                     activation_kernel<FCUDA_ACTIVATION_GELU_TANH>};
 
 int activation(float* out, const float* in, size_t n, int type, float alpha, float beta, float lower, float upper,
                cudaStream_t s) {

@@ -123,7 +123,7 @@ static inline int persistent_grid(Kernel kern, int threads, int smem, long long 
 enum ProfKind { PROF_TENSOR_GEMM = 0, PROF_IGEMM = 1, PROF_WINO_INPUT = 2, PROF_WINO_OUTPUT = 3, PROF_POOL = 4,
                 PROF_DEPTHWISE = 5, PROF_ELEMENTWISE = 6, PROF_DECONV = 7, PROF_RESIZE = 8, PROF_DETECTION = 9,
                 PROF_ROUTE = 10, PROF_RCNN = 11, PROF_INSTANCE_NORM = 12, PROF_PIXEL_SHUFFLE = 13, PROF_ACTIVATION = 14,
-                PROF_KINDS = 15 };
+                PROF_ATTENTION = 15, PROF_LAYER_NORM = 16, PROF_KINDS = 17 };
 int prof_begin(cudaStream_t s, int kind, double algo_flops, double mma_flops, double algo_bytes);  // -1 when off
 void prof_end(int idx, cudaStream_t s);
 void profile_collect_kind(int kind, double* total_ms, double* algo_flops, double* mma_flops, double* algo_bytes,

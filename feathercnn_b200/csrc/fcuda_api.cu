@@ -4,6 +4,7 @@
 #include "fcuda.h"
 
 #include "activation.cuh"
+#include "attention.cuh"
 #include "binary_op.cuh"
 #include "common.cuh"
 #include "conv_direct.cuh"
@@ -12,6 +13,7 @@
 #include "depthwise.cuh"
 #include "detection.cuh"
 #include "instance_norm.cuh"
+#include "layer_norm.cuh"
 #include "layers.cuh"
 #include "lrn.cuh"
 #include "normalize.cuh"
@@ -878,13 +880,46 @@ int fcuda_clip_forward(float* output, const float* input, size_t n, float min, f
 int fcuda_activation_forward(float* output, const float* input, size_t n, int type, float alpha, float beta,
                              void* stream) {
     if (!output || !input || n == 0) return -100;
-    if (type < FCUDA_ACTIVATION_SIGMOID || type > FCUDA_ACTIVATION_HARDSWISH) return -200;
+    if ((type < FCUDA_ACTIVATION_SIGMOID || type > FCUDA_ACTIVATION_HARDSWISH) && type != FCUDA_ACTIVATION_GELU &&
+        type != FCUDA_ACTIVATION_GELU_TANH)
+        return -200;
     const bool hard = type == FCUDA_ACTIVATION_HARDSIGMOID || type == FCUDA_ACTIVATION_HARDSWISH;
     if (hard && (alpha == 0.f || !isfinite(alpha) || !isfinite(beta))) return -200;
     // ncnn's HardSigmoid / HardSwish load_param, in fp32
     const float lower = hard ? -beta / alpha : 0.f;
     const float upper = hard ? 1.f / alpha + lower : 0.f;
     return activation(output, input, n, type, alpha, beta, lower, upper, as_stream(stream));
+}
+
+int fcuda_layer_norm_forward(float* output, const float* input, int n, long long rows, const float* gamma,
+                             const float* beta, float eps, void* stream) {
+    if (!output || !input || n < 1 || rows < 1) return -100;
+    if (!gamma != !beta || !(eps >= 0.f) || !isfinite(eps)) return -200;
+    return layer_norm(output, input, n, rows, gamma, beta, eps, as_stream(stream));
+}
+
+// [lo, hi) byte range of the rows a [batch][l][ld] operand reads (cols floats of each row)
+static void attn_range(const float* p, int ld, long long rows, int cols, uintptr_t* lo, uintptr_t* hi) {
+    *lo = reinterpret_cast<uintptr_t>(p);
+    *hi = *lo + (static_cast<uintptr_t>(rows - 1) * ld + cols) * sizeof(float);
+}
+
+int fcuda_attention_forward(float* o, const float* q, int ldq, const float* k, int ldk, const float* v, int ldv,
+                            int batch, int heads, int d, int lq, int lk, float scale, void* stream) {
+    if (!o || !q || !k || !v || batch < 1 || heads < 1 || lq < 1 || lk < 1) return -100;
+    if (d < 16 || d > 128 || d % 16 != 0) return -200;
+    const long long e = static_cast<long long>(heads) * d;
+    if (e > INT32_MAX || ldq < e || ldk < e || ldv < e) return -200;
+    if (static_cast<long long>(heads) * ((lq + 63) / 64) > 65535) return -200;
+    if (scale == 0.f || !isfinite(scale)) return -200;
+    uintptr_t olo, ohi, lo, hi;
+    attn_range(o, static_cast<int>(e), static_cast<long long>(batch) * lq, static_cast<int>(e), &olo, &ohi);
+    const struct { const float* p; int ld; int l; } ops[3] = {{q, ldq, lq}, {k, ldk, lk}, {v, ldv, lk}};
+    for (const auto& op : ops) {
+        attn_range(op.p, op.ld, static_cast<long long>(batch) * op.l, static_cast<int>(e), &lo, &hi);
+        if (lo < ohi && olo < hi) return -200;
+    }
+    return attention(o, q, ldq, k, ldk, v, ldv, batch, heads, d, lq, lk, scale, as_stream(stream));
 }
 
 int fcuda_prelu_forward(float* output, const float* input, int channels, size_t plane, const float* slope, int num_slope,

@@ -3,8 +3,9 @@
 // DetectionOutput, VGG-SSD's Normalize, YOLO's YoloDetectionOutput and Yolov3DetectionOutput, ShuffleNet's ShuffleChannel
 // and Slice, AlexNet's and GoogLeNet's LRN, Faster R-CNN's Proposal and ROIPooling, R-FCN's PSROIPooling, fast neural
 // style's InstanceNorm and Padding, super-resolution's PixelShuffle, BinaryOp (the element-wise ops onnx2ncnn and pnnx
-// write, residual adds among them), and the activations Sigmoid, TanH, Swish, HardSigmoid and HardSwish (MobileNet-v3,
-// EfficientNet, ESPCN), 42 in all, mapped onto this host's layer classes.  A table of {type name,
+// write, residual adds among them), the activations Sigmoid, TanH, Swish, HardSigmoid and HardSwish (MobileNet-v3,
+// EfficientNet, ESPCN), and Vision Transformers' GELU, LayerNorm, MemoryData and MultiHeadAttention, 46 in all, mapped
+// onto this host's layer classes.  A table of {type name,
 // factory} pairs instead of one macro line per layer; the
 // DEFINE_LAYER_CREATOR / REGISTER_LAYER_CREATOR macros of <feather/layer_factory.h> remain the plugin API for user layers.
 #include <feather/layer_factory.h>
@@ -31,6 +32,7 @@
 #include "layers/route_layers.h"
 #include "layers/scale_layer.h"
 #include "layers/style_layers.h"
+#include "layers/transformer_layers.h"
 #include "layers/yolo_layers.h"
 
 namespace feather {
@@ -93,6 +95,10 @@ const BuiltIn kBuiltIns[] = {
     {"Swish", make_layer<ActivationLayer>},
     {"HardSigmoid", make_layer<ActivationLayer>},
     {"HardSwish", make_layer<ActivationLayer>},
+    {"GELU", make_layer<ActivationLayer>},
+    {"LayerNorm", make_layer<LayerNormLayer>},
+    {"MemoryData", make_layer<MemoryDataLayer>},
+    {"MultiHeadAttention", make_layer<MultiHeadAttentionLayer>},
 };
 
 }  // namespace

@@ -21,10 +21,21 @@ public:
         }
         return 0;
     }
+    // A rank-2 blob takes order 0 (a view) and 1 (the transpose, how pnnx writes flatten(2).transpose(1, 2)).
     int Reshape() {
-        const Blob<float>* b = bottoms[0];
+        Blob<float>* b = bottoms[0];
+        if (b->dims() == 2 && order <= 1) {
+            if (order == 0) {
+                tops[0]->ViewExternal(b->data(), b->num(), 1, b->height(), b->width(), 2);
+            } else {
+                tops[0]->ReshapeWithRealloc(b->num(), 1, b->width(), b->height());
+                tops[0]->set_dims(2);
+            }
+            return 0;
+        }
         if (b->dims() != 3) {
-            LOGE("Layer %s: Permute takes a rank-3 blob, not rank %d", this->name.c_str(), b->dims());
+            LOGE("Layer %s: Permute order_type %d of a rank-%d blob is not supported (rank 3, or rank 2 with order 0 or 1)",
+                 this->name.c_str(), order, b->dims());
             return FEATHER_ERR_UNSUPPORTED;
         }
         static const int kAxes[6][3] = {{0, 1, 2}, {0, 2, 1}, {1, 0, 2}, {1, 2, 0}, {2, 0, 1}, {2, 1, 0}};
@@ -34,6 +45,7 @@ public:
     }
     int Forward() {
         const Blob<float>* b = bottoms[0];
+        if (b->dims() == 2 && order == 0) return 0;
         return fcuda_permute_forward(tops[0]->data(), b->data(), static_cast<int>(b->channels()), static_cast<int>(b->height()),
                                      static_cast<int>(b->width()), order, static_cast<int>(b->num()), stream());
     }

@@ -41,15 +41,31 @@ public:
         return rc;
     }
 
+    // ncnn's rule for a rank-2 bottom of w == num_input and h > 1: each row is one input vector (a Transformer's
+    // tokens), and the top is rank 2 with w = num_output.  Otherwise each image is one input vector.
     int Reshape() {
         const Blob<float>* bottom_blob = bottoms[0];
         const size_t per_image = bottom_blob->channels() * bottom_blob->height() * bottom_blob->width();
+        if (bottom_blob->dims() == 2 && bottom_blob->width() == input_size && bottom_blob->height() > 1) {
+            if (bottom_blob->num() * bottom_blob->height() > 0x7fffffffu) return FEATHER_ERR_UNSUPPORTED;
+            rows = static_cast<int>(bottom_blob->num() * bottom_blob->height());
+            this->tops[0]->ReshapeWithRealloc(static_cast<int>(bottom_blob->num()), 1,
+                                              static_cast<int>(bottom_blob->height()), static_cast<int>(output_size));
+            this->tops[0]->set_dims(2);
+            size_t scratch = 0, dull = 0;
+            int rc = fcuda_inner_product_get_buffer_size(static_cast<int>(input_size), static_cast<int>(output_size),
+                                                         rows, &scratch, &dull);
+            if (rc) return rc;
+            MEMPOOL_CHECK_RETURN(this->common_mempool->Request(sizeof(float) * scratch));
+            return 0;
+        }
         if (input_size != per_image) {
             LOGE("In Layer %s: Bottom %s data size %zu is inconsistant with expected input size %zu.", this->name.c_str(),
                  bottom_blob->name.c_str(), per_image, input_size);
             return FEATHER_ERR_WEIGHTS;
         }
         const int batch = bottom_blob->num();
+        rows = batch;
         this->tops[0]->ReshapeWithRealloc(batch, static_cast<int>(output_size), 1, 1);
         size_t scratch = 0, dull = 0;
         int rc = fcuda_inner_product_get_buffer_size(static_cast<int>(input_size), static_cast<int>(output_size), batch,
@@ -80,8 +96,8 @@ public:
         float* buffer = NULL;
         MEMPOOL_CHECK_RETURN(this->common_mempool->GetPtr(&buffer));
         return fcuda_inner_product_forward(static_cast<int>(input_size), static_cast<int>(output_size), tops[0]->data(),
-                                           bottoms[0]->data(), kernel_data, bias_data, buffer, fuse_relu ? 1 : 0,
-                                           bottoms[0]->num(), stream());
+                                           bottoms[0]->data(), kernel_data, bias_data, buffer, fuse_relu ? 1 : 0, rows,
+                                           stream());
     }
 
     int Fuse(Layer* next_layer) {  // inner_product_layer.h:43-53
@@ -101,6 +117,7 @@ protected:
     float* bias_data;
     bool fuse_relu;
     Blob<float>* packed;
+    int rows = 0;  // input vectors per Forward: the batch, or batch * h for a rank-2 bottom
 };
 
 }  // inline namespace b200

@@ -19,6 +19,7 @@
 #include "layers/pixel_shuffle_layer.h"
 #include "layers/resize_layers.h"
 #include "layers/route_layers.h"
+#include "layers/transformer_layers.h"
 
 namespace feather {
 inline namespace b200 {  // ABI tag: keeps these symbols apart from the reference build when both are loaded
@@ -491,9 +492,14 @@ int Net::BuildBlobMap() {
 // Forward
 // ---------------------------------------------------------------------------------------------------------
 int Net::Reshape() {
+    // MemoryData holds one copy per image of the batch the first Input was fed
+    int batch = 1;
+    std::map<std::string, Blob<float>*>::iterator in = blob_map.find(input_name_);
+    if (in != blob_map.end() && in->second->num() > 0) batch = static_cast<int>(in->second->num());
     for (size_t i = 0; i < layers.size(); ++i) {
         Layer* layer = layers[i];
         if (layer->_fused_away) continue;
+        if (MemoryDataLayer* md = dynamic_cast<MemoryDataLayer*>(layer)) md->set_batch(batch);
         const int gr = layer->Reshape();
         if (gr != 0) {
             LOGE("Layer %s failed to generate tops (%d)", layer->name.c_str(), gr);

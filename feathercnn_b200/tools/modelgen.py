@@ -12,7 +12,8 @@ that exercises every layer type, single-shot detectors (MobileNet-SSD, VGG-SSD 3
 R-CNN, py-R-FCN's ResNet-50 R-FCN and a tiny one of each), fast neural style transfer (TransformerNet, with a tiny
 one), super-resolution (Real-ESRGAN's SRVGGNetCompact and EDSR baseline, with a tiny PixelShuffle net, and ESPCN), ShuffleNet-v2
 with a small routing probe net, and the nets of ncnn's activation layers (MobileNet-v3 Large / Small and EfficientNet-B0
-in torchvision's layouts, with a small squeeze-and-excitation net).  Weight
+in torchvision's layouts, with a small squeeze-and-excitation net), and Vision Transformers (ViT-B/16, ViT-S/16 and
+ViT-Ti/16 in torchvision's layout, with a tiny one).  Weight
 statistics follow SURVEY.md §8(d).
 """
 from __future__ import annotations
@@ -246,6 +247,7 @@ class ModelWriter:
         self._layer("Split", name, [bottom], tops)
         for t in tops:
             self.shape[t] = self.shape[bottom]
+            self.rank[t] = self.rank.get(bottom, 3)
         return tops
 
     def eltwise(self, name, bottoms, top=None):
@@ -262,6 +264,7 @@ class ModelWriter:
             assert len(bottoms) == 2, (name, bottoms)
             self._layer("BinaryOp", name, bottoms, [top], {0: op})
             self.shape[top] = tuple(np.broadcast_shapes(*(self.shape[b] for b in bottoms)))
+            self.rank[top] = max(self.rank.get(b, 3) for b in bottoms)
         else:
             assert len(bottoms) == 1, (name, bottoms)
             self._layer("BinaryOp", name, bottoms, [top], {0: op, 1: 1, 2: f"{float(scalar):e}"})
@@ -324,6 +327,7 @@ class ModelWriter:
         self._layer("Permute", name, [bottom], [top], {0: order})
         axes = [(0, 1, 2), (0, 2, 1), (1, 0, 2), (1, 2, 0), (2, 0, 1), (2, 1, 0)][order]
         self.shape[top] = tuple(self.shape[bottom][a] for a in axes)
+        self.rank[top] = self.rank.get(bottom, 3)
         return top
 
     def flatten(self, name, bottom, top=None):
@@ -554,6 +558,68 @@ class ModelWriter:
             oh, ow = outh or h - hoff, outw or w - woff
         assert coff + oc <= c and hoff + oh <= h and woff + ow <= w, (name, self.shape[bottom], (oc, oh, ow))
         self.shape[top] = (oc, oh, ow)
+        return top
+
+    # ---- Vision Transformer layers (token blobs are rank 2: w = features, h = tokens) -----------------------------
+    def memory_data(self, name, w, h=0, c=0, data=None, std=0.02):
+        """ncnn MemoryData 0=w 1=h 2=c (the rank is the number of leading dims given): `data` (w * h * c raw floats), or
+        normal(0, std) draws."""
+        shape = (max(c, 1), max(h, 1), w)
+        data = self.rng.standard_normal(shape) * std if data is None else data
+        params = {k: v for k, v in ((0, w), (1, h), (2, c)) if v}
+        self._layer("MemoryData", name, [], [name], params)
+        self._weights(np.asarray(data, np.float32).reshape(shape), False)
+        self.shape[name] = shape
+        self.rank[name] = len(params)
+        return name
+
+    def layer_norm(self, name, bottom, eps=1e-6, top=None):
+        """ncnn LayerNorm 0=affine_size (the bottom's w) 1=eps 2=1; gamma uniform(0.8, 1.2), beta uniform(-0.1, 0.1)."""
+        top = top or name
+        n = self.shape[bottom][2]
+        self._layer("LayerNorm", name, [bottom], [top], {0: n, 1: f"{eps:e}", 2: 1})
+        self._weights(self.rng.uniform(0.8, 1.2, n).astype(np.float32), False)
+        self._weights(self.rng.uniform(-0.1, 0.1, n).astype(np.float32), False)
+        self.shape[top] = self.shape[bottom]
+        self.rank[top] = self.rank.get(bottom, 3)
+        return top
+
+    def linear(self, name, bottom, out, top=None):
+        """InnerProduct on a rank-2 token blob: each row is one input vector (ncnn's rule), the top is rank 2.  Weights
+        normal(0, 1 / sqrt(in)), bias uniform(-0.1, 0.1)."""
+        top = top or name
+        _, h, n_in = self.shape[bottom]
+        assert self.rank.get(bottom, 3) == 2 and h > 1, (name, self.shape[bottom])
+        wts = (self.rng.standard_normal((out, n_in)) / np.sqrt(n_in)).astype(np.float32)
+        self._layer("InnerProduct", name, [bottom], [top], {0: out, 1: 1, 2: wts.size})
+        self._weights(wts, True)
+        self._weights(self.rng.uniform(-0.1, 0.1, out).astype(np.float32), False)
+        self.shape[top] = (1, h, out)
+        self.rank[top] = 2
+        self.flops += 2.0 * out * n_in * h
+        return top
+
+    def gelu(self, name, bottom, fast=0, top=None):
+        """ncnn GELU 0=fast_gelu (written when 1)."""
+        top = top or name
+        self._layer("GELU", name, [bottom], [top], {0: 1} if fast else None)
+        self.shape[top] = self.shape[bottom]
+        self.rank[top] = self.rank.get(bottom, 3)
+        return top
+
+    def multihead_attention(self, name, bottom, heads, top=None):
+        """ncnn MultiHeadAttention of one bottom (q = k = v): 0=embed_dim 1=num_heads 2=embed_dim^2, default scale.
+        Weights q_w, q_b, k_w, k_b, v_w, v_b, out_w, out_b (matrices normal(0, 1 / sqrt(E)) flagged, biases
+        uniform(-0.1, 0.1) raw)."""
+        top = top or name
+        _, l, e = self.shape[bottom]
+        self._layer("MultiHeadAttention", name, [bottom], [top], {0: e, 1: heads, 2: e * e})
+        for _ in range(4):
+            self._weights((self.rng.standard_normal((e, e)) / np.sqrt(e)).astype(np.float32), True)
+            self._weights(self.rng.uniform(-0.1, 0.1, e).astype(np.float32), False)
+        self.shape[top] = (1, l, e)
+        self.rank[top] = 2
+        self.flops += 8.0 * l * e * e + 4.0 * l * l * e
         return top
 
     # ---- output ------------------------------------------------------------------------------
@@ -1607,6 +1673,69 @@ def se_tiny(seed=0, size=16, classes=10) -> ModelWriter:
     return m
 
 
+
+def vit(patch=16, dim=768, depth=12, heads=12, mlp_dim=3072, size=224, classes=1000, seed=0) -> ModelWriter:
+    """torchvision's VisionTransformer as pnnx exports it: the patch convolution, Reshape + Permute 0=1 to tokens, a
+    MemoryData class token concatenated in front, a MemoryData position embedding added by BinaryOp; per encoder block
+    LayerNorm (eps 1e-6), MultiHeadAttention, BinaryOp ADD, LayerNorm, InnerProduct, GELU, InnerProduct, BinaryOp ADD;
+    the final LayerNorm, the class token cut out by Crop 1=0 4=1, and the InnerProduct head (`logits`)."""
+    m = ModelWriter(seed)
+    g = size // patch
+    x = m.input("data", 3, size, size)
+    x = m.conv("conv_proj", x, dim, patch, patch, 0, gain=np.sqrt(1.0 / (3 * patch * patch)))
+    x = m.permute("tokens", m.reshape("flatten", x, g * g, dim), 1)
+    x = m.concat("cat_cls", [m.memory_data("class_token", dim, 1), x], axis=0)
+    x = m.binary_op("add_pos", [x, m.memory_data("pos_embedding", dim, g * g + 1)], 0)
+    for i in range(depth):
+        b = f"layer{i}"
+        skip, x = m.split(f"{b}_split1", x, [f"{b}_skip1", f"{b}_in1"])
+        x = m.multihead_attention(f"{b}_attn", m.layer_norm(f"{b}_ln1", x), heads)
+        x = m.binary_op(f"{b}_add1", [skip, x], 0)
+        skip, x = m.split(f"{b}_split2", x, [f"{b}_skip2", f"{b}_in2"])
+        x = m.gelu(f"{b}_gelu", m.linear(f"{b}_fc1", m.layer_norm(f"{b}_ln2", x), mlp_dim))
+        x = m.binary_op(f"{b}_add2", [skip, m.linear(f"{b}_fc2", x, dim)], 0)
+    x = m.crop("cls", m.layer_norm("ln", x), hoff=0, outh=1)
+    m.fc("logits", x, classes)
+    return m
+
+
+def vit_b_16(seed=0, size=224, classes=1000) -> ModelWriter:
+    """ViT-B/16: 768 wide, 12 blocks of 12 heads (head_dim 64), MLP 3072."""
+    return vit(16, 768, 12, 12, 3072, size, classes, seed)
+
+
+def vit_s_16(seed=0, size=224, classes=1000) -> ModelWriter:
+    """ViT-S/16 (DeiT-S's shape): 384 wide, 12 blocks of 6 heads (head_dim 64), MLP 1536."""
+    return vit(16, 384, 12, 6, 1536, size, classes, seed)
+
+
+def vit_ti_16(seed=0, size=224, classes=1000) -> ModelWriter:
+    """ViT-Ti/16 (DeiT-Ti's shape): 192 wide, 12 blocks of 3 heads (head_dim 64), MLP 768."""
+    return vit(16, 192, 12, 3, 768, size, classes, seed)
+
+
+def vit_tiny(seed=0, size=32, classes=10) -> ModelWriter:
+    """A ViT at float64-checkable size: 8 x 8 patches of a 32 x 32 image (17 tokens), 64 wide, three blocks of 4, 2 and
+    1 heads (head_dim 16, 32 and 64), MLP 128."""
+    m = ModelWriter(seed)
+    patch, dim, g = 8, 64, size // 8
+    x = m.input("data", 3, size, size)
+    x = m.conv("conv_proj", x, dim, patch, patch, 0, gain=np.sqrt(1.0 / (3 * patch * patch)))
+    x = m.permute("tokens", m.reshape("flatten", x, g * g, dim), 1)
+    x = m.concat("cat_cls", [m.memory_data("class_token", dim, 1), x], axis=0)
+    x = m.binary_op("add_pos", [x, m.memory_data("pos_embedding", dim, g * g + 1)], 0)
+    for i, heads in enumerate((4, 2, 1)):
+        b = f"layer{i}"
+        skip, x = m.split(f"{b}_split1", x, [f"{b}_skip1", f"{b}_in1"])
+        x = m.multihead_attention(f"{b}_attn", m.layer_norm(f"{b}_ln1", x), heads)
+        x = m.binary_op(f"{b}_add1", [skip, x], 0)
+        skip, x = m.split(f"{b}_split2", x, [f"{b}_skip2", f"{b}_in2"])
+        x = m.gelu(f"{b}_gelu", m.linear(f"{b}_fc1", m.layer_norm(f"{b}_ln2", x), 128))
+        x = m.binary_op(f"{b}_add2", [skip, m.linear(f"{b}_fc2", x, dim)], 0)
+    x = m.crop("cls", m.layer_norm("ln", x), hoff=0, outh=1)
+    m.fc("logits", x, classes)
+    return m
+
 ZOO = {"single_conv": single_conv, "vgg16": vgg16, "resnet50": resnet50, "mobilenet_v1": mobilenet_v1, "mini": mini,
        "decoder_tiny": decoder_tiny, "fcn8s_tiny": fcn8s_tiny, "deeplab_head_tiny": deeplab_head_tiny,
        "mobilenet_v2": mobilenet_v2, "prelu_tiny": prelu_tiny, "mobilenet_ssd": mobilenet_ssd, "ssd_tiny": ssd_tiny,
@@ -1617,7 +1746,8 @@ ZOO = {"single_conv": single_conv, "vgg16": vgg16, "resnet50": resnet50, "mobile
        "rfcn_resnet50": rfcn_resnet50, "rfcn_tiny": rfcn_tiny, "fast_neural_style": fast_neural_style,
        "style_tiny": style_tiny, "srvgg_compact": srvgg_compact, "edsr_baseline": edsr_baseline, "sr_tiny": sr_tiny,
        "mobilenet_v3_large": mobilenet_v3_large, "mobilenet_v3_small": mobilenet_v3_small,
-       "efficientnet_b0": efficientnet_b0, "espcn": espcn, "se_tiny": se_tiny}
+       "efficientnet_b0": efficientnet_b0, "espcn": espcn, "se_tiny": se_tiny, "vit_b_16": vit_b_16,
+       "vit_s_16": vit_s_16, "vit_ti_16": vit_ti_16, "vit_tiny": vit_tiny}
 
 
 def synthetic_input(shape, index: int = 0) -> np.ndarray:

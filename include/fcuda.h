@@ -269,12 +269,27 @@ enum FcudaActivationType {
     FCUDA_ACTIVATION_TANH = 1,
     FCUDA_ACTIVATION_SWISH = 2,
     FCUDA_ACTIVATION_HARDSIGMOID = 3,
-    FCUDA_ACTIVATION_HARDSWISH = 4
+    FCUDA_ACTIVATION_HARDSWISH = 4,
+    FCUDA_ACTIVATION_GELU = 6,
+    FCUDA_ACTIVATION_GELU_TANH = 7
 };
+/* GELU (ncnn's GELU layer; 0=fast_gelu picks the form; Vision Transformers' MLP).  5 stays unassigned and is rejected,
+ * so no value that was invalid for the five types above gains a meaning it did not have.
+ *   GELU         y = fl(fl(0.5 x) * fl(1 + erff(fl(x * c))))               c = fl(1 / sqrt(2))
+ *   GELU_TANH    y = fl(fl(0.5 x) * fl(1 + tanhf(fl(k0 * fl(x + fl(k1 * fl(fl(x * x) * x)))))))
+ *                                                                            k0 = fl(sqrt(2 / pi)), k1 = 0.044715f
+ * against f = 0.5 x (1 + erf(x / sqrt 2)), resp. 0.5 x (1 + tanh(sqrt(2 / pi) (x + 0.044715 x^3))) in float64 (what
+ * torch.nn.GELU computes with approximate 'none' / 'tanh'):
+ *   |y - f| <= 2^-21 |x| + 2^-23 |f| + 2^-148        (both forms, finite x)
+ * erff and tanhf are 2 ulp (at most 2^-22 for a value of magnitude <= 1); their argument carries <= 7 roundings
+ * (k0, k1, c included) of terms of one sign, and the derivative bound |z| (1 - tanh^2 z) <= 0.45 (resp. 1.13 |u|
+ * e^-u^2 <= 0.43) keeps the argument's share under 2^-23; 1 + t adds one rounding of <= 2^-23.  Multiplied by 0.5 |x|
+ * that is under 2^-21 |x|; the last product adds 2^-24 |f|.  The absolute term covers the loss of 1 + t to cancellation
+ * for x far below 0, where f is tiny and y may round to +-0.  NaN propagates. */
 /* y = act(x) over n floats, `type` an FcudaActivationType; alpha and beta are read by HARDSIGMOID / HARDSWISH only.  One
  * launch (profiling kind 14).  output == input is allowed.  Allocates nothing and does not synchronise.
- * -100: NULL output or input, or n == 0.  -200: a type outside 0..4, or, for HARDSIGMOID / HARDSWISH, alpha 0 or not
- * finite, or beta not finite.  Both are decided before any launch. */
+ * -100: NULL output or input, or n == 0.  -200: a type that is not an FcudaActivationType, or, for HARDSIGMOID /
+ * HARDSWISH, alpha 0 or not finite, or beta not finite.  Both are decided before any launch. */
 int fcuda_activation_forward(float* output, const float* input, size_t n, int type, float alpha, float beta,
                              void* stream);
 /* ncnn's PReLU (the reference has none): y = x < 0 ? x * slope[c] : x over (batch, channels, plane) with num_slope ==
@@ -385,6 +400,57 @@ int fcuda_instance_norm_forward(float* output, const float* input, int channels,
  * it pads, h * w or the padded plane over 2^31 - 1 floats, a non-zero pad with output == input. */
 int fcuda_padding_forward(float* output, const float* input, int channels, int h, int w, const FcudaPad* pad, int batch,
                           void* stream);
+/* ncnn's LayerNorm (Vision Transformers): each of `rows` rows of n contiguous floats is normalised over itself,
+ *   y = (x - mean) / sqrt(var + eps) * gamma[i] + beta[i]     (i the position in the row; biased variance, eps inside
+ * the square root, as torch.nn.LayerNorm).  A rank-2 blob's rows are its h rows (n = w); a rank-3 blob takes n = w
+ * (every row of every channel) or n = w * h (every channel plane).  gamma and beta are n floats each, or both NULL.
+ * Rounding order (every operation fp32, rounded once; fixed, with no atomics, so the bits do not depend on the batch, the
+ * launch geometry or the alignment): one warp per row.  Lane l (0..31) adds x[l + 32 j] for j = 0, 1, ... in order
+ * from 0.f; a 32-lane xor-shuffle tree (offsets 16, 8, 4, 2, 1) gives the sum, mean = sum / n.  With d = x - mean,
+ * lane l accumulates q = fmaf(d, d, q) over the same elements in the same order and the same tree gives Q; var = Q / n,
+ * r = __frsqrt_rn(var + eps), y = fmaf(d * r, gamma, beta) (y = d * r without gamma / beta).  Rows of at most 1024
+ * floats are read once into registers; longer rows are read again for each pass.
+ * Error bound (first order; float64 quantities of the row: mean mu, biased variance s2, sigma = sqrt(s2 + eps),
+ * M = mean |x|, U = 2^-24, L = ceil(n / 32) + 5 the length of the longest addition chain):
+ *   e = (L + 1) U M,   rho = (L + 6) U + (e / sigma)^2,
+ *   |y - y64| <= |gamma| (rho |x - mu| + (1 + rho) e) / sigma + 2^-23 (|y64| + |gamma| |x - mu| / sigma) + 2^-149
+ * (gamma = 1, beta = 0 without the affine).  One launch (profiling kind 16).  output == input is allowed.  Allocates
+ * nothing and does not synchronise.  -100: a NULL output or input, n or rows < 1.  -200: exactly one of gamma / beta
+ * NULL, eps negative or not finite.  Both are decided before any launch. */
+int fcuda_layer_norm_forward(float* output, const float* input, int n, long long rows, const float* gamma,
+                             const float* beta, float eps, void* stream);
+/* Scaled dot-product attention of ncnn's MultiHeadAttention (torch.nn.MultiheadAttention without a mask or dropout),
+ * after the input projections and before the output projection.  Q, K and V are row-major fp32 buffers
+ * [batch][Lq or Lk][ld]; head h of image b reads columns h * d .. h * d + d - 1 of its rows (ldq / ldk / ldv in floats,
+ * so one [N L][3E] buffer of a fused QKV projection is read in place with ld = 3E).  O is [batch][Lq][heads * d]:
+ *   O[b][i][h d + c] = sum_j softmax_j(scale * Q_i . K_j) V[j][c]   over the keys j < Lk of image b, head h.
+ * One CTA (128 threads) per (image, head, 64-query tile); it walks the key tiles of 64 in order.  S = Q K^T and O = P V
+ * run on wgmma in BF16x3 (each operand x = p1 + p2 + r, |r| <= 2^-16 |x|, three bf16 products p2 q1 + p1 q2 + p1 q1 into
+ * fp32): Q and P are split in registers, K and V as they are staged into shared memory.  The softmax is online in fp32:
+ * s = fl(S scale), running max m, p = expf(s - m), the running sum l and O rescaled by expf(m_old - m_new) per tile,
+ * O / l once at the end.  Key tails are masked to -inf (their K and V staged as 0); query tails are not stored.  The
+ * bits do not depend on how the batch is split across calls.
+ * Error bound against float64 attention of the same fp32 Q, K, V (per element; U = 2^-24, T = ceil(Lk / 64) key tiles,
+ * s*_ij = scale Q_i . K_j and m*_i = max_j s*_ij in float64, p*_ij = exp(s*_ij - m*_i), a_ij = sum_c |Q_ic| |K_jc|,
+ * W_ic = sum_j p*_ij |V_jc| / sum_j p*_ij):
+ *   D_i   = max_j ( |scale| a_ij (2^-14 + (d + 1) 2^-21) + (T + 1) U |s*_ij - m*_i| )
+ *   eta_i = 2.01 ( D_i + (T + 1) 2^-22 + (2 T + 18) U )
+ *   |O_ic - O*_ic| <= ( 2.01 eta_i + 2^-14 + (3 Lk + 3 T + 1) 2^-23 ) W_ic + 2^-126
+ * D_i bounds the error of each exponent's argument: the BF16x3 product drops p2 q2 and the residuals (<= 3 2^-16 +
+ * O(2^-24) of a_ij), the tensor core accumulates 3 d products in fp32 (<= 2^-23 each, counted as d 2^-21 with
+ * headroom), s and s - m round once each, and the running maxima differ by at most max |s - m| per rescale.  eta_i
+ * bounds the relative error of each weight p: exp of the argument error, expf's 2 ulp per p and per rescale, and the
+ * fp32 row sum l (a chain of at most 2 T + 18 additions).  A softmax of weights with relative errors <= eta moves the
+ * convex combination by at most 2 eta / (1 - eta) W.  The P V product adds the BF16x3 terms of P and V (2^-14) and the
+ * fp32 accumulation of 3 Lk products, T rescales and the final division.  expf's 2 ulp is the CUDA C Programming
+ * Guide's bound.  This bound is derived, not measured.
+ * Allocates nothing and does not synchronise, so it can be captured in a CUDA graph.  One launch (profiling kind 15);
+ * images go on grid x (no 65535 cap), heads and query tiles on y.
+ * -100: a NULL pointer, batch, heads, Lq or Lk < 1.  -200: d not a multiple of 16 in 16..128, an ld below heads * d, o
+ * overlapping q, k or v, heads * ceil(Lq / 64) over 65535, or a scale that is 0 or not finite.  Both are decided before
+ * any launch. */
+int fcuda_attention_forward(float* o, const float* q, int ldq, const float* k, int ldk, const float* v, int ldv,
+                            int batch, int heads, int d, int lq, int lk, float scale, void* stream);
 /* SoftmaxLayer::Forward (src/layers/softmax_layer.h:32-55): over each image's whole blob. */
 int fcuda_softmax_forward(float* output, const float* input, size_t n_per_image, int batch, void* stream);
 /* DropoutLayer::Forward (src/layers/dropout_layer.h:36-57): y = x*scale (copy when scale == 1). */
@@ -810,7 +876,8 @@ int fcuda_profile_collect(double* total_ms, double* algo_flops, double* mma_flop
  * Crop), 9 detection (Permute, axis Softmax, PriorBox, decode, NMS, merge; YOLO decode, select, mask, sweep), 10 channel
  * routing (fcuda_route_forward), 11 two-stage detection (Proposal decode, select, mask, sweep; ROIPooling; PSROIPooling),
  * 12 instance normalisation / padding (InstanceNorm, Padding), 13 pixel shuffle (PixelShuffle, alone or with its fused
- * upsampled-input add), 14 activation (Sigmoid, TanH, Swish, HardSigmoid, HardSwish), < 0 all.  algo_bytes = the bytes the operation must move (inputs
+ * upsampled-input add), 14 activation (Sigmoid, TanH, Swish, HardSigmoid, HardSwish, GELU), 15 attention
+ * (fcuda_attention_forward), 16 layer normalisation (LayerNorm), < 0 all.  algo_bytes = the bytes the operation must move (inputs
  * read once + outputs written once). */
 int fcuda_profile_collect_kind(int kind, double* total_ms, double* algo_flops, double* mma_flops, double* algo_bytes,
                                long long* launches);
